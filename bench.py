@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- Daala per-block encode hot path on B200: Mpixels/s on 4K 4:2:0 intra.
+"""bench.py -- Daala per-block encode hot path on an H100: Mpixels/s on 4K 4:2:0 intra.
 
 A "step" = one pass of the keyframe hot path over a batch of `--frames` synthetic
 3840x2160 4:2:0 frames (SURVEY.md 8(d) content, seeded) through the keyframe engine
@@ -16,7 +16,8 @@ A "step" = one pass of the keyframe hot path over a batch of `--frames` syntheti
   --impl reference : the reference's own CPU code (oracle/_ref, SIMD build, one process per
           usable host core) on whole 4K frames of the same workload
 
-Prints ONE JSON line (rank 0).
+Prints ONE JSON line (rank 0).  --dump-outputs DIR writes, after the timed steps, a fixed sample of what
+the last timed step computed (reconstruction, coefficient planes, per-band PVQ results) as DIR/<name>.npy.
 """
 import argparse
 import json
@@ -70,6 +71,8 @@ def parse():
     ap.add_argument("--prepass", type=int, default=0, help="luma no-reference searches ahead of the chains (1) or inside them (0)")
     ap.add_argument("--level-chains", type=int, default=0, help="luma intra chains level-synchronously (1) instead of the dependency queue (0)")
     ap.add_argument("--shard", default="frames", choices=["frames", "sbrow"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a seeded sample of the last timed step's outputs as DIR/<name>.npy (float32/float64)")
     return ap.parse_args()
 
 
@@ -292,7 +295,58 @@ def block_sizes_text():
 
 
 # --------------------------------------------------------------------------
-# B200 arm
+# output dump (--dump-outputs)
+# --------------------------------------------------------------------------
+DUMP_SAMPLES = 1 << 20      # values kept per array: 8 arrays stay under 64 MB in all
+
+
+def _sample(a, seed):
+    """`a` flattened, or DUMP_SAMPLES of its values at seeded positions (ascending) when it is larger."""
+    import numpy as np
+    flat = np.ascontiguousarray(a).reshape(-1)
+    if flat.size <= DUMP_SAMPLES:
+        return flat
+    return flat[np.sort(np.random.default_rng(seed).integers(0, flat.size, DUMP_SAMPLES))]
+
+
+def dump_outputs(path, eng):
+    """What the device-resident step leaves on the device for its caller: the u8 reconstruction and the
+    int32 coefficient plane of every plane, and every block's per-band PVQ results (gain, theta,
+    max_theta, K) in (frame, plane, y, x) order of the blocks, so that the dump does not depend on the
+    order the device lists were built in."""
+    import numpy as np
+    from daala_b200 import engine, pvq
+    os.makedirs(path, exist_ok=True)
+    out = {}
+    for p in range(3):
+        out["recon%d" % p] = _sample(eng.recon_plane(p), 10 + p).astype(np.float32)
+        out["coeffs%d" % p] = _sample(eng.coeff_plane(p), 20 + p).astype(np.float64)
+    cnt = eng.counts()
+    for name, key, seed in (("luma", "n_luma", 30), ("chroma", "n_chroma", 31)):
+        n = int(cnt[engine.CNT[key]])
+        blocks = eng.download(getattr(eng.buf, name + "_blocks"), (n,), pvq.BLOCK_DTYPE)
+        res = eng.download(getattr(eng.buf, name + "_res"), (n, 9, 4), np.int16)
+        order = np.lexsort((blocks["x0"], blocks["y0"], blocks["pli"], blocks["frame"]))
+        out[name + "_band_results"] = _sample(res[order], seed).astype(np.float32)
+    for k, v in out.items():
+        np.save(os.path.join(path, k + ".npy"), v)
+    return out
+
+
+def gpu_identity(index):
+    """Name and power limit of the GPU the numbers were measured on."""
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30)
+        name, power, sm_max = [x.strip() for x in r.stdout.strip().split(",")[:3]]
+        return {"name": name, "power_limit_w": float(power), "sm_max_mhz": float(sm_max)}
+    except (OSError, ValueError, subprocess.SubprocessError):
+        import torch
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None, "sm_max_mhz": None}
+
+
+# --------------------------------------------------------------------------
+# GPU arm
 # --------------------------------------------------------------------------
 def run_b200(args):
     import zlib
@@ -371,6 +425,8 @@ def run_b200(args):
     if rank == 0:
         sampler.start()
     ms = max_over_ranks(eng0.time_device(engine.PH_ALL, use_graph, args.steps))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng0)
     # the same with both engines' graphs in flight (inputs resident, no copies): the tail of one batch's luma
     # dependency chains overlaps the next batch's work
     ms_pipelined = None
@@ -425,12 +481,7 @@ def run_b200(args):
     value = px_job / (ms / args.steps * 1e-3) / 1e6
     e2e = px_job / (ms_e2e / args.steps * 1e-3) / 1e6
     algo_bytes = FWD_BYTES_PER_PX * geom.frame_w * geom.frame_h * F
-    peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(peaks_path):
-        peak = float(json.load(open(peaks_path))["hbm_gbs"])
-        peak_src = "measured (MEASURED_PEAKS.json)"
-    else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+    peak, peak_src = 3350.0, "H100 SXM data sheet, HBM3 (not measured)"
     achieved = algo_bytes / (ms_fwd * 1e-3) / 1e9
     dom_bytes = 20.0 * float(eng0.totals.luma_coefs)    # K_pvq = 20 B per coded coefficient (SURVEY.md 8(d))
 
@@ -439,7 +490,6 @@ def run_b200(args):
             dist.destroy_process_group()
         return
 
-    profiles = load_profile_notes()
     out = {
         "metric": METRIC, "value": round(value, 2), "unit": UNIT, "n_gpus": world, "steps": args.steps,
         "warmup": max(args.warmup, 3), "ms_per_step": round(ms / args.steps, 4), "higher_is_better": True,
@@ -466,19 +516,18 @@ def run_b200(args):
             "value": round(px_job / (ms_pipelined / args.steps * 1e-3) / 1e6, 2), "ms_per_step": round(ms_pipelined / args.steps, 4),
             "note": "both engines' graphs enqueued back to back on their own streams, inputs resident, wall clock"},
         "gpu_launches": eng0.launches_per_step() * args.steps,
+        "gpu": gpu_identity(local),
         "clocks": clocks,
         # dominant kernel by time: the persistent luma PVQ kernel -- a greedy double-precision search bound by
         # dependency latency and FP64/integer issue, not HBM; its HBM fraction is reported as the contract asks
         "roofline": {"kernel": "k_pvq_persist<intra> (luma PVQ search + H/V intra prediction wavefront)", "bound": "hbm",
                      "achieved": round(dom_bytes / (ms_dom * 1e-3) / 1e9, 1), "peak": peak, "peak_source": peak_src,
                      "unit": "GB/s", "frac": round(dom_bytes / (ms_dom * 1e-3) / 1e9 / peak, 4),
-                     "traffic": profiles.get("pvq_traffic"), "traffic_source": profiles.get("pvq_traffic_source"),
                      "algorithmic_bytes_per_launch": int(dom_bytes), "ms_per_launch": round(ms_dom, 4),
                      "note": "latency/issue-bound search; see roofline_transform for the HBM-bound kernel"},
         # the fused lapped-filter + DCT kernel the north star sets its HBM target on
         "roofline_transform": {"kernel": "k_forward_sb_tma", "bound": "hbm", "achieved": round(achieved, 1),
                                "peak": peak, "peak_source": peak_src, "unit": "GB/s", "frac": round(achieved / peak, 4),
-                               "traffic": profiles.get("fwd_traffic"), "traffic_source": profiles.get("fwd_traffic_source"),
                                "algorithmic_bytes_per_launch": int(algo_bytes), "ms_per_launch": round(ms_fwd, 4)},
         "kernels_ms": {k: round(v, 4) for k, v in phase_ms.items()},
     }
@@ -515,17 +564,6 @@ def run_b200(args):
         dist.destroy_process_group()
     if out.get("parity_failed"):
         sys.exit(1)
-
-
-def load_profile_notes():
-    """DRAM traffic per launch from the committed ncu captures (profiles/r2_traffic.json), if present."""
-    path = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if os.path.exists(path):
-        try:
-            return json.load(open(path))
-        except ValueError:
-            pass
-    return {}
 
 
 def main():

@@ -1,4 +1,4 @@
-"""daala_b200 -- B200-native (sm_100a) per-block encode hot path of xiph/daala.
+"""daala_b200 -- H100-native (sm_90a) per-block encode hot path of xiph/daala.
 
 The product is the CUDA library `libdaala_b200.so` (C ABI: include/daala_b200.h);
 this package is the thin Python host side: ctypes bindings (`_native`), frame

@@ -1,4 +1,4 @@
-"""Builds daala_b200/libdaala_b200.so (in-tree) with nvcc for sm_100a.
+"""Builds daala_b200/libdaala_b200.so (in-tree) with nvcc for sm_90a (H100).
 
 The library is the product: hand-written CUDA kernels plus the C-ABI layer of
 include/daala_b200.h.  nvcc cross-compiles without a GPU.
@@ -15,8 +15,9 @@ OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libdaala_b200.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + [
+    "-lineinfo", "-O3", "-std=c++17",
     # double-precision PVQ search must follow the reference's operation order:
     # no FMA contraction, IEEE division and square root (SURVEY.md 7.4.3)
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true",
@@ -63,7 +64,7 @@ def build(verbose=False, force=False):
         for l in logs:
             sys.stderr.write(l)
     if jobs or not os.path.exists(LIB):
-        run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+        run([NVCC, "-shared", "-o", LIB] + objs + ARCH)
     return LIB
 
 

@@ -512,6 +512,6 @@ int daala_b200_device_count(void) {
   return n;
 }
 
-const char* daala_b200_version(void) { return "daala_b200 0.1 (sm_100a)"; }
+const char* daala_b200_version(void) { return "daala_b200 0.1 (sm_90a)"; }
 
 }  // extern "C"

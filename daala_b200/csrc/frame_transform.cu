@@ -1,4 +1,4 @@
-// Fused lapped-transform frame kernels for sm_100a.
+// Fused lapped-transform frame kernels for sm_90a (H100).
 //
 // Forward  (encoder analysis), one CTA per superblock of one plane:
 //   u8 pixels -> (p-128)<<4 -> superblock-edge prefilter -> per split node
@@ -45,6 +45,7 @@ namespace daala_b200 {
 constexpr int kThreads = DAALA_XFORM_THREADS;
 constexpr int kPostThreads = 128;               // superblock-edge postfilter kernel
 constexpr int kCtasPerSm = 512 / kThreads;      // 128 registers per thread
+constexpr int kGridCap = 132 * 8;               // grid-stride kernels: 8 CTAs on each of the H100's 132 SMs
 constexpr int kMaxB = 64;            // superblock edge in luma pixels
 constexpr int kHalo = 2;             // lapping reaches 2 samples across an edge
 constexpr int kMaxT = kMaxB + 2 * kHalo;
@@ -55,7 +56,7 @@ constexpr int kMaxPitch = kMaxT + 1; // 69 = 5 mod 32; chroma 37 = 5 mod 32
 // (x, y, frame); the (B+4)^2 window of a superblock is fetched by ONE
 // cp.async.bulk.tensor issued by thread 0.  The innermost start coordinate of
 // a tiled TMA copy must be 16-byte aligned (an unaligned x raises "illegal
-// instruction" on sm_100; measured with tools/probe/tma_probe.cu), so the box
+// instruction"; measured with tools/probe/tma_probe.cu), so the box
 // starts 16 samples left of the superblock and is 96 (luma) / 64 (chroma)
 // bytes wide; the window proper begins at byte 14 of each row.  Out-of-frame
 // samples are zero filled by the hardware, so frame borders need no branches.
@@ -902,7 +903,7 @@ int daala_b200_launch_plane_sb_filter(int32_t* c, int stride, int nhsb, int nvsb
     long total = vertical_taps ? (long)nhsb * sbw * (nvsb - 1) : (long)nvsb * sbh * (nhsb - 1);
     if (total <= 0) continue;
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > kGridCap) blocks = kGridCap;
     if (post) k_plane_sb_edges<true><<<blocks, 256, 0, stream>>>(c, stride, nhsb, nvsb, sbw, sbh, vertical_taps);
     else k_plane_sb_edges<false><<<blocks, 256, 0, stream>>>(c, stride, nhsb, nvsb, sbw, sbh, vertical_taps);
   }
@@ -933,7 +934,7 @@ int daala_b200_launch_haar_blocks(int32_t* blocks, int count, int ln, int invers
 int daala_b200_launch_filter4(int32_t* v, long count, int post, cudaStream_t stream) {
   if (count <= 0) return 0;
   int blocks = (int)((count + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kGridCap) blocks = kGridCap;
   k_filter4_batch<<<blocks, 256, 0, stream>>>(v, count, post);
   return (int)cudaGetLastError();
 }
@@ -941,7 +942,7 @@ int daala_b200_launch_filter4(int32_t* v, long count, int post, cudaStream_t str
 int daala_b200_launch_lapfilter(int32_t* v, long count, int n, int post, cudaStream_t stream) {
   if (count <= 0) return 0;
   int blocks = (int)((count + 127) / 128);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kGridCap) blocks = kGridCap;
   if (n == 4) k_filter4_batch<<<blocks, 128, 0, stream>>>(v, count, post);
   else if (n == 8) k_lapfilter_batch<8><<<blocks, 128, 0, stream>>>(v, count, post);
   else if (n == 16) k_lapfilter_batch<16><<<blocks, 128, 0, stream>>>(v, count, post);

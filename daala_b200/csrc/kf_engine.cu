@@ -687,7 +687,7 @@ __device__ __forceinline__ void run_item(const Stage& S, uint32_t item, int lane
 // chunk of a dependency-free item list, the context of every band parked in an HBM record in between.
 // Why: the fused per-band code is ~50 KB of straight-line SASS plus the search loops, far beyond the
 // instruction cache; the persistent kernel spends most of its issue slots waiting for instruction fetch
-// (profiles/r2d_pvq_persist_ncu.txt: no_instruction 4.7 cycles per issued instruction).  One phase at a
+// (no_instruction is the first stall reason).  One phase at a
 // time on the whole GPU keeps the resident code small.  Only items without dependencies can go this way
 // (chroma; luma bands 3 / 6); the intra chains stay in the persistent kernel.
 struct ItemGeom {

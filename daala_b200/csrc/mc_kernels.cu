@@ -1,4 +1,4 @@
-// Motion compensation and block-matching kernels for sm_100a (8-bit path).
+// Motion compensation and block-matching kernels for sm_90a (H100, 8-bit path).
 //
 // k_obmc_blocks:    for each block of a list, up to four 1/8-pel predictions
 //                   (6-tap separable windowed-sinc interpolation) and the

@@ -399,8 +399,8 @@ __device__ int quantise_band_coop(const Group<G, E>& grp, int32_t* out, const in
   const double dist0 = best_dist;
   // One candidate list and ONE search / rate call site for both passes of pvq_theta (with-reference
   // candidates in (k, gain) order, src/pvq_encoder.c:504-560, then the no-reference gains, :573-606):
-  // the search is most of this kernel's code, and its instruction footprint is what the warps stall on
-  // (profiles/r1p_pvq_chroma_ncu.txt), so it is instantiated once.
+  // the search is most of this kernel's code, and its instruction footprint is what the warps stall on,
+  // so it is instantiated once.
   CandC items[22];
   int nitems = 0;
   if (r_nonnull && corr > 0) {

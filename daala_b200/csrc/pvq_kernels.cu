@@ -1,4 +1,4 @@
-// PVQ band quantisation kernels for sm_100a.
+// PVQ band quantisation kernels for sm_90a (H100).
 //
 // k_pvq_bands<NMAX>: one THREAD quantises one band (partition) of one
 //   transform block -- the full gain / theta / K candidate search of the
@@ -1172,7 +1172,7 @@ int daala_b200_pvq_encode_bands_mode(const daala_b200_pvq_params* prm, const uin
     return (int)cudaGetLastError();
   }
   if (mode == 0) {
-    // measured best on B200 (tools/probe/time_modes_ref.py, real with-reference data): scalar threads
+    // chosen by timing (tools/probe/time_modes_ref.py, real with-reference data): scalar threads
     // for the short bands, a whole warp (32 lanes x 4 registers, capped at 80 registers = 6 CTAs per
     // SM) for the 128-coefficient bands
     if (cls < 2) return daala_b200_pvq_encode_bands(prm, band_list, count, nmax, stream);

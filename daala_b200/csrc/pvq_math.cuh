@@ -34,7 +34,7 @@ static __constant__ double kRsqrtSmall[16] = {1.000000, 0.707107, 0.577350, 0.50
                                        0.377964, 0.353553, 0.333333, 0.316228, 0.301511, 0.288675,
                                        0.277350, 0.267261, 0.258199, 0.250000};
 // the rare large argument: out of line, the double-precision sqrt + divide sequences are long and this
-// is used inside the hottest loops (instruction-cache footprint, profiles/r1p_pvq_chroma_ncu.txt)
+// is used inside the hottest loops (instruction-cache footprint)
 static __device__ __noinline__ double rsqrt_large(int i) { return 1. / sqrt((double)i); }
 __device__ __forceinline__ double rsqrt_small_tbl(int i) {
   if (i <= 16) return kRsqrtSmall[i - 1];

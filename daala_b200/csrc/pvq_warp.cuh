@@ -6,8 +6,8 @@
 // neighbour, src/intra.c:37), so everything the reference does serially per band but is independent per
 // CANDIDATE runs one candidate per lane; (2) the greedy pulse search costs one redux.sync per pulse
 // instead of a five-level shuffle tree; (3) a small instruction footprint: the kernel is bound by
-// instruction fetch as soon as its straight-line code outgrows the 32 KB L1.5 instruction cache
-// (profiles/r2c_*), so the long double-precision sequences (log, acos, sqrt, divide) and the
+// instruction fetch as soon as its straight-line code outgrows the 32 KB L1.5 instruction cache,
+// so the long double-precision sequences (log, acos, sqrt, divide) and the
 // fixed-point helpers exist once, out of line, and only the search loop is specialised by band size.
 //
 //  * Element j of the band lives in lane j % 32, slot j / 32, in registers (1 slot for n <= 32, 4 for

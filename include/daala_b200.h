@@ -1,4 +1,4 @@
-/* daala_b200.h -- C ABI of libdaala_b200.so: a B200 (sm_100a) implementation of
+/* daala_b200.h -- C ABI of libdaala_b200.so: an H100 (sm_90a) implementation of
  * the per-block encode hot path of xiph/daala.
  *
  * Two families of entry points:

@@ -4,7 +4,7 @@
  * tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg as the
  * CHECKER.  Nothing in daala_b200/ may include, link or call this.
  * Pinned against the real reference (oracle/_ref/libdaala_ref.so, built from
- * /root/reference by oracle/Makefile) in tests/test_oracle_port.py.
+ * the reference sources by oracle/Makefile) in tests/test_oracle_port.py.
  */
 #ifndef DAALA_ORACLE_PORT_H
 #define DAALA_ORACLE_PORT_H

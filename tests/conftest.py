@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -25,5 +25,5 @@ def ref():
     from tests import oracle_lib
     lib = oracle_lib.load_ref()
     if lib is None:
-        pytest.skip("oracle/_ref/libdaala_ref.so not built (needs /root/reference)")
+        pytest.skip("oracle/_ref/libdaala_ref.so not built (needs the reference sources)")
     return lib

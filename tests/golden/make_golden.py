@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """Generates tests/golden/reference_vectors.npz by EXECUTING the reference build (oracle/_ref, compiled
-from /root/reference by oracle/Makefile) on seeded inputs.  The reference ships no golden vectors
+from the reference sources by oracle/Makefile) on seeded inputs.  The reference ships no golden vectors
 (SURVEY.md 4 / 8(c)); these are ours, so that the plain-C port (and through it the CUDA path) stays
 pinned where oracle/_ref cannot be rebuilt.  Run from the repo root:  python tests/golden/make_golden.py
+(`... make_golden.py digests` writes tests/golden/reference_digests.npz instead).
 
 Inputs are stored next to the outputs (not regenerated from seeds), except for whole planes, which are
 rebuilt by daala_b200.synth (deterministic integer generator) and stored as CRC-32 of the reference output.
@@ -125,7 +126,7 @@ def real_map_crcs(lib, prefix, qm, qm_inv, bsize):
 
 def main():
     ref = oracle_lib.load_ref()
-    assert ref is not None, "needs oracle/_ref (make -C oracle ref, with /root/reference present)"
+    assert ref is not None, "needs oracle/_ref (make -C oracle ref, with the reference sources present)"
     rng = np.random.default_rng(20260923)
     g = {}
     # 2-D DCTs, Haar
@@ -235,5 +236,68 @@ def main():
     print("wrote %s (%d arrays, %d bytes)" % (path, len(g), os.path.getsize(path)))
 
 
+THETA_SETS = [("seed%d" % s, dict(seed=s, per_combo=3)) for s in (1, 2, 3, 4, 5)] + [("large_k", None)]
+
+
+def theta_case_set(name):
+    """The pvq_theta cases of tests/test_emu_pvq_warp.py recorded under `name`."""
+    kw = dict(THETA_SETS)[name]
+    return pvq_cases.large_k_cases() if kw is None else pvq_cases.cases(**kw)
+
+
+def tf_cases():
+    """Seeded calls of the TF helpers (src/tf.c:38-277) with strided source and destination, every size the
+    codec's blocks can take: (name, destination shape, source, trailing arguments)."""
+    rng = np.random.default_rng(5)
+
+    def case(name, shape_dst, shape_src, *args):
+        return name, shape_dst, rng.integers(-4000, 4000, size=shape_src).astype(np.int32), args
+
+    for n in (4, 8, 16, 32, 64):
+        h = n // 2
+        yield case("od_tf_up_h_lp", (n, n + 2), (n, n + 5), h, n)
+        yield case("od_tf_up_v_lp", (n, n + 2), (n, n + 5), h, n)
+        yield case("od_tf_up_hv_lp", (n, n + 2), (n, n + 5), h, h, n)
+        yield case("od_tf_down_hv", (n, n + 2), (n, n + 5), n)
+        yield case("od_tf_filter_2d", (n, n + 2), (n, n + 5), n)
+        yield case("od_tf_filter_inv_2d", (n, n + 2), (n, n + 5), n)
+    for n in (4, 8, 16, 32):
+        yield case("od_tf_up_hv", (2 * n, 2 * n + 1), (2 * n, 2 * n + 3), n)
+    for cur in range(5):
+        for dest in range(cur + 1):
+            for filt in (0, 1):
+                n = 4 << cur
+                yield case("od_convert_block_down", (n, n + 1), (n, n + 3), cur, dest, filt)
+
+
+def run_tf(lib, case):
+    """One tf_cases() call through `lib`; the destination starts filled with 77 so that stray writes show."""
+    name, shape_dst, src, args = case
+    d = np.full(shape_dst, 77, np.int32)
+    getattr(lib, name)(addr(d), shape_dst[1], addr(src), src.shape[1], *args)
+    return d
+
+
+def main_digests():
+    """tests/golden/reference_digests.npz: the reference's pvq_theta (speed = 1) on every case the device
+    quantiser's CPU emulation is checked on, as pvq_cases.digest rows and skip_diff, and the CRC-32 of
+    every tf_cases() result of the reference's TF helpers."""
+    ref = oracle_lib.load_ref()
+    assert ref is not None, "needs oracle/_ref (make -C oracle ref, with the reference sources present)"
+    qm, qm_inv = pvq_cases.reference_qm(ref)
+    g = {}
+    for name, _ in THETA_SETS:
+        rows, sd = [], []
+        for c in theta_case_set(name):
+            a = pvq_cases.run_theta(ref, "ref", c, qm, qm_inv)
+            rows.append(pvq_cases.digest(a))
+            sd.append(a["skip_diff"])
+        g[name], g[name + "_skip_diff"] = np.array(rows, np.int64), np.array(sd, np.float64)
+    g["tf_crc"] = np.array([crc(run_tf(ref, c)) for c in tf_cases()], np.uint32)
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_digests.npz")
+    np.savez_compressed(path, **g)
+    print("wrote %s (%d arrays, %d bytes)" % (path, len(g), os.path.getsize(path)))
+
+
 if __name__ == "__main__":
-    main()
+    main_digests() if sys.argv[1:] == ["digests"] else main()

@@ -1,6 +1,7 @@
 """Seeded PVQ band test cases shared by the CPU pin tests and the GPU parity
 tests (test infrastructure)."""
 import ctypes
+import zlib
 
 import numpy as np
 
@@ -87,3 +88,19 @@ def run_theta(lib, prefix, c, qm, qm_inv):
     ny = n if it.value == -1 else n - 1
     return dict(gain=g, itheta=it.value, max_theta=mt.value, k=vk.value, y=y[:ny].copy(), out=out,
                 skip_diff=sd.value)
+
+
+def large_k_cases():
+    """Fine quantisers on large vectors: K in the hundreds to thousands (all-RDO searches, 64-bit sums)."""
+    rng = np.random.default_rng(7)
+    for q0 in (16, 40, 500, 620):
+        for n in (8, 15, 32, 128):
+            for kf, pli in ((1, 0), (1, 1), (0, 0)):
+                x0, r0 = make_band(rng, n, "big")
+                yield dict(n=n, kind="big", is_keyframe=kf, pli=pli, beta=4096, q0=q0, x0=x0, r0=r0, qm_off=5, lam=0.147)
+
+
+def digest(r):
+    """[gain, itheta, max_theta, K, CRC-32 of the pulses and the synthesised band] of a run_theta result."""
+    vec = np.ascontiguousarray(r["y"], np.int32).tobytes() + np.ascontiguousarray(r["out"], np.int32).tobytes()
+    return [int(r["gain"]), int(r["itheta"]), int(r["max_theta"]), int(r["k"]), zlib.crc32(vec) & 0xffffffff]

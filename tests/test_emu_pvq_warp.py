@@ -1,6 +1,7 @@
 """The warp-per-band PVQ quantiser of the device (daala_b200/csrc/pvq_warp.cuh) compiled for the host
 on a SIMT emulation (tests/emu/simt_emu.h: 32 fibres, warp collectives as rendezvous) and pinned
-against the reference build's pvq_theta -- the same source the CUDA kernels include, so the candidate
+against the reference build's pvq_theta, whose results on these cases tests/golden/make_golden.py recorded
+in tests/golden/reference_digests.npz -- the same source the CUDA kernels include, so the candidate
 parallelisation, the event order and the redux-screened pulse search are checked on the CPU."""
 import ctypes
 import os
@@ -9,12 +10,14 @@ import subprocess
 import numpy as np
 import pytest
 
-from tests import oracle_lib, pvq_cases
+from tests import pvq_cases
+from tests.golden import make_golden
 from tests.oracle_lib import addr
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 BUILD = os.path.join(HERE, "emu", "_build")
+GOLDEN = os.path.join(HERE, "golden")
 
 
 def _build(name, extra):
@@ -48,9 +51,22 @@ def _run(emu, c, qm, qm_inv):
     return dict(gain=g, itheta=it.value, max_theta=mt.value, k=vk.value, y=y[:ny].copy(), out=out, skip_diff=sd.value)
 
 
-def _same(a, b):
-    return (all(a[k] == b[k] for k in ("gain", "itheta", "max_theta", "k", "skip_diff")) and np.array_equal(a["y"], b["y"])
-            and np.array_equal(a["out"], b["out"]))
+def _reference_qm():
+    g = np.load(os.path.join(GOLDEN, "reference_vectors.npz"))
+    return g["qm"], g["qm_inv"]
+
+
+def _check_case_set(emu, name, qm, qm_inv):
+    """Runs the emulated quantiser on the recorded case set `name`; returns the reference's K of every case."""
+    gold = np.load(os.path.join(GOLDEN, "reference_digests.npz"))
+    rows, skip_diff = gold[name], gold[name + "_skip_diff"]
+    cases = list(make_golden.theta_case_set(name))
+    assert len(cases) == len(rows)
+    for c, want, want_sd in zip(cases, rows.tolist(), skip_diff.tolist()):
+        got = _run(emu, c, qm, qm_inv)
+        assert pvq_cases.digest(got) == want and got["skip_diff"] == want_sd, (
+            {k: c[k] for k in ("n", "kind", "is_keyframe", "pli", "beta", "q0", "lam")}, want, want_sd, got)
+    return rows[:, 3]
 
 
 # the second build lowers the "products are exact" bound so that the literal-scan path of the plain
@@ -63,7 +79,6 @@ def _same(a, b):
                                                     ("libpvq_warp_emu.so", [], (4,), True),
                                                     ("libpvq_warp_emu.so", [], (5,), "prepass")])
 def test_warp_quantiser_matches_reference(name, extra, seeds, split, monkeypatch):
-    ref = oracle_lib.load_ref()
     emu = _build(name, extra)
     # "prepass": keyframe luma bands with their no-reference events searched ahead of time and imported
     monkeypatch.delenv("DAALA_B200_EMU_SPLIT", raising=False)
@@ -72,15 +87,11 @@ def test_warp_quantiser_matches_reference(name, extra, seeds, split, monkeypatch
         monkeypatch.setenv("DAALA_B200_EMU_PREPASS", "1")
     elif split:
         monkeypatch.setenv("DAALA_B200_EMU_SPLIT", "1")
-    qm, qm_inv = pvq_cases.reference_qm(ref)
+    qm, qm_inv = _reference_qm()
     stats = (ctypes.c_longlong * 4).in_dll(emu, "daala_b200_pvq_warp_stats")
     n = 0
     for seed in seeds:
-        for c in pvq_cases.cases(seed=seed, per_combo=3):
-            want = pvq_cases.run_theta(ref, "ref", c, qm, qm_inv)
-            got = _run(emu, c, qm, qm_inv)
-            assert _same(want, got), ({k: c[k] for k in ("n", "kind", "is_keyframe", "pli", "beta", "q0", "lam")}, want, got)
-            n += 1
+        n += len(_check_case_set(emu, "seed%d" % seed, qm, qm_inv))
     # coverage: unique-contender fast path, both exact fallbacks, and (second build) the literal scan
     assert n >= 400 and stats[0] > 0 and stats[1] > 0 and stats[2] > 0
     if extra:
@@ -89,18 +100,7 @@ def test_warp_quantiser_matches_reference(name, extra, seeds, split, monkeypatch
 
 def test_warp_quantiser_large_k():
     """Fine quantisers on large vectors: K in the hundreds to thousands (all-RDO searches, 64-bit sums)."""
-    ref = oracle_lib.load_ref()
     emu = _build("libpvq_warp_emu.so", [])
-    qm, qm_inv = pvq_cases.reference_qm(ref)
-    rng = np.random.default_rng(7)
-    kmax = 0
-    for q0 in (16, 40, 500, 620):
-        for n in (8, 15, 32, 128):
-            for kf, pli in ((1, 0), (1, 1), (0, 0)):
-                x0, r0 = pvq_cases.make_band(rng, n, "big")
-                c = dict(n=n, kind="big", is_keyframe=kf, pli=pli, beta=4096, q0=q0, x0=x0, r0=r0, qm_off=5, lam=0.147)
-                want = pvq_cases.run_theta(ref, "ref", c, qm, qm_inv)
-                got = _run(emu, c, qm, qm_inv)
-                assert _same(want, got), (q0, n, kf, pli, want, got)
-                kmax = max(kmax, want["k"])
-    assert kmax > 1000
+    qm, qm_inv = _reference_qm()
+    ks = _check_case_set(emu, "large_k", qm, qm_inv)
+    assert len(ks) == 48 and ks.max() > 1000

@@ -1,7 +1,6 @@
 """HotPath with the work lists built on the device (daala_b200/lists_torch.py) against the numpy-built
-lists: identical planes.  The tensor-op construction is verified on CPU tensors
-(tests/test_host_logic.py); its CUDA execution has not been exercised yet (round 1 ran out of GPU
-budget), first ran on a B200 in round 2."""
+lists: identical planes.  The tensor-op construction is also verified on CPU tensors
+(tests/test_host_logic.py)."""
 import os
 
 import numpy as np

@@ -1,8 +1,5 @@
 """GPU parity of the distortion kernel (csrc/dist_kernels.cu) against the pinned CPU oracle
-(oracle/port_dist.c, bit-identical to od_compute_dist by tests/test_oracle_dering.py).
-
-The kernel was written after round 1's GPU budget was spent and has not run on a device yet: the test
-first ran on a B200 in round 2."""
+(oracle/port_dist.c, bit-identical to od_compute_dist by tests/test_oracle_dering.py)."""
 import ctypes
 import os
 

@@ -17,7 +17,7 @@ REF = os.path.join(ROOT, "oracle", "_ref", "libdaala_ref.so")
 
 def _run(w, h, nframes, timeout):
     if not (os.path.exists(EXE) and os.path.exists(REF)):
-        pytest.skip("oracle/_ref/daala_dropin_test not built (needs /root/reference in the build container)")
+        pytest.skip("oracle/_ref/daala_dropin_test not built (needs the reference sources)")
     r = subprocess.run([EXE, REF, str(w), str(h), str(nframes)], capture_output=True, text=True, timeout=timeout)
     print(r.stdout)
     assert r.returncode == 0, (r.stdout[-2000:], r.stderr[-2000:])

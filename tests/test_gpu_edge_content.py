@@ -1,6 +1,5 @@
 """Edge-case pictures (SURVEY.md 8(d): flat-128, pure noise; plus saturated black / white) through the
-device keyframe chain against the oracle.  Added after round 1's GPU budget was spent: same kernels as
-the verified tests, new inputs. First run on a B200 in round 2."""
+device keyframe chain against the oracle: same kernels as the other tests, new inputs."""
 import os
 
 import numpy as np

@@ -1,6 +1,7 @@
 """GPU parity of the fused lapped-transform kernels (through the C ABI of
 libdaala_b200.so) against the CPU oracle: bit-exact, integer work."""
 import ctypes
+import os
 import zlib
 
 import numpy as np
@@ -274,44 +275,30 @@ def test_tma_and_plain_load_forward_agree(torch_cuda):
 
 def test_dropin_tf_symbols_match_reference(torch_cuda):
     """The TF helpers of src/tf.c:38-277 with host pointers (csrc/tf_kernels.cu) against the reference
-    build's own functions, strided source and destination, every size the codec's blocks can take; the
-    reversibility the reference documents (od_tf_down_hv inverts od_tf_up_hv, the inverse filter undoes
-    the filter) is checked on the device results as well."""
+    build's own functions (their results recorded as CRC-32 in tests/golden/reference_digests.npz by
+    tests/golden/make_golden.py), strided source and destination, every size the codec's blocks can take;
+    the reversibility the reference documents (od_tf_down_hv inverts od_tf_up_hv, the inverse filter
+    undoes the filter) is checked on the device results as well."""
     from daala_b200 import _native
+    from tests.golden import make_golden
     L = _native.lib()
-    ref = oracle_lib.load_ref()
     a = oracle_lib.addr
-    rng = np.random.default_rng(5)
-
-    def both(name, shape_dst, shape_src, *args):
-        src = (rng.integers(-4000, 4000, size=shape_src)).astype(np.int32)
-        d_gpu = np.full(shape_dst, 77, np.int32)
-        d_cpu = np.full(shape_dst, 77, np.int32)
-        getattr(L, name)(a(d_gpu), shape_dst[1], a(src), shape_src[1], *args)
-        getattr(ref, name)(a(d_cpu), shape_dst[1], a(src), shape_src[1], *args)
-        assert np.array_equal(d_gpu, d_cpu), name
-        return src, d_gpu
-
-    for n in (4, 8, 16, 32, 64):
-        h = n // 2
-        both("od_tf_up_h_lp", (n, n + 2), (n, n + 5), h, n)
-        both("od_tf_up_v_lp", (n, n + 2), (n, n + 5), h, n)
-        both("od_tf_up_hv_lp", (n, n + 2), (n, n + 5), h, h, n)
-        both("od_tf_down_hv", (n, n + 2), (n, n + 5), n)
-        both("od_tf_filter_2d", (n, n + 2), (n, n + 5), n)
-        src, f = both("od_tf_filter_inv_2d", (n, n + 2), (n, n + 5), n)
-        back = np.zeros((n, n), np.int32)
-        fc = np.ascontiguousarray(f[:, :n])
-        L.od_tf_filter_2d(a(back), n, a(fc), n, n)
-        assert np.array_equal(back, src[:, :n])
-    for n in (4, 8, 16, 32):
-        src, up = both("od_tf_up_hv", (2 * n, 2 * n + 1), (2 * n, 2 * n + 3), n)
-        down = np.zeros((2 * n, 2 * n), np.int32)
-        upc = np.ascontiguousarray(up[:, :2 * n])
-        L.od_tf_down_hv(a(down), 2 * n, a(upc), 2 * n, 2 * n)
-        assert np.array_equal(down, src[:, :2 * n])
-    for cur in range(5):
-        for dest in range(cur + 1):
-            for filt in (0, 1):
-                n = 4 << cur
-                both("od_convert_block_down", (n, n + 1), (n, n + 3), cur, dest, filt)
+    gold = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_digests.npz")
+    want = np.load(gold)["tf_crc"].tolist()
+    cases = list(make_golden.tf_cases())
+    assert len(cases) == len(want)
+    for case, crc in zip(cases, want):
+        name, _, src, args = case
+        d = make_golden.run_tf(L, case)
+        assert make_golden.crc(d) == crc, (name, src.shape, args)
+        n = args[-1]
+        if name == "od_tf_filter_inv_2d":
+            back = np.zeros((n, n), np.int32)
+            fc = np.ascontiguousarray(d[:, :n])   # keep alive across the call
+            L.od_tf_filter_2d(a(back), n, a(fc), n, n)
+            assert np.array_equal(back, src[:, :n])
+        if name == "od_tf_up_hv":
+            down = np.zeros((2 * n, 2 * n), np.int32)
+            upc = np.ascontiguousarray(d[:, :2 * n])
+            L.od_tf_down_hv(a(down), 2 * n, a(upc), 2 * n, 2 * n)
+            assert np.array_equal(down, src[:, :2 * n])

@@ -327,7 +327,7 @@ def test_dropin_link_test_binary_resolves_filter_and_dct_symbols_from_the_librar
     dynamic linker takes it from the library) and the vtable initialisers must come from the shim."""
     exe = os.path.join(ROOT, "oracle", "_ref", "daala_dropin_test")
     if not os.path.exists(exe):
-        pytest.skip("oracle/_ref/daala_dropin_test not built (needs /root/reference)")
+        pytest.skip("oracle/_ref/daala_dropin_test not built (needs the reference sources)")
     syms = subprocess.run(["nm", exe], capture_output=True, text=True, check=True).stdout.splitlines()
     kind = {ln.split()[-1]: ln.split()[-2] for ln in syms if len(ln.split()) >= 2}
     for name in ("od_apply_prefilter_frame_sbs", "od_apply_postfilter_frame_sbs", "od_prefilter_split",

@@ -1,5 +1,5 @@
 """Y4M in -> keyframe engine (GPU) -> reconstructed Y4M out + symbol statistics: the data path of
-`encoder_example -v <quant> -k 1` (all-intra) without the entropy coder.  Needs a B200.
+`encoder_example -v <quant> -k 1` (all-intra) without the entropy coder.  Needs an H100.
 
   python tools/encode_y4m.py in.y4m recon.y4m [--q0 72] [--batch 16] [--bsize 3] [--dering 2]
 

@@ -9,7 +9,7 @@ od_bin_fdct32 :4219, od_bin_idct32 :4321, od_bin_fdct64 :4422, od_bin_idct64
 be bit-exact.  This script turns each function into a flat, scope-free list of
 register operations (our own IR, written to daala_b200/csrc/gen/dct_ir.json).
 All code generation (CUDA device functions, the plain-C oracle port) starts
-from that IR -- see tools/gen_dct.py.  /root/reference is needed only when the
+from that IR -- see tools/gen_dct.py.  The reference sources are needed only when the
 IR is (re)extracted, never at build or run time.
 
 How: the C preprocessor expands the macro tree (with OD_DCT_RSHIFT kept
@@ -26,7 +26,7 @@ import tempfile
 
 from pycparser import c_ast, c_parser
 
-REF = os.environ.get("DAALA_REF", "/root/reference")
+REF = os.environ.get("DAALA_REF", os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "reference"))
 OUT = os.path.join(os.path.dirname(__file__), "..", "daala_b200", "csrc", "gen", "dct_ir.json")
 
 PRELUDE = """

@@ -2,7 +2,7 @@
 """Dev-time tool: block-size maps the WHOLE reference encoder decides (public API, OD_SET_QUANT 20,
 complexity 7 -- BASELINE.json's configuration) for bench.py's four synthetic 3840x2160 frames, saved as
 daala_b200/data/bench_bsize_4k.npz for `bench.py --block-sizes reference`.  Needs oracle/_ref
-(i.e. /root/reference); the saved maps travel with the repository."""
+(i.e. the reference sources); the saved maps travel with the repository."""
 import ctypes
 import os
 import sys

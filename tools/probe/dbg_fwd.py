@@ -1,5 +1,5 @@
-import sys, zlib, numpy as np, torch
-sys.path.insert(0, '/root/repo')
+import os, sys, zlib, numpy as np, torch
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 from daala_b200 import synth
 from daala_b200.frame import FrameBuffers, Geometry
 from tests import frame_oracle, oracle_lib

@@ -1,5 +1,5 @@
 #!/bin/bash
-# tiny end-to-end run of tools/encode_y4m.py on a B200 (synthetic 3-frame 200x130 clip)
+# tiny end-to-end run of tools/encode_y4m.py on an H100 (synthetic 3-frame 200x130 clip)
 set -e
 python - <<'PY'
 import sys; sys.path.insert(0, '.')
