@@ -176,7 +176,8 @@ __global__ void __launch_bounds__(1024) k_tile_scan(const __grid_constant__ List
     L.cnt[kTotalHi] = 0;
     L.cnt[kNHeads] = 0;
     L.cnt[kNHeads0] = 0;
-    if (tot.x > L.max_luma || 2 * tot.z > L.max_chroma) L.cnt[kError] = 1;
+    // set on every step, so that an over-capacity batch does not flag the batches after it
+    L.cnt[kError] = tot.x > L.max_luma || 2 * tot.z > L.max_chroma ? 1 : 0;
   }
 }
 
@@ -1720,6 +1721,14 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   if (!kf || !io) return (int)cudaErrorInvalidValue;
   cudaStream_t s = kf->stream;
   const int F = kf->F;
+  if (!io->bsize) return (int)cudaErrorInvalidValue;
+  // refuse a batch with more blocks than the work lists hold before anything is copied or launched: the
+  // step would otherwise run on truncated lists
+  daala_b200_kf_totals tot;
+  if (io->totals) tot = *io->totals;
+  else daala_b200_kf_count_blocks(io->bsize, F, (long long)kf->nhsb * 8 * kf->nvsb * 8, kf->nhsb * 8, kf->nhsb, kf->nvsb,
+                                  kf->cfg.sb_row0, kf->cfg.sb_rows, &tot);
+  if (tot.n_luma > kf->lists.max_luma || tot.n_chroma > kf->lists.max_chroma) return (int)cudaErrorInvalidValue;
   for (int p = 0; p < 3; p++) {
     if (!io->pixels[p]) return (int)cudaErrorInvalidValue;
     KF_CHECK(cudaMemcpyAsync(kf->pixels[p], io->pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
@@ -1740,11 +1749,6 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     if (rc) return rc;
     KF_CHECK(cudaEventRecord(g_last_compute, s));
   }
-  daala_b200_kf_totals tot;
-  if (io->totals) tot = *io->totals;
-  else daala_b200_kf_count_blocks(io->bsize, F, (long long)kf->nhsb * 8 * kf->nvsb * 8, kf->nhsb * 8, kf->nhsb, kf->nvsb,
-                                  kf->cfg.sb_row0, kf->cfg.sb_rows, &tot);
-  if (tot.n_luma > kf->lists.max_luma || tot.n_chroma > kf->lists.max_chroma) return (int)cudaErrorInvalidValue;
   for (int p = 0; p < 3; p++)
     if (io->pixels_out[p])
       KF_CHECK(cudaMemcpyAsync(io->pixels_out[p], kf->pixels_out[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,

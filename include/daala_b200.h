@@ -566,7 +566,9 @@ int daala_b200_kf_time_device(daala_b200_kf *kf, int phases, int use_graph, int 
 /* Host-side totals implied by block-size maps (sizes of the result arrays). */
 int daala_b200_kf_count_blocks(const uint8_t *bsize, int nframes, long long frame_pitch, int bstride, int nhsb,
                                int nvsb, int sb_row0, int sb_rows, daala_b200_kf_totals *out);
-/* H2D of the inputs, the whole step, D2H of the requested outputs: enqueued, not waited for. */
+/* H2D of the inputs, the whole step, D2H of the requested outputs: enqueued, not waited for.  A batch with more
+   luma or chroma blocks than the engine's capacity (see max_blocks_div) returns cudaErrorInvalidValue before
+   anything is copied or launched. */
 int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
 int daala_b200_kf_wait(daala_b200_kf *kf);
 int daala_b200_kf_encode(daala_b200_kf *kf, const daala_b200_kf_io *io);   /* submit + wait */

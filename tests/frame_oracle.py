@@ -65,11 +65,14 @@ def pvq_plane_pred(lib, prefix, d, geom, pli, bsize, q0, use_masking, lam, qm, q
 
 
 def keyframe_chain(lib, prefix, planes, geom, bsize, q0, qm_q4, use_masking=1, lam=0.147, qm=None, qm_inv=None,
-                   record=True, dering_levels=None, dering_search=None):
+                   record=True, dering_levels=None, dering_search=None, symbols=False):
     """One keyframe through the oracle's whole chain (forward -> PVQ with luma H/V intra prediction and
     chroma CfL -> inverse).  Returns per plane a dict: dq (quantised coefficient plane), recon (u8),
     stats, and with record=True rec ([h/4, w/4, 9, 4] int16 band decisions at each block's origin,
     -32768 where no band) and yplane (pulse vectors in raster order).
+    symbols=True adds, at each block's origin in 4-sample units like rec, skip_diff ([h/4, w/4] float64,
+    NaN where no block starts) and flip ([h/4, w/4] int32: the keyframe CfL sign flip, 0 or 1; -1 where no
+    block starts).
     dering_levels: [nvsb, nhsb] levels -> reconstruction through the deringing application.
     dering_search: dict(coded_quantizer=, dering_lambda=, qm=1) -> the levels are searched the way the encoder does
     (src/encode.c:2708-2811, reference build only) and returned as out[0]["dering_levels"]."""
@@ -88,15 +91,22 @@ def keyframe_chain(lib, prefix, planes, geom, bsize, q0, qm_q4, use_masking=1, l
         rec = np.full((ph // 4, pw // 4, 9, 4), -32768, np.int16) if record else None
         yplane = np.zeros((ph, pw), np.int32) if record else None
         lp = addr(np.ascontiguousarray(luma_q, dtype=np.int32)) if pli else None
-        fn = getattr(lib, "oracle_%s_pvq_plane_rec" % prefix)
-        fn(addr(d), None, geom.nhsb, geom.nvsb, geom.xdec[pli], pli, addr(bs), bs.shape[1], int(q0), 1,
-           int(use_masking), ctypes.c_double(lam), addr(np.ascontiguousarray(qm)),
-           addr(np.ascontiguousarray(qm_inv)), addr(q4), addr(stats), 1 if pli == 0 else 0, lp,
-           addr(rec) if record else None, addr(yplane) if record else None)
+        args = [addr(d), None, geom.nhsb, geom.nvsb, geom.xdec[pli], pli, addr(bs), bs.shape[1], int(q0), 1,
+                int(use_masking), ctypes.c_double(lam), addr(np.ascontiguousarray(qm)),
+                addr(np.ascontiguousarray(qm_inv)), addr(q4), addr(stats), 1 if pli == 0 else 0, lp,
+                addr(rec) if record else None, addr(yplane) if record else None]
+        if symbols:
+            skip = np.full((ph // 4, pw // 4), np.nan, np.float64)
+            flip = np.full((ph // 4, pw // 4), -1, np.int32)
+            getattr(lib, "oracle_%s_pvq_plane_sym" % prefix)(*args, addr(skip), addr(flip))
+        else:
+            getattr(lib, "oracle_%s_pvq_plane_rec" % prefix)(*args)
         if pli == 0:
             luma_q = d
         recon = inverse_plane(lib, prefix, d, geom, pli, bsize, 1) if dering_levels is None and dering_search is None else None
         out.append(dict(dq=d, recon=recon, stats=stats, rec=rec, yplane=yplane))
+        if symbols:
+            out[-1].update(skip_diff=skip, flip=flip)
     if dering_levels is not None:
         # reconstruction with the deringing application (levels [nvsb, nhsb] given): oracle/pipeline_driver.inc
         ds = [np.ascontiguousarray(o["dq"], np.int32).copy() for o in out]

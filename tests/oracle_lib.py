@@ -12,9 +12,12 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ORACLE = os.path.join(ROOT, "oracle")
-# a checkout of the xiph/daala sources, by default next to this repository; without it the checker
-# libraries under oracle/_ref are used as they are (or are absent)
-REF_SRC = os.environ.get("DAALA_REF", os.path.join(os.path.dirname(ROOT), "reference"))
+# a checkout of the xiph/daala sources: the one named by DAALA_REF, else one next to this repository, else the
+# read-only system-wide checkout at /root/reference; without any of them the checker libraries under oracle/_ref
+# are used as they are (or are absent)
+_REF_CANDIDATES = ([os.environ["DAALA_REF"]] if os.environ.get("DAALA_REF") else
+                   [os.path.join(os.path.dirname(ROOT), "reference"), "/root/reference"])
+REF_SRC = next((p for p in _REF_CANDIDATES if os.path.isdir(os.path.join(p, "src"))), _REF_CANDIDATES[0])
 
 c_int = ctypes.c_int
 c_double = ctypes.c_double

@@ -83,6 +83,72 @@ def _frames(geom, n, q_seed=0, mode="mixed", pic=None):
     return frames
 
 
+def _zorder_map(geom, nframes, sizes):
+    """Block-size maps [F, UH, UW] with the blocks `sizes` (values 0..4, largest first) laid out one after the
+    other in z-order through the superblocks of frame 0, then frame 1, ...  Sizes are powers of four units and
+    come in descending order, so every block lands on a position aligned to its size."""
+    bh, bw = geom.bsize_shape
+    maps = np.full((nframes, bh, bw), 255, np.uint8)
+    sbs = [(f, sy, sx) for f in range(nframes) for sy in range(geom.nvsb) for sx in range(geom.nhsb)]
+    pos = 0
+    for b in sorted(sizes, reverse=True):
+        units = 1 if b == 0 else 4 ** (b - 1)
+        f, sy, sx = sbs[pos // 64]
+        z = pos % 64
+        uy = sum(((z >> (2 * i + 1)) & 1) << i for i in range(3))
+        ux = sum(((z >> (2 * i)) & 1) << i for i in range(3))
+        n = 1 if b == 0 else 1 << (b - 1)
+        maps[f, sy * 8 + uy:sy * 8 + uy + n, sx * 8 + ux:sx * 8 + ux + n] = b
+        pos += units
+    assert pos == 64 * len(sbs) and (maps != 255).all()
+    return maps
+
+
+@pytest.mark.parametrize("binding", ["luma", "chroma"])
+def test_engine_block_capacity_boundary(binding):
+    """max_blocks_div = 2 halves the work-list capacities.  A batch whose luma (or chroma) block count equals
+    the capacity exactly is encoded bit-exactly; the same batch with a few more blocks is refused by submit
+    before anything runs, and the next valid batch on the same engine is exact again."""
+    from daala_b200 import _native, engine, synth
+    from daala_b200.frame import Geometry
+    F = 2
+    if binding == "luma":
+        # 75 4x4 units, 9 8x8 blocks, 11 16x16 blocks over 128 units: 320 luma and 190 chroma blocks
+        geom = Geometry(64, 64)
+        sizes = [0] * 75 + [1] * 9 + [2] * 11
+        over = [0] * 76 + [1] * 8 + [2] * 11          # one 8x8 unit more as four 4x4 blocks: 3 luma blocks more
+    else:
+        # 128 8x8 blocks, 32 16x16 blocks over 256 units: 160 luma and 320 chroma blocks
+        geom = Geometry(128, 64)
+        sizes = [1] * 128 + [2] * 32
+        over = [1] * 132 + [2] * 31                   # one 16x16 block split into 8x8 blocks: 6 chroma blocks more
+    q0, q4 = 72, np.full((3, 30), 16, np.uint8)
+    eng = engine.KeyframeEngine(geom, nframes=F, q0=q0, pvq_qm_q4=q4, split_free=1, max_blocks_div=2)
+    cap = {"luma": eng.buf.max_luma_blocks, "chroma": eng.buf.max_chroma_blocks}
+    nunits = F * geom.bsize_shape[0] * geom.bsize_shape[1]
+    assert cap == {"luma": nunits * 2 + 64, "chroma": nunits + 64}
+    maps, over_maps = _zorder_map(geom, F, sizes), _zorder_map(geom, F, over)
+    tot, tot_over = eng.count_blocks(maps), eng.count_blocks(over_maps)
+    n = {"luma": tot.n_luma, "chroma": tot.n_chroma}
+    n_over = {"luma": tot_over.n_luma, "chroma": tot_over.n_chroma}
+    other = "chroma" if binding == "luma" else "luma"
+    assert n[binding] == cap[binding] and n[other] <= cap[other], (n, cap)
+    assert n_over[binding] > cap[binding] and n_over[other] <= cap[other], (n_over, cap)
+    frames = _frames(geom, F, q_seed=11)
+    exact = [(frames[f][0], maps[f]) for f in range(F)]
+    out = _check_batch(eng, geom, exact, q0, q4)
+    assert int(out["counts"][engine.CNT["n_luma"]]) == n["luma"] and int(out["counts"][engine.CNT["error"]]) == 0
+    # over capacity: refused with cudaErrorInvalidValue (1) before any copy or launch
+    eng.stage_inputs([np.stack([f[0][p] for f in frames]) for p in range(3)], over_maps)
+    eng.prepare_io()
+    with pytest.raises(_native.CudaError, match="cudaError 1 "):
+        eng.submit()
+    # the engine is still usable, and its counters do not carry an error over
+    out = _check_batch(eng, geom, [(f[0], m) for f, m in zip(_frames(geom, F, q_seed=12), maps)], q0, q4)
+    assert int(out["counts"][engine.CNT["error"]]) == 0
+    eng.close()
+
+
 def test_engine_lists_are_consistent():
     """Descriptors partition the coding-order buffers; neighbours are the same-size top / left blocks;
     the item lists hold every dependency-free (block, band) once, the chain heads are the chain items without a
