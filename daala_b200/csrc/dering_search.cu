@@ -173,7 +173,8 @@ extern "C" int daala_b200_dering_decide(const double* dist, int nhdr, int nvdr, 
 }
 
 extern "C" int daala_b200_dering_plane_batch(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
-                                             long long x_pitch, long long dir_pitch, long long thr_pitch, void* stream);
+                                             long long x_pitch, long long dir_pitch, long long thr_pitch, uint8_t* y8,
+                                             void* stream);
 
 extern "C" int daala_b200_dering_search(const daala_b200_dering_search_params* p, uint16_t* cdf, int increment,
                                         uint8_t* levels, double* dist_out, void* stream_) {
@@ -282,7 +283,7 @@ extern "C" int daala_b200_dering_search_enqueue(const daala_b200_dering_search_b
       dp.overlap = 1;
       dp.coeff_shift = 4;
       dp.dir_format = gi == 1 ? 1 : 2;   // the direction search runs once; later passes re-use direction and variance
-      const int r = daala_b200_dering_plane_batch(&dp, F, filt_pitch, b->etmp_pitch, (long long)nsb * 64, 0, st);
+      const int r = daala_b200_dering_plane_batch(&dp, F, filt_pitch, b->etmp_pitch, (long long)nsb * 64, 0, nullptr, st);
       if (r) return r;
       plane = b->filt;
       ppitch = filt_pitch;

@@ -967,14 +967,8 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
 // od_encode_coefficients' final deringing application (src/encode.c:2812-2842) with the per-superblock levels
 // given by the caller (the level SEARCH is serial: CDF adaptation + neighbour context; like the block sizes its
 // result is an input of the hot path): etmp = ctmp after the SB-edge postfilter, od_dering of every superblock
-// with threshold = OD_DERING_GAIN_TABLE[level] * quantizer^0.84182 (* 0.6 on chroma), od_coeff_to_ref_plane.
-// (c + 8 >> 4) + 128 clamped: od_coeff_to_ref_plane, src/state.c:1283
-__global__ void k_i16_to_u8(const int16_t* __restrict__ src, uint8_t* __restrict__ dst, long n) {
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-    const int v = ((src[i] + 8) >> 4) + 128;
-    dst[i] = (uint8_t)(v < 0 ? 0 : v > 255 ? 255 : v);
-  }
-}
+// with threshold = OD_DERING_GAIN_TABLE[level] * quantizer^0.84182 (* 0.6 on chroma), od_coeff_to_ref_plane
+// (the deringing kernel stores the u8 reconstruction itself).
 // thr[pl][f][sb] = table[pl][level[f][sb]]
 __global__ void k_dering_thresholds(const uint8_t* __restrict__ level, int32_t* __restrict__ thr_luma,
                                     int32_t* __restrict__ thr_chroma, int n, int4 tl_lo, int2 tl_hi, int4 tc_lo, int2 tc_hi) {
@@ -1000,7 +994,8 @@ extern "C" int daala_b200_launch_inverse(const daala_b200_frame* prm, int nplane
 extern "C" int daala_b200_launch_inverse_lapped_only(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
 extern "C" int daala_b200_launch_sb_postfilter_store(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
 extern "C" int daala_b200_dering_plane_batch(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
-                                             long long x_pitch, long long dir_pitch, long long thr_pitch, void* stream);
+                                             long long x_pitch, long long dir_pitch, long long thr_pitch, uint8_t* y8,
+                                             void* stream);
 
 struct daala_b200_kf {
   daala_b200_kf_config cfg;
@@ -1034,7 +1029,8 @@ struct daala_b200_kf {
   // deringing stage
   uint8_t* dering_level;           // [F][nvsb][nhsb]
   int32_t *dering_thr[2];          // luma / chroma thresholds per superblock
-  int16_t *dering_in[3], *dering_out[3];
+  int16_t* dering_in[3];           // etmp: the planes after the SB-edge postfilter
+  int16_t* dering_filt;            // level search (cfg.dering == 2): one filtered luma candidate, [F][h][w]
   int32_t* dering_dir;             // [F][nvsb*8][nhsb*8]
   uint8_t* dering_skip;            // all zero: keyframes never mark a block skipped (src/encode.c:1690)
   int dering_tbl[2][6];
@@ -1274,12 +1270,9 @@ static int kf_alloc(daala_b200_kf* kf) {
     KF_CHECK(dalloc(kf, &kf->dering_thr[1], nsb));
     KF_CHECK(dalloc(kf, &kf->dering_dir, nsb * 64));
     KF_CHECK(dalloc(kf, &kf->dering_skip, nsb * 256 + 64));
-    for (int p = 0; p < 3; p++) {
-      const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
-      KF_CHECK(dalloc(kf, &kf->dering_in[p], n));
-      KF_CHECK(dalloc(kf, &kf->dering_out[p], n));
-    }
+    for (int p = 0; p < 3; p++) KF_CHECK(dalloc(kf, &kf->dering_in[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F));
     if (kf->cfg.dering == 2) {
+      KF_CHECK(dalloc(kf, &kf->dering_filt, (size_t)kf->plane_w[0] * kf->plane_h[0] * F));
       KF_CHECK(dalloc(kf, &kf->dering_orig, nsb * 4096));
       KF_CHECK(dalloc(kf, &kf->dering_cand, nsb * 4096));
       KF_CHECK(dalloc(kf, &kf->dering_dist, nsb * 6));
@@ -1383,7 +1376,7 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
   if ((phases & DAALA_B200_KF_INVERSE) && kf->cfg.dering) {
     // iDCT + split postfilters -> lapped planes; SB-edge postfilter -> etmp (int16, the fused kernel's optional
     // output); od_dering of all frames per plane in one launch, luma first (it writes the direction map chroma
-    // reads); -> u8
+    // reads), storing the u8 reconstruction
     int rc = daala_b200_launch_inverse_lapped_only(&kf->frame, 3, s);
     if (rc) return rc;
     daala_b200_frame f16 = kf->frame;
@@ -1408,7 +1401,7 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
       sb.qm_is_flat = kf->cfg.qm_is_flat;
       sb.use_activity_masking = kf->cfg.use_masking;
       sb.dering_lambda = kf->cfg.dering_lambda;
-      sb.filt = kf->dering_out[0];     // free until the final application below overwrites it
+      sb.filt = kf->dering_filt;
       sb.orig = kf->dering_orig;
       sb.cand = kf->dering_cand;
       sb.dir = kf->dering_dir;
@@ -1428,7 +1421,7 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
       const long long per = (long long)kf->plane_w[p] * kf->plane_h[p];
       daala_b200_dering_params dp;
       memset(&dp, 0, sizeof(dp));
-      dp.y = kf->dering_out[p];
+      dp.y = nullptr;   // u8 output only
       dp.x = kf->dering_in[p];
       dp.dir = kf->dering_dir;
       dp.bskip = kf->dering_skip;
@@ -1444,11 +1437,9 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
       dp.overlap = 1;      // OD_DERING_CHECK_OVERLAP
       dp.coeff_shift = 4;  // OD_COEFF_SHIFT
       dp.dir_format = search ? 2 : 0;   // after a search the direction map is already there (packed with the variance)
-      rc = daala_b200_dering_plane_batch(&dp, kf->F, per, per, (long long)nsb * 64, nsb, s);
+      rc = daala_b200_dering_plane_batch(&dp, kf->F, per, per, (long long)nsb * 64, nsb, kf->pixels_out[p], s);
       if (rc) return rc;
     }
-    for (int p = 0; p < 3; p++)
-      k_i16_to_u8<<<wide, 256, 0, s>>>(kf->dering_out[p], kf->pixels_out[p], (long)kf->plane_w[p] * kf->plane_h[p] * kf->F);
   }
   return (int)cudaGetLastError();
 }
@@ -1555,10 +1546,8 @@ void daala_b200_kf_destroy(daala_b200_kf* kf) {
   cudaFree(kf->dering_thr[1]);
   cudaFree(kf->dering_dir);
   cudaFree(kf->dering_skip);
-  for (int p = 0; p < 3; p++) {
-    cudaFree(kf->dering_in[p]);
-    cudaFree(kf->dering_out[p]);
-  }
+  for (int p = 0; p < 3; p++) cudaFree(kf->dering_in[p]);
+  cudaFree(kf->dering_filt);
   cudaFree(L.succ_bottom);
   cudaFree(L.succ_right);
   cudaFree(L.cnt);
@@ -1592,7 +1581,7 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   n += 3 + 1 + (kf->cfg.split_free > 1 ? split(kf->luma) : 0) + (kf->luma.pre_ev ? 2 : 0);   // luma: begin, gather, [prepass], chains, finish
   n += 4 + (kf->cfg.split_free > 0 ? split(kf->chroma) : 1);                      // chroma: begin, cfl, gather, bands, finish
   if (!kf->cfg.dering) n += 2;                                                    // inverse, SB postfilter + store
-  else n += 1 + 1 + 1 + 3 + 3;   // inverse, SB postfilter -> int16, thresholds, dering per plane, store
+  else n += 1 + 1 + 1 + 3;       // inverse, SB postfilter -> int16, thresholds, dering + u8 store per plane
   if (kf->cfg.dering == 2) n += 5 + 6 + 6 + 1;   // level search: 5 filtered candidates, 6 packs, 6 distortion passes, decision
   return n;
 }
