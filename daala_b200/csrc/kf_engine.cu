@@ -13,7 +13,8 @@
 //        dependency order and wait on per-(block, band) flags of the neighbours they read
 //        (acquire / release) -- no per-wave launches
 //     -> chroma-from-luma prediction + CfL flip + chroma PVQ (same persistent kernel, no dependencies)
-//     -> iDCT + lapped postfilters -> u8 reconstruction, packed symbols for the host entropy coder.
+//     -> iDCT + lapped postfilters -> u8 reconstruction, packed symbols for the host entropy coder
+//     -> (config.symbol_stream) the same symbols per frame in bitstream order with 8/16-bit pulses.
 //
 // Nothing returns to the host between the H2D of the inputs and the D2H of the results; list sizes
 // live in device memory (`cnt`), every kernel is launched with a fixed grid and loops / pulls tickets
@@ -981,6 +982,309 @@ __global__ void k_dering_thresholds(const uint8_t* __restrict__ level, int32_t* 
   thr_chroma[i] = tc[g];
 }
 
+// ---- symbol stream (optional, config.symbol_stream) -------------------------------------------------------
+// The PVQ symbols of every frame in bitstream order (include/daala_b200.h, daala_b200_kf_sym_block): per
+// superblock in raster order planes 0, 1, 2, inside a plane the quadtree leaves depth-first with children
+// top-left, top-right, bottom-left, bottom-right (od_encode_recursive, src/encode.c:1780-1787, called per
+// superblock and plane at src/encode.c:2605-2656).  That depth-first order is the Z order of the leaves'
+// origins, so a block's position is its superblock's base plus the number of leaves of its plane whose origin
+// comes first in Z order: a warp scan over the 64 units of a superblock in Z order.  Then per block the band
+// count and pulse bytes (they depend on K), a prefix scan over the blocks in stream order, and the pack.
+struct Sym {
+  const uint8_t* bsize;
+  int bstride;
+  long long bsize_pitch;
+  int F, nhsb, sb_rows, u_row0;
+  int nsb;                         // superblocks per frame in this shard (nhsb * sb_rows)
+  uint32_t* unit_rank;             // [F][sb_rows*8][nhsb*8]: luma | chroma << 16 leaves earlier in the superblock
+  uint32_t* sb_cnt;                // [F*nsb]: luma | chroma-per-plane << 16 leaves of the superblock
+  int32_t* sb_base;                // [F*nsb]: first slot of the superblock (exclusive prefix over the batch)
+  uint32_t* order;                 // [cap_blocks]: slot -> block (bit 31: chroma list)
+  longlong2* off;                  // [cap_blocks]: (bands, pulse bytes) of the slot, then exclusive prefixes
+  longlong2* tile;                 // [ntiles]: tile sums, then exclusive prefixes
+  long long* tot;                  // [4]: slots, bands, pulse bytes of the batch
+  int ntiles, cap_blocks;
+  long long cap_bands, cap_bytes;
+  daala_b200_kf_sym_frame* index;  // [F]
+  daala_b200_kf_sym_block* blocks; // [cap_blocks]
+  short4* bands;                   // [cap_bands]
+  uint8_t* pulses;                 // [cap_bytes]
+  const daala_b200_pvq_block* list[2];   // luma / chroma block lists and their PVQ results
+  const short4* res[2];
+  const int32_t* y[2];
+  const double* skip_diff[2];
+  const int32_t* flip;
+  const int32_t* cnt;
+  int max_luma, max_chroma;
+};
+
+// Bytes the band's pulses take in the stream: the n - (itheta != -1) values pvq_encode_partition hands to
+// od_encode_pvq_codeword (src/pvq_encoder.c:719-720), one byte each for K <= 127, two above.
+__device__ __forceinline__ int sym_band_bytes(int band, short4 r) {
+  if (r.w <= 0) return 0;
+  const int n = band_start(band + 1) - band_start(band) - (r.y != -1);
+  return r.w > 127 ? 2 * n : n;
+}
+
+// One warp per superblock: lane l holds the units 2l and 2l + 1 in Z order.
+__global__ void __launch_bounds__(256) k_sym_rank(const __grid_constant__ Sym S) {
+  const int lane = threadIdx.x & 31;
+  const int sb = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (sb >= S.F * S.nsb) return;   // whole warps
+  const int f = sb / S.nsb, r = sb % S.nsb;
+  const int sby = r / S.nhsb, sbx = r % S.nhsb;
+  const int uw = S.nhsb * 8;
+  uint32_t v[2];
+  long long at[2];
+  for (int h = 0; h < 2; h++) {
+    const int m = 2 * lane + h;    // Z order: x in the even bits, y in the odd bits
+    const int dx = (m & 1) | ((m >> 1) & 2) | ((m >> 2) & 4);
+    const int dy = ((m >> 1) & 1) | ((m >> 2) & 2) | ((m >> 3) & 4);
+    const int ux = sbx * 8 + dx, uy = S.u_row0 + sby * 8 + dy;
+    const int b = S.bsize[f * S.bsize_pitch + (long long)uy * S.bstride + ux];
+    const int4 c = unit_counts(b, ux, uy);
+    v[h] = (uint32_t)c.x | ((uint32_t)c.z << 16);
+    at[h] = ((long long)f * S.sb_rows * 8 + (uy - S.u_row0)) * uw + ux;
+  }
+  const uint32_t s = v[0] + v[1];
+  uint32_t inc = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t a = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += a;
+  }
+  S.unit_rank[at[0]] = inc - s;
+  S.unit_rank[at[1]] = inc - s + v[0];
+  if (lane == 31) S.sb_cnt[sb] = inc;
+}
+
+// One CTA: exclusive scan of the superblocks' block counts (luma + 2 chroma planes) -> first slots.
+__global__ void __launch_bounds__(1024) k_sym_sb_scan(const __grid_constant__ Sym S) {
+  __shared__ int part[1024];
+  __shared__ int carry;
+  const int t = threadIdx.x;
+  const int n = S.F * S.nsb;
+  if (t == 0) carry = 0;
+  __syncthreads();
+  for (int base = 0; base < n; base += 1024) {
+    const int i = base + t;
+    const uint32_t c = i < n ? S.sb_cnt[i] : 0u;
+    const int v = (int)(c & 0xffff) + 2 * (int)(c >> 16);
+    part[t] = v;
+    __syncthreads();
+    for (int o = 1; o < 1024; o <<= 1) {
+      const int a = t >= o ? part[t - o] : 0;
+      __syncthreads();
+      part[t] += a;
+      __syncthreads();
+    }
+    const int incl = part[t], c0 = carry;
+    if (i < n) S.sb_base[i] = c0 + incl - v;
+    __syncthreads();
+    if (t == 1023) carry = c0 + incl;
+    __syncthreads();
+  }
+  if (t == 0) S.tot[0] = min(carry, S.cap_blocks);
+}
+
+// Per block (luma list, then chroma list): its slot, and the slot's band count and pulse bytes.
+__global__ void __launch_bounds__(256) k_sym_place(const __grid_constant__ Sym S) {
+  const int nl = min(S.cnt[kNLuma], S.max_luma), nc = min(S.cnt[kNChroma], S.max_chroma);
+  const int uw = S.nhsb * 8;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nl + nc; i += gridDim.x * blockDim.x) {
+    const int ch = i >= nl;
+    const int blk = ch ? i - nl : i;
+    const daala_b200_pvq_block b = S.list[ch][blk];
+    const int sh = ch ? 2 : 3;   // plane samples per 8x8 luma unit: 4 (4:2:0 chroma) or 8
+    const int ux = b.x0 >> sh, uy = b.y0 >> sh;
+    const int sb = b.frame * S.nsb + ((uy - S.u_row0) >> 3) * S.nhsb + (ux >> 3);
+    const uint32_t rk = S.unit_rank[((long long)b.frame * S.sb_rows * 8 + (uy - S.u_row0)) * uw + ux];
+    const uint32_t sc = S.sb_cnt[sb];
+    int pos = S.sb_base[sb];
+    if (!ch) pos += (int)(rk & 0xffff) + (b.bs == 0 ? ((b.y0 >> 2) & 1) * 2 + ((b.x0 >> 2) & 1) : 0);
+    else pos += (int)(sc & 0xffff) + (b.pli - 1) * (int)(sc >> 16) + (int)(rk >> 16);
+    if (pos >= S.cap_blocks) continue;
+    S.order[pos] = (uint32_t)blk | (ch ? 0x80000000u : 0u);
+    const short4* r = S.res[ch] + (size_t)blk * 9;
+    const int nb = num_bands(b.bs);
+    long long bytes = 0;
+    for (int j = 0; j < nb; j++) bytes += sym_band_bytes(j, r[j]);
+    S.off[pos] = make_longlong2(nb, bytes);
+  }
+}
+
+__device__ __forceinline__ longlong2 add2(longlong2 a, longlong2 b) { return make_longlong2(a.x + b.x, a.y + b.y); }
+
+__global__ void __launch_bounds__(kTile) k_sym_tile_sums(const __grid_constant__ Sym S) {
+  __shared__ longlong2 part[32];
+  const long long i = (long long)blockIdx.x * kTile + threadIdx.x;
+  longlong2 v = i < S.tot[0] ? S.off[i] : make_longlong2(0, 0);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    v.x += __shfl_xor_sync(0xffffffffu, v.x, o);
+    v.y += __shfl_xor_sync(0xffffffffu, v.y, o);
+  }
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    longlong2 s = make_longlong2(0, 0);
+    for (int w = 0; w < kTile / 32; w++) s = add2(s, part[w]);
+    S.tile[blockIdx.x] = s;
+  }
+}
+
+// One CTA: exclusive scan of the tile sums in place; the batch's band and byte totals.
+__global__ void __launch_bounds__(1024) k_sym_tile_scan(const __grid_constant__ Sym S) {
+  __shared__ longlong2 part[1024];
+  __shared__ longlong2 carry;
+  const int t = threadIdx.x;
+  if (t == 0) carry = make_longlong2(0, 0);
+  __syncthreads();
+  for (int base = 0; base < S.ntiles; base += 1024) {
+    const int i = base + t;
+    const longlong2 v = i < S.ntiles ? S.tile[i] : make_longlong2(0, 0);
+    part[t] = v;
+    __syncthreads();
+    for (int o = 1; o < 1024; o <<= 1) {
+      const longlong2 a = t >= o ? part[t - o] : make_longlong2(0, 0);
+      __syncthreads();
+      part[t] = add2(part[t], a);
+      __syncthreads();
+    }
+    const longlong2 incl = part[t], c = carry;
+    if (i < S.ntiles) S.tile[i] = make_longlong2(c.x + incl.x - v.x, c.y + incl.y - v.y);
+    __syncthreads();
+    if (t == 1023) carry = add2(c, incl);
+    __syncthreads();
+  }
+  if (t == 0) {
+    S.tot[1] = carry.x;
+    S.tot[2] = carry.y;
+  }
+}
+
+// Per slot: (bands, bytes) -> exclusive prefixes over the batch, in place.
+__global__ void __launch_bounds__(kTile) k_sym_offsets(const __grid_constant__ Sym S) {
+  __shared__ longlong2 wsum[32];
+  const long long i = (long long)blockIdx.x * kTile + threadIdx.x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const bool valid = i < S.tot[0];
+  const longlong2 v = valid ? S.off[i] : make_longlong2(0, 0);
+  longlong2 s = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const long long ax = __shfl_up_sync(0xffffffffu, s.x, o), ay = __shfl_up_sync(0xffffffffu, s.y, o);
+    if (lane >= o) s = make_longlong2(s.x + ax, s.y + ay);
+  }
+  if (lane == 31) wsum[warp] = s;
+  __syncthreads();
+  longlong2 pre = S.tile[blockIdx.x];
+  for (int w = 0; w < warp; w++) pre = add2(pre, wsum[w]);
+  if (valid) S.off[i] = make_longlong2(pre.x + s.x - v.x, pre.y + s.y - v.y);
+}
+
+// One warp per slot: the block record, its band records and the pulses of its bands with K > 0.
+__global__ void __launch_bounds__(256) k_sym_pack(const __grid_constant__ Sym S) {
+  const int lane = threadIdx.x & 31;
+  const long long n = S.tot[0];
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (long long slot = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; slot < n; slot += nwarps) {
+    const uint32_t id = S.order[slot];
+    const int ch = id >> 31, blk = (int)(id & 0x7fffffffu);
+    const daala_b200_pvq_block b = S.list[ch][blk];
+    const long long first = S.sb_base[b.frame * S.nsb];   // the frame's first slot
+    const longlong2 o = S.off[slot], o0 = first < n ? S.off[first] : o;
+    const short4* r = S.res[ch] + (size_t)blk * 9;
+    const int nb = num_bands(b.bs);
+    int bytes = 0;
+    for (int j = 0; j < nb; j++) bytes += sym_band_bytes(j, r[j]);
+    // only an over-capacity step (flagged in counts[kError]; submit refuses such a batch) can leave stale slots
+    if (o.x + nb > S.cap_bands || o.y + bytes > S.cap_bytes) continue;
+    if (lane == 0) {
+      daala_b200_kf_sym_block rec;
+      rec.skip_diff = S.skip_diff[ch][blk];
+      rec.pulse_off = (uint32_t)(o.y - o0.y);
+      rec.band_off = (uint32_t)(o.x - o0.x);
+      rec.x0 = b.x0;
+      rec.y0 = b.y0;
+      rec.bs = b.bs;
+      rec.pli = b.pli;
+      rec.flip = ch ? (uint8_t)S.flip[blk] : 0;
+      rec.reserved = 0;
+      S.blocks[slot] = rec;
+    }
+    if (lane < nb) S.bands[o.x + lane] = r[lane];
+    const int32_t* y = S.y[ch] + b.coef_off;
+    uint8_t* dst = S.pulses + o.y;
+    for (int j = 0; j < nb; j++) {
+      const short4 q = r[j];
+      const int len = sym_band_bytes(j, q);
+      if (!len) continue;
+      const int st = band_start(j);
+      if (q.w > 127) {
+        for (int t = lane; t < len / 2; t += 32) {
+          const int v = y[st + t];
+          dst[2 * t] = (uint8_t)(v & 0xff);
+          dst[2 * t + 1] = (uint8_t)((v >> 8) & 0xff);
+        }
+      } else {
+        for (int t = lane; t < len; t += 32) dst[t] = (uint8_t)(y[st + t] & 0xff);
+      }
+      dst += len;
+    }
+  }
+}
+
+// Per frame: where its blocks, bands and pulse bytes are in the batch-wide arrays.
+__global__ void k_sym_index(const __grid_constant__ Sym S) {
+  for (int f = threadIdx.x; f < S.F; f += blockDim.x) {
+    const long long n = S.tot[0];
+    const long long s0 = S.sb_base[f * S.nsb];
+    const long long s1 = f + 1 < S.F ? S.sb_base[(f + 1) * S.nsb] : n;
+    const longlong2 a = s0 < n ? S.off[s0] : make_longlong2(S.tot[1], S.tot[2]);
+    const longlong2 e = s1 < n ? S.off[s1] : make_longlong2(S.tot[1], S.tot[2]);
+    daala_b200_kf_sym_frame x;
+    x.first_block = s0;
+    x.n_blocks = s1 - s0;
+    x.first_band = a.x;
+    x.n_bands = e.x - a.x;
+    x.first_byte = a.y;
+    x.n_bytes = e.y - a.y;
+    S.index[f] = x;
+  }
+}
+
+// Copy of the used part of each stream array into the caller's pinned host buffers (device-addressable):
+// the lengths are only known on the device.  Segment 0 index, 1 block records, 2 band records, 3 pulses.
+struct SymCopy {
+  const uint8_t* src[4];
+  uint8_t* dst[4];
+  long long unit[4];               // bytes per element; segment 0 has a fixed length
+  long long cap[4];                // bytes: the smaller of the host buffer and the device array
+  long long index_bytes;
+  const long long* tot;
+};
+
+__global__ void __launch_bounds__(256) k_sym_copy(const __grid_constant__ SymCopy C) {
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long nth = (long long)gridDim.x * blockDim.x;
+  for (int seg = 0; seg < 4; seg++) {
+    if (!C.dst[seg]) continue;
+    const long long want = seg == 0 ? C.index_bytes : C.tot[seg - 1] * C.unit[seg];
+    const long long len = want < C.cap[seg] ? want : C.cap[seg];
+    const uint8_t* s = C.src[seg];
+    uint8_t* d = C.dst[seg];
+    long long done = 0;
+    if ((((uintptr_t)s | (uintptr_t)d) & 15) == 0) {
+      const long long n16 = len >> 4;
+      for (long long i = tid; i < n16; i += nth)
+        reinterpret_cast<uint4*>(d)[i] = reinterpret_cast<const uint4*>(s)[i];
+      done = n16 << 4;
+    }
+    for (long long i = done + tid; i < len; i += nth) d[i] = s[i];
+  }
+}
+
 }  // namespace kf
 }  // namespace daala_b200
 
@@ -1039,6 +1343,7 @@ struct daala_b200_kf {
   double* dering_dist;
   Lists lists;
   Stage luma, chroma;
+  Sym sym;                         // symbol stream (cfg.symbol_stream); zero otherwise
   daala_b200_frame frame;
   size_t bytes_allocated;
   size_t chain_cap;                // entries of the chain queue (heads / ring)
@@ -1238,6 +1543,46 @@ static int kf_alloc(daala_b200_kf* kf) {
   rc = setup_stage(kf->chroma, true);
   if (rc) return rc;
   (void)luma_px;
+  if (kf->cfg.symbol_stream) {
+    Sym& Y = kf->sym;
+    memset(&Y, 0, sizeof(Y));
+    Y.bsize = kf->bsize;
+    Y.bstride = UW;
+    Y.bsize_pitch = (long long)UW * UH;
+    Y.F = F;
+    Y.nhsb = kf->nhsb;
+    Y.sb_rows = kf->cfg.sb_rows;
+    Y.u_row0 = L.u_row0;
+    Y.nsb = kf->nhsb * kf->cfg.sb_rows;
+    Y.cap_blocks = L.max_luma + L.max_chroma;
+    Y.ntiles = (Y.cap_blocks + kTile - 1) / kTile;
+    // every band has at least 8 coefficients and 4x4 / 8x8 blocks have one band per 16: bands <= coefficients / 16
+    const size_t ncoef = (luma_shard_px + 1024) + (luma_shard_px / 2 + 1024);
+    KF_CHECK(dalloc(kf, &Y.unit_rank, (size_t)F * L.u_rows * UW));
+    KF_CHECK(dalloc(kf, &Y.sb_cnt, (size_t)F * Y.nsb));
+    KF_CHECK(dalloc(kf, &Y.sb_base, (size_t)F * Y.nsb));
+    KF_CHECK(dalloc(kf, &Y.order, (size_t)Y.cap_blocks));
+    KF_CHECK(dalloc(kf, &Y.off, (size_t)Y.cap_blocks));
+    KF_CHECK(dalloc(kf, &Y.tile, (size_t)Y.ntiles));
+    KF_CHECK(dalloc(kf, &Y.tot, (size_t)4));
+    KF_CHECK(dalloc(kf, &Y.index, (size_t)F));
+    KF_CHECK(dalloc(kf, &Y.blocks, (size_t)Y.cap_blocks));
+    Y.cap_bands = (long long)(ncoef / 16);
+    Y.cap_bytes = (long long)(2 * ncoef);
+    KF_CHECK(dalloc(kf, &Y.bands, ncoef / 16));
+    KF_CHECK(dalloc(kf, &Y.pulses, 2 * ncoef));
+    for (int c = 0; c < 2; c++) {
+      const Stage& S = c ? kf->chroma : kf->luma;
+      Y.list[c] = S.prm.blocks;
+      Y.res[c] = reinterpret_cast<const short4*>(S.res_pack);
+      Y.y[c] = S.prm.y;
+      Y.skip_diff[c] = S.prm.res_skip_diff;
+    }
+    Y.flip = kf->chroma.prm.res_flip;
+    Y.cnt = L.cnt;
+    Y.max_luma = L.max_luma;
+    Y.max_chroma = L.max_chroma;
+  }
 
   daala_b200_frame& f = kf->frame;
   memset(&f, 0, sizeof(f));
@@ -1368,6 +1713,17 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
     if (kf->cfg.split_free > 0) enqueue_split<false>(kf, kf->chroma, s);
     else k_pvq_persist<false><<<persist, kPersistThreads, 0, s>>>(kf->chroma);
     if (!core) k_finish_scatter<<<wide, 256, 0, s>>>(kf->chroma);
+    if (!core && kf->cfg.symbol_stream) {
+      const Sym& Y = kf->sym;
+      k_sym_rank<<<(Y.F * Y.nsb + 7) / 8, 256, 0, s>>>(Y);
+      k_sym_sb_scan<<<1, 1024, 0, s>>>(Y);
+      k_sym_place<<<wide, 256, 0, s>>>(Y);
+      k_sym_tile_sums<<<Y.ntiles, kTile, 0, s>>>(Y);
+      k_sym_tile_scan<<<1, 1024, 0, s>>>(Y);
+      k_sym_offsets<<<Y.ntiles, kTile, 0, s>>>(Y);
+      k_sym_pack<<<wide, 256, 0, s>>>(Y);
+      k_sym_index<<<1, 256, 0, s>>>(Y);
+    }
   }
   if ((phases & DAALA_B200_KF_INVERSE) && !kf->cfg.dering) {
     int rc = daala_b200_launch_inverse(&kf->frame, 3, s);
@@ -1551,6 +1907,18 @@ void daala_b200_kf_destroy(daala_b200_kf* kf) {
   cudaFree(L.succ_bottom);
   cudaFree(L.succ_right);
   cudaFree(L.cnt);
+  Sym& Y = kf->sym;
+  cudaFree(Y.unit_rank);
+  cudaFree(Y.sb_cnt);
+  cudaFree(Y.sb_base);
+  cudaFree(Y.order);
+  cudaFree(Y.off);
+  cudaFree(Y.tile);
+  cudaFree(Y.tot);
+  cudaFree(Y.index);
+  cudaFree(Y.blocks);
+  cudaFree(Y.bands);
+  cudaFree(Y.pulses);
   for (Stage* S : {&kf->luma, &kf->chroma}) {
     cudaFree(S->prm.in);
     cudaFree(S->prm.ref);
@@ -1583,6 +1951,7 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   if (!kf->cfg.dering) n += 2;                                                    // inverse, SB postfilter + store
   else n += 1 + 1 + 1 + 3;       // inverse, SB postfilter -> int16, thresholds, dering + u8 store per plane
   if (kf->cfg.dering == 2) n += 5 + 6 + 6 + 1;   // level search: 5 filtered candidates, 6 packs, 6 distortion passes, decision
+  if (kf->cfg.symbol_stream) n += 8;             // symbol stream: rank, superblock scan, place, 3 scan kernels, pack, index
   return n;
 }
 
@@ -1699,6 +2068,34 @@ int daala_b200_kf_count_blocks(const uint8_t* bsize, int nframes, long long fram
   return 0;
 }
 
+// Worst-case lengths of the symbol stream arrays for a batch with the given totals: every block, every band
+// (9 per block, and never more than one per 16 coefficients: 4x4 and 8x8 blocks have exactly that many, larger
+// ones fewer), two bytes per coded coefficient.
+int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals* t, int nframes, daala_b200_kf_sym_bounds* out) {
+  if (!t || !out || nframes <= 0) return (int)cudaErrorInvalidValue;
+  const long long blocks = t->n_luma + t->n_chroma, coefs = t->luma_coefs + t->chroma_coefs;
+  out->index = nframes;
+  out->blocks = blocks;
+  out->bands = 9 * blocks < coefs / 16 ? 9 * blocks : coefs / 16;
+  out->pulse_bytes = 2 * coefs;
+  return 0;
+}
+
+// A requested stream buffer: large enough, and pinned host memory the device can write (its device address).
+static int sym_target(const void* p, long long cap, long long need, uint8_t** dev) {
+  *dev = nullptr;
+  if (!p) return 0;
+  if (cap < need) return (int)cudaErrorInvalidValue;
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return (int)cudaErrorInvalidValue;
+  }
+  if (a.type != cudaMemoryTypeHost || !a.devicePointer) return (int)cudaErrorInvalidValue;
+  *dev = (uint8_t*)a.devicePointer;
+  return 0;
+}
+
 // With level_chains the compute phases of different engines never overlap on the device: the level kernel
 // synchronises its whole grid and needs every CTA resident, which two such kernels in flight could deny
 // each other.  Copies of one
@@ -1718,6 +2115,36 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   else daala_b200_kf_count_blocks(io->bsize, F, (long long)kf->nhsb * 8 * kf->nvsb * 8, kf->nhsb * 8, kf->nhsb, kf->nvsb,
                                   kf->cfg.sb_row0, kf->cfg.sb_rows, &tot);
   if (tot.n_luma > kf->lists.max_luma || tot.n_chroma > kf->lists.max_chroma) return (int)cudaErrorInvalidValue;
+  // symbol stream: the engine must produce it, and every requested buffer must hold the worst case and be pinned
+  SymCopy sc;
+  memset(&sc, 0, sizeof(sc));
+  const bool want_sym = io->sym_index || io->sym_blocks || io->sym_bands || io->sym_pulses;
+  if (want_sym) {
+    if (!kf->cfg.symbol_stream) return (int)cudaErrorInvalidValue;
+    daala_b200_kf_sym_bounds bd;
+    daala_b200_kf_symbol_bounds(&tot, F, &bd);
+    int e = sym_target(io->sym_index, io->sym_index_cap, bd.index, &sc.dst[0]);
+    if (!e) e = sym_target(io->sym_blocks, io->sym_blocks_cap, bd.blocks, &sc.dst[1]);
+    if (!e) e = sym_target(io->sym_bands, io->sym_bands_cap, bd.bands, &sc.dst[2]);
+    if (!e) e = sym_target(io->sym_pulses, io->sym_pulses_cap, bd.pulse_bytes, &sc.dst[3]);
+    if (e) return e;
+    const Sym& Y = kf->sym;
+    sc.src[0] = (const uint8_t*)Y.index;
+    sc.src[1] = (const uint8_t*)Y.blocks;
+    sc.src[2] = (const uint8_t*)Y.bands;
+    sc.src[3] = Y.pulses;
+    sc.unit[1] = sizeof(daala_b200_kf_sym_block);
+    sc.unit[2] = 4 * sizeof(int16_t);
+    sc.unit[3] = 1;
+    sc.index_bytes = (long long)F * sizeof(daala_b200_kf_sym_frame);
+    sc.tot = Y.tot;
+    const long long host[4] = {io->sym_index_cap * (long long)sizeof(daala_b200_kf_sym_frame),
+                               io->sym_blocks_cap * (long long)sizeof(daala_b200_kf_sym_block),
+                               io->sym_bands_cap * 8, io->sym_pulses_cap};
+    const long long dev[4] = {sc.index_bytes, (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_block),
+                              Y.cap_bands * 8, Y.cap_bytes};
+    for (int i = 0; i < 4; i++) sc.cap[i] = host[i] < dev[i] ? host[i] : dev[i];
+  }
   for (int p = 0; p < 3; p++) {
     if (!io->pixels[p]) return (int)cudaErrorInvalidValue;
     KF_CHECK(cudaMemcpyAsync(kf->pixels[p], io->pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
@@ -1754,6 +2181,10 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   if (io->counts) KF_CHECK(cudaMemcpyAsync(io->counts, kf->lists.cnt, sizeof(int32_t) * 32, cudaMemcpyDeviceToHost, s));
   if (io->dering_level_out && kf->cfg.dering)
     KF_CHECK(cudaMemcpyAsync(io->dering_level_out, kf->dering_level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyDeviceToHost, s));
+  if (want_sym) {
+    k_sym_copy<<<kf->sms * 4, 256, 0, s>>>(sc);
+    KF_CHECK(cudaGetLastError());
+  }
   return 0;
 }
 

@@ -24,7 +24,8 @@ class Config(ctypes.Structure):
                 ("qm_stride", c_int), ("pvq_norm_lambda", ctypes.c_double), ("pvq_qm_q4", (ctypes.c_ubyte * 32) * 3),
                 ("qm", c_void_p), ("qm_inv", c_void_p), ("sb_row0", c_int), ("sb_rows", c_int),
                 ("max_blocks_div", c_int), ("persist_ctas_per_sm", c_int), ("split_free", c_int), ("dering", c_int), ("noref_prepass", c_int), ("level_chains", c_int), ("stream", c_void_p),
-                ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double)]
+                ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
+                ("symbol_stream", c_int)]
 
 
 class Totals(ctypes.Structure):
@@ -36,7 +37,13 @@ class IO(ctypes.Structure):
                 ("pixels_out", c_void_p * 3), ("luma_blocks", c_void_p), ("chroma_blocks", c_void_p),
                 ("luma_res", c_void_p), ("chroma_res", c_void_p), ("luma_y16", c_void_p), ("chroma_y16", c_void_p),
                 ("luma_skip_diff", c_void_p), ("chroma_skip_diff", c_void_p), ("chroma_flip", c_void_p),
-                ("counts", c_void_p), ("dering_level_out", c_void_p)]
+                ("counts", c_void_p), ("dering_level_out", c_void_p),
+                ("sym_index", c_void_p), ("sym_index_cap", c_ll), ("sym_blocks", c_void_p), ("sym_blocks_cap", c_ll),
+                ("sym_bands", c_void_p), ("sym_bands_cap", c_ll), ("sym_pulses", c_void_p), ("sym_pulses_cap", c_ll)]
+
+
+class SymBounds(ctypes.Structure):
+    _fields_ = [("index", c_ll), ("blocks", c_ll), ("bands", c_ll), ("pulse_bytes", c_ll)]
 
 
 class Buffers(ctypes.Structure):
@@ -69,6 +76,7 @@ def _bind():
                                              ctypes.POINTER(Totals)]
     for name in ("daala_b200_kf_submit", "daala_b200_kf_encode"):
         getattr(L, name).argtypes = [c_void_p, ctypes.POINTER(IO)]
+    L.daala_b200_kf_symbol_bounds.argtypes = [ctypes.POINTER(Totals), c_int, ctypes.POINTER(SymBounds)]
     L.daala_b200_kf_wait.argtypes = [c_void_p]
     L.daala_b200_device_copy.argtypes = [c_void_p, c_void_p, ctypes.c_size_t, c_int]
     L.daala_b200_host_alloc.argtypes = [ctypes.c_size_t]
@@ -103,7 +111,7 @@ class KeyframeEngine:
 
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
                  qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=0, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
-                 qm_is_flat=0, dering_lambda=None, pinned=True):
+                 qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0):
         self.L = _bind()
         self.geom, self.F = geom, nframes
         if qm is None:
@@ -132,6 +140,8 @@ class KeyframeEngine:
         cfg.dering_lambda = float(0.67 * pvq.PVQ_LAMBDA * q0 * q0 if dering_lambda is None else dering_lambda)
         self.dering_lambda = cfg.dering_lambda
         self.dering = int(dering)
+        cfg.symbol_stream = int(symbol_stream)
+        self.symbol_stream = int(symbol_stream)
         self.kf = self.L.daala_b200_kf_create(ctypes.byref(cfg))
         if not self.kf:
             raise RuntimeError("daala_b200_kf_create failed (no CUDA device, or out of memory)")
@@ -169,8 +179,8 @@ class KeyframeEngine:
                 what, rc, self.L.daala_b200_kf_error(self.kf).decode() if self.kf else ""))
 
     # --- host buffers --------------------------------------------------------------------------
-    def _arr(self, name, shape, dtype):
-        """(Re)usable host array `name`; pinned when the engine was created with pinned=True."""
+    def _arr(self, name, shape, dtype, pinned=None):
+        """(Re)usable host array `name`; pinned when the engine was created with pinned=True (or `pinned`)."""
         cur = self._host.get(name)
         n = int(np.prod(shape))
         if cur is not None:
@@ -179,7 +189,7 @@ class KeyframeEngine:
                 return a.reshape(-1)[:n].reshape(shape)
             if isinstance(cur, Pinned):
                 cur.free()
-        if self.pinned:
+        if self.pinned if pinned is None else pinned:
             cur = Pinned((max(n, 1),), dtype)
             self._host[name] = cur
             return cur.array[:n].reshape(shape)
@@ -214,8 +224,19 @@ class KeyframeEngine:
         b[...] = bsize
         self.totals = self.count_blocks(b)
 
-    def prepare_io(self, symbols=True, recon=True):
-        """Builds the daala_b200_kf_io record over the staged inputs and result buffers sized for them."""
+    def symbol_bounds(self, totals=None):
+        """Worst-case lengths (index, blocks, bands, pulse_bytes) of the symbol stream arrays for `totals`
+        (default: those of the staged batch), from daala_b200_kf_symbol_bounds."""
+        b = SymBounds()
+        self._check(self.L.daala_b200_kf_symbol_bounds(ctypes.byref(totals or self.totals), self.F, ctypes.byref(b)),
+                    "symbol_bounds")
+        return b
+
+    def prepare_io(self, symbols=True, recon=True, stream=None):
+        """Builds the daala_b200_kf_io record over the staged inputs and result buffers sized for them.
+        stream (default: whether the engine was created with symbol_stream=1) adds the symbol stream buffers
+        sym_index, sym_blocks, sym_bands and sym_pulses (daala_b200/symbols.py), pinned and sized by
+        daala_b200_kf_symbol_bounds; only their used part is copied back."""
         g, t = self.geom, self.totals
         io = IO()
         for p in range(3):
@@ -248,9 +269,20 @@ class KeyframeEngine:
         if self.dering:
             out["dering_levels"] = self._arr("dlev_out", (self.F, g.nvsb, g.nhsb), np.uint8)
             io.dering_level_out = out["dering_levels"].ctypes.data
+        self.d2h_bytes = sum(v.nbytes for v in out.values())
+        if self.symbol_stream if stream is None else stream:
+            from . import symbols as sym
+            b = self.symbol_bounds(t)
+            out["sym_index"] = self._arr("si", (self.F, 6), np.int64, pinned=True)
+            out["sym_blocks"] = self._arr("sb", (int(b.blocks),), sym.BLOCK_DTYPE, pinned=True)
+            out["sym_bands"] = self._arr("sn", (int(b.bands), 4), np.int16, pinned=True)
+            out["sym_pulses"] = self._arr("sp", (int(b.pulse_bytes),), np.uint8, pinned=True)
+            for k, cap in (("sym_index", b.index), ("sym_blocks", b.blocks), ("sym_bands", b.bands),
+                           ("sym_pulses", b.pulse_bytes)):
+                setattr(io, k, out[k].ctypes.data)
+                setattr(io, k + "_cap", int(cap))
         self._io, self._out = io, out
         self.h2d_bytes = sum(int(np.prod(g.plane_shape(p))) for p in range(3)) * self.F + int(np.prod(g.bsize_shape)) * self.F
-        self.d2h_bytes = sum(v.nbytes for v in out.values())
         return out
 
     def submit(self):
@@ -260,13 +292,20 @@ class KeyframeEngine:
         self._check(self.L.daala_b200_kf_wait(self.kf), "kf_wait")
         return self._out
 
-    def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None):
+    def stream_d2h_bytes(self):
+        """Bytes the last submit copied of the symbol stream (after wait): the index and the used part of the
+        other three arrays."""
+        from . import symbols as sym
+        idx = self._out["sym_index"]
+        return idx.nbytes + int(idx[:, 1].sum()) * sym.BLOCK_DTYPE.itemsize + int(idx[:, 3].sum()) * 8 + int(idx[:, 5].sum())
+
+    def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None):
         """One batch end to end through the C ABI with host buffers; returns the result arrays (views of
         the engine's host buffers: copy what must survive the next call)."""
         self.stage_inputs(planes, bsize)
         if self.dering == 1:
             self.stage_dering_levels(dering_levels)
-        self.prepare_io(symbols, recon)
+        self.prepare_io(symbols, recon, stream)
         self.submit()
         out = self.wait()
         if int(out["counts"][CNT["error"]]):

@@ -492,11 +492,47 @@ typedef struct daala_b200_kf_config {
   int coded_quantizer;         /* state->coded_quantizer (scale of od_compute_dist, src/encode.c:1221); dering == 2 */
   int qm_is_flat;              /* enc->qm == OD_FLAT_QM: od_compute_dist is the plain squared error; dering == 2 */
   double dering_lambda;        /* enc->dering_lambda (src/rate.c:1086); dering == 2 */
+  int symbol_stream;           /* 1: every step also packs the PVQ symbols of each frame in bitstream order
+                                  (daala_b200_kf_sym_block below) for daala_b200_kf_io.sym_*; 0 (default): the step
+                                  is exactly the one without the stream */
 } daala_b200_kf_config;
 
 typedef struct daala_b200_kf_totals {
   long long n_luma, luma_coefs, n_chroma, chroma_coefs;
 } daala_b200_kf_totals;
+
+/* Symbol stream (config.symbol_stream): what the serial entropy coder reads, per frame in bitstream order.
+   Coding order: superblocks in raster order (of the engine's shard, sb_row0 / sb_rows), in each planes 0, 1, 2,
+   in each plane the quadtree leaves depth-first with the children top-left, top-right, bottom-left,
+   bottom-right (od_encode_recursive, reference src/encode.c:1780-1787 and :2605-2656; with 4:2:0 one 4x4 chroma
+   block per 8x8 unit whose luma is coded as 4x4 blocks).  For a batch, three arrays hold the frames one after
+   the other, and a per-frame index (daala_b200_kf_sym_frame) says where each frame's part is:
+     blocks  one daala_b200_kf_sym_block per leaf block;
+     bands   per block nbands(bs) = 1, 4, 7, 9, 9 records {coded gain index, itheta, max_theta, K} as int16[4]
+             (the values of daala_b200_kf_io.*_res), in band order;
+     pulses  per band with K > 0 the n - (itheta != -1) values pvq_encode_partition hands to od_encode_pvq_codeword
+             (src/pvq_encoder.c:719-720; n = the band's size), each an int8 when K <= 127 and a little-endian
+             int16 otherwise (|y| <= K, so K gives the width).  Bands with K = 0 have no bytes. */
+typedef struct daala_b200_kf_sym_block {   /* 24 bytes, 8-byte aligned */
+  double skip_diff;        /* the block's skip_diff (as daala_b200_kf_io.*_skip_diff) */
+  uint32_t pulse_off;      /* byte offset of the block's first pulse inside its frame's pulse bytes */
+  uint32_t band_off;       /* index of the block's first band record inside its frame's band records */
+  uint16_t x0, y0;         /* top-left sample of the block inside its plane */
+  uint8_t bs;              /* log2(n) - 2 */
+  uint8_t pli;             /* plane 0, 1, 2 */
+  uint8_t flip;            /* keyframe CfL sign flip (chroma); 0 for luma */
+  uint8_t reserved;        /* 0 */
+} daala_b200_kf_sym_block;
+
+typedef struct daala_b200_kf_sym_frame {   /* one frame's part of the batch-wide arrays (indices, not bytes, */
+  int64_t first_block, n_blocks;           /* except for the pulses) */
+  int64_t first_band, n_bands;
+  int64_t first_byte, n_bytes;
+} daala_b200_kf_sym_frame;
+
+typedef struct daala_b200_kf_sym_bounds {  /* worst-case lengths, in the units of the daala_b200_kf_io.sym_* capacities */
+  long long index, blocks, bands, pulse_bytes;
+} daala_b200_kf_sym_bounds;
 
 /* Host buffers of one batch.  Inputs: padded planes [nframes][plane_h][plane_w] u8 and block-size
    maps [nframes][nvsb*8][nhsb*8] (one byte per 8x8 luma unit = log2(size) - 2).  Outputs (each may be
@@ -519,6 +555,17 @@ typedef struct daala_b200_kf_io {
   int32_t *chroma_flip;
   int32_t *counts;                      /* 32 ints of device-side counters (diagnostics) */
   uint8_t *dering_level_out;            /* [nframes][nvsb][nhsb]: the levels applied (config.dering == 2: the searched ones) */
+  /* Symbol stream (config.symbol_stream): pinned host buffers (daala_b200_host_alloc / cudaHostAlloc) with their
+     capacities in frames, block records, band records and bytes, at least daala_b200_kf_symbol_bounds; NULL = not
+     copied.  Only the used part of each array is copied, by a kernel that reads the lengths on the device. */
+  daala_b200_kf_sym_frame *sym_index;
+  long long sym_index_cap;
+  daala_b200_kf_sym_block *sym_blocks;
+  long long sym_blocks_cap;
+  int16_t *sym_bands;                   /* [n][4] */
+  long long sym_bands_cap;
+  uint8_t *sym_pulses;
+  long long sym_pulses_cap;
 } daala_b200_kf_io;
 
 typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, device-resident callers) */
@@ -566,9 +613,14 @@ int daala_b200_kf_time_device(daala_b200_kf *kf, int phases, int use_graph, int 
 /* Host-side totals implied by block-size maps (sizes of the result arrays). */
 int daala_b200_kf_count_blocks(const uint8_t *bsize, int nframes, long long frame_pitch, int bstride, int nhsb,
                                int nvsb, int sb_row0, int sb_rows, daala_b200_kf_totals *out);
+/* Worst-case lengths of the symbol stream arrays of a batch with these totals: every block, every band, two bytes
+   per coefficient. */
+int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daala_b200_kf_sym_bounds *out);
 /* H2D of the inputs, the whole step, D2H of the requested outputs: enqueued, not waited for.  A batch with more
    luma or chroma blocks than the engine's capacity (see max_blocks_div) returns cudaErrorInvalidValue before
-   anything is copied or launched. */
+   anything is copied or launched; so does a request for symbol stream outputs from an engine created without
+   symbol_stream, a stream capacity below daala_b200_kf_symbol_bounds, or a stream buffer that is not pinned host
+   memory. */
 int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
 int daala_b200_kf_wait(daala_b200_kf *kf);
 int daala_b200_kf_encode(daala_b200_kf *kf, const daala_b200_kf_io *io);   /* submit + wait */
