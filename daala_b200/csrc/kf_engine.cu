@@ -504,21 +504,12 @@ __global__ void __launch_bounds__(256) k_cfl_plane(const __grid_constant__ Stage
   }
 }
 
-// resident CTAs per SM the persistent PVQ kernel is compiled for (register cap = 65536 / 128 / this)
-#ifndef DAALA_PERSIST_SPECIALISE
-#define DAALA_PERSIST_SPECIALISE 0
-#endif
-#ifndef DAALA_PERSIST_MIN_CTAS
-#define DAALA_PERSIST_MIN_CTAS 8
-#endif
-// warps per CTA of the persistent kernel.  1: a warp that runs out of work frees its registers and shared
+// One warp per CTA of the persistent kernel: a warp that runs out of work frees its registers and shared
 // memory at once (a CTA only retires when all of its warps have), so the next kernel -- another engine's
 // batch -- fills the SM while the last dependency chains of this one are still being walked.
-#ifndef DAALA_PERSIST_WARPS
-#define DAALA_PERSIST_WARPS 1
-#endif
-constexpr int kPersistThreads = 32 * DAALA_PERSIST_WARPS;
-constexpr int kPersistCtas = DAALA_PERSIST_MIN_CTAS * 4 / DAALA_PERSIST_WARPS;   // per SM, same number of warps
+constexpr int kPersistThreads = 32;
+// resident CTAs per SM the persistent PVQ kernel is compiled for (register cap = 65536 / 32 / this = 64)
+constexpr int kPersistCtas = 32;
 constexpr uint32_t kNoItem = 0xffffffffu;
 constexpr uint32_t kExit = 0xfffffffeu;
 
@@ -656,25 +647,11 @@ __device__ __forceinline__ void run_item(const Stage& S, uint32_t item, int lane
   int itheta, max_theta, k;
   double skip_term;
   const bool pre = kIntra && S.pre_ev && band != 3 && band != 6;
-  // size-class specialised instantiations (DAALA_PERSIST_SPECIALISE): a band then executes less straight-line
-  // code, at the price of a larger kernel
   const int32_t* pev = pre ? S.pre_ev + (off >> 3) * kPreEvWords : nullptr;
   const int16_t* psn = pre ? S.pre_snap + 2 * off : nullptr;
-  int gain;
-#if DAALA_PERSIST_SPECIALISE
-  if (bn > 32)
-    gain = quantise_band_warp<2>(lane, snap, S.rsqrt_tbl, prm.out + off, prm.in + off, prm.ref + off, bn, q, prm.y + off,
-                                 &itheta, &max_theta, &k, beta, &skip_term, prm.is_keyframe, pli, prm.qm + qoff,
-                                 prm.qm_inv + qoff, prm.pvq_norm_lambda, pev, psn);
-  else
-    gain = quantise_band_warp<1>(lane, snap, S.rsqrt_tbl, prm.out + off, prm.in + off, prm.ref + off, bn, q, prm.y + off,
-                                 &itheta, &max_theta, &k, beta, &skip_term, prm.is_keyframe, pli, prm.qm + qoff,
-                                 prm.qm_inv + qoff, prm.pvq_norm_lambda, pev, psn);
-#else
-  gain = quantise_band_warp<0>(lane, snap, S.rsqrt_tbl, prm.out + off, prm.in + off, prm.ref + off, bn, q, prm.y + off,
-                               &itheta, &max_theta, &k, beta, &skip_term, prm.is_keyframe, pli, prm.qm + qoff,
-                               prm.qm_inv + qoff, prm.pvq_norm_lambda, pev, psn);
-#endif
+  const int gain = quantise_band_warp<0>(lane, snap, S.rsqrt_tbl, prm.out + off, prm.in + off, prm.ref + off, bn, q,
+                                         prm.y + off, &itheta, &max_theta, &k, beta, &skip_term, prm.is_keyframe, pli,
+                                         prm.qm + qoff, prm.qm_inv + qoff, prm.pvq_norm_lambda, pev, psn);
   if (lane == 0) {
     const size_t r = (size_t)blk * 9 + band;
     prm.res_skip_term[r] = skip_term;
@@ -864,7 +841,7 @@ __global__ void __launch_bounds__(128, 4) k_pvq_levels(const __grid_constant__ S
 // successor (band 0 forks) into the chain queue.
 template <bool kIntra>
 __global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(const __grid_constant__ Stage S) {
-  __shared__ int16_t snap_all[DAALA_PERSIST_WARPS][kSnapEntries];   // per warp: the pulses of every search event of a band
+  __shared__ int16_t snap_all[kPersistThreads / 32][kSnapEntries];   // per warp: the pulses of every search event of a band
   const int lane = threadIdx.x & 31;
   int16_t* snap = snap_all[threadIdx.x >> 5];
   int done = 0;

@@ -499,7 +499,7 @@ k_pvq_bands_coop(const __grid_constant__ daala_b200_pvq_params prm, const uint32
 // ---------------------------------------------------------------------------
 // Work ordering.  The trip counts of the search (candidates x pulses) grow with the band's gain, and
 // the lanes of a warp wait for the slowest one: a launch whose entries are grouped by expected work
-// runs 1.3-2x faster than the same entries in raster order (tools/probe/time_sorted.py).  Results are
+// runs 1.3-2x faster than the same entries in raster order (measured on real data).  Results are
 // stored per (block, band), so the order inside a launch is free.  Three small kernels bucket a band
 // list by (wave, work bin), heaviest first: keys + histogram, exclusive scan, scatter.
 // ---------------------------------------------------------------------------
@@ -716,163 +716,13 @@ __global__ void k_coding_order_scatter(const __grid_constant__ daala_b200_pvq_pa
   }
 }
 
-// ---------------------------------------------------------------------------
-// Keyframe luma with the reference's H/V intra prediction (od_hv_intra_pred,
-// src/intra.c:37): the prediction of a block is row 0 / column 0 of the
-// QUANTISED coefficients of its top / left neighbour of the same size, so
-// blocks form dependency chains (SURVEY.md 0.8).  One warp owns one block and
-// runs its whole chain link: wait for the neighbours' done flags, build the
-// prediction, quantise every band (group-cooperative quantiser, 32 lanes),
-// write the reconstruction into the coefficient plane, publish its own flag.
-// Blocks are listed in raster order of their origin, so a block's neighbours
-// always have smaller indices: the lowest unfinished block is resident and
-// never waits on a later one (CTAs are dispatched in index order), hence no
-// deadlock.
-// ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(128)
-k_pvq_luma_intra(const __grid_constant__ daala_b200_pvq_params prm, const int32_t* __restrict__ ids,
-                 const int32_t* __restrict__ dep_top, const int32_t* __restrict__ dep_left, int* done, int epoch,
-                 int nblocks) {
-  const int slot = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (slot >= nblocks) return;
-  const int blk = ids ? ids[slot] : slot;
-  const Group<32, 4> grp;
-  const daala_b200_pvq_block b = prm.blocks[blk];
-  const int bs = b.bs, ln = bs + 2, n = 1 << ln;
-  const int len = ln >= 5 ? 512 : 1 << (2 * ln);
-  const int stride = prm.plane_stride[0];
-  int32_t* d = prm.coef_plane[0] + b.frame * prm.plane_frame_pitch[0] + (size_t)b.y0 * stride + b.x0;
-  const int top = dep_top[blk], left = dep_left[blk];
-  if (lane == 0) {
-    if (top >= 0) while (ld_acquire(done + top) != epoch) __nanosleep(64);
-    if (left >= 0) while (ld_acquire(done + left) != epoch) __nanosleep(64);
-  }
-  __syncwarp();
-  // g1/g2: energies of the neighbours' first three AC terms decide whether the
-  // low-frequency row or column is predicted (double sums of exact integers)
-  double g1 = 0, g2 = 0;
-  if (top >= 0) for (int i = 1; i < 4; i++) { double v = d[-(ptrdiff_t)n * stride + i]; g1 += v * v; }
-  if (left >= 0) for (int i = 1; i < 4; i++) { double v = d[(ptrdiff_t)i * stride - n]; g2 += v * v; }
-  const bool low_from_top = g1 > g2;
-  int32_t* vin = prm.in + b.coef_off;
-  int32_t* vref = prm.ref + b.coef_off;
-  for (int i = lane; i < len; i += 32) {
-    int r = 0, c = 0;
-    if (i) {
-      int v, sh;
-      if (i < 16) { v = kScan4[i - 1]; sh = 2; }
-      else if (i < 64) { v = kScan8[i - 16]; sh = 3; }
-      else if (i < 256) { v = kScan16[i - 64]; sh = 4; }
-      else { v = kScan32[i - 256]; sh = 5; }
-      r = v >> sh;
-      c = v & ((1 << sh) - 1);
-    }
-    vin[i] = d[(size_t)r * stride + c];
-    int32_t p = 0;
-    if (r == 0 && c > 0 && top >= 0 && (c >= 4 || low_from_top)) p = d[-(ptrdiff_t)n * stride + c];
-    if (c == 0 && r > 0 && left >= 0 && (r >= 4 || !low_from_top)) p = d[(ptrdiff_t)r * stride - n];
-    vref[i] = p;
-  }
-  __syncwarp();
-  const int nb = num_bands(bs);
-  double sd = 0;
-  for (int band = 0; band < nb; band++) {
-    const int start = band_start(band);
-    const int bn = band_start(band + 1) - start;
-    const size_t off = (size_t)b.coef_off + start;
-    int qidx = bs * (bs + 1) + (band + 1) - (band + 1) / 3;
-    int q = (prm.q0 * prm.pvq_qm_q4[0][qidx]) >> 4;
-    if (q < 1) q = 1;
-    const int beta = (prm.use_masking && bs > 0) ? kBeta15 : kBeta1;
-    const int qoff = ((((1 << (2 * bs)) - 1) << 4) / 3) + start;
-    int itheta, max_theta, k;
-    double skip_term;
-    int gain = quantise_band_coop<32, 4, false>(grp, prm.out + off, prm.in + off, prm.ref + off, bn, q, prm.y + off,
-                                                &itheta, &max_theta, &k, beta, &skip_term, 1, 0, prm.qm + qoff,
-                                                prm.qm_inv + qoff, prm.pvq_norm_lambda);
-    sd += skip_term;
-    if (lane == 0) {
-      const size_t r = (size_t)blk * 9 + band;
-      prm.res_gain[r] = gain;
-      prm.res_theta[r] = itheta;
-      prm.res_max_theta[r] = max_theta;
-      prm.res_k[r] = k;
-      prm.res_skip_term[r] = skip_term;
-    }
-  }
-  __syncwarp();
-  if (lane == 0) {
-    prm.res_skip_diff[blk] = sd;
-    prm.res_flip[blk] = 0;
-    prm.res_dc[blk] = 0;
-    prm.out[b.coef_off] = vin[0];
-  }
-  // od_init_skipped_coeffs + od_coding_order_to_raster (DC untouched on keyframes)
-  const int32_t* vout = prm.out + b.coef_off;
-  if (ln >= 5) {
-    for (int i = lane; i < n * n; i += 32) if (i) d[(size_t)(i >> ln) * stride + (i & (n - 1))] = 0;
-    __syncwarp();
-  }
-  for (int i = lane + 1; i < len; i += 32) {
-    int v, sh;
-    if (i < 16) { v = kScan4[i - 1]; sh = 2; }
-    else if (i < 64) { v = kScan8[i - 16]; sh = 3; }
-    else if (i < 256) { v = kScan16[i - 64]; sh = 4; }
-    else { v = kScan32[i - 256]; sh = 5; }
-    d[(size_t)(v >> sh) * stride + (v & ((1 << sh) - 1))] = vout[i];
-  }
-  if (prm.y16) for (int i = lane; i < len; i += 32) prm.y16[b.coef_off + i] = (int16_t)prm.y[b.coef_off + i];
-  __threadfence();
-  __syncwarp();
-  if (lane == 0) st_release(done + blk, epoch);
-}
-
-// Wave-synchronous alternative to the chain kernels: the host sorts luma blocks by
-// dependency depth; every wave (all blocks of one depth, their neighbours finished in
-// earlier waves) runs the ordinary batched kernels.  This kernel is the wave's gather:
-// `in` <- coefficient plane, `ref` <- H/V intra prediction from the quantised neighbours
-// (has_top / has_left: the neighbour of the same size exists, src/intra.c:46-47).
-__global__ void k_intra_pred_gather(const __grid_constant__ daala_b200_pvq_params prm,
-                                    const int32_t* __restrict__ dep_top, const int32_t* __restrict__ dep_left,
-                                    int first, int nblocks) {
-  const int slot = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (slot >= nblocks) return;
-  const int blk = first + slot;
-  const daala_b200_pvq_block b = prm.blocks[blk];
-  const int ln = b.bs + 2, n = 1 << ln;
-  const int len = ln >= 5 ? 512 : 1 << (2 * ln);
-  const int stride = prm.plane_stride[0];
-  const int32_t* d = prm.coef_plane[0] + b.frame * prm.plane_frame_pitch[0] + (size_t)b.y0 * stride + b.x0;
-  const bool top = dep_top[blk] >= 0, left = dep_left[blk] >= 0;
-  double g1 = 0, g2 = 0;
-  if (top) for (int i = 1; i < 4; i++) { double v = d[-(ptrdiff_t)n * stride + i]; g1 += v * v; }
-  if (left) for (int i = 1; i < 4; i++) { double v = d[(ptrdiff_t)i * stride - n]; g2 += v * v; }
-  const bool low_from_top = g1 > g2;
-  int32_t* vin = prm.in + b.coef_off;
-  int32_t* vref = prm.ref + b.coef_off;
-  for (int i = lane; i < len; i += 32) {
-    int r = 0, c = 0;
-    if (i) {
-      int v, sh;
-      if (i < 16) { v = kScan4[i - 1]; sh = 2; }
-      else if (i < 64) { v = kScan8[i - 16]; sh = 3; }
-      else if (i < 256) { v = kScan16[i - 64]; sh = 4; }
-      else { v = kScan32[i - 256]; sh = 5; }
-      r = v >> sh;
-      c = v & ((1 << sh) - 1);
-    }
-    vin[i] = d[(size_t)r * stride + c];
-    int32_t p = 0;
-    if (r == 0 && c > 0 && top && (c >= 4 || low_from_top)) p = d[-(ptrdiff_t)n * stride + c];
-    if (c == 0 && r > 0 && left && (r >= 4 || !low_from_top)) p = d[(ptrdiff_t)r * stride - n];
-    vref[i] = p;
-  }
-}
-
-// Band-granular form of the same prediction.  od_hv_intra_pred only fills row 0 and column 0 of the
-// block (src/intra.c:53-60), and the neighbour it reads has the SAME size, so coefficient (0, c) /
-// (r, 0) sits at the same coding-order index -- and in the same band -- in both blocks: band b of a
-// block depends on band b of its top / left neighbour only.  Of the bands of OD_BAND_OFFSETS, 1/4/7
+// Keyframe luma with the reference's H/V intra prediction (od_hv_intra_pred, src/intra.c:37): the
+// prediction of a block is row 0 / column 0 of the QUANTISED coefficients of its top / left neighbour
+// of the same size, so blocks form dependency chains (SURVEY.md 0.8).  It is built band by band:
+// od_hv_intra_pred only fills row 0 and column 0 of the block (src/intra.c:53-60), and the neighbour
+// it reads has the SAME size, so coefficient (0, c) / (r, 0) sits at the same coding-order index -- and
+// in the same band -- in both blocks: band b of a block depends on band b of its top / left neighbour
+// only.  Of the bands of OD_BAND_OFFSETS, 1/4/7
 // hold row-0 coefficients (top chain only), 2/5/8 column-0 coefficients (left chain only), 3/6 neither
 // (no dependency at all) and 0 the three low coefficients of each, whose source is chosen by the
 // neighbours' energies (:51-52, :55-60) -- again band-0 values only.  One warp per band-list entry
@@ -909,108 +759,6 @@ __global__ void k_intra_band_ref(const __grid_constant__ daala_b200_pvq_params p
     if (c == 0 && r > 0 && ol && (r >= 4 || !low_from_top)) p = ol[i];
     vref[i] = p;
   }
-}
-
-// Same chain link with one CTA per block and one WARP PER BAND (NB = bands of
-// this block size): the bands of a block are independent once the prediction
-// is known, so the latency of a link is the slowest band instead of their sum.
-// Dependencies only ever connect blocks of the SAME size (od_hv_intra_pred
-// tests the neighbour's size), so every size class is its own wavefront and
-// gets its own launch; `ids` lists the class's blocks in raster order.
-template <int NB>
-__global__ void __launch_bounds__(32 * NB)
-k_pvq_luma_intra_cta(const __grid_constant__ daala_b200_pvq_params prm, const int32_t* __restrict__ ids,
-                     const int32_t* __restrict__ dep_top, const int32_t* __restrict__ dep_left, int* done,
-                     int epoch) {
-  const int blk = ids[blockIdx.x];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const Group<32, 4> grp;
-  const daala_b200_pvq_block b = prm.blocks[blk];
-  const int bs = b.bs, ln = bs + 2, n = 1 << ln;
-  const int len = ln >= 5 ? 512 : 1 << (2 * ln);
-  const int stride = prm.plane_stride[0];
-  int32_t* d = prm.coef_plane[0] + b.frame * prm.plane_frame_pitch[0] + (size_t)b.y0 * stride + b.x0;
-  const int top = dep_top[blk], left = dep_left[blk];
-  if (threadIdx.x == 0) {
-    if (top >= 0) while (ld_acquire(done + top) != epoch) __nanosleep(32);
-    if (left >= 0) while (ld_acquire(done + left) != epoch) __nanosleep(32);
-  }
-  __syncthreads();
-  double g1 = 0, g2 = 0;
-  if (top >= 0) for (int i = 1; i < 4; i++) { double v = d[-(ptrdiff_t)n * stride + i]; g1 += v * v; }
-  if (left >= 0) for (int i = 1; i < 4; i++) { double v = d[(ptrdiff_t)i * stride - n]; g2 += v * v; }
-  const bool low_from_top = g1 > g2;
-  int32_t* vin = prm.in + b.coef_off;
-  int32_t* vref = prm.ref + b.coef_off;
-  for (int i = threadIdx.x; i < len; i += 32 * NB) {
-    int r = 0, c = 0;
-    if (i) {
-      int v, sh;
-      if (i < 16) { v = kScan4[i - 1]; sh = 2; }
-      else if (i < 64) { v = kScan8[i - 16]; sh = 3; }
-      else if (i < 256) { v = kScan16[i - 64]; sh = 4; }
-      else { v = kScan32[i - 256]; sh = 5; }
-      r = v >> sh;
-      c = v & ((1 << sh) - 1);
-    }
-    vin[i] = d[(size_t)r * stride + c];
-    int32_t p = 0;
-    if (r == 0 && c > 0 && top >= 0 && (c >= 4 || low_from_top)) p = d[-(ptrdiff_t)n * stride + c];
-    if (c == 0 && r > 0 && left >= 0 && (r >= 4 || !low_from_top)) p = d[(ptrdiff_t)r * stride - n];
-    vref[i] = p;
-  }
-  __syncthreads();
-  {
-    const int band = warp;
-    const int start = band_start(band);
-    const int bn = band_start(band + 1) - start;
-    const size_t off = (size_t)b.coef_off + start;
-    int qidx = bs * (bs + 1) + (band + 1) - (band + 1) / 3;
-    int q = (prm.q0 * prm.pvq_qm_q4[0][qidx]) >> 4;
-    if (q < 1) q = 1;
-    const int beta = (prm.use_masking && bs > 0) ? kBeta15 : kBeta1;
-    const int qoff = ((((1 << (2 * bs)) - 1) << 4) / 3) + start;
-    int itheta, max_theta, k;
-    double skip_term;
-    int gain = quantise_band_coop<32, 4, false>(grp, prm.out + off, prm.in + off, prm.ref + off, bn, q, prm.y + off,
-                                                &itheta, &max_theta, &k, beta, &skip_term, 1, 0, prm.qm + qoff,
-                                                prm.qm_inv + qoff, prm.pvq_norm_lambda);
-    if (lane == 0) {
-      const size_t r = (size_t)blk * 9 + band;
-      prm.res_gain[r] = gain;
-      prm.res_theta[r] = itheta;
-      prm.res_max_theta[r] = max_theta;
-      prm.res_k[r] = k;
-      prm.res_skip_term[r] = skip_term;
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double sd = 0;
-    for (int i = 0; i < NB; i++) sd += prm.res_skip_term[(size_t)blk * 9 + i];
-    prm.res_skip_diff[blk] = sd;
-    prm.res_flip[blk] = 0;
-    prm.res_dc[blk] = 0;
-    prm.out[b.coef_off] = vin[0];
-  }
-  const int32_t* vout = prm.out + b.coef_off;
-  if (ln >= 5) {
-    for (int i = threadIdx.x; i < n * n; i += 32 * NB) if (i) d[(size_t)(i >> ln) * stride + (i & (n - 1))] = 0;
-    __syncthreads();
-  }
-  for (int i = threadIdx.x + 1; i < len; i += 32 * NB) {
-    int v, sh;
-    if (i < 16) { v = kScan4[i - 1]; sh = 2; }
-    else if (i < 64) { v = kScan8[i - 16]; sh = 3; }
-    else if (i < 256) { v = kScan16[i - 64]; sh = 4; }
-    else { v = kScan32[i - 256]; sh = 5; }
-    d[(size_t)(v >> sh) * stride + (v & ((1 << sh) - 1))] = vout[i];
-  }
-  if (prm.y16)
-    for (int i = threadIdx.x; i < len; i += 32 * NB) prm.y16[b.coef_off + i] = (int16_t)prm.y[b.coef_off + i];
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) st_release(done + blk, epoch);
 }
 
 // Chroma-from-luma prediction of keyframe chroma blocks (od_resample_luma_coeffs,
@@ -1137,44 +885,19 @@ int daala_b200_pvq_encode_bands(const daala_b200_pvq_params* prm, const uint32_t
   return (int)cudaGetLastError();
 }
 
-// mode 0: best measured mix (see below), 3: all group-cooperative, default geometry, 1: same with the literal
-// sequential arg-max scan forced (test hook), 2: scalar thread-per-band kernels,
-// 10 + c: cooperative kernels with alternative lanes-per-band geometry c (tuning).
+// mode 0: best measured mix (see below), 1: group-cooperative kernels with the literal sequential arg-max scan
+// forced (test hook), 2: scalar thread-per-band kernels, 3: group-cooperative kernels everywhere.  Any other mode
+// is refused before anything is launched.
 int daala_b200_pvq_encode_bands_mode(const daala_b200_pvq_params* prm, const uint32_t* band_list, int count,
                                      int nmax, int mode, void* stream) {
+  if (mode < 0 || mode > 3) return (int)cudaErrorInvalidValue;
   if (count <= 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
   if (mode == 2) return daala_b200_pvq_encode_bands(prm, band_list, count, nmax, stream);
   const int cls = nmax <= 16 ? 0 : nmax <= 32 ? 1 : 2;
-  if (mode >= 20 && mode < 40) {
-    // occupancy experiments (tools/probe/time_modes_ref.py): 20/21 scalar kernels capped at 80 / 64
-    // registers (mode 2 = 64), 30/31 default cooperative geometry capped at 96 / 80 registers
-    const int blocks = (count + 127) / 128;
-    if (mode == 20) {
-      if (cls == 0) k_pvq_bands<16, 6><<<blocks, 128, 0, s>>>(*prm, band_list, count);
-      else if (cls == 1) k_pvq_bands<32, 6><<<blocks, 128, 0, s>>>(*prm, band_list, count);
-      else k_pvq_bands<128, 6><<<blocks, 128, 0, s>>>(*prm, band_list, count);
-    } else if (mode == 21) {
-      if (cls == 0) k_pvq_bands<16, 8><<<blocks, 128, 0, s>>>(*prm, band_list, count);
-      else if (cls == 1) k_pvq_bands<32, 8><<<blocks, 128, 0, s>>>(*prm, band_list, count);
-      else k_pvq_bands<128, 8><<<blocks, 128, 0, s>>>(*prm, band_list, count);
-    } else if (mode == 30) {
-      if (cls == 0) launch_coop<4, 4, false, 5>(prm, band_list, count, s);
-      else if (cls == 1) launch_coop<8, 4, false, 5>(prm, band_list, count, s);
-      else launch_coop<32, 4, false, 5>(prm, band_list, count, s);
-    } else if (mode == 31) {
-      if (cls == 0) launch_coop<4, 4, false, 6>(prm, band_list, count, s);
-      else if (cls == 1) launch_coop<8, 4, false, 6>(prm, band_list, count, s);
-      else launch_coop<32, 4, false, 6>(prm, band_list, count, s);
-    } else {
-      return (int)cudaErrorInvalidValue;
-    }
-    return (int)cudaGetLastError();
-  }
   if (mode == 0) {
-    // chosen by timing (tools/probe/time_modes_ref.py, real with-reference data): scalar threads
-    // for the short bands, a whole warp (32 lanes x 4 registers, capped at 80 registers = 6 CTAs per
-    // SM) for the 128-coefficient bands
+    // chosen by timing on real with-reference data: scalar threads for the short bands, a whole warp
+    // (32 lanes x 4 registers, capped at 80 registers = 6 CTAs per SM) for the 128-coefficient bands
     if (cls < 2) return daala_b200_pvq_encode_bands(prm, band_list, count, nmax, stream);
     launch_coop<32, 4, false, 6>(prm, band_list, count, s);
     return (int)cudaGetLastError();
@@ -1184,38 +907,10 @@ int daala_b200_pvq_encode_bands_mode(const daala_b200_pvq_params* prm, const uin
     else if (cls == 1) launch_coop<8, 4, true>(prm, band_list, count, s);
     else launch_coop<32, 4, true>(prm, band_list, count, s);
   } else {
-    const int cfg = mode >= 10 ? mode - 10 : 0;  // mode 3 -> geometry 0
-    if (cls == 0) {
-      if (cfg == 0) launch_coop<4, 4, false>(prm, band_list, count, s);
-      else if (cfg == 1) launch_coop<2, 8, false>(prm, band_list, count, s);
-      else launch_coop<1, 16, false>(prm, band_list, count, s);
-    } else if (cls == 1) {
-      if (cfg == 0) launch_coop<8, 4, false>(prm, band_list, count, s);
-      else if (cfg == 1) launch_coop<4, 8, false>(prm, band_list, count, s);
-      else launch_coop<2, 16, false>(prm, band_list, count, s);
-    } else {
-      if (cfg == 0) launch_coop<32, 4, false>(prm, band_list, count, s);
-      else if (cfg == 1) launch_coop<16, 8, false>(prm, band_list, count, s);
-      else if (cfg == 2) launch_coop<8, 16, false>(prm, band_list, count, s);
-      else launch_coop<4, 32, false>(prm, band_list, count, s);
-    }
+    if (cls == 0) launch_coop<4, 4, false>(prm, band_list, count, s);
+    else if (cls == 1) launch_coop<8, 4, false>(prm, band_list, count, s);
+    else launch_coop<32, 4, false>(prm, band_list, count, s);
   }
-  return (int)cudaGetLastError();
-}
-
-int daala_b200_pvq_luma_intra(const daala_b200_pvq_params* prm, const int32_t* dep_top, const int32_t* dep_left,
-                              int32_t* done, int epoch, int nblocks, void* stream) {
-  if (nblocks <= 0) return 0;
-  k_pvq_luma_intra<<<(nblocks * 32 + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*prm, nullptr, dep_top, dep_left,
-                                                                                 done, epoch, nblocks);
-  return (int)cudaGetLastError();
-}
-
-int daala_b200_pvq_intra_gather(const daala_b200_pvq_params* prm, const int32_t* dep_top, const int32_t* dep_left,
-                                int first, int count, void* stream) {
-  if (count <= 0) return 0;
-  k_intra_pred_gather<<<(count * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(*prm, dep_top, dep_left, first,
-                                                                                  count);
   return (int)cudaGetLastError();
 }
 
@@ -1250,41 +945,6 @@ int daala_b200_pvq_intra_band_ref(const daala_b200_pvq_params* prm, const int32_
   if (count <= 0) return 0;
   k_intra_band_ref<<<(count * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(*prm, dep_top, dep_left, band_list,
                                                                                count);
-  return (int)cudaGetLastError();
-}
-
-int daala_b200_pvq_block_finish_range(const daala_b200_pvq_params* prm, int first, int count, void* stream) {
-  if (count <= 0) return 0;
-  k_block_finish<<<(count + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*prm, first, count);
-  return (int)cudaGetLastError();
-}
-
-int daala_b200_coding_order_scatter_range(const daala_b200_pvq_params* prm, int first, int count, void* stream) {
-  if (count <= 0) return 0;
-  k_coding_order_scatter<<<(count * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(*prm, first, count);
-  return (int)cudaGetLastError();
-}
-
-// Warp-per-block kernel restricted to the blocks listed in `ids` (used for the 4x4 class).
-int daala_b200_pvq_luma_intra_ids(const daala_b200_pvq_params* prm, const int32_t* ids, int count,
-                                  const int32_t* dep_top, const int32_t* dep_left, int32_t* done, int epoch,
-                                  void* stream) {
-  if (count <= 0) return 0;
-  k_pvq_luma_intra<<<(count * 32 + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*prm, ids, dep_top, dep_left, done,
-                                                                               epoch, count);
-  return (int)cudaGetLastError();
-}
-
-// One launch for the blocks of one size (`bs` = 1..4) listed in `ids`.
-int daala_b200_pvq_luma_intra_class(const daala_b200_pvq_params* prm, const int32_t* ids, int count, int bs,
-                                    const int32_t* dep_top, const int32_t* dep_left, int32_t* done, int epoch,
-                                    void* stream) {
-  if (count <= 0) return 0;
-  cudaStream_t s = (cudaStream_t)stream;
-  if (bs == 1) k_pvq_luma_intra_cta<4><<<count, 128, 0, s>>>(*prm, ids, dep_top, dep_left, done, epoch);
-  else if (bs == 2) k_pvq_luma_intra_cta<7><<<count, 224, 0, s>>>(*prm, ids, dep_top, dep_left, done, epoch);
-  else if (bs >= 3) k_pvq_luma_intra_cta<9><<<count, 288, 0, s>>>(*prm, ids, dep_top, dep_left, done, epoch);
-  else return (int)cudaErrorInvalidValue;
   return (int)cudaGetLastError();
 }
 

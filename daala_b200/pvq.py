@@ -51,20 +51,10 @@ def _bind():
     for name in ("daala_b200_pvq_block_finish", "daala_b200_pvq_cfl_flip", "daala_b200_coding_order_scatter"):
         getattr(L, name).argtypes = [pp, ctypes.c_int, ctypes.c_void_p]
     L.daala_b200_coding_order_gather.argtypes = [pp, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
-    L.daala_b200_pvq_luma_intra.argtypes = [pp, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
-                                            ctypes.c_int, ctypes.c_void_p]
-    L.daala_b200_pvq_luma_intra_ids.argtypes = [pp, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
-                                                ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
-    L.daala_b200_pvq_luma_intra_class.argtypes = [pp, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
-                                                  ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
-    L.daala_b200_pvq_intra_gather.argtypes = [pp, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
-                                              ctypes.c_void_p]
     L.daala_b200_pvq_intra_band_ref.argtypes = [pp, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
                                                   ctypes.c_void_p]
     L.daala_b200_pvq_order_by_work.argtypes = [pp, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                  ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    L.daala_b200_pvq_block_finish_range.argtypes = [pp, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
-    L.daala_b200_coding_order_scatter_range.argtypes = [pp, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
     L.daala_b200_pvq_cfl_pred.argtypes = [pp, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_int, ctypes.c_int,
                                           ctypes.c_void_p]
     L._pvq_bound = True
@@ -350,6 +340,12 @@ def native_keyframe_lists(bsize_maps, geom, nthreads=8):
     return out
 
 
+# Luma chain waves of fewer bands than this (per size class) use the group-cooperative kernels: shorter latency
+# than the default mix (measured crossover of the scalar and 16-lane kernels).
+COOP_WAVE_BANDS = {16: 32768, 32: 65536, 128: 0}
+COOP_WAVE_MODE = 3
+
+
 class PvqBatch:
     """Device state of one PVQ batch: coding-order buffers, result arrays and
     the launch sequence gather -> [CfL flip] -> bands -> finish -> scatter."""
@@ -410,10 +406,8 @@ class PvqBatch:
                 p.pvq_qm_q4[pli][i] = int(pvq_qm_q4[pli][i])
         self.params = p
         self.is_keyframe = int(is_keyframe)
-        # kernel choice of daala_b200_pvq_encode_bands_mode (0 = measured-best mix); per size class
-        # override (None = self.mode) for tuning
+        # kernel choice of daala_b200_pvq_encode_bands_mode (0 = measured-best mix)
         self.mode = 0
-        self.class_mode = {16: None, 32: None, 128: None}
         # bucket every launch's entries by expected search work (daala_b200_pvq_order_by_work)
         self.order_by_work = True
         self._order_bins = torch.zeros(_bind().daala_b200_pvq_order_bins(), dtype=torch.int32, device=dev)
@@ -460,8 +454,7 @@ class PvqBatch:
                 n += self._order(lst, self.ordered[nmax], nmax, s)
                 lst = self.ordered[nmax]
             if lst.numel():
-                mode = self.mode if self.class_mode[nmax] is None else self.class_mode[nmax]
-                _native.check(L.daala_b200_pvq_encode_bands_mode(p, lst.data_ptr(), lst.numel(), nmax, mode, s),
+                _native.check(L.daala_b200_pvq_encode_bands_mode(p, lst.data_ptr(), lst.numel(), nmax, self.mode, s),
                               "pvq_bands")
                 n += 1
         _native.check(L.daala_b200_pvq_block_finish(p, self.nblocks, s), "block_finish")
@@ -473,28 +466,16 @@ class PvqBatch:
                       "scatter")
 
     # --- keyframe predictors -------------------------------------------------
-    def _intra_streams_and_tuning(self):
+    def _intra_streams(self):
         dev = self.device
         if dev.type == "cuda":
             self.chain_streams = {k: torch.cuda.Stream(device=dev, priority=-1) for k in (16, 32, 128)}
             self.bulk_stream = torch.cuda.Stream(device=dev)
         else:                       # host-side dry runs of the list plumbing (tests)
             self.chain_streams, self.bulk_stream = {}, None
-        # waves smaller than this many bands use the group-cooperative kernels (shorter latency)
-        # (tools/probe/time_bandwaves.py, time_modes_ref.py: crossover of the scalar / 16-lane kernels)
-        self.small_wave = {16: 32768, 32: 65536, 128: 0}
-        self.small_mode = 3
-        if os.environ.get("DAALA_B200_SMALL_WAVE"):          # tuning hook: "n16,n32,n128"
-            self.small_wave = dict(zip((16, 32, 128), map(int, os.environ["DAALA_B200_SMALL_WAVE"].split(","))))
-        if os.environ.get("DAALA_B200_ONE_CHAIN_STREAM") and self.chain_streams:     # tuning hook
-            one = self.chain_streams[128]
-            self.chain_streams = {k: one for k in self.chain_streams}
-            self.bulk_stream = one
-        self.intra_mode = "bands"
 
     def setup_intra_device(self, lists):
-        """setup_intra for descriptors built on the device (lists_torch.keyframe_lists output): only the
-        band-granular wavefront ("bands") is available, the block-granular alternatives need host arrays."""
+        """setup_intra for descriptors built on the device (lists_torch.keyframe_lists output)."""
         dev = self.device
         self.dep_top, self.dep_left = lists["dep_top"].to(dev), lists["dep_left"].to(dev)
         self.max_depth = int(lists["depth"].max().item()) if self.nblocks else 0
@@ -507,39 +488,18 @@ class PvqBatch:
         need = max([v.numel() for v in self.chain_lists.values()] + [v.numel() for v in self.bulk_lists.values()] + [1])
         if need > self._order_keys.numel():
             self._order_keys = torch.zeros(need, dtype=torch.int16, device=dev)
-        self._intra_streams_and_tuning()
+        self._intra_streams()
 
     def setup_intra(self, top, left, depth):
         """Luma-only batch whose blocks are sorted by dependency depth (see
-        `sort_by_depth`): neighbour indices for the chain kernels, wave ranges and
-        per-wave band-list slices for the wave-synchronous path."""
+        `sort_by_depth`): neighbour indices and the band-granular wave lists."""
         dev = self.device
         self.dep_top = torch.from_numpy(np.ascontiguousarray(top)).to(dev)
         self.dep_left = torch.from_numpy(np.ascontiguousarray(left)).to(dev)
-        self.done = torch.zeros(self.nblocks, dtype=torch.int32, device=dev)
-        self.epoch = 0
         self.max_depth = int(depth.max()) if len(depth) else 0
-        # chain kernels: per block size, indices in (depth, raster) order
-        self.class_ids = [torch.from_numpy(np.nonzero(self.blocks_np["bs"] == bs)[0].astype(np.int32)).to(dev)
-                          for bs in range(5)]
-        self.class_streams = [torch.cuda.Stream(device=dev) for _ in range(5)] if dev.type == "cuda" else []
-        # waves: contiguous block ranges of equal depth
-        edges = np.concatenate([[0], np.nonzero(np.diff(depth))[0] + 1, [len(depth)]]) if len(depth) else np.array([0])
-        self.waves = [(int(a), int(b - a)) for a, b in zip(edges[:-1], edges[1:])]
-        # band lists ordered by (wave, band, block) so that a wave is a slice of each class list
-        lists = band_lists(self.blocks_np)
-        self.wave_lists, self.wave_slices = {}, {}
-        for k, v in lists.items():
-            blk, band = (v >> 4).astype(np.int64), (v & 15).astype(np.int64)
-            order = np.lexsort((blk, band, depth[blk]))
-            v = v[order]
-            self.wave_lists[k] = torch.from_numpy(v.view(np.int32)).to(dev)
-            d = depth[(v >> 4).astype(np.int64)]
-            cuts = np.searchsorted(d, np.arange(1, self.max_depth + 2))
-            self.wave_slices[k] = [(int(a), int(b - a)) for a, b in zip(cuts[:-1], cuts[1:])]
-        # band-granular waves (default): band b of a block depends on band b of the same-size top
-        # (bands 1/4/7), left (2/5/8), both (0) or no (3/6) neighbour -- see k_intra_band_ref.  Every
-        # size class is a closed dependency system, so each gets its own stream and wave sequence.
+        # band b of a block depends on band b of the same-size top (bands 1/4/7), left (2/5/8),
+        # both (0) or no (3/6) neighbour -- see k_intra_band_ref.  Every size class is a closed
+        # dependency system, so each gets its own stream and wave sequence.
         bulk, chain, self.chain_slices = band_wave_lists(self.blocks_np, top, left, depth)
         as_dev = lambda v: torch.from_numpy(np.ascontiguousarray(v).view(np.int32)).to(dev)  # noqa: E731
         self.bulk_lists = {k: as_dev(v) for k, v in bulk.items()}
@@ -551,90 +511,50 @@ class PvqBatch:
             self.chain_waves[k] = torch.from_numpy(w.view(np.int16)).to(dev)
             self.chain_ordered[k] = torch.empty_like(self.chain_lists[k])
             self.bulk_ordered[k] = torch.empty_like(self.bulk_lists[k])
-        self._intra_streams_and_tuning()
+        self._intra_streams()
 
     def run_luma_intra(self, stream=None):
         L = _bind()
         p = ctypes.byref(self.params)
-        if self.intra_mode == "bands":
-            main = stream if stream is not None else torch.cuda.current_stream(self.device)
-            _native.check(L.daala_b200_coding_order_gather(p, self.nblocks, 0, self._s(main)), "gather(in)")
-            n = 1
-            top, left = self.dep_top.data_ptr(), self.dep_left.data_ptr()
-            chain_lists, bulk_lists = self.chain_lists, self.bulk_lists
-            if self.order_by_work:
-                for k in (128, 32, 16):
-                    n += self._order(self.chain_lists[k], self.chain_ordered[k], k, self._s(main),
-                                     self.chain_waves[k], max(1, len(self.chain_slices[k])))
-                    n += self._order(self.bulk_lists[k], self.bulk_ordered[k], k, self._s(main))
-                chain_lists, bulk_lists = self.chain_ordered, self.bulk_ordered
-            # latency-bound chains first (high-priority streams), the dependency-free bands fill the GPU behind
-            for k in (128, 32, 16):
-                st = self.chain_streams[k]
-                st.wait_stream(main)
-                sp = ctypes.c_void_p(st.cuda_stream)
-                for w, (a, c) in enumerate(self.chain_slices[k]):
-                    if not c:
-                        continue
-                    ptr = chain_lists[k].data_ptr() + 4 * a
-                    if w > 0:
-                        _native.check(L.daala_b200_pvq_intra_band_ref(p, top, left, ptr, c, sp), "intra_band_ref")
-                        n += 1
-                    mode = self.small_mode if c < self.small_wave[k] else self.mode
-                    _native.check(L.daala_b200_pvq_encode_bands_mode(p, ptr, c, k, mode, sp), "pvq_bands")
-                    n += 1
-            self.bulk_stream.wait_stream(main)
-            sp = ctypes.c_void_p(self.bulk_stream.cuda_stream)
-            for k in (128, 32):
-                lst = bulk_lists[k]
-                if lst.numel():
-                    _native.check(L.daala_b200_pvq_encode_bands_mode(p, lst.data_ptr(), lst.numel(), k, self.mode, sp),
-                                  "pvq_bands")
-                    n += 1
-            for st in list(self.chain_streams.values()) + [self.bulk_stream]:
-                main.wait_stream(st)
-            _native.check(L.daala_b200_pvq_block_finish(p, self.nblocks, self._s(main)), "block_finish")
-            _native.check(L.daala_b200_coding_order_scatter(p, self.nblocks, self._s(main)), "scatter")
-            return n + 2
-        if self.intra_mode == "waves":
-            s = self._s(stream)
-            n = 0
-            for w, (first, count) in enumerate(self.waves):
-                _native.check(L.daala_b200_pvq_intra_gather(p, self.dep_top.data_ptr(), self.dep_left.data_ptr(),
-                                                            first, count, s), "intra_gather")
-                for nmax in (128, 32, 16):
-                    a, c = self.wave_slices[nmax][w]
-                    if c:
-                        ptr = self.wave_lists[nmax].data_ptr() + 4 * a
-                        _native.check(L.daala_b200_pvq_encode_bands_mode(p, ptr, c, nmax, self.mode, s), "pvq_bands")
-                        n += 1
-                _native.check(L.daala_b200_pvq_block_finish_range(p, first, count, s), "finish_range")
-                _native.check(L.daala_b200_coding_order_scatter_range(p, first, count, s), "scatter_range")
-                n += 3
-            return n
-        self.epoch += 1
-        deps = (self.dep_top.data_ptr(), self.dep_left.data_ptr(), self.done.data_ptr(), self.epoch)
-        if self.intra_mode == "chain_single":
-            _native.check(L.daala_b200_pvq_luma_intra(p, *deps, self.nblocks, self._s(stream)), "pvq_luma_intra")
-            return 1
-        # "chain": one launch per block size, concurrently on side streams that fork from / join the caller's
         main = stream if stream is not None else torch.cuda.current_stream(self.device)
-        n = 0
-        for bs in (4, 3, 2, 1, 0):
-            ids = self.class_ids[bs]
-            if not ids.numel():
-                continue
-            st = self.class_streams[bs]
+        _native.check(L.daala_b200_coding_order_gather(p, self.nblocks, 0, self._s(main)), "gather(in)")
+        n = 1
+        top, left = self.dep_top.data_ptr(), self.dep_left.data_ptr()
+        chain_lists, bulk_lists = self.chain_lists, self.bulk_lists
+        if self.order_by_work:
+            for k in (128, 32, 16):
+                n += self._order(self.chain_lists[k], self.chain_ordered[k], k, self._s(main),
+                                 self.chain_waves[k], max(1, len(self.chain_slices[k])))
+                n += self._order(self.bulk_lists[k], self.bulk_ordered[k], k, self._s(main))
+            chain_lists, bulk_lists = self.chain_ordered, self.bulk_ordered
+        # latency-bound chains first (high-priority streams), the dependency-free bands fill the GPU behind
+        for k in (128, 32, 16):
+            st = self.chain_streams[k]
             st.wait_stream(main)
             sp = ctypes.c_void_p(st.cuda_stream)
-            if bs == 0:
-                _native.check(L.daala_b200_pvq_luma_intra_ids(p, ids.data_ptr(), ids.numel(), *deps, sp), "intra_ids")
-            else:
-                _native.check(L.daala_b200_pvq_luma_intra_class(p, ids.data_ptr(), ids.numel(), bs, *deps, sp),
-                              "intra_class")
+            for w, (a, c) in enumerate(self.chain_slices[k]):
+                if not c:
+                    continue
+                ptr = chain_lists[k].data_ptr() + 4 * a
+                if w > 0:
+                    _native.check(L.daala_b200_pvq_intra_band_ref(p, top, left, ptr, c, sp), "intra_band_ref")
+                    n += 1
+                mode = COOP_WAVE_MODE if c < COOP_WAVE_BANDS[k] else self.mode
+                _native.check(L.daala_b200_pvq_encode_bands_mode(p, ptr, c, k, mode, sp), "pvq_bands")
+                n += 1
+        self.bulk_stream.wait_stream(main)
+        sp = ctypes.c_void_p(self.bulk_stream.cuda_stream)
+        for k in (128, 32):
+            lst = bulk_lists[k]
+            if lst.numel():
+                _native.check(L.daala_b200_pvq_encode_bands_mode(p, lst.data_ptr(), lst.numel(), k, self.mode, sp),
+                              "pvq_bands")
+                n += 1
+        for st in list(self.chain_streams.values()) + [self.bulk_stream]:
             main.wait_stream(st)
-            n += 1
-        return n
+        _native.check(L.daala_b200_pvq_block_finish(p, self.nblocks, self._s(main)), "block_finish")
+        _native.check(L.daala_b200_coding_order_scatter(p, self.nblocks, self._s(main)), "scatter")
+        return n + 2
 
     def cfl_pred(self, pred_plane, stream=None):
         """Fill the chroma prediction plane ([F, h/2, w/2] int32) from the quantised luma."""

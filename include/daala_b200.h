@@ -290,25 +290,10 @@ int daala_b200_pvq_encode_bands(const daala_b200_pvq_params *prm, const uint32_t
    band for n = 128), 1 = group-cooperative kernels with the literal sequential
    arg-max scan forced (test hook for the rare inexact-product regime), 2 = scalar
    kernels everywhere (what _encode_bands launches), 3 = group-cooperative
-   kernels everywhere, 10 + c = alternative lanes-per-band geometries, 20/21/30/31 =
-   register-cap (occupancy) variants (tuning). */
+   kernels everywhere.  All four give identical results.  Any other mode returns
+   cudaErrorInvalidValue before anything is launched, also when count <= 0. */
 int daala_b200_pvq_encode_bands_mode(const daala_b200_pvq_params *prm, const uint32_t *band_list, int count,
                                      int nmax, int mode, void *stream);
-/* Keyframe luma WITH the reference's H/V intra prediction (od_hv_intra_pred,
-   src/intra.c:37; od_encode_compute_pred, src/encode.c:858): one warp per block runs gather,
-   prediction from the quantised neighbours, every band, and the scatter back into
-   coef_plane[0]; blocks wait for their top / left same-size neighbours through `done`
-   (done[i] == epoch once block i is reconstructed).  `blocks` must list luma blocks only, in
-   raster order of their origin per frame; dep_top / dep_left give the neighbour's block index or
-   -1 (daala_b200/pvq.py: intra_dependencies).  Fills the same result arrays as the band kernels. */
-int daala_b200_pvq_luma_intra(const daala_b200_pvq_params *prm, const int32_t *dep_top, const int32_t *dep_left,
-                              int32_t *done, int epoch, int nblocks, void *stream);
-/* Wave-synchronous form of the same computation: luma blocks sorted by dependency depth; for
-   each wave (blocks [first, first+count) of one depth) the caller runs _intra_gather, the band
-   kernels on the wave's slices of the band lists, _block_finish_range and
-   _coding_order_scatter_range.  dep_top / dep_left only need their sign here. */
-int daala_b200_pvq_intra_gather(const daala_b200_pvq_params *prm, const int32_t *dep_top, const int32_t *dep_left,
-                                int first, int count, void *stream);
 /* Work ordering of a band list (3 kernel launches): `ordered` receives the entries of `band_list`
    bucketed by (wave, expected search work), heaviest first inside each wave.  The lanes of a warp of
    the band kernels then run similar trip counts (1.3-2x on real data); results do not depend on the
@@ -320,7 +305,8 @@ int daala_b200_pvq_order_by_work(const daala_b200_pvq_params *prm, const uint32_
                                  uint16_t *keys, int32_t *bins, void *stream);
 int daala_b200_pvq_order_bins(void);
 
-/* Band-granular wavefront (the default): od_hv_intra_pred (src/intra.c:37) couples band b of a block
+/* Keyframe luma with the reference's H/V intra prediction, as a band-granular wavefront
+   (od_encode_compute_pred, src/encode.c:858): od_hv_intra_pred (src/intra.c:37) couples band b of a block
    only to band b of the same-size top / left neighbour (row-0 bands 1/4/7: top, column-0 bands 2/5/8:
    left, bands 3/6: none, band 0: both).  For the entries of `band_list` ((block << 4) | band, all of
    one dependency depth >= 2) this writes the bands' slices of `ref` from the neighbours' `out`; the
@@ -328,18 +314,6 @@ int daala_b200_pvq_order_bins(void);
    the neighbour block in prm->blocks or -1. */
 int daala_b200_pvq_intra_band_ref(const daala_b200_pvq_params *prm, const int32_t *dep_top, const int32_t *dep_left,
                                   const uint32_t *band_list, int count, void *stream);
-int daala_b200_pvq_block_finish_range(const daala_b200_pvq_params *prm, int first, int count, void *stream);
-int daala_b200_coding_order_scatter_range(const daala_b200_pvq_params *prm, int first, int count, void *stream);
-/* The same split by block size (chains only connect blocks of equal size): `ids` lists the
-   blocks of one size in raster order.  _ids: one warp per block (used for 4x4 blocks);
-   _class (bs = 1..4): one CTA per block, one warp per band.  The launches of different sizes are
-   independent and may run on different streams. */
-int daala_b200_pvq_luma_intra_ids(const daala_b200_pvq_params *prm, const int32_t *ids, int count,
-                                  const int32_t *dep_top, const int32_t *dep_left, int32_t *done, int epoch,
-                                  void *stream);
-int daala_b200_pvq_luma_intra_class(const daala_b200_pvq_params *prm, const int32_t *ids, int count, int bs,
-                                    const int32_t *dep_top, const int32_t *dep_left, int32_t *done, int epoch,
-                                    void *stream);
 /* Chroma-from-luma prediction planes for keyframe chroma blocks (od_resample_luma_coeffs,
    src/intra.c:72, 4:2:0) from the quantised luma plane coef_plane[0]; bit 7 of a block's `xdec`
    field marks "the luma area is coded as 4x4 blocks" (TF merge + OD_CFL_SCALING4). */

@@ -168,7 +168,7 @@ def test_pvq_kernel_variants_agree(is_keyframe, with_pred):
     import torch
     geom, cur, pred, batch, qm_q4 = _setup((640, 384), is_keyframe, with_pred, q0=30, seed=12)
     outs = []
-    for mode in (2, 0, 1, 3, 11, 12, 13):
+    for mode in (2, 0, 1, 3):
         batch.mode = mode
         for t in (batch.out, batch.y, batch.res_gain, batch.res_theta, batch.res_k, batch.res_skip_term):
             t.zero_()
@@ -183,8 +183,7 @@ def test_pvq_kernel_variants_agree(is_keyframe, with_pred):
             assert torch.equal(a, b)
 
 
-@pytest.mark.parametrize("intra_mode", ["bands", "waves", "chain", "chain_single"])
-def test_keyframe_with_intra_and_cfl_prediction_matches_frame_oracle(intra_mode):
+def test_keyframe_with_intra_and_cfl_prediction_matches_frame_oracle():
     """The complete keyframe chain of the reference on the GPU: forward, luma PVQ
     with H/V intra prediction (dependency wavefront), chroma PVQ with CfL, inverse."""
     import torch
@@ -205,7 +204,6 @@ def test_keyframe_with_intra_and_cfl_prediction_matches_frame_oracle(intra_mode)
         hp.fb.upload(planes, bsize, frame=f)
         frames.append((planes, bsize))
     hp.set_block_sizes([b for _, b in frames])
-    hp.batch_luma.intra_mode = intra_mode
     hp.run()
     torch.cuda.synchronize()
     qm, qm_inv = pvq.default_qm(True)

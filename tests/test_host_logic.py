@@ -200,7 +200,7 @@ def test_hot_path_plumbing_is_identical_with_device_built_lists():
                                                        b.batch_luma.bulk_lists[k].numel())
     assert torch.equal(a.batch_luma.dep_top, b.batch_luma.dep_top)
     assert torch.equal(a.batch_luma.dep_left, b.batch_luma.dep_left)
-    assert a.batch_luma.max_depth == b.batch_luma.max_depth and b.batch_luma.intra_mode == "bands"
+    assert a.batch_luma.max_depth == b.batch_luma.max_depth
 
 
 def test_header_is_plain_c_and_reference_arm_prints_the_contract_line(tmp_path):
@@ -243,6 +243,19 @@ def test_library_exports_every_declared_symbol():
     assert not missing, missing
     assert L.daala_b200_version().startswith(b"daala_b200")
     assert L.daala_b200_device_count() >= 0
+
+
+def test_unknown_pvq_kernel_modes_are_refused_before_any_launch():
+    """daala_b200_pvq_encode_bands_mode knows modes 0-3; any other mode returns cudaErrorInvalidValue (1) even for
+    an empty band list, so nothing is launched and no device is needed to check it."""
+    import ctypes
+    from daala_b200 import pvq
+    L = pvq._bind()
+    prm = pvq.PvqParams()
+    for mode in (4, 11, 20, 30, -1):
+        assert L.daala_b200_pvq_encode_bands_mode(ctypes.byref(prm), None, 0, 128, mode, None) == 1, mode
+    for mode in range(4):
+        assert L.daala_b200_pvq_encode_bands_mode(ctypes.byref(prm), None, 0, 128, mode, None) == 0, mode
 
 
 def test_native_struct_layouts_match_the_header():
