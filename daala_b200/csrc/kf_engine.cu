@@ -510,6 +510,10 @@ __global__ void __launch_bounds__(256) k_cfl_plane(const __grid_constant__ Stage
 constexpr int kPersistThreads = 32;
 // resident CTAs per SM the persistent PVQ kernel is compiled for (register cap = 65536 / 32 / this = 64)
 constexpr int kPersistCtas = 32;
+// all of them resident: per CTA the warp's scratch (quantise_band_warp) plus the 1 KB the SM reserves, within
+// the 228 KB of shared memory an sm_90 SM has (kf_alloc checks the same at run time)
+static_assert(kPersistCtas * (kPersistThreads / 32 * kSnapEntries * (int)sizeof(int16_t) + 1024) <= 228 * 1024,
+              "k_pvq_persist's shared scratch does not fit kPersistCtas CTAs per SM");
 constexpr uint32_t kNoItem = 0xffffffffu;
 constexpr uint32_t kExit = 0xfffffffeu;
 
@@ -841,7 +845,8 @@ __global__ void __launch_bounds__(128, 4) k_pvq_levels(const __grid_constant__ S
 // successor (band 0 forks) into the chain queue.
 template <bool kIntra>
 __global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(const __grid_constant__ Stage S) {
-  __shared__ int16_t snap_all[kPersistThreads / 32][kSnapEntries];   // per warp: the pulses of every search event of a band
+  // per warp: the pulses of every search event of a band and the band's parked context (quantise_band_warp)
+  __shared__ __align__(16) int16_t snap_all[kPersistThreads / 32][kSnapEntries];
   const int lane = threadIdx.x & 31;
   int16_t* snap = snap_all[threadIdx.x >> 5];
   int done = 0;
@@ -1430,6 +1435,23 @@ static int kf_alloc(daala_b200_kf* kf) {
     KF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pvq_levels, 128, 0));
     if (per_sm < 1) return (int)cudaErrorLaunchOutOfResources;
     kf->lvl_grid = per_sm * kf->sms;   // all CTAs resident: the kernel synchronises the whole grid
+  }
+  {
+    // the persistent grid is sized to be resident at once: 32 one-warp CTAs with kSnapEntries of shared
+    // scratch each (plus the 1 KB the SM reserves per CTA) need 223 of the SM's 228 KB
+    const int want = kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas;
+    int per_sm[2] = {0, 0};
+    KF_CHECK(cudaFuncSetAttribute(k_pvq_persist<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                  cudaSharedmemCarveoutMaxShared));
+    KF_CHECK(cudaFuncSetAttribute(k_pvq_persist<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                  cudaSharedmemCarveoutMaxShared));
+    KF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[0], k_pvq_persist<true>, kPersistThreads, 0));
+    KF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[1], k_pvq_persist<false>, kPersistThreads, 0));
+    if (per_sm[0] < want || per_sm[1] < want) {
+      snprintf(kf->err, sizeof(kf->err), "k_pvq_persist: %d / %d CTAs per SM resident, %d wanted", per_sm[0],
+               per_sm[1], want);
+      return (int)cudaErrorLaunchOutOfResources;
+    }
   }
   KF_CHECK(dalloc(kf, &L.heads, kf->chain_cap));
   KF_CHECK(dalloc(kf, &L.heads0, (size_t)L.max_luma));

@@ -7,10 +7,11 @@ namespace daala_b200 {
 namespace pvq {
 
 // Band boundaries in coding order (OD_BAND_OFFSETS, src/partition.c:85-91).
+// 1, then 16, 24, 32 times 4^g for g = 0, 1, 2: arithmetic rather than a table, which a run-time index
+// would put in local memory.
 __device__ __forceinline__ int band_start(int band) {
-  // 1,16,24,32,64,96,128,256,384,512
-  const int t[10] = {1, 16, 24, 32, 64, 96, 128, 256, 384, 512};
-  return t[band];
+  const int g = (band - 1) / 3, r = (band - 1) - 3 * g;
+  return band == 0 ? 1 : (16 + 8 * r) << (2 * g);
 }
 
 __device__ __forceinline__ int num_bands(int bs) { return bs == 0 ? 1 : bs == 1 ? 4 : bs == 2 ? 7 : 9; }

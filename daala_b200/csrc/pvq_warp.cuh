@@ -50,7 +50,6 @@ namespace pvq {
 
 constexpr unsigned kFull = 0xffffffffu;
 constexpr int kMaxEvents = 14;                      // <= 12 with-reference K values + 2 no-reference gains
-constexpr int kSnapEntries = kMaxEvents * kMaxN;    // int16 entries of per-warp scratch
 constexpr int kRsqrtEntries = 1 << 16;              // table of the reference's 1/sqrt(i), i < 65536
 constexpr int kLogEntries = 1 << 12;                // table of .9 * (M_LOG2E * log(ts)) behind it
 constexpr int kTableDoubles = kRsqrtEntries + kLogEntries;
@@ -159,10 +158,10 @@ __device__ __forceinline__ void householder_apply_warp(int lane, bool big, int (
 
 // What one search phase (with-reference: the reflected vector without element m; no-reference: the
 // vector itself) keeps for all its events.
+// |x| <= 32768 converts exactly to float and double, so the reference's fabs((double)(float)xcoeff[j]) is
+// (double)xa[j], converted where it is used rather than kept in registers.
 struct SearchVec {
   int xa[4];      // |x|, 0 past the end
-  double xd[4];   // == fabs((double)(float)xcoeff[j]): |int16| is exact in float
-  float xf[4];
   double xx, norm_1, l1_norm;
   double delta_rate;   // 3. / nn
   int xmax, nn;
@@ -176,8 +175,6 @@ __device__ __forceinline__ void search_init(int lane, SearchVec& v, const int (&
   for (int e = 0; e < E; e++) {
     const int a = e * 32 + lane < nn ? abs(src[e]) : 0;
     v.xa[e] = a;
-    v.xd[e] = (double)a;
-    v.xf[e] = (float)a;
     sxx += (long long)a * a;
     sl1 += a;
     xmax = a > xmax ? a : xmax;
@@ -217,7 +214,7 @@ __device__ __forceinline__ void search_event(int lane, const SearchVec& v, int (
     int si = 0;
 #pragma unroll
     for (int e = 0; e < E; e++) {
-      const double tmp = k * v.xd[e] * l1_inv;
+      const double tmp = k * (double)v.xa[e] * l1_inv;
       const int f = (int)floor(tmp);
       ya[e] = (e * 32 + lane < nn && f > 0) ? f : 0;
       sxy += (long long)v.xa[e] * ya[e];
@@ -255,7 +252,7 @@ __device__ __forceinline__ void search_event(int lane, const SearchVec& v, int (
         unsigned key[E], kmax = 0;
 #pragma unroll
         for (int e = 0; e < E; e++) {
-          float a = xyf + v.xf[e];
+          float a = xyf + (float)v.xa[e];
           a *= a;
           const float b = yyf1 + (float)(2 * ya[e]);
           key[e] = e * 32 + lane < nn ? __float_as_uint(__fdividef(a, b)) : 0u;
@@ -288,7 +285,7 @@ __device__ __forceinline__ void search_event(int lane, const SearchVec& v, int (
         const int j = e * 32 + lane;
         const int arg = iyy + 2 * ya[e] + 1;
         const double ryy = arg < kRsqrtEntries ? rsq[arg] : nl_rsqrt_small((int)(yy + 2 * ya[e] + 1));
-        double t = xy + v.xd[e];
+        double t = xy + (double)v.xa[e];
         t = 2 * t * v.norm_1 * ryy - lambda * j * (delta_rate + j * accel_rate);
         tval[e] = t;
         key[e] = j < nn ? ordered_key((float)t) : (int)0x80000000;
@@ -350,8 +347,9 @@ __device__ __forceinline__ void search_event(int lane, const SearchVec& v, int (
   *yy_out = yy;
 }
 
-// What the three phases of one band share: registers in the fused path (quantise_band_warp), records in
-// HBM when the phases run as separate kernels (band_state_store / _load).
+// What the three phases of one band share.  Between the phases it is parked in a record (band_ctx_*):
+// in the warp's shared scratch when one warp runs them back to back (quantise_band_warp), in HBM when they
+// run as separate kernels.
 struct BandCtx {
   int x16[4], r16[4], xr[4];             // the vectors (int16 values), r16 after od_compute_householder
   int32_t cg, g, gain_offset;            // uniform
@@ -364,11 +362,22 @@ struct BandCtx {
   int e_sum, e_k, e_zero;
 };
 
-// ---- the context as a record in HBM (phases as separate kernels) ---------------------------------------
+// ---- the context as a record -----------------------------------------------------------------------------
 // vec: int16 [3][vstride] (x16, r16, xr); lanes: int32 [kCtxLaneWords][16] (only lanes 0..15 carry
 // candidates / events); uni: int32 [kCtxUniWords].
 constexpr int kCtxLaneWords = 24;
 constexpr int kCtxUniWords = 16;
+// The per-warp scratch quantise_band_warp takes, in int16 entries (4-byte aligned): the pulses of every
+// search event (kMaxEvents rows of kMaxN), then the parked context (vec with vstride kMaxN, lanes, uni).
+constexpr int kSnapEntries = kMaxEvents * kMaxN + 3 * kMaxN + 2 * (kCtxLaneWords * 16 + kCtxUniWords);
+
+// Orders a warp's stores to a record before its lanes read each other's entries.  (The host emulation
+// switches lanes only at collectives, in lane order, and every entry is read by its writer or a higher lane.)
+#ifdef __CUDACC__
+__device__ __forceinline__ void ctx_sync() { __syncwarp(); }
+#else
+inline void ctx_sync() {}
+#endif
 
 __device__ __forceinline__ void ctx_put_d(int32_t* lanes, int w, int lane, double v) {
   lanes[w * 16 + lane] = __double2loint(v);
@@ -668,7 +677,7 @@ __device__ __forceinline__ void band_setup(int lane, BandCtx& B, const int32_t* 
   }
 }
 
-// Phase B: the searches of all events.  `snap`: kSnapEntries int16 private to the band.
+// Phase B: the searches of all events.  `snap`: kMaxEvents rows of snap_stride int16, private to the band.
 template <int kMode>
 __device__ __forceinline__ void band_search(int lane, BandCtx& B, int n, int16_t* snap, int snap_stride,
                                             const double* rsq, const int32_t* pre_ev = nullptr,
@@ -717,8 +726,13 @@ __device__ __forceinline__ void band_search(int lane, BandCtx& B, int n, int16_t
       // (the first no-reference candidate of the list restarts the pulse reuse: prev_k = 0)
       phase = want;
       prev_k = 0;
-      if (big) search_init<4>(lane, sv, noref_ev ? x16 : xr, noref_ev ? n : n - 1);
-      else search_init<1>(lane, sv, noref_ev ? x16 : xr, noref_ev ? n : n - 1);
+      // element-wise: a reference to one of the two arrays, chosen at run time, would put both (and the
+      // context around them) in local memory
+      int src[4];
+#pragma unroll
+      for (int e = 0; e < 4; e++) src[e] = noref_ev ? x16[e] : xr[e];
+      if (big) search_init<4>(lane, sv, src, noref_ev ? n : n - 1);
+      else search_init<1>(lane, sv, src, noref_ev ? n : n - 1);
     }
     double xy = 0, yy = 0;
     const bool zero_ev = !noref_ev && kcur == 0;
@@ -979,6 +993,9 @@ __device__ __forceinline__ void band_noref_export(int lane, const BandCtx& B, in
 
 // One band by one warp, the three phases back to back.  `snap`: kSnapEntries int16 of scratch private to
 // the warp (shared memory); `rsq`: kTableDoubles doubles filled by pvq_fill_rsqrt_table.
+// The context is parked in the scratch between the phases, so that only what the search reads is live
+// across it: held in registers throughout, the whole context does not fit the 64 registers a thread of the
+// persistent kernel has and would spill to local memory.
 template <int kMode = 0>
 __device__ __forceinline__ int quantise_band_warp(int lane, int16_t* snap, const double* rsq, int32_t* out, const int32_t* x0,
                                                   const int32_t* r0, int n, int q0, int32_t* yout, int* itheta,
@@ -986,9 +1003,25 @@ __device__ __forceinline__ int quantise_band_warp(int lane, int16_t* snap, const
                                                   int pli, const int16_t* qm, const int16_t* qm_inv,
                                                   double pvq_norm_lambda, const int32_t* pre_ev = nullptr,
                                                   const int16_t* pre_snap = nullptr) {
+  int16_t* vec = snap + kMaxEvents * kMaxN;
+  int32_t* lanes = reinterpret_cast<int32_t*>(vec + 3 * kMaxN);
+  int32_t* uni = lanes + kCtxLaneWords * 16;
+  {
+    BandCtx B;
+    band_setup<kMode>(lane, B, x0, r0, n, q0, beta, is_keyframe, pli, qm, pvq_norm_lambda, rsq);
+    ctx_sync();   // the previous band's reads of the record come first
+    band_ctx_store_setup(lane, B, n, vec, kMaxN, lanes, uni);
+  }
+  ctx_sync();
+  {
+    BandCtx B;
+    band_ctx_load_search(lane, B, n, vec, kMaxN, lanes);
+    band_search<kMode>(lane, B, n, snap, kMaxN, rsq, pre_ev, pre_snap);
+    band_ctx_store_search(lane, B, lanes);
+  }
+  ctx_sync();
   BandCtx B;
-  band_setup<kMode>(lane, B, x0, r0, n, q0, beta, is_keyframe, pli, qm, pvq_norm_lambda, rsq);
-  band_search<kMode>(lane, B, n, snap, kMaxN, rsq, pre_ev, pre_snap);
+  band_ctx_load_finish(lane, B, n, vec, kMaxN, lanes, uni);
   return band_finish<kMode>(lane, B, snap, kMaxN, out, r0, n, q0, yout, itheta, max_theta, vk, beta, skip_term, is_keyframe, pli,
                      qm_inv, pvq_norm_lambda);
 }
