@@ -573,6 +573,7 @@ __device__ __forceinline__ uint32_t next_item(const Stage& S, int lane, int* don
     if (fin >= 0) {
       // every warp holds at most one ticket: slots [fin, fin + #warps] cover all of them, now and later
       const int nw = (gridDim.x * blockDim.x) >> 5;
+#pragma unroll 1
       for (int i = lane; i <= nw; i += 32) st_release((int*)&S.ring[fin + i], (int)kExit);
     }
     head = __shfl_sync(0xffffffffu, head, 0);

@@ -187,33 +187,28 @@ __device__ __forceinline__ void search_init(int lane, SearchVec& v, const int (&
   v.nn = nn;
 }
 
-// pvq_search_rdo_double (src/pvq_encoder.c:93) on magnitudes: ya = pulses so far (prev_k of them) in,
-// k pulses out; *xy_out, *yy_out = the reference's running sums at the end.
-template <int E>
-__device__ __forceinline__ void search_event(int lane, const SearchVec& v, int (&ya)[4], int k, int prev_k,
-                                             double lambda, const double* rsq, double* xy_out, double* yy_out) {
+// The start of pvq_search_rdo_double (src/pvq_encoder.c:93) on magnitudes: the pulses reused from the
+// previous search (prev_k of them) or the projection onto the pyramid; *xy, *yy = the running sums, returns
+// the number of pulses placed.  One copy for both size classes (`big`: 4 slots), outside the per-pulse loop.
+__device__ __forceinline__ int search_start(int lane, const SearchVec& v, int (&ya)[4], int k, int prev_k, bool big,
+                                            double* xy, double* yy) {
   const int nn = v.nn;
-  double xy = 0, yy = 0;
-  int i = 0;
+  long long sxy = 0, syy = 0;
+  int si = 0;
   if (prev_k > 0 && prev_k <= k) {
-    long long sxy = 0, syy = 0;
-    int si = 0;
 #pragma unroll
-    for (int e = 0; e < E; e++) {
+    for (int e = 0; e < 4; e++) {
+      if (e && !big) break;
       if (e * 32 + lane >= nn) ya[e] = 0;
       sxy += (long long)v.xa[e] * ya[e];
       syy += (long long)ya[e] * ya[e];
       si += ya[e];
     }
-    xy = (double)wsum64(sxy);
-    yy = (double)wsum64(syy);
-    i = wsum(si);
   } else if (k > 2) {
     const double l1_inv = nl_div(1., v.l1_norm > 1e-100 ? v.l1_norm : 1e-100);
-    long long sxy = 0, syy = 0;
-    int si = 0;
 #pragma unroll
-    for (int e = 0; e < E; e++) {
+    for (int e = 0; e < 4; e++) {
+      if (e && !big) break;
       const double tmp = k * (double)v.xa[e] * l1_inv;
       const int f = (int)floor(tmp);
       ya[e] = (e * 32 + lane < nn && f > 0) ? f : 0;
@@ -221,13 +216,25 @@ __device__ __forceinline__ void search_event(int lane, const SearchVec& v, int (
       syy += (long long)ya[e] * ya[e];
       si += ya[e];
     }
-    xy = (double)wsum64(sxy);
-    yy = (double)wsum64(syy);
-    i = wsum(si);
   } else {
 #pragma unroll
-    for (int e = 0; e < E; e++) ya[e] = 0;
+    for (int e = 0; e < 4; e++) ya[e] = 0;
+    *xy = 0;
+    *yy = 0;
+    return 0;
   }
+  *xy = (double)wsum64(sxy);
+  *yy = (double)wsum64(syy);
+  return wsum(si);
+}
+
+// The per-pulse loop of pvq_search_rdo_double, specialised by the slots per lane: from i pulses (ya, xy, yy
+// as search_start left them) to k; *xy_out, *yy_out = the reference's running sums at the end.
+template <int E>
+__device__ __forceinline__ void search_event(int lane, const SearchVec& v, int (&ya)[4], int k, int i, double xy,
+                                             double yy, double lambda, const double* rsq, double* xy_out,
+                                             double* yy_out) {
+  const int nn = v.nn;
   const int rdo_pulses = 1 + k / 4;
   double delta_rate = v.delta_rate;
   double accel_rate = 0.;
@@ -309,26 +316,37 @@ __device__ __forceinline__ void search_event(int lane, const SearchVec& v, int (
       const unsigned who = __ballot_sync(kFull, mine >= 0);
       pos = __shfl_sync(kFull, mine, __ffs(who) - 1);
     } else {
-      // the reference's sequential scan restricted to the contenders, in index order
+      // the reference's sequential scan restricted to the contenders, in index order: one loop body for
+      // all slots
       pos = -1;
       double ba = 0, bb = 1;
+      unsigned mk[E];
 #pragma unroll
-      for (int e = 0; e < E; e++) {
-        unsigned mk = __ballot_sync(kFull, cont[e]);
-        while (mk) {
-          const int l = __ffs(mk) - 1;
-          mk &= mk - 1;
-          if (plain) {
-            const int xj = __shfl_sync(kFull, v.xa[e], l);
-            const int yj = __shfl_sync(kFull, ya[e], l);
-            double a = xy + (double)xj;
-            const double b = yy + 2 * yj + 1;
-            a *= a;
-            if (pos < 0 || a * bb > ba * b) { ba = a; bb = b; pos = e * 32 + l; }
-          } else {
-            const double t = wfetch(tval[e], l);
-            if (pos < 0 || t > ba) { ba = t; pos = e * 32 + l; }
-          }
+      for (int e = 0; e < E; e++) mk[e] = __ballot_sync(kFull, cont[e]);
+      int e = 0;
+      unsigned m = mk[0];
+      for (;;) {
+        while (!m && ++e < E) {
+#pragma unroll
+          for (int t = 1; t < E; t++) if (e == t) m = mk[t];
+        }
+        if (!m) break;
+        const int l = __ffs(m) - 1;
+        m &= m - 1;
+        int sxa = v.xa[0], sya = ya[0];
+        double stv = tval[0];
+#pragma unroll
+        for (int t = 1; t < E; t++) if (e == t) { sxa = v.xa[t]; sya = ya[t]; stv = tval[t]; }
+        if (plain) {
+          const int xj = __shfl_sync(kFull, sxa, l);
+          const int yj = __shfl_sync(kFull, sya, l);
+          double a = xy + (double)xj;
+          const double b = yy + 2 * yj + 1;
+          a *= a;
+          if (pos < 0 || a * bb > ba * b) { ba = a; bb = b; pos = e * 32 + l; }
+        } else {
+          const double t = wfetch(stv, l);
+          if (pos < 0 || t > ba) { ba = t; pos = e * 32 + l; }
         }
       }
     }
@@ -741,8 +759,9 @@ __device__ __forceinline__ void band_search(int lane, BandCtx& B, int n, int16_t
       for (int e = 0; e < 4; e++) ya[e] = 0;
     } else {
       const double lambda = wfetch(c_lambda, leader);
-      if (big) search_event<4>(lane, sv, ya, kcur, prev_k, lambda, rsq, &xy, &yy);
-      else search_event<1>(lane, sv, ya, kcur, prev_k, lambda, rsq, &xy, &yy);
+      const int i = search_start(lane, sv, ya, kcur, prev_k, big, &xy, &yy);
+      if (big) search_event<4>(lane, sv, ya, kcur, i, xy, yy, lambda, rsq, &xy, &yy);
+      else search_event<1>(lane, sv, ya, kcur, i, xy, yy, lambda, rsq, &xy, &yy);
     }
     prev_k = kcur;
     int sj = 0;
