@@ -16,6 +16,12 @@
 //     -> iDCT + lapped postfilters -> u8 reconstruction, packed symbols for the host entropy coder
 //     -> (config.symbol_stream) the same symbols per frame in bitstream order with 8/16-bit pulses.
 //
+// config.inter: the residual of a batch of P frames the same way.  The motion-compensated prediction planes are
+// a second input; they take the same forward transform (no DC Haar pyramid on either side) and their
+// coefficients `md` are the reference vector of every band (pvq_theta with is_keyframe = 0).  Without an intra
+// predictor every (block, band) of every plane is dependency-free: luma and chroma both go through the three
+// phase kernels (k_pvq_split) and the persistent chain kernel is not launched.
+//
 // Nothing returns to the host between the H2D of the inputs and the D2H of the results; list sizes
 // live in device memory (`cnt`), every kernel is launched with a fixed grid and loops / pulls tickets
 // up to the device-side counts, so the step is captured once into a CUDA graph.
@@ -43,7 +49,7 @@ using namespace daala_b200::pvq;
 // ---- device-side counters ----------------------------------------------------------------------
 enum Cnt {
   kNLuma = 0, kNChroma, kLumaCoefs, kChromaCoefs,
-  kNItemsL = 4,      // [3] luma dependency-free items per class (bands 3 / 6: classes 1 / 2)
+  kNItemsL = 4,      // [3] luma dependency-free items per class (bands 3 / 6: classes 1 / 2; inter: every band)
   kNItemsC = 7,      // [3] chroma items per class (n <= 16, 32, 128)
   kTotalHi = 14,     // luma chain items in total
   kNHeads = 15,      // row / column chain items ready from the start (no same-size neighbour to wait for)
@@ -372,6 +378,21 @@ __global__ void __launch_bounds__(256) k_chroma_items(const __grid_constant__ Li
   }
 }
 
+// Inter frames: no intra predictor, so every luma (block, band) is a dependency-free item as well; item
+// encoding and classes of k_chroma_items, in place of k_luma_deps.
+__global__ void __launch_bounds__(256) k_luma_items(const __grid_constant__ Lists L) {
+  const int n = min(L.cnt[kNLuma], L.max_luma);
+  const int nth = gridDim.x * blockDim.x;
+  for (int base = blockIdx.x * blockDim.x; base < n; base += nth) {   // whole warps: append() is warp-aggregated
+    const int blk = base + threadIdx.x;
+    const int nb = blk < n ? num_bands(L.luma[blk].bs) : 0;
+    for (int band = 0; band < 9; band++) {
+      const int c = band_class(band);
+      append(L.items_l[c], &L.cnt[kNItemsL + c], band < nb, ((uint32_t)blk << 4) | band);
+    }
+  }
+}
+
 // ---- PVQ stage -----------------------------------------------------------------------------------
 struct Stage {
   daala_b200_pvq_params prm;
@@ -415,9 +436,11 @@ struct Stage {
   int cfl_stride;
 };
 
-// raster -> coding order of every block (od_raster_to_coding_order, src/partition.c:123); chroma:
-// also the CfL prediction and its sign flip (src/pvq_encoder.c:847-871).  One warp per block.
-template <bool kChroma>
+// raster -> coding order of every block (od_raster_to_coding_order, src/partition.c:123); keyframe chroma:
+// also the CfL prediction and its sign flip (src/pvq_encoder.c:847-871); inter frames, all planes alike: the
+// reference vector is the transformed prediction md (prm.pred_plane), never flipped.  One warp per block.
+enum { kGatherLuma = 0, kGatherChroma = 1, kGatherInter = 2 };
+template <int kKind>
 __global__ void __launch_bounds__(256) k_gather(const __grid_constant__ Stage S) {
   const daala_b200_pvq_params& prm = S.prm;
   const int n = min(S.cnt[S.n_blocks_at], S.max_blocks);
@@ -430,8 +453,16 @@ __global__ void __launch_bounds__(256) k_gather(const __grid_constant__ Stage S)
     const int stride = prm.plane_stride[b.pli];
     const int32_t* src = prm.coef_plane[b.pli] + b.frame * prm.plane_frame_pitch[b.pli] + (size_t)b.y0 * stride + b.x0;
     int32_t* vin = prm.in + b.coef_off;
-    if (!kChroma) {
+    if (kKind == kGatherLuma) {
       for (int i = lane; i < len; i += 32) vin[i] = i == 0 ? src[0] : src[scan_to_raster(i, ln, stride)];
+    } else if (kKind == kGatherInter) {
+      const int32_t* psrc = prm.pred_plane[b.pli] + b.frame * prm.plane_frame_pitch[b.pli] + (size_t)b.y0 * stride + b.x0;
+      int32_t* vref = prm.ref + b.coef_off;
+      for (int i = lane; i < len; i += 32) {
+        const int at = i == 0 ? 0 : scan_to_raster(i, ln, stride);
+        vin[i] = src[at];
+        vref[i] = psrc[at];
+      }
     } else {
       const int32_t* psrc = S.cfl_plane + b.frame * S.cfl_pitch + (size_t)b.y0 * S.cfl_stride + b.x0;
       int32_t* vref = prm.ref + b.coef_off;
@@ -918,6 +949,10 @@ __global__ void k_begin_pvq(int32_t* cnt, int luma) {
 // (scalar_out[0] = dblock[0], src/encode.c:1381), od_init_skipped_coeffs (src/state.c:1347) +
 // od_coding_order_to_raster (src/partition.c:157) back into the coefficient plane, pulses packed to
 // 16 bits for the host entropy coder.  One warp per block.
+// kInter: DC is the scalar quantisation of in[0] - ref[0] with the band-0 quantiser (od_block_encode's
+// non-keyframe branch; the index goes to prm.res_dc), and the uncoded tail of 32x32 / 64x64 blocks is the
+// transformed prediction (od_init_skipped_coeffs for inter frames).
+template <bool kInter>
 __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ Stage S) {
   const daala_b200_pvq_params& prm = S.prm;
   const int n = min(S.cnt[S.n_blocks_at], S.max_blocks);
@@ -935,10 +970,28 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
       double sd = 0;
       for (int i = 0; i < nb; i++) sd += prm.res_skip_term[(size_t)blk * 9 + i];
       prm.res_skip_diff[blk] = sd;
-      prm.out[b.coef_off] = prm.in[b.coef_off];
+      if (!kInter) {
+        prm.out[b.coef_off] = prm.in[b.coef_off];
+      } else {
+        int dc_quant = (prm.q0 * prm.pvq_qm_q4[b.pli][b.bs * (b.bs + 1)]) >> 4;
+        if (dc_quant < 1) dc_quant = 1;
+        const int32_t r = prm.ref[b.coef_off], diff = prm.in[b.coef_off] - r;
+        int qdc = 0;
+        if (abs(diff) >= dc_quant * 141 / 256) {
+          const int half = ((dc_quant + 1) >> 1) - 1;
+          qdc = (diff + (diff < 0 ? -half : half)) / dc_quant;
+        }
+        prm.out[b.coef_off] = dst[0] = qdc * dc_quant + r;
+        prm.res_dc[blk] = qdc;
+      }
     }
     if (ln >= 5) {
-      for (int i = lane; i < nn * nn; i += 32) if (i) dst[(size_t)(i >> ln) * stride + (i & (nn - 1))] = 0;
+      const int32_t* mdp = kInter ? prm.pred_plane[b.pli] + b.frame * prm.plane_frame_pitch[b.pli] + (size_t)b.y0 * stride + b.x0
+                                  : nullptr;
+      for (int i = lane; i < nn * nn; i += 32) {
+        const size_t at = (size_t)(i >> ln) * stride + (i & (nn - 1));
+        if (i) dst[at] = kInter ? mdp[at] : 0;
+      }
       __syncwarp();
     }
     for (int i = lane + 1; i < len; i += 32) dst[scan_to_raster(i, ln, stride)] = src[i];
@@ -1298,6 +1351,8 @@ struct daala_b200_kf {
   int32_t* coeffs[3];
   int32_t* lapped[3];
   uint8_t* pixels_out[3];
+  uint8_t* pred_pixels[3];         // cfg.inter: the prediction planes and their transform md
+  int32_t* pred_coeffs[3];
   uint8_t* bsize;
   int32_t* cfl_plane;
   int16_t *qm, *qm_inv;
@@ -1328,6 +1383,7 @@ struct daala_b200_kf {
   Stage luma, chroma;
   Sym sym;                         // symbol stream (cfg.symbol_stream); zero otherwise
   daala_b200_frame frame;
+  daala_b200_frame frame_pred;     // cfg.inter: `frame` with the prediction planes as the forward transform's input / output
   size_t bytes_allocated;
   size_t chain_cap;                // entries of the chain queue (heads / ring)
   int sms;
@@ -1356,6 +1412,7 @@ static cudaError_t dalloc(daala_b200_kf* kf, T** p, size_t n) {
 
 static int kf_alloc(daala_b200_kf* kf) {
   const int F = kf->F;
+  const bool inter = kf->cfg.inter != 0;
   const long long luma_px = (long long)kf->plane_w[0] * kf->plane_h[0];
   for (int p = 0; p < 3; p++) {
     const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
@@ -1363,10 +1420,14 @@ static int kf_alloc(daala_b200_kf* kf) {
     KF_CHECK(dalloc(kf, &kf->coeffs[p], n));
     KF_CHECK(dalloc(kf, &kf->lapped[p], n));
     KF_CHECK(dalloc(kf, &kf->pixels_out[p], n));
+    if (inter) {
+      KF_CHECK(dalloc(kf, &kf->pred_pixels[p], n));
+      KF_CHECK(dalloc(kf, &kf->pred_coeffs[p], n));
+    }
   }
   const int UW = kf->nhsb * 8, UH = kf->nvsb * 8;
   KF_CHECK(dalloc(kf, &kf->bsize, (size_t)F * UW * UH));
-  KF_CHECK(dalloc(kf, &kf->cfl_plane, (size_t)kf->plane_w[1] * kf->plane_h[1] * F));
+  if (!inter) KF_CHECK(dalloc(kf, &kf->cfl_plane, (size_t)kf->plane_w[1] * kf->plane_h[1] * F));
   KF_CHECK(dalloc(kf, &kf->qm, (size_t)2 * kf->cfg.qm_stride));
   KF_CHECK(dalloc(kf, &kf->qm_inv, (size_t)2 * kf->cfg.qm_stride));
   KF_CHECK(dalloc(kf, &kf->rsqrt_tbl, (size_t)kTableDoubles));
@@ -1394,21 +1455,26 @@ static int kf_alloc(daala_b200_kf* kf) {
   KF_CHECK(dalloc(kf, &L.unit_lbase, (size_t)F * UW * UH));
   KF_CHECK(dalloc(kf, &L.luma, (size_t)L.max_luma));
   KF_CHECK(dalloc(kf, &L.chroma, (size_t)L.max_chroma));
-  KF_CHECK(dalloc(kf, &L.dep_top, (size_t)L.max_luma));
-  KF_CHECK(dalloc(kf, &L.dep_left, (size_t)L.max_luma));
-  KF_CHECK(dalloc(kf, &L.succ_bottom, (size_t)L.max_luma));
-  KF_CHECK(dalloc(kf, &L.succ_right, (size_t)L.max_luma));
+  // the intra dependency structure (neighbours, chain heads, ring) is a keyframe matter
+  const size_t ndep = inter ? 0 : (size_t)L.max_luma;
+  KF_CHECK(dalloc(kf, &L.dep_top, ndep));
+  KF_CHECK(dalloc(kf, &L.dep_left, ndep));
+  KF_CHECK(dalloc(kf, &L.succ_bottom, ndep));
+  KF_CHECK(dalloc(kf, &L.succ_right, ndep));
   // item capacities follow from the pixel count alone: one band per 4x4 block is the densest case
   const size_t luma_shard_px = (size_t)F * L.u_rows * UW * 64;
   kf->chain_cap = luma_shard_px / 16 + 64 + (size_t)kf->sms * 64;   // + one exit slot per persistent warp
-  const size_t cap_l[3] = {64, luma_shard_px / 64 + 64, luma_shard_px / 256 + 64};   // bands 3 / 6 only
+  // keyframes: bands 3 / 6 only.  inter: every band; class 0 (bands 0..2) is densest on an all-4x4 map (one item
+  // per block) or an all-8x8 one (three per block), classes 1 / 2 on all-8x8 / all-16x16 maps, one item per block
+  const size_t cap_l0 = (size_t)L.max_luma * 3 < luma_shard_px / 16 ? (size_t)L.max_luma * 3 : luma_shard_px / 16;
+  const size_t cap_l[3] = {inter ? cap_l0 + 64 : 64, luma_shard_px / 64 + 64, luma_shard_px / 256 + 64};
   const size_t cap_c[3] = {(size_t)L.max_chroma * 3 / 2 + 64, luma_shard_px / 4 * 2 * 3 / 64 + 64,
                            luma_shard_px / 4 * 2 * 3 / 256 + 64};
   for (int c = 0; c < 3; c++) {
     KF_CHECK(dalloc(kf, &L.items_l[c], cap_l[c]));
     KF_CHECK(dalloc(kf, &L.items_c[c], cap_c[c]));
   }
-  if (kf->cfg.split_free > 0) {
+  if (kf->cfg.split_free > 0 || inter) {
     // context records of one chunk of items per class (pvq_warp.cuh: band_ctx_*)
     const int slots[3] = {1 << 19, 1 << 19, 3 << 15};
     for (int c = 0; c < 3; c++) {
@@ -1454,8 +1520,8 @@ static int kf_alloc(daala_b200_kf* kf) {
       return (int)cudaErrorLaunchOutOfResources;
     }
   }
-  KF_CHECK(dalloc(kf, &L.heads, kf->chain_cap));
-  KF_CHECK(dalloc(kf, &L.heads0, (size_t)L.max_luma));
+  KF_CHECK(dalloc(kf, &L.heads, inter ? 0 : kf->chain_cap));
+  KF_CHECK(dalloc(kf, &L.heads0, ndep));
   KF_CHECK(dalloc(kf, &L.cnt, (size_t)kCntWords));
 
   auto setup_stage = [&](Stage& S, bool chroma) -> int {
@@ -1475,17 +1541,18 @@ static int kf_alloc(daala_b200_kf* kf) {
     KF_CHECK(dalloc(kf, &S.res_pack, nblk * 9 * 4));
     p.res_gain = p.res_theta = p.res_max_theta = p.res_k = nullptr;   // packed into res_pack here
     p.res_dc = nullptr;
+    if (inter) KF_CHECK(dalloc(kf, &p.res_dc, nblk));
     p.qm = kf->qm;
     p.qm_inv = kf->qm_inv;
     for (int i = 0; i < 3; i++) {
       p.coef_plane[i] = kf->coeffs[i];
-      p.pred_plane[i] = nullptr;
+      p.pred_plane[i] = kf->pred_coeffs[i];
       p.plane_frame_pitch[i] = (long long)kf->plane_w[i] * kf->plane_h[i];
       p.plane_stride[i] = kf->plane_w[i];
     }
     p.qm_stride = kf->cfg.qm_stride;
     p.q0 = kf->cfg.q0 > 1 ? kf->cfg.q0 : 1;
-    p.is_keyframe = 1;
+    p.is_keyframe = inter ? 0 : 1;
     p.use_masking = kf->cfg.use_masking;
     p.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
     memcpy(p.pvq_qm_q4, kf->cfg.pvq_qm_q4, sizeof(p.pvq_qm_q4));
@@ -1529,8 +1596,8 @@ static int kf_alloc(daala_b200_kf* kf) {
       S.succ_right = L.succ_right;
       S.heads = L.heads;
       S.heads0 = L.heads0;
-      KF_CHECK(dalloc(kf, &S.ring, kf->chain_cap));
-      KF_CHECK(dalloc(kf, &S.join0, nblk));
+      KF_CHECK(dalloc(kf, &S.ring, inter ? 0 : kf->chain_cap));
+      KF_CHECK(dalloc(kf, &S.join0, ndep));
     } else {
       S.cfl_plane = kf->cfl_plane;
       S.cfl_pitch = (long long)kf->plane_w[1] * kf->plane_h[1];
@@ -1604,10 +1671,15 @@ static int kf_alloc(daala_b200_kf* kf) {
   f.nvsb = kf->nvsb;
   f.pic_w = kf->cfg.pic_w;
   f.pic_h = kf->cfg.pic_h;
-  f.haar_dc = 1;
+  f.haar_dc = inter ? 0 : 1;
   f.nframes = F;
   f.sb_row0 = kf->cfg.sb_row0;
   f.sb_rows = kf->cfg.sb_rows;
+  kf->frame_pred = f;
+  for (int p = 0; p < 3; p++) {
+    kf->frame_pred.plane[p].pixels = kf->pred_pixels[p];
+    kf->frame_pred.plane[p].coeffs = kf->pred_coeffs[p];
+  }
   if (kf->cfg.dering) {
     const size_t nsb = (size_t)F * kf->nhsb * kf->nvsb;
     KF_CHECK(dalloc(kf, &kf->dering_level, nsb));
@@ -1660,7 +1732,41 @@ static void enqueue_split(daala_b200_kf* kf, const Stage& S, cudaStream_t s) {
   }
 }
 
+// config.inter: the same step for P-frame residuals.  Both plane sets through the forward transform (two
+// launches: the kernel's tensor maps describe one pixel allocation each), every band of both stages through
+// the phase kernels with the transformed prediction as reference.
+static int kf_enqueue_step_inter(daala_b200_kf* kf, int phases) {
+  cudaStream_t s = kf->stream;
+  const Lists& L = kf->lists;
+  const int wide = kf->sms * 8;
+  if (phases & DAALA_B200_KF_LISTS) {
+    k_unit_tile_sums<<<L.ntiles, kTile, 0, s>>>(L);
+    k_tile_scan<<<1, 1024, 0, s>>>(L);
+    k_unit_emit<<<L.ntiles, kTile, 0, s>>>(L);
+    k_luma_items<<<wide, 256, 0, s>>>(L);
+    k_chroma_items<<<wide, 256, 0, s>>>(L);
+  }
+  if (phases & DAALA_B200_KF_FORWARD) {
+    int rc = daala_b200_launch_forward(&kf->frame, 3, s);
+    if (!rc) rc = daala_b200_launch_forward(&kf->frame_pred, 3, s);
+    if (rc) return rc;
+  }
+  const bool core = (phases & DAALA_B200_KF_SEARCH_ONLY) != 0;
+  for (const Stage* S : {&kf->luma, &kf->chroma}) {
+    if (!(phases & (S == &kf->luma ? DAALA_B200_KF_PVQ_LUMA : DAALA_B200_KF_PVQ_CHROMA))) continue;
+    if (!core) k_gather<kGatherInter><<<wide, 256, 0, s>>>(*S);
+    enqueue_split<false>(kf, *S, s);
+    if (!core) k_finish_scatter<true><<<wide, 256, 0, s>>>(*S);
+  }
+  if (phases & DAALA_B200_KF_INVERSE) {
+    int rc = daala_b200_launch_inverse(&kf->frame, 3, s);
+    if (rc) return rc;
+  }
+  return (int)cudaGetLastError();
+}
+
 static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
+  if (kf->cfg.inter) return kf_enqueue_step_inter(kf, phases);
   cudaStream_t s = kf->stream;
   const Lists& L = kf->lists;
   const int wide = kf->sms * 8;
@@ -1692,7 +1798,7 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
         cudaMemsetAsync(kf->luma.join0, 0, (size_t)kf->luma.max_blocks * sizeof(int32_t), s) != cudaSuccess)
       return (int)cudaGetLastError();
     k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, 1);
-    if (!core) k_gather<false><<<wide, 256, 0, s>>>(kf->luma);
+    if (!core) k_gather<kGatherLuma><<<wide, 256, 0, s>>>(kf->luma);
     if (kf->cfg.split_free > 1) enqueue_split<true>(kf, kf->luma, s);
     if (kf->luma.pre_ev) {
       k_pvq_prepass<2><<<kf->sms * 16, 128, 0, s>>>(kf->luma);
@@ -1704,15 +1810,15 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
     } else {
       k_pvq_persist<true><<<persist, kPersistThreads, 0, s>>>(kf->luma);
     }
-    if (!core) k_finish_scatter<<<wide, 256, 0, s>>>(kf->luma);
+    if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->luma);
   }
   if (phases & DAALA_B200_KF_PVQ_CHROMA) {
     k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, 0);
     if (!core) k_cfl_plane<<<wide, 256, 0, s>>>(kf->chroma, kf->cfl_plane);
-    if (!core) k_gather<true><<<wide, 256, 0, s>>>(kf->chroma);
+    if (!core) k_gather<kGatherChroma><<<wide, 256, 0, s>>>(kf->chroma);
     if (kf->cfg.split_free > 0) enqueue_split<false>(kf, kf->chroma, s);
     else k_pvq_persist<false><<<persist, kPersistThreads, 0, s>>>(kf->chroma);
-    if (!core) k_finish_scatter<<<wide, 256, 0, s>>>(kf->chroma);
+    if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->chroma);
     if (!core && kf->cfg.symbol_stream) {
       const Sym& Y = kf->sym;
       k_sym_rank<<<(Y.F * Y.nsb + 7) / 8, 256, 0, s>>>(Y);
@@ -1802,7 +1908,25 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
 
 extern "C" {
 
+// why the last daala_b200_kf_create of this thread returned NULL (daala_b200_kf_error(NULL))
+static thread_local char g_create_err[256] = "null engine";
+
 daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
+  snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: invalid configuration");
+  if (cfg && cfg->inter) {
+    // P-frame residual mode is defined for whole frames through the phase kernels, without the stages whose
+    // inter form this engine does not have
+    const char* with = cfg->inter != 1 ? "a value other than 0 or 1"
+                       : cfg->dering ? "dering (the all-zero skip map of the deringing stage is a keyframe property)"
+                       : cfg->symbol_stream ? "symbol_stream (its block record has no DC field)"
+                       : cfg->noref_prepass ? "noref_prepass"
+                       : cfg->level_chains ? "level_chains"
+                       : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
+    if (with) {
+      snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: inter is not defined with %s", with);
+      return nullptr;
+    }
+  }
   if (!cfg || cfg->pic_w <= 0 || cfg->pic_h <= 0 || cfg->nframes <= 0 || cfg->nframes > 255 || !cfg->qm ||
       !cfg->qm_inv || cfg->qm_stride <= 0)
     return nullptr;
@@ -1844,6 +1968,7 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   }
   if (kf_alloc(kf) != 0) {
     fprintf(stderr, "daala_b200_kf_create: %s\n", kf->err);
+    snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: %s", kf->err);
     // leak-free teardown is the destroy function's job
     daala_b200_kf_destroy(kf);
     return nullptr;
@@ -1861,6 +1986,8 @@ void daala_b200_kf_destroy(daala_b200_kf* kf) {
     cudaFree(kf->coeffs[p]);
     cudaFree(kf->lapped[p]);
     cudaFree(kf->pixels_out[p]);
+    cudaFree(kf->pred_pixels[p]);
+    cudaFree(kf->pred_coeffs[p]);
   }
   cudaFree(kf->bsize);
   cudaFree(kf->cfl_plane);
@@ -1928,6 +2055,7 @@ void daala_b200_kf_destroy(daala_b200_kf* kf) {
     cudaFree(S->prm.res_skip_term);
     cudaFree(S->prm.res_skip_diff);
     cudaFree(S->prm.res_flip);
+    cudaFree(S->prm.res_dc);
     cudaFree(S->res_pack);
     cudaFree(S->ring);
     cudaFree(S->join0);
@@ -1938,12 +2066,14 @@ void daala_b200_kf_destroy(daala_b200_kf* kf) {
   free(kf);
 }
 
-const char* daala_b200_kf_error(const daala_b200_kf* kf) { return kf ? kf->err : "null engine"; }
+const char* daala_b200_kf_error(const daala_b200_kf* kf) { return kf ? kf->err : g_create_err; }
 
 // Kernel launches of one whole step (kf_enqueue_step with DAALA_B200_KF_ALL), memset nodes not counted.
 int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   if (!kf) return 0;
   auto split = [](const Stage& S) { return 3 * (S.sp_chunks[0] + S.sp_chunks[1] + S.sp_chunks[2]); };
+  // inter: work lists, two forward launches, per stage gather + phase kernels + finish, inverse + SB postfilter
+  if (kf->cfg.inter) return 5 + 2 + (2 + split(kf->luma)) + (2 + split(kf->chroma)) + 2;
   int n = 5 + (kf->cfg.level_chains ? 2 : 0);                                    // work lists
   n += 1;                                                                         // forward
   n += 3 + 1 + (kf->cfg.split_free > 1 ? split(kf->luma) : 0) + (kf->luma.pre_ev ? 2 : 0);   // luma: begin, gather, [prepass], chains, finish
@@ -1991,6 +2121,10 @@ int daala_b200_kf_device_buffers(daala_b200_kf* kf, daala_b200_kf_buffers* out) 
   out->max_chroma_blocks = kf->lists.max_chroma;
   out->stream = kf->stream;
   out->bytes_allocated = (long long)kf->bytes_allocated;
+  for (int p = 0; p < 3; p++) {
+    out->pred_pixels[p] = kf->pred_pixels[p];
+    out->pred_coeffs[p] = kf->pred_coeffs[p];
+  }
   return 0;
 }
 
@@ -2115,6 +2249,10 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   else daala_b200_kf_count_blocks(io->bsize, F, (long long)kf->nhsb * 8 * kf->nvsb * 8, kf->nhsb * 8, kf->nhsb, kf->nvsb,
                                   kf->cfg.sb_row0, kf->cfg.sb_rows, &tot);
   if (tot.n_luma > kf->lists.max_luma || tot.n_chroma > kf->lists.max_chroma) return (int)cudaErrorInvalidValue;
+  if (kf->cfg.inter && (!io->pred_pixels[0] || !io->pred_pixels[1] || !io->pred_pixels[2] || !io->luma_dc || !io->chroma_dc)) {
+    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: an inter engine needs pred_pixels[0..2], luma_dc and chroma_dc");
+    return (int)cudaErrorInvalidValue;
+  }
   // symbol stream: the engine must produce it, and every requested buffer must hold the worst case and be pinned
   SymCopy sc;
   memset(&sc, 0, sizeof(sc));
@@ -2149,6 +2287,9 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     if (!io->pixels[p]) return (int)cudaErrorInvalidValue;
     KF_CHECK(cudaMemcpyAsync(kf->pixels[p], io->pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
                              cudaMemcpyHostToDevice, s));
+    if (kf->cfg.inter)
+      KF_CHECK(cudaMemcpyAsync(kf->pred_pixels[p], io->pred_pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
+                               cudaMemcpyHostToDevice, s));
   }
   const size_t map_bytes = (size_t)kf->nhsb * 8 * kf->nvsb * 8 * F;
   KF_CHECK(cudaMemcpyAsync(kf->bsize, io->bsize, map_bytes, cudaMemcpyHostToDevice, s));
@@ -2178,6 +2319,10 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   if (io->luma_skip_diff) KF_CHECK(cudaMemcpyAsync(io->luma_skip_diff, kf->luma.prm.res_skip_diff, 8 * (size_t)tot.n_luma, cudaMemcpyDeviceToHost, s));
   if (io->chroma_skip_diff) KF_CHECK(cudaMemcpyAsync(io->chroma_skip_diff, kf->chroma.prm.res_skip_diff, 8 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));
   if (io->chroma_flip) KF_CHECK(cudaMemcpyAsync(io->chroma_flip, kf->chroma.prm.res_flip, 4 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));
+  if (kf->cfg.inter) {
+    KF_CHECK(cudaMemcpyAsync(io->luma_dc, kf->luma.prm.res_dc, 4 * (size_t)tot.n_luma, cudaMemcpyDeviceToHost, s));
+    KF_CHECK(cudaMemcpyAsync(io->chroma_dc, kf->chroma.prm.res_dc, 4 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));
+  }
   if (io->counts) KF_CHECK(cudaMemcpyAsync(io->counts, kf->lists.cnt, sizeof(int32_t) * 32, cudaMemcpyDeviceToHost, s));
   if (io->dering_level_out && kf->cfg.dering)
     KF_CHECK(cudaMemcpyAsync(io->dering_level_out, kf->dering_level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyDeviceToHost, s));

@@ -1,7 +1,9 @@
 """Host side of the keyframe engine (include/daala_b200.h, "Keyframe engine"; csrc/kf_engine.cu):
 ctypes binding + numpy marshalling.  The engine is the batched equivalent of od_encode_coefficients
 (reference src/encode.c:2539) for keyframes without the entropy coder: u8 planes + block-size maps in,
-reconstruction + PVQ symbols out, everything in between on the GPU (work lists included).
+reconstruction + PVQ symbols out, everything in between on the GPU (work lists included).  Created with
+inter=1 the same engine codes P-frame residuals: the motion-compensated prediction planes are a second input
+(`pred=`), and each block's scalar-quantised DC index is a further output.
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -25,7 +27,7 @@ class Config(ctypes.Structure):
                 ("qm", c_void_p), ("qm_inv", c_void_p), ("sb_row0", c_int), ("sb_rows", c_int),
                 ("max_blocks_div", c_int), ("persist_ctas_per_sm", c_int), ("split_free", c_int), ("dering", c_int), ("noref_prepass", c_int), ("level_chains", c_int), ("stream", c_void_p),
                 ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
-                ("symbol_stream", c_int)]
+                ("symbol_stream", c_int), ("inter", c_int)]
 
 
 class Totals(ctypes.Structure):
@@ -39,7 +41,8 @@ class IO(ctypes.Structure):
                 ("luma_skip_diff", c_void_p), ("chroma_skip_diff", c_void_p), ("chroma_flip", c_void_p),
                 ("counts", c_void_p), ("dering_level_out", c_void_p),
                 ("sym_index", c_void_p), ("sym_index_cap", c_ll), ("sym_blocks", c_void_p), ("sym_blocks_cap", c_ll),
-                ("sym_bands", c_void_p), ("sym_bands_cap", c_ll), ("sym_pulses", c_void_p), ("sym_pulses_cap", c_ll)]
+                ("sym_bands", c_void_p), ("sym_bands_cap", c_ll), ("sym_pulses", c_void_p), ("sym_pulses_cap", c_ll),
+                ("pred_pixels", c_void_p * 3), ("luma_dc", c_void_p), ("chroma_dc", c_void_p)]
 
 
 class SymBounds(ctypes.Structure):
@@ -55,7 +58,7 @@ class Buffers(ctypes.Structure):
                 ("luma_res", c_void_p), ("chroma_res", c_void_p), ("luma_y16", c_void_p), ("chroma_y16", c_void_p),
                 ("luma_skip_diff", c_void_p), ("chroma_skip_diff", c_void_p), ("chroma_flip", c_void_p),
                 ("max_luma_blocks", c_int), ("max_chroma_blocks", c_int), ("stream", c_void_p),
-                ("bytes_allocated", c_ll)]
+                ("bytes_allocated", c_ll), ("pred_pixels", c_void_p * 3), ("pred_coeffs", c_void_p * 3)]
 
 
 def _bind():
@@ -111,7 +114,7 @@ class KeyframeEngine:
 
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
                  qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=0, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
-                 qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0):
+                 qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0):
         self.L = _bind()
         self.geom, self.F = geom, nframes
         if qm is None:
@@ -142,9 +145,12 @@ class KeyframeEngine:
         self.dering = int(dering)
         cfg.symbol_stream = int(symbol_stream)
         self.symbol_stream = int(symbol_stream)
+        cfg.inter = int(inter)
+        self.inter = int(inter)
         self.kf = self.L.daala_b200_kf_create(ctypes.byref(cfg))
         if not self.kf:
-            raise RuntimeError("daala_b200_kf_create failed (no CUDA device, or out of memory)")
+            raise RuntimeError("daala_b200_kf_create failed (refused configuration, no CUDA device, or out of memory): %s"
+                               % self.L.daala_b200_kf_error(None).decode())
         self.buf = Buffers()
         self._check(self.L.daala_b200_kf_device_buffers(self.kf, ctypes.byref(self.buf)), "device_buffers")
         self.sb_row0 = sb_row0
@@ -213,13 +219,22 @@ class KeyframeEngine:
         a = self._arr("dlev", (self.F, g.nvsb, g.nhsb), np.uint8)
         a[...] = levels
 
-    def stage_inputs(self, planes, bsize):
+    def _check_pred(self, pred):
+        if bool(self.inter) != (pred is not None):
+            raise ValueError("pred= planes are required by an inter engine and refused by a keyframe engine")
+
+    def stage_inputs(self, planes, bsize, pred=None):
         """Copies one batch into the engine's (pinned) host input buffers.  planes: per plane an array
-        [F, h, w] u8 (padded geometry); bsize: [F, nvsb*8, nhsb*8]."""
+        [F, h, w] u8 (padded geometry); bsize: [F, nvsb*8, nhsb*8]; pred (inter engines): the
+        motion-compensated prediction planes, shaped like `planes`."""
         g = self.geom
+        self._check_pred(pred)
         for p in range(3):
             a = self._arr("in%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
             a[...] = planes[p]
+            if self.inter:
+                a = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
+                a[...] = pred[p]
         b = self._arr("bsize", (self.F,) + tuple(g.bsize_shape), np.uint8)
         b[...] = bsize
         self.totals = self.count_blocks(b)
@@ -264,6 +279,12 @@ class KeyframeEngine:
             for k in ("luma_blocks", "chroma_blocks", "luma_res", "chroma_res", "luma_y16", "chroma_y16",
                       "luma_skip_diff", "chroma_skip_diff", "chroma_flip"):
                 setattr(io, k, out[k].ctypes.data)
+        if self.inter:
+            for p in range(3):
+                io.pred_pixels[p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8).ctypes.data
+            out["luma_dc"] = self._arr("ld", (int(t.n_luma),), np.int32)
+            out["chroma_dc"] = self._arr("cd", (int(t.n_chroma),), np.int32)
+            io.luma_dc, io.chroma_dc = out["luma_dc"].ctypes.data, out["chroma_dc"].ctypes.data
         out["counts"] = self._arr("cnt", (32,), np.int32)
         io.counts = out["counts"].ctypes.data
         if self.dering:
@@ -282,7 +303,8 @@ class KeyframeEngine:
                 setattr(io, k, out[k].ctypes.data)
                 setattr(io, k + "_cap", int(cap))
         self._io, self._out = io, out
-        self.h2d_bytes = sum(int(np.prod(g.plane_shape(p))) for p in range(3)) * self.F + int(np.prod(g.bsize_shape)) * self.F
+        self.h2d_bytes = (sum(int(np.prod(g.plane_shape(p))) for p in range(3)) * self.F * (2 if self.inter else 1)
+                          + int(np.prod(g.bsize_shape)) * self.F)
         return out
 
     def submit(self):
@@ -299,10 +321,10 @@ class KeyframeEngine:
         idx = self._out["sym_index"]
         return idx.nbytes + int(idx[:, 1].sum()) * sym.BLOCK_DTYPE.itemsize + int(idx[:, 3].sum()) * 8 + int(idx[:, 5].sum())
 
-    def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None):
+    def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None, pred=None):
         """One batch end to end through the C ABI with host buffers; returns the result arrays (views of
-        the engine's host buffers: copy what must survive the next call)."""
-        self.stage_inputs(planes, bsize)
+        the engine's host buffers: copy what must survive the next call).  pred: see stage_inputs."""
+        self.stage_inputs(planes, bsize, pred)
         if self.dering == 1:
             self.stage_dering_levels(dering_levels)
         self.prepare_io(symbols, recon, stream)
@@ -323,12 +345,14 @@ class KeyframeEngine:
                     "kf_time_device")
         return float(ms.value)
 
-    def upload(self, planes, bsize):
+    def upload(self, planes, bsize, pred=None):
         g = self.geom
+        self._check_pred(pred)
         for p in range(3):
-            a = np.ascontiguousarray(planes[p], np.uint8)
-            assert a.shape == (self.F,) + g.plane_shape(p)
-            self._check(self.L.daala_b200_device_copy(self.buf.pixels[p], a.ctypes.data, a.nbytes, 0), "upload")
+            for dst, src in ((self.buf.pixels[p], planes[p]),) + (((self.buf.pred_pixels[p], pred[p]),) if self.inter else ()):
+                a = np.ascontiguousarray(src, np.uint8)
+                assert a.shape == (self.F,) + g.plane_shape(p)
+                self._check(self.L.daala_b200_device_copy(dst, a.ctypes.data, a.nbytes, 0), "upload")
         b = np.ascontiguousarray(bsize, np.uint8)
         assert b.shape == (self.F,) + tuple(g.bsize_shape)
         self._check(self.L.daala_b200_device_copy(self.buf.bsize, b.ctypes.data, b.nbytes, 0), "upload")
@@ -345,6 +369,10 @@ class KeyframeEngine:
 
     def coeff_plane(self, p):
         return self.download(self.buf.coeffs[p], (self.F,) + self.geom.plane_shape(p), np.int32)
+
+    def pred_coeff_plane(self, p):
+        """The transformed prediction md of plane p (inter engines)."""
+        return self.download(self.buf.pred_coeffs[p], (self.F,) + self.geom.plane_shape(p), np.int32)
 
     def recon_plane(self, p):
         return self.download(self.buf.pixels_out[p], (self.F,) + self.geom.plane_shape(p), np.uint8)

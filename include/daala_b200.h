@@ -469,6 +469,20 @@ typedef struct daala_b200_kf_config {
   int symbol_stream;           /* 1: every step also packs the PVQ symbols of each frame in bitstream order
                                   (daala_b200_kf_sym_block below) for daala_b200_kf_io.sym_*; 0 (default): the step
                                   is exactly the one without the stream */
+  int inter;                   /* 0 (default): keyframes, exactly the engine described above.
+                                  1: P-frame residual mode.  Every frame is coded as od_encode_coefficients codes a
+                                  non-key frame, entropy coding and the coder-state skip decision left to the host:
+                                  the motion-compensated prediction is an INPUT (daala_b200_kf_io.pred_pixels), it
+                                  goes through the same prefilters + fDCT as the source (no DC Haar pyramid on either)
+                                  and is the reference vector of every band of every plane (pvq_theta with
+                                  is_keyframe = 0: no H/V intra prediction, no CfL, no flip).  No band depends on
+                                  another block, so luma and chroma both run as the three phase kernels of
+                                  split_free and the persistent chain kernel is not launched.  DC is the scalar
+                                  quantisation of in[0] - ref[0] with the band-0 quantiser (index in
+                                  daala_b200_kf_io.luma_dc / chroma_dc); the uncoded tail of 32x32 / 64x64 blocks is
+                                  the transformed prediction (od_init_skipped_coeffs for inter frames).
+                                  Not defined, and refused by daala_b200_kf_create, together with dering,
+                                  symbol_stream, noref_prepass, level_chains or a row shard (sb_rows > 0) */
 } daala_b200_kf_config;
 
 typedef struct daala_b200_kf_totals {
@@ -540,6 +554,10 @@ typedef struct daala_b200_kf_io {
   long long sym_bands_cap;
   uint8_t *sym_pulses;
   long long sym_pulses_cap;
+  /* config.inter only (required there, ignored otherwise). */
+  const uint8_t *pred_pixels[3];        /* motion-compensated prediction planes, shapes and padding of `pixels` */
+  int32_t *luma_dc, *chroma_dc;         /* [n_blocks]: the scalar-quantised DC index qdc of each block (keyframes code
+                                           DC in the Haar pyramid instead), block order of luma_res / chroma_res */
 } daala_b200_kf_io;
 
 typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, device-resident callers) */
@@ -563,6 +581,8 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
   int max_luma_blocks, max_chroma_blocks;
   void *stream;
   long long bytes_allocated;
+  uint8_t *pred_pixels[3];              /* config.inter: the prediction pixels and their transform md (the */
+  int32_t *pred_coeffs[3];              /* layout of pixels / coeffs); NULL otherwise */
 } daala_b200_kf_buffers;
 
 #define DAALA_B200_KF_LISTS 1
@@ -576,6 +596,7 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
 
 daala_b200_kf *daala_b200_kf_create(const daala_b200_kf_config *cfg);   /* NULL on failure */
 void daala_b200_kf_destroy(daala_b200_kf *kf);
+/* The engine's last error message; with kf == NULL why this thread's last daala_b200_kf_create returned NULL. */
 const char *daala_b200_kf_error(const daala_b200_kf *kf);
 int daala_b200_kf_device_buffers(daala_b200_kf *kf, daala_b200_kf_buffers *out);
 int daala_b200_kf_launches_per_step(const daala_b200_kf *kf);   /* kernel launches of one whole step */
@@ -590,11 +611,12 @@ int daala_b200_kf_count_blocks(const uint8_t *bsize, int nframes, long long fram
 /* Worst-case lengths of the symbol stream arrays of a batch with these totals: every block, every band, two bytes
    per coefficient. */
 int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daala_b200_kf_sym_bounds *out);
-/* H2D of the inputs, the whole step, D2H of the requested outputs: enqueued, not waited for.  A batch with more
+/* With config.inter, DAALA_B200_KF_PVQ_LUMA selects the luma phase kernels.
+   H2D of the inputs, the whole step, D2H of the requested outputs: enqueued, not waited for.  A batch with more
    luma or chroma blocks than the engine's capacity (see max_blocks_div) returns cudaErrorInvalidValue before
    anything is copied or launched; so does a request for symbol stream outputs from an engine created without
-   symbol_stream, a stream capacity below daala_b200_kf_symbol_bounds, or a stream buffer that is not pinned host
-   memory. */
+   symbol_stream, a stream capacity below daala_b200_kf_symbol_bounds, a stream buffer that is not pinned host
+   memory, or (config.inter) a NULL pred_pixels plane, luma_dc or chroma_dc. */
 int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
 int daala_b200_kf_wait(daala_b200_kf *kf);
 int daala_b200_kf_encode(daala_b200_kf *kf, const daala_b200_kf_io *io);   /* submit + wait */
