@@ -55,6 +55,7 @@ enum Cnt {
   kNHeads = 15,      // row / column chain items ready from the start (no same-size neighbour to wait for)
   kNHeads0 = 16,     // band-0 items ready from the start
   kError = 17,
+  kDepsDone = 18,    // CTAs of k_luma_deps that have finished (the last one scans the chain heads' weight bins)
   // the words the persistent kernels hammer with atomics each sit in a 128-byte line of their own
   kHeadLoL = 32,     // ticket of the luma dependency-free lists
   kHeadLoC = 64,     // ticket of the chroma lists
@@ -63,6 +64,7 @@ enum Cnt {
   kDoneHi = 160,     // band-0 items finished (flushed by warps when they go idle)
   kHeadCh = 192,     // ticket of the row / column chain heads
   kWaiters = 224,    // warps parked on a future band-0 slot
+  kTraceN = 240,     // DAALA_B200_CHAIN_TRACE: records written by k_pvq_persist<true>
   kCntWords = 256
 };
 
@@ -87,8 +89,14 @@ struct Lists {
   int32_t* succ_right;
   uint32_t* items_l[3];            // dependency-free luma items per class
   uint32_t* items_c[3];
-  uint32_t* heads;                 // row / column chain items that are ready from the start
+  uint32_t* heads;                 // row / column chain items that are ready from the start, heaviest chain first
   uint32_t* heads0;                // band-0 items that are ready from the start
+  // chain heads as k_luma_deps finds them, each with its bin in descending order of chain weight; k_luma_deps
+  // counts the bins and its last CTA scans them, k_chroma_items scatters the heads into `heads`
+  uint32_t* heads_raw;
+  int32_t* head_bin;
+  int32_t* head_hist;              // [kLevelBins] counts, then exclusive offsets
+  int32_t* head_cursor;            // [kLevelBins]
   int32_t* cnt;                    // [kCntWords]
   // level path: chain items counting-sorted by dependency level (position along the chain in units of the
   // block size; larger bands first inside a level)
@@ -183,6 +191,7 @@ __global__ void __launch_bounds__(1024) k_tile_scan(const __grid_constant__ List
     L.cnt[kTotalHi] = 0;
     L.cnt[kNHeads] = 0;
     L.cnt[kNHeads0] = 0;
+    L.cnt[kDepsDone] = 0;
     // set on every step, so that an over-capacity batch does not flag the batches after it
     L.cnt[kError] = tot.x > L.max_luma || 2 * tot.z > L.max_chroma ? 1 : 0;
   }
@@ -249,22 +258,88 @@ __device__ __forceinline__ int level_bin(int band, int bs, int x0, int y0, int y
   return lvl * 3 + (2 - band_class(band));
 }
 
-// warp-aggregated append of `v` to list[*counter] by the lanes with `pred`
-__device__ __forceinline__ void append(uint32_t* list, int32_t* counter, bool pred, uint32_t v) {
+// warp-aggregated append of `v` to list[*counter] by the lanes with `pred`; the index written, or -1
+__device__ __forceinline__ int append(uint32_t* list, int32_t* counter, bool pred, uint32_t v) {
   const unsigned m = __ballot_sync(__activemask(), pred);
-  if (!pred) return;
+  if (!pred) return -1;
   const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
   int base = 0;
   if (lane == leader) base = atomicAdd(counter, __popc(m));
   base = __shfl_sync(m, base, leader);
-  list[base + __popc(m & ((1u << lane) - 1u))] = v;
+  const int pos = base + __popc(m & ((1u << lane) - 1u));
+  list[pos] = v;
+  return pos;
+}
+
+// warp-aggregated atomicAdd(&ctr[key], 1) by the calling lanes; the old value of the lane's own slot
+__device__ __forceinline__ int count_key(int32_t* ctr, int key) {
+  const unsigned same = __match_any_sync(__activemask(), key);
+  const int lane = threadIdx.x & 31, leader = __ffs(same) - 1;
+  int base = 0;
+  if (lane == leader) base = atomicAdd(&ctr[key], __popc(same));
+  return __shfl_sync(same, base, leader) + __popc(same & ((1u << lane) - 1u));
+}
+
+// Cost of one chain item per band class (n <= 16, 32, 128 coefficients) in units of 10 us: the mean duration of an
+// item of the class in k_pvq_persist<intra> while every warp is busy, 73 / 89 / 178 us on bench.py's workload (one
+// H100 80GB HBM3 at 700 W, tools/chain_timeline.py, DESIGN.md section 5).  A chain's weight is its length in blocks
+// times this; the bin of the weight orders the chain heads.
+constexpr int kChainCost0 = 7, kChainCost1 = 9, kChainCost2 = 18;
+__device__ __forceinline__ int weight_bin(int len, int band) {
+  const int c = band_class(band);
+  const int w = len * (c == 0 ? kChainCost0 : c == 1 ? kChainCost1 : kChainCost2);
+  return kLevelBins - 1 - min(w, kLevelBins - 1);   // heaviest first
+}
+
+// Length in blocks of the column (down) or row chain that starts at the block (x0, y0, bs) of `map`: its
+// same-size successors, by the test k_luma_deps uses for dep_top / dep_left, inside the coded unit rows.
+__device__ int chain_length(const Lists& L, const uint8_t* map, int x0, int y0, int bs, bool down) {
+  const int nn = 4 << bs, y_end = (L.u_row0 + L.u_rows) * 8, x_end = L.UW * 8;
+  int len = 1;
+  for (int x = x0 + (down ? 0 : nn), y = y0 + (down ? nn : 0); x < x_end && y < y_end;
+       x += down ? 0 : nn, y += down ? nn : 0, len++) {
+    if (map[(long long)(y >> 3) * L.bstride + (x >> 3)] != bs) break;
+    const int py = down ? y - 1 : y, px = down ? x : x - 1;
+    if (map[(long long)(py >> 3) * L.bstride + (px >> 3)] != bs) break;
+  }
+  return len;
+}
+
+// One CTA of kThreads: exclusive scan of kLevelBins counts in place (+ a copy as scatter cursors).  The counts are
+// read past L1: the last CTA of k_luma_deps scans what the other CTAs of that launch counted.
+template <int kThreads>
+__device__ __forceinline__ void scan_bins(int32_t* hist, int32_t* cursor) {
+  __shared__ int part[kThreads];
+  constexpr int kPer = kLevelBins / kThreads;
+  const int t = threadIdx.x;
+  int v[kPer], sum = 0;
+#pragma unroll
+  for (int i = 0; i < kPer; i++) {
+    v[i] = __ldcg(hist + t * kPer + i);
+    sum += v[i];
+  }
+  part[t] = sum;
+  __syncthreads();
+  for (int o = 1; o < kThreads; o <<= 1) {
+    const int add = t >= o ? part[t - o] : 0;
+    __syncthreads();
+    part[t] += add;
+    __syncthreads();
+  }
+  int run = part[t] - sum;
+#pragma unroll
+  for (int i = 0; i < kPer; i++) {
+    hist[t * kPer + i] = run;
+    cursor[t * kPer + i] = run;
+    run += v[i];
+  }
 }
 
 // Luma dependency structure.  od_hv_intra_pred (src/intra.c:37) predicts band b of a block from band b of
 // the same-size TOP neighbour (row-0 bands 1/4/7), the LEFT one (column-0 bands 2/5/8), both (band 0) or
 // nothing (bands 3/6).  Per block: the two neighbours and, inverted, the blocks that wait for this one;
 // per (block, band): a dependency-free item, a chain head (ready now) or a chain link (made ready by the
-// persistent kernel when its neighbours are done).
+// persistent kernel when its neighbours are done).  Row / column chain heads also get the weight bin of their chain.
 __global__ void __launch_bounds__(256) k_luma_deps(const __grid_constant__ Lists L) {
   const int n = min(L.cnt[kNLuma], L.max_luma);
   const int nth = gridDim.x * blockDim.x;
@@ -294,6 +369,14 @@ __global__ void __launch_bounds__(256) k_luma_deps(const __grid_constant__ Lists
       if (left >= 0) L.succ_right[left] = blk;
     }
     const int nb = in ? num_bands(bs) : 0;
+    // lengths of the column / row chains this block starts (the same for every band of a size class)
+    int len_down = 0, len_across = 0;
+    if (nb > 1) {
+      const daala_b200_pvq_block b = L.luma[blk];
+      const uint8_t* map = L.bsize + b.frame * L.bsize_pitch;
+      if (top < 0) len_down = chain_length(L, map, b.x0, b.y0, bs, true);
+      if (left < 0) len_across = chain_length(L, map, b.x0, b.y0, bs, false);
+    }
     int chain = 0;
     for (int band = 0; band < 9; band++) {
       const bool has = band < nb;
@@ -301,9 +384,18 @@ __global__ void __launch_bounds__(256) k_luma_deps(const __grid_constant__ Lists
       const int r = band % 3;
       const bool waits = band == 0 ? (top >= 0 || left >= 0) : r == 1 ? top >= 0 : left >= 0;
       const uint32_t item = ((uint32_t)blk << 4) | band;
-      if (band == 3 || band == 6) append(L.items_l[band_class(band)], &L.cnt[kNItemsL + band_class(band)], has, item);
-      else if (band == 0) append(L.heads0, &L.cnt[kNHeads0], has && !waits, item);
-      else append(L.heads, &L.cnt[kNHeads], has && !waits, item);
+      if (band == 3 || band == 6) {
+        append(L.items_l[band_class(band)], &L.cnt[kNItemsL + band_class(band)], has, item);
+      } else if (band == 0) {
+        append(L.heads0, &L.cnt[kNHeads0], has && !waits, item);
+      } else {
+        const int pos = append(L.heads_raw, &L.cnt[kNHeads], has && !waits, item);
+        if (pos >= 0) {
+          const int bin = weight_bin(r == 1 ? len_down : len_across, band);
+          L.head_bin[pos] = bin;
+          count_key(L.head_hist, bin);
+        }
+      }
       chain += has && !is_free;
       if (has && !is_free && L.lvl_hist) {
         const daala_b200_pvq_block b = L.luma[blk];
@@ -315,34 +407,21 @@ __global__ void __launch_bounds__(256) k_luma_deps(const __grid_constant__ Lists
     for (int o = 16; o > 0; o >>= 1) chain += __shfl_xor_sync(0xffffffffu, chain, o);
     if ((threadIdx.x & 31) == 0 && chain) atomicAdd(&L.cnt[kTotalHi], chain);
   }
+  // the last CTA to finish scans the weight bins of the chain heads; k_chroma_items sorts them
+  __shared__ bool last;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(&L.cnt[kDepsDone], 1) == (int)gridDim.x - 1;
+  __syncthreads();
+  if (last) {
+    __threadfence();
+    scan_bins<256>(L.head_hist, L.head_cursor);
+  }
 }
 
 // One CTA: exclusive scan of the level bins in place (+ a copy as scatter cursors).
 __global__ void __launch_bounds__(1024) k_level_scan(const __grid_constant__ Lists L) {
-  __shared__ int part[1024];
-  constexpr int kPer = kLevelBins / 1024;
-  const int t = threadIdx.x;
-  int v[kPer], sum = 0;
-#pragma unroll
-  for (int i = 0; i < kPer; i++) {
-    v[i] = L.lvl_hist[t * kPer + i];
-    sum += v[i];
-  }
-  part[t] = sum;
-  __syncthreads();
-  for (int o = 1; o < 1024; o <<= 1) {
-    const int add = t >= o ? part[t - o] : 0;
-    __syncthreads();
-    part[t] += add;
-    __syncthreads();
-  }
-  int run = part[t] - sum;
-#pragma unroll
-  for (int i = 0; i < kPer; i++) {
-    L.lvl_hist[t * kPer + i] = run;
-    L.lvl_cursor[t * kPer + i] = run;
-    run += v[i];
-  }
+  scan_bins<1024>(L.lvl_hist, L.lvl_cursor);
 }
 
 __global__ void __launch_bounds__(256) k_level_scatter(const __grid_constant__ Lists L) {
@@ -358,8 +437,12 @@ __global__ void __launch_bounds__(256) k_level_scatter(const __grid_constant__ L
   }
 }
 
-// Chroma items: no dependencies between blocks; compaction per class (order is free).
+// Chroma items: no dependencies between blocks; compaction per class (order is free).  Keyframes: first the luma
+// chain heads into `heads` by the weight bins k_luma_deps scanned, heaviest first (the order inside a bin is free).
 __global__ void __launch_bounds__(256) k_chroma_items(const __grid_constant__ Lists L) {
+  const int nh = L.cnt[kNHeads];   // 0 in inter mode
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nh; i += gridDim.x * blockDim.x)
+    L.heads[count_key(L.head_cursor, L.head_bin[i])] = L.heads_raw[i];
   const int n = min(L.cnt[kNChroma], L.max_chroma);
   for (int blk = blockIdx.x * blockDim.x + threadIdx.x; blk < n; blk += gridDim.x * blockDim.x) {
     const int bs = L.chroma[blk].bs;
@@ -397,8 +480,8 @@ __global__ void __launch_bounds__(256) k_luma_items(const __grid_constant__ List
 struct Stage {
   daala_b200_pvq_params prm;
   const uint32_t* items[3];        // dependency-free items per class (taken largest class first)
-  // luma only: row / column chain heads (static list; a chain is then walked by one warp), and the
-  // band-0 queue = [heads0 (static) | ring filled at run time]
+  // luma only: row / column chain heads, heaviest chain first (static list; a chain is then walked by one
+  // warp), and the band-0 queue = [heads0 (static) | ring filled at run time]
   const uint32_t* heads;
   const uint32_t* heads0;
   uint32_t* ring;
@@ -434,7 +517,51 @@ struct Stage {
   const int32_t* cfl_plane;        // chroma: prediction plane (chroma geometry), else NULL
   long long cfl_pitch;
   int cfl_stride;
+#ifdef DAALA_B200_CHAIN_TRACE
+  struct ChainTraceRec* trace;     // luma: one record per item k_pvq_persist<true> runs, up to trace_cap
+  int trace_cap;
+#endif
 };
+
+#ifdef DAALA_B200_CHAIN_TRACE
+// Timeline of the luma chain kernel, compiled only into the library tools/chain_timeline.py builds (the production
+// kernel does not contain it).  32 bytes per item.
+struct ChainTraceRec {
+  unsigned long long t0, t1;       // %globaltimer (ns) when the warp started / finished the item
+  uint32_t item;                   // (block << 4) | band
+  uint32_t cta;                    // one warp per CTA
+  uint16_t sm;
+  uint8_t bs;
+  uint8_t kind;                    // 0 band-0 queue slot, 1 row / column chain head, 2 free item, 3 chain successor
+  uint32_t pad;
+};
+
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+
+__device__ __noinline__ void trace_item(const Stage& S, uint32_t item, int kind, unsigned long long t0, int lane) {
+  __syncwarp();
+  if (lane != 0) return;
+  const unsigned long long t1 = globaltimer();
+  const int i = atomicAdd(&S.cnt[kTraceN], 1);
+  if (i >= S.trace_cap) return;
+  uint32_t sm;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+  ChainTraceRec r;
+  r.t0 = t0;
+  r.t1 = t1;
+  r.item = item;
+  r.cta = blockIdx.x;
+  r.sm = (uint16_t)sm;
+  r.bs = (uint8_t)S.prm.blocks[item >> 4].bs;
+  r.kind = (uint8_t)kind;
+  r.pad = 0;
+  S.trace[i] = r;
+}
+#endif
 
 // raster -> coding order of every block (od_raster_to_coding_order, src/partition.c:123); keyframe chroma:
 // also the CfL prediction and its sign flip (src/pvq_encoder.c:847-871); inter frames, all planes alike: the
@@ -886,9 +1013,19 @@ __global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(c
   for (;;) {
     uint32_t item = next_item<kIntra>(S, lane, &done, &waiter);
     if (item == kNoItem) return;
+#ifdef DAALA_B200_CHAIN_TRACE
+    int kind = (item & 15) == 0 ? 0 : (item & 15) == 3 || (item & 15) == 6 ? 2 : 1;
+#endif
     for (;;) {
       const int band = (int)(item & 15);
+#ifdef DAALA_B200_CHAIN_TRACE
+      const unsigned long long t0 = globaltimer();
+#endif
       run_item<kIntra>(S, item, lane, snap);
+#ifdef DAALA_B200_CHAIN_TRACE
+      if (kIntra) trace_item(S, item, kind, t0, lane);
+      kind = 3;
+#endif
       if (!kIntra || band == 3 || band == 6) break;
       done += band == 0;
       // results of this item -> visible to whoever runs a successor (this warp included: other lanes)
@@ -939,6 +1076,9 @@ __global__ void k_begin_pvq(int32_t* cnt, int luma) {
       cnt[kDoneHi] = 0;
       cnt[kHeadCh] = 0;
       cnt[kWaiters] = 0;
+#ifdef DAALA_B200_CHAIN_TRACE
+      cnt[kTraceN] = 0;
+#endif
     } else {
       cnt[kHeadLoC] = 0;
     }
@@ -1521,6 +1661,10 @@ static int kf_alloc(daala_b200_kf* kf) {
     }
   }
   KF_CHECK(dalloc(kf, &L.heads, inter ? 0 : kf->chain_cap));
+  KF_CHECK(dalloc(kf, &L.heads_raw, inter ? 0 : kf->chain_cap));
+  KF_CHECK(dalloc(kf, &L.head_bin, inter ? 0 : kf->chain_cap));
+  KF_CHECK(dalloc(kf, &L.head_hist, inter ? 0 : (size_t)kLevelBins));
+  KF_CHECK(dalloc(kf, &L.head_cursor, inter ? 0 : (size_t)kLevelBins));
   KF_CHECK(dalloc(kf, &L.heads0, ndep));
   KF_CHECK(dalloc(kf, &L.cnt, (size_t)kCntWords));
 
@@ -1589,6 +1733,12 @@ static int kf_alloc(daala_b200_kf* kf) {
     S.head_lo_at = chroma ? kHeadLoC : kHeadLoL;
     S.n_blocks_at = chroma ? kNChroma : kNLuma;
     S.max_blocks = (int)nblk;
+#ifdef DAALA_B200_CHAIN_TRACE
+    if (!chroma && !inter) {
+      S.trace_cap = (int)(luma_shard_px / 16);   // one band per 16 pixels at most
+      KF_CHECK(dalloc(kf, &S.trace, (size_t)S.trace_cap));
+    }
+#endif
     if (!chroma) {
       S.dep_top = L.dep_top;
       S.dep_left = L.dep_left;
@@ -1778,6 +1928,7 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
     if (cudaMemsetAsync(L.succ_bottom, 0xff, nl, s) != cudaSuccess || cudaMemsetAsync(L.succ_right, 0xff, nl, s) != cudaSuccess)
       return (int)cudaGetLastError();
     if (L.lvl_hist && cudaMemsetAsync(L.lvl_hist, 0, sizeof(int32_t) * kLevelBins, s) != cudaSuccess) return (int)cudaGetLastError();
+    if (cudaMemsetAsync(L.head_hist, 0, sizeof(int32_t) * kLevelBins, s) != cudaSuccess) return (int)cudaGetLastError();
     k_luma_deps<<<wide, 256, 0, s>>>(L);
     if (L.lvl_hist) {
       k_level_scan<<<1, 1024, 0, s>>>(L);
@@ -2012,6 +2163,10 @@ void daala_b200_kf_destroy(daala_b200_kf* kf) {
     cudaFree(L.items_c[c]);
   }
   cudaFree(L.heads);
+  cudaFree(L.heads_raw);
+  cudaFree(L.head_bin);
+  cudaFree(L.head_hist);
+  cudaFree(L.head_cursor);
   cudaFree(L.heads0);
   cudaFree(L.lvl_hist);
   cudaFree(L.lvl_cursor);
@@ -2061,12 +2216,26 @@ void daala_b200_kf_destroy(daala_b200_kf* kf) {
     cudaFree(S->join0);
     cudaFree(S->pre_ev);
     cudaFree(S->pre_snap);
+#ifdef DAALA_B200_CHAIN_TRACE
+    cudaFree(S->trace);
+#endif
   }
   if (kf->own_stream) cudaStreamDestroy(kf->stream);
   free(kf);
 }
 
 const char* daala_b200_kf_error(const daala_b200_kf* kf) { return kf ? kf->err : g_create_err; }
+
+#ifdef DAALA_B200_CHAIN_TRACE
+// tools/chain_timeline.py: the luma chain kernel's trace records (device) and their capacity; the count written by
+// the last luma stage is counts[kTraceN]
+int daala_b200_kf_chain_trace(daala_b200_kf* kf, void** recs, int* cap) {
+  if (!kf || !recs || !cap) return (int)cudaErrorInvalidValue;
+  *recs = kf->luma.trace;
+  *cap = kf->luma.trace_cap;
+  return 0;
+}
+#endif
 
 // Kernel launches of one whole step (kf_enqueue_step with DAALA_B200_KF_ALL), memset nodes not counted.
 int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
@@ -2108,6 +2277,8 @@ int daala_b200_kf_device_buffers(daala_b200_kf* kf, daala_b200_kf_buffers* out) 
   }
   out->luma_heads = kf->lists.heads;
   out->luma_heads0 = kf->lists.heads0;
+  out->luma_heads_raw = kf->lists.heads_raw;
+  out->luma_head_bin = kf->lists.head_bin;
   out->succ_bottom = kf->lists.succ_bottom;
   out->succ_right = kf->lists.succ_right;
   out->luma_res = kf->luma.res_pack;

@@ -58,7 +58,8 @@ class Buffers(ctypes.Structure):
                 ("luma_res", c_void_p), ("chroma_res", c_void_p), ("luma_y16", c_void_p), ("chroma_y16", c_void_p),
                 ("luma_skip_diff", c_void_p), ("chroma_skip_diff", c_void_p), ("chroma_flip", c_void_p),
                 ("max_luma_blocks", c_int), ("max_chroma_blocks", c_int), ("stream", c_void_p),
-                ("bytes_allocated", c_ll), ("pred_pixels", c_void_p * 3), ("pred_coeffs", c_void_p * 3)]
+                ("bytes_allocated", c_ll), ("pred_pixels", c_void_p * 3), ("pred_coeffs", c_void_p * 3),
+                ("luma_heads_raw", c_void_p), ("luma_head_bin", c_void_p)]
 
 
 def _bind():

@@ -572,7 +572,8 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
   int32_t *dep_top, *dep_left;          /* same-size neighbour above / left of each luma block, or -1 */
   int32_t *succ_bottom, *succ_right;    /* the inverse: the block that waits for this one, or -1 */
   uint32_t *luma_items[3];              /* dependency-free luma items (bands 3 / 6) per class */
-  uint32_t *luma_heads;                 /* row / column chain items ready from the start; counts[15] of them */
+  uint32_t *luma_heads;                 /* row / column chain items ready from the start; counts[15] of them, in
+                                           descending order of chain weight (the order the chain kernel takes them) */
   uint32_t *luma_heads0;                /* band-0 items ready from the start; counts[16] of them */
   uint32_t *chroma_items[3];
   int16_t *luma_res, *chroma_res, *luma_y16, *chroma_y16;
@@ -583,6 +584,8 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
   long long bytes_allocated;
   uint8_t *pred_pixels[3];              /* config.inter: the prediction pixels and their transform md (the */
   int32_t *pred_coeffs[3];              /* layout of pixels / coeffs); NULL otherwise */
+  uint32_t *luma_heads_raw;             /* luma_heads in the order the dependency builder found them, and the */
+  int32_t *luma_head_bin;               /* weight bin of each: 12287 - min(chain length x class cost, 12287) */
 } daala_b200_kf_buffers;
 
 #define DAALA_B200_KF_LISTS 1
