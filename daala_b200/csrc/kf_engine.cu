@@ -17,7 +17,8 @@
 //     -> (config.symbol_stream) the same symbols per frame in bitstream order with 8/16-bit pulses.
 //
 // config.inter: the residual of a batch of P frames the same way.  The motion-compensated prediction planes are
-// a second input; they take the same forward transform (no DC Haar pyramid on either side) and their
+// a second input (config.inter_mc: made in the graph from MV grids and a pool of reference pictures, before the
+// forward transform); they take the same forward transform (no DC Haar pyramid on either side) and their
 // coefficients `md` are the reference vector of every band (pvq_theta with is_keyframe = 0).  Without an intra
 // predictor every (block, band) of every plane is dependency-free: luma and chroma both go through the three
 // phase kernels (k_pvq_split) and the persistent chain kernel is not launched.
@@ -36,6 +37,7 @@
 
 #include "daala_b200.h"
 #include "dering_search.h"
+#include "mc_batch.h"
 #include "gen/coding_order.inc"
 #include "pvq_math.cuh"
 #include "pvq_warp.cuh"
@@ -56,6 +58,8 @@ enum Cnt {
   kNHeads0 = 16,     // band-0 items ready from the start
   kError = 17,
   kDepsDone = 18,    // CTAs of k_luma_deps that have finished (the last one scans the chain heads' weight bins)
+  kMcBadRef = 19,    // config.inter_mc: leaf corners whose vertex has a ref other than GOLD / PREV
+  kMcBeyond = 20,    //                  corner windows reaching past the reference's edge extension
   // the words the persistent kernels hammer with atomics each sit in a 128-byte line of their own
   kHeadLoL = 32,     // ticket of the luma dependency-free lists
   kHeadLoC = 64,     // ticket of the chroma lists
@@ -1524,6 +1528,13 @@ struct daala_b200_kf {
   Sym sym;                         // symbol stream (cfg.symbol_stream); zero otherwise
   daala_b200_frame frame;
   daala_b200_frame frame_pred;     // cfg.inter: `frame` with the prediction planes as the forward transform's input / output
+  // cfg.inter_mc: the reference-picture pool, slot map, MV grids and per-MV-block leaf segments
+  uint8_t* ref_pixels[3];
+  int32_t* ref_slot;
+  daala_b200_mv_pt* mv_grid;
+  uint32_t* mc_leaves;
+  int32_t* mc_nleaves;
+  daala_b200_mc_batch mc;
   size_t bytes_allocated;
   size_t chain_cap;                // entries of the chain queue (heads / ring)
   int sms;
@@ -1568,6 +1579,29 @@ static int kf_alloc(daala_b200_kf* kf) {
   const int UW = kf->nhsb * 8, UH = kf->nvsb * 8;
   KF_CHECK(dalloc(kf, &kf->bsize, (size_t)F * UW * UH));
   if (!inter) KF_CHECK(dalloc(kf, &kf->cfl_plane, (size_t)kf->plane_w[1] * kf->plane_h[1] * F));
+  if (kf->cfg.inter_mc) {
+    daala_b200_mc_batch& B = kf->mc;
+    const size_t nsb = (size_t)kf->nhsb * kf->nvsb;
+    for (int p = 0; p < 3; p++) {
+      KF_CHECK(dalloc(kf, &kf->ref_pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * kf->cfg.mc_refs));
+      B.ref[p] = kf->ref_pixels[p];
+      B.pred[p] = kf->pred_pixels[p];
+      B.plane_w[p] = kf->plane_w[p];
+      B.plane_h[p] = kf->plane_h[p];
+    }
+    KF_CHECK(dalloc(kf, &kf->ref_slot, (size_t)2 * F));
+    KF_CHECK(dalloc(kf, &kf->mv_grid, (size_t)F * (kf->nvsb * 8 + 1) * (kf->nhsb * 8 + 1)));
+    KF_CHECK(dalloc(kf, &kf->mc_leaves, (size_t)F * nsb * 64));
+    KF_CHECK(dalloc(kf, &kf->mc_nleaves, (size_t)F * nsb));
+    B.grid = kf->mv_grid;
+    B.ref_slot = kf->ref_slot;
+    B.leaves = kf->mc_leaves;
+    B.nleaves = kf->mc_nleaves;
+    B.F = F;
+    B.nhsb = kf->nhsb;
+    B.nvsb = kf->nvsb;
+    B.nslots = kf->cfg.mc_refs;
+  }
   KF_CHECK(dalloc(kf, &kf->qm, (size_t)2 * kf->cfg.qm_stride));
   KF_CHECK(dalloc(kf, &kf->qm_inv, (size_t)2 * kf->cfg.qm_stride));
   KF_CHECK(dalloc(kf, &kf->rsqrt_tbl, (size_t)kTableDoubles));
@@ -1667,6 +1701,8 @@ static int kf_alloc(daala_b200_kf* kf) {
   KF_CHECK(dalloc(kf, &L.head_cursor, inter ? 0 : (size_t)kLevelBins));
   KF_CHECK(dalloc(kf, &L.heads0, ndep));
   KF_CHECK(dalloc(kf, &L.cnt, (size_t)kCntWords));
+  kf->mc.bad_ref = L.cnt + kMcBadRef;
+  kf->mc.beyond = L.cnt + kMcBeyond;
 
   auto setup_stage = [&](Stage& S, bool chroma) -> int {
     memset(&S, 0, sizeof(S));
@@ -1895,9 +1931,15 @@ static int kf_enqueue_step_inter(daala_b200_kf* kf, int phases) {
     k_unit_emit<<<L.ntiles, kTile, 0, s>>>(L);
     k_luma_items<<<wide, 256, 0, s>>>(L);
     k_chroma_items<<<wide, 256, 0, s>>>(L);
+    if (kf->cfg.inter_mc) {
+      if (cudaMemsetAsync(L.cnt + kMcBadRef, 0, 2 * sizeof(int32_t), s) != cudaSuccess) return (int)cudaGetLastError();
+      int rc = daala_b200_launch_mc_leaves(&kf->mc, wide, s);
+      if (rc) return rc;
+    }
   }
   if (phases & DAALA_B200_KF_FORWARD) {
-    int rc = daala_b200_launch_forward(&kf->frame, 3, s);
+    int rc = kf->cfg.inter_mc ? daala_b200_launch_mc_obmc(&kf->mc, wide, s) : 0;
+    if (!rc) rc = daala_b200_launch_forward(&kf->frame, 3, s);
     if (!rc) rc = daala_b200_launch_forward(&kf->frame_pred, 3, s);
     if (rc) return rc;
   }
@@ -2064,6 +2106,14 @@ static thread_local char g_create_err[256] = "null engine";
 
 daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: invalid configuration");
+  if (cfg && cfg->inter_mc && (cfg->inter_mc != 1 || cfg->inter != 1)) {
+    snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: inter_mc is 0 or 1, and 1 requires inter = 1");
+    return nullptr;
+  }
+  if (cfg && cfg->mc_refs < 0) {
+    snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: mc_refs < 0");
+    return nullptr;
+  }
   if (cfg && cfg->inter) {
     // P-frame residual mode is defined for whole frames through the phase kernels, without the stages whose
     // inter form this engine does not have
@@ -2088,6 +2138,8 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   kf->nhsb = (cfg->pic_w + 63) / 64;
   kf->nvsb = (cfg->pic_h + 63) / 64;
   kf->F = cfg->nframes;
+  if (kf->cfg.inter_mc && kf->cfg.mc_refs == 0) kf->cfg.mc_refs = 2 * kf->F;
+  if (!kf->cfg.inter_mc) kf->cfg.mc_refs = 0;
   if (kf->cfg.sb_rows <= 0) {
     kf->cfg.sb_row0 = 0;
     kf->cfg.sb_rows = kf->nvsb;
@@ -2139,7 +2191,12 @@ void daala_b200_kf_destroy(daala_b200_kf* kf) {
     cudaFree(kf->pixels_out[p]);
     cudaFree(kf->pred_pixels[p]);
     cudaFree(kf->pred_coeffs[p]);
+    cudaFree(kf->ref_pixels[p]);
   }
+  cudaFree(kf->ref_slot);
+  cudaFree(kf->mv_grid);
+  cudaFree(kf->mc_leaves);
+  cudaFree(kf->mc_nleaves);
   cudaFree(kf->bsize);
   cudaFree(kf->cfl_plane);
   cudaFree(kf->qm);
@@ -2241,8 +2298,10 @@ int daala_b200_kf_chain_trace(daala_b200_kf* kf, void** recs, int* cap) {
 int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   if (!kf) return 0;
   auto split = [](const Stage& S) { return 3 * (S.sp_chunks[0] + S.sp_chunks[1] + S.sp_chunks[2]); };
-  // inter: work lists, two forward launches, per stage gather + phase kernels + finish, inverse + SB postfilter
-  if (kf->cfg.inter) return 5 + 2 + (2 + split(kf->luma)) + (2 + split(kf->chroma)) + 2;
+  // inter: work lists, two forward launches, per stage gather + phase kernels + finish, inverse + SB postfilter;
+  // inter_mc: leaf enumeration and OBMC
+  if (kf->cfg.inter)
+    return 5 + 2 + (2 + split(kf->luma)) + (2 + split(kf->chroma)) + 2 + (kf->cfg.inter_mc ? 2 : 0);
   int n = 5 + (kf->cfg.level_chains ? 2 : 0);                                    // work lists
   n += 1;                                                                         // forward
   n += 3 + 1 + (kf->cfg.split_free > 1 ? split(kf->luma) : 0) + (kf->luma.pre_ev ? 2 : 0);   // luma: begin, gather, [prepass], chains, finish
@@ -2295,7 +2354,11 @@ int daala_b200_kf_device_buffers(daala_b200_kf* kf, daala_b200_kf_buffers* out) 
   for (int p = 0; p < 3; p++) {
     out->pred_pixels[p] = kf->pred_pixels[p];
     out->pred_coeffs[p] = kf->pred_coeffs[p];
+    out->ref_pixels[p] = kf->ref_pixels[p];
   }
+  out->ref_slot = kf->ref_slot;
+  out->mv_grid = kf->mv_grid;
+  out->mc_refs = kf->cfg.mc_refs;
   return 0;
 }
 
@@ -2420,9 +2483,25 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   else daala_b200_kf_count_blocks(io->bsize, F, (long long)kf->nhsb * 8 * kf->nvsb * 8, kf->nhsb * 8, kf->nhsb, kf->nvsb,
                                   kf->cfg.sb_row0, kf->cfg.sb_rows, &tot);
   if (tot.n_luma > kf->lists.max_luma || tot.n_chroma > kf->lists.max_chroma) return (int)cudaErrorInvalidValue;
-  if (kf->cfg.inter && (!io->pred_pixels[0] || !io->pred_pixels[1] || !io->pred_pixels[2] || !io->luma_dc || !io->chroma_dc)) {
+  const bool have_pred = io->pred_pixels[0] || io->pred_pixels[1] || io->pred_pixels[2];
+  if (kf->cfg.inter && !kf->cfg.inter_mc &&
+      (!io->pred_pixels[0] || !io->pred_pixels[1] || !io->pred_pixels[2] || !io->luma_dc || !io->chroma_dc)) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: an inter engine needs pred_pixels[0..2], luma_dc and chroma_dc");
     return (int)cudaErrorInvalidValue;
+  }
+  if (kf->cfg.inter_mc) {
+    const char* why = !io->luma_dc || !io->chroma_dc ? "luma_dc and chroma_dc are required"
+                      : !io->mv_grid ? "mv_grid is required"
+                      : !io->ref_pixels[0] || !io->ref_pixels[1] || !io->ref_pixels[2] ? "ref_pixels[0..2] are required"
+                      : !io->ref_slot ? "ref_slot is required"
+                      : have_pred ? "pred_pixels is refused: the engine makes the prediction"
+                      : io->nrefs < 1 || io->nrefs > kf->cfg.mc_refs ? "nrefs is outside [1, mc_refs]" : nullptr;
+    for (int i = 0; !why && i < 2 * F; i++)
+      if (io->ref_slot[i] < 0 || io->ref_slot[i] >= io->nrefs) why = "a ref_slot entry is outside [0, nrefs)";
+    if (why) {
+      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: inter_mc: %s", why);
+      return (int)cudaErrorInvalidValue;
+    }
   }
   // symbol stream: the engine must produce it, and every requested buffer must hold the worst case and be pinned
   SymCopy sc;
@@ -2458,9 +2537,18 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     if (!io->pixels[p]) return (int)cudaErrorInvalidValue;
     KF_CHECK(cudaMemcpyAsync(kf->pixels[p], io->pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
                              cudaMemcpyHostToDevice, s));
-    if (kf->cfg.inter)
+    if (kf->cfg.inter_mc)
+      KF_CHECK(cudaMemcpyAsync(kf->ref_pixels[p], io->ref_pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * io->nrefs,
+                               cudaMemcpyHostToDevice, s));
+    else if (kf->cfg.inter)
       KF_CHECK(cudaMemcpyAsync(kf->pred_pixels[p], io->pred_pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
                                cudaMemcpyHostToDevice, s));
+  }
+  if (kf->cfg.inter_mc) {
+    KF_CHECK(cudaMemcpyAsync(kf->ref_slot, io->ref_slot, sizeof(int32_t) * 2 * F, cudaMemcpyHostToDevice, s));
+    KF_CHECK(cudaMemcpyAsync(kf->mv_grid, io->mv_grid,
+                             sizeof(daala_b200_mv_pt) * F * (kf->nvsb * 8 + 1) * (kf->nhsb * 8 + 1),
+                             cudaMemcpyHostToDevice, s));
   }
   const size_t map_bytes = (size_t)kf->nhsb * 8 * kf->nvsb * 8 * F;
   KF_CHECK(cudaMemcpyAsync(kf->bsize, io->bsize, map_bytes, cudaMemcpyHostToDevice, s));
@@ -2490,6 +2578,10 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   if (io->luma_skip_diff) KF_CHECK(cudaMemcpyAsync(io->luma_skip_diff, kf->luma.prm.res_skip_diff, 8 * (size_t)tot.n_luma, cudaMemcpyDeviceToHost, s));
   if (io->chroma_skip_diff) KF_CHECK(cudaMemcpyAsync(io->chroma_skip_diff, kf->chroma.prm.res_skip_diff, 8 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));
   if (io->chroma_flip) KF_CHECK(cudaMemcpyAsync(io->chroma_flip, kf->chroma.prm.res_flip, 4 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));
+  for (int p = 0; p < 3; p++)
+    if (kf->cfg.inter_mc && io->pred_pixels_out[p])
+      KF_CHECK(cudaMemcpyAsync(io->pred_pixels_out[p], kf->pred_pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
+                               cudaMemcpyDeviceToHost, s));
   if (kf->cfg.inter) {
     KF_CHECK(cudaMemcpyAsync(io->luma_dc, kf->luma.prm.res_dc, 4 * (size_t)tot.n_luma, cudaMemcpyDeviceToHost, s));
     KF_CHECK(cudaMemcpyAsync(io->chroma_dc, kf->chroma.prm.res_dc, 4 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));

@@ -20,6 +20,7 @@
 #include <stdint.h>
 
 #include "daala_b200.h"
+#include "mc_batch.h"
 
 namespace daala_b200 {
 namespace mc {
@@ -36,31 +37,51 @@ __constant__ short kSubpel[8][6] = {
 
 __device__ __forceinline__ unsigned char clamp255(int v) { return (unsigned char)(v < 0 ? 0 : v > 255 ? 255 : v); }
 
-// CTA-cooperative single-MV prediction of an nx x ny block into `out` (row
-// stride nx).  `src` points at the block's own position in the reference
-// plane; mv in 1/8 pel.  `buf` holds (ny + 5) * nx int16.
-__device__ void predict_block(unsigned char* out, short* buf, const unsigned char* src, int stride,
-                              int mvx, int mvy, int lx, int ly) {
+// Reference pixels as predict_block reads them: at (y, x) relative to a base.
+// DirectRef: a pointer into a plane whose padding holds every displaced window (the section-B entry points pass
+// the block's own position).  ClampedRef: a frame-sized w x h plane read at coordinates clamped to it, which is
+// od_img_edge_ext's extension (src/state.c:1102) without a padded copy, and never leaves the plane.
+struct DirectRef {
+  const unsigned char* p;
+  int stride;
+  __device__ __forceinline__ int at(int y, int x) const { return p[(ptrdiff_t)y * stride + x]; }
+  __device__ __forceinline__ bool same(const DirectRef& o) const { return p == o.p; }
+};
+
+struct ClampedRef {
+  const unsigned char* p;
+  int stride, w, h;
+  __device__ __forceinline__ int at(int y, int x) const {
+    return p[(ptrdiff_t)min(max(y, 0), h - 1) * stride + min(max(x, 0), w - 1)];
+  }
+  __device__ __forceinline__ bool same(const ClampedRef& o) const { return p == o.p; }
+};
+
+// CTA-cooperative single-MV prediction of an nx x ny block at (x, y) of `ref` into `out` (row stride nx);
+// mv in 1/8 pel.  `buf` holds (ny + 5) * nx int16.
+template <class R>
+__device__ void predict_block(unsigned char* out, short* buf, const R& ref, int x, int y, int mvx, int mvy,
+                              int lx, int ly) {
   const int nx = 1 << lx, ny = 1 << ly;
   const int fxi = mvx & 7, fyi = mvy & 7;
-  const unsigned char* p = src + (mvx >> 3) + (mvy >> 3) * stride;
+  x += mvx >> 3;
+  y += mvy >> 3;
   if (!fxi && !fyi) {
-    for (int i = threadIdx.x; i < nx * ny; i += blockDim.x) out[i] = p[(i >> lx) * stride + (i & (nx - 1))];
+    for (int i = threadIdx.x; i < nx * ny; i += blockDim.x) out[i] = ref.at(y + (i >> lx), x + (i & (nx - 1)));
     __syncthreads();
     return;
   }
   // Horizontal stage, rows -2 .. ny+2, biased by -(128 << 7) to fit int16.
   for (int i = threadIdx.x; i < nx * (ny + kApron); i += blockDim.x) {
-    int r = (i >> lx) - 2, c = i & (nx - 1);
-    const unsigned char* row = p + r * stride + c;
+    const int r = y + (i >> lx) - 2, c = x + (i & (nx - 1));
     int v;
     if (fxi) {
       v = 0;
 #pragma unroll
-      for (int k = 0; k < 6; k++) v += row[k - 2] * kSubpel[fxi][k];
+      for (int k = 0; k < 6; k++) v += ref.at(r, c + k - 2) * kSubpel[fxi][k];
       v -= 128 << 7;
     } else {
-      v = (row[0] << 7) - (128 << 7);
+      v = (ref.at(r, c) << 7) - (128 << 7);
     }
     buf[i] = (short)v;
   }
@@ -112,20 +133,22 @@ __device__ __forceinline__ SplitWeights split_weights(int oc, int s, int lx, int
   return w;
 }
 
-// OBMC prediction of one block (od_mc_predict_singleref, src/mc.c:1965) by the CTA into out[j * out_stride + i]:
-// up to four single-MV predictions (re-used when two corners share a MV) + od_mc_blend_full(_split)8_c.
+// OBMC prediction of one block by the CTA into out[j * out_stride + i]: od_mc_predict (src/mc.c:2006) with each
+// corner's own reference picture ref[k], the block at (b.x0, b.y0) of each.  Up to four single-MV predictions --
+// two corners share one when both their vector and their picture are the same, as od_mc_predict_singleref
+// (:1965) shares equal vectors of one picture -- then od_mc_blend_full(_split)8_c.
+template <class R>
 __device__ void obmc_block(unsigned char* out, int out_stride, unsigned char (&pred)[4][kMaxN * kMaxN], short* buf,
-                           const unsigned char* ref, int ref_stride, const daala_b200_mc_block& b) {
+                           const R (&ref)[4], const daala_b200_mc_block& b) {
   const int lx = b.log_xblk, ly = b.log_yblk;
   const int nx = 1 << lx, ny = 1 << ly;
-  const unsigned char* src = ref + (size_t)b.y0 * ref_stride + b.x0;
   int which[4];
   for (int k = 0; k < 4; k++) {
     which[k] = k;
     for (int q = 0; q < k; q++) {
-      if (b.mvx[q] == b.mvx[k] && b.mvy[q] == b.mvy[k]) { which[k] = which[q]; break; }
+      if (b.mvx[q] == b.mvx[k] && b.mvy[q] == b.mvy[k] && ref[q].same(ref[k])) { which[k] = which[q]; break; }
     }
-    if (which[k] == k) predict_block(pred[k], buf, src, ref_stride, b.mvx[k], b.mvy[k], lx, ly);
+    if (which[k] == k) predict_block(pred[k], buf, ref[k], b.x0, b.y0, b.mvx[k], b.mvy[k], lx, ly);
   }
   const unsigned char* p0 = pred[which[0]];
   const unsigned char* p1 = pred[which[1]];
@@ -160,7 +183,8 @@ k_obmc_blocks(const unsigned char* __restrict__ ref, int ref_stride, unsigned ch
   __shared__ unsigned char pred[4][kMaxN * kMaxN];
   __shared__ short buf[(kMaxN + kApron) * kMaxN];
   const daala_b200_mc_block b = blocks[blockIdx.x];
-  obmc_block(dst + (size_t)b.y0 * dst_stride + b.x0, dst_stride, pred, buf, ref, ref_stride, b);
+  const DirectRef r = {ref, ref_stride}, refs[4] = {r, r, r, r};
+  obmc_block(dst + (size_t)b.y0 * dst_stride + b.x0, dst_stride, pred, buf, refs, b);
 }
 
 // 8-point Walsh-Hadamard on registers (ordering is irrelevant for a sum of magnitudes).
@@ -189,7 +213,7 @@ k_match_candidates(const unsigned char* __restrict__ cur, int cur_stride, const 
   short* buf = reinterpret_cast<short*>(work);
   const daala_b200_match_job job = jobs[blockIdx.x];
   const int ln = job.log_blk, n = 1 << ln;
-  predict_block(pred, buf, ref + (size_t)job.y0 * ref_stride + job.x0, ref_stride, job.mvx, job.mvy, ln, ln);
+  predict_block(pred, buf, DirectRef{ref, ref_stride}, job.x0, job.y0, job.mvx, job.mvy, ln, ln);
   const unsigned char* c0 = cur + (size_t)job.y0 * cur_stride + job.x0;
   int acc = 0;
   if (!use_satd) {
@@ -274,7 +298,7 @@ k_predict1fmv(const unsigned char* __restrict__ ref, int ref_stride, unsigned ch
   __shared__ short buf[(kMaxN + kApron) * kMaxN];
   const daala_b200_match_job job = jobs[blockIdx.x];
   const int lx = job.log_blk, ly = log_yblk_override >= 0 ? log_yblk_override : lx;
-  predict_block(pred, buf, ref + (size_t)job.y0 * ref_stride + job.x0, ref_stride, job.mvx, job.mvy, lx, ly);
+  predict_block(pred, buf, DirectRef{ref, ref_stride}, job.x0, job.y0, job.mvx, job.mvy, lx, ly);
   unsigned char* out = dst + (size_t)blockIdx.x * dst_pitch;
   for (int i = threadIdx.x; i < (1 << (lx + ly)); i += blockDim.x) out[i] = pred[i];
 }
@@ -332,8 +356,8 @@ k_bma_sad(const __grid_constant__ BmaPlanes P, const daala_b200_bma_job* __restr
     const int dec = pli > 0;
     const int ln = job.log_mvb_sz + 3 - dec, n = 1 << ln;   // OD_LOG_MVBSIZE_MIN = 3
     int x = job.bx >> dec, y = job.by >> dec;
-    predict_block(pred, buf, P.ref[pli] + (ptrdiff_t)y * P.ref_stride[pli] + x, P.ref_stride[pli],
-                  job.mvx * (1 << (2 - dec)), job.mvy * (1 << (2 - dec)), ln, ln);
+    predict_block(pred, buf, DirectRef{P.ref[pli], P.ref_stride[pli]}, x, y, job.mvx * (1 << (2 - dec)),
+                  job.mvy * (1 << (2 - dec)), ln, ln);
     int w = n, h = n, px = 0, py = 0;
     if (x < 0) { w += x; px = -x; x = 0; }
     if (y < 0) { h += y; py = -y; y = 0; }
@@ -376,7 +400,8 @@ k_est_sad(const __grid_constant__ BmaPlanes P, const daala_b200_mc_block* __rest
     const daala_b200_mc_block b = blocks[3 * blockIdx.x + pli];
     const int dec = pli > 0;
     const int nx = 1 << b.log_xblk, ny = 1 << b.log_yblk;
-    obmc_block(blend, nx, pred, buf, P.ref[pli], P.ref_stride[pli], b);
+    const DirectRef r = {P.ref[pli], P.ref_stride[pli]}, refs[4] = {r, r, r, r};
+    obmc_block(blend, nx, pred, buf, refs, b);
     __syncthreads();
     const int plane_w = (P.pic_w + dec) >> dec, plane_h = (P.pic_h + dec) >> dec;   // OD_PLANE_SZ
     const int w = min(nx, plane_w - (int)b.x0), h = min(ny, plane_h - (int)b.y0);
@@ -400,6 +425,132 @@ k_est_sad(const __grid_constant__ BmaPlanes P, const daala_b200_mc_block* __rest
     __syncthreads();
   }
   if (threadIdx.x == 0) result[blockIdx.x] = total;
+}
+
+// ---- P-frame prediction from MV grids (the keyframe engine's config.inter_mc; mc_batch.h) ---------------------
+//
+// k_mc_leaves: one warp per (frame, 64x64 MV block).  Lane t follows the 8x8 cells t and t + 32 down
+// od_state_pred_block's recursion (src/state.c:673-709: split where the centre vertex is valid, down to 8x8);
+// the cell at a leaf's top-left corner writes the leaf, with its outside corner oc and split state s, into the
+// block's 64-slot segment (a block has at most 64 leaves, so no scan is needed).  Record: cell (j * 8 + i) |
+// log size l << 6 | oc << 8 | s << 10.  The same leaves serve all three planes.
+// k_mc_obmc: per (frame, MV block, plane) the OBMC prediction of each leaf, every corner from the pool slot of its
+// vertex's picture.
+
+__constant__ int kVertD[22] = {0, 0, 1, 1, 0, 0, 1, 2, 0, 0, 2, 1, 0, -1, 1, 1, 0, -1, 0, 1, 1, -1};   // OD_VERT_D
+// offsets into OD_VERT_D of OD_VERT_SETUP_DX / _DY [oc][s] (src/state.c:593-625; OD_VERT_DY = OD_VERT_D)
+__constant__ unsigned char kSetupDX[4][4] = {{9, 1, 9, 1}, {13, 13, 1, 1}, {18, 1, 18, 1}, {5, 5, 1, 1}};
+__constant__ unsigned char kSetupDY[4][4] = {{4, 4, 0, 0}, {8, 0, 8, 0}, {12, 12, 0, 0}, {17, 0, 17, 0}};
+
+__device__ __forceinline__ int div_pow2_re(int x, int shift) {   // OD_DIV_POW2_RE, src/odintrin.h:149
+  return shift ? (x + (((1 << shift) + ((x >> shift) & 1) - 1) >> 1)) >> shift : x;
+}
+
+// The vertex of corner k of the leaf at vertex (vx, vy) (od_state_pred_block_from_setup, src/state.c:647-651).
+__device__ __forceinline__ const daala_b200_mv_pt& leaf_corner(const daala_b200_mv_pt* g, int gstride, int vx, int vy,
+                                                               int l, int oc, int s, int k) {
+  return g[(vy + (kVertD[kSetupDY[oc][s] + k] << l)) * gstride + vx + (kVertD[kSetupDX[oc][s] + k] << l)];
+}
+
+__global__ void __launch_bounds__(256) k_mc_leaves(const __grid_constant__ daala_b200_mc_batch B) {
+  const int lane = threadIdx.x & 31;
+  const int nsb = B.nhsb * B.nvsb, gstride = B.nhsb * 8 + 1;
+  const long long per_frame = (long long)gstride * (B.nvsb * 8 + 1);
+  int bad = 0, beyond = 0;
+  for (int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < B.F * nsb; w += (gridDim.x * blockDim.x) >> 5) {
+    const int f = w / nsb, sb = w - f * nsb;
+    const int vx0 = (sb % B.nhsb) * 8, vy0 = (sb / B.nhsb) * 8;
+    const daala_b200_mv_pt* g = B.grid + f * per_frame;
+    uint32_t rec[2];
+    bool emit[2];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int cell = lane + 32 * h, i = cell & 7, j = cell >> 3;
+      int bx = 0, by = 0, l = 3;
+      while (l > 0) {
+        const int half = 1 << (l - 1);
+        if (!g[(vy0 + by + half) * gstride + vx0 + bx + half].valid) break;
+        if (i >= bx + half) bx += half;
+        if (j >= by + half) by += half;
+        l--;
+      }
+      emit[h] = i == bx && j == by;
+      const int vx = vx0 + bx, vy = vy0 + by;
+      int oc = 0, s = 3;
+      if (l < 3) {
+        const int mask = (1 << (l + 1)) - 1;
+        oc = (vx & mask) != 0;
+        if (vy & mask) oc = 3 - oc;
+        // OD_VERT_DX = OD_VERT_D + 1, OD_VERT_DY = OD_VERT_D
+        const int c1 = (oc + 1) & 3, c3 = (oc + 3) & 3;
+        s = g[(vy + (kVertD[c1] << l)) * gstride + vx + (kVertD[c1 + 1] << l)].valid |
+            g[(vy + (kVertD[c3] << l)) * gstride + vx + (kVertD[c3 + 1] << l)].valid << 1;
+      }
+      rec[h] = (uint32_t)(by * 8 + bx) | l << 6 | oc << 8 | s << 10;
+      if (!emit[h]) continue;
+      for (int k = 0; k < 4; k++) {
+        const daala_b200_mv_pt& v = leaf_corner(g, gstride, vx, vy, l, oc, s, k);
+        bad += v.ref > 1;
+        for (int p = 0; p < 3; p++) {
+          const int dec = p > 0, pad = 64 >> dec, n = 1 << (l + 3 - dec);
+          const int x = (vx << (3 - dec)) + (div_pow2_re(v.mv[0], dec) >> 3);
+          const int y = (vy << (3 - dec)) + (div_pow2_re(v.mv[1], dec) >> 3);
+          beyond += x - 2 < -pad || x + n + 2 > B.plane_w[p] - 1 + pad || y - 2 < -pad || y + n + 2 > B.plane_h[p] - 1 + pad;
+        }
+      }
+    }
+    const unsigned b0 = __ballot_sync(0xffffffffu, emit[0]), b1 = __ballot_sync(0xffffffffu, emit[1]);
+    const unsigned lt = (1u << lane) - 1;
+    uint32_t* seg = B.leaves + (size_t)w * 64;
+    if (emit[0]) seg[__popc(b0 & lt)] = rec[0];
+    if (emit[1]) seg[__popc(b0) + __popc(b1 & lt)] = rec[1];
+    if (lane == 0) B.nleaves[w] = __popc(b0) + __popc(b1);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    bad += __shfl_xor_sync(0xffffffffu, bad, o);
+    beyond += __shfl_xor_sync(0xffffffffu, beyond, o);
+  }
+  if (lane == 0 && bad) atomicAdd(B.bad_ref, bad);
+  if (lane == 0 && beyond) atomicAdd(B.beyond, beyond);
+}
+
+__global__ void __launch_bounds__(kThreads) k_mc_obmc(const __grid_constant__ daala_b200_mc_batch B) {
+  __shared__ unsigned char pred[4][kMaxN * kMaxN];
+  __shared__ short buf[(kMaxN + kApron) * kMaxN];
+  const int nsb = B.nhsb * B.nvsb, gstride = B.nhsb * 8 + 1;
+  const long long per_frame = (long long)gstride * (B.nvsb * 8 + 1);
+  for (int u = blockIdx.x; u < B.F * nsb * 3; u += gridDim.x) {
+    const int p = u % 3, w = u / 3, f = w / nsb, sb = w - f * nsb;
+    const int dec = p > 0, pw = B.plane_w[p], ph = B.plane_h[p];
+    const int vx0 = (sb % B.nhsb) * 8, vy0 = (sb / B.nhsb) * 8;
+    const daala_b200_mv_pt* g = B.grid + f * per_frame;
+    const size_t plane = (size_t)pw * ph;
+    // submit checks the slots; a device-resident caller's are kept inside the pool
+    const int gold = min(max(B.ref_slot[2 * f], 0), B.nslots - 1), prev = min(max(B.ref_slot[2 * f + 1], 0), B.nslots - 1);
+    unsigned char* out = B.pred[p] + f * plane;
+    const int n = B.nleaves[w];
+    for (int q = 0; q < n; q++) {
+      const uint32_t r = B.leaves[(size_t)w * 64 + q];
+      const int vx = vx0 + (r & 7), vy = vy0 + ((r >> 3) & 7), l = (r >> 6) & 3, oc = (r >> 8) & 3, s = (r >> 10) & 3;
+      daala_b200_mc_block b;
+      ClampedRef refs[4];
+      for (int k = 0; k < 4; k++) {
+        const daala_b200_mv_pt& v = leaf_corner(g, gstride, vx, vy, l, oc, s, k);
+        b.mvx[k] = div_pow2_re(v.mv[0], dec);
+        b.mvy[k] = div_pow2_re(v.mv[1], dec);
+        // a ref other than GOLD reads PREV (counted by k_mc_leaves)
+        refs[k] = ClampedRef{B.ref[p] + (size_t)(v.ref == 0 ? gold : prev) * plane, pw, pw, ph};
+      }
+      b.x0 = (uint16_t)(vx << (3 - dec));
+      b.y0 = (uint16_t)(vy << (3 - dec));
+      b.log_xblk = b.log_yblk = (uint8_t)(l + 3 - dec);
+      b.oc = (uint8_t)oc;
+      b.s = (uint8_t)s;
+      obmc_block(out + (size_t)b.y0 * pw + b.x0, pw, pred, buf, refs, b);
+      __syncthreads();   // pred / buf are the next leaf's
+    }
+  }
 }
 
 }  // namespace mc
@@ -468,6 +619,16 @@ int daala_b200_mc_predict1fmv_batch(const uint8_t* ref, int ref_stride, uint8_t*
                                     const daala_b200_match_job* jobs, int count, int log_yblk, void* stream) {
   if (count <= 0) return 0;
   k_predict1fmv<<<count, kThreads, 0, (cudaStream_t)stream>>>(ref, ref_stride, dst, dst_pitch, jobs, log_yblk);
+  return (int)cudaGetLastError();
+}
+
+int daala_b200_launch_mc_leaves(const daala_b200_mc_batch* b, int grid, cudaStream_t stream) {
+  k_mc_leaves<<<grid, 256, 0, stream>>>(*b);
+  return (int)cudaGetLastError();
+}
+
+int daala_b200_launch_mc_obmc(const daala_b200_mc_batch* b, int grid, cudaStream_t stream) {
+  k_mc_obmc<<<grid, kThreads, 0, stream>>>(*b);
   return (int)cudaGetLastError();
 }
 

@@ -3,14 +3,16 @@ ctypes binding + numpy marshalling.  The engine is the batched equivalent of od_
 (reference src/encode.c:2539) for keyframes without the entropy coder: u8 planes + block-size maps in,
 reconstruction + PVQ symbols out, everything in between on the GPU (work lists included).  Created with
 inter=1 the same engine codes P-frame residuals: the motion-compensated prediction planes are a second input
-(`pred=`), and each block's scalar-quantised DC index is a further output.
+(`pred=`), and each block's scalar-quantised DC index is a further output.  With inter_mc=1 the engine makes
+that prediction itself from each frame's MV grid and its GOLD / PREV pictures in a pool of reference pictures
+(`refs=`, `ref_slot=`, `mv_grid=`), as od_state_mc_predict does, and returns it as `pred0..2`.
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
 
 import numpy as np
 
-from . import _native, pvq
+from . import _native, mvgrid, pvq
 from .frame import Geometry
 
 c_int, c_ll, c_void_p = ctypes.c_int, ctypes.c_longlong, ctypes.c_void_p
@@ -18,7 +20,7 @@ c_int, c_ll, c_void_p = ctypes.c_int, ctypes.c_longlong, ctypes.c_void_p
 PH_LISTS, PH_FORWARD, PH_PVQ_LUMA, PH_INVERSE, PH_PVQ_CHROMA = 1, 2, 4, 8, 16
 PH_PVQ, PH_ALL, PH_SEARCH_ONLY = 20, 31, 64
 CNT = dict(n_luma=0, n_chroma=1, luma_coefs=2, chroma_coefs=3, items_l=4, items_c=7,
-           total_hi=14, n_heads=15, n_heads0=16, error=17)
+           total_hi=14, n_heads=15, n_heads0=16, error=17, mc_bad_ref=19, mc_beyond=20)
 
 
 class Config(ctypes.Structure):
@@ -27,7 +29,7 @@ class Config(ctypes.Structure):
                 ("qm", c_void_p), ("qm_inv", c_void_p), ("sb_row0", c_int), ("sb_rows", c_int),
                 ("max_blocks_div", c_int), ("persist_ctas_per_sm", c_int), ("split_free", c_int), ("dering", c_int), ("noref_prepass", c_int), ("level_chains", c_int), ("stream", c_void_p),
                 ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
-                ("symbol_stream", c_int), ("inter", c_int)]
+                ("symbol_stream", c_int), ("inter", c_int), ("inter_mc", c_int), ("mc_refs", c_int)]
 
 
 class Totals(ctypes.Structure):
@@ -42,7 +44,9 @@ class IO(ctypes.Structure):
                 ("counts", c_void_p), ("dering_level_out", c_void_p),
                 ("sym_index", c_void_p), ("sym_index_cap", c_ll), ("sym_blocks", c_void_p), ("sym_blocks_cap", c_ll),
                 ("sym_bands", c_void_p), ("sym_bands_cap", c_ll), ("sym_pulses", c_void_p), ("sym_pulses_cap", c_ll),
-                ("pred_pixels", c_void_p * 3), ("luma_dc", c_void_p), ("chroma_dc", c_void_p)]
+                ("pred_pixels", c_void_p * 3), ("luma_dc", c_void_p), ("chroma_dc", c_void_p),
+                ("ref_pixels", c_void_p * 3), ("nrefs", c_int), ("ref_slot", c_void_p), ("mv_grid", c_void_p),
+                ("pred_pixels_out", c_void_p * 3)]
 
 
 class SymBounds(ctypes.Structure):
@@ -59,7 +63,8 @@ class Buffers(ctypes.Structure):
                 ("luma_skip_diff", c_void_p), ("chroma_skip_diff", c_void_p), ("chroma_flip", c_void_p),
                 ("max_luma_blocks", c_int), ("max_chroma_blocks", c_int), ("stream", c_void_p),
                 ("bytes_allocated", c_ll), ("pred_pixels", c_void_p * 3), ("pred_coeffs", c_void_p * 3),
-                ("luma_heads_raw", c_void_p), ("luma_head_bin", c_void_p)]
+                ("luma_heads_raw", c_void_p), ("luma_head_bin", c_void_p), ("ref_pixels", c_void_p * 3),
+                ("ref_slot", c_void_p), ("mv_grid", c_void_p), ("mc_refs", c_int)]
 
 
 def _bind():
@@ -115,7 +120,7 @@ class KeyframeEngine:
 
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
                  qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=0, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
-                 qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0):
+                 qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0, inter_mc=0, mc_refs=0):
         self.L = _bind()
         self.geom, self.F = geom, nframes
         if qm is None:
@@ -148,6 +153,9 @@ class KeyframeEngine:
         self.symbol_stream = int(symbol_stream)
         cfg.inter = int(inter)
         self.inter = int(inter)
+        cfg.inter_mc, cfg.mc_refs = int(inter_mc), int(mc_refs)
+        self.inter_mc = int(inter_mc)
+        self.nrefs = 0
         self.kf = self.L.daala_b200_kf_create(ctypes.byref(cfg))
         if not self.kf:
             raise RuntimeError("daala_b200_kf_create failed (refused configuration, no CUDA device, or out of memory): %s"
@@ -221,8 +229,25 @@ class KeyframeEngine:
         a[...] = levels
 
     def _check_pred(self, pred):
-        if bool(self.inter) != (pred is not None):
-            raise ValueError("pred= planes are required by an inter engine and refused by a keyframe engine")
+        if bool(self.inter and not self.inter_mc) != (pred is not None):
+            raise ValueError("pred= planes are required by an inter engine and refused by a keyframe engine "
+                             "and by an inter_mc engine")
+
+    def stage_mc(self, refs, ref_slot, mv_grid):
+        """Copies one batch's prediction inputs (inter_mc engines) into the host buffers.  refs: per plane an
+        array [nrefs, h, w] u8 (frame-sized reference pictures); ref_slot: [F, 2] pool slots of each frame's GOLD
+        and PREV picture; mv_grid: [F, nvsb*8 + 1, nhsb*8 + 1] mvgrid.MV_PT_DTYPE (mvgrid.pack)."""
+        g = self.geom
+        if not self.inter_mc or refs is None or ref_slot is None or mv_grid is None:
+            raise ValueError("refs=, ref_slot= and mv_grid= go with an inter_mc engine, and it needs all three")
+        self.nrefs = int(np.shape(refs[0])[0])
+        for p in range(3):
+            a = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8)
+            a[...] = refs[p]
+        a = self._arr("slot", (self.F, 2), np.int32)
+        a[...] = ref_slot
+        a = self._arr("grid", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1), mvgrid.MV_PT_DTYPE)
+        a[...] = mv_grid
 
     def stage_inputs(self, planes, bsize, pred=None):
         """Copies one batch into the engine's (pinned) host input buffers.  planes: per plane an array
@@ -233,7 +258,7 @@ class KeyframeEngine:
         for p in range(3):
             a = self._arr("in%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
             a[...] = planes[p]
-            if self.inter:
+            if self.inter and not self.inter_mc:
                 a = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
                 a[...] = pred[p]
         b = self._arr("bsize", (self.F,) + tuple(g.bsize_shape), np.uint8)
@@ -280,9 +305,18 @@ class KeyframeEngine:
             for k in ("luma_blocks", "chroma_blocks", "luma_res", "chroma_res", "luma_y16", "chroma_y16",
                       "luma_skip_diff", "chroma_skip_diff", "chroma_flip"):
                 setattr(io, k, out[k].ctypes.data)
-        if self.inter:
+        if self.inter_mc:
             for p in range(3):
-                io.pred_pixels[p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8).ctypes.data
+                io.ref_pixels[p] = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8).ctypes.data
+                out["pred%d" % p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
+                io.pred_pixels_out[p] = out["pred%d" % p].ctypes.data
+            io.nrefs = self.nrefs
+            io.ref_slot = self._arr("slot", (self.F, 2), np.int32).ctypes.data
+            io.mv_grid = self._arr("grid", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1), mvgrid.MV_PT_DTYPE).ctypes.data
+        if self.inter:
+            if not self.inter_mc:
+                for p in range(3):
+                    io.pred_pixels[p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8).ctypes.data
             out["luma_dc"] = self._arr("ld", (int(t.n_luma),), np.int32)
             out["chroma_dc"] = self._arr("cd", (int(t.n_chroma),), np.int32)
             io.luma_dc, io.chroma_dc = out["luma_dc"].ctypes.data, out["chroma_dc"].ctypes.data
@@ -304,8 +338,11 @@ class KeyframeEngine:
                 setattr(io, k, out[k].ctypes.data)
                 setattr(io, k + "_cap", int(cap))
         self._io, self._out = io, out
-        self.h2d_bytes = (sum(int(np.prod(g.plane_shape(p))) for p in range(3)) * self.F * (2 if self.inter else 1)
-                          + int(np.prod(g.bsize_shape)) * self.F)
+        px = sum(int(np.prod(g.plane_shape(p))) for p in range(3))
+        self.h2d_bytes = px * self.F * (2 if self.inter and not self.inter_mc else 1) + int(np.prod(g.bsize_shape)) * self.F
+        if self.inter_mc:
+            self.h2d_bytes += (px * self.nrefs + 8 * self.F
+                               + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * mvgrid.MV_PT_DTYPE.itemsize)
         return out
 
     def submit(self):
@@ -322,10 +359,16 @@ class KeyframeEngine:
         idx = self._out["sym_index"]
         return idx.nbytes + int(idx[:, 1].sum()) * sym.BLOCK_DTYPE.itemsize + int(idx[:, 3].sum()) * 8 + int(idx[:, 5].sum())
 
-    def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None, pred=None):
+    def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None, pred=None, refs=None,
+               ref_slot=None, mv_grid=None):
         """One batch end to end through the C ABI with host buffers; returns the result arrays (views of
-        the engine's host buffers: copy what must survive the next call).  pred: see stage_inputs."""
+        the engine's host buffers: copy what must survive the next call).  pred: see stage_inputs; refs, ref_slot,
+        mv_grid (inter_mc engines, which also return the prediction as pred0..2): see stage_mc.  Raises when the
+        batch exceeded the block capacity, or (inter_mc) when a used vertex names a picture other than GOLD / PREV
+        or a vector reaches past the reference's edge extension: the reference encoder's result is undefined there."""
         self.stage_inputs(planes, bsize, pred)
+        if self.inter_mc or refs is not None or ref_slot is not None or mv_grid is not None:
+            self.stage_mc(refs, ref_slot, mv_grid)
         if self.dering == 1:
             self.stage_dering_levels(dering_levels)
         self.prepare_io(symbols, recon, stream)
@@ -333,6 +376,11 @@ class KeyframeEngine:
         out = self.wait()
         if int(out["counts"][CNT["error"]]):
             raise RuntimeError("keyframe engine: block capacity exceeded (max_blocks_div too large)")
+        if self.inter_mc:
+            bad, beyond = int(out["counts"][CNT["mc_bad_ref"]]), int(out["counts"][CNT["mc_beyond"]])
+            if bad or beyond:
+                raise RuntimeError("keyframe engine: MV grid outside the reference's definition: %d leaf corners with a "
+                                   "ref other than GOLD / PREV, %d corner windows past the edge extension" % (bad, beyond))
         return out
 
     # --- device-resident use -------------------------------------------------------------------
@@ -350,7 +398,7 @@ class KeyframeEngine:
         g = self.geom
         self._check_pred(pred)
         for p in range(3):
-            for dst, src in ((self.buf.pixels[p], planes[p]),) + (((self.buf.pred_pixels[p], pred[p]),) if self.inter else ()):
+            for dst, src in ((self.buf.pixels[p], planes[p]),) + (((self.buf.pred_pixels[p], pred[p]),) if pred is not None else ()):
                 a = np.ascontiguousarray(src, np.uint8)
                 assert a.shape == (self.F,) + g.plane_shape(p)
                 self._check(self.L.daala_b200_device_copy(dst, a.ctypes.data, a.nbytes, 0), "upload")

@@ -19,6 +19,9 @@ _DY = _D[0:4]
 _SETUP_DX = [[9, 1, 9, 1], [13, 13, 1, 1], [18, 1, 18, 1], [5, 5, 1, 1]]   # offsets into OD_VERT_D
 _SETUP_DY = [[4, 4, 0, 0], [8, 0, 8, 0], [12, 12, 0, 0], [17, 0, 17, 0]]   # offsets into OD_VERT_DY (= D)
 LOG_MVB_DELTA0 = 3   # OD_LOG_MVBSIZE_MAX - OD_LOG_MVBSIZE_MIN
+# daala_b200_mv_pt (include/daala_b200.h): one vertex as od_mv_grid_pt holds it; ref 0 = OD_FRAME_GOLD, 1 = _PREV
+MV_PT_DTYPE = np.dtype([("mv", "<i4", 2), ("valid", "u1"), ("ref", "u1"), ("pad_", "u1", 2)])
+assert MV_PT_DTYPE.itemsize == 12
 
 
 def _div_pow2_re(x, shift):
@@ -66,17 +69,21 @@ def block_list(valid, mv, xdec=0):
     return blocks_for(*leaves(valid), mv, xdec)
 
 
-def blocks_for(vx, vy, l, oc, s, mv, xdec=0):
-    """Block records of given MV blocks (vertex position, log size, outside corner, split state): what
-    od_state_pred_block_from_setup (src/state.c:627) derives for one plane."""
+def corners(vx, vy, l, oc, s):
+    """The grid vertices (gx, gy) of the four corners of given MV blocks, in od_mc_predict's rotational order."""
     vx, vy, l, oc, s = (np.asarray(a, np.int64) for a in (vx, vy, l, oc, s))
     d = np.array(_D)
     sdx = np.array(_SETUP_DX)[oc, s]   # offsets
     sdy = np.array(_SETUP_DY)[oc, s]
+    return [(vx + (d[sdx + k] << l), vy + (d[sdy + k] << l)) for k in range(4)]
+
+
+def blocks_for(vx, vy, l, oc, s, mv, xdec=0):
+    """Block records of given MV blocks (vertex position, log size, outside corner, split state): what
+    od_state_pred_block_from_setup (src/state.c:627) derives for one plane."""
+    vx, vy, l, oc, s = (np.asarray(a, np.int64) for a in (vx, vy, l, oc, s))
     blocks = np.zeros(len(vx), mc.MC_BLOCK_DTYPE)
-    for k in range(4):
-        gx = vx + (d[sdx + k] << l)
-        gy = vy + (d[sdy + k] << l)
+    for k, (gx, gy) in enumerate(corners(vx, vy, l, oc, s)):
         blocks["mvx"][:, k] = _div_pow2_re(mv[gy, gx, 0].astype(np.int64), xdec)
         blocks["mvy"][:, k] = _div_pow2_re(mv[gy, gx, 1].astype(np.int64), xdec)
     blocks["x0"] = vx << (3 - xdec)
@@ -84,3 +91,19 @@ def blocks_for(vx, vy, l, oc, s, mv, xdec=0):
     blocks["log_xblk"] = blocks["log_yblk"] = l + 3 - xdec
     blocks["oc"], blocks["s"] = oc, s
     return blocks
+
+
+def pack(valid, mv, ref):
+    """MV_PT_DTYPE records of grids given as `valid` [..., nv+1, nh+1] (bool / 0-1), `mv` [..., nv+1, nh+1, 2]
+    (1/8 luma pixel) and `ref` (0 = GOLD, 1 = PREV), any leading (frame) dimensions."""
+    valid = np.asarray(valid)
+    out = np.zeros(valid.shape, MV_PT_DTYPE)
+    out["valid"] = valid
+    out["mv"] = mv
+    out["ref"] = ref
+    return out
+
+
+def unpack(grid):
+    """(valid, mv, ref) arrays of MV_PT_DTYPE records: the inverse of pack."""
+    return grid["valid"].copy(), grid["mv"].copy(), grid["ref"].copy()

@@ -87,3 +87,23 @@ def block_size_map(geom, mode="mixed", seed=7):
         for sx in range(0, bw, 8):
             fill(sy, sx, 4)
     return m
+
+
+def mv_grid(geom, seed=0, p_split=(0.6, 0.5, 0.4), p_gold=0.5, umv=32):
+    """A seeded MV grid for one P frame of `geom`: (valid, mv, ref) with (nvsb*8 + 1) x (nhsb*8 + 1) vertices.
+    The corners of every 64x64 MV block are valid; a vertex that is the centre of a 64, 32 or 16 block is valid
+    with probability p_split[0], [1], [2] (every split level occurs), the other vertices with 1/2.  Vectors are
+    uniform in +-umv luma pixels (od_mv_est keeps them within OD_UMV_CLAMP = 32, src/mcenc.c:2467-2478) in 1/8
+    pel; ref is GOLD (0) with probability p_gold, else PREV (1)."""
+    rng = np.random.default_rng(seed)
+    nv, nh = geom.nvsb * 8 + 1, geom.nhsb * 8 + 1
+    vy, vx = np.mgrid[0:nv, 0:nh]
+    p = np.full((nv, nh), 0.5)
+    for lvl, step in enumerate((8, 4, 2)):
+        centre = (vx % step == step // 2) & (vy % step == step // 2)
+        p[centre] = p_split[lvl]
+    valid = rng.random((nv, nh)) < p
+    valid[(vx % 8 == 0) & (vy % 8 == 0)] = True
+    mv = rng.integers(-umv * 8, umv * 8 + 1, size=(nv, nh, 2)).astype(np.int32)
+    ref = (rng.random((nv, nh)) >= p_gold).astype(np.uint8)
+    return valid.astype(np.uint8), mv, ref

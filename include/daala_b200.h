@@ -483,7 +483,27 @@ typedef struct daala_b200_kf_config {
                                   the transformed prediction (od_init_skipped_coeffs for inter frames).
                                   Not defined, and refused by daala_b200_kf_create, together with dering,
                                   symbol_stream, noref_prepass, level_chains or a row shard (sb_rows > 0) */
+  int inter_mc;                /* 0 (default): with inter, the prediction planes are the host input pred_pixels.
+                                  1: the engine makes the prediction itself, as od_state_mc_predict does
+                                  (reference src/state.c:932), from each frame's MV grid
+                                  (daala_b200_kf_io.mv_grid) and its GOLD and PREV pictures in a pool of reference
+                                  pictures (daala_b200_kf_io.ref_pixels / ref_slot).  Two steps inside the graph: the
+                                  leaves of od_state_pred_block's split recursion per 64x64 MV block (work-list
+                                  phase) and the OBMC prediction of every leaf in all three planes (forward phase,
+                                  before the transforms).  Reference pixels outside the picture are read at the
+                                  nearest edge pixel, which is the reference's edge extension inside its 64 / 32
+                                  pixels of padding.  Requires inter = 1; refused by daala_b200_kf_create
+                                  otherwise */
+  int mc_refs;                 /* inter_mc: capacity of the reference-picture pool in pictures; 0 = 2 * nframes */
 } daala_b200_kf_config;
+
+/* One vertex of a P frame's MV grid, as od_mv_grid_pt (reference src/mc.h:73-84) holds it after od_mv_est. */
+typedef struct daala_b200_mv_pt {  /* 12 bytes */
+  int32_t mv[2];           /* x, y in 1/8 luma pixel */
+  uint8_t valid;           /* the vertex is coded: the MV block with this vertex at its centre is split */
+  uint8_t ref;             /* picture the vector points into: 0 = OD_FRAME_GOLD, 1 = OD_FRAME_PREV */
+  uint8_t pad_[2];
+} daala_b200_mv_pt;
 
 typedef struct daala_b200_kf_totals {
   long long n_luma, luma_coefs, n_chroma, chroma_coefs;
@@ -558,6 +578,14 @@ typedef struct daala_b200_kf_io {
   const uint8_t *pred_pixels[3];        /* motion-compensated prediction planes, shapes and padding of `pixels` */
   int32_t *luma_dc, *chroma_dc;         /* [n_blocks]: the scalar-quantised DC index qdc of each block (keyframes code
                                            DC in the Haar pyramid instead), block order of luma_res / chroma_res */
+  /* config.inter_mc only (required there except pred_pixels_out; pred_pixels must then be NULL). */
+  const uint8_t *ref_pixels[3];         /* pool of nrefs reference pictures [nrefs][plane_h][plane_w] u8: each the
+                                           frame-sized area of one of state->ref_imgs, without the edge extension */
+  int nrefs;                            /* pictures in the pool, 1..mc_refs */
+  const int32_t *ref_slot;              /* [nframes][2]: pool slots of each frame's GOLD and PREV pictures (equal
+                                           when the frame predicts from one picture) */
+  const daala_b200_mv_pt *mv_grid;      /* [nframes][nvsb*8 + 1][nhsb*8 + 1]: each frame's state->mv_grid */
+  uint8_t *pred_pixels_out[3];          /* optional: the prediction planes the engine made, layout of pixels */
 } daala_b200_kf_io;
 
 typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, device-resident callers) */
@@ -586,6 +614,10 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
   int32_t *pred_coeffs[3];              /* layout of pixels / coeffs); NULL otherwise */
   uint32_t *luma_heads_raw;             /* luma_heads in the order the dependency builder found them, and the */
   int32_t *luma_head_bin;               /* weight bin of each: 12287 - min(chain length x class cost, 12287) */
+  uint8_t *ref_pixels[3];               /* config.inter_mc: the reference-picture pool ([mc_refs][plane_h][plane_w]), */
+  int32_t *ref_slot;                    /* the slot map ([nframes][2]) and the MV grids ([nframes][nvsb*8 + 1] */
+  daala_b200_mv_pt *mv_grid;            /* [nhsb*8 + 1]) the prediction step reads; NULL otherwise */
+  int mc_refs;                          /* pictures the pool holds (0 without inter_mc) */
 } daala_b200_kf_buffers;
 
 #define DAALA_B200_KF_LISTS 1
@@ -619,7 +651,11 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    luma or chroma blocks than the engine's capacity (see max_blocks_div) returns cudaErrorInvalidValue before
    anything is copied or launched; so does a request for symbol stream outputs from an engine created without
    symbol_stream, a stream capacity below daala_b200_kf_symbol_bounds, a stream buffer that is not pinned host
-   memory, or (config.inter) a NULL pred_pixels plane, luma_dc or chroma_dc. */
+   memory, or (config.inter) a NULL pred_pixels plane, luma_dc or chroma_dc.  With config.inter_mc it refuses, the same
+   way, a NULL mv_grid, ref_pixels plane or ref_slot, pred_pixels given, nrefs outside [1, mc_refs] and a slot outside
+   [0, nrefs).  The step counts in `counts` the leaf corners whose vertex has a ref other than 0 or 1 (counts[19]) and
+   the corner windows (with the 6-tap filter's apron of -2..+3 pixels) that reach more than 64 luma / 32 chroma
+   pixels outside the plane (counts[20]), where the reference encoder's result is undefined. */
 int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
 int daala_b200_kf_wait(daala_b200_kf *kf);
 int daala_b200_kf_encode(daala_b200_kf *kf, const daala_b200_kf_io *io);   /* submit + wait */
