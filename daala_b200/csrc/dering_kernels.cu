@@ -127,10 +127,12 @@ __device__ __forceinline__ int lo16(uint32_t w) { return (int)(int16_t)(w & 0xff
 __device__ __forceinline__ int hi16(uint32_t w) { return (int)w >> 16; }
 
 // frames of a batch: blockIdx.z, element pitches between consecutive frames (all zero for a single plane);
-// y8 (nullable): store the u8 reconstruction there (pitch y, stride ystride) instead of the int16 plane y
+// y8 (nullable): store the u8 reconstruction there (pitch y, stride ystride) instead of the int16 plane y;
+// skip: pitch of the skip map (0: one map for every frame)
 struct BatchPitch {
   long long y, x, dir, thr;
   uint8_t* y8;
+  long long skip;
 };
 
 __global__ void __launch_bounds__(256, 4) k_dering_sb(const __grid_constant__ daala_b200_dering_params p,
@@ -241,7 +243,7 @@ __global__ void __launch_bounds__(256, 4) k_dering_sb(const __grid_constant__ da
     }
     // per-plane skip flags, one per 4x4 block of THIS plane: 16 >> xdec flags per superblock side
     // (call site src/encode.c:2789-2791)
-    const uint8_t* sk = p.bskip + (size_t)(sby * (16 >> p.xdec)) * p.skip_stride + sbx * (16 >> p.xdec);
+    const uint8_t* sk = p.bskip + z * bp.skip + (size_t)(sby * (16 >> p.xdec)) * p.skip_stride + sbx * (16 >> p.xdec);
     bool all = true;
     for (int i = v0; i < v1; i++)
       for (int j = u0; j < u1; j++) all = all && sk[(ptrdiff_t)(((by << 1) >> p.xdec) + i) * p.skip_stride + ((bx << 1) >> p.xdec) + j];
@@ -306,7 +308,7 @@ extern "C" int daala_b200_dering_plane(const daala_b200_dering_params* prm, void
   // not in place: a superblock's apron would read its neighbours' filtered output
   if (!prm->x || !prm->y || (const void*)prm->x == (const void*)prm->y) return (int)cudaErrorInvalidValue;
   dim3 grid(prm->nhsb, prm->nvsb);
-  daala_b200::dering::BatchPitch bp = {0, 0, 0, 0, nullptr};
+  daala_b200::dering::BatchPitch bp = {0, 0, 0, 0, nullptr, 0};
   daala_b200::dering::k_dering_sb<<<grid, 256, 0, (cudaStream_t)stream>>>(*prm, bp);
   return (int)cudaGetLastError();
 }
@@ -320,7 +322,20 @@ extern "C" int daala_b200_dering_plane_batch(const daala_b200_dering_params* prm
   if (!prm || nframes < 1 || prm->nhsb < 1 || prm->nvsb < 1 || prm->xdec < 0 || prm->xdec > 1) return (int)cudaErrorInvalidValue;
   if (!prm->x || (!prm->y && !y8) || (const void*)prm->x == (const void*)prm->y) return (int)cudaErrorInvalidValue;
   dim3 grid(prm->nhsb, prm->nvsb, nframes);
-  daala_b200::dering::BatchPitch bp = {y_pitch, x_pitch, dir_pitch, thr_pitch, y8};
+  daala_b200::dering::BatchPitch bp = {y_pitch, x_pitch, dir_pitch, thr_pitch, y8, 0};
+  daala_b200::dering::k_dering_sb<<<grid, 256, 0, (cudaStream_t)stream>>>(*prm, bp);
+  return (int)cudaGetLastError();
+}
+
+// The same with a skip map per frame, skip_pitch bytes apart (internal: the P-frame finishing pass, whose frames each
+// have their own state->bskip).
+extern "C" int daala_b200_dering_plane_batch_skip(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
+                                                  long long x_pitch, long long dir_pitch, long long thr_pitch,
+                                                  long long skip_pitch, uint8_t* y8, void* stream) {
+  if (!prm || nframes < 1 || prm->nhsb < 1 || prm->nvsb < 1 || prm->xdec < 0 || prm->xdec > 1) return (int)cudaErrorInvalidValue;
+  if (!prm->x || (!prm->y && !y8) || (const void*)prm->x == (const void*)prm->y) return (int)cudaErrorInvalidValue;
+  dim3 grid(prm->nhsb, prm->nvsb, nframes);
+  daala_b200::dering::BatchPitch bp = {y_pitch, x_pitch, dir_pitch, thr_pitch, y8, skip_pitch};
   daala_b200::dering::k_dering_sb<<<grid, 256, 0, (cudaStream_t)stream>>>(*prm, bp);
   return (int)cudaGetLastError();
 }

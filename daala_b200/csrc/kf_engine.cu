@@ -521,6 +521,7 @@ struct Stage {
   const int32_t* cfl_plane;        // chroma: prediction plane (chroma geometry), else NULL
   long long cfl_pitch;
   int cfl_stride;
+  int32_t* dc_resid;               // config.inter_finish: per block in[0] - ref[0], else NULL
 #ifdef DAALA_B200_CHAIN_TRACE
   struct ChainTraceRec* trace;     // luma: one record per item k_pvq_persist<true> runs, up to trace_cap
   int trace_cap;
@@ -1127,6 +1128,7 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
         }
         prm.out[b.coef_off] = dst[0] = qdc * dc_quant + r;
         prm.res_dc[blk] = qdc;
+        if (S.dc_resid) S.dc_resid[blk] = diff;
       }
     }
     if (ln >= 5) {
@@ -1150,16 +1152,96 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
 // result is an input of the hot path): etmp = ctmp after the SB-edge postfilter, od_dering of every superblock
 // with threshold = OD_DERING_GAIN_TABLE[level] * quantizer^0.84182 (* 0.6 on chroma), od_coeff_to_ref_plane
 // (the deringing kernel stores the u8 reconstruction itself).
-// thr[pl][f][sb] = table[pl][level[f][sb]]
+// thr[pl][f][sb] = table[pl][level[f][sb]].  P-frame finishing pass: `coded` (else NULL) flags the superblocks with a
+// coded 4x4 luma unit; the others are forced to level 0 (src/encode.c:2724-2738), and the level applied goes to
+// `applied`.
 __global__ void k_dering_thresholds(const uint8_t* __restrict__ level, int32_t* __restrict__ thr_luma,
-                                    int32_t* __restrict__ thr_chroma, int n, int4 tl_lo, int2 tl_hi, int4 tc_lo, int2 tc_hi) {
+                                    int32_t* __restrict__ thr_chroma, int n, int4 tl_lo, int2 tl_hi, int4 tc_lo, int2 tc_hi,
+                                    const uint8_t* __restrict__ coded = nullptr, uint8_t* __restrict__ applied = nullptr) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int tl[6] = {tl_lo.x, tl_lo.y, tl_lo.z, tl_lo.w, tl_hi.x, tl_hi.y};
   const int tc[6] = {tc_lo.x, tc_lo.y, tc_lo.z, tc_lo.w, tc_hi.x, tc_hi.y};
-  const int g = level[i] < 6 ? level[i] : 5;
+  int g = level[i] < 6 ? level[i] : 5;
+  if (coded) {
+    if (!coded[i]) g = 0;
+    applied[i] = (uint8_t)g;
+  }
   thr_luma[i] = tl[g];
   thr_chroma[i] = tc[g];
+}
+
+// ---- P-frame finishing pass (config.inter_finish) ----------------------------------------------------------------
+// The host coder's per-block decisions applied to the coefficients of the last step, in a plane of their own (the
+// step's d / md stay as they are), and the skip map they imply.  Both kernels walk the luma list, then the chroma list.
+struct Fin {
+  const daala_b200_pvq_block* blocks[2];   // luma, chroma
+  const uint8_t* skip[2];                  // per block: 0 or 1
+  const int32_t* dc[2];                    // per block: the final DC index
+  const int32_t* cnt;
+  int max_blocks[2];
+  const int32_t* d[3];                     // the step's `d` and `md` planes
+  const int32_t* md[3];
+  int32_t* out[3];                         // patched planes
+  long long plane_pitch[3];
+  int plane_stride[3];
+  uint8_t* bskip[3];                       // [F][plane_h / 4][skip_stride]
+  long long skip_pitch[3];
+  int skip_stride;                         // state->skip_stride = nhsb * 16
+  uint8_t* coded;                          // [F][nvsb][nhsb]: a luma 4x4 unit of the superblock is coded (preset 0)
+  int nhsb, nvsb;
+  int q0;
+  uint8_t pvq_qm_q4[3][32];
+};
+
+// block i of the two lists together (luma first), or false past their end
+__device__ __forceinline__ bool fin_block(const Fin& P, int i, int* list, int* blk) {
+  const int nl = min(P.cnt[kNLuma], P.max_blocks[0]), nc = min(P.cnt[kNChroma], P.max_blocks[1]);
+  if (i >= nl + nc) return false;
+  *list = i >= nl;
+  *blk = i >= nl ? i - nl : i;
+  return true;
+}
+
+// One warp per block.  skip = 0: the step's coefficients; skip = 1: md over the whole block (AC = prediction,
+// src/pvq_encoder.c:975; the late skip's d = md, src/encode.c:1444-1448); either way DC = md[0] + dc * dc_quant
+// (src/encode.c:1373-1374 with the band-0 quantiser of :1333-1334).
+__global__ void __launch_bounds__(256) k_fin_patch(const __grid_constant__ Fin P) {
+  const int lane = threadIdx.x & 31;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  int list, blk;
+  for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; fin_block(P, i, &list, &blk); i += nwarps) {
+    const daala_b200_pvq_block b = P.blocks[list][blk];
+    const int ln = b.bs + 2, nn = 1 << ln;
+    const int stride = P.plane_stride[b.pli];
+    const size_t o = b.frame * P.plane_pitch[b.pli] + (size_t)b.y0 * stride + b.x0;
+    const int32_t* src = (P.skip[list][blk] ? P.md[b.pli] : P.d[b.pli]) + o;
+    const int32_t* mdp = P.md[b.pli] + o;
+    int32_t* dst = P.out[b.pli] + o;
+    int dc_quant = (P.q0 * P.pvq_qm_q4[b.pli][b.bs * (b.bs + 1)]) >> 4;
+    if (dc_quant < 1) dc_quant = 1;
+    const int32_t dc0 = mdp[0] + P.dc[list][blk] * dc_quant;
+    for (int k = lane; k < nn * nn; k += 32) {
+      const size_t at = (size_t)(k >> ln) * stride + (k & (nn - 1));
+      dst[at] = k ? src[at] : dc0;
+    }
+  }
+}
+
+// One warp per block: bskip = skip && dc == 0 over the block's 4x4 units (src/encode.c:1690-1691, :1821-1825), and
+// the coded flag of the superblock of a luma block that is not skipped.
+__global__ void __launch_bounds__(256) k_fin_skip_map(const __grid_constant__ Fin P) {
+  const int lane = threadIdx.x & 31;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  int list, blk;
+  for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; fin_block(P, i, &list, &blk); i += nwarps) {
+    const daala_b200_pvq_block b = P.blocks[list][blk];
+    const uint8_t s = P.skip[list][blk] && P.dc[list][blk] == 0;
+    const int nu = 1 << b.bs;   // 4x4 units per side
+    uint8_t* m = P.bskip[b.pli] + b.frame * P.skip_pitch[b.pli] + (size_t)(b.y0 >> 2) * P.skip_stride + (b.x0 >> 2);
+    for (int k = lane; k < nu * nu; k += 32) m[(size_t)(k >> b.bs) * P.skip_stride + (k & (nu - 1))] = s;
+    if (lane == 0 && b.pli == 0 && !s) P.coded[((size_t)b.frame * P.nvsb + (b.y0 >> 6)) * P.nhsb + (b.x0 >> 6)] = 1;
+  }
 }
 
 // ---- symbol stream (optional, config.symbol_stream) -------------------------------------------------------
@@ -1480,6 +1562,9 @@ extern "C" int daala_b200_launch_sb_postfilter_store(const daala_b200_frame* prm
 extern "C" int daala_b200_dering_plane_batch(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
                                              long long x_pitch, long long dir_pitch, long long thr_pitch, uint8_t* y8,
                                              void* stream);
+extern "C" int daala_b200_dering_plane_batch_skip(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
+                                                  long long x_pitch, long long dir_pitch, long long thr_pitch,
+                                                  long long skip_pitch, uint8_t* y8, void* stream);
 
 struct daala_b200_kf {
   daala_b200_kf_config cfg;
@@ -1535,6 +1620,23 @@ struct daala_b200_kf {
   uint32_t* mc_leaves;
   int32_t* mc_nleaves;
   daala_b200_mc_batch mc;
+  // cfg.inter_finish: the finishing pass's inputs (decisions per block, levels), its planes (patched coefficients,
+  // inverted in place; etmp; the reconstruction), the skip maps, the superblock flags, and its own CUDA graph
+  uint8_t* fin_skip[2];
+  int32_t* fin_dc[2];
+  int32_t* dc_resid[2];
+  int32_t* fin_coeffs[3];
+  int16_t* fin_post16[3];
+  uint8_t* fin_pixels[3];
+  uint8_t* fin_bskip[3];
+  uint8_t *fin_level_in, *fin_level, *fin_coded;
+  Fin fin;
+  cudaGraph_t fin_graph;
+  cudaGraphExec_t fin_exec;
+  bool fin_captured;
+  int fin_dc_limit;                // largest |dc| finish accepts: DAALA_B200_KF_FINISH_DC_LIMIT / the largest dc_quant
+  bool have_step;                  // a step has been submitted; last_tot are its totals
+  daala_b200_kf_totals last_tot;
   size_t bytes_allocated;
   size_t chain_cap;                // entries of the chain queue (heads / ring)
   int sms;
@@ -1880,6 +1982,8 @@ static int kf_alloc(daala_b200_kf* kf) {
       KF_CHECK(dalloc(kf, &kf->dering_cand, nsb * 4096));
       KF_CHECK(dalloc(kf, &kf->dering_dist, nsb * 6));
     }
+  }
+  {
     // thresholds per level: (int)(OD_DERING_GAIN_TABLE[gi] * pow(quantizer, 0.84182) * (luma ? 1 : 0.6)), src/encode.c:2697,2822
     const double gain[6] = {0, 0.5, 0.707, 1, 1.41, 2};
     const double base = pow((double)kf->cfg.q0, 0.84182);
@@ -1887,6 +1991,56 @@ static int kf_alloc(daala_b200_kf* kf) {
       kf->dering_tbl[0][g] = (int)(gain[g] * base * 1);
       kf->dering_tbl[1][g] = (int)(gain[g] * base * 0.6);
     }
+  }
+  if (kf->cfg.inter_finish) {
+    const size_t nsb = (size_t)F * kf->nhsb * kf->nvsb;
+    Fin& P = kf->fin;
+    memset(&P, 0, sizeof(P));
+    for (int c = 0; c < 2; c++) {
+      const Stage& S = c ? kf->chroma : kf->luma;
+      KF_CHECK(dalloc(kf, &kf->fin_skip[c], (size_t)S.max_blocks));
+      KF_CHECK(dalloc(kf, &kf->fin_dc[c], (size_t)S.max_blocks));
+      KF_CHECK(dalloc(kf, &kf->dc_resid[c], (size_t)S.max_blocks));
+      (c ? kf->chroma : kf->luma).dc_resid = kf->dc_resid[c];
+      P.blocks[c] = S.prm.blocks;
+      P.skip[c] = kf->fin_skip[c];
+      P.dc[c] = kf->fin_dc[c];
+      P.max_blocks[c] = S.max_blocks;
+    }
+    P.cnt = L.cnt;
+    P.skip_stride = kf->nhsb * 16;
+    for (int p = 0; p < 3; p++) {
+      const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
+      KF_CHECK(dalloc(kf, &kf->fin_coeffs[p], n));
+      KF_CHECK(dalloc(kf, &kf->fin_post16[p], n));
+      KF_CHECK(dalloc(kf, &kf->fin_pixels[p], n));
+      P.skip_pitch[p] = (long long)(kf->plane_h[p] / 4) * P.skip_stride;
+      KF_CHECK(dalloc(kf, &kf->fin_bskip[p], (size_t)P.skip_pitch[p] * F));
+      P.d[p] = kf->coeffs[p];
+      P.md[p] = kf->pred_coeffs[p];
+      P.out[p] = kf->fin_coeffs[p];
+      P.plane_pitch[p] = (long long)kf->plane_w[p] * kf->plane_h[p];
+      P.plane_stride[p] = kf->plane_w[p];
+      P.bskip[p] = kf->fin_bskip[p];
+    }
+    KF_CHECK(dalloc(kf, &kf->fin_level_in, nsb));
+    KF_CHECK(dalloc(kf, &kf->fin_level, nsb));
+    KF_CHECK(dalloc(kf, &kf->fin_coded, nsb));
+    KF_CHECK(dalloc(kf, &kf->dering_thr[0], nsb));
+    KF_CHECK(dalloc(kf, &kf->dering_thr[1], nsb));
+    KF_CHECK(dalloc(kf, &kf->dering_dir, nsb * 64));
+    P.coded = kf->fin_coded;
+    P.nhsb = kf->nhsb;
+    P.nvsb = kf->nvsb;
+    P.q0 = kf->luma.prm.q0;
+    memcpy(P.pvq_qm_q4, kf->cfg.pvq_qm_q4, sizeof(P.pvq_qm_q4));
+    int dq_max = 1;
+    for (int p = 0; p < 3; p++)
+      for (int bs = 0; bs < 5; bs++) {
+        const int dq = (P.q0 * P.pvq_qm_q4[p][bs * (bs + 1)]) >> 4;
+        if (dq > dq_max) dq_max = dq;
+      }
+    kf->fin_dc_limit = DAALA_B200_KF_FINISH_DC_LIMIT / dq_max;
   }
   // dalloc's cudaMemset runs on the legacy default stream, asynchronously, and the engine's stream does not
   // synchronise with it (cudaStreamNonBlocking): wait for every clear before anything is launched -- the table
@@ -2099,6 +2253,57 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
   return (int)cudaGetLastError();
 }
 
+// config.inter_finish: the kernels of the finishing pass, between the H2D of the decisions / levels and the D2H of
+// the results.  Patch and skip map, the inverse in place on the patched plane (iDCT + split postfilters), SB-edge
+// postfilter -> etmp (int16), thresholds with the forced level 0, od_dering of every plane with the real skip maps
+// storing the u8 reconstruction.
+static int kf_enqueue_finish(daala_b200_kf* kf) {
+  cudaStream_t s = kf->stream;
+  const int wide = kf->sms * 8;
+  const int nsb = kf->nhsb * kf->nvsb;
+  if (cudaMemsetAsync(kf->fin_coded, 0, (size_t)kf->F * nsb, s) != cudaSuccess) return (int)cudaGetLastError();
+  k_fin_patch<<<wide, 256, 0, s>>>(kf->fin);
+  k_fin_skip_map<<<wide, 256, 0, s>>>(kf->fin);
+  daala_b200_frame f = kf->frame;
+  for (int p = 0; p < 3; p++) {
+    f.plane[p].coeffs = f.plane[p].lapped = kf->fin_coeffs[p];   // k_inverse_sb only touches its own superblock
+    f.plane[p].pixels_out = kf->fin_pixels[p];
+    f.post16[p] = kf->fin_post16[p];
+  }
+  int rc = daala_b200_launch_inverse_lapped_only(&f, 3, s);
+  if (!rc) rc = daala_b200_launch_sb_postfilter_store(&f, 3, s);
+  if (rc) return rc;
+  k_dering_thresholds<<<(kf->F * nsb + 255) / 256, 256, 0, s>>>(
+      kf->fin_level_in, kf->dering_thr[0], kf->dering_thr[1], kf->F * nsb,
+      make_int4(kf->dering_tbl[0][0], kf->dering_tbl[0][1], kf->dering_tbl[0][2], kf->dering_tbl[0][3]),
+      make_int2(kf->dering_tbl[0][4], kf->dering_tbl[0][5]),
+      make_int4(kf->dering_tbl[1][0], kf->dering_tbl[1][1], kf->dering_tbl[1][2], kf->dering_tbl[1][3]),
+      make_int2(kf->dering_tbl[1][4], kf->dering_tbl[1][5]), kf->fin_coded, kf->fin_level);
+  for (int p = 0; p < 3; p++) {
+    const long long per = (long long)kf->plane_w[p] * kf->plane_h[p];
+    daala_b200_dering_params dp;
+    memset(&dp, 0, sizeof(dp));
+    dp.y = nullptr;   // u8 output only
+    dp.x = kf->fin_post16[p];
+    dp.dir = kf->dering_dir;
+    dp.bskip = kf->fin_bskip[p];
+    dp.sb_threshold = kf->dering_thr[p ? 1 : 0];
+    dp.ystride = dp.xstride = kf->plane_w[p];
+    dp.dir_stride = kf->nhsb * 8;
+    dp.skip_stride = kf->fin.skip_stride;
+    dp.nhsb = kf->nhsb;
+    dp.nvsb = kf->nvsb;
+    dp.xdec = p ? 1 : 0;
+    dp.pli = p;
+    dp.overlap = 1;      // OD_DERING_CHECK_OVERLAP
+    dp.coeff_shift = 4;  // OD_COEFF_SHIFT
+    rc = daala_b200_dering_plane_batch_skip(&dp, kf->F, per, per, (long long)nsb * 64, nsb, kf->fin.skip_pitch[p],
+                                            kf->fin_pixels[p], s);
+    if (rc) return rc;
+  }
+  return (int)cudaGetLastError();
+}
+
 extern "C" {
 
 // why the last daala_b200_kf_create of this thread returned NULL (daala_b200_kf_error(NULL))
@@ -2108,6 +2313,10 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: invalid configuration");
   if (cfg && cfg->inter_mc && (cfg->inter_mc != 1 || cfg->inter != 1)) {
     snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: inter_mc is 0 or 1, and 1 requires inter = 1");
+    return nullptr;
+  }
+  if (cfg && cfg->inter_finish && (cfg->inter_finish != 1 || cfg->inter != 1)) {
+    snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: inter_finish is 0 or 1, and 1 requires inter = 1");
     return nullptr;
   }
   if (cfg && cfg->mc_refs < 0) {
@@ -2184,6 +2393,22 @@ void daala_b200_kf_destroy(daala_b200_kf* kf) {
   cudaStreamSynchronize(kf->stream);
   if (kf->exec) cudaGraphExecDestroy(kf->exec);
   if (kf->graph) cudaGraphDestroy(kf->graph);
+  if (kf->fin_exec) cudaGraphExecDestroy(kf->fin_exec);
+  if (kf->fin_graph) cudaGraphDestroy(kf->fin_graph);
+  for (int c = 0; c < 2; c++) {
+    cudaFree(kf->fin_skip[c]);
+    cudaFree(kf->fin_dc[c]);
+    cudaFree(kf->dc_resid[c]);
+  }
+  for (int p = 0; p < 3; p++) {
+    cudaFree(kf->fin_coeffs[p]);
+    cudaFree(kf->fin_post16[p]);
+    cudaFree(kf->fin_pixels[p]);
+    cudaFree(kf->fin_bskip[p]);
+  }
+  cudaFree(kf->fin_level_in);
+  cudaFree(kf->fin_level);
+  cudaFree(kf->fin_coded);
   for (int p = 0; p < 3; p++) {
     cudaFree(kf->pixels[p]);
     cudaFree(kf->coeffs[p]);
@@ -2565,6 +2790,8 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     if (rc) return rc;
     KF_CHECK(cudaEventRecord(g_last_compute, s));
   }
+  kf->have_step = true;
+  kf->last_tot = tot;
   for (int p = 0; p < 3; p++)
     if (io->pixels_out[p])
       KF_CHECK(cudaMemcpyAsync(io->pixels_out[p], kf->pixels_out[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
@@ -2586,6 +2813,10 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     KF_CHECK(cudaMemcpyAsync(io->luma_dc, kf->luma.prm.res_dc, 4 * (size_t)tot.n_luma, cudaMemcpyDeviceToHost, s));
     KF_CHECK(cudaMemcpyAsync(io->chroma_dc, kf->chroma.prm.res_dc, 4 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));
   }
+  if (kf->cfg.inter_finish && io->luma_dc_resid)
+    KF_CHECK(cudaMemcpyAsync(io->luma_dc_resid, kf->dc_resid[0], 4 * (size_t)tot.n_luma, cudaMemcpyDeviceToHost, s));
+  if (kf->cfg.inter_finish && io->chroma_dc_resid)
+    KF_CHECK(cudaMemcpyAsync(io->chroma_dc_resid, kf->dc_resid[1], 4 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));
   if (io->counts) KF_CHECK(cudaMemcpyAsync(io->counts, kf->lists.cnt, sizeof(int32_t) * 32, cudaMemcpyDeviceToHost, s));
   if (io->dering_level_out && kf->cfg.dering)
     KF_CHECK(cudaMemcpyAsync(io->dering_level_out, kf->dering_level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyDeviceToHost, s));
@@ -2593,6 +2824,66 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     k_sym_copy<<<kf->sms * 4, 256, 0, s>>>(sc);
     KF_CHECK(cudaGetLastError());
   }
+  return 0;
+}
+
+int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
+  if (!kf || !io) return (int)cudaErrorInvalidValue;
+  const int F = kf->F;
+  const size_t nsb = (size_t)F * kf->nhsb * kf->nvsb;
+  const long long nb[2] = {kf->last_tot.n_luma, kf->last_tot.n_chroma};
+  const uint8_t* skip[2] = {io->luma_skip, io->chroma_skip};
+  const int32_t* dc[2] = {io->luma_dc, io->chroma_dc};
+  // every refusal before anything is copied or launched
+  const char* why = !kf->cfg.inter_finish ? "the engine was created without inter_finish"
+                    : !kf->have_step ? "no step has been submitted"
+                    : !skip[0] || !skip[1] || !dc[0] || !dc[1] ? "luma_skip, chroma_skip, luma_dc and chroma_dc are required"
+                                                               : nullptr;
+  for (int c = 0; !why && c < 2; c++)
+    for (long long i = 0; i < nb[c]; i++) {
+      if (skip[c][i] > 1) {
+        why = "a skip value is neither 0 nor 1";
+        break;
+      }
+      if (dc[c][i] > kf->fin_dc_limit || dc[c][i] < -kf->fin_dc_limit) {
+        why = "a |dc| exceeds DAALA_B200_KF_FINISH_DC_LIMIT / the largest dc_quant";
+        break;
+      }
+    }
+  for (size_t i = 0; !why && io->dering_level && i < nsb; i++)
+    if (io->dering_level[i] > 5) why = "a dering level is above 5";
+  if (why) {
+    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_finish: %s", why);
+    return (int)cudaErrorInvalidValue;
+  }
+  cudaStream_t s = kf->stream;
+  for (int c = 0; c < 2; c++) {
+    KF_CHECK(cudaMemcpyAsync(kf->fin_skip[c], skip[c], (size_t)nb[c], cudaMemcpyHostToDevice, s));
+    KF_CHECK(cudaMemcpyAsync(kf->fin_dc[c], dc[c], 4 * (size_t)nb[c], cudaMemcpyHostToDevice, s));
+  }
+  if (io->dering_level) KF_CHECK(cudaMemcpyAsync(kf->fin_level_in, io->dering_level, nsb, cudaMemcpyHostToDevice, s));
+  else KF_CHECK(cudaMemsetAsync(kf->fin_level_in, 0, nsb, s));
+  if (!kf->fin_captured) {
+    // as the step's graph: a first run outside the capture loads the kernels
+    int rc = kf_enqueue_finish(kf);
+    if (rc) return rc;
+    KF_CHECK(cudaStreamSynchronize(s));
+    KF_CHECK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    rc = kf_enqueue_finish(kf);
+    cudaError_t e = cudaStreamEndCapture(s, &kf->fin_graph);
+    if (rc) return rc;
+    KF_CHECK(e);
+    KF_CHECK(cudaGraphInstantiate(&kf->fin_exec, kf->fin_graph, 0));
+    kf->fin_captured = true;
+  }
+  KF_CHECK(cudaGraphLaunch(kf->fin_exec, s));
+  for (int p = 0; p < 3; p++) {
+    const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
+    if (io->pixels_out[p]) KF_CHECK(cudaMemcpyAsync(io->pixels_out[p], kf->fin_pixels[p], n, cudaMemcpyDeviceToHost, s));
+    if (io->bskip_out[p])
+      KF_CHECK(cudaMemcpyAsync(io->bskip_out[p], kf->fin_bskip[p], (size_t)kf->fin.skip_pitch[p] * F, cudaMemcpyDeviceToHost, s));
+  }
+  if (io->dering_level_out) KF_CHECK(cudaMemcpyAsync(io->dering_level_out, kf->fin_level, nsb, cudaMemcpyDeviceToHost, s));
   return 0;
 }
 

@@ -5,7 +5,9 @@ reconstruction + PVQ symbols out, everything in between on the GPU (work lists i
 inter=1 the same engine codes P-frame residuals: the motion-compensated prediction planes are a second input
 (`pred=`), and each block's scalar-quantised DC index is a further output.  With inter_mc=1 the engine makes
 that prediction itself from each frame's MV grid and its GOLD / PREV pictures in a pool of reference pictures
-(`refs=`, `ref_slot=`, `mv_grid=`), as od_state_mc_predict does, and returns it as `pred0..2`.
+(`refs=`, `ref_slot=`, `mv_grid=`), as od_state_mc_predict does, and returns it as `pred0..2`.  With inter_finish=1
+`encode` also returns each block's unquantised DC residual, and `finish` takes the host coder's skip and DC decisions
+and deringing levels and returns the reconstruction the decoder makes, with its skip maps.
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -29,7 +31,8 @@ class Config(ctypes.Structure):
                 ("qm", c_void_p), ("qm_inv", c_void_p), ("sb_row0", c_int), ("sb_rows", c_int),
                 ("max_blocks_div", c_int), ("persist_ctas_per_sm", c_int), ("split_free", c_int), ("dering", c_int), ("noref_prepass", c_int), ("level_chains", c_int), ("stream", c_void_p),
                 ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
-                ("symbol_stream", c_int), ("inter", c_int), ("inter_mc", c_int), ("mc_refs", c_int)]
+                ("symbol_stream", c_int), ("inter", c_int), ("inter_mc", c_int), ("mc_refs", c_int),
+                ("inter_finish", c_int)]
 
 
 class Totals(ctypes.Structure):
@@ -46,7 +49,13 @@ class IO(ctypes.Structure):
                 ("sym_bands", c_void_p), ("sym_bands_cap", c_ll), ("sym_pulses", c_void_p), ("sym_pulses_cap", c_ll),
                 ("pred_pixels", c_void_p * 3), ("luma_dc", c_void_p), ("chroma_dc", c_void_p),
                 ("ref_pixels", c_void_p * 3), ("nrefs", c_int), ("ref_slot", c_void_p), ("mv_grid", c_void_p),
-                ("pred_pixels_out", c_void_p * 3)]
+                ("pred_pixels_out", c_void_p * 3), ("luma_dc_resid", c_void_p), ("chroma_dc_resid", c_void_p)]
+
+
+class FinishIO(ctypes.Structure):
+    _fields_ = [("luma_skip", c_void_p), ("chroma_skip", c_void_p), ("luma_dc", c_void_p), ("chroma_dc", c_void_p),
+                ("dering_level", c_void_p), ("pixels_out", c_void_p * 3), ("bskip_out", c_void_p * 3),
+                ("dering_level_out", c_void_p)]
 
 
 class SymBounds(ctypes.Structure):
@@ -85,6 +94,7 @@ def _bind():
                                              ctypes.POINTER(Totals)]
     for name in ("daala_b200_kf_submit", "daala_b200_kf_encode"):
         getattr(L, name).argtypes = [c_void_p, ctypes.POINTER(IO)]
+    L.daala_b200_kf_finish.argtypes = [c_void_p, ctypes.POINTER(FinishIO)]
     L.daala_b200_kf_symbol_bounds.argtypes = [ctypes.POINTER(Totals), c_int, ctypes.POINTER(SymBounds)]
     L.daala_b200_kf_wait.argtypes = [c_void_p]
     L.daala_b200_device_copy.argtypes = [c_void_p, c_void_p, ctypes.c_size_t, c_int]
@@ -120,7 +130,8 @@ class KeyframeEngine:
 
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
                  qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=0, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
-                 qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0, inter_mc=0, mc_refs=0):
+                 qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0, inter_mc=0, mc_refs=0,
+                 inter_finish=0):
         self.L = _bind()
         self.geom, self.F = geom, nframes
         if qm is None:
@@ -155,6 +166,8 @@ class KeyframeEngine:
         self.inter = int(inter)
         cfg.inter_mc, cfg.mc_refs = int(inter_mc), int(mc_refs)
         self.inter_mc = int(inter_mc)
+        cfg.inter_finish = int(inter_finish)
+        self.inter_finish = int(inter_finish)
         self.nrefs = 0
         self.kf = self.L.daala_b200_kf_create(ctypes.byref(cfg))
         if not self.kf:
@@ -320,6 +333,10 @@ class KeyframeEngine:
             out["luma_dc"] = self._arr("ld", (int(t.n_luma),), np.int32)
             out["chroma_dc"] = self._arr("cd", (int(t.n_chroma),), np.int32)
             io.luma_dc, io.chroma_dc = out["luma_dc"].ctypes.data, out["chroma_dc"].ctypes.data
+        if self.inter_finish:
+            out["luma_dc_resid"] = self._arr("ldr", (int(t.n_luma),), np.int32)
+            out["chroma_dc_resid"] = self._arr("cdr", (int(t.n_chroma),), np.int32)
+            io.luma_dc_resid, io.chroma_dc_resid = out["luma_dc_resid"].ctypes.data, out["chroma_dc_resid"].ctypes.data
         out["counts"] = self._arr("cnt", (32,), np.int32)
         io.counts = out["counts"].ctypes.data
         if self.dering:
@@ -382,6 +399,52 @@ class KeyframeEngine:
                 raise RuntimeError("keyframe engine: MV grid outside the reference's definition: %d leaf corners with a "
                                    "ref other than GOLD / PREV, %d corner windows past the edge extension" % (bad, beyond))
         return out
+
+    def prepare_finish(self, luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels=None):
+        """Stages the host coder's decisions for the last submitted batch (inter_finish engines) and builds the
+        daala_b200_kf_finish_io record; returns the result arrays finish_submit fills: recon0..2, bskip0..2
+        ([F, plane_h / 4, nhsb * 16] u8, state->bskip[pli] of each frame with row stride state->skip_stride; a chroma
+        row's columns past plane_w / 4 stay 0) and dering_levels ([F, nvsb, nhsb], the levels applied)."""
+        g, t = self.geom, self.totals
+        fio = FinishIO()
+        n = {"luma": int(t.n_luma), "chroma": int(t.n_chroma)}
+        for kind, sk, dc in (("luma", luma_skip, luma_dc), ("chroma", chroma_skip, chroma_dc)):
+            a = self._arr("fs_" + kind, (n[kind],), np.uint8)
+            a[...] = sk
+            setattr(fio, kind + "_skip", a.ctypes.data)
+            a = self._arr("fd_" + kind, (n[kind],), np.int32)
+            a[...] = dc
+            setattr(fio, kind + "_dc", a.ctypes.data)
+        if dering_levels is not None:
+            a = self._arr("flev", (self.F, g.nvsb, g.nhsb), np.uint8)
+            a[...] = dering_levels
+            fio.dering_level = a.ctypes.data
+        out = {}
+        for p in range(3):
+            out["recon%d" % p] = self._arr("fout%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
+            fio.pixels_out[p] = out["recon%d" % p].ctypes.data
+            out["bskip%d" % p] = self._arr("fskip%d" % p, (self.F, g.plane_shape(p)[0] // 4, g.nhsb * 16), np.uint8)
+            fio.bskip_out[p] = out["bskip%d" % p].ctypes.data
+        out["dering_levels"] = self._arr("flev_out", (self.F, g.nvsb, g.nhsb), np.uint8)
+        fio.dering_level_out = out["dering_levels"].ctypes.data
+        # one skip byte and one int32 DC per block, the levels
+        self.finish_h2d_bytes = 5 * sum(n.values()) + (self.F * g.nvsb * g.nhsb if dering_levels is not None else 0)
+        self.finish_d2h_bytes = sum(v.nbytes for v in out.values())
+        self._fio, self._fout = fio, out
+        return out
+
+    def finish_submit(self):
+        self._check(self.L.daala_b200_kf_finish(self.kf, ctypes.byref(self._fio)), "kf_finish")
+
+    def finish(self, luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels=None):
+        """The finishing pass of the last encoded P-frame batch (inter_finish engines): per block (block order of
+        the luma / chroma results of encode) the host coder's skip decision (0 or 1) and final DC index, per
+        superblock the deringing level (None: all 0).  Returns the reconstruction the decoder makes, the skip maps
+        and the levels applied (see prepare_finish); views of the engine's host buffers."""
+        self.prepare_finish(luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels)
+        self.finish_submit()
+        self.wait()
+        return self._fout
 
     # --- device-resident use -------------------------------------------------------------------
     def run_device(self, phases=PH_ALL, graph=True):

@@ -495,6 +495,11 @@ typedef struct daala_b200_kf_config {
                                   pixels of padding.  Requires inter = 1; refused by daala_b200_kf_create
                                   otherwise */
   int mc_refs;                 /* inter_mc: capacity of the reference-picture pool in pictures; 0 = 2 * nframes */
+  int inter_finish;            /* 0 (default): nothing below exists; the engine is exactly the one without this field.
+                                  1: the engine also has the finishing pass daala_b200_kf_finish (the host coder's skip
+                                  and DC decisions, the skip map bskip, deringing over it, final reconstruction), and
+                                  each step writes daala_b200_kf_io.luma_dc_resid / chroma_dc_resid.  Requires inter = 1;
+                                  refused by daala_b200_kf_create otherwise */
 } daala_b200_kf_config;
 
 /* One vertex of a P frame's MV grid, as od_mv_grid_pt (reference src/mc.h:73-84) holds it after od_mv_est. */
@@ -586,7 +591,37 @@ typedef struct daala_b200_kf_io {
                                            when the frame predicts from one picture) */
   const daala_b200_mv_pt *mv_grid;      /* [nframes][nvsb*8 + 1][nhsb*8 + 1]: each frame's state->mv_grid */
   uint8_t *pred_pixels_out[3];          /* optional: the prediction planes the engine made, layout of pixels */
+  /* config.inter_finish only (optional, NULL = not copied). */
+  int32_t *luma_dc_resid, *chroma_dc_resid; /* [n_blocks]: each block's unquantised DC residual in[0] - ref[0] (what the
+                                           host's od_rdo_quant quantises, src/pvq_encoder.c:886 / :956), block order
+                                           of luma_dc / chroma_dc */
 } daala_b200_kf_io;
+
+/* The finishing pass of a P-frame batch (config.inter_finish), daala_b200_kf_finish: the host coder's per-block
+   decisions in, the reconstruction the decoder will make out.  Decision arrays are in the block order of
+   luma_res / chroma_res of the last submitted step.
+     skip = 0: the block's coefficients are those the step coded, with d[0] = md[0] + dc * dc_quant;
+     skip = 1: d = md over the whole block (the PVQ skip of src/pvq_encoder.c:951-977, AC = prediction; the late
+               skip of src/encode.c:1412-1450 is skip = 1 with dc = 0), then d[0] = md[0] + dc * dc_quant.
+   dc_quant = max(1, q0 * pvq_qm_q4[pli][bs * (bs + 1)] >> 4), the step's band-0 quantiser.  A block counts as
+   skipped in bskip when skip && dc == 0 (od_pvq_encode's return value with has_dc_skip, src/encode.c:1364-1371,
+   :1690-1691).  Then the inverse, the split and superblock-edge postfilters (they ignore the skip flags without
+   OD_DEBLOCKING, src/filter.c:1505-1509, :1596-1598) and the deringing of src/encode.c:2695-2842 with the given
+   levels: a superblock none of whose 4x4 luma units is coded is forced to level 0 (:2724-2738), chroma thresholds
+   are x0.6, od_dering reads the real skip map (src/dering.c:297-325).  |dc| must not exceed
+   DAALA_B200_KF_FINISH_DC_LIMIT / DQ, DQ the largest dc_quant of the engine over planes and block sizes, so that
+   dc * dc_quant stays within 2^30 and md[0] + dc * dc_quant within od_coeff. */
+#define DAALA_B200_KF_FINISH_DC_LIMIT (1 << 30)
+typedef struct daala_b200_kf_finish_io {
+  const uint8_t *luma_skip, *chroma_skip;  /* [n_blocks]: 0 or 1 (required) */
+  const int32_t *luma_dc, *chroma_dc;      /* [n_blocks]: the final DC index of each block (required) */
+  const uint8_t *dering_level;             /* [nframes][nvsb][nhsb] levels 0..5; NULL = all 0 */
+  uint8_t *pixels_out[3];                  /* optional: the reconstruction, layout of daala_b200_kf_io.pixels */
+  uint8_t *bskip_out[3];                   /* optional: state->bskip[pli] of every frame, [nframes][plane_h / 4][nhsb * 16]
+                                              (one byte per 4x4 block of the plane, row stride state->skip_stride for
+                                              every plane; the columns past plane_w / 4 of a chroma row are 0) */
+  uint8_t *dering_level_out;               /* optional: [nframes][nvsb][nhsb] the levels applied */
+} daala_b200_kf_finish_io;
 
 typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, device-resident callers) */
   uint8_t *pixels[3];
@@ -657,6 +692,14 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    the corner windows (with the 6-tap filter's apron of -2..+3 pixels) that reach more than 64 luma / 32 chroma
    pixels outside the plane (counts[20]), where the reference encoder's result is undefined. */
 int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
+/* The finishing pass (config.inter_finish, see daala_b200_kf_finish_io) on the last submitted step: H2D of the
+   decisions and levels, the pass's kernels as one CUDA graph (captured at the first call), D2H of the requested
+   outputs; enqueued on the engine's stream like submit, waited for with daala_b200_kf_wait.  The step's outputs and
+   its d / md planes are not modified (the decisions are applied to a plane of their own), so the pass may run any
+   number of times after one step.  Refused with cudaErrorInvalidValue and a message in daala_b200_kf_error, before
+   anything is copied or launched: an engine without inter_finish, no step submitted yet, a NULL decision array, a
+   skip value other than 0 or 1, a level above 5, a |dc| above DAALA_B200_KF_FINISH_DC_LIMIT / DQ. */
+int daala_b200_kf_finish(daala_b200_kf *kf, const daala_b200_kf_finish_io *io);
 int daala_b200_kf_wait(daala_b200_kf *kf);
 int daala_b200_kf_encode(daala_b200_kf *kf, const daala_b200_kf_io *io);   /* submit + wait */
 int daala_b200_device_copy(void *dst, const void *src, size_t bytes, int kind);  /* 0 H2D, 1 D2H, 2 D2D; synchronous */
