@@ -13,8 +13,9 @@
 //    the decided levels above and to the left: a few thousand scalar steps per 4K frame, run on the host
 //    (daala_b200_dering_decide, also exported on its own: it is the part the reference's decoder shares,
 //    src/decode.c:1040-1053).
-// Host-driven (allocates its scratch per call); not part of the keyframe engine's graph, which applies levels
-// it is given.  Parity: tests/test_host_logic.py (decision vs the reference's CDF functions),
+// daala_b200_dering_search is host-driven (allocates its scratch per call).  daala_b200_dering_search_enqueue is the
+// batched, graph-capturable form, decision on the device included, that the keyframe engine (dering = 2) and the
+// P-frame finishing pass (inter_finish = 2, real skip maps, uncoded superblocks left out, one context) run.  Parity: tests/test_host_logic.py (decision vs the reference's CDF functions),
 // tests/test_gpu_dering.py (whole search vs the reference's loop, oracle/ref_hooks_encode.c).
 #include <cuda_runtime.h>
 #include <math.h>
@@ -65,16 +66,18 @@ __global__ void __launch_bounds__(256) k_pack_sb_batch(const int16_t* __restrict
   }
 }
 
-// The decision of daala_b200_dering_decide on the device, one thread per (key)frame: every frame starts from the
-// initial CDFs (the adaptation state is reset per frame).  Same operations as the host function; log() is the CUDA
-// library's, so a decision could differ from the host's only where two scores agree to the last bits.
+// The decision of daala_b200_dering_decide on the device, one thread per frame: every frame starts from the initial
+// CDFs (the adaptation state is reset per frame, src/encode.c:3080).  Same operations as the host function, `coded`
+// (nullable, [F][nsb]) and `is_keyframe` included; log() is the CUDA library's, so a decision could differ from the
+// host's only where two scores agree to the last bits.
 __global__ void k_dering_decide(const double* __restrict__ dist, int nframes, int nhdr, int nvdr, double lambda,
-                                uint8_t* __restrict__ levels) {
+                                const uint8_t* __restrict__ coded, int is_keyframe, uint8_t* __restrict__ levels) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= nframes) return;
   const int nsb = nhdr * nvdr;
   const size_t per_level = (size_t)nframes * nsb;
   const double* d = dist + (size_t)f * nsb;
+  const uint8_t* cf = coded ? coded + (size_t)f * nsb : nullptr;
   uint8_t* lv = levels + (size_t)f * nsb;
   unsigned short cdf[kContexts][kLevels];
   for (int c = 0; c < kContexts; c++)
@@ -82,11 +85,17 @@ __global__ void k_dering_decide(const double* __restrict__ dist, int nframes, in
   for (int sby = 0; sby < nvdr; sby++) {
     for (int sbx = 0; sbx < nhdr; sbx++) {
       const int sb = sby * nhdr + sbx;
+      if (cf && !cf[sb]) {   // every 4x4 block skipped: not searched, not signalled (src/encode.c:2727-2738)
+        lv[sb] = 0;
+        continue;
+      }
       int left = 0, up = 0;
-      if (sby > 0) left = up = lv[sb - nhdr];
-      if (sbx > 0) {
-        left = lv[sb - 1];
-        if (sby == 0) up = left;
+      if (is_keyframe) {
+        if (sby > 0) left = up = lv[sb - nhdr];
+        if (sbx > 0) {
+          left = lv[sb - 1];
+          if (sby == 0) up = left;
+        }
       }
       unsigned short* m = cdf[up + left];
       const int total = m[kLevels - 1];
@@ -172,9 +181,9 @@ extern "C" int daala_b200_dering_decide(const double* dist, int nhdr, int nvdr, 
   return 0;
 }
 
-extern "C" int daala_b200_dering_plane_batch(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
-                                             long long x_pitch, long long dir_pitch, long long thr_pitch, uint8_t* y8,
-                                             void* stream);
+extern "C" int daala_b200_dering_plane_batch_skip(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
+                                                  long long x_pitch, long long dir_pitch, long long thr_pitch,
+                                                  long long skip_pitch, uint8_t* y8, void* stream);
 
 extern "C" int daala_b200_dering_search(const daala_b200_dering_search_params* p, uint16_t* cdf, int increment,
                                         uint8_t* levels, double* dist_out, void* stream_) {
@@ -255,8 +264,8 @@ extern "C" int daala_b200_dering_search(const daala_b200_dering_search_params* p
 }
 
 extern "C" int daala_b200_dering_search_enqueue(const daala_b200_dering_search_batch* b, void* stream_) {
-  if (!b || !b->etmp || !b->src || !b->filt || !b->orig || !b->cand || !b->dir || !b->zskip || !b->dist || !b->levels ||
-      b->nframes < 1 || b->nhsb < 1 || b->nvsb < 1)
+  if (!b || !b->etmp || !b->src || !b->filt || !b->orig || !b->cand || !b->dir || !b->bskip || !b->dist || !b->levels ||
+      b->nframes < 1 || b->nhsb < 1 || b->nvsb < 1 || b->skip_stride < b->nhsb * 16 || b->skip_pitch < 0)
     return (int)cudaErrorInvalidValue;
   cudaStream_t st = (cudaStream_t)stream_;
   const int nsb = b->nhsb * b->nvsb, F = b->nframes;
@@ -272,18 +281,19 @@ extern "C" int daala_b200_dering_search_enqueue(const daala_b200_dering_search_b
       dp.y = b->filt;
       dp.x = b->etmp;
       dp.dir = b->dir;
-      dp.bskip = b->zskip;
+      dp.bskip = b->bskip;
       dp.ystride = w;
       dp.xstride = b->etmp_stride;
       dp.dir_stride = b->nhsb * 8;
-      dp.skip_stride = b->nhsb * 16;
+      dp.skip_stride = b->skip_stride;
       dp.nhsb = b->nhsb;
       dp.nvsb = b->nvsb;
       dp.threshold = b->threshold[gi];
       dp.overlap = 1;
       dp.coeff_shift = 4;
       dp.dir_format = gi == 1 ? 1 : 2;   // the direction search runs once; later passes re-use direction and variance
-      const int r = daala_b200_dering_plane_batch(&dp, F, filt_pitch, b->etmp_pitch, (long long)nsb * 64, 0, nullptr, st);
+      const int r = daala_b200_dering_plane_batch_skip(&dp, F, filt_pitch, b->etmp_pitch, (long long)nsb * 64, 0,
+                                                       b->skip_pitch, nullptr, st);
       if (r) return r;
       plane = b->filt;
       ppitch = filt_pitch;
@@ -297,6 +307,7 @@ extern "C" int daala_b200_dering_search_enqueue(const daala_b200_dering_search_b
                                           b->coded_quantizer, b->dist + (size_t)gi * F * nsb, st);
     if (r) return r;
   }
-  k_dering_decide<<<(F + 31) / 32, 32, 0, st>>>(b->dist, F, b->nhsb, b->nvsb, b->dering_lambda, b->levels);
+  k_dering_decide<<<(F + 31) / 32, 32, 0, st>>>(b->dist, F, b->nhsb, b->nvsb, b->dering_lambda, b->coded,
+                                                b->is_keyframe, b->levels);
   return (int)cudaGetLastError();
 }

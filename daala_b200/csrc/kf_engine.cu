@@ -1601,11 +1601,11 @@ struct daala_b200_kf {
   uint8_t* dering_level;           // [F][nvsb][nhsb]
   int32_t *dering_thr[2];          // luma / chroma thresholds per superblock
   int16_t* dering_in[3];           // etmp: the planes after the SB-edge postfilter
-  int16_t* dering_filt;            // level search (cfg.dering == 2): one filtered luma candidate, [F][h][w]
+  int16_t* dering_filt;            // level search (cfg.dering == 2 or inter_finish == 2): one filtered luma candidate, [F][h][w]
   int32_t* dering_dir;             // [F][nvsb*8][nhsb*8]
   uint8_t* dering_skip;            // all zero: keyframes never mark a block skipped (src/encode.c:1690)
   int dering_tbl[2][6];
-  // level search (cfg.dering == 2): packed superblock pairs and the 6 x F x nsb distortions
+  // level search (cfg.dering == 2 or inter_finish == 2): packed superblock pairs and the 6 x F x nsb distortions
   int32_t *dering_orig, *dering_cand;
   double* dering_dist;
   Lists lists;
@@ -2029,6 +2029,13 @@ static int kf_alloc(daala_b200_kf* kf) {
     KF_CHECK(dalloc(kf, &kf->dering_thr[0], nsb));
     KF_CHECK(dalloc(kf, &kf->dering_thr[1], nsb));
     KF_CHECK(dalloc(kf, &kf->dering_dir, nsb * 64));
+    if (kf->cfg.inter_finish == 2) {
+      // the level search's scratch, in the keyframe search's fields (dering and inter exclude each other)
+      KF_CHECK(dalloc(kf, &kf->dering_filt, (size_t)kf->plane_w[0] * kf->plane_h[0] * F));
+      KF_CHECK(dalloc(kf, &kf->dering_orig, nsb * 4096));
+      KF_CHECK(dalloc(kf, &kf->dering_cand, nsb * 4096));
+      KF_CHECK(dalloc(kf, &kf->dering_dist, nsb * 6));
+    }
     P.coded = kf->fin_coded;
     P.nhsb = kf->nhsb;
     P.nvsb = kf->nvsb;
@@ -2214,7 +2221,11 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
       sb.orig = kf->dering_orig;
       sb.cand = kf->dering_cand;
       sb.dir = kf->dering_dir;
-      sb.zskip = kf->dering_skip;
+      sb.bskip = kf->dering_skip;   // one all-zero map for every frame
+      sb.skip_stride = kf->nhsb * 16;
+      sb.skip_pitch = 0;
+      sb.coded = nullptr;
+      sb.is_keyframe = 1;
       sb.dist = kf->dering_dist;
       sb.levels = kf->dering_level;
       rc = daala_b200_dering_search_enqueue(&sb, s);
@@ -2255,8 +2266,9 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
 
 // config.inter_finish: the kernels of the finishing pass, between the H2D of the decisions / levels and the D2H of
 // the results.  Patch and skip map, the inverse in place on the patched plane (iDCT + split postfilters), SB-edge
-// postfilter -> etmp (int16), thresholds with the forced level 0, od_dering of every plane with the real skip maps
-// storing the u8 reconstruction.
+// postfilter -> etmp (int16), [inter_finish = 2: the level search of src/encode.c:2708-2811 on etmp, the step's
+// source luma and the pass's skip maps -> fin_level_in], thresholds with the forced level 0, od_dering of every plane
+// with the real skip maps storing the u8 reconstruction.
 static int kf_enqueue_finish(daala_b200_kf* kf) {
   cudaStream_t s = kf->stream;
   const int wide = kf->sms * 8;
@@ -2273,6 +2285,38 @@ static int kf_enqueue_finish(daala_b200_kf* kf) {
   int rc = daala_b200_launch_inverse_lapped_only(&f, 3, s);
   if (!rc) rc = daala_b200_launch_sb_postfilter_store(&f, 3, s);
   if (rc) return rc;
+  const bool search = kf->cfg.inter_finish == 2;
+  if (search) {
+    // the P-frame form of the keyframe search: the frame's own skip maps under every filtered candidate, superblocks
+    // without a coded luma 4x4 unit neither scored nor adapted, context 0 (src/encode.c:2720-2811)
+    daala_b200_dering_search_batch sb;
+    memset(&sb, 0, sizeof(sb));
+    sb.etmp = kf->fin_post16[0];
+    sb.src = kf->pixels[0];
+    sb.etmp_pitch = sb.src_pitch = (long long)kf->plane_w[0] * kf->plane_h[0];
+    sb.etmp_stride = sb.src_stride = kf->plane_w[0];
+    sb.nframes = kf->F;
+    sb.nhsb = kf->nhsb;
+    sb.nvsb = kf->nvsb;
+    for (int g = 0; g < 6; g++) sb.threshold[g] = kf->dering_tbl[0][g];
+    sb.coded_quantizer = kf->cfg.coded_quantizer;
+    sb.qm_is_flat = kf->cfg.qm_is_flat;
+    sb.use_activity_masking = kf->cfg.use_masking;
+    sb.dering_lambda = kf->cfg.dering_lambda;
+    sb.bskip = kf->fin_bskip[0];
+    sb.skip_stride = kf->fin.skip_stride;
+    sb.skip_pitch = kf->fin.skip_pitch[0];
+    sb.coded = kf->fin_coded;
+    sb.is_keyframe = 0;
+    sb.filt = kf->dering_filt;
+    sb.orig = kf->dering_orig;
+    sb.cand = kf->dering_cand;
+    sb.dir = kf->dering_dir;
+    sb.dist = kf->dering_dist;
+    sb.levels = kf->fin_level_in;   // what the thresholds read; its level 0 agrees with the forced one
+    rc = daala_b200_dering_search_enqueue(&sb, s);
+    if (rc) return rc;
+  }
   k_dering_thresholds<<<(kf->F * nsb + 255) / 256, 256, 0, s>>>(
       kf->fin_level_in, kf->dering_thr[0], kf->dering_thr[1], kf->F * nsb,
       make_int4(kf->dering_tbl[0][0], kf->dering_tbl[0][1], kf->dering_tbl[0][2], kf->dering_tbl[0][3]),
@@ -2297,6 +2341,9 @@ static int kf_enqueue_finish(daala_b200_kf* kf) {
     dp.pli = p;
     dp.overlap = 1;      // OD_DERING_CHECK_OVERLAP
     dp.coeff_shift = 4;  // OD_COEFF_SHIFT
+    // after a search the direction map is already there, packed with the variance; neither depends on the skip map
+    // (src/dering.c:280-287)
+    dp.dir_format = search ? 2 : 0;
     rc = daala_b200_dering_plane_batch_skip(&dp, kf->F, per, per, (long long)nsb * 64, nsb, kf->fin.skip_pitch[p],
                                             kf->fin_pixels[p], s);
     if (rc) return rc;
@@ -2315,8 +2362,9 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
     snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: inter_mc is 0 or 1, and 1 requires inter = 1");
     return nullptr;
   }
-  if (cfg && cfg->inter_finish && (cfg->inter_finish != 1 || cfg->inter != 1)) {
-    snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: inter_finish is 0 or 1, and 1 requires inter = 1");
+  if (cfg && cfg->inter_finish && (cfg->inter_finish < 0 || cfg->inter_finish > 2 || cfg->inter != 1)) {
+    snprintf(g_create_err, sizeof(g_create_err),
+             "daala_b200_kf_create: inter_finish is 0, 1 or 2, and 1 and 2 require inter = 1");
     return nullptr;
   }
   if (cfg && cfg->mc_refs < 0) {
@@ -2838,7 +2886,9 @@ int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
   const char* why = !kf->cfg.inter_finish ? "the engine was created without inter_finish"
                     : !kf->have_step ? "no step has been submitted"
                     : !skip[0] || !skip[1] || !dc[0] || !dc[1] ? "luma_skip, chroma_skip, luma_dc and chroma_dc are required"
-                                                               : nullptr;
+                    : kf->cfg.inter_finish == 2 && io->dering_level
+                        ? "dering_level must be NULL on an inter_finish = 2 engine (the pass searches the levels)"
+                        : nullptr;
   for (int c = 0; !why && c < 2; c++)
     for (long long i = 0; i < nb[c]; i++) {
       if (skip[c][i] > 1) {
@@ -2861,8 +2911,9 @@ int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
     KF_CHECK(cudaMemcpyAsync(kf->fin_skip[c], skip[c], (size_t)nb[c], cudaMemcpyHostToDevice, s));
     KF_CHECK(cudaMemcpyAsync(kf->fin_dc[c], dc[c], 4 * (size_t)nb[c], cudaMemcpyHostToDevice, s));
   }
+  // inter_finish = 2: the graph's search writes fin_level_in
   if (io->dering_level) KF_CHECK(cudaMemcpyAsync(kf->fin_level_in, io->dering_level, nsb, cudaMemcpyHostToDevice, s));
-  else KF_CHECK(cudaMemsetAsync(kf->fin_level_in, 0, nsb, s));
+  else if (kf->cfg.inter_finish == 1) KF_CHECK(cudaMemsetAsync(kf->fin_level_in, 0, nsb, s));
   if (!kf->fin_captured) {
     // as the step's graph: a first run outside the capture loads the kernels
     int rc = kf_enqueue_finish(kf);

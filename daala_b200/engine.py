@@ -7,7 +7,9 @@ inter=1 the same engine codes P-frame residuals: the motion-compensated predicti
 that prediction itself from each frame's MV grid and its GOLD / PREV pictures in a pool of reference pictures
 (`refs=`, `ref_slot=`, `mv_grid=`), as od_state_mc_predict does, and returns it as `pred0..2`.  With inter_finish=1
 `encode` also returns each block's unquantised DC residual, and `finish` takes the host coder's skip and DC decisions
-and deringing levels and returns the reconstruction the decoder makes, with its skip maps.
+and deringing levels and returns the reconstruction the decoder makes, with its skip maps.  With inter_finish=2 the pass
+searches the deringing levels itself (the reference's P-frame search: real skip maps, uncoded superblocks left out,
+one CDF context) and returns them with the reconstruction made at those levels.
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -153,8 +155,8 @@ class KeyframeEngine:
         cfg.level_chains = int(level_chains)
         cfg.noref_prepass = int(noref_prepass)
         cfg.dering = int(dering)
-        # dering == 2 (level search): scale of od_compute_dist and enc->dering_lambda = 0.67 * OD_PVQ_LAMBDA * q^2
-        # (src/rate.c:1086; the target quantizer is this engine's q0)
+        # dering == 2 or inter_finish == 2 (level search): scale of od_compute_dist and enc->dering_lambda =
+        # 0.67 * OD_PVQ_LAMBDA * q^2 (src/rate.c:1086; the target quantizer is this engine's q0)
         cfg.coded_quantizer = int(coded_quantizer)
         cfg.qm_is_flat = int(qm_is_flat)
         cfg.dering_lambda = float(0.67 * pvq.PVQ_LAMBDA * q0 * q0 if dering_lambda is None else dering_lambda)
@@ -404,7 +406,9 @@ class KeyframeEngine:
         """Stages the host coder's decisions for the last submitted batch (inter_finish engines) and builds the
         daala_b200_kf_finish_io record; returns the result arrays finish_submit fills: recon0..2, bskip0..2
         ([F, plane_h / 4, nhsb * 16] u8, state->bskip[pli] of each frame with row stride state->skip_stride; a chroma
-        row's columns past plane_w / 4 stay 0) and dering_levels ([F, nvsb, nhsb], the levels applied)."""
+        row's columns past plane_w / 4 stay 0) and dering_levels ([F, nvsb, nhsb], the levels applied; on an
+        inter_finish=2 engine the levels the pass searched, and dering_levels must be None: the C call refuses
+        levels there)."""
         g, t = self.geom, self.totals
         fio = FinishIO()
         n = {"luma": int(t.n_luma), "chroma": int(t.n_chroma)}
@@ -439,8 +443,9 @@ class KeyframeEngine:
     def finish(self, luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels=None):
         """The finishing pass of the last encoded P-frame batch (inter_finish engines): per block (block order of
         the luma / chroma results of encode) the host coder's skip decision (0 or 1) and final DC index, per
-        superblock the deringing level (None: all 0).  Returns the reconstruction the decoder makes, the skip maps
-        and the levels applied (see prepare_finish); views of the engine's host buffers."""
+        superblock the deringing level (None: all 0; inter_finish=2 engines search the levels, so None there).
+        Returns the reconstruction the decoder makes, the skip maps and the levels applied (see prepare_finish);
+        views of the engine's host buffers."""
         self.prepare_finish(luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels)
         self.finish_submit()
         self.wait()

@@ -463,9 +463,11 @@ typedef struct daala_b200_kf_config {
                                   level-synchronous kernel (phases separated by grid barriers); implies
                                   split_free = 2 */
   void *stream;                /* cudaStream_t to run on, or NULL: the engine creates its own */
-  int coded_quantizer;         /* state->coded_quantizer (scale of od_compute_dist, src/encode.c:1221); dering == 2 */
-  int qm_is_flat;              /* enc->qm == OD_FLAT_QM: od_compute_dist is the plain squared error; dering == 2 */
-  double dering_lambda;        /* enc->dering_lambda (src/rate.c:1086); dering == 2 */
+  int coded_quantizer;         /* state->coded_quantizer (scale of od_compute_dist, src/encode.c:1221); dering == 2 or
+                                  inter_finish == 2 */
+  int qm_is_flat;              /* enc->qm == OD_FLAT_QM: od_compute_dist is the plain squared error; dering == 2 or
+                                  inter_finish == 2 */
+  double dering_lambda;        /* enc->dering_lambda (src/rate.c:1086); dering == 2 or inter_finish == 2 */
   int symbol_stream;           /* 1: every step also packs the PVQ symbols of each frame in bitstream order
                                   (daala_b200_kf_sym_block below) for daala_b200_kf_io.sym_*; 0 (default): the step
                                   is exactly the one without the stream */
@@ -498,8 +500,11 @@ typedef struct daala_b200_kf_config {
   int inter_finish;            /* 0 (default): nothing below exists; the engine is exactly the one without this field.
                                   1: the engine also has the finishing pass daala_b200_kf_finish (the host coder's skip
                                   and DC decisions, the skip map bskip, deringing over it, final reconstruction), and
-                                  each step writes daala_b200_kf_io.luma_dc_resid / chroma_dc_resid.  Requires inter = 1;
-                                  refused by daala_b200_kf_create otherwise */
+                                  each step writes daala_b200_kf_io.luma_dc_resid / chroma_dc_resid.
+                                  2: the same pass, which also SEARCHES the deringing levels of every frame instead of
+                                  taking them (src/encode.c:2708-2811 for a P frame, see daala_b200_kf_finish_io);
+                                  needs coded_quantizer / qm_is_flat / dering_lambda above.
+                                  1 and 2 require inter = 1; refused by daala_b200_kf_create otherwise */
 } daala_b200_kf_config;
 
 /* One vertex of a P frame's MV grid, as od_mv_grid_pt (reference src/mc.h:73-84) holds it after od_mv_est. */
@@ -610,17 +615,26 @@ typedef struct daala_b200_kf_io {
    levels: a superblock none of whose 4x4 luma units is coded is forced to level 0 (:2724-2738), chroma thresholds
    are x0.6, od_dering reads the real skip map (src/dering.c:297-325).  |dc| must not exceed
    DAALA_B200_KF_FINISH_DC_LIMIT / DQ, DQ the largest dc_quant of the engine over planes and block sizes, so that
-   dc * dc_quant stays within 2^30 and md[0] + dc * dc_quant within od_coeff. */
+   dc * dc_quant stays within 2^30 and md[0] + dc * dc_quant within od_coeff.
+   config.inter_finish = 2: the pass searches the levels itself, between the superblock-edge postfilter and the
+   deringing, as the keyframe search of config.dering = 2 with the three rules of a P frame: every filtered candidate
+   reads the frame's own luma skip map; a superblock with no coded 4x4 luma unit is not searched, gets level 0 and does
+   not adapt the CDF; the CDF context is always 0 (no up / left neighbours).  The score of a level is od_compute_dist of
+   the candidate against the step's source luma plus dering_lambda times its cost under the frame's adaptive CDF, which
+   starts from the initial CDFs for every frame.  dering_level must then be NULL; dering_level_out returns the searched
+   levels, which are the levels applied (the host coder codes them and adapts its own dering CDF with them). */
 #define DAALA_B200_KF_FINISH_DC_LIMIT (1 << 30)
 typedef struct daala_b200_kf_finish_io {
   const uint8_t *luma_skip, *chroma_skip;  /* [n_blocks]: 0 or 1 (required) */
   const int32_t *luma_dc, *chroma_dc;      /* [n_blocks]: the final DC index of each block (required) */
-  const uint8_t *dering_level;             /* [nframes][nvsb][nhsb] levels 0..5; NULL = all 0 */
+  const uint8_t *dering_level;             /* [nframes][nvsb][nhsb] levels 0..5; NULL = all 0.  config.inter_finish = 2:
+                                              must be NULL (the pass searches them) */
   uint8_t *pixels_out[3];                  /* optional: the reconstruction, layout of daala_b200_kf_io.pixels */
   uint8_t *bskip_out[3];                   /* optional: state->bskip[pli] of every frame, [nframes][plane_h / 4][nhsb * 16]
                                               (one byte per 4x4 block of the plane, row stride state->skip_stride for
                                               every plane; the columns past plane_w / 4 of a chroma row are 0) */
-  uint8_t *dering_level_out;               /* optional: [nframes][nvsb][nhsb] the levels applied */
+  uint8_t *dering_level_out;               /* optional: [nframes][nvsb][nhsb] the levels applied (config.inter_finish
+                                              = 2: the searched ones) */
 } daala_b200_kf_finish_io;
 
 typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, device-resident callers) */
@@ -693,12 +707,13 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    pixels outside the plane (counts[20]), where the reference encoder's result is undefined. */
 int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
 /* The finishing pass (config.inter_finish, see daala_b200_kf_finish_io) on the last submitted step: H2D of the
-   decisions and levels, the pass's kernels as one CUDA graph (captured at the first call), D2H of the requested
-   outputs; enqueued on the engine's stream like submit, waited for with daala_b200_kf_wait.  The step's outputs and
-   its d / md planes are not modified (the decisions are applied to a plane of their own), so the pass may run any
-   number of times after one step.  Refused with cudaErrorInvalidValue and a message in daala_b200_kf_error, before
-   anything is copied or launched: an engine without inter_finish, no step submitted yet, a NULL decision array, a
-   skip value other than 0 or 1, a level above 5, a |dc| above DAALA_B200_KF_FINISH_DC_LIMIT / DQ. */
+   decisions and levels, the pass's kernels as one CUDA graph (captured at the first call; with config.inter_finish
+   = 2 it includes the level search), D2H of the requested outputs; enqueued on the engine's stream like submit,
+   waited for with daala_b200_kf_wait.  The step's outputs and its d / md planes are not modified (the decisions are
+   applied to a plane of their own), so the pass may run any number of times after one step.  Refused with
+   cudaErrorInvalidValue and a message in daala_b200_kf_error, before anything is copied or launched: an engine
+   without inter_finish, no step submitted yet, a NULL decision array, a skip value other than 0 or 1, a level above
+   5, a |dc| above DAALA_B200_KF_FINISH_DC_LIMIT / DQ, and (config.inter_finish = 2) a non-NULL dering_level. */
 int daala_b200_kf_finish(daala_b200_kf *kf, const daala_b200_kf_finish_io *io);
 int daala_b200_kf_wait(daala_b200_kf *kf);
 int daala_b200_kf_encode(daala_b200_kf *kf, const daala_b200_kf_io *io);   /* submit + wait */
