@@ -25,6 +25,7 @@
 #include <stdint.h>
 
 #include "daala_b200.h"
+#include "dering_search.h"
 
 namespace daala_b200 {
 namespace dering {
@@ -303,39 +304,31 @@ __global__ void __launch_bounds__(256, 4) k_dering_sb(const __grid_constant__ da
 }  // namespace dering
 }  // namespace daala_b200
 
-extern "C" int daala_b200_dering_plane(const daala_b200_dering_params* prm, void* stream) {
-  if (!prm || prm->nhsb < 1 || prm->nvsb < 1 || prm->xdec < 0 || prm->xdec > 1) return (int)cudaErrorInvalidValue;
+// `nframes` planes of one geometry in one launch (internal: the keyframe engine's deringing stage, the P-frame
+// finishing pass and the level search; the exported entry points below are its single-plane and one-skip-map forms).
+// Element pitches between consecutive frames; skip_pitch: bytes between the frames' skip maps (0: one map for every
+// frame, as on keyframes).  y8 (nullable): write the u8 reconstruction od_coeff_to_ref_plane makes of the filtered
+// plane there, with the int16 plane's strides, instead of the int16 plane (prm->y may then be null).
+int daala_b200_dering_plane_frames(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
+                                   long long x_pitch, long long dir_pitch, long long thr_pitch, long long skip_pitch,
+                                   uint8_t* y8, void* stream) {
+  if (!prm || nframes < 1 || prm->nhsb < 1 || prm->nvsb < 1 || prm->xdec < 0 || prm->xdec > 1) return (int)cudaErrorInvalidValue;
   // not in place: a superblock's apron would read its neighbours' filtered output
-  if (!prm->x || !prm->y || (const void*)prm->x == (const void*)prm->y) return (int)cudaErrorInvalidValue;
-  dim3 grid(prm->nhsb, prm->nvsb);
-  daala_b200::dering::BatchPitch bp = {0, 0, 0, 0, nullptr, 0};
-  daala_b200::dering::k_dering_sb<<<grid, 256, 0, (cudaStream_t)stream>>>(*prm, bp);
-  return (int)cudaGetLastError();
-}
-
-// The same for `nframes` planes of one geometry in one launch (internal: the keyframe engine's deringing stage and
-// the level search).  y8 (nullable): write the u8 reconstruction od_coeff_to_ref_plane makes of the filtered plane
-// there, with the int16 plane's strides, instead of the int16 plane (prm->y may then be null).
-extern "C" int daala_b200_dering_plane_batch(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
-                                             long long x_pitch, long long dir_pitch, long long thr_pitch, uint8_t* y8,
-                                             void* stream) {
-  if (!prm || nframes < 1 || prm->nhsb < 1 || prm->nvsb < 1 || prm->xdec < 0 || prm->xdec > 1) return (int)cudaErrorInvalidValue;
-  if (!prm->x || (!prm->y && !y8) || (const void*)prm->x == (const void*)prm->y) return (int)cudaErrorInvalidValue;
-  dim3 grid(prm->nhsb, prm->nvsb, nframes);
-  daala_b200::dering::BatchPitch bp = {y_pitch, x_pitch, dir_pitch, thr_pitch, y8, 0};
-  daala_b200::dering::k_dering_sb<<<grid, 256, 0, (cudaStream_t)stream>>>(*prm, bp);
-  return (int)cudaGetLastError();
-}
-
-// The same with a skip map per frame, skip_pitch bytes apart (internal: the P-frame finishing pass, whose frames each
-// have their own state->bskip).
-extern "C" int daala_b200_dering_plane_batch_skip(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
-                                                  long long x_pitch, long long dir_pitch, long long thr_pitch,
-                                                  long long skip_pitch, uint8_t* y8, void* stream) {
-  if (!prm || nframes < 1 || prm->nhsb < 1 || prm->nvsb < 1 || prm->xdec < 0 || prm->xdec > 1) return (int)cudaErrorInvalidValue;
   if (!prm->x || (!prm->y && !y8) || (const void*)prm->x == (const void*)prm->y) return (int)cudaErrorInvalidValue;
   dim3 grid(prm->nhsb, prm->nvsb, nframes);
   daala_b200::dering::BatchPitch bp = {y_pitch, x_pitch, dir_pitch, thr_pitch, y8, skip_pitch};
   daala_b200::dering::k_dering_sb<<<grid, 256, 0, (cudaStream_t)stream>>>(*prm, bp);
   return (int)cudaGetLastError();
+}
+
+extern "C" int daala_b200_dering_plane(const daala_b200_dering_params* prm, void* stream) {
+  if (prm && !prm->y) return (int)cudaErrorInvalidValue;
+  return daala_b200_dering_plane_frames(prm, 1, 0, 0, 0, 0, 0, nullptr, stream);
+}
+
+// The batch with one skip map for every frame.
+extern "C" int daala_b200_dering_plane_batch(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
+                                             long long x_pitch, long long dir_pitch, long long thr_pitch, uint8_t* y8,
+                                             void* stream) {
+  return daala_b200_dering_plane_frames(prm, nframes, y_pitch, x_pitch, dir_pitch, thr_pitch, 0, y8, stream);
 }

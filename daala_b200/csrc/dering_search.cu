@@ -13,9 +13,10 @@
 //    the decided levels above and to the left: a few thousand scalar steps per 4K frame, run on the host
 //    (daala_b200_dering_decide, also exported on its own: it is the part the reference's decoder shares,
 //    src/decode.c:1040-1053).
-// daala_b200_dering_search is host-driven (allocates its scratch per call).  daala_b200_dering_search_enqueue is the
-// batched, graph-capturable form, decision on the device included, that the keyframe engine (dering = 2) and the
-// P-frame finishing pass (inter_finish = 2, real skip maps, uncoded superblocks left out, one context) run.  Parity: tests/test_host_logic.py (decision vs the reference's CDF functions),
+// daala_b200_dering_search is host-driven (allocates its scratch per call, one frame).  daala_b200_dering_search_enqueue
+// is the batched, graph-capturable form, decision on the device included, that the keyframe engine (dering = 2) and the
+// P-frame finishing pass (inter_finish = 2, real skip maps, uncoded superblocks left out, one context) run.  Both score
+// the candidates with enqueue_candidates.  Parity: tests/test_host_logic.py (decision vs the reference's CDF functions),
 // tests/test_gpu_dering.py (whole search vs the reference's loop, oracle/ref_hooks_encode.c).
 #include <cuda_runtime.h>
 #include <math.h>
@@ -35,23 +36,8 @@ constexpr int kContexts = 2 * kLevels - 1;
 // OD_DERING_GAIN_TABLE, src/dering.c:50
 const double kGain[kLevels] = {0, 0.5, 0.707, 1, 1.41, 2};
 
-// One CTA per superblock: cand <- the superblock of `plane` as od_coeff, orig (optional) <- the source
-// superblock as (p - 128) << 4.
-__global__ void __launch_bounds__(256) k_pack_sb(const int16_t* __restrict__ plane, int pstride,
-                                                 const uint8_t* __restrict__ src, int sstride, int nhsb,
-                                                 int32_t* __restrict__ cand, int32_t* __restrict__ orig) {
-  const int sb = blockIdx.x, sbx = sb % nhsb, sby = sb / nhsb;
-  const int16_t* p = plane + (size_t)sby * 64 * pstride + sbx * 64;
-  int32_t* c = cand + (size_t)sb * 4096;
-  for (int idx = threadIdx.x; idx < 4096; idx += 256) c[idx] = p[(size_t)(idx >> 6) * pstride + (idx & 63)];
-  if (orig) {
-    const uint8_t* s = src + (size_t)sby * 64 * sstride + sbx * 64;
-    int32_t* o = orig + (size_t)sb * 4096;
-    for (int idx = threadIdx.x; idx < 4096; idx += 256) o[idx] = ((int)s[(size_t)(idx >> 6) * sstride + (idx & 63)] - 128) * 16;
-  }
-}
-
-// The same for a batch: grid (nsb, F).
+// One CTA per superblock of each frame, grid (nsb, F): cand <- the superblock of `plane` as od_coeff, orig
+// (optional) <- the source superblock as (p - 128) << 4.
 __global__ void __launch_bounds__(256) k_pack_sb_batch(const int16_t* __restrict__ plane, long long ppitch, int pstride,
                                                        const uint8_t* __restrict__ src, long long spitch, int sstride,
                                                        int nhsb, int32_t* __restrict__ cand, int32_t* __restrict__ orig) {
@@ -181,9 +167,60 @@ extern "C" int daala_b200_dering_decide(const double* dist, int nhdr, int nvdr, 
   return 0;
 }
 
-extern "C" int daala_b200_dering_plane_batch_skip(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
-                                                  long long x_pitch, long long dir_pitch, long long thr_pitch,
-                                                  long long skip_pitch, uint8_t* y8, void* stream);
+
+void daala_b200_dering_threshold_table(int quantizer, int tbl[2][6]) {
+  const double base = pow((double)quantizer, 0.84182);   // src/encode.c:2694
+  for (int g = 0; g < kLevels; g++) {
+    tbl[0][g] = (int)(kGain[g] * base);
+    tbl[1][g] = (int)(kGain[g] * base * 0.6);
+  }
+}
+
+// The distortion of every candidate of every superblock of the batch, b->dist[gi][f * nsb + sb]: the unfiltered plane
+// (gi = 0) and the five filtered ones, each packed next to the source and measured.  The first filter pass finds the
+// directions and stores them with the variance (dir_format 1); the later passes filter the same plane and re-use them.
+static int enqueue_candidates(const daala_b200_dering_search_batch* b, cudaStream_t st) {
+  const int nsb = b->nhsb * b->nvsb, F = b->nframes;
+  const int w = b->nhsb * 64, h = b->nvsb * 64;
+  const long long filt_pitch = (long long)w * h;
+  for (int gi = 0; gi < kLevels; gi++) {
+    const int16_t* plane = b->etmp;
+    long long ppitch = b->etmp_pitch;
+    int pstride = b->etmp_stride;
+    if (gi) {
+      daala_b200_dering_params dp;
+      memset(&dp, 0, sizeof(dp));
+      dp.y = b->filt;
+      dp.x = b->etmp;
+      dp.dir = b->dir;
+      dp.bskip = b->bskip;
+      dp.ystride = w;
+      dp.xstride = b->etmp_stride;
+      dp.dir_stride = b->nhsb * 8;
+      dp.skip_stride = b->skip_stride;
+      dp.nhsb = b->nhsb;
+      dp.nvsb = b->nvsb;
+      dp.threshold = b->threshold[gi];
+      dp.overlap = 1;
+      dp.coeff_shift = 4;
+      dp.dir_format = gi == 1 ? 1 : 2;
+      const int r = daala_b200_dering_plane_frames(&dp, F, filt_pitch, b->etmp_pitch, (long long)nsb * 64, 0,
+                                                   b->skip_pitch, nullptr, st);
+      if (r) return r;
+      plane = b->filt;
+      ppitch = filt_pitch;
+      pstride = w;
+    }
+    k_pack_sb_batch<<<dim3(nsb, F), 256, 0, st>>>(plane, ppitch, pstride, b->src, b->src_pitch, b->src_stride, b->nhsb,
+                                                  b->cand, gi == 0 ? b->orig : nullptr);
+    cudaError_t e = cudaGetLastError();
+    if (e) return (int)e;
+    const int r = daala_b200_compute_dist(b->orig, b->cand, F * nsb, 64, b->qm_is_flat, b->use_activity_masking,
+                                          b->coded_quantizer, b->dist + (size_t)gi * F * nsb, st);
+    if (r) return r;
+  }
+  return 0;
+}
 
 extern "C" int daala_b200_dering_search(const daala_b200_dering_search_params* p, uint16_t* cdf, int increment,
                                         uint8_t* levels, double* dist_out, void* stream_) {
@@ -192,57 +229,42 @@ extern "C" int daala_b200_dering_search(const daala_b200_dering_search_params* p
   const int nhsb = p->nhsb, nvsb = p->nvsb, nsb = nhsb * nvsb;
   const int w = nhsb * 64, h = nvsb * 64;
   const int skip_stride = p->bskip ? p->skip_stride : nhsb * 16;
-  int16_t* filt = nullptr;
-  int32_t *orig = nullptr, *cand = nullptr, *dir = nullptr;
+  daala_b200_dering_search_batch b;
+  memset(&b, 0, sizeof(b));
   uint8_t* zskip = nullptr;
-  double* ddist = nullptr;
   cudaError_t e = cudaSuccess;
   auto done = [&](cudaError_t err) {
-    cudaFree(filt); cudaFree(orig); cudaFree(cand); cudaFree(dir); cudaFree(zskip); cudaFree(ddist);
+    cudaFree(b.filt); cudaFree(b.orig); cudaFree(b.cand); cudaFree(b.dir); cudaFree(zskip); cudaFree(b.dist);
     return (int)err;
   };
-  if ((e = cudaMalloc(&filt, sizeof(int16_t) * (size_t)w * h))) return done(e);
-  if ((e = cudaMalloc(&orig, sizeof(int32_t) * (size_t)nsb * 4096))) return done(e);
-  if ((e = cudaMalloc(&cand, sizeof(int32_t) * (size_t)nsb * 4096))) return done(e);
-  if ((e = cudaMalloc(&dir, sizeof(int32_t) * (size_t)nsb * 64))) return done(e);
-  if ((e = cudaMalloc(&ddist, sizeof(double) * (size_t)kLevels * nsb))) return done(e);
+  if ((e = cudaMalloc(&b.filt, sizeof(int16_t) * (size_t)w * h))) return done(e);
+  if ((e = cudaMalloc(&b.orig, sizeof(int32_t) * (size_t)nsb * 4096))) return done(e);
+  if ((e = cudaMalloc(&b.cand, sizeof(int32_t) * (size_t)nsb * 4096))) return done(e);
+  if ((e = cudaMalloc(&b.dir, sizeof(int32_t) * (size_t)nsb * 64))) return done(e);
+  if ((e = cudaMalloc(&b.dist, sizeof(double) * (size_t)kLevels * nsb))) return done(e);
   if (!p->bskip) {
     if ((e = cudaMalloc(&zskip, (size_t)nsb * 256))) return done(e);
     if ((e = cudaMemsetAsync(zskip, 0, (size_t)nsb * 256, st))) return done(e);
   }
-  const double base_threshold = pow((double)p->quantizer, 0.84182);   // src/encode.c:2694
-  for (int gi = 0; gi < kLevels; gi++) {
-    const int16_t* plane = p->etmp;
-    int pstride = p->etmp_stride;
-    if (gi) {
-      daala_b200_dering_params dp;
-      memset(&dp, 0, sizeof(dp));
-      dp.y = filt;
-      dp.x = p->etmp;
-      dp.dir = dir;
-      dp.bskip = p->bskip ? p->bskip : zskip;
-      dp.ystride = w;
-      dp.xstride = p->etmp_stride;
-      dp.dir_stride = nhsb * 8;
-      dp.skip_stride = skip_stride;
-      dp.nhsb = nhsb;
-      dp.nvsb = nvsb;
-      dp.threshold = (int)(kGain[gi] * base_threshold);
-      dp.overlap = 1;
-      dp.coeff_shift = 4;
-      int r = daala_b200_dering_plane(&dp, st);
-      if (r) return done((cudaError_t)r);
-      plane = filt;
-      pstride = w;
-    }
-    k_pack_sb<<<nsb, 256, 0, st>>>(plane, pstride, p->src, p->src_stride, nhsb, cand, gi == 0 ? orig : nullptr);
-    if ((e = cudaGetLastError())) return done(e);
-    int r = daala_b200_compute_dist(orig, cand, nsb, 64, p->qm_is_flat, p->use_activity_masking, p->coded_quantizer,
-                                    ddist + (size_t)gi * nsb, st);
-    if (r) return done((cudaError_t)r);
-  }
+  b.etmp = p->etmp;
+  b.src = p->src;
+  b.etmp_stride = p->etmp_stride;
+  b.src_stride = p->src_stride;
+  b.nframes = 1;
+  b.nhsb = nhsb;
+  b.nvsb = nvsb;
+  int tbl[2][6];
+  daala_b200_dering_threshold_table(p->quantizer, tbl);
+  memcpy(b.threshold, tbl[0], sizeof(b.threshold));
+  b.coded_quantizer = p->coded_quantizer;
+  b.qm_is_flat = p->qm_is_flat;
+  b.use_activity_masking = p->use_activity_masking;
+  b.bskip = p->bskip ? p->bskip : zskip;
+  b.skip_stride = skip_stride;
+  const int rc = enqueue_candidates(&b, st);
+  if (rc) return done((cudaError_t)rc);
   std::vector<double> hdist((size_t)kLevels * nsb);
-  if ((e = cudaMemcpyAsync(hdist.data(), ddist, sizeof(double) * hdist.size(), cudaMemcpyDeviceToHost, st))) return done(e);
+  if ((e = cudaMemcpyAsync(hdist.data(), b.dist, sizeof(double) * hdist.size(), cudaMemcpyDeviceToHost, st))) return done(e);
   // superblocks whose 4x4 blocks are all skipped are neither searched nor signalled
   std::vector<uint8_t> coded;
   if (p->bskip) {
@@ -268,46 +290,9 @@ extern "C" int daala_b200_dering_search_enqueue(const daala_b200_dering_search_b
       b->nframes < 1 || b->nhsb < 1 || b->nvsb < 1 || b->skip_stride < b->nhsb * 16 || b->skip_pitch < 0)
     return (int)cudaErrorInvalidValue;
   cudaStream_t st = (cudaStream_t)stream_;
-  const int nsb = b->nhsb * b->nvsb, F = b->nframes;
-  const int w = b->nhsb * 64, h = b->nvsb * 64;
-  const long long filt_pitch = (long long)w * h;
-  for (int gi = 0; gi < kLevels; gi++) {
-    const int16_t* plane = b->etmp;
-    long long ppitch = b->etmp_pitch;
-    int pstride = b->etmp_stride;
-    if (gi) {
-      daala_b200_dering_params dp;
-      memset(&dp, 0, sizeof(dp));
-      dp.y = b->filt;
-      dp.x = b->etmp;
-      dp.dir = b->dir;
-      dp.bskip = b->bskip;
-      dp.ystride = w;
-      dp.xstride = b->etmp_stride;
-      dp.dir_stride = b->nhsb * 8;
-      dp.skip_stride = b->skip_stride;
-      dp.nhsb = b->nhsb;
-      dp.nvsb = b->nvsb;
-      dp.threshold = b->threshold[gi];
-      dp.overlap = 1;
-      dp.coeff_shift = 4;
-      dp.dir_format = gi == 1 ? 1 : 2;   // the direction search runs once; later passes re-use direction and variance
-      const int r = daala_b200_dering_plane_batch_skip(&dp, F, filt_pitch, b->etmp_pitch, (long long)nsb * 64, 0,
-                                                       b->skip_pitch, nullptr, st);
-      if (r) return r;
-      plane = b->filt;
-      ppitch = filt_pitch;
-      pstride = w;
-    }
-    k_pack_sb_batch<<<dim3(nsb, F), 256, 0, st>>>(plane, ppitch, pstride, b->src, b->src_pitch, b->src_stride, b->nhsb,
-                                                  b->cand, gi == 0 ? b->orig : nullptr);
-    cudaError_t e = cudaGetLastError();
-    if (e) return (int)e;
-    const int r = daala_b200_compute_dist(b->orig, b->cand, F * nsb, 64, b->qm_is_flat, b->use_activity_masking,
-                                          b->coded_quantizer, b->dist + (size_t)gi * F * nsb, st);
-    if (r) return r;
-  }
-  k_dering_decide<<<(F + 31) / 32, 32, 0, st>>>(b->dist, F, b->nhsb, b->nvsb, b->dering_lambda, b->coded,
-                                                b->is_keyframe, b->levels);
+  const int r = enqueue_candidates(b, st);
+  if (r) return r;
+  k_dering_decide<<<(b->nframes + 31) / 32, 32, 0, st>>>(b->dist, b->nframes, b->nhsb, b->nvsb, b->dering_lambda,
+                                                         b->coded, b->is_keyframe, b->levels);
   return (int)cudaGetLastError();
 }

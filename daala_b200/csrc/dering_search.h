@@ -4,6 +4,8 @@
 #pragma once
 #include <stdint.h>
 
+#include "daala_b200.h"
+
 struct daala_b200_dering_search_batch {
   const int16_t* etmp;      // [F] luma planes after the SB-edge postfilter (state->etmp[0]), row stride = width
   const uint8_t* src;       // [F] source luma planes
@@ -30,3 +32,14 @@ struct daala_b200_dering_search_batch {
   uint8_t* levels;          // out: [F][nvsb * nhsb]
 };
 extern "C" int daala_b200_dering_search_enqueue(const daala_b200_dering_search_batch* b, void* stream);
+
+// The deringing threshold of every level at `quantizer` (src/encode.c:2697, :2822): tbl[0][g] luma,
+// (int)(OD_DERING_GAIN_TABLE[g] * quantizer^0.84182); tbl[1][g] chroma, the same product * 0.6.
+void daala_b200_dering_threshold_table(int quantizer, int tbl[2][6]);
+
+// od_dering of `nframes` planes of one geometry in one launch (csrc/dering_kernels.cu): element pitches between the
+// frames' planes, direction maps and threshold maps, skip_pitch bytes between their skip maps (0: one map for every
+// frame); y8 (nullable) receives the u8 reconstruction instead of the int16 plane.
+int daala_b200_dering_plane_frames(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
+                                   long long x_pitch, long long dir_pitch, long long thr_pitch, long long skip_pitch,
+                                   uint8_t* y8, void* stream);

@@ -34,6 +34,8 @@
 #include <string.h>
 
 #include <mutex>
+#include <new>
+#include <vector>
 
 #include "daala_b200.h"
 #include "dering_search.h"
@@ -1559,12 +1561,24 @@ extern "C" int daala_b200_launch_forward(const daala_b200_frame* prm, int nplane
 extern "C" int daala_b200_launch_inverse(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
 extern "C" int daala_b200_launch_inverse_lapped_only(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
 extern "C" int daala_b200_launch_sb_postfilter_store(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
-extern "C" int daala_b200_dering_plane_batch(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
-                                             long long x_pitch, long long dir_pitch, long long thr_pitch, uint8_t* y8,
-                                             void* stream);
-extern "C" int daala_b200_dering_plane_batch_skip(const daala_b200_dering_params* prm, int nframes, long long y_pitch,
-                                                  long long x_pitch, long long dir_pitch, long long thr_pitch,
-                                                  long long skip_pitch, uint8_t* y8, void* stream);
+
+// One deringing pass over the batch (od_encode_coefficients' final application, src/encode.c:2812-2842): the step's on
+// keyframes (config.dering) or the finishing pass's on P frames (config.inter_finish).  The two differ only in the data
+// below, so enqueue_dering runs either.
+struct Dering {
+  daala_b200_frame frame;          // the planes it inverts; post16 = etmp, pixels_out = the u8 reconstruction
+  const uint8_t* skip[3];          // per plane: [F][plane_h / 4][skip_stride], skip_pitch[p] apart (0: one map)
+  long long skip_pitch[3];
+  int skip_stride;
+  uint8_t* level;                  // [F][nvsb][nhsb]: what the thresholds read and the search writes
+  const uint8_t* coded;            // nullable: superblocks with a coded luma 4x4 unit; the others get level 0 ...
+  uint8_t* applied;                // ... and the level applied lands here
+  int tbl[2][6];                   // luma / chroma threshold per level
+  int32_t* thr[2];                 // luma / chroma threshold per superblock
+  int32_t* dir;                    // [F][nvsb*8][nhsb*8]
+  bool search;                     // the level search runs first, described by `sb`
+  daala_b200_dering_search_batch sb;
+};
 
 struct daala_b200_kf {
   daala_b200_kf_config cfg;
@@ -1597,17 +1611,7 @@ struct daala_b200_kf {
   int16_t* lv_snap;
   int32_t* lv_bar;
   int lvl_slots, lvl_grid;
-  // deringing stage
-  uint8_t* dering_level;           // [F][nvsb][nhsb]
-  int32_t *dering_thr[2];          // luma / chroma thresholds per superblock
-  int16_t* dering_in[3];           // etmp: the planes after the SB-edge postfilter
-  int16_t* dering_filt;            // level search (cfg.dering == 2 or inter_finish == 2): one filtered luma candidate, [F][h][w]
-  int32_t* dering_dir;             // [F][nvsb*8][nhsb*8]
-  uint8_t* dering_skip;            // all zero: keyframes never mark a block skipped (src/encode.c:1690)
-  int dering_tbl[2][6];
-  // level search (cfg.dering == 2 or inter_finish == 2): packed superblock pairs and the 6 x F x nsb distortions
-  int32_t *dering_orig, *dering_cand;
-  double* dering_dist;
+  Dering dering;                   // cfg.dering or cfg.inter_finish
   Lists lists;
   Stage luma, chroma;
   Sym sym;                         // symbol stream (cfg.symbol_stream); zero otherwise
@@ -1620,16 +1624,15 @@ struct daala_b200_kf {
   uint32_t* mc_leaves;
   int32_t* mc_nleaves;
   daala_b200_mc_batch mc;
-  // cfg.inter_finish: the finishing pass's inputs (decisions per block, levels), its planes (patched coefficients,
-  // inverted in place; etmp; the reconstruction), the skip maps, the superblock flags, and its own CUDA graph
+  // cfg.inter_finish: the finishing pass's inputs (decisions per block), its planes (patched coefficients, inverted in
+  // place; the reconstruction), the skip maps, the superblock flags, the levels applied, and its own CUDA graph
   uint8_t* fin_skip[2];
   int32_t* fin_dc[2];
   int32_t* dc_resid[2];
   int32_t* fin_coeffs[3];
-  int16_t* fin_post16[3];
   uint8_t* fin_pixels[3];
   uint8_t* fin_bskip[3];
-  uint8_t *fin_level_in, *fin_level, *fin_coded;
+  uint8_t *fin_level, *fin_coded;
   Fin fin;
   cudaGraph_t fin_graph;
   cudaGraphExec_t fin_exec;
@@ -1637,6 +1640,7 @@ struct daala_b200_kf {
   int fin_dc_limit;                // largest |dc| finish accepts: DAALA_B200_KF_FINISH_DC_LIMIT / the largest dc_quant
   bool have_step;                  // a step has been submitted; last_tot are its totals
   daala_b200_kf_totals last_tot;
+  std::vector<void*> allocs;       // every device buffer dalloc made; daala_b200_kf_destroy frees these
   size_t bytes_allocated;
   size_t chain_cap;                // entries of the chain queue (heads / ring)
   int sms;
@@ -1657,6 +1661,7 @@ static cudaError_t dalloc(daala_b200_kf* kf, T** p, size_t n) {
   const size_t bytes = (n ? n : 1) * sizeof(T);
   cudaError_t e = cudaMalloc((void**)p, bytes);
   if (e == cudaSuccess) {
+    kf->allocs.push_back(*p);
     kf->bytes_allocated += bytes;
     e = cudaMemset(*p, 0, bytes);
   }
@@ -1968,30 +1973,6 @@ static int kf_alloc(daala_b200_kf* kf) {
     kf->frame_pred.plane[p].pixels = kf->pred_pixels[p];
     kf->frame_pred.plane[p].coeffs = kf->pred_coeffs[p];
   }
-  if (kf->cfg.dering) {
-    const size_t nsb = (size_t)F * kf->nhsb * kf->nvsb;
-    KF_CHECK(dalloc(kf, &kf->dering_level, nsb));
-    KF_CHECK(dalloc(kf, &kf->dering_thr[0], nsb));
-    KF_CHECK(dalloc(kf, &kf->dering_thr[1], nsb));
-    KF_CHECK(dalloc(kf, &kf->dering_dir, nsb * 64));
-    KF_CHECK(dalloc(kf, &kf->dering_skip, nsb * 256 + 64));
-    for (int p = 0; p < 3; p++) KF_CHECK(dalloc(kf, &kf->dering_in[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F));
-    if (kf->cfg.dering == 2) {
-      KF_CHECK(dalloc(kf, &kf->dering_filt, (size_t)kf->plane_w[0] * kf->plane_h[0] * F));
-      KF_CHECK(dalloc(kf, &kf->dering_orig, nsb * 4096));
-      KF_CHECK(dalloc(kf, &kf->dering_cand, nsb * 4096));
-      KF_CHECK(dalloc(kf, &kf->dering_dist, nsb * 6));
-    }
-  }
-  {
-    // thresholds per level: (int)(OD_DERING_GAIN_TABLE[gi] * pow(quantizer, 0.84182) * (luma ? 1 : 0.6)), src/encode.c:2697,2822
-    const double gain[6] = {0, 0.5, 0.707, 1, 1.41, 2};
-    const double base = pow((double)kf->cfg.q0, 0.84182);
-    for (int g = 0; g < 6; g++) {
-      kf->dering_tbl[0][g] = (int)(gain[g] * base * 1);
-      kf->dering_tbl[1][g] = (int)(gain[g] * base * 0.6);
-    }
-  }
   if (kf->cfg.inter_finish) {
     const size_t nsb = (size_t)F * kf->nhsb * kf->nvsb;
     Fin& P = kf->fin;
@@ -2012,7 +1993,6 @@ static int kf_alloc(daala_b200_kf* kf) {
     for (int p = 0; p < 3; p++) {
       const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
       KF_CHECK(dalloc(kf, &kf->fin_coeffs[p], n));
-      KF_CHECK(dalloc(kf, &kf->fin_post16[p], n));
       KF_CHECK(dalloc(kf, &kf->fin_pixels[p], n));
       P.skip_pitch[p] = (long long)(kf->plane_h[p] / 4) * P.skip_stride;
       KF_CHECK(dalloc(kf, &kf->fin_bskip[p], (size_t)P.skip_pitch[p] * F));
@@ -2023,19 +2003,8 @@ static int kf_alloc(daala_b200_kf* kf) {
       P.plane_stride[p] = kf->plane_w[p];
       P.bskip[p] = kf->fin_bskip[p];
     }
-    KF_CHECK(dalloc(kf, &kf->fin_level_in, nsb));
     KF_CHECK(dalloc(kf, &kf->fin_level, nsb));
     KF_CHECK(dalloc(kf, &kf->fin_coded, nsb));
-    KF_CHECK(dalloc(kf, &kf->dering_thr[0], nsb));
-    KF_CHECK(dalloc(kf, &kf->dering_thr[1], nsb));
-    KF_CHECK(dalloc(kf, &kf->dering_dir, nsb * 64));
-    if (kf->cfg.inter_finish == 2) {
-      // the level search's scratch, in the keyframe search's fields (dering and inter exclude each other)
-      KF_CHECK(dalloc(kf, &kf->dering_filt, (size_t)kf->plane_w[0] * kf->plane_h[0] * F));
-      KF_CHECK(dalloc(kf, &kf->dering_orig, nsb * 4096));
-      KF_CHECK(dalloc(kf, &kf->dering_cand, nsb * 4096));
-      KF_CHECK(dalloc(kf, &kf->dering_dist, nsb * 6));
-    }
     P.coded = kf->fin_coded;
     P.nhsb = kf->nhsb;
     P.nvsb = kf->nvsb;
@@ -2049,6 +2018,65 @@ static int kf_alloc(daala_b200_kf* kf) {
       }
     kf->fin_dc_limit = DAALA_B200_KF_FINISH_DC_LIMIT / dq_max;
   }
+  // the deringing pass: the step's on keyframes (cfg.dering) or the finishing pass's (cfg.inter_finish); inter refuses
+  // dering, so an engine has at most one.  Level 2 of either searches the levels first.
+  const int dering = kf->cfg.dering ? kf->cfg.dering : kf->cfg.inter_finish;
+  if (dering) {
+    const size_t nsb = (size_t)F * kf->nhsb * kf->nvsb;
+    Dering& D = kf->dering;
+    D.frame = kf->frame;
+    D.skip_stride = kf->nhsb * 16;
+    uint8_t* zero_skip = nullptr;   // keyframes never mark a block skipped (src/encode.c:1690): one map for all frames
+    if (!kf->cfg.inter_finish) KF_CHECK(dalloc(kf, &zero_skip, nsb * 256 + 64));
+    for (int p = 0; p < 3; p++) {
+      KF_CHECK(dalloc(kf, &D.frame.post16[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F));
+      if (kf->cfg.inter_finish) {
+        // the patched coefficients, inverted in place (k_inverse_sb only touches its own superblock)
+        D.frame.plane[p].coeffs = D.frame.plane[p].lapped = kf->fin_coeffs[p];
+        D.frame.plane[p].pixels_out = kf->fin_pixels[p];
+        D.skip[p] = kf->fin_bskip[p];
+        D.skip_pitch[p] = kf->fin.skip_pitch[p];
+      } else {
+        D.skip[p] = zero_skip;
+      }
+    }
+    KF_CHECK(dalloc(kf, &D.level, nsb));
+    KF_CHECK(dalloc(kf, &D.thr[0], nsb));
+    KF_CHECK(dalloc(kf, &D.thr[1], nsb));
+    KF_CHECK(dalloc(kf, &D.dir, nsb * 64));
+    D.coded = kf->fin_coded;
+    D.applied = kf->fin_level;
+    daala_b200_dering_threshold_table(kf->cfg.q0, D.tbl);
+    D.search = dering == 2;
+    if (D.search) {
+      // src/encode.c:2708-2811 for every frame of the batch.  P frames (src/encode.c:2720-2811): the frame's own skip
+      // map under every candidate, superblocks without a coded luma 4x4 unit neither scored nor adapted, context 0
+      daala_b200_dering_search_batch& b = D.sb;
+      b.etmp = D.frame.post16[0];
+      b.src = kf->pixels[0];
+      b.etmp_pitch = b.src_pitch = (long long)kf->plane_w[0] * kf->plane_h[0];
+      b.etmp_stride = b.src_stride = kf->plane_w[0];
+      b.nframes = F;
+      b.nhsb = kf->nhsb;
+      b.nvsb = kf->nvsb;
+      memcpy(b.threshold, D.tbl[0], sizeof(b.threshold));
+      b.coded_quantizer = kf->cfg.coded_quantizer;
+      b.qm_is_flat = kf->cfg.qm_is_flat;
+      b.use_activity_masking = kf->cfg.use_masking;
+      b.dering_lambda = kf->cfg.dering_lambda;
+      b.bskip = D.skip[0];
+      b.skip_stride = D.skip_stride;
+      b.skip_pitch = D.skip_pitch[0];
+      b.coded = D.coded;
+      b.is_keyframe = inter ? 0 : 1;
+      KF_CHECK(dalloc(kf, &b.filt, (size_t)kf->plane_w[0] * kf->plane_h[0] * F));
+      KF_CHECK(dalloc(kf, &b.orig, nsb * 4096));
+      KF_CHECK(dalloc(kf, &b.cand, nsb * 4096));
+      KF_CHECK(dalloc(kf, &b.dist, nsb * 6));
+      b.dir = D.dir;
+      b.levels = D.level;   // what the thresholds read; on P frames its level 0 agrees with the forced one
+    }
+  }
   // dalloc's cudaMemset runs on the legacy default stream, asynchronously, and the engine's stream does not
   // synchronise with it (cudaStreamNonBlocking): wait for every clear before anything is launched -- the table
   // fill below used to race with the clear of its own buffer (intermittently all-zero 1/sqrt table)
@@ -2058,6 +2086,52 @@ static int kf_alloc(daala_b200_kf* kf) {
   KF_CHECK(cudaStreamSynchronize(kf->stream));
   return 0;
 }
+
+// The deringing pass D over the whole batch: iDCT + split postfilters -> lapped planes; SB-edge postfilter -> etmp
+// (int16, the fused kernel's optional output); [the level search -> D.level]; thresholds per superblock; od_dering of
+// all frames per plane in one launch, luma first (it writes the direction map chroma reads), storing the u8
+// reconstruction.
+static int enqueue_dering(daala_b200_kf* kf, const Dering& D, cudaStream_t s) {
+  int rc = daala_b200_launch_inverse_lapped_only(&D.frame, 3, s);
+  if (!rc) rc = daala_b200_launch_sb_postfilter_store(&D.frame, 3, s);
+  if (!rc && D.search) rc = daala_b200_dering_search_enqueue(&D.sb, s);
+  if (rc) return rc;
+  const int nsb = kf->nhsb * kf->nvsb;
+  k_dering_thresholds<<<(kf->F * nsb + 255) / 256, 256, 0, s>>>(
+      D.level, D.thr[0], D.thr[1], kf->F * nsb, make_int4(D.tbl[0][0], D.tbl[0][1], D.tbl[0][2], D.tbl[0][3]),
+      make_int2(D.tbl[0][4], D.tbl[0][5]), make_int4(D.tbl[1][0], D.tbl[1][1], D.tbl[1][2], D.tbl[1][3]),
+      make_int2(D.tbl[1][4], D.tbl[1][5]), D.coded, D.applied);
+  for (int p = 0; p < 3; p++) {
+    const long long per = (long long)kf->plane_w[p] * kf->plane_h[p];
+    daala_b200_dering_params dp;
+    memset(&dp, 0, sizeof(dp));
+    dp.y = nullptr;   // u8 output only
+    dp.x = D.frame.post16[p];
+    dp.dir = D.dir;
+    dp.bskip = D.skip[p];
+    dp.sb_threshold = D.thr[p ? 1 : 0];
+    dp.ystride = dp.xstride = kf->plane_w[p];
+    dp.dir_stride = kf->nhsb * 8;
+    dp.skip_stride = D.skip_stride;
+    dp.nhsb = kf->nhsb;
+    dp.nvsb = kf->nvsb;
+    dp.xdec = p ? 1 : 0;
+    dp.pli = p;
+    dp.overlap = 1;      // OD_DERING_CHECK_OVERLAP
+    dp.coeff_shift = 4;  // OD_COEFF_SHIFT
+    // after a search the direction map is already there, packed with the variance; neither depends on the skip map
+    // (src/dering.c:280-287)
+    dp.dir_format = D.search ? 2 : 0;
+    rc = daala_b200_dering_plane_frames(&dp, kf->F, per, per, (long long)nsb * 64, nsb, D.skip_pitch[p],
+                                        D.frame.plane[p].pixels_out, s);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+// Kernel launches of enqueue_dering: inverse, SB postfilter -> int16, [level search: 5 filtered candidates, 6 packs,
+// 6 distortion passes, decision], thresholds, dering + u8 store per plane.
+static int dering_launches(const Dering& D) { return 1 + 1 + (D.search ? 5 + 6 + 6 + 1 : 0) + 1 + 3; }
 
 // Everything between "inputs are in HBM" and "results are in HBM", on kf->stream.
 // the three phase kernels over every chunk of every class of a stage's dependency-free lists
@@ -2185,169 +2259,25 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
       k_sym_index<<<1, 256, 0, s>>>(Y);
     }
   }
-  if ((phases & DAALA_B200_KF_INVERSE) && !kf->cfg.dering) {
-    int rc = daala_b200_launch_inverse(&kf->frame, 3, s);
+  if (phases & DAALA_B200_KF_INVERSE) {
+    int rc = kf->cfg.dering ? enqueue_dering(kf, kf->dering, s) : daala_b200_launch_inverse(&kf->frame, 3, s);
     if (rc) return rc;
-  }
-  if ((phases & DAALA_B200_KF_INVERSE) && kf->cfg.dering) {
-    // iDCT + split postfilters -> lapped planes; SB-edge postfilter -> etmp (int16, the fused kernel's optional
-    // output); od_dering of all frames per plane in one launch, luma first (it writes the direction map chroma
-    // reads), storing the u8 reconstruction
-    int rc = daala_b200_launch_inverse_lapped_only(&kf->frame, 3, s);
-    if (rc) return rc;
-    daala_b200_frame f16 = kf->frame;
-    for (int p = 0; p < 3; p++) f16.post16[p] = kf->dering_in[p];
-    rc = daala_b200_launch_sb_postfilter_store(&f16, 3, s);
-    if (rc) return rc;
-    const int nsb = kf->nhsb * kf->nvsb;
-    const bool search = kf->cfg.dering == 2;
-    if (search) {
-      // the level search of src/encode.c:2708-2811 for every frame of the batch: levels -> kf->dering_level
-      daala_b200_dering_search_batch sb;
-      memset(&sb, 0, sizeof(sb));
-      sb.etmp = kf->dering_in[0];
-      sb.src = kf->pixels[0];
-      sb.etmp_pitch = sb.src_pitch = (long long)kf->plane_w[0] * kf->plane_h[0];
-      sb.etmp_stride = sb.src_stride = kf->plane_w[0];
-      sb.nframes = kf->F;
-      sb.nhsb = kf->nhsb;
-      sb.nvsb = kf->nvsb;
-      for (int g = 0; g < 6; g++) sb.threshold[g] = kf->dering_tbl[0][g];
-      sb.coded_quantizer = kf->cfg.coded_quantizer;
-      sb.qm_is_flat = kf->cfg.qm_is_flat;
-      sb.use_activity_masking = kf->cfg.use_masking;
-      sb.dering_lambda = kf->cfg.dering_lambda;
-      sb.filt = kf->dering_filt;
-      sb.orig = kf->dering_orig;
-      sb.cand = kf->dering_cand;
-      sb.dir = kf->dering_dir;
-      sb.bskip = kf->dering_skip;   // one all-zero map for every frame
-      sb.skip_stride = kf->nhsb * 16;
-      sb.skip_pitch = 0;
-      sb.coded = nullptr;
-      sb.is_keyframe = 1;
-      sb.dist = kf->dering_dist;
-      sb.levels = kf->dering_level;
-      rc = daala_b200_dering_search_enqueue(&sb, s);
-      if (rc) return rc;
-    }
-    k_dering_thresholds<<<(kf->F * nsb + 255) / 256, 256, 0, s>>>(
-        kf->dering_level, kf->dering_thr[0], kf->dering_thr[1], kf->F * nsb,
-        make_int4(kf->dering_tbl[0][0], kf->dering_tbl[0][1], kf->dering_tbl[0][2], kf->dering_tbl[0][3]),
-        make_int2(kf->dering_tbl[0][4], kf->dering_tbl[0][5]),
-        make_int4(kf->dering_tbl[1][0], kf->dering_tbl[1][1], kf->dering_tbl[1][2], kf->dering_tbl[1][3]),
-        make_int2(kf->dering_tbl[1][4], kf->dering_tbl[1][5]));
-    for (int p = 0; p < 3; p++) {
-      const long long per = (long long)kf->plane_w[p] * kf->plane_h[p];
-      daala_b200_dering_params dp;
-      memset(&dp, 0, sizeof(dp));
-      dp.y = nullptr;   // u8 output only
-      dp.x = kf->dering_in[p];
-      dp.dir = kf->dering_dir;
-      dp.bskip = kf->dering_skip;
-      dp.sb_threshold = kf->dering_thr[p ? 1 : 0];
-      dp.ystride = dp.xstride = kf->plane_w[p];
-      dp.dir_stride = kf->nhsb * 8;
-      dp.skip_stride = kf->nhsb * 16;
-      dp.nhsb = kf->nhsb;
-      dp.nvsb = kf->nvsb;
-      dp.xdec = p ? 1 : 0;
-      dp.pli = p;
-      dp.threshold = 0;
-      dp.overlap = 1;      // OD_DERING_CHECK_OVERLAP
-      dp.coeff_shift = 4;  // OD_COEFF_SHIFT
-      dp.dir_format = search ? 2 : 0;   // after a search the direction map is already there (packed with the variance)
-      rc = daala_b200_dering_plane_batch(&dp, kf->F, per, per, (long long)nsb * 64, nsb, kf->pixels_out[p], s);
-      if (rc) return rc;
-    }
   }
   return (int)cudaGetLastError();
 }
 
 // config.inter_finish: the kernels of the finishing pass, between the H2D of the decisions / levels and the D2H of
-// the results.  Patch and skip map, the inverse in place on the patched plane (iDCT + split postfilters), SB-edge
-// postfilter -> etmp (int16), [inter_finish = 2: the level search of src/encode.c:2708-2811 on etmp, the step's
-// source luma and the pass's skip maps -> fin_level_in], thresholds with the forced level 0, od_dering of every plane
-// with the real skip maps storing the u8 reconstruction.
+// the results.  Patch and skip map, then the deringing pass with the real skip maps (enqueue_dering: the inverse in
+// place on the patched plane, [inter_finish = 2: the level search], thresholds with the forced level 0, od_dering).
 static int kf_enqueue_finish(daala_b200_kf* kf) {
   cudaStream_t s = kf->stream;
   const int wide = kf->sms * 8;
-  const int nsb = kf->nhsb * kf->nvsb;
-  if (cudaMemsetAsync(kf->fin_coded, 0, (size_t)kf->F * nsb, s) != cudaSuccess) return (int)cudaGetLastError();
+  if (cudaMemsetAsync(kf->fin_coded, 0, (size_t)kf->F * kf->nhsb * kf->nvsb, s) != cudaSuccess)
+    return (int)cudaGetLastError();
   k_fin_patch<<<wide, 256, 0, s>>>(kf->fin);
   k_fin_skip_map<<<wide, 256, 0, s>>>(kf->fin);
-  daala_b200_frame f = kf->frame;
-  for (int p = 0; p < 3; p++) {
-    f.plane[p].coeffs = f.plane[p].lapped = kf->fin_coeffs[p];   // k_inverse_sb only touches its own superblock
-    f.plane[p].pixels_out = kf->fin_pixels[p];
-    f.post16[p] = kf->fin_post16[p];
-  }
-  int rc = daala_b200_launch_inverse_lapped_only(&f, 3, s);
-  if (!rc) rc = daala_b200_launch_sb_postfilter_store(&f, 3, s);
+  const int rc = enqueue_dering(kf, kf->dering, s);
   if (rc) return rc;
-  const bool search = kf->cfg.inter_finish == 2;
-  if (search) {
-    // the P-frame form of the keyframe search: the frame's own skip maps under every filtered candidate, superblocks
-    // without a coded luma 4x4 unit neither scored nor adapted, context 0 (src/encode.c:2720-2811)
-    daala_b200_dering_search_batch sb;
-    memset(&sb, 0, sizeof(sb));
-    sb.etmp = kf->fin_post16[0];
-    sb.src = kf->pixels[0];
-    sb.etmp_pitch = sb.src_pitch = (long long)kf->plane_w[0] * kf->plane_h[0];
-    sb.etmp_stride = sb.src_stride = kf->plane_w[0];
-    sb.nframes = kf->F;
-    sb.nhsb = kf->nhsb;
-    sb.nvsb = kf->nvsb;
-    for (int g = 0; g < 6; g++) sb.threshold[g] = kf->dering_tbl[0][g];
-    sb.coded_quantizer = kf->cfg.coded_quantizer;
-    sb.qm_is_flat = kf->cfg.qm_is_flat;
-    sb.use_activity_masking = kf->cfg.use_masking;
-    sb.dering_lambda = kf->cfg.dering_lambda;
-    sb.bskip = kf->fin_bskip[0];
-    sb.skip_stride = kf->fin.skip_stride;
-    sb.skip_pitch = kf->fin.skip_pitch[0];
-    sb.coded = kf->fin_coded;
-    sb.is_keyframe = 0;
-    sb.filt = kf->dering_filt;
-    sb.orig = kf->dering_orig;
-    sb.cand = kf->dering_cand;
-    sb.dir = kf->dering_dir;
-    sb.dist = kf->dering_dist;
-    sb.levels = kf->fin_level_in;   // what the thresholds read; its level 0 agrees with the forced one
-    rc = daala_b200_dering_search_enqueue(&sb, s);
-    if (rc) return rc;
-  }
-  k_dering_thresholds<<<(kf->F * nsb + 255) / 256, 256, 0, s>>>(
-      kf->fin_level_in, kf->dering_thr[0], kf->dering_thr[1], kf->F * nsb,
-      make_int4(kf->dering_tbl[0][0], kf->dering_tbl[0][1], kf->dering_tbl[0][2], kf->dering_tbl[0][3]),
-      make_int2(kf->dering_tbl[0][4], kf->dering_tbl[0][5]),
-      make_int4(kf->dering_tbl[1][0], kf->dering_tbl[1][1], kf->dering_tbl[1][2], kf->dering_tbl[1][3]),
-      make_int2(kf->dering_tbl[1][4], kf->dering_tbl[1][5]), kf->fin_coded, kf->fin_level);
-  for (int p = 0; p < 3; p++) {
-    const long long per = (long long)kf->plane_w[p] * kf->plane_h[p];
-    daala_b200_dering_params dp;
-    memset(&dp, 0, sizeof(dp));
-    dp.y = nullptr;   // u8 output only
-    dp.x = kf->fin_post16[p];
-    dp.dir = kf->dering_dir;
-    dp.bskip = kf->fin_bskip[p];
-    dp.sb_threshold = kf->dering_thr[p ? 1 : 0];
-    dp.ystride = dp.xstride = kf->plane_w[p];
-    dp.dir_stride = kf->nhsb * 8;
-    dp.skip_stride = kf->fin.skip_stride;
-    dp.nhsb = kf->nhsb;
-    dp.nvsb = kf->nvsb;
-    dp.xdec = p ? 1 : 0;
-    dp.pli = p;
-    dp.overlap = 1;      // OD_DERING_CHECK_OVERLAP
-    dp.coeff_shift = 4;  // OD_COEFF_SHIFT
-    // after a search the direction map is already there, packed with the variance; neither depends on the skip map
-    // (src/dering.c:280-287)
-    dp.dir_format = search ? 2 : 0;
-    rc = daala_b200_dering_plane_batch_skip(&dp, kf->F, per, per, (long long)nsb * 64, nsb, kf->fin.skip_pitch[p],
-                                            kf->fin_pixels[p], s);
-    if (rc) return rc;
-  }
   return (int)cudaGetLastError();
 }
 
@@ -2388,7 +2318,7 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   if (!cfg || cfg->pic_w <= 0 || cfg->pic_h <= 0 || cfg->nframes <= 0 || cfg->nframes > 255 || !cfg->qm ||
       !cfg->qm_inv || cfg->qm_stride <= 0)
     return nullptr;
-  daala_b200_kf* kf = (daala_b200_kf*)calloc(1, sizeof(daala_b200_kf));
+  daala_b200_kf* kf = new (std::nothrow) daala_b200_kf();   // value-initialised: every field zero
   if (!kf) return nullptr;
   kf->cfg = *cfg;
   if (kf->cfg.level_chains && kf->cfg.split_free < 2) kf->cfg.split_free = 2;   // the level kernel only walks the chains
@@ -2407,13 +2337,13 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   }
   // coefficient offsets are 32-bit (ADVICE r1): the whole batch must stay below 2^31 coded coefficients
   if ((long long)kf->plane_w[0] * kf->plane_h[0] * kf->F >= (1ll << 31)) {
-    free(kf);
+    delete kf;
     return nullptr;
   }
   int dev = 0;
   cudaDeviceProp prop;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess) {
-    free(kf);
+    delete kf;
     return nullptr;
   }
   kf->sms = prop.multiProcessorCount;
@@ -2421,7 +2351,7 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
     kf->stream = (cudaStream_t)cfg->stream;
   } else {
     if (cudaStreamCreateWithFlags(&kf->stream, cudaStreamNonBlocking) != cudaSuccess) {
-      free(kf);
+      delete kf;
       return nullptr;
     }
     kf->own_stream = true;
@@ -2443,115 +2373,9 @@ void daala_b200_kf_destroy(daala_b200_kf* kf) {
   if (kf->graph) cudaGraphDestroy(kf->graph);
   if (kf->fin_exec) cudaGraphExecDestroy(kf->fin_exec);
   if (kf->fin_graph) cudaGraphDestroy(kf->fin_graph);
-  for (int c = 0; c < 2; c++) {
-    cudaFree(kf->fin_skip[c]);
-    cudaFree(kf->fin_dc[c]);
-    cudaFree(kf->dc_resid[c]);
-  }
-  for (int p = 0; p < 3; p++) {
-    cudaFree(kf->fin_coeffs[p]);
-    cudaFree(kf->fin_post16[p]);
-    cudaFree(kf->fin_pixels[p]);
-    cudaFree(kf->fin_bskip[p]);
-  }
-  cudaFree(kf->fin_level_in);
-  cudaFree(kf->fin_level);
-  cudaFree(kf->fin_coded);
-  for (int p = 0; p < 3; p++) {
-    cudaFree(kf->pixels[p]);
-    cudaFree(kf->coeffs[p]);
-    cudaFree(kf->lapped[p]);
-    cudaFree(kf->pixels_out[p]);
-    cudaFree(kf->pred_pixels[p]);
-    cudaFree(kf->pred_coeffs[p]);
-    cudaFree(kf->ref_pixels[p]);
-  }
-  cudaFree(kf->ref_slot);
-  cudaFree(kf->mv_grid);
-  cudaFree(kf->mc_leaves);
-  cudaFree(kf->mc_nleaves);
-  cudaFree(kf->bsize);
-  cudaFree(kf->cfl_plane);
-  cudaFree(kf->qm);
-  cudaFree(kf->qm_inv);
-  cudaFree(kf->rsqrt_tbl);
-  for (int c = 0; c < 3; c++) {
-    cudaFree(kf->sp_vec[c]);
-    cudaFree(kf->sp_lanes[c]);
-    cudaFree(kf->sp_uni[c]);
-    cudaFree(kf->sp_snap[c]);
-  }
-  Lists& L = kf->lists;
-  cudaFree(L.tile_sum);
-  cudaFree(L.unit_lbase);
-  cudaFree(L.luma);
-  cudaFree(L.chroma);
-  cudaFree(L.dep_top);
-  cudaFree(L.dep_left);
-  for (int c = 0; c < 3; c++) {
-    cudaFree(L.items_l[c]);
-    cudaFree(L.items_c[c]);
-  }
-  cudaFree(L.heads);
-  cudaFree(L.heads_raw);
-  cudaFree(L.head_bin);
-  cudaFree(L.head_hist);
-  cudaFree(L.head_cursor);
-  cudaFree(L.heads0);
-  cudaFree(L.lvl_hist);
-  cudaFree(L.lvl_cursor);
-  cudaFree(L.lvl_items);
-  cudaFree(kf->lv_vec);
-  cudaFree(kf->lv_lanes);
-  cudaFree(kf->lv_uni);
-  cudaFree(kf->lv_snap);
-  cudaFree(kf->lv_bar);
-  cudaFree(kf->dering_level);
-  cudaFree(kf->dering_orig);
-  cudaFree(kf->dering_cand);
-  cudaFree(kf->dering_dist);
-  cudaFree(kf->dering_thr[0]);
-  cudaFree(kf->dering_thr[1]);
-  cudaFree(kf->dering_dir);
-  cudaFree(kf->dering_skip);
-  for (int p = 0; p < 3; p++) cudaFree(kf->dering_in[p]);
-  cudaFree(kf->dering_filt);
-  cudaFree(L.succ_bottom);
-  cudaFree(L.succ_right);
-  cudaFree(L.cnt);
-  Sym& Y = kf->sym;
-  cudaFree(Y.unit_rank);
-  cudaFree(Y.sb_cnt);
-  cudaFree(Y.sb_base);
-  cudaFree(Y.order);
-  cudaFree(Y.off);
-  cudaFree(Y.tile);
-  cudaFree(Y.tot);
-  cudaFree(Y.index);
-  cudaFree(Y.blocks);
-  cudaFree(Y.bands);
-  cudaFree(Y.pulses);
-  for (Stage* S : {&kf->luma, &kf->chroma}) {
-    cudaFree(S->prm.in);
-    cudaFree(S->prm.ref);
-    cudaFree(S->prm.out);
-    cudaFree(S->prm.y);
-    cudaFree(S->prm.y16);
-    cudaFree(S->prm.res_skip_term);
-    cudaFree(S->prm.res_skip_diff);
-    cudaFree(S->prm.res_flip);
-    cudaFree(S->prm.res_dc);
-    cudaFree(S->res_pack);
-    cudaFree(S->ring);
-    cudaFree(S->join0);
-    cudaFree(S->pre_ev);
-    cudaFree(S->pre_snap);
-#ifdef DAALA_B200_CHAIN_TRACE
-    cudaFree(S->trace);
-#endif
-  }
+  for (void* p : kf->allocs) cudaFree(p);
   if (kf->own_stream) cudaStreamDestroy(kf->stream);
-  free(kf);
+  delete kf;
 }
 
 const char* daala_b200_kf_error(const daala_b200_kf* kf) { return kf ? kf->err : g_create_err; }
@@ -2579,9 +2403,7 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   n += 1;                                                                         // forward
   n += 3 + 1 + (kf->cfg.split_free > 1 ? split(kf->luma) : 0) + (kf->luma.pre_ev ? 2 : 0);   // luma: begin, gather, [prepass], chains, finish
   n += 4 + (kf->cfg.split_free > 0 ? split(kf->chroma) : 1);                      // chroma: begin, cfl, gather, bands, finish
-  if (!kf->cfg.dering) n += 2;                                                    // inverse, SB postfilter + store
-  else n += 1 + 1 + 1 + 3;       // inverse, SB postfilter -> int16, thresholds, dering + u8 store per plane
-  if (kf->cfg.dering == 2) n += 5 + 6 + 6 + 1;   // level search: 5 filtered candidates, 6 packs, 6 distortion passes, decision
+  n += kf->cfg.dering ? dering_launches(kf->dering) : 2;                          // [deringing pass | inverse, SB postfilter + store]
   if (kf->cfg.symbol_stream) n += 8;             // symbol stream: rank, superblock scan, place, 3 scan kernels, pack, index
   return n;
 }
@@ -2827,7 +2649,7 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   KF_CHECK(cudaMemcpyAsync(kf->bsize, io->bsize, map_bytes, cudaMemcpyHostToDevice, s));
   if (kf->cfg.dering == 1) {
     if (!io->dering_level) return (int)cudaErrorInvalidValue;
-    KF_CHECK(cudaMemcpyAsync(kf->dering_level, io->dering_level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyHostToDevice, s));
+    KF_CHECK(cudaMemcpyAsync(kf->dering.level, io->dering_level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyHostToDevice, s));
   }
   int rc;
   {
@@ -2867,7 +2689,7 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     KF_CHECK(cudaMemcpyAsync(io->chroma_dc_resid, kf->dc_resid[1], 4 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));
   if (io->counts) KF_CHECK(cudaMemcpyAsync(io->counts, kf->lists.cnt, sizeof(int32_t) * 32, cudaMemcpyDeviceToHost, s));
   if (io->dering_level_out && kf->cfg.dering)
-    KF_CHECK(cudaMemcpyAsync(io->dering_level_out, kf->dering_level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyDeviceToHost, s));
+    KF_CHECK(cudaMemcpyAsync(io->dering_level_out, kf->dering.level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyDeviceToHost, s));
   if (want_sym) {
     k_sym_copy<<<kf->sms * 4, 256, 0, s>>>(sc);
     KF_CHECK(cudaGetLastError());
@@ -2911,9 +2733,9 @@ int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
     KF_CHECK(cudaMemcpyAsync(kf->fin_skip[c], skip[c], (size_t)nb[c], cudaMemcpyHostToDevice, s));
     KF_CHECK(cudaMemcpyAsync(kf->fin_dc[c], dc[c], 4 * (size_t)nb[c], cudaMemcpyHostToDevice, s));
   }
-  // inter_finish = 2: the graph's search writes fin_level_in
-  if (io->dering_level) KF_CHECK(cudaMemcpyAsync(kf->fin_level_in, io->dering_level, nsb, cudaMemcpyHostToDevice, s));
-  else if (kf->cfg.inter_finish == 1) KF_CHECK(cudaMemsetAsync(kf->fin_level_in, 0, nsb, s));
+  // inter_finish = 2: the graph's search writes the levels
+  if (io->dering_level) KF_CHECK(cudaMemcpyAsync(kf->dering.level, io->dering_level, nsb, cudaMemcpyHostToDevice, s));
+  else if (kf->cfg.inter_finish == 1) KF_CHECK(cudaMemsetAsync(kf->dering.level, 0, nsb, s));
   if (!kf->fin_captured) {
     // as the step's graph: a first run outside the capture loads the kernels
     int rc = kf_enqueue_finish(kf);
