@@ -33,6 +33,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <mutex>
 #include <new>
 #include <vector>
@@ -1246,6 +1247,30 @@ __global__ void __launch_bounds__(256) k_fin_skip_map(const __grid_constant__ Fi
   }
 }
 
+// cfg.inter_mc with cfg.inter_finish: the pass's reconstruction of frame f into slot slot[f] of the reference-picture
+// pool (-1: not stored), the last node of the finishing graph.  The table lives on the device so that the one
+// captured graph serves every call.  A frame's planes have the pool's layout, and the pool's clamped reads are the
+// reference's edge extension (DESIGN §3.5), so the picture is stored as it is.
+struct PoolStore {
+  const uint8_t* src[3];           // fin_pixels: [F][plane_h][plane_w]
+  uint8_t* pool[3];                // ref_pixels: [mc_refs][plane_h][plane_w]
+  long long plane_bytes[3];        // plane_h * plane_w, a multiple of 16 * 32 (plane widths are multiples of 32)
+  const int32_t* slot;             // [F]
+};
+
+// One launch for every frame and plane: blockIdx.y = frame * 3 + plane, the CTAs of a plane stride over its rows as
+// 16-byte words (a plane is a whole number of words, and every row starts on one).
+__global__ void __launch_bounds__(256) k_fin_pool_store(const __grid_constant__ PoolStore S) {
+  const int f = blockIdx.y / 3, p = blockIdx.y - 3 * f;
+  const int slot = S.slot[f];
+  if (slot < 0) return;
+  const long long n = S.plane_bytes[p] >> 4;
+  const uint4* __restrict__ src = reinterpret_cast<const uint4*>(S.src[p] + f * S.plane_bytes[p]);
+  uint4* __restrict__ dst = reinterpret_cast<uint4*>(S.pool[p] + slot * S.plane_bytes[p]);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    dst[i] = src[i];
+}
+
 // ---- symbol stream (optional, config.symbol_stream) -------------------------------------------------------
 // The PVQ symbols of every frame in bitstream order (include/daala_b200.h, daala_b200_kf_sym_block): per
 // superblock in raster order planes 0, 1, 2, inside a plane the quadtree leaves depth-first with children
@@ -1638,6 +1663,11 @@ struct daala_b200_kf {
   cudaGraphExec_t fin_exec;
   bool fin_captured;
   int fin_dc_limit;                // largest |dc| finish accepts: DAALA_B200_KF_FINISH_DC_LIMIT / the largest dc_quant
+  // cfg.inter_mc with cfg.inter_finish: the pool slot of each frame's reconstruction (finish_io.ref_slot_out, -1 = not
+  // stored) and the store that reads it
+  int32_t* fin_slot_out;
+  PoolStore store;
+  std::vector<uint8_t> slot_filled;  // cfg.inter_mc, per pool slot: something has written a picture there
   bool have_step;                  // a step has been submitted; last_tot are its totals
   daala_b200_kf_totals last_tot;
   std::vector<void*> allocs;       // every device buffer dalloc made; daala_b200_kf_destroy frees these
@@ -2017,6 +2047,16 @@ static int kf_alloc(daala_b200_kf* kf) {
         if (dq > dq_max) dq_max = dq;
       }
     kf->fin_dc_limit = DAALA_B200_KF_FINISH_DC_LIMIT / dq_max;
+    if (kf->cfg.inter_mc) {
+      KF_CHECK(dalloc(kf, &kf->fin_slot_out, (size_t)F));
+      PoolStore& W = kf->store;
+      for (int p = 0; p < 3; p++) {
+        W.src[p] = kf->fin_pixels[p];
+        W.pool[p] = kf->ref_pixels[p];
+        W.plane_bytes[p] = (long long)kf->plane_w[p] * kf->plane_h[p];
+      }
+      W.slot = kf->fin_slot_out;
+    }
   }
   // the deringing pass: the step's on keyframes (cfg.dering) or the finishing pass's (cfg.inter_finish); inter refuses
   // dering, so an engine has at most one.  Level 2 of either searches the levels first.
@@ -2268,7 +2308,8 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
 
 // config.inter_finish: the kernels of the finishing pass, between the H2D of the decisions / levels and the D2H of
 // the results.  Patch and skip map, then the deringing pass with the real skip maps (enqueue_dering: the inverse in
-// place on the patched plane, [inter_finish = 2: the level search], thresholds with the forced level 0, od_dering).
+// place on the patched plane, [inter_finish = 2: the level search], thresholds with the forced level 0, od_dering),
+// [inter_mc: the store of the reconstruction into the pool slots of fin_slot_out].
 static int kf_enqueue_finish(daala_b200_kf* kf) {
   cudaStream_t s = kf->stream;
   const int wide = kf->sms * 8;
@@ -2278,6 +2319,7 @@ static int kf_enqueue_finish(daala_b200_kf* kf) {
   k_fin_skip_map<<<wide, 256, 0, s>>>(kf->fin);
   const int rc = enqueue_dering(kf, kf->dering, s);
   if (rc) return rc;
+  if (kf->fin_slot_out) k_fin_pool_store<<<dim3(wide > kf->F ? wide / kf->F : 1, 3 * kf->F), 256, 0, s>>>(kf->store);
   return (int)cudaGetLastError();
 }
 
@@ -2327,6 +2369,7 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   kf->F = cfg->nframes;
   if (kf->cfg.inter_mc && kf->cfg.mc_refs == 0) kf->cfg.mc_refs = 2 * kf->F;
   if (!kf->cfg.inter_mc) kf->cfg.mc_refs = 0;
+  kf->slot_filled.assign((size_t)kf->cfg.mc_refs, 0);
   if (kf->cfg.sb_rows <= 0) {
     kf->cfg.sb_row0 = 0;
     kf->cfg.sb_rows = kf->nvsb;
@@ -2584,15 +2627,32 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: an inter engine needs pred_pixels[0..2], luma_dc and chroma_dc");
     return (int)cudaErrorInvalidValue;
   }
+  if (io->ref_resident && !kf->cfg.inter_mc) {
+    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: ref_resident needs an engine with inter_mc");
+    return (int)cudaErrorInvalidValue;
+  }
   if (kf->cfg.inter_mc) {
+    const bool resident = io->ref_resident != 0;
+    const bool any_ref = io->ref_pixels[0] || io->ref_pixels[1] || io->ref_pixels[2];
     const char* why = !io->luma_dc || !io->chroma_dc ? "luma_dc and chroma_dc are required"
                       : !io->mv_grid ? "mv_grid is required"
-                      : !io->ref_pixels[0] || !io->ref_pixels[1] || !io->ref_pixels[2] ? "ref_pixels[0..2] are required"
+                      : io->ref_resident != 0 && io->ref_resident != 1 ? "ref_resident is 0 or 1"
+                      : resident && any_ref ? "ref_resident: ref_pixels must be NULL (the step reads the pool as it stands)"
+                      : resident && io->nrefs != 0 ? "ref_resident: nrefs must be 0"
+                      : !resident && (!io->ref_pixels[0] || !io->ref_pixels[1] || !io->ref_pixels[2])
+                          ? "ref_pixels[0..2] are required"
                       : !io->ref_slot ? "ref_slot is required"
                       : have_pred ? "pred_pixels is refused: the engine makes the prediction"
-                      : io->nrefs < 1 || io->nrefs > kf->cfg.mc_refs ? "nrefs is outside [1, mc_refs]" : nullptr;
-    for (int i = 0; !why && i < 2 * F; i++)
-      if (io->ref_slot[i] < 0 || io->ref_slot[i] >= io->nrefs) why = "a ref_slot entry is outside [0, nrefs)";
+                      : !resident && (io->nrefs < 1 || io->nrefs > kf->cfg.mc_refs) ? "nrefs is outside [1, mc_refs]"
+                                                                                    : nullptr;
+    for (int i = 0; !why && i < 2 * F; i++) {
+      const int32_t r = io->ref_slot[i];
+      if (!resident && (r < 0 || r >= io->nrefs)) why = "a ref_slot entry is outside [0, nrefs)";
+      else if (resident && (r < 0 || r >= kf->cfg.mc_refs)) why = "ref_resident: a ref_slot entry is outside [0, mc_refs)";
+      else if (resident && !kf->slot_filled[r])
+        why = "ref_resident: a ref_slot entry names a pool slot that holds no picture (pool_load, a host-upload "
+              "submit or a finish with ref_slot_out writes one)";
+    }
     if (why) {
       snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: inter_mc: %s", why);
       return (int)cudaErrorInvalidValue;
@@ -2632,14 +2692,16 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     if (!io->pixels[p]) return (int)cudaErrorInvalidValue;
     KF_CHECK(cudaMemcpyAsync(kf->pixels[p], io->pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
                              cudaMemcpyHostToDevice, s));
-    if (kf->cfg.inter_mc)
-      KF_CHECK(cudaMemcpyAsync(kf->ref_pixels[p], io->ref_pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * io->nrefs,
-                               cudaMemcpyHostToDevice, s));
-    else if (kf->cfg.inter)
+    if (kf->cfg.inter_mc) {
+      if (!io->ref_resident)
+        KF_CHECK(cudaMemcpyAsync(kf->ref_pixels[p], io->ref_pixels[p],
+                                 (size_t)kf->plane_w[p] * kf->plane_h[p] * io->nrefs, cudaMemcpyHostToDevice, s));
+    } else if (kf->cfg.inter)
       KF_CHECK(cudaMemcpyAsync(kf->pred_pixels[p], io->pred_pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
                                cudaMemcpyHostToDevice, s));
   }
   if (kf->cfg.inter_mc) {
+    if (!io->ref_resident) std::fill(kf->slot_filled.begin(), kf->slot_filled.begin() + io->nrefs, 1);
     KF_CHECK(cudaMemcpyAsync(kf->ref_slot, io->ref_slot, sizeof(int32_t) * 2 * F, cudaMemcpyHostToDevice, s));
     KF_CHECK(cudaMemcpyAsync(kf->mv_grid, io->mv_grid,
                              sizeof(daala_b200_mv_pt) * F * (kf->nvsb * 8 + 1) * (kf->nhsb * 8 + 1),
@@ -2710,7 +2772,15 @@ int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
                     : !skip[0] || !skip[1] || !dc[0] || !dc[1] ? "luma_skip, chroma_skip, luma_dc and chroma_dc are required"
                     : kf->cfg.inter_finish == 2 && io->dering_level
                         ? "dering_level must be NULL on an inter_finish = 2 engine (the pass searches the levels)"
+                    : io->ref_slot_out && !kf->fin_slot_out
+                        ? "ref_slot_out needs an engine with inter_mc (the reference-picture pool)"
                         : nullptr;
+  for (int f = 0; !why && io->ref_slot_out && f < F; f++) {
+    const int32_t r = io->ref_slot_out[f];
+    if (r < -1 || r >= kf->cfg.mc_refs) why = "a ref_slot_out entry is outside [-1, mc_refs)";
+    for (int g = 0; !why && r >= 0 && g < f; g++)
+      if (io->ref_slot_out[g] == r) why = "two frames name the same ref_slot_out slot";
+  }
   for (int c = 0; !why && c < 2; c++)
     for (long long i = 0; i < nb[c]; i++) {
       if (skip[c][i] > 1) {
@@ -2736,6 +2806,9 @@ int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
   // inter_finish = 2: the graph's search writes the levels
   if (io->dering_level) KF_CHECK(cudaMemcpyAsync(kf->dering.level, io->dering_level, nsb, cudaMemcpyHostToDevice, s));
   else if (kf->cfg.inter_finish == 1) KF_CHECK(cudaMemsetAsync(kf->dering.level, 0, nsb, s));
+  // the graph's pool store reads the slot table: NULL stores nothing (every entry -1)
+  if (io->ref_slot_out) KF_CHECK(cudaMemcpyAsync(kf->fin_slot_out, io->ref_slot_out, 4 * (size_t)F, cudaMemcpyHostToDevice, s));
+  else if (kf->fin_slot_out) KF_CHECK(cudaMemsetAsync(kf->fin_slot_out, 0xFF, 4 * (size_t)F, s));
   if (!kf->fin_captured) {
     // as the step's graph: a first run outside the capture loads the kernels
     int rc = kf_enqueue_finish(kf);
@@ -2750,6 +2823,8 @@ int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
     kf->fin_captured = true;
   }
   KF_CHECK(cudaGraphLaunch(kf->fin_exec, s));
+  for (int f = 0; io->ref_slot_out && f < F; f++)
+    if (io->ref_slot_out[f] >= 0) kf->slot_filled[io->ref_slot_out[f]] = 1;
   for (int p = 0; p < 3; p++) {
     const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
     if (io->pixels_out[p]) KF_CHECK(cudaMemcpyAsync(io->pixels_out[p], kf->fin_pixels[p], n, cudaMemcpyDeviceToHost, s));
@@ -2757,6 +2832,24 @@ int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
       KF_CHECK(cudaMemcpyAsync(io->bskip_out[p], kf->fin_bskip[p], (size_t)kf->fin.skip_pitch[p] * F, cudaMemcpyDeviceToHost, s));
   }
   if (io->dering_level_out) KF_CHECK(cudaMemcpyAsync(io->dering_level_out, kf->fin_level, nsb, cudaMemcpyDeviceToHost, s));
+  return 0;
+}
+
+int daala_b200_kf_pool_load(daala_b200_kf* kf, int slot, const uint8_t* const planes[3]) {
+  if (!kf) return (int)cudaErrorInvalidValue;
+  const char* why = !kf->cfg.inter_mc ? "the engine was created without inter_mc (it has no reference-picture pool)"
+                    : slot < 0 || slot >= kf->cfg.mc_refs ? "slot is outside [0, mc_refs)"
+                    : !planes || !planes[0] || !planes[1] || !planes[2] ? "planes[0..2] are required"
+                                                                        : nullptr;
+  if (why) {
+    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_pool_load: %s", why);
+    return (int)cudaErrorInvalidValue;
+  }
+  for (int p = 0; p < 3; p++) {
+    const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p];
+    KF_CHECK(cudaMemcpyAsync(kf->ref_pixels[p] + slot * n, planes[p], n, cudaMemcpyDefault, kf->stream));
+  }
+  kf->slot_filled[slot] = 1;
   return 0;
 }
 

@@ -9,7 +9,10 @@ that prediction itself from each frame's MV grid and its GOLD / PREV pictures in
 `encode` also returns each block's unquantised DC residual, and `finish` takes the host coder's skip and DC decisions
 and deringing levels and returns the reconstruction the decoder makes, with its skip maps.  With inter_finish=2 the pass
 searches the deringing levels itself (the reference's P-frame search: real skip maps, uncoded superblocks left out,
-one CDF context) and returns them with the reconstruction made at those levels.
+one CDF context) and returns them with the reconstruction made at those levels.  An engine with inter_mc and
+inter_finish codes a sequence without moving pictures through the host: `finish(..., ref_slot_out=)` stores each
+frame's reconstruction into a pool slot on the device, `encode(..., resident=True)` predicts from the pool as it stands,
+and `pool_load` seeds a slot from host memory or from another engine's device buffer (a GOP's keyframe).
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -51,13 +54,14 @@ class IO(ctypes.Structure):
                 ("sym_bands", c_void_p), ("sym_bands_cap", c_ll), ("sym_pulses", c_void_p), ("sym_pulses_cap", c_ll),
                 ("pred_pixels", c_void_p * 3), ("luma_dc", c_void_p), ("chroma_dc", c_void_p),
                 ("ref_pixels", c_void_p * 3), ("nrefs", c_int), ("ref_slot", c_void_p), ("mv_grid", c_void_p),
-                ("pred_pixels_out", c_void_p * 3), ("luma_dc_resid", c_void_p), ("chroma_dc_resid", c_void_p)]
+                ("pred_pixels_out", c_void_p * 3), ("luma_dc_resid", c_void_p), ("chroma_dc_resid", c_void_p),
+                ("ref_resident", c_int)]
 
 
 class FinishIO(ctypes.Structure):
     _fields_ = [("luma_skip", c_void_p), ("chroma_skip", c_void_p), ("luma_dc", c_void_p), ("chroma_dc", c_void_p),
                 ("dering_level", c_void_p), ("pixels_out", c_void_p * 3), ("bskip_out", c_void_p * 3),
-                ("dering_level_out", c_void_p)]
+                ("dering_level_out", c_void_p), ("ref_slot_out", c_void_p)]
 
 
 class SymBounds(ctypes.Structure):
@@ -97,6 +101,7 @@ def _bind():
     for name in ("daala_b200_kf_submit", "daala_b200_kf_encode"):
         getattr(L, name).argtypes = [c_void_p, ctypes.POINTER(IO)]
     L.daala_b200_kf_finish.argtypes = [c_void_p, ctypes.POINTER(FinishIO)]
+    L.daala_b200_kf_pool_load.argtypes = [c_void_p, c_int, ctypes.POINTER(c_void_p)]
     L.daala_b200_kf_symbol_bounds.argtypes = [ctypes.POINTER(Totals), c_int, ctypes.POINTER(SymBounds)]
     L.daala_b200_kf_wait.argtypes = [c_void_p]
     L.daala_b200_device_copy.argtypes = [c_void_p, c_void_p, ctypes.c_size_t, c_int]
@@ -171,6 +176,8 @@ class KeyframeEngine:
         cfg.inter_finish = int(inter_finish)
         self.inter_finish = int(inter_finish)
         self.nrefs = 0
+        self.resident = False
+        self._pool_src = []
         self.kf = self.L.daala_b200_kf_create(ctypes.byref(cfg))
         if not self.kf:
             raise RuntimeError("daala_b200_kf_create failed (refused configuration, no CUDA device, or out of memory): %s"
@@ -248,17 +255,25 @@ class KeyframeEngine:
             raise ValueError("pred= planes are required by an inter engine and refused by a keyframe engine "
                              "and by an inter_mc engine")
 
-    def stage_mc(self, refs, ref_slot, mv_grid):
+    def stage_mc(self, refs, ref_slot, mv_grid, resident=False):
         """Copies one batch's prediction inputs (inter_mc engines) into the host buffers.  refs: per plane an
-        array [nrefs, h, w] u8 (frame-sized reference pictures); ref_slot: [F, 2] pool slots of each frame's GOLD
-        and PREV picture; mv_grid: [F, nvsb*8 + 1, nhsb*8 + 1] mvgrid.MV_PT_DTYPE (mvgrid.pack)."""
+        array [nrefs, h, w] u8 (frame-sized reference pictures), uploaded into pool slots [0, nrefs); ref_slot: [F, 2]
+        pool slots of each frame's GOLD and PREV picture; mv_grid: [F, nvsb*8 + 1, nhsb*8 + 1] mvgrid.MV_PT_DTYPE
+        (mvgrid.pack).  resident=True: the step reads the pool as it stands (ref_resident), refs must be None and
+        every slot named must hold a picture (pool_load, an earlier upload, or a finish with ref_slot_out)."""
         g = self.geom
-        if not self.inter_mc or refs is None or ref_slot is None or mv_grid is None:
+        if resident:
+            if not self.inter_mc or refs is not None or ref_slot is None or mv_grid is None:
+                raise ValueError("resident=True goes with an inter_mc engine, needs ref_slot= and mv_grid=, and "
+                                 "refuses refs= (the step reads the pool as it stands)")
+        elif not self.inter_mc or refs is None or ref_slot is None or mv_grid is None:
             raise ValueError("refs=, ref_slot= and mv_grid= go with an inter_mc engine, and it needs all three")
-        self.nrefs = int(np.shape(refs[0])[0])
-        for p in range(3):
-            a = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8)
-            a[...] = refs[p]
+        self.resident = bool(resident)
+        self.nrefs = 0 if resident else int(np.shape(refs[0])[0])
+        if not resident:
+            for p in range(3):
+                a = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8)
+                a[...] = refs[p]
         a = self._arr("slot", (self.F, 2), np.int32)
         a[...] = ref_slot
         a = self._arr("grid", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1), mvgrid.MV_PT_DTYPE)
@@ -321,8 +336,10 @@ class KeyframeEngine:
                       "luma_skip_diff", "chroma_skip_diff", "chroma_flip"):
                 setattr(io, k, out[k].ctypes.data)
         if self.inter_mc:
+            io.ref_resident = int(self.resident)
             for p in range(3):
-                io.ref_pixels[p] = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8).ctypes.data
+                if not self.resident:
+                    io.ref_pixels[p] = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8).ctypes.data
                 out["pred%d" % p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
                 io.pred_pixels_out[p] = out["pred%d" % p].ctypes.data
             io.nrefs = self.nrefs
@@ -369,6 +386,7 @@ class KeyframeEngine:
 
     def wait(self):
         self._check(self.L.daala_b200_kf_wait(self.kf), "kf_wait")
+        self._pool_src = []
         return self._out
 
     def stream_d2h_bytes(self):
@@ -379,15 +397,15 @@ class KeyframeEngine:
         return idx.nbytes + int(idx[:, 1].sum()) * sym.BLOCK_DTYPE.itemsize + int(idx[:, 3].sum()) * 8 + int(idx[:, 5].sum())
 
     def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None, pred=None, refs=None,
-               ref_slot=None, mv_grid=None):
+               ref_slot=None, mv_grid=None, resident=False):
         """One batch end to end through the C ABI with host buffers; returns the result arrays (views of
         the engine's host buffers: copy what must survive the next call).  pred: see stage_inputs; refs, ref_slot,
-        mv_grid (inter_mc engines, which also return the prediction as pred0..2): see stage_mc.  Raises when the
+        mv_grid, resident (inter_mc engines, which also return the prediction as pred0..2): see stage_mc.  Raises when the
         batch exceeded the block capacity, or (inter_mc) when a used vertex names a picture other than GOLD / PREV
         or a vector reaches past the reference's edge extension: the reference encoder's result is undefined there."""
         self.stage_inputs(planes, bsize, pred)
-        if self.inter_mc or refs is not None or ref_slot is not None or mv_grid is not None:
-            self.stage_mc(refs, ref_slot, mv_grid)
+        if self.inter_mc or refs is not None or ref_slot is not None or mv_grid is not None or resident:
+            self.stage_mc(refs, ref_slot, mv_grid, resident)
         if self.dering == 1:
             self.stage_dering_levels(dering_levels)
         self.prepare_io(symbols, recon, stream)
@@ -402,13 +420,14 @@ class KeyframeEngine:
                                    "ref other than GOLD / PREV, %d corner windows past the edge extension" % (bad, beyond))
         return out
 
-    def prepare_finish(self, luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels=None):
+    def prepare_finish(self, luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels=None, ref_slot_out=None):
         """Stages the host coder's decisions for the last submitted batch (inter_finish engines) and builds the
         daala_b200_kf_finish_io record; returns the result arrays finish_submit fills: recon0..2, bskip0..2
         ([F, plane_h / 4, nhsb * 16] u8, state->bskip[pli] of each frame with row stride state->skip_stride; a chroma
         row's columns past plane_w / 4 stay 0) and dering_levels ([F, nvsb, nhsb], the levels applied; on an
         inter_finish=2 engine the levels the pass searched, and dering_levels must be None: the C call refuses
-        levels there)."""
+        levels there).  ref_slot_out (engines with inter_mc too): [F] int32, the pool slot that receives each frame's
+        reconstruction, -1 = not stored; None stores nothing."""
         g, t = self.geom, self.totals
         fio = FinishIO()
         n = {"luma": int(t.n_luma), "chroma": int(t.n_chroma)}
@@ -423,6 +442,10 @@ class KeyframeEngine:
             a = self._arr("flev", (self.F, g.nvsb, g.nhsb), np.uint8)
             a[...] = dering_levels
             fio.dering_level = a.ctypes.data
+        if ref_slot_out is not None:
+            a = self._arr("fslot", (self.F,), np.int32)
+            a[...] = ref_slot_out
+            fio.ref_slot_out = a.ctypes.data
         out = {}
         for p in range(3):
             out["recon%d" % p] = self._arr("fout%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
@@ -431,8 +454,9 @@ class KeyframeEngine:
             fio.bskip_out[p] = out["bskip%d" % p].ctypes.data
         out["dering_levels"] = self._arr("flev_out", (self.F, g.nvsb, g.nhsb), np.uint8)
         fio.dering_level_out = out["dering_levels"].ctypes.data
-        # one skip byte and one int32 DC per block, the levels
-        self.finish_h2d_bytes = 5 * sum(n.values()) + (self.F * g.nvsb * g.nhsb if dering_levels is not None else 0)
+        # one skip byte and one int32 DC per block, the levels, the slot table
+        self.finish_h2d_bytes = (5 * sum(n.values()) + (self.F * g.nvsb * g.nhsb if dering_levels is not None else 0)
+                                 + (4 * self.F if ref_slot_out is not None else 0))
         self.finish_d2h_bytes = sum(v.nbytes for v in out.values())
         self._fio, self._fout = fio, out
         return out
@@ -440,16 +464,34 @@ class KeyframeEngine:
     def finish_submit(self):
         self._check(self.L.daala_b200_kf_finish(self.kf, ctypes.byref(self._fio)), "kf_finish")
 
-    def finish(self, luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels=None):
+    def finish(self, luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels=None, ref_slot_out=None):
         """The finishing pass of the last encoded P-frame batch (inter_finish engines): per block (block order of
         the luma / chroma results of encode) the host coder's skip decision (0 or 1) and final DC index, per
-        superblock the deringing level (None: all 0; inter_finish=2 engines search the levels, so None there).
+        superblock the deringing level (None: all 0; inter_finish=2 engines search the levels, so None there), and
+        per frame the pool slot that receives its reconstruction (ref_slot_out, engines with inter_mc; None: none).
         Returns the reconstruction the decoder makes, the skip maps and the levels applied (see prepare_finish);
         views of the engine's host buffers."""
-        self.prepare_finish(luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels)
+        self.prepare_finish(luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels, ref_slot_out)
         self.finish_submit()
         self.wait()
         return self._fout
+
+    def pool_load(self, slot, planes):
+        """Enqueues the copy of one frame-sized picture into pool slot `slot` (inter_mc engines), ordered with submit
+        and finish on the engine's stream.  planes: three [h, w] u8 host arrays (padded geometry), or three device
+        addresses, e.g. a keyframe engine's buf.pixels_out[p] + f * plane bytes (that engine waited for first)."""
+        g = self.geom
+        ptrs = (c_void_p * 3)()
+        for p in range(3):
+            if isinstance(planes[p], (int, np.integer)):
+                ptrs[p] = int(planes[p])
+            elif planes[p] is not None:
+                a = np.ascontiguousarray(planes[p], np.uint8)
+                if a.shape != g.plane_shape(p):
+                    raise ValueError("pool_load: plane %d is %s, the engine's plane is %s" % (p, a.shape, g.plane_shape(p)))
+                self._pool_src.append(a)   # the copy may still read it until wait()
+                ptrs[p] = a.ctypes.data
+        self._check(self.L.daala_b200_kf_pool_load(self.kf, int(slot), ptrs), "kf_pool_load")
 
     # --- device-resident use -------------------------------------------------------------------
     def run_device(self, phases=PH_ALL, graph=True):
@@ -490,6 +532,10 @@ class KeyframeEngine:
     def pred_coeff_plane(self, p):
         """The transformed prediction md of plane p (inter engines)."""
         return self.download(self.buf.pred_coeffs[p], (self.F,) + self.geom.plane_shape(p), np.int32)
+
+    def pool_plane(self, p):
+        """The reference-picture pool of plane p, [mc_refs, h, w] u8 (inter_mc engines)."""
+        return self.download(self.buf.ref_pixels[p], (self.buf.mc_refs,) + self.geom.plane_shape(p), np.uint8)
 
     def recon_plane(self, p):
         return self.download(self.buf.pixels_out[p], (self.F,) + self.geom.plane_shape(p), np.uint8)

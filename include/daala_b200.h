@@ -600,6 +600,13 @@ typedef struct daala_b200_kf_io {
   int32_t *luma_dc_resid, *chroma_dc_resid; /* [n_blocks]: each block's unquantised DC residual in[0] - ref[0] (what the
                                            host's od_rdo_quant quantises, src/pvq_encoder.c:886 / :956), block order
                                            of luma_dc / chroma_dc */
+  /* config.inter_mc only.  0 (default): the step uploads ref_pixels into slots [0, nrefs) of the engine's pool, as
+     described above.  1: the step reads the pool as it stands and uploads no picture; ref_pixels[0..2] must then be
+     NULL and nrefs 0, and every ref_slot entry must lie in [0, mc_refs) and name a slot that holds a picture.  A slot
+     holds one once daala_b200_kf_pool_load, a submit with ref_resident = 0 (slots [0, nrefs)) or a finish with
+     daala_b200_kf_finish_io.ref_slot_out has written it.  Everything is ordered by call order on the engine's
+     stream: a step submitted before the finish that rewrites its PREV slot reads the old picture. */
+  int ref_resident;
 } daala_b200_kf_io;
 
 /* The finishing pass of a P-frame batch (config.inter_finish), daala_b200_kf_finish: the host coder's per-block
@@ -635,6 +642,15 @@ typedef struct daala_b200_kf_finish_io {
                                               every plane; the columns past plane_w / 4 of a chroma row are 0) */
   uint8_t *dering_level_out;               /* optional: [nframes][nvsb][nhsb] the levels applied (config.inter_finish
                                               = 2: the searched ones) */
+  const int32_t *ref_slot_out;             /* optional, engines with config.inter_mc and inter_finish: [nframes] the slot
+                                              of the engine's reference-picture pool that receives frame f's
+                                              reconstruction after the final deringing, -1 = not stored; NULL = nothing
+                                              stored.  The picture is stored as the pass made it, which is a valid
+                                              reference as it is (the prediction's clamped reads are the edge
+                                              extension).  Entries must lie in [-1, mc_refs) and name distinct slots.
+                                              Rewriting a slot the last step read (a frame's own PREV slot) is legal:
+                                              the step's prediction and md are already made, and a repeated finish
+                                              reads md, never the pool; the last finish wins. */
 } daala_b200_kf_finish_io;
 
 typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, device-resident callers) */
@@ -702,7 +718,8 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    symbol_stream, a stream capacity below daala_b200_kf_symbol_bounds, a stream buffer that is not pinned host
    memory, or (config.inter) a NULL pred_pixels plane, luma_dc or chroma_dc.  With config.inter_mc it refuses, the same
    way, a NULL mv_grid, ref_pixels plane or ref_slot, pred_pixels given, nrefs outside [1, mc_refs] and a slot outside
-   [0, nrefs).  The step counts in `counts` the leaf corners whose vertex has a ref other than 0 or 1 (counts[19]) and
+   [0, nrefs); with ref_resident = 1 it refuses instead ref_pixels given, nrefs other than 0, a slot outside
+   [0, mc_refs) and a slot that holds no picture.  The step counts in `counts` the leaf corners whose vertex has a ref other than 0 or 1 (counts[19]) and
    the corner windows (with the 6-tap filter's apron of -2..+3 pixels) that reach more than 64 luma / 32 chroma
    pixels outside the plane (counts[20]), where the reference encoder's result is undefined. */
 int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
@@ -713,8 +730,19 @@ int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
    applied to a plane of their own), so the pass may run any number of times after one step.  Refused with
    cudaErrorInvalidValue and a message in daala_b200_kf_error, before anything is copied or launched: an engine
    without inter_finish, no step submitted yet, a NULL decision array, a skip value other than 0 or 1, a level above
-   5, a |dc| above DAALA_B200_KF_FINISH_DC_LIMIT / DQ, and (config.inter_finish = 2) a non-NULL dering_level. */
+   5, a |dc| above DAALA_B200_KF_FINISH_DC_LIMIT / DQ, (config.inter_finish = 2) a non-NULL dering_level, and a
+   ref_slot_out on an engine without inter_mc, with an entry outside [-1, mc_refs) or with two frames naming one slot.
+   With ref_slot_out the pass's last kernel copies each stored frame's reconstruction into its pool slot. */
 int daala_b200_kf_finish(daala_b200_kf *kf, const daala_b200_kf_finish_io *io);
+/* Enqueues on the engine's stream the copies of one frame-sized picture (planes[p]: [plane_h][plane_w] u8, the layout
+   of one frame of daala_b200_kf_io.pixels) into slot `slot` of the reference-picture pool (config.inter_mc), with
+   cudaMemcpyDefault: the source may be host memory or device memory of the engine's device, for example a keyframe
+   engine's daala_b200_kf_buffers.pixels_out[p] + f * plane_h[p] * plane_w[p], which brings a GOP's keyframe into the
+   pool without a host round trip (wait for that engine first: the copy runs on this engine's stream).  Host buffers must stay valid until daala_b200_kf_wait, as submit's.  Ordered by
+   call order with submit and finish: a step submitted before the load reads the slot's previous picture.  Refused
+   with cudaErrorInvalidValue and a message in daala_b200_kf_error, before anything is copied: an engine without
+   inter_mc, a slot outside [0, mc_refs) and a NULL plane. */
+int daala_b200_kf_pool_load(daala_b200_kf *kf, int slot, const uint8_t *const planes[3]);
 int daala_b200_kf_wait(daala_b200_kf *kf);
 int daala_b200_kf_encode(daala_b200_kf *kf, const daala_b200_kf_io *io);   /* submit + wait */
 int daala_b200_device_copy(void *dst, const void *src, size_t bytes, int kind);  /* 0 H2D, 1 D2H, 2 D2D; synchronous */
