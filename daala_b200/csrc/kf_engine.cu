@@ -524,7 +524,7 @@ struct Stage {
   const int32_t* cfl_plane;        // chroma: prediction plane (chroma geometry), else NULL
   long long cfl_pitch;
   int cfl_stride;
-  int32_t* dc_resid;               // config.inter_finish: per block in[0] - ref[0], else NULL
+  int32_t* dc_resid;               // config.inter_finish or symbol_stream = 2: per block in[0] - ref[0], else NULL
 #ifdef DAALA_B200_CHAIN_TRACE
   struct ChainTraceRec* trace;     // luma: one record per item k_pvq_persist<true> runs, up to trace_cap
   int trace_cap;
@@ -1305,6 +1305,10 @@ struct Sym {
   const int32_t* flip;
   const int32_t* cnt;
   int max_luma, max_chroma;
+  // symbol_stream = 2 (P frames): the DC record of each slot, from the step's DC index and unquantised residual
+  daala_b200_kf_sym_dc* dc;        // [cap_blocks]
+  const int32_t* qdc[2];
+  const int32_t* dc_resid[2];
 };
 
 // Bytes the band's pulses take in the stream: the n - (itheta != -1) values pvq_encode_partition hands to
@@ -1472,7 +1476,9 @@ __global__ void __launch_bounds__(kTile) k_sym_offsets(const __grid_constant__ S
   if (valid) S.off[i] = make_longlong2(pre.x + s.x - v.x, pre.y + s.y - v.y);
 }
 
-// One warp per slot: the block record, its band records and the pulses of its bands with K > 0.
+// One warp per slot: the block record, its band records and the pulses of its bands with K > 0.  kInter (symbol_stream
+// = 2): flip is 0 (P frames have no CfL; res_flip is never written) and the slot's DC record is written too.
+template <bool kInter>
 __global__ void __launch_bounds__(256) k_sym_pack(const __grid_constant__ Sym S) {
   const int lane = threadIdx.x & 31;
   const long long n = S.tot[0];
@@ -1498,9 +1504,15 @@ __global__ void __launch_bounds__(256) k_sym_pack(const __grid_constant__ Sym S)
       rec.y0 = b.y0;
       rec.bs = b.bs;
       rec.pli = b.pli;
-      rec.flip = ch ? (uint8_t)S.flip[blk] : 0;
+      rec.flip = !kInter && ch ? (uint8_t)S.flip[blk] : 0;
       rec.reserved = 0;
       S.blocks[slot] = rec;
+      if (kInter) {
+        daala_b200_kf_sym_dc d;
+        d.qdc = S.qdc[ch][blk];
+        d.dc_resid = S.dc_resid[ch][blk];
+        S.dc[slot] = d;
+      }
     }
     if (lane < nb) S.bands[o.x + lane] = r[lane];
     const int32_t* y = S.y[ch] + b.coef_off;
@@ -1544,12 +1556,14 @@ __global__ void k_sym_index(const __grid_constant__ Sym S) {
 }
 
 // Copy of the used part of each stream array into the caller's pinned host buffers (device-addressable):
-// the lengths are only known on the device.  Segment 0 index, 1 block records, 2 band records, 3 pulses.
+// the lengths are only known on the device.  Segment 0 index, 1 block records, 2 band records, 3 pulses, 4 DC records
+// (one per block record).
+constexpr int kSymSegs = 5;
 struct SymCopy {
-  const uint8_t* src[4];
-  uint8_t* dst[4];
-  long long unit[4];               // bytes per element; segment 0 has a fixed length
-  long long cap[4];                // bytes: the smaller of the host buffer and the device array
+  const uint8_t* src[kSymSegs];
+  uint8_t* dst[kSymSegs];
+  long long unit[kSymSegs];        // bytes per element; segment 0 has a fixed length
+  long long cap[kSymSegs];         // bytes: the smaller of the host buffer and the device array
   long long index_bytes;
   const long long* tot;
 };
@@ -1557,9 +1571,9 @@ struct SymCopy {
 __global__ void __launch_bounds__(256) k_sym_copy(const __grid_constant__ SymCopy C) {
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long nth = (long long)gridDim.x * blockDim.x;
-  for (int seg = 0; seg < 4; seg++) {
+  for (int seg = 0; seg < kSymSegs; seg++) {
     if (!C.dst[seg]) continue;
-    const long long want = seg == 0 ? C.index_bytes : C.tot[seg - 1] * C.unit[seg];
+    const long long want = seg == 0 ? C.index_bytes : C.tot[seg == 4 ? 0 : seg - 1] * C.unit[seg];
     const long long len = want < C.cap[seg] ? want : C.cap[seg];
     const uint8_t* s = C.src[seg];
     uint8_t* d = C.dst[seg];
@@ -1571,6 +1585,32 @@ __global__ void __launch_bounds__(256) k_sym_copy(const __grid_constant__ SymCop
       done = n16 << 4;
     }
     for (long long i = done + tid; i < len; i += nth) d[i] = s[i];
+  }
+}
+
+// symbol_stream = 2 with inter_finish: the finishing pass's decisions given in stream order (finish_io.stream_skip /
+// stream_dc, staged in skip / dc) scattered into the block order the pass reads, through the step's slot -> block map.
+// The first node of the finishing graph; `form` (set by each finish call) is 0 for the classic form, which the call
+// copied into fin_skip / fin_dc itself.
+struct Unstream {
+  const uint32_t* order;           // Sym.order
+  const long long* tot;            // Sym.tot: tot[0] slots
+  const uint8_t* skip;             // [cap_blocks] in stream order
+  const int32_t* dc;
+  uint8_t* fin_skip[2];            // luma / chroma, block order
+  int32_t* fin_dc[2];
+  const int32_t* form;             // 1: stream form
+};
+
+__global__ void __launch_bounds__(256) k_fin_unstream(const __grid_constant__ Unstream U) {
+  if (!*U.form) return;
+  const long long n = U.tot[0];
+  for (long long slot = (long long)blockIdx.x * blockDim.x + threadIdx.x; slot < n;
+       slot += (long long)gridDim.x * blockDim.x) {
+    const uint32_t id = U.order[slot];
+    const int ch = id >> 31, blk = (int)(id & 0x7fffffffu);
+    U.fin_skip[ch][blk] = U.skip[slot];
+    U.fin_dc[ch][blk] = U.dc[slot];
   }
 }
 
@@ -1667,6 +1707,12 @@ struct daala_b200_kf {
   // stored) and the store that reads it
   int32_t* fin_slot_out;
   PoolStore store;
+  // cfg.symbol_stream = 2 with cfg.inter_finish: the decisions of a stream-order finish (staged), the form flag
+  // k_fin_unstream reads, and its parameters
+  uint8_t* fin_stream_skip;
+  int32_t* fin_stream_dc;
+  int32_t* fin_form;
+  Unstream unstream;
   std::vector<uint8_t> slot_filled;  // cfg.inter_mc, per pool slot: something has written a picture there
   bool have_step;                  // a step has been submitted; last_tot are its totals
   daala_b200_kf_totals last_tot;
@@ -1933,6 +1979,14 @@ static int kf_alloc(daala_b200_kf* kf) {
   rc = setup_stage(kf->chroma, true);
   if (rc) return rc;
   (void)luma_px;
+  // the unquantised DC residual per block: what the host's od_rdo_quant needs, returned classically (inter_finish) or
+  // in the stream's DC records (symbol_stream = 2)
+  if (kf->cfg.inter_finish || kf->cfg.symbol_stream == 2)
+    for (int c = 0; c < 2; c++) {
+      Stage& S = c ? kf->chroma : kf->luma;
+      KF_CHECK(dalloc(kf, &kf->dc_resid[c], (size_t)S.max_blocks));
+      S.dc_resid = kf->dc_resid[c];
+    }
   if (kf->cfg.symbol_stream) {
     Sym& Y = kf->sym;
     memset(&Y, 0, sizeof(Y));
@@ -1972,6 +2026,13 @@ static int kf_alloc(daala_b200_kf* kf) {
     Y.cnt = L.cnt;
     Y.max_luma = L.max_luma;
     Y.max_chroma = L.max_chroma;
+    if (kf->cfg.symbol_stream == 2) {
+      KF_CHECK(dalloc(kf, &Y.dc, (size_t)Y.cap_blocks));
+      for (int c = 0; c < 2; c++) {
+        Y.qdc[c] = (c ? kf->chroma : kf->luma).prm.res_dc;
+        Y.dc_resid[c] = kf->dc_resid[c];
+      }
+    }
   }
 
   daala_b200_frame& f = kf->frame;
@@ -2011,8 +2072,6 @@ static int kf_alloc(daala_b200_kf* kf) {
       const Stage& S = c ? kf->chroma : kf->luma;
       KF_CHECK(dalloc(kf, &kf->fin_skip[c], (size_t)S.max_blocks));
       KF_CHECK(dalloc(kf, &kf->fin_dc[c], (size_t)S.max_blocks));
-      KF_CHECK(dalloc(kf, &kf->dc_resid[c], (size_t)S.max_blocks));
-      (c ? kf->chroma : kf->luma).dc_resid = kf->dc_resid[c];
       P.blocks[c] = S.prm.blocks;
       P.skip[c] = kf->fin_skip[c];
       P.dc[c] = kf->fin_dc[c];
@@ -2056,6 +2115,21 @@ static int kf_alloc(daala_b200_kf* kf) {
         W.plane_bytes[p] = (long long)kf->plane_w[p] * kf->plane_h[p];
       }
       W.slot = kf->fin_slot_out;
+    }
+    if (kf->cfg.symbol_stream == 2) {
+      Unstream& U = kf->unstream;
+      KF_CHECK(dalloc(kf, &kf->fin_stream_skip, (size_t)kf->sym.cap_blocks));
+      KF_CHECK(dalloc(kf, &kf->fin_stream_dc, (size_t)kf->sym.cap_blocks));
+      KF_CHECK(dalloc(kf, &kf->fin_form, (size_t)1));
+      U.order = kf->sym.order;
+      U.tot = kf->sym.tot;
+      U.skip = kf->fin_stream_skip;
+      U.dc = kf->fin_stream_dc;
+      for (int c = 0; c < 2; c++) {
+        U.fin_skip[c] = kf->fin_skip[c];
+        U.fin_dc[c] = kf->fin_dc[c];
+      }
+      U.form = kf->fin_form;
     }
   }
   // the deringing pass: the step's on keyframes (cfg.dering) or the finishing pass's (cfg.inter_finish); inter refuses
@@ -2193,6 +2267,20 @@ static void enqueue_split(daala_b200_kf* kf, const Stage& S, cudaStream_t s) {
   }
 }
 
+// The symbol stream of the step (cfg.symbol_stream), after both stages' k_finish_scatter: rank, superblock scan,
+// place, the three scan kernels, pack (kInter: with the DC records), index.
+template <bool kInter>
+static void enqueue_sym(const Sym& Y, int wide, cudaStream_t s) {
+  k_sym_rank<<<(Y.F * Y.nsb + 7) / 8, 256, 0, s>>>(Y);
+  k_sym_sb_scan<<<1, 1024, 0, s>>>(Y);
+  k_sym_place<<<wide, 256, 0, s>>>(Y);
+  k_sym_tile_sums<<<Y.ntiles, kTile, 0, s>>>(Y);
+  k_sym_tile_scan<<<1, 1024, 0, s>>>(Y);
+  k_sym_offsets<<<Y.ntiles, kTile, 0, s>>>(Y);
+  k_sym_pack<kInter><<<wide, 256, 0, s>>>(Y);
+  k_sym_index<<<1, 256, 0, s>>>(Y);
+}
+
 // config.inter: the same step for P-frame residuals.  Both plane sets through the forward transform (two
 // launches: the kernel's tensor maps describe one pixel allocation each), every band of both stages through
 // the phase kernels with the transformed prediction as reference.
@@ -2225,6 +2313,7 @@ static int kf_enqueue_step_inter(daala_b200_kf* kf, int phases) {
     enqueue_split<false>(kf, *S, s);
     if (!core) k_finish_scatter<true><<<wide, 256, 0, s>>>(*S);
   }
+  if (!core && (phases & DAALA_B200_KF_PVQ_CHROMA) && kf->cfg.symbol_stream) enqueue_sym<true>(kf->sym, wide, s);
   if (phases & DAALA_B200_KF_INVERSE) {
     int rc = daala_b200_launch_inverse(&kf->frame, 3, s);
     if (rc) return rc;
@@ -2287,17 +2376,7 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
     if (kf->cfg.split_free > 0) enqueue_split<false>(kf, kf->chroma, s);
     else k_pvq_persist<false><<<persist, kPersistThreads, 0, s>>>(kf->chroma);
     if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->chroma);
-    if (!core && kf->cfg.symbol_stream) {
-      const Sym& Y = kf->sym;
-      k_sym_rank<<<(Y.F * Y.nsb + 7) / 8, 256, 0, s>>>(Y);
-      k_sym_sb_scan<<<1, 1024, 0, s>>>(Y);
-      k_sym_place<<<wide, 256, 0, s>>>(Y);
-      k_sym_tile_sums<<<Y.ntiles, kTile, 0, s>>>(Y);
-      k_sym_tile_scan<<<1, 1024, 0, s>>>(Y);
-      k_sym_offsets<<<Y.ntiles, kTile, 0, s>>>(Y);
-      k_sym_pack<<<wide, 256, 0, s>>>(Y);
-      k_sym_index<<<1, 256, 0, s>>>(Y);
-    }
+    if (!core && kf->cfg.symbol_stream) enqueue_sym<false>(kf->sym, wide, s);
   }
   if (phases & DAALA_B200_KF_INVERSE) {
     int rc = kf->cfg.dering ? enqueue_dering(kf, kf->dering, s) : daala_b200_launch_inverse(&kf->frame, 3, s);
@@ -2307,12 +2386,14 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
 }
 
 // config.inter_finish: the kernels of the finishing pass, between the H2D of the decisions / levels and the D2H of
-// the results.  Patch and skip map, then the deringing pass with the real skip maps (enqueue_dering: the inverse in
-// place on the patched plane, [inter_finish = 2: the level search], thresholds with the forced level 0, od_dering),
-// [inter_mc: the store of the reconstruction into the pool slots of fin_slot_out].
+// the results.  [symbol_stream = 2: the stream-order decisions into block order], patch and skip map, then the
+// deringing pass with the real skip maps (enqueue_dering: the inverse in place on the patched plane, [inter_finish = 2:
+// the level search], thresholds with the forced level 0, od_dering), [inter_mc: the store of the reconstruction into
+// the pool slots of fin_slot_out].
 static int kf_enqueue_finish(daala_b200_kf* kf) {
   cudaStream_t s = kf->stream;
   const int wide = kf->sms * 8;
+  if (kf->fin_form) k_fin_unstream<<<wide, 256, 0, s>>>(kf->unstream);
   if (cudaMemsetAsync(kf->fin_coded, 0, (size_t)kf->F * kf->nhsb * kf->nvsb, s) != cudaSuccess)
     return (int)cudaGetLastError();
   k_fin_patch<<<wide, 256, 0, s>>>(kf->fin);
@@ -2339,6 +2420,12 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
              "daala_b200_kf_create: inter_finish is 0, 1 or 2, and 1 and 2 require inter = 1");
     return nullptr;
   }
+  if (cfg && (cfg->symbol_stream < 0 || cfg->symbol_stream > 2 || (cfg->symbol_stream == 2 && cfg->inter != 1))) {
+    snprintf(g_create_err, sizeof(g_create_err),
+             "daala_b200_kf_create: symbol_stream is 0, 1 or 2, and 2 requires inter = 1 (a keyframe's DC goes through "
+             "the Haar pyramid and has no scalar index)");
+    return nullptr;
+  }
   if (cfg && cfg->mc_refs < 0) {
     snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: mc_refs < 0");
     return nullptr;
@@ -2348,7 +2435,8 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
     // inter form this engine does not have
     const char* with = cfg->inter != 1 ? "a value other than 0 or 1"
                        : cfg->dering ? "dering (the all-zero skip map of the deringing stage is a keyframe property)"
-                       : cfg->symbol_stream ? "symbol_stream (its block record has no DC field)"
+                       : cfg->symbol_stream == 1 ? "symbol_stream = 1 (its block record has no DC field; "
+                                                   "symbol_stream = 2 is the P-frame stream)"
                        : cfg->noref_prepass ? "noref_prepass"
                        : cfg->level_chains ? "level_chains"
                        : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
@@ -2440,8 +2528,10 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   auto split = [](const Stage& S) { return 3 * (S.sp_chunks[0] + S.sp_chunks[1] + S.sp_chunks[2]); };
   // inter: work lists, two forward launches, per stage gather + phase kernels + finish, inverse + SB postfilter;
   // inter_mc: leaf enumeration and OBMC
+  // [symbol_stream = 2: the 8 stream kernels]
   if (kf->cfg.inter)
-    return 5 + 2 + (2 + split(kf->luma)) + (2 + split(kf->chroma)) + 2 + (kf->cfg.inter_mc ? 2 : 0);
+    return 5 + 2 + (2 + split(kf->luma)) + (2 + split(kf->chroma)) + 2 + (kf->cfg.inter_mc ? 2 : 0) +
+           (kf->cfg.symbol_stream ? 8 : 0);
   int n = 5 + (kf->cfg.level_chains ? 2 : 0);                                    // work lists
   n += 1;                                                                         // forward
   n += 3 + 1 + (kf->cfg.split_free > 1 ? split(kf->luma) : 0) + (kf->luma.pre_ev ? 2 : 0);   // luma: begin, gather, [prepass], chains, finish
@@ -2622,8 +2712,10 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
                                   kf->cfg.sb_row0, kf->cfg.sb_rows, &tot);
   if (tot.n_luma > kf->lists.max_luma || tot.n_chroma > kf->lists.max_chroma) return (int)cudaErrorInvalidValue;
   const bool have_pred = io->pred_pixels[0] || io->pred_pixels[1] || io->pred_pixels[2];
+  // symbol_stream = 2: the stream's DC records carry the DC indices, so the classic arrays are optional
+  const bool need_dc = kf->cfg.symbol_stream != 2 && (!io->luma_dc || !io->chroma_dc);
   if (kf->cfg.inter && !kf->cfg.inter_mc &&
-      (!io->pred_pixels[0] || !io->pred_pixels[1] || !io->pred_pixels[2] || !io->luma_dc || !io->chroma_dc)) {
+      (!io->pred_pixels[0] || !io->pred_pixels[1] || !io->pred_pixels[2] || need_dc)) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: an inter engine needs pred_pixels[0..2], luma_dc and chroma_dc");
     return (int)cudaErrorInvalidValue;
   }
@@ -2634,7 +2726,7 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   if (kf->cfg.inter_mc) {
     const bool resident = io->ref_resident != 0;
     const bool any_ref = io->ref_pixels[0] || io->ref_pixels[1] || io->ref_pixels[2];
-    const char* why = !io->luma_dc || !io->chroma_dc ? "luma_dc and chroma_dc are required"
+    const char* why = need_dc ? "luma_dc and chroma_dc are required"
                       : !io->mv_grid ? "mv_grid is required"
                       : io->ref_resident != 0 && io->ref_resident != 1 ? "ref_resident is 0 or 1"
                       : resident && any_ref ? "ref_resident: ref_pixels must be NULL (the step reads the pool as it stands)"
@@ -2661,32 +2753,41 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   // symbol stream: the engine must produce it, and every requested buffer must hold the worst case and be pinned
   SymCopy sc;
   memset(&sc, 0, sizeof(sc));
-  const bool want_sym = io->sym_index || io->sym_blocks || io->sym_bands || io->sym_pulses;
+  const bool want_sym = io->sym_index || io->sym_blocks || io->sym_bands || io->sym_pulses || io->sym_dc;
   if (want_sym) {
     if (!kf->cfg.symbol_stream) return (int)cudaErrorInvalidValue;
+    if (io->sym_dc && kf->cfg.symbol_stream != 2) {
+      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: sym_dc needs an engine with symbol_stream = 2");
+      return (int)cudaErrorInvalidValue;
+    }
     daala_b200_kf_sym_bounds bd;
     daala_b200_kf_symbol_bounds(&tot, F, &bd);
     int e = sym_target(io->sym_index, io->sym_index_cap, bd.index, &sc.dst[0]);
     if (!e) e = sym_target(io->sym_blocks, io->sym_blocks_cap, bd.blocks, &sc.dst[1]);
     if (!e) e = sym_target(io->sym_bands, io->sym_bands_cap, bd.bands, &sc.dst[2]);
     if (!e) e = sym_target(io->sym_pulses, io->sym_pulses_cap, bd.pulse_bytes, &sc.dst[3]);
+    if (!e) e = sym_target(io->sym_dc, io->sym_dc_cap, bd.blocks, &sc.dst[4]);
     if (e) return e;
     const Sym& Y = kf->sym;
     sc.src[0] = (const uint8_t*)Y.index;
     sc.src[1] = (const uint8_t*)Y.blocks;
     sc.src[2] = (const uint8_t*)Y.bands;
     sc.src[3] = Y.pulses;
+    sc.src[4] = (const uint8_t*)Y.dc;
     sc.unit[1] = sizeof(daala_b200_kf_sym_block);
     sc.unit[2] = 4 * sizeof(int16_t);
     sc.unit[3] = 1;
+    sc.unit[4] = sizeof(daala_b200_kf_sym_dc);
     sc.index_bytes = (long long)F * sizeof(daala_b200_kf_sym_frame);
     sc.tot = Y.tot;
-    const long long host[4] = {io->sym_index_cap * (long long)sizeof(daala_b200_kf_sym_frame),
-                               io->sym_blocks_cap * (long long)sizeof(daala_b200_kf_sym_block),
-                               io->sym_bands_cap * 8, io->sym_pulses_cap};
-    const long long dev[4] = {sc.index_bytes, (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_block),
-                              Y.cap_bands * 8, Y.cap_bytes};
-    for (int i = 0; i < 4; i++) sc.cap[i] = host[i] < dev[i] ? host[i] : dev[i];
+    const long long host[kSymSegs] = {io->sym_index_cap * (long long)sizeof(daala_b200_kf_sym_frame),
+                                      io->sym_blocks_cap * (long long)sizeof(daala_b200_kf_sym_block),
+                                      io->sym_bands_cap * 8, io->sym_pulses_cap,
+                                      io->sym_dc_cap * (long long)sizeof(daala_b200_kf_sym_dc)};
+    const long long dev[kSymSegs] = {sc.index_bytes, (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_block),
+                                     Y.cap_bands * 8, Y.cap_bytes,
+                                     Y.dc ? (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_dc) : 0};
+    for (int i = 0; i < kSymSegs; i++) sc.cap[i] = host[i] < dev[i] ? host[i] : dev[i];
   }
   for (int p = 0; p < 3; p++) {
     if (!io->pixels[p]) return (int)cudaErrorInvalidValue;
@@ -2741,13 +2842,13 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     if (kf->cfg.inter_mc && io->pred_pixels_out[p])
       KF_CHECK(cudaMemcpyAsync(io->pred_pixels_out[p], kf->pred_pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
                                cudaMemcpyDeviceToHost, s));
-  if (kf->cfg.inter) {
+  if (kf->cfg.inter && io->luma_dc)
     KF_CHECK(cudaMemcpyAsync(io->luma_dc, kf->luma.prm.res_dc, 4 * (size_t)tot.n_luma, cudaMemcpyDeviceToHost, s));
+  if (kf->cfg.inter && io->chroma_dc)
     KF_CHECK(cudaMemcpyAsync(io->chroma_dc, kf->chroma.prm.res_dc, 4 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));
-  }
-  if (kf->cfg.inter_finish && io->luma_dc_resid)
+  if (kf->dc_resid[0] && io->luma_dc_resid)
     KF_CHECK(cudaMemcpyAsync(io->luma_dc_resid, kf->dc_resid[0], 4 * (size_t)tot.n_luma, cudaMemcpyDeviceToHost, s));
-  if (kf->cfg.inter_finish && io->chroma_dc_resid)
+  if (kf->dc_resid[1] && io->chroma_dc_resid)
     KF_CHECK(cudaMemcpyAsync(io->chroma_dc_resid, kf->dc_resid[1], 4 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));
   if (io->counts) KF_CHECK(cudaMemcpyAsync(io->counts, kf->lists.cnt, sizeof(int32_t) * 32, cudaMemcpyDeviceToHost, s));
   if (io->dering_level_out && kf->cfg.dering)
@@ -2764,12 +2865,23 @@ int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
   const int F = kf->F;
   const size_t nsb = (size_t)F * kf->nhsb * kf->nvsb;
   const long long nb[2] = {kf->last_tot.n_luma, kf->last_tot.n_chroma};
-  const uint8_t* skip[2] = {io->luma_skip, io->chroma_skip};
-  const int32_t* dc[2] = {io->luma_dc, io->chroma_dc};
+  // the decisions in block order (the classic form: luma, chroma) or in stream order (one array of nb[0] + nb[1])
+  const bool stream = io->stream_skip || io->stream_dc;
+  const bool classic = io->luma_skip || io->chroma_skip || io->luma_dc || io->chroma_dc;
+  const int nforms = stream ? 1 : 2;
+  const long long ns[2] = {stream ? nb[0] + nb[1] : nb[0], stream ? 0 : nb[1]};
+  const uint8_t* skip[2] = {stream ? io->stream_skip : io->luma_skip, io->chroma_skip};
+  const int32_t* dc[2] = {stream ? io->stream_dc : io->luma_dc, io->chroma_dc};
   // every refusal before anything is copied or launched
   const char* why = !kf->cfg.inter_finish ? "the engine was created without inter_finish"
                     : !kf->have_step ? "no step has been submitted"
-                    : !skip[0] || !skip[1] || !dc[0] || !dc[1] ? "luma_skip, chroma_skip, luma_dc and chroma_dc are required"
+                    : stream && classic
+                        ? "both forms of the decisions are given (luma_skip / chroma_skip / luma_dc / chroma_dc and "
+                          "stream_skip / stream_dc): give one"
+                    : stream && !kf->fin_form ? "stream_skip / stream_dc need an engine with symbol_stream = 2"
+                    : stream && (!io->stream_skip || !io->stream_dc) ? "stream_skip and stream_dc are required together"
+                    : !stream && (!skip[0] || !skip[1] || !dc[0] || !dc[1])
+                        ? "luma_skip, chroma_skip, luma_dc and chroma_dc are required"
                     : kf->cfg.inter_finish == 2 && io->dering_level
                         ? "dering_level must be NULL on an inter_finish = 2 engine (the pass searches the levels)"
                     : io->ref_slot_out && !kf->fin_slot_out
@@ -2781,8 +2893,8 @@ int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
     for (int g = 0; !why && r >= 0 && g < f; g++)
       if (io->ref_slot_out[g] == r) why = "two frames name the same ref_slot_out slot";
   }
-  for (int c = 0; !why && c < 2; c++)
-    for (long long i = 0; i < nb[c]; i++) {
+  for (int c = 0; !why && c < nforms; c++)
+    for (long long i = 0; i < ns[c]; i++) {
       if (skip[c][i] > 1) {
         why = "a skip value is neither 0 nor 1";
         break;
@@ -2799,10 +2911,17 @@ int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
     return (int)cudaErrorInvalidValue;
   }
   cudaStream_t s = kf->stream;
-  for (int c = 0; c < 2; c++) {
-    KF_CHECK(cudaMemcpyAsync(kf->fin_skip[c], skip[c], (size_t)nb[c], cudaMemcpyHostToDevice, s));
-    KF_CHECK(cudaMemcpyAsync(kf->fin_dc[c], dc[c], 4 * (size_t)nb[c], cudaMemcpyHostToDevice, s));
+  if (stream) {
+    KF_CHECK(cudaMemcpyAsync(kf->fin_stream_skip, skip[0], (size_t)ns[0], cudaMemcpyHostToDevice, s));
+    KF_CHECK(cudaMemcpyAsync(kf->fin_stream_dc, dc[0], 4 * (size_t)ns[0], cudaMemcpyHostToDevice, s));
+  } else {
+    for (int c = 0; c < 2; c++) {
+      KF_CHECK(cudaMemcpyAsync(kf->fin_skip[c], skip[c], (size_t)nb[c], cudaMemcpyHostToDevice, s));
+      KF_CHECK(cudaMemcpyAsync(kf->fin_dc[c], dc[c], 4 * (size_t)nb[c], cudaMemcpyHostToDevice, s));
+    }
   }
+  // the graph's k_fin_unstream reads the form: the one captured graph serves both
+  if (kf->fin_form) KF_CHECK(cudaMemsetAsync(kf->fin_form, stream ? 1 : 0, sizeof(int32_t), s));
   // inter_finish = 2: the graph's search writes the levels
   if (io->dering_level) KF_CHECK(cudaMemcpyAsync(kf->dering.level, io->dering_level, nsb, cudaMemcpyHostToDevice, s));
   else if (kf->cfg.inter_finish == 1) KF_CHECK(cudaMemsetAsync(kf->dering.level, 0, nsb, s));

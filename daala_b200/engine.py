@@ -13,6 +13,8 @@ one CDF context) and returns them with the reconstruction made at those levels. 
 inter_finish codes a sequence without moving pictures through the host: `finish(..., ref_slot_out=)` stores each
 frame's reconstruction into a pool slot on the device, `encode(..., resident=True)` predicts from the pool as it stands,
 and `pool_load` seeds a slot from host memory or from another engine's device buffer (a GOP's keyframe).
+With inter=1 and symbol_stream=2 each step also returns the P-frame symbol stream (the stream of symbol_stream=1 with a
+DC record per block: qdc and the unquantised residual), and `finish_stream` takes the decisions back in that order.
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -55,13 +57,14 @@ class IO(ctypes.Structure):
                 ("pred_pixels", c_void_p * 3), ("luma_dc", c_void_p), ("chroma_dc", c_void_p),
                 ("ref_pixels", c_void_p * 3), ("nrefs", c_int), ("ref_slot", c_void_p), ("mv_grid", c_void_p),
                 ("pred_pixels_out", c_void_p * 3), ("luma_dc_resid", c_void_p), ("chroma_dc_resid", c_void_p),
-                ("ref_resident", c_int)]
+                ("ref_resident", c_int), ("sym_dc", c_void_p), ("sym_dc_cap", c_ll)]
 
 
 class FinishIO(ctypes.Structure):
     _fields_ = [("luma_skip", c_void_p), ("chroma_skip", c_void_p), ("luma_dc", c_void_p), ("chroma_dc", c_void_p),
                 ("dering_level", c_void_p), ("pixels_out", c_void_p * 3), ("bskip_out", c_void_p * 3),
-                ("dering_level_out", c_void_p), ("ref_slot_out", c_void_p)]
+                ("dering_level_out", c_void_p), ("ref_slot_out", c_void_p), ("stream_skip", c_void_p),
+                ("stream_dc", c_void_p)]
 
 
 class SymBounds(ctypes.Structure):
@@ -303,11 +306,13 @@ class KeyframeEngine:
                     "symbol_bounds")
         return b
 
-    def prepare_io(self, symbols=True, recon=True, stream=None):
+    def prepare_io(self, symbols=True, recon=True, stream=None, pred=True):
         """Builds the daala_b200_kf_io record over the staged inputs and result buffers sized for them.
-        stream (default: whether the engine was created with symbol_stream=1) adds the symbol stream buffers
-        sym_index, sym_blocks, sym_bands and sym_pulses (daala_b200/symbols.py), pinned and sized by
-        daala_b200_kf_symbol_bounds; only their used part is copied back."""
+        stream (default: whether the engine was created with symbol_stream) adds the symbol stream buffers
+        sym_index, sym_blocks, sym_bands and sym_pulses (daala_b200/symbols.py), and sym_dc on a symbol_stream=2
+        engine, pinned and sized by daala_b200_kf_symbol_bounds; only their used part is copied back.  On a
+        symbol_stream=2 engine symbols=False also leaves out the classic DC arrays (the stream carries them).
+        pred=False (inter_mc engines): the prediction planes are not copied back."""
         g, t = self.geom, self.totals
         io = IO()
         for p in range(3):
@@ -340,8 +345,9 @@ class KeyframeEngine:
             for p in range(3):
                 if not self.resident:
                     io.ref_pixels[p] = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8).ctypes.data
-                out["pred%d" % p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
-                io.pred_pixels_out[p] = out["pred%d" % p].ctypes.data
+                if pred:
+                    out["pred%d" % p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
+                    io.pred_pixels_out[p] = out["pred%d" % p].ctypes.data
             io.nrefs = self.nrefs
             io.ref_slot = self._arr("slot", (self.F, 2), np.int32).ctypes.data
             io.mv_grid = self._arr("grid", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1), mvgrid.MV_PT_DTYPE).ctypes.data
@@ -349,10 +355,12 @@ class KeyframeEngine:
             if not self.inter_mc:
                 for p in range(3):
                     io.pred_pixels[p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8).ctypes.data
+        classic_dc = symbols or self.symbol_stream != 2
+        if self.inter and classic_dc:
             out["luma_dc"] = self._arr("ld", (int(t.n_luma),), np.int32)
             out["chroma_dc"] = self._arr("cd", (int(t.n_chroma),), np.int32)
             io.luma_dc, io.chroma_dc = out["luma_dc"].ctypes.data, out["chroma_dc"].ctypes.data
-        if self.inter_finish:
+        if (self.inter_finish or self.symbol_stream == 2) and classic_dc:
             out["luma_dc_resid"] = self._arr("ldr", (int(t.n_luma),), np.int32)
             out["chroma_dc_resid"] = self._arr("cdr", (int(t.n_chroma),), np.int32)
             io.luma_dc_resid, io.chroma_dc_resid = out["luma_dc_resid"].ctypes.data, out["chroma_dc_resid"].ctypes.data
@@ -373,6 +381,9 @@ class KeyframeEngine:
                            ("sym_pulses", b.pulse_bytes)):
                 setattr(io, k, out[k].ctypes.data)
                 setattr(io, k + "_cap", int(cap))
+            if self.symbol_stream == 2:
+                out["sym_dc"] = self._arr("sd", (int(b.blocks),), sym.DC_DTYPE, pinned=True)
+                io.sym_dc, io.sym_dc_cap = out["sym_dc"].ctypes.data, int(b.blocks)
         self._io, self._out = io, out
         px = sum(int(np.prod(g.plane_shape(p))) for p in range(3))
         self.h2d_bytes = px * self.F * (2 if self.inter and not self.inter_mc else 1) + int(np.prod(g.bsize_shape)) * self.F
@@ -391,10 +402,12 @@ class KeyframeEngine:
 
     def stream_d2h_bytes(self):
         """Bytes the last submit copied of the symbol stream (after wait): the index and the used part of the
-        other three arrays."""
+        other arrays (block records, band records, pulses and, on symbol_stream=2 engines, DC records)."""
         from . import symbols as sym
         idx = self._out["sym_index"]
-        return idx.nbytes + int(idx[:, 1].sum()) * sym.BLOCK_DTYPE.itemsize + int(idx[:, 3].sum()) * 8 + int(idx[:, 5].sum())
+        blocks = int(idx[:, 1].sum())
+        dc = blocks * sym.DC_DTYPE.itemsize if "sym_dc" in self._out else 0
+        return idx.nbytes + blocks * sym.BLOCK_DTYPE.itemsize + int(idx[:, 3].sum()) * 8 + int(idx[:, 5].sum()) + dc
 
     def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None, pred=None, refs=None,
                ref_slot=None, mv_grid=None, resident=False):
@@ -428,7 +441,7 @@ class KeyframeEngine:
         inter_finish=2 engine the levels the pass searched, and dering_levels must be None: the C call refuses
         levels there).  ref_slot_out (engines with inter_mc too): [F] int32, the pool slot that receives each frame's
         reconstruction, -1 = not stored; None stores nothing."""
-        g, t = self.geom, self.totals
+        t = self.totals
         fio = FinishIO()
         n = {"luma": int(t.n_luma), "chroma": int(t.n_chroma)}
         for kind, sk, dc in (("luma", luma_skip, luma_dc), ("chroma", chroma_skip, chroma_dc)):
@@ -438,6 +451,26 @@ class KeyframeEngine:
             a = self._arr("fd_" + kind, (n[kind],), np.int32)
             a[...] = dc
             setattr(fio, kind + "_dc", a.ctypes.data)
+        return self._prepare_finish_rest(fio, sum(n.values()), dering_levels, ref_slot_out)
+
+    def prepare_finish_stream(self, skip, dc, dering_levels=None, ref_slot_out=None):
+        """prepare_finish with the decisions in stream order (symbol_stream=2 engines with inter_finish): skip and dc
+        have one entry per block record of the last step's stream, frames one after the other (the order of its
+        sym_blocks).  symbols.stream_to_classic gives each record's index in the classic block order."""
+        t = self.totals
+        fio = FinishIO()
+        n = int(t.n_luma) + int(t.n_chroma)
+        a = self._arr("fs_stream", (n,), np.uint8)
+        a[...] = skip
+        fio.stream_skip = a.ctypes.data
+        a = self._arr("fd_stream", (n,), np.int32)
+        a[...] = dc
+        fio.stream_dc = a.ctypes.data
+        return self._prepare_finish_rest(fio, n, dering_levels, ref_slot_out)
+
+    def _prepare_finish_rest(self, fio, nblocks, dering_levels, ref_slot_out):
+        """The levels, the slot table and the result buffers of a finish record whose decisions are staged."""
+        g = self.geom
         if dering_levels is not None:
             a = self._arr("flev", (self.F, g.nvsb, g.nhsb), np.uint8)
             a[...] = dering_levels
@@ -455,7 +488,7 @@ class KeyframeEngine:
         out["dering_levels"] = self._arr("flev_out", (self.F, g.nvsb, g.nhsb), np.uint8)
         fio.dering_level_out = out["dering_levels"].ctypes.data
         # one skip byte and one int32 DC per block, the levels, the slot table
-        self.finish_h2d_bytes = (5 * sum(n.values()) + (self.F * g.nvsb * g.nhsb if dering_levels is not None else 0)
+        self.finish_h2d_bytes = (5 * nblocks + (self.F * g.nvsb * g.nhsb if dering_levels is not None else 0)
                                  + (4 * self.F if ref_slot_out is not None else 0))
         self.finish_d2h_bytes = sum(v.nbytes for v in out.values())
         self._fio, self._fout = fio, out
@@ -472,6 +505,13 @@ class KeyframeEngine:
         Returns the reconstruction the decoder makes, the skip maps and the levels applied (see prepare_finish);
         views of the engine's host buffers."""
         self.prepare_finish(luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels, ref_slot_out)
+        self.finish_submit()
+        self.wait()
+        return self._fout
+
+    def finish_stream(self, skip, dc, dering_levels=None, ref_slot_out=None):
+        """finish with the decisions in the order of the last step's symbol stream (see prepare_finish_stream)."""
+        self.prepare_finish_stream(skip, dc, dering_levels, ref_slot_out)
         self.finish_submit()
         self.wait()
         return self._fout

@@ -1,5 +1,7 @@
 """The keyframe engine's symbol stream (include/daala_b200.h, "Symbol stream"; config.symbol_stream = 1): per
-frame the PVQ symbols the serial entropy coder reads, in bitstream order.
+frame the PVQ symbols the serial entropy coder reads, in bitstream order.  The P-frame stream (symbol_stream = 2,
+inter = 1) is the same with flip = 0 and a DC_DTYPE record per block record (sym_dc, same index): the step's scalar
+DC index and the unquantised DC residual.
 
 For each frame of a batch the index (int64[6]: first block, block count, first band, band count, first pulse
 byte, pulse byte count) locates three parts inside batch-wide arrays:
@@ -10,8 +12,9 @@ byte, pulse byte count) locates three parts inside batch-wide arrays:
 Coding order: superblocks in raster order, planes 0, 1, 2, inside a plane the quadtree leaves depth-first with
 the children top-left, top-right, bottom-left, bottom-right (od_encode_recursive, reference src/encode.c).
 
-This module holds the dtypes, a reader, `coding_order` (a walk of that recursion over a block-size map) and
-`pack_reference` (the expected stream built with numpy from the engine's classic outputs)."""
+This module holds the dtypes, a reader, `coding_order` (a walk of that recursion over a block-size map),
+`pack_reference` (the expected stream built with numpy from the engine's classic outputs) and `stream_to_classic`
+(each stream record's index in the classic block order)."""
 import numpy as np
 
 BLOCK_DTYPE = np.dtype([("skip_diff", "<f8"), ("pulse_off", "<u4"), ("band_off", "<u4"), ("x0", "<u2"),
@@ -21,6 +24,8 @@ INDEX_FIELDS = ("first_block", "n_blocks", "first_band", "n_bands", "first_byte"
 NBANDS = np.array([1, 4, 7, 9, 9])
 BAND_EDGES = np.array([1, 16, 24, 32, 64, 96, 128, 256, 384, 512])   # OD_BAND_OFFSETS in coding order
 ORDER_DTYPE = np.dtype([("pli", "u1"), ("x0", "<u2"), ("y0", "<u2"), ("bs", "u1")])
+DC_DTYPE = np.dtype([("qdc", "<i4"), ("dc_resid", "<i4")])
+assert DC_DTYPE.itemsize == 8
 
 
 def _excl(a):
@@ -46,9 +51,10 @@ def _band_numbers(bs):
 
 
 def read_frame(out, f):
-    """Frame f of a submit's stream outputs (sym_index, sym_blocks, sym_bands, sym_pulses): dict with `blocks`
-    (BLOCK_DTYPE), `bands` (int16[B, 4]), `band_block` (block of each band), `band_no` (band number inside its
-    block) and `pulses` (per band an int32 vector of its coded values; empty when K = 0)."""
+    """Frame f of a submit's stream outputs (sym_index, sym_blocks, sym_bands, sym_pulses[, sym_dc]): dict with
+    `blocks` (BLOCK_DTYPE), `bands` (int16[B, 4]), `band_block` (block of each band), `band_no` (band number inside
+    its block), `pulses` (per band an int32 vector of its coded values; empty when K = 0) and, when the outputs have
+    sym_dc, `dc` (DC_DTYPE, one record per block)."""
     idx = out["sym_index"][f]
     b0, nb, n0, nn, y0, ny = (int(v) for v in idx)
     blocks = out["sym_blocks"][b0:b0 + nb]
@@ -73,7 +79,10 @@ def read_frame(out, f):
     v = np.where(w == 2, (lo | (hi << 8)).astype(np.uint16).view(np.int16), lo.astype(np.uint8).view(np.int8))
     v = v.astype(np.int32)
     pulses = np.split(v, np.cumsum(n)[:-1]) if nn else []
-    return dict(blocks=blocks, bands=bands, band_block=band_block, band_no=band_no, pulses=pulses)
+    r = dict(blocks=blocks, bands=bands, band_block=band_block, band_no=band_no, pulses=pulses)
+    if "sym_dc" in out:
+        r["dc"] = out["sym_dc"][b0:b0 + nb]
+    return r
 
 
 def coding_order(bsize, geom, sb_row0=0, sb_rows=None):
@@ -115,9 +124,10 @@ def _zrank(x0, y0, pli):
     return y0 >> sh, x0 >> sh, z
 
 
-def pack_blocks(x0, y0, bs, pli, flip, skip_diff, res, y, y_off):
+def pack_blocks(x0, y0, bs, pli, flip, skip_diff, res, y, y_off, qdc=None, dc_resid=None):
     """One frame's stream parts from its blocks listed in coding order: band records res[i, :nbands] and
-    pulse vectors in coding order at y[y_off[i]:] (DC at index 0).  Returns (blocks, bands, pulses)."""
+    pulse vectors in coding order at y[y_off[i]:] (DC at index 0).  Returns (blocks, bands, pulses), and with qdc
+    and dc_resid (P frames) also the DC records."""
     n = len(bs)
     bs = np.asarray(bs).astype(np.int64)
     band_no, per = _band_numbers(bs)
@@ -140,28 +150,38 @@ def pack_blocks(x0, y0, bs, pli, flip, skip_diff, res, y, y_off):
     pulses[pos] = (v & 0xff).astype(np.uint8)
     m = w == 2
     pulses[pos[m] + 1] = ((v[m] >> 8) & 0xff).astype(np.uint8)
-    return blocks, bands, pulses
+    if qdc is None:
+        return blocks, bands, pulses
+    dc = np.zeros(n, DC_DTYPE)
+    dc["qdc"], dc["dc_resid"] = qdc, dc_resid
+    return blocks, bands, pulses, dc
 
 
 def concat_frames(parts):
-    """Batch-wide (index, blocks, bands, pulses) from per-frame (blocks, bands, pulses)."""
+    """Batch-wide (index, blocks, bands, pulses[, dc]) from per-frame (blocks, bands, pulses[, dc])."""
     index = np.zeros((len(parts), 6), np.int64)
     pos = np.zeros(3, np.int64)
-    for f, (b, n, p) in enumerate(parts):
+    for f, (b, n, p) in enumerate(q[:3] for q in parts):
         index[f] = (pos[0], len(b), pos[1], len(n), pos[2], len(p))
         pos += (len(b), len(n), len(p))
     cat = (lambda xs, dt, shape: np.concatenate(xs) if xs else np.zeros(shape, dt))
-    return dict(sym_index=index, sym_blocks=cat([p[0] for p in parts], BLOCK_DTYPE, (0,)),
-                sym_bands=cat([p[1] for p in parts], np.int16, (0, 4)),
-                sym_pulses=cat([p[2] for p in parts], np.uint8, (0,)))
+    r = dict(sym_index=index, sym_blocks=cat([p[0] for p in parts], BLOCK_DTYPE, (0,)),
+             sym_bands=cat([p[1] for p in parts], np.int16, (0, 4)),
+             sym_pulses=cat([p[2] for p in parts], np.uint8, (0,)))
+    if parts and len(parts[0]) == 4:
+        r["sym_dc"] = cat([p[3] for p in parts], DC_DTYPE, (0,))
+    return r
 
 
 def pack_reference(out, frames):
     """The stream the engine must produce, built from a submit's classic outputs (luma_/chroma_blocks, _res,
     _y16, _skip_diff, chroma_flip) for the frames `frames` (list, or a count = frames 0 .. count-1).  Blocks are
     put in bitstream order by sorting on (superblock, plane, Z order of the origin), independently of how the
-    device ranks them.  Returns dict(sym_index, sym_blocks, sym_bands, sym_pulses) over those frames."""
+    device ranks them.  Returns dict(sym_index, sym_blocks, sym_bands, sym_pulses) over those frames.  The outputs of
+    a P-frame step (they have luma_dc / chroma_dc, and luma_dc_resid / chroma_dc_resid must be there too) give the
+    P-frame stream: flip 0 and sym_dc from *_dc and *_dc_resid."""
     frames = list(range(frames)) if np.isscalar(frames) else list(frames)
+    inter = "luma_dc" in out
     lb, cb = out["luma_blocks"], out["chroma_blocks"]
     nl_coefs = len(out["luma_y16"])
     y = np.concatenate([out["luma_y16"], out["chroma_y16"]])
@@ -171,14 +191,42 @@ def pack_reference(out, frames):
         blk = np.concatenate([lb[sl], cb[sc]])
         res = np.concatenate([out["luma_res"][sl], out["chroma_res"][sc]])
         skip = np.concatenate([out["luma_skip_diff"][sl], out["chroma_skip_diff"][sc]])
-        flip = np.concatenate([np.zeros(len(sl), np.int64), out["chroma_flip"][sc].astype(np.int64)])
+        flip = np.zeros(len(blk), np.int64)
+        if not inter:
+            flip[len(sl):] = out["chroma_flip"][sc]
         y_off = np.concatenate([lb["coef_off"][sl].astype(np.int64), cb["coef_off"][sc].astype(np.int64) + nl_coefs])
         pli = blk["pli"].astype(np.int64)
         sby, sbx, z = _zrank(blk["x0"], blk["y0"], pli)
         o = np.lexsort((z, pli, sbx, sby))
+        dc = {}
+        if inter:
+            for k in ("dc", "dc_resid"):
+                dc[k] = np.concatenate([out["luma_" + k][sl], out["chroma_" + k][sc]])[o]
         parts.append(pack_blocks(blk["x0"][o], blk["y0"][o], blk["bs"][o], pli[o], flip[o], skip[o], res[o], y,
-                                 y_off[o]))
+                                 y_off[o], dc.get("dc"), dc.get("dc_resid")))
     return concat_frames(parts)
+
+
+def stream_to_classic(out):
+    """For every block record of a submit's stream (sym_index, sym_blocks), in the order of sym_blocks (frames one
+    after the other), the index of the same block in the classic block order (luma_blocks i -> i, chroma_blocks
+    i -> n_luma + i).  A decision array `d` in classic order is `d[stream_to_classic(out)]` in stream order (what
+    KeyframeEngine.finish_stream takes)."""
+
+    def key(frame, pli, x0, y0):
+        return ((np.asarray(frame, np.int64) * 3 + pli) << 32) | (np.asarray(y0, np.int64) << 16) | np.asarray(x0, np.int64)
+
+    lb, cb = out["luma_blocks"], out["chroma_blocks"]
+    classic = np.concatenate([key(b["frame"], b["pli"].astype(np.int64), b["x0"], b["y0"]) for b in (lb, cb)])
+    idx = out["sym_index"]
+    n = int(idx[:, 1].sum())
+    sb = out["sym_blocks"][:n]
+    stream = key(np.repeat(np.arange(len(idx)), idx[:, 1]), sb["pli"].astype(np.int64), sb["x0"], sb["y0"])
+    o = np.argsort(classic, kind="stable")
+    pos = np.minimum(np.searchsorted(classic[o], stream), max(len(o) - 1, 0))
+    assert n == len(classic) and np.array_equal(classic[o][pos], stream), \
+        "the stream's blocks are not the classic lists' blocks"
+    return o[pos]
 
 
 def stream_equal(got, want, frames_got, frames_want=None):
@@ -192,7 +240,13 @@ def stream_equal(got, want, frames_got, frames_want=None):
                 bad.append((fg, name, int(ig[col]), int(iw[col])))
         if bad:
             continue
-        for key, c0, c1 in (("sym_blocks", 0, 1), ("sym_bands", 2, 3), ("sym_pulses", 4, 5)):
+        parts = (("sym_blocks", 0, 1), ("sym_bands", 2, 3), ("sym_pulses", 4, 5))
+        if "sym_dc" in got or "sym_dc" in want:
+            parts += (("sym_dc", 0, 1),)
+        for key, c0, c1 in parts:
+            if key not in got or key not in want:
+                bad.append((fg, key, "missing"))
+                continue
             a = got[key][ig[c0]:ig[c0] + ig[c1]]
             b = want[key][iw[c0]:iw[c0] + iw[c1]]
             if a.tobytes() != b.tobytes():

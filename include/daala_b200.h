@@ -470,7 +470,12 @@ typedef struct daala_b200_kf_config {
   double dering_lambda;        /* enc->dering_lambda (src/rate.c:1086); dering == 2 or inter_finish == 2 */
   int symbol_stream;           /* 1: every step also packs the PVQ symbols of each frame in bitstream order
                                   (daala_b200_kf_sym_block below) for daala_b200_kf_io.sym_*; 0 (default): the step
-                                  is exactly the one without the stream */
+                                  is exactly the one without the stream.
+                                  2: the P-frame stream (requires inter = 1): the stream of 1 with flip = 0 and one
+                                  daala_b200_kf_sym_dc record per block (daala_b200_kf_io.sym_dc); with inter_finish
+                                  the finishing pass also takes its decisions in stream order
+                                  (daala_b200_kf_finish_io.stream_skip / stream_dc).  1 is refused with inter (a
+                                  keyframe block has no scalar DC), 2 without it; other values are refused */
   int inter;                   /* 0 (default): keyframes, exactly the engine described above.
                                   1: P-frame residual mode.  Every frame is coded as od_encode_coefficients codes a
                                   non-key frame, entropy coding and the coder-state skip decision left to the host:
@@ -484,7 +489,8 @@ typedef struct daala_b200_kf_config {
                                   daala_b200_kf_io.luma_dc / chroma_dc); the uncoded tail of 32x32 / 64x64 blocks is
                                   the transformed prediction (od_init_skipped_coeffs for inter frames).
                                   Not defined, and refused by daala_b200_kf_create, together with dering,
-                                  symbol_stream, noref_prepass, level_chains or a row shard (sb_rows > 0) */
+                                  symbol_stream = 1 (2 is its stream), noref_prepass, level_chains or a row shard
+                                  (sb_rows > 0) */
   int inter_mc;                /* 0 (default): with inter, the prediction planes are the host input pred_pixels.
                                   1: the engine makes the prediction itself, as od_state_mc_predict does
                                   (reference src/state.c:932), from each frame's MV grid
@@ -500,7 +506,8 @@ typedef struct daala_b200_kf_config {
   int inter_finish;            /* 0 (default): nothing below exists; the engine is exactly the one without this field.
                                   1: the engine also has the finishing pass daala_b200_kf_finish (the host coder's skip
                                   and DC decisions, the skip map bskip, deringing over it, final reconstruction), and
-                                  each step writes daala_b200_kf_io.luma_dc_resid / chroma_dc_resid.
+                                  each step writes daala_b200_kf_io.luma_dc_resid / chroma_dc_resid (as does an engine
+                                  with symbol_stream = 2).
                                   2: the same pass, which also SEARCHES the deringing levels of every frame instead of
                                   taking them (src/encode.c:2708-2811 for a P frame, see daala_b200_kf_finish_io);
                                   needs coded_quantizer / qm_is_flat / dering_lambda above.
@@ -541,6 +548,14 @@ typedef struct daala_b200_kf_sym_block {   /* 24 bytes, 8-byte aligned */
   uint8_t flip;            /* keyframe CfL sign flip (chroma); 0 for luma */
   uint8_t reserved;        /* 0 */
 } daala_b200_kf_sym_block;
+
+/* symbol_stream = 2 (P frames): one record per block record, at the same index as the daala_b200_kf_sym_block it
+   belongs to (a frame's part is first_block / n_blocks of the index, as for the block records). */
+typedef struct daala_b200_kf_sym_dc {      /* 8 bytes */
+  int32_t qdc;             /* the step's scalar DC index (as daala_b200_kf_io.luma_dc / chroma_dc) */
+  int32_t dc_resid;        /* the unquantised DC residual in[0] - ref[0] (as daala_b200_kf_io.*_dc_resid), what the
+                              host's od_rdo_quant quantises (src/pvq_encoder.c:886 / :956) */
+} daala_b200_kf_sym_dc;
 
 typedef struct daala_b200_kf_sym_frame {   /* one frame's part of the batch-wide arrays (indices, not bytes, */
   int64_t first_block, n_blocks;           /* except for the pulses) */
@@ -584,7 +599,8 @@ typedef struct daala_b200_kf_io {
   long long sym_bands_cap;
   uint8_t *sym_pulses;
   long long sym_pulses_cap;
-  /* config.inter only (required there, ignored otherwise). */
+  /* config.inter only (required there, ignored otherwise; luma_dc / chroma_dc are optional with symbol_stream = 2,
+     whose sym_dc carries the same indices). */
   const uint8_t *pred_pixels[3];        /* motion-compensated prediction planes, shapes and padding of `pixels` */
   int32_t *luma_dc, *chroma_dc;         /* [n_blocks]: the scalar-quantised DC index qdc of each block (keyframes code
                                            DC in the Haar pyramid instead), block order of luma_res / chroma_res */
@@ -596,7 +612,7 @@ typedef struct daala_b200_kf_io {
                                            when the frame predicts from one picture) */
   const daala_b200_mv_pt *mv_grid;      /* [nframes][nvsb*8 + 1][nhsb*8 + 1]: each frame's state->mv_grid */
   uint8_t *pred_pixels_out[3];          /* optional: the prediction planes the engine made, layout of pixels */
-  /* config.inter_finish only (optional, NULL = not copied). */
+  /* config.inter_finish or symbol_stream = 2 only (optional, NULL = not copied). */
   int32_t *luma_dc_resid, *chroma_dc_resid; /* [n_blocks]: each block's unquantised DC residual in[0] - ref[0] (what the
                                            host's od_rdo_quant quantises, src/pvq_encoder.c:886 / :956), block order
                                            of luma_dc / chroma_dc */
@@ -607,6 +623,11 @@ typedef struct daala_b200_kf_io {
      daala_b200_kf_finish_io.ref_slot_out has written it.  Everything is ordered by call order on the engine's
      stream: a step submitted before the finish that rewrites its PREV slot reads the old picture. */
   int ref_resident;
+  /* config.symbol_stream = 2 only: the DC records of the stream (daala_b200_kf_sym_dc), a pinned host buffer with its
+     capacity in records, at least daala_b200_kf_symbol_bounds(...).blocks; NULL = not copied.  Only the used part is
+     copied, as for the other stream arrays. */
+  daala_b200_kf_sym_dc *sym_dc;
+  long long sym_dc_cap;
 } daala_b200_kf_io;
 
 /* The finishing pass of a P-frame batch (config.inter_finish), daala_b200_kf_finish: the host coder's per-block
@@ -651,6 +672,11 @@ typedef struct daala_b200_kf_finish_io {
                                               Rewriting a slot the last step read (a frame's own PREV slot) is legal:
                                               the step's prediction and md are already made, and a repeated finish
                                               reads md, never the pool; the last finish wins. */
+  /* The decisions in stream order (engines with config.symbol_stream = 2): one entry per block of the last submitted
+     step, in the order of that step's sym_blocks, frames one after the other (n_luma + n_chroma entries).  A call
+     gives either these two or the four classic arrays above, never both; the same checks apply to either form. */
+  const uint8_t *stream_skip;              /* 0 or 1 */
+  const int32_t *stream_dc;                /* the final DC index */
 } daala_b200_kf_finish_io;
 
 typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, device-resident callers) */
@@ -715,8 +741,9 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    H2D of the inputs, the whole step, D2H of the requested outputs: enqueued, not waited for.  A batch with more
    luma or chroma blocks than the engine's capacity (see max_blocks_div) returns cudaErrorInvalidValue before
    anything is copied or launched; so does a request for symbol stream outputs from an engine created without
-   symbol_stream, a stream capacity below daala_b200_kf_symbol_bounds, a stream buffer that is not pinned host
-   memory, or (config.inter) a NULL pred_pixels plane, luma_dc or chroma_dc.  With config.inter_mc it refuses, the same
+   symbol_stream (sym_dc: without symbol_stream = 2), a stream capacity below daala_b200_kf_symbol_bounds, a stream
+   buffer that is not pinned host memory, or (config.inter) a NULL pred_pixels plane, luma_dc or chroma_dc (the last
+   two are optional with symbol_stream = 2).  With config.inter_mc it refuses, the same
    way, a NULL mv_grid, ref_pixels plane or ref_slot, pred_pixels given, nrefs outside [1, mc_refs] and a slot outside
    [0, nrefs); with ref_resident = 1 it refuses instead ref_pixels given, nrefs other than 0, a slot outside
    [0, mc_refs) and a slot that holds no picture.  The step counts in `counts` the leaf corners whose vertex has a ref other than 0 or 1 (counts[19]) and
@@ -729,10 +756,13 @@ int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
    waited for with daala_b200_kf_wait.  The step's outputs and its d / md planes are not modified (the decisions are
    applied to a plane of their own), so the pass may run any number of times after one step.  Refused with
    cudaErrorInvalidValue and a message in daala_b200_kf_error, before anything is copied or launched: an engine
-   without inter_finish, no step submitted yet, a NULL decision array, a skip value other than 0 or 1, a level above
+   without inter_finish, no step submitted yet, a NULL decision array (neither form complete), both forms given, the
+   stream form on an engine without symbol_stream = 2, a skip value other than 0 or 1, a level above
    5, a |dc| above DAALA_B200_KF_FINISH_DC_LIMIT / DQ, (config.inter_finish = 2) a non-NULL dering_level, and a
    ref_slot_out on an engine without inter_mc, with an entry outside [-1, mc_refs) or with two frames naming one slot.
-   With ref_slot_out the pass's last kernel copies each stored frame's reconstruction into its pool slot. */
+   With ref_slot_out the pass's last kernel copies each stored frame's reconstruction into its pool slot.  With the
+   stream form the decisions are copied into staging buffers and the pass's first kernel scatters them into block
+   order through the step's slot -> block map. */
 int daala_b200_kf_finish(daala_b200_kf *kf, const daala_b200_kf_finish_io *io);
 /* Enqueues on the engine's stream the copies of one frame-sized picture (planes[p]: [plane_h][plane_w] u8, the layout
    of one frame of daala_b200_kf_io.pixels) into slot `slot` of the reference-picture pool (config.inter_mc), with

@@ -13,13 +13,22 @@ Two loops of steps (submit, wait for the step's outputs, finish), run alternatel
   resident           the submit reads the pool on the device (ref_resident), the finish stores its reconstruction
                      into slots 16..31 (ref_slot_out) and still copies it to the host (pixels_out);
   resident_no_recon  the same without pixels_out.
-Both loops request the same step outputs (block records, band records, pulses, DC indices, the prediction) and no
-skip maps or levels from the finish.  Before timing: after 3 steps the round trip's and the resident loop's outputs
+These three request the same step outputs (block records, band records, pulses, DC indices, the prediction) and no
+skip maps or levels from the finish.  Two more loops copy neither the reconstruction nor the prediction, so that the
+difference between them is the P-frame symbol stream's alone:
+  classic_no_pred    resident_no_recon without the prediction planes (prepare_io(pred=False));
+  stream             an engine with symbol_stream = 2: the step returns only the stream (index, block, band, pulse and
+                     DC records, the used part of each) and the finish takes the same decisions in stream order
+                     (finish_io.stream_skip / stream_dc).  Before timing: after 3 steps the round trip's and the resident loop's outputs
 and pools must be identical, and, when oracle/_ref was built, frame 0 of the first step is checked against the oracle
-(prediction against od_state_mc_predict, reconstruction against inverse_frame_inter_finish).
+(prediction against od_state_mc_predict, reconstruction against inverse_frame_inter_finish).  The stream loop's first
+step must equal symbols.pack_reference of the resident loop's classic outputs of the same step, and after 3 steps its
+pool must equal the resident loop's.
 
 Reports per-step wall time (host clock around --steps steps ending in a stream synchronise, --rounds rounds), the H2D
-and D2H bytes of a step, and the card's name and power limit.  --profile: a run of its own that times
+and D2H bytes of a step, the device time of the step graph with symbol_stream 0 and 2 (CUDA events around --steps graph
+replays, --rounds alternating rounds: their difference is the stream kernels' cost), and the card's name and power
+limit.  --profile: a run of its own that times
 k_fin_pool_store with torch.profiler over --steps resident steps and sets its bytes (read + write of every stored
 plane) against the 3.35 TB/s of the H100 SXM data sheet.  Needs a CUDA device; prints one JSON line.
 
@@ -50,7 +59,8 @@ class Loop:
         eng.stage_inputs(planes, bsize)
         resident = mode != "round_trip"
         eng.stage_mc(None if resident else pool, slot, packed, resident=resident)
-        self.out = eng.prepare_io(symbols=True, recon=False)
+        lean = mode in ("classic_no_pred", "stream")
+        self.out = eng.prepare_io(symbols=mode != "stream", recon=False, pred=not lean)
         self.io = eng._io
         self.h2d, self.d2h = eng.h2d_bytes, eng.d2h_bytes
         self.px = [int(np.prod(geom.plane_shape(p))) for p in range(3)]
@@ -62,19 +72,23 @@ class Loop:
         import numpy as np
         from daala_b200 import engine
         eng, F = self.eng, self.F
-        eng.prepare_finish(*dec, ref_slot_out=None if self.mode == "round_trip" else np.arange(F, 2 * F, dtype=np.int32))
+        store = None if self.mode == "round_trip" else np.arange(F, 2 * F, dtype=np.int32)
+        if self.mode == "stream":   # dec: (skip, dc, levels) in stream order
+            eng.prepare_finish_stream(*dec, ref_slot_out=store)
+        else:
+            eng.prepare_finish(*dec, ref_slot_out=store)
         fio = engine.FinishIO.from_buffer_copy(eng._fio)
         for p in range(3):
             fio.bskip_out[p] = None
             if self.mode == "round_trip":
                 fio.pixels_out[p] = self.host_pool[p].ctypes.data + F * self.px[p]
-            elif self.mode == "resident_no_recon":
+            elif self.mode != "resident":
                 fio.pixels_out[p] = None
         fio.dering_level_out = None
         self.fio = fio
         self.recon = [eng._fout["recon%d" % p] for p in range(3)] if self.mode == "resident" else None
         self.finish_h2d = eng.finish_h2d_bytes
-        self.finish_d2h = 0 if self.mode == "resident_no_recon" else sum(self.px) * F
+        self.finish_d2h = sum(self.px) * F if self.mode in ("round_trip", "resident") else 0
 
     def step(self):
         eng = self.eng
@@ -129,7 +143,7 @@ def main():
     args = ap.parse_args()
     import numpy as np
     import bench
-    from daala_b200 import _native, engine, mvgrid, synth
+    from daala_b200 import _native, engine, mvgrid, symbols, synth
     from daala_b200.frame import Geometry
     if _native.lib().daala_b200_device_count() < 1:
         sys.exit("bench_engine_pool.py needs a CUDA device: nothing is measured without one")
@@ -198,11 +212,27 @@ def main():
     trip.set_decisions(dec)
     bare = Loop(res_eng, geom, F, planes, bsize, slot, packed, None, "resident_no_recon")
     bare.set_decisions(dec)
+    lean = Loop(res_eng, geom, F, planes, bsize, slot, packed, None, "classic_no_pred")
+    lean.set_decisions(dec)
+    # the stream loop: its own engine and pool; a first submit gives the stream order the decisions are permuted into
+    st_eng = engine.KeyframeEngine(geom, symbol_stream=2, **common)
+    for s in range(2 * F):
+        st_eng.pool_load(s, [pool0[p][s] for p in range(3)])
+    stream = Loop(st_eng, geom, F, planes, bsize, slot, packed, None, "stream")
+    st_eng._check(st_eng.L.daala_b200_kf_submit(st_eng.kf, ctypes.byref(stream.io)), "kf_submit")
+    sout = st_eng.wait()
+    perm = symbols.stream_to_classic(dict(out, sym_index=np.array(sout["sym_index"]), sym_blocks=np.array(sout["sym_blocks"])))
+    stream.set_decisions((np.concatenate([dec[0], dec[2]])[perm], np.concatenate([dec[1], dec[3]])[perm], dec[4]))
 
     # parity: frame 0 of the first step against the oracle, then 3 steps of both loops equal
     res.step()
     trip.step()
+    stream.step()
     res_eng.wait()
+    st_eng.wait()
+    bad = symbols.stream_equal(stream.out, symbols.pack_reference(res.out, F), range(F))
+    if bad:
+        sys.exit("bench_engine_pool.py: the stream differs from the classic outputs of the same step: %s" % (bad[:4],))
     mism = oracle_check(geom, res, [pool0[p][0] for p in range(3)], [pool0[p][F] for p in range(3)], grids[0], bsize,
                         q4, dec, bench.Q0)
     if mism:
@@ -210,6 +240,7 @@ def main():
     for _ in range(2):
         res.step()
         trip.step()
+        stream.step()
     res_eng.wait()
     trip_eng.wait()
     diff = 0
@@ -221,31 +252,51 @@ def main():
     rp, tp = res.pool(), trip.pool()
     diff += sum(int(np.count_nonzero(rp[p] != tp[p])) for p in range(3))
     diff += sum(int(np.count_nonzero(res.recon[p] != tp[p][F:])) for p in range(3))
+    sp = stream.pool()
+    diff += sum(int(np.count_nonzero(rp[p] != sp[p])) for p in range(3))
     if diff:
-        sys.exit("bench_engine_pool.py: after 3 steps the resident loop differs from the round trip (%d values)" % diff)
+        sys.exit("bench_engine_pool.py: after 3 steps the resident and stream loops differ from the round trip (%d values)"
+                 % diff)
+    stream.d2h += st_eng.stream_d2h_bytes()   # the used part of the stream arrays (the same every step)
 
-    loops = {"round_trip": trip, "resident": res, "resident_no_recon": bare}
+    loops = {"round_trip": trip, "resident": res, "resident_no_recon": bare, "classic_no_pred": lean, "stream": stream}
     for lp in loops.values():
         lp.timed(1)
     rounds = {name: [] for name in loops}
     for _ in range(args.rounds):
         for name, lp in loops.items():
             rounds[name].append(lp.timed(args.steps))
+    # the step graph alone, symbol_stream 0 against 2, on the same inputs and pool
+    graph = {"symbol_stream_0": [], "symbol_stream_2": []}
+    for e in (res_eng, st_eng):
+        e.time_device(engine.PH_ALL, True, 1)
+    for _ in range(args.rounds):
+        graph["symbol_stream_0"].append(res_eng.time_device(engine.PH_ALL, True, args.steps) / args.steps)
+        graph["symbol_stream_2"].append(st_eng.time_device(engine.PH_ALL, True, args.steps) / args.steps)
     line = {"workload": "%d independent sequences of synthetic 3840x2160 4:2:0 frames, shipped block-size maps and "
                         "deringing levels, q0 %d, mc_refs %d (GOLD slot f, PREV slot %d + f), seeded MV grids, 30 %% of "
                         "the blocks skipped with DC 0; a step = submit, wait, finish" % (F, bench.Q0, 2 * F, F),
             "gpu": bench.gpu_identity(0), "steps_per_round": args.steps, "rounds": args.rounds,
             "parity_checked": ("frame 0 of the first step against od_state_mc_predict and inverse_frame_inter_finish "
                                "(reference build)" if mism is not None else "oracle/_ref not built: frame 0 not checked")
-                              + "; 3 steps of both loops: outputs and pools identical"}
+                              + "; 3 steps of the round trip and the resident loop: outputs and pools identical; the "
+                                "stream loop's first stream equals pack_reference of the resident loop's outputs, its "
+                                "pool after 3 steps the resident loop's"}
     for name, lp in loops.items():
         line[name] = {"ms_per_step": round(statistics.median(rounds[name]), 3),
                       "ms_per_step_rounds": [round(v, 3) for v in rounds[name]],
                       "h2d_bytes_per_step": int(lp.h2d + lp.finish_h2d),
                       "d2h_bytes_per_step": int(lp.d2h + lp.finish_d2h)}
     line["h2d_saved_bytes_per_step"] = line["round_trip"]["h2d_bytes_per_step"] - line["resident"]["h2d_bytes_per_step"]
+    line["stream_d2h_saved_bytes_per_step"] = (line["classic_no_pred"]["d2h_bytes_per_step"]
+                                               - line["stream"]["d2h_bytes_per_step"])
+    line["step_graph_ms"] = {k: {"median": round(statistics.median(v), 3), "rounds": [round(x, 3) for x in v]}
+                             for k, v in graph.items()}
+    line["stream_kernels_ms_per_step"] = round(statistics.median(graph["symbol_stream_2"])
+                                               - statistics.median(graph["symbol_stream_0"]), 3)
     trip_eng.close()
     res_eng.close()
+    st_eng.close()
     print(json.dumps(line), flush=True)
 
 
