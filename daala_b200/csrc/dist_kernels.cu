@@ -2,113 +2,29 @@
 // od_compute_dist_8x8 :1111, od_compute_dist :1180) for a batch of packed n x n block pairs --
 // SURVEY.md 8(f) rank 2: the metric the deringing level search and the block-size decision evaluate.
 //
-// Parity: tests/test_gpu_dist.py against oracle/port_dist.c (bit-identical to od_compute_dist); consumer:
-// the deringing level search, csrc/dering_search.cu.
+// Parity: tests/test_gpu_dist.py against oracle/port_dist.c (bit-identical to od_compute_dist); consumers:
+// the deringing level search, csrc/dering_search.cu, and (through dist_device.cuh) the late-skip kernel.
 //
-// Mapping: one 64-thread CTA per block pair.  The error x - y is low-passed by the separable [1 5 1]
-// kernel in shared memory (integer, exact); one thread per 8x8 sub-block then evaluates the nine
-// overlapping 4x4 window variances and the activity factor in double precision in the reference's
-// operation order, and thread 0 adds the sub-block results in raster order (double addition is not
-// associative).  sqrt is IEEE (-prec-sqrt=true); pow comes from the CUDA math library (<= 2 ulp), so
-// the result is compared with a 1e-12 relative tolerance rather than bit for bit.
+// Mapping: one 64-thread CTA per block pair running block_dist (dist_device.cuh, which gives the operation order).
+// sqrt is IEEE (-prec-sqrt=true); pow comes from the CUDA math library (<= 2 ulp), so the HVS result is compared
+// with a 1e-12 relative tolerance rather than bit for bit.
 #include <cuda_runtime.h>
-#include <limits.h>
-#include <math.h>
 #include <stdint.h>
 
 #include "daala_b200.h"
+#include "dist_device.cuh"
 
 namespace daala_b200 {
 namespace dist {
 
-__device__ __forceinline__ int window_var(const int32_t* p, int stride) {
-  int s = 0, s2 = 0;
-#pragma unroll
-  for (int i = 0; i < 4; i++) {
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      const int t = p[i * stride + j] >> 2;
-      s += t;
-      s2 += t * t;
-    }
-  }
-  return s2 - (s * s >> 4);
-}
-
-__global__ void __launch_bounds__(64)
+__global__ void __launch_bounds__(kDistThreads)
 k_compute_dist(const int32_t* __restrict__ xs, const int32_t* __restrict__ ys, int n, int qm_is_flat,
                int use_activity_masking, double scale, double* __restrict__ out) {
   extern __shared__ __align__(16) int32_t smem[];
-  const int nn = n * n;
-  const int32_t* x = xs + (size_t)blockIdx.x * nn;
-  const int32_t* y = ys + (size_t)blockIdx.x * nn;
-  if (qm_is_flat) {
-    // plain squared error, accumulated in index order by one thread (double order)
-    if (threadIdx.x == 0) {
-      double total = 0;
-      for (int i = 0; i < nn; i++) {
-        const double d = x[i] - y[i];
-        total += d * d;
-      }
-      out[blockIdx.x] = total;
-    }
-    return;
-  }
-  int32_t* err = smem;            // n*n
-  int32_t* rows = smem + nn;      // n*n, then reused for the low-passed error
-  double* part = (double*)(smem + 2 * nn);   // (n/8)^2 sub-block results
-  for (int i = threadIdx.x; i < nn; i += 64) err[i] = x[i] - y[i];
-  __syncthreads();
-  for (int idx = threadIdx.x; idx < nn; idx += 64) {
-    const int i = idx / n, j = idx - i * n;
-    const int32_t* e = err + i * n;
-    int32_t v;
-    if (j == 0) v = 5 * e[0] + 2 * e[1];
-    else if (j == n - 1) v = 5 * e[n - 1] + 2 * e[n - 2];
-    else v = 5 * e[j] + e[j - 1] + e[j + 1];
-    rows[idx] = v;
-  }
-  __syncthreads();
-  // vertical pass into err (the raw error is no longer needed)
-  for (int idx = threadIdx.x; idx < nn; idx += 64) {
-    const int i = idx / n, j = idx - i * n;
-    int32_t v;
-    if (i == 0) v = 5 * rows[j] + 2 * rows[n + j];
-    else if (i == n - 1) v = 5 * rows[(n - 1) * n + j] + 2 * rows[(n - 2) * n + j];
-    else v = 5 * rows[idx] + rows[idx - n] + rows[idx + n];
-    err[idx] = v;
-  }
-  __syncthreads();
-  const int nb = n >> 3;
-  if ((int)threadIdx.x < nb * nb) {
-    const int bi = threadIdx.x / nb, bj = threadIdx.x - bi * nb;
-    const int32_t* px = x + bi * 8 * n + bj * 8;
-    const int32_t* py = y + bi * 8 * n + bj * 8;
-    const int32_t* lp = err + bi * 8 * n + bj * 8;
-    double inv_sum = 0, texture = 0, energy = 0;
-    int lowest = INT_MAX;
-    for (int i = 0; i < 3; i++) {
-      for (int j = 0; j < 3; j++) {
-        const int vx = window_var(px + 2 * i * n + 2 * j, n);
-        const int vy = window_var(py + 2 * i * n + 2 * j, n);
-        if (vx < lowest) lowest = vx;
-        inv_sum += 1. / (1 + vx);
-        texture += vx - 2 * sqrt(vx * (double)vy) + vy;
-      }
-    }
-    const double stat = use_activity_masking ? 9. / inv_sum : (double)lowest;
-    const double activity = (use_activity_masking ? 1.95 : 1.62) * pow(.25 + stat / (1 << 2 * 4), -1. / 6);
-    for (int i = 0; i < 8; i++)
-      for (int j = 0; j < 8; j++) energy += lp[i * n + j] * (double)lp[i * n + j];
-    energy *= 0.92 / (7 * 7 * 7 * 7);
-    part[threadIdx.x] = activity * activity * (energy + texture);
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double total = 0;
-    for (int k = 0; k < nb * nb; k++) total += part[k];
-    out[blockIdx.x] = total * scale;
-  }
+  const size_t nn = (size_t)n * n;
+  const double d = block_dist(xs + blockIdx.x * nn, n, 0, ys + blockIdx.x * nn, n, 0, __ffs(n) - 1, 1, qm_is_flat,
+                              use_activity_masking, scale, smem);
+  if (threadIdx.x == 0) out[blockIdx.x] = d;
 }
 
 }  // namespace dist
@@ -118,16 +34,13 @@ extern "C" int daala_b200_compute_dist(const int32_t* x, const int32_t* y, int c
                                        int use_activity_masking, int coded_quantizer, double* out, void* stream) {
   if (count <= 0) return 0;
   if (n != 8 && n != 16 && n != 32 && n != 64) return (int)cudaErrorInvalidValue;
-  // src/encode.c:1221-1223: 1.7 below coded quantizer 36, 1.2 from 47, linear in between
-  const double scale = coded_quantizer >= 47 ? 1.2 : coded_quantizer <= 36 ? 1.7
-                       : 1.7 + (1.2 - 1.7) * (coded_quantizer - 36) / (47 - 36);
-  const size_t smem = sizeof(int32_t) * 2 * n * n + sizeof(double) * (n / 8) * (n / 8);
+  const size_t smem = daala_b200::dist::dist_scratch_bytes(n);
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(daala_b200::dist::k_compute_dist, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)smem);
     if (e != cudaSuccess) return (int)e;
   }
-  daala_b200::dist::k_compute_dist<<<count, 64, smem, (cudaStream_t)stream>>>(x, y, n, qm_is_flat, use_activity_masking,
-                                                                              scale, out);
+  daala_b200::dist::k_compute_dist<<<count, daala_b200::dist::kDistThreads, smem, (cudaStream_t)stream>>>(
+      x, y, n, qm_is_flat, use_activity_masking, daala_b200::dist::dist_scale(coded_quantizer), out);
   return (int)cudaGetLastError();
 }

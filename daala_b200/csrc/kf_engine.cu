@@ -21,7 +21,8 @@
 // forward transform); they take the same forward transform (no DC Haar pyramid on either side) and their
 // coefficients `md` are the reference vector of every band (pvq_theta with is_keyframe = 0).  Without an intra
 // predictor every (block, band) of every plane is dependency-free: luma and chroma both go through the three
-// phase kernels (k_pvq_split) and the persistent chain kernel is not launched.
+// phase kernels (k_pvq_split) and the persistent chain kernel is not launched.  config.late_skip adds the four
+// late-skip distortions of every block (late_skip.cu) after the finishing scatter of both stages.
 //
 // Nothing returns to the host between the H2D of the inputs and the D2H of the results; list sizes
 // live in device memory (`cnt`), every kernel is launched with a fixed grid and loops / pulls tickets
@@ -40,6 +41,7 @@
 
 #include "daala_b200.h"
 #include "dering_search.h"
+#include "late_skip.h"
 #include "mc_batch.h"
 #include "gen/coding_order.inc"
 #include "pvq_math.cuh"
@@ -1309,6 +1311,9 @@ struct Sym {
   daala_b200_kf_sym_dc* dc;        // [cap_blocks]
   const int32_t* qdc[2];
   const int32_t* dc_resid[2];
+  // with config.late_skip: the late-skip record of each slot, from the block-order records (else NULL)
+  daala_b200_kf_late_skip* late_skip;   // [cap_blocks]
+  const daala_b200_kf_late_skip* ls_block[2];
 };
 
 // Bytes the band's pulses take in the stream: the n - (itheta != -1) values pvq_encode_partition hands to
@@ -1477,7 +1482,8 @@ __global__ void __launch_bounds__(kTile) k_sym_offsets(const __grid_constant__ S
 }
 
 // One warp per slot: the block record, its band records and the pulses of its bands with K > 0.  kInter (symbol_stream
-// = 2): flip is 0 (P frames have no CfL; res_flip is never written) and the slot's DC record is written too.
+// = 2): flip is 0 (P frames have no CfL; res_flip is never written) and the slot's DC record is written too, and with
+// config.late_skip its late-skip record.
 template <bool kInter>
 __global__ void __launch_bounds__(256) k_sym_pack(const __grid_constant__ Sym S) {
   const int lane = threadIdx.x & 31;
@@ -1512,6 +1518,7 @@ __global__ void __launch_bounds__(256) k_sym_pack(const __grid_constant__ Sym S)
         d.qdc = S.qdc[ch][blk];
         d.dc_resid = S.dc_resid[ch][blk];
         S.dc[slot] = d;
+        if (S.late_skip) S.late_skip[slot] = S.ls_block[ch][blk];
       }
     }
     if (lane < nb) S.bands[o.x + lane] = r[lane];
@@ -1557,8 +1564,8 @@ __global__ void k_sym_index(const __grid_constant__ Sym S) {
 
 // Copy of the used part of each stream array into the caller's pinned host buffers (device-addressable):
 // the lengths are only known on the device.  Segment 0 index, 1 block records, 2 band records, 3 pulses, 4 DC records
-// (one per block record).
-constexpr int kSymSegs = 5;
+// and 5 late-skip records (one per block record each).
+constexpr int kSymSegs = 6;
 struct SymCopy {
   const uint8_t* src[kSymSegs];
   uint8_t* dst[kSymSegs];
@@ -1573,7 +1580,7 @@ __global__ void __launch_bounds__(256) k_sym_copy(const __grid_constant__ SymCop
   const long long nth = (long long)gridDim.x * blockDim.x;
   for (int seg = 0; seg < kSymSegs; seg++) {
     if (!C.dst[seg]) continue;
-    const long long want = seg == 0 ? C.index_bytes : C.tot[seg == 4 ? 0 : seg - 1] * C.unit[seg];
+    const long long want = seg == 0 ? C.index_bytes : C.tot[seg >= 4 ? 0 : seg - 1] * C.unit[seg];
     const long long len = want < C.cap[seg] ? want : C.cap[seg];
     const uint8_t* s = C.src[seg];
     uint8_t* d = C.dst[seg];
@@ -1713,6 +1720,11 @@ struct daala_b200_kf {
   int32_t* fin_stream_dc;
   int32_t* fin_form;
   Unstream unstream;
+  // cfg.late_skip: the unquantised coefficients (a copy of `coeffs` taken before the finishing scatter), the records
+  // per block of each list, and the parameters of the late-skip launches
+  int32_t* d_orig[3];
+  daala_b200_kf_late_skip* late_skip[2];
+  daala_b200_late_skip_batch lsb;
   std::vector<uint8_t> slot_filled;  // cfg.inter_mc, per pool slot: something has written a picture there
   bool have_step;                  // a step has been submitted; last_tot are its totals
   daala_b200_kf_totals last_tot;
@@ -2034,6 +2046,42 @@ static int kf_alloc(daala_b200_kf* kf) {
       }
     }
   }
+  if (kf->cfg.late_skip) {
+    daala_b200_late_skip_batch& B = kf->lsb;
+    memset(&B, 0, sizeof(B));
+    long long px = 0;
+    for (int p = 0; p < 3; p++) {
+      const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
+      KF_CHECK(dalloc(kf, &kf->d_orig[p], n));
+      px += (long long)n;
+      B.d_orig[p] = kf->d_orig[p];
+      B.d[p] = kf->coeffs[p];
+      B.md[p] = kf->pred_coeffs[p];
+      B.plane_pitch[p] = (long long)kf->plane_w[p] * kf->plane_h[p];
+      B.plane_stride[p] = kf->plane_w[p];
+    }
+    for (int c = 0; c < 2; c++) {
+      const Stage& S = c ? kf->chroma : kf->luma;
+      KF_CHECK(dalloc(kf, &kf->late_skip[c], (size_t)S.max_blocks));
+      B.blocks[c] = S.prm.blocks;
+      B.count[c] = L.cnt + S.n_blocks_at;
+      B.max_blocks[c] = S.max_blocks;
+      B.out[c] = kf->late_skip[c];
+    }
+    KF_CHECK(dalloc(kf, &B.cls_items, (size_t)daala_b200_late_skip_class_caps(px, B.cls_off, B.cls_cap)));
+    KF_CHECK(dalloc(kf, &B.cls_n, (size_t)4));
+    B.q0 = kf->luma.prm.q0;
+    memcpy(B.pvq_qm_q4, kf->cfg.pvq_qm_q4, sizeof(B.pvq_qm_q4));
+    B.qm_is_flat = kf->cfg.qm_is_flat;
+    B.use_activity_masking = kf->cfg.use_masking;
+    B.coded_quantizer = kf->cfg.coded_quantizer;
+    if (kf->cfg.symbol_stream == 2) {
+      Sym& Y = kf->sym;
+      KF_CHECK(dalloc(kf, &Y.late_skip, (size_t)Y.cap_blocks));
+      Y.ls_block[0] = kf->late_skip[0];
+      Y.ls_block[1] = kf->late_skip[1];
+    }
+  }
 
   daala_b200_frame& f = kf->frame;
   memset(&f, 0, sizeof(f));
@@ -2303,7 +2351,13 @@ static int kf_enqueue_step_inter(daala_b200_kf* kf, int phases) {
   if (phases & DAALA_B200_KF_FORWARD) {
     int rc = kf->cfg.inter_mc ? daala_b200_launch_mc_obmc(&kf->mc, wide, s) : 0;
     if (!rc) rc = daala_b200_launch_forward(&kf->frame, 3, s);
-    if (!rc) rc = daala_b200_launch_forward(&kf->frame_pred, 3, s);
+    if (rc) return rc;
+    // late_skip: the unquantised coefficients, before k_finish_scatter<true> overwrites them with the coded ones
+    for (int p = 0; kf->cfg.late_skip && p < 3; p++)
+      if (cudaMemcpyAsync(kf->d_orig[p], kf->coeffs[p], sizeof(int32_t) * kf->plane_w[p] * kf->plane_h[p] * kf->F,
+                          cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+        return (int)cudaGetLastError();
+    rc = daala_b200_launch_forward(&kf->frame_pred, 3, s);
     if (rc) return rc;
   }
   const bool core = (phases & DAALA_B200_KF_SEARCH_ONLY) != 0;
@@ -2312,6 +2366,10 @@ static int kf_enqueue_step_inter(daala_b200_kf* kf, int phases) {
     if (!core) k_gather<kGatherInter><<<wide, 256, 0, s>>>(*S);
     enqueue_split<false>(kf, *S, s);
     if (!core) k_finish_scatter<true><<<wide, 256, 0, s>>>(*S);
+  }
+  if (!core && (phases & DAALA_B200_KF_PVQ_CHROMA) && kf->cfg.late_skip) {
+    const int rc = daala_b200_late_skip_enqueue(&kf->lsb, kf->sms * 3, s);
+    if (rc) return rc;
   }
   if (!core && (phases & DAALA_B200_KF_PVQ_CHROMA) && kf->cfg.symbol_stream) enqueue_sym<true>(kf->sym, wide, s);
   if (phases & DAALA_B200_KF_INVERSE) {
@@ -2426,6 +2484,11 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
              "the Haar pyramid and has no scalar index)");
     return nullptr;
   }
+  if (cfg && cfg->late_skip && (cfg->late_skip != 1 || cfg->inter != 1)) {
+    snprintf(g_create_err, sizeof(g_create_err),
+             "daala_b200_kf_create: late_skip is 0 or 1, and 1 requires inter = 1 (keyframes have no late skip)");
+    return nullptr;
+  }
   if (cfg && cfg->mc_refs < 0) {
     snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: mc_refs < 0");
     return nullptr;
@@ -2528,10 +2591,10 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   auto split = [](const Stage& S) { return 3 * (S.sp_chunks[0] + S.sp_chunks[1] + S.sp_chunks[2]); };
   // inter: work lists, two forward launches, per stage gather + phase kernels + finish, inverse + SB postfilter;
   // inter_mc: leaf enumeration and OBMC
-  // [symbol_stream = 2: the 8 stream kernels]
+  // [symbol_stream = 2: the 8 stream kernels]; [late_skip: the size-class split and one launch per class]
   if (kf->cfg.inter)
     return 5 + 2 + (2 + split(kf->luma)) + (2 + split(kf->chroma)) + 2 + (kf->cfg.inter_mc ? 2 : 0) +
-           (kf->cfg.symbol_stream ? 8 : 0);
+           (kf->cfg.symbol_stream ? 8 : 0) + (kf->cfg.late_skip ? kLateSkipLaunches : 0);
   int n = 5 + (kf->cfg.level_chains ? 2 : 0);                                    // work lists
   n += 1;                                                                         // forward
   n += 3 + 1 + (kf->cfg.split_free > 1 ? split(kf->luma) : 0) + (kf->luma.pre_ev ? 2 : 0);   // luma: begin, gather, [prepass], chains, finish
@@ -2750,10 +2813,21 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
       return (int)cudaErrorInvalidValue;
     }
   }
+  // late-skip records: only an engine with late_skip has them, and only a symbol_stream = 2 engine in stream order
+  const char* ls_why = (io->luma_late_skip || io->chroma_late_skip || io->sym_late_skip) && !kf->cfg.late_skip
+                           ? "luma_late_skip / chroma_late_skip / sym_late_skip need an engine with late_skip = 1"
+                       : io->sym_late_skip && kf->cfg.symbol_stream != 2
+                           ? "sym_late_skip needs an engine with symbol_stream = 2"
+                           : nullptr;
+  if (ls_why) {
+    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", ls_why);
+    return (int)cudaErrorInvalidValue;
+  }
   // symbol stream: the engine must produce it, and every requested buffer must hold the worst case and be pinned
   SymCopy sc;
   memset(&sc, 0, sizeof(sc));
-  const bool want_sym = io->sym_index || io->sym_blocks || io->sym_bands || io->sym_pulses || io->sym_dc;
+  const bool want_sym = io->sym_index || io->sym_blocks || io->sym_bands || io->sym_pulses || io->sym_dc ||
+                        io->sym_late_skip;
   if (want_sym) {
     if (!kf->cfg.symbol_stream) return (int)cudaErrorInvalidValue;
     if (io->sym_dc && kf->cfg.symbol_stream != 2) {
@@ -2768,25 +2842,35 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     if (!e) e = sym_target(io->sym_pulses, io->sym_pulses_cap, bd.pulse_bytes, &sc.dst[3]);
     if (!e) e = sym_target(io->sym_dc, io->sym_dc_cap, bd.blocks, &sc.dst[4]);
     if (e) return e;
+    if (sym_target(io->sym_late_skip, io->sym_late_skip_cap, bd.blocks, &sc.dst[5])) {
+      snprintf(kf->err, sizeof(kf->err),
+               "daala_b200_kf_submit: sym_late_skip must be pinned host memory of at least "
+               "daala_b200_kf_symbol_bounds(...).blocks records");
+      return (int)cudaErrorInvalidValue;
+    }
     const Sym& Y = kf->sym;
     sc.src[0] = (const uint8_t*)Y.index;
     sc.src[1] = (const uint8_t*)Y.blocks;
     sc.src[2] = (const uint8_t*)Y.bands;
     sc.src[3] = Y.pulses;
     sc.src[4] = (const uint8_t*)Y.dc;
+    sc.src[5] = (const uint8_t*)Y.late_skip;
     sc.unit[1] = sizeof(daala_b200_kf_sym_block);
     sc.unit[2] = 4 * sizeof(int16_t);
     sc.unit[3] = 1;
     sc.unit[4] = sizeof(daala_b200_kf_sym_dc);
+    sc.unit[5] = sizeof(daala_b200_kf_late_skip);
     sc.index_bytes = (long long)F * sizeof(daala_b200_kf_sym_frame);
     sc.tot = Y.tot;
     const long long host[kSymSegs] = {io->sym_index_cap * (long long)sizeof(daala_b200_kf_sym_frame),
                                       io->sym_blocks_cap * (long long)sizeof(daala_b200_kf_sym_block),
                                       io->sym_bands_cap * 8, io->sym_pulses_cap,
-                                      io->sym_dc_cap * (long long)sizeof(daala_b200_kf_sym_dc)};
+                                      io->sym_dc_cap * (long long)sizeof(daala_b200_kf_sym_dc),
+                                      io->sym_late_skip_cap * (long long)sizeof(daala_b200_kf_late_skip)};
     const long long dev[kSymSegs] = {sc.index_bytes, (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_block),
                                      Y.cap_bands * 8, Y.cap_bytes,
-                                     Y.dc ? (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_dc) : 0};
+                                     Y.dc ? (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_dc) : 0,
+                                     Y.late_skip ? (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_late_skip) : 0};
     for (int i = 0; i < kSymSegs; i++) sc.cap[i] = host[i] < dev[i] ? host[i] : dev[i];
   }
   for (int p = 0; p < 3; p++) {
@@ -2850,6 +2934,12 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     KF_CHECK(cudaMemcpyAsync(io->luma_dc_resid, kf->dc_resid[0], 4 * (size_t)tot.n_luma, cudaMemcpyDeviceToHost, s));
   if (kf->dc_resid[1] && io->chroma_dc_resid)
     KF_CHECK(cudaMemcpyAsync(io->chroma_dc_resid, kf->dc_resid[1], 4 * (size_t)tot.n_chroma, cudaMemcpyDeviceToHost, s));
+  if (io->luma_late_skip)
+    KF_CHECK(cudaMemcpyAsync(io->luma_late_skip, kf->late_skip[0], sizeof(daala_b200_kf_late_skip) * tot.n_luma,
+                             cudaMemcpyDeviceToHost, s));
+  if (io->chroma_late_skip)
+    KF_CHECK(cudaMemcpyAsync(io->chroma_late_skip, kf->late_skip[1], sizeof(daala_b200_kf_late_skip) * tot.n_chroma,
+                             cudaMemcpyDeviceToHost, s));
   if (io->counts) KF_CHECK(cudaMemcpyAsync(io->counts, kf->lists.cnt, sizeof(int32_t) * 32, cudaMemcpyDeviceToHost, s));
   if (io->dering_level_out && kf->cfg.dering)
     KF_CHECK(cudaMemcpyAsync(io->dering_level_out, kf->dering.level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyDeviceToHost, s));

@@ -15,6 +15,9 @@ frame's reconstruction into a pool slot on the device, `encode(..., resident=Tru
 and `pool_load` seeds a slot from host memory or from another engine's device buffer (a GOP's keyframe).
 With inter=1 and symbol_stream=2 each step also returns the P-frame symbol stream (the stream of symbol_stream=1 with a
 DC record per block: qdc and the unquantised residual), and `finish_stream` takes the decisions back in that order.
+With inter=1 and late_skip=1 each step also returns the four late-skip distortions of every block
+(symbols.LATE_SKIP_DTYPE; `luma_late_skip` / `chroma_late_skip`, and `sym_late_skip` in stream order), from which the
+host coder takes the reference's late-skip decision (daala_b200/lateskip.py).
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -39,7 +42,7 @@ class Config(ctypes.Structure):
                 ("max_blocks_div", c_int), ("persist_ctas_per_sm", c_int), ("split_free", c_int), ("dering", c_int), ("noref_prepass", c_int), ("level_chains", c_int), ("stream", c_void_p),
                 ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
                 ("symbol_stream", c_int), ("inter", c_int), ("inter_mc", c_int), ("mc_refs", c_int),
-                ("inter_finish", c_int)]
+                ("inter_finish", c_int), ("late_skip", c_int)]
 
 
 class Totals(ctypes.Structure):
@@ -57,7 +60,9 @@ class IO(ctypes.Structure):
                 ("pred_pixels", c_void_p * 3), ("luma_dc", c_void_p), ("chroma_dc", c_void_p),
                 ("ref_pixels", c_void_p * 3), ("nrefs", c_int), ("ref_slot", c_void_p), ("mv_grid", c_void_p),
                 ("pred_pixels_out", c_void_p * 3), ("luma_dc_resid", c_void_p), ("chroma_dc_resid", c_void_p),
-                ("ref_resident", c_int), ("sym_dc", c_void_p), ("sym_dc_cap", c_ll)]
+                ("ref_resident", c_int), ("sym_dc", c_void_p), ("sym_dc_cap", c_ll),
+                ("luma_late_skip", c_void_p), ("chroma_late_skip", c_void_p), ("sym_late_skip", c_void_p),
+                ("sym_late_skip_cap", c_ll)]
 
 
 class FinishIO(ctypes.Structure):
@@ -141,7 +146,7 @@ class KeyframeEngine:
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
                  qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=0, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
                  qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0, inter_mc=0, mc_refs=0,
-                 inter_finish=0):
+                 inter_finish=0, late_skip=0):
         self.L = _bind()
         self.geom, self.F = geom, nframes
         if qm is None:
@@ -178,6 +183,9 @@ class KeyframeEngine:
         self.inter_mc = int(inter_mc)
         cfg.inter_finish = int(inter_finish)
         self.inter_finish = int(inter_finish)
+        # late_skip: od_compute_dist with coded_quantizer, qm_is_flat and use_masking above
+        cfg.late_skip = int(late_skip)
+        self.late_skip = int(late_skip)
         self.nrefs = 0
         self.resident = False
         self._pool_src = []
@@ -310,7 +318,9 @@ class KeyframeEngine:
         """Builds the daala_b200_kf_io record over the staged inputs and result buffers sized for them.
         stream (default: whether the engine was created with symbol_stream) adds the symbol stream buffers
         sym_index, sym_blocks, sym_bands and sym_pulses (daala_b200/symbols.py), and sym_dc on a symbol_stream=2
-        engine, pinned and sized by daala_b200_kf_symbol_bounds; only their used part is copied back.  On a
+        engine (and sym_late_skip on one with late_skip too), pinned and sized by daala_b200_kf_symbol_bounds; only
+        their used part is copied back.  late_skip engines return luma_late_skip / chroma_late_skip
+        (symbols.LATE_SKIP_DTYPE per block, block order) with the symbols.  On a
         symbol_stream=2 engine symbols=False also leaves out the classic DC arrays (the stream carries them).
         pred=False (inter_mc engines): the prediction planes are not copied back."""
         g, t = self.geom, self.totals
@@ -340,6 +350,11 @@ class KeyframeEngine:
             for k in ("luma_blocks", "chroma_blocks", "luma_res", "chroma_res", "luma_y16", "chroma_y16",
                       "luma_skip_diff", "chroma_skip_diff", "chroma_flip"):
                 setattr(io, k, out[k].ctypes.data)
+            if self.late_skip:
+                from . import symbols as sym
+                out["luma_late_skip"] = self._arr("lls", (nl,), sym.LATE_SKIP_DTYPE)
+                out["chroma_late_skip"] = self._arr("cls", (nc,), sym.LATE_SKIP_DTYPE)
+                io.luma_late_skip, io.chroma_late_skip = out["luma_late_skip"].ctypes.data, out["chroma_late_skip"].ctypes.data
         if self.inter_mc:
             io.ref_resident = int(self.resident)
             for p in range(3):
@@ -384,6 +399,9 @@ class KeyframeEngine:
             if self.symbol_stream == 2:
                 out["sym_dc"] = self._arr("sd", (int(b.blocks),), sym.DC_DTYPE, pinned=True)
                 io.sym_dc, io.sym_dc_cap = out["sym_dc"].ctypes.data, int(b.blocks)
+                if self.late_skip:
+                    out["sym_late_skip"] = self._arr("sls", (int(b.blocks),), sym.LATE_SKIP_DTYPE, pinned=True)
+                    io.sym_late_skip, io.sym_late_skip_cap = out["sym_late_skip"].ctypes.data, int(b.blocks)
         self._io, self._out = io, out
         px = sum(int(np.prod(g.plane_shape(p))) for p in range(3))
         self.h2d_bytes = px * self.F * (2 if self.inter and not self.inter_mc else 1) + int(np.prod(g.bsize_shape)) * self.F
@@ -402,11 +420,13 @@ class KeyframeEngine:
 
     def stream_d2h_bytes(self):
         """Bytes the last submit copied of the symbol stream (after wait): the index and the used part of the
-        other arrays (block records, band records, pulses and, on symbol_stream=2 engines, DC records)."""
+        other arrays (block records, band records, pulses and, on symbol_stream=2 engines, DC records and, with
+        late_skip, late-skip records)."""
         from . import symbols as sym
         idx = self._out["sym_index"]
         blocks = int(idx[:, 1].sum())
         dc = blocks * sym.DC_DTYPE.itemsize if "sym_dc" in self._out else 0
+        dc += blocks * sym.LATE_SKIP_DTYPE.itemsize if "sym_late_skip" in self._out else 0
         return idx.nbytes + blocks * sym.BLOCK_DTYPE.itemsize + int(idx[:, 3].sum()) * 8 + int(idx[:, 5].sum()) + dc
 
     def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None, pred=None, refs=None,

@@ -1,7 +1,7 @@
 """The keyframe engine's symbol stream (include/daala_b200.h, "Symbol stream"; config.symbol_stream = 1): per
 frame the PVQ symbols the serial entropy coder reads, in bitstream order.  The P-frame stream (symbol_stream = 2,
 inter = 1) is the same with flip = 0 and a DC_DTYPE record per block record (sym_dc, same index): the step's scalar
-DC index and the unquantised DC residual.
+DC index and the unquantised DC residual; with late_skip = 1 also a LATE_SKIP_DTYPE record (sym_late_skip).
 
 For each frame of a batch the index (int64[6]: first block, block count, first band, band count, first pulse
 byte, pulse byte count) locates three parts inside batch-wide arrays:
@@ -26,6 +26,10 @@ BAND_EDGES = np.array([1, 16, 24, 32, 64, 96, 128, 256, 384, 512])   # OD_BAND_O
 ORDER_DTYPE = np.dtype([("pli", "u1"), ("x0", "<u2"), ("y0", "<u2"), ("bs", "u1")])
 DC_DTYPE = np.dtype([("qdc", "<i4"), ("dc_resid", "<i4")])
 assert DC_DTYPE.itemsize == 8
+# config.late_skip: daala_b200_kf_late_skip, one per block (block order) or per block record (sym_late_skip)
+LATE_SKIP_DTYPE = np.dtype([("dist_skip", "<f8"), ("noskip_coded_dc0", "<f8"), ("noskip_coded_dcq", "<f8"),
+                            ("noskip_pred_dcq", "<f8")])
+assert LATE_SKIP_DTYPE.itemsize == 32
 
 
 def _excl(a):

@@ -512,6 +512,12 @@ typedef struct daala_b200_kf_config {
                                   taking them (src/encode.c:2708-2811 for a P frame, see daala_b200_kf_finish_io);
                                   needs coded_quantizer / qm_is_flat / dering_lambda above.
                                   1 and 2 require inter = 1; refused by daala_b200_kf_create otherwise */
+  int late_skip;               /* 0 (default): nothing below exists; the engine is exactly the one without this field.
+                                  1: each step also computes the late-skip distortions of every block
+                                  (daala_b200_kf_late_skip below, returned through daala_b200_kf_io.luma_late_skip /
+                                  chroma_late_skip / sym_late_skip), with coded_quantizer, qm_is_flat and use_masking
+                                  (enc->use_activity_masking) above.  Requires inter = 1; other values, and 1 without
+                                  inter, are refused by daala_b200_kf_create */
 } daala_b200_kf_config;
 
 /* One vertex of a P frame's MV grid, as od_mv_grid_pt (reference src/mc.h:73-84) holds it after od_mv_est. */
@@ -556,6 +562,33 @@ typedef struct daala_b200_kf_sym_dc {      /* 8 bytes */
   int32_t dc_resid;        /* the unquantised DC residual in[0] - ref[0] (as daala_b200_kf_io.*_dc_resid), what the
                               host's od_rdo_quant quantises (src/pvq_encoder.c:886 / :956) */
 } daala_b200_kf_sym_dc;
+
+/* config.late_skip = 1: the four distortions od_block_encode's late skip (reference src/encode.c:1412-1450) can ask
+   for, one record per block.  All are od_compute_dist(c_orig, c, n) of src/encode.c:1180 (coded_quantizer, qm_is_flat,
+   use_masking of the config), n = 4 << bs with the plane-local bs.  c_orig is the block's samples after the SB-edge
+   and split prefilters (`c` at src/encode.c:1283), mc_orig the same for the prediction; every other c is the leaf
+   iDCT (no postfilter, the c_noskip of :1420-1423) of a candidate coefficient block:
+     dist_skip          d = md, the late skip (:1444-1448); its reconstruction is mc_orig itself;
+     noskip_coded_dc0   AC as the step coded it (its `d`, with md as the uncoded tail of 32x32 / 64x64 blocks),
+                        d[0] = md[0];
+     noskip_coded_dcq   the same AC, d[0] = md[0] + q1 * dc_quant;
+     noskip_pred_dcq    AC = md (the PVQ skip, src/pvq_encoder.c:975), d[0] = md[0] + q1 * dc_quant;
+   dc_quant = max(1, q0 * pvq_qm_q4[pli][bs * (bs + 1)] >> 4) is the step's band-0 quantiser and
+   q1 = OD_DIV_R0(dc_resid, dc_quant), dc_resid = in[0] - ref[0] (daala_b200_kf_sym_dc.dc_resid).
+   Why these four: od_rdo_quant (src/pvq_encoder.c:730-741) returns 0 or q1 whatever the coder's DC rate, and the AC
+   is either coded or md.  Of the four (AC, DC) pairs, (md, 0) is od_pvq_encode's own skip (no late-skip test; its
+   distortion is dist_skip); the other three are the dist_noskip candidates.  The host coder picks the record field
+   of its (pvq_skip, dc) pair -- (0, 0) noskip_coded_dc0, (0, q1) noskip_coded_dcq, (1, q1) noskip_pred_dcq -- and runs
+   the reference's test (:1431) with its own rates and enc->bs_rdo_lambda:
+     late skip  <=>  dist_skip + lambda * rate_skip < dist_noskip + lambda * rate_noskip
+   then, when it wins, hands skip = 1, dc = 0 for the block to daala_b200_kf_finish.  Blocks with bs = 0 (4x4 luma
+   and 4x4 chroma) have no late skip (has_late_skip_rdo, :1280) and an all-zero record. */
+typedef struct daala_b200_kf_late_skip {   /* 32 bytes */
+  double dist_skip;         /* od_compute_dist(c_orig, mc_orig, n) */
+  double noskip_coded_dc0;  /* od_compute_dist(c_orig, idct(coded AC, d[0] = md[0]), n) */
+  double noskip_coded_dcq;  /* ... coded AC, d[0] = md[0] + q1 * dc_quant */
+  double noskip_pred_dcq;   /* ... AC = md (PVQ skip), d[0] = md[0] + q1 * dc_quant */
+} daala_b200_kf_late_skip;
 
 typedef struct daala_b200_kf_sym_frame {   /* one frame's part of the batch-wide arrays (indices, not bytes, */
   int64_t first_block, n_blocks;           /* except for the pulses) */
@@ -628,6 +661,14 @@ typedef struct daala_b200_kf_io {
      copied, as for the other stream arrays. */
   daala_b200_kf_sym_dc *sym_dc;
   long long sym_dc_cap;
+  /* config.late_skip = 1 only (optional, NULL = not copied): the late-skip records (daala_b200_kf_late_skip) in the
+     block order of luma_res / chroma_res ([n_blocks] each) ... */
+  daala_b200_kf_late_skip *luma_late_skip, *chroma_late_skip;
+  /* ... and, with symbol_stream = 2, in stream order: one record per block record at the same index as sym_blocks, a
+     pinned host buffer with its capacity in records, at least daala_b200_kf_symbol_bounds(...).blocks.  Only the used
+     part is copied, as for sym_dc. */
+  daala_b200_kf_late_skip *sym_late_skip;
+  long long sym_late_skip_cap;
 } daala_b200_kf_io;
 
 /* The finishing pass of a P-frame batch (config.inter_finish), daala_b200_kf_finish: the host coder's per-block
@@ -743,7 +784,8 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    anything is copied or launched; so does a request for symbol stream outputs from an engine created without
    symbol_stream (sym_dc: without symbol_stream = 2), a stream capacity below daala_b200_kf_symbol_bounds, a stream
    buffer that is not pinned host memory, or (config.inter) a NULL pred_pixels plane, luma_dc or chroma_dc (the last
-   two are optional with symbol_stream = 2).  With config.inter_mc it refuses, the same
+   two are optional with symbol_stream = 2), a late-skip output on an engine without late_skip, and sym_late_skip
+   without symbol_stream = 2 (each with a message in daala_b200_kf_error).  With config.inter_mc it refuses, the same
    way, a NULL mv_grid, ref_pixels plane or ref_slot, pred_pixels given, nrefs outside [1, mc_refs] and a slot outside
    [0, nrefs); with ref_resident = 1 it refuses instead ref_pixels given, nrefs other than 0, a slot outside
    [0, mc_refs) and a slot that holds no picture.  The step counts in `counts` the leaf corners whose vertex has a ref other than 0 or 1 (counts[19]) and
