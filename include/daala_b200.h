@@ -684,7 +684,11 @@ typedef struct daala_b200_kf_io {
    levels: a superblock none of whose 4x4 luma units is coded is forced to level 0 (:2724-2738), chroma thresholds
    are x0.6, od_dering reads the real skip map (src/dering.c:297-325).  |dc| must not exceed
    DAALA_B200_KF_FINISH_DC_LIMIT / DQ, DQ the largest dc_quant of the engine over planes and block sizes, so that
-   dc * dc_quant stays within 2^30 and md[0] + dc * dc_quant within od_coeff.
+   dc * dc_quant stays within 2^30 and md[0] + dc * dc_quant within od_coeff.  The pass equals the reference bit for
+   bit while every sample of the reconstruction before deringing (state->ctmp, after the superblock-edge postfilter)
+   fits int16, as it always does for 8-bit content with decisions near the step's own DC indices: the pass keeps that
+   plane only as the int16 deringing input (state->etmp, src/encode.c:2703-2705), so beyond it a superblock at level 0,
+   and the level search's unfiltered candidate, see the int16 truncation where the reference keeps od_coeff.
    config.inter_finish = 2: the pass searches the levels itself, between the superblock-edge postfilter and the
    deringing, as the keyframe search of config.dering = 2 with the three rules of a P frame: every filtered candidate
    reads the frame's own luma skip map; a superblock with no coded 4x4 luma unit is not searched, gets level 0 and does

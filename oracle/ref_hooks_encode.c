@@ -189,3 +189,72 @@ int oracle_ref_dering_search(unsigned char *src, int src_stride, const od_coeff 
   free(enc);
   return 0;
 }
+
+/* The quantizer settings the reference encoder itself uses for a keyframe followed by one P frame, through the
+   public API: OD_SET_QUANT = quant, OD_SET_ACTIVITY_MASKING = masking, OD_SET_QM = qm (OD_FLAT_QM / OD_HVS_QM), on a
+   mid-grey w x h picture (rate control is off, so nothing here depends on the content).  After each frame is
+   coded, f = 0 (keyframe) / 1 (P frame), it reads back from the encoder context: quantizer[f] and
+   coded_quantizer[f] (state.quantizer / coded_quantizer), pvq_qm_q4[f][3][OD_QM_SIZE], qm_out[f] / qm_inv_out[f]
+   ([OD_QM_BUFFER_SIZE] each), pvq_norm_lambda[f] and dering_lambda[f]. */
+int oracle_ref_encoder_settings(int w, int h, int quant, int masking, int qm, int *quantizer, int *coded_quantizer,
+ unsigned char *pvq_qm_q4, int16_t *qm_out, int16_t *qm_inv_out, double *pvq_norm_lambda, double *dering_lambda) {
+  daala_info info;
+  daala_enc_ctx *enc;
+  daala_image img;
+  daala_packet op;
+  unsigned char *planes[3];
+  int pli;
+  int f;
+  int ret;
+  daala_info_init(&info);
+  info.pic_width = w;
+  info.pic_height = h;
+  info.timebase_numerator = 30;
+  info.timebase_denominator = 1;
+  info.frame_duration = 1;
+  info.pixel_aspect_numerator = 1;
+  info.pixel_aspect_denominator = 1;
+  info.nplanes = 3;
+  info.plane_info[0].xdec = info.plane_info[0].ydec = 0;
+  info.plane_info[1].xdec = info.plane_info[1].ydec = 1;
+  info.plane_info[2].xdec = info.plane_info[2].ydec = 1;
+  info.keyframe_rate = 256;
+  enc = daala_encode_create(&info);
+  if (enc == NULL) return -1;
+  if (daala_encode_ctl(enc, OD_SET_QUANT, &quant, sizeof(quant)) != OD_SUCCESS
+   || daala_encode_ctl(enc, OD_SET_ACTIVITY_MASKING, &masking, sizeof(masking)) != OD_SUCCESS
+   || daala_encode_ctl(enc, OD_SET_QM, &qm, sizeof(qm)) != OD_SUCCESS) {
+    daala_encode_free(enc);
+    return -2;
+  }
+  img.nplanes = 3;
+  img.width = w;
+  img.height = h;
+  ret = 0;
+  for (pli = 0; pli < 3; pli++) {
+    planes[pli] = (unsigned char *)malloc((size_t)w*h);
+    memset(planes[pli], 128, (size_t)w*h);
+    img.planes[pli].data = planes[pli];
+    img.planes[pli].xdec = img.planes[pli].ydec = pli > 0;
+    img.planes[pli].xstride = 1;
+    img.planes[pli].ystride = pli == 0 ? w : (w + 1) >> 1;
+    img.planes[pli].bitdepth = 8;
+  }
+  for (f = 0; f < 2 && ret == 0; f++) {
+    if (daala_encode_img_in(enc, &img, 1) < 0) ret = -3;
+    else if (daala_encode_packet_out(enc, f == 1, &op) <= 0) ret = -4;
+    else if ((f == 0) != (enc->state.frame_type == OD_I_FRAME)) ret = -5;
+    else {
+      quantizer[f] = enc->state.quantizer;
+      coded_quantizer[f] = enc->state.coded_quantizer;
+      memcpy(pvq_qm_q4 + f*3*OD_QM_SIZE, enc->state.pvq_qm_q4, 3*OD_QM_SIZE);
+      memcpy(qm_out + f*OD_QM_BUFFER_SIZE, enc->state.qm, sizeof(*qm_out)*OD_QM_BUFFER_SIZE);
+      memcpy(qm_inv_out + f*OD_QM_BUFFER_SIZE, enc->state.qm_inv, sizeof(*qm_inv_out)*OD_QM_BUFFER_SIZE);
+      pvq_norm_lambda[f] = enc->pvq_norm_lambda;
+      dering_lambda[f] = enc->dering_lambda;
+    }
+  }
+  for (pli = 0; pli < 3; pli++) free(planes[pli]);
+  daala_encode_free(enc);
+  return ret;
+}

@@ -3,7 +3,8 @@
 from the reference sources by oracle/Makefile) on seeded inputs.  The reference ships no golden vectors
 (SURVEY.md 4 / 8(c)); these are ours, so that the plain-C port (and through it the CUDA path) stays
 pinned where oracle/_ref cannot be rebuilt.  Run from the repo root:  python tests/golden/make_golden.py
-(`... make_golden.py digests` writes tests/golden/reference_digests.npz instead).
+(`... make_golden.py digests` writes tests/golden/reference_digests.npz instead, `... make_golden.py settings`
+tests/golden/encoder_settings.npz).
 
 Inputs are stored next to the outputs (not regenerated from seeds), except for whole planes, which are
 rebuilt by daala_b200.synth (deterministic integer generator) and stored as CRC-32 of the reference output.
@@ -236,12 +237,15 @@ def main():
     print("wrote %s (%d arrays, %d bytes)" % (path, len(g), os.path.getsize(path)))
 
 
-THETA_SETS = [("seed%d" % s, dict(seed=s, per_combo=3)) for s in (1, 2, 3, 4, 5)] + [("large_k", None)]
+THETA_SETS = ([("seed%d" % s, dict(seed=s, per_combo=3)) for s in (1, 2, 3, 4, 5)] + [("large_k", None)] +
+              [("quantizer_range", "quantizer_range")])
 
 
 def theta_case_set(name):
     """The pvq_theta cases of tests/test_emu_pvq_warp.py recorded under `name`."""
     kw = dict(THETA_SETS)[name]
+    if kw == "quantizer_range":
+        return pvq_cases.quantizer_range_cases()
     return pvq_cases.large_k_cases() if kw is None else pvq_cases.cases(**kw)
 
 
@@ -299,5 +303,63 @@ def main_digests():
     print("wrote %s (%d arrays, %d bytes)" % (path, len(g), os.path.getsize(path)))
 
 
+# The encoder's quantizer setting (OD_SET_QUANT) at each sweep point of tests/test_gpu_engine_quantizer_range.py.  The
+# keyframe gets a finer coded quantizer than the P frame that follows it (src/rate.c:765-835): 1 is the finest setting
+# (keyframe 4, P frame 6), 435 the first whose keyframe reaches 60 and P frame 63, the coarsest coded quantizer; 49's
+# frames (40, 44) lie in od_compute_dist's interpolated range, coded quantizers 36..47.
+SETTINGS_QUANT = (1, 5, 12, 18, 28, 49, 162, 435)
+# (use_activity_masking, qm): OD_HVS_QM = 1 with and without masking, OD_FLAT_QM = 0 with masking
+SETTINGS_CONFIGS = ((1, 1), (0, 1), (1, 0))
+SETTINGS_PIC = (64, 64)
+
+
+def capture_settings(ref, quant, masking, qm):
+    """oracle_ref_encoder_settings: what the encoder set for its keyframe (index 0) and the P frame after it (1)."""
+    S = 2 * pvq_cases.OD_QM_STRIDE
+    out = dict(quantizer=np.zeros(2, np.int32), coded_quantizer=np.zeros(2, np.int32),
+               pvq_qm_q4=np.zeros((2, 3, 30), np.uint8), qm=np.zeros((2, S), np.int16), qm_inv=np.zeros((2, S), np.int16),
+               pvq_norm_lambda=np.zeros(2), dering_lambda=np.zeros(2))
+    rc = ref.oracle_ref_encoder_settings(SETTINGS_PIC[0], SETTINGS_PIC[1], int(quant), int(masking), int(qm),
+                                         *[addr(out[k]) for k in ("quantizer", "coded_quantizer", "pvq_qm_q4", "qm",
+                                                                  "qm_inv", "pvq_norm_lambda", "dering_lambda")])
+    assert rc == 0, rc
+    # od_init_qm (src/pvq.c:322) writes only part of the state's buffers; the rest is whatever the allocator left there
+    written = pvq_cases.reference_qm(ref, hvs=bool(qm))[0] != 0
+    out["qm"][:, ~written] = 0
+    out["qm_inv"][:, ~written] = 0
+    return out
+
+
+def main_settings():
+    """tests/golden/encoder_settings.npz: capture_settings at every SETTINGS_QUANT x SETTINGS_CONFIGS point, arrays
+    [point][config][frame]...; the matrices, which depend on qm alone, once per kind (qm_hvs / qm_flat)."""
+    ref = oracle_lib.load_ref()
+    assert ref is not None, "needs oracle/_ref (make -C oracle ref, with the reference sources present)"
+    keys = ("quantizer", "coded_quantizer", "pvq_qm_q4", "pvq_norm_lambda", "dering_lambda")
+    g = {k: [] for k in keys}
+    mats = {}
+    for quant in SETTINGS_QUANT:
+        rows = {k: [] for k in keys}
+        for masking, qm in SETTINGS_CONFIGS:
+            s = capture_settings(ref, quant, masking, qm)
+            name = "hvs" if qm else "flat"
+            for m in ("qm", "qm_inv"):
+                assert np.array_equal(s[m][0], s[m][1])
+                mats.setdefault(m + "_" + name, s[m][0])
+                assert np.array_equal(mats[m + "_" + name], s[m][0])
+            for k in keys:
+                rows[k].append(s[k])
+        for k in keys:
+            g[k].append(np.stack(rows[k]))
+    g = {k: np.stack(v) for k, v in g.items()}
+    g.update(mats)
+    g["quant"] = np.array(SETTINGS_QUANT, np.int32)
+    g["configs"] = np.array(SETTINGS_CONFIGS, np.int32)
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "encoder_settings.npz")
+    np.savez_compressed(path, **g)
+    print("wrote %s (%d arrays, %d bytes)" % (path, len(g), os.path.getsize(path)))
+
+
 if __name__ == "__main__":
-    main_digests() if sys.argv[1:] == ["digests"] else main()
+    mode = sys.argv[1:]
+    main_digests() if mode == ["digests"] else main_settings() if mode == ["settings"] else main()

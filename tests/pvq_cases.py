@@ -100,6 +100,31 @@ def large_k_cases():
                 yield dict(n=n, kind="big", is_keyframe=kf, pli=pli, beta=4096, q0=q0, x0=x0, r0=r0, qm_off=5, lam=0.147)
 
 
+QUANTIZER_RANGE_Q = (1101, 2190, 4728, 8191, 18430, 36000, 65535, 130521)
+
+
+def quantizer_range_cases(seed=11):
+    """Band quantisers from just above cases()' largest up to 130521 = 8191 * 255 >> 4 (the coarsest coded quantizer
+    times the largest pvq_qm_q4 entry), every kind, size and (keyframe, plane, beta) combination.  Each vector is
+    scaled so that its gain is 0.5 to 40 quantisers: K from 0 to about 200."""
+    rng = np.random.default_rng(seed)
+    kinds = ["pred", "weak", "zero_ref", "zero_x", "big", "tiny", "sparse"]
+    for n in (15, 8, 32, 128):
+        for kind in kinds:
+            for is_keyframe, pli in ((1, 0), (1, 1), (0, 0), (0, 2)):
+                for beta in (4096, 6144):
+                    if beta == 6144 and (pli != 0 or n == 15):
+                        continue
+                    for q0 in QUANTIZER_RANGE_Q:
+                        x0, r0 = make_band(rng, n, kind)
+                        norm = max(1.0, float(np.sqrt(np.sum(x0.astype(np.float64) ** 2))),
+                                   float(np.sqrt(np.sum(r0.astype(np.float64) ** 2))))
+                        s = q0 * rng.uniform(0.5, 40.0) / norm
+                        yield dict(n=n, kind=kind, is_keyframe=is_keyframe, pli=pli, beta=beta, q0=q0,
+                                   x0=np.round(x0 * s).astype(np.int32), r0=np.round(r0 * s).astype(np.int32),
+                                   qm_off=int(rng.integers(1, 64)), lam=float(rng.choice([0.147, 0.05, 0.3])))
+
+
 def digest(r):
     """[gain, itheta, max_theta, K, CRC-32 of the pulses and the synthesised band] of a run_theta result."""
     vec = np.ascontiguousarray(r["y"], np.int32).tobytes() + np.ascontiguousarray(r["out"], np.int32).tobytes()

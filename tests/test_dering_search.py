@@ -38,13 +38,14 @@ def synth_pair(rng, nhsb, nvsb, ring):
     return np.ascontiguousarray(src), np.ascontiguousarray(ctmp)
 
 
-def ref_search(ref, src, ctmp, nhsb, nvsb, q, masking, keyframe, lam, bskip, cdf, increment=128, qm=1):
+def ref_search(ref, src, ctmp, nhsb, nvsb, q, masking, keyframe, lam, bskip, cdf, increment=128, qm=1, coded_quantizer=None):
     nsb = nhsb * nvsb
     levels = np.zeros(nsb, np.uint8)
     dist = np.zeros((LEVELS, nsb), np.float64)
     ref.oracle_ref_dering_search.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p] + [ctypes.c_int] * 7 + [
         ctypes.c_double, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
-    r = ref.oracle_ref_dering_search(addr(src), src.shape[1], addr(ctmp), nhsb, nvsb, q, q, qm, masking, keyframe, lam,
+    r = ref.oracle_ref_dering_search(addr(src), src.shape[1], addr(ctmp), nhsb, nvsb, q,
+                                     q if coded_quantizer is None else coded_quantizer, qm, masking, keyframe, lam,
                                      addr(bskip) if bskip is not None else None,
                                      bskip.shape[1] if bskip is not None else 0, addr(cdf), increment, addr(levels), addr(dist))
     assert r == 0

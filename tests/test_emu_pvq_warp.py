@@ -104,3 +104,27 @@ def test_warp_quantiser_large_k():
     qm, qm_inv = _reference_qm()
     ks = _check_case_set(emu, "large_k", qm, qm_inv)
     assert len(ks) == 48 and ks.max() > 1000
+
+
+def test_warp_quantiser_quantizer_range():
+    """Band quantisers 1101 to 130521 (pvq_cases.quantizer_range_cases): the coarse end of the encoder's coded
+    quantizers times its quantisation matrices, where most bands code a handful of pulses or none."""
+    emu = _build("libpvq_warp_emu.so", [])
+    qm, qm_inv = _reference_qm()
+    ks = _check_case_set(emu, "quantizer_range", qm, qm_inv)
+    assert (ks == 0).any() and ks.max() > 100
+
+
+def test_port_quantiser_quantizer_range():
+    """The oracle's plain-C port of pvq_theta on the same recorded cases."""
+    from tests import oracle_lib
+    port = oracle_lib.load_port()
+    qm, qm_inv = _reference_qm()
+    gold = np.load(os.path.join(GOLDEN, "reference_digests.npz"))
+    rows, skip_diff = gold["quantizer_range"], gold["quantizer_range_skip_diff"]
+    cases = list(make_golden.theta_case_set("quantizer_range"))
+    assert len(cases) == len(rows)
+    for c, want, want_sd in zip(cases, rows.tolist(), skip_diff.tolist()):
+        got = pvq_cases.run_theta(port, "port", c, qm, qm_inv)
+        assert pvq_cases.digest(got) == want and got["skip_diff"] == want_sd, (
+            {k: c[k] for k in ("n", "kind", "is_keyframe", "pli", "beta", "q0", "lam")}, want, want_sd, got)

@@ -54,8 +54,9 @@ def _at_origins(blocks, values, geom, pli, frame, fill, dtype):
     return out
 
 
-def _compare(out, coeffs, md, geom, frames, q0, q4, frame_ids=None):
-    """out / coeffs / md: the engine's results for the batch `frames` = [(planes, pred, bsize)]."""
+def _compare(out, coeffs, md, geom, frames, q0, q4, frame_ids=None, **chain_kw):
+    """out / coeffs / md: the engine's results for the batch `frames` = [(planes, pred, bsize)]; chain_kw: the
+    engine's use_masking / qm / qm_inv when they are not the defaults."""
     from daala_b200 import engine
     lib, prefix = _oracle()
     tabs = _coding_tables()
@@ -64,7 +65,7 @@ def _compare(out, coeffs, md, geom, frames, q0, q4, frame_ids=None):
         if frame_ids is not None and f not in frame_ids:
             wants.append(None)
             continue
-        want = inter_oracle.inter_chain(lib, prefix, planes, pred, geom, bsize, q0, q4)
+        want = inter_oracle.inter_chain(lib, prefix, planes, pred, geom, bsize, q0, q4, **chain_kw)
         wants.append(want)
         for pli in range(3):
             kind = "luma" if pli == 0 else "chroma"
