@@ -18,7 +18,8 @@
 //
 // config.inter: the residual of a batch of P frames the same way.  The motion-compensated prediction planes are
 // a second input (config.inter_mc: made in the graph from MV grids and a pool of reference pictures, before the
-// forward transform); they take the same forward transform (no DC Haar pyramid on either side) and their
+// forward transform; config.mc_next adds B frames: a NEXT picture per frame and each vertex's second vector mv1);
+// they take the same forward transform (no DC Haar pyramid on either side) and their
 // coefficients `md` are the reference vector of every band (pvq_theta with is_keyframe = 0).  Without an intra
 // predictor every (block, band) of every plane is dependency-free: luma and chroma both go through the three
 // phase kernels (k_pvq_split) and the persistent chain kernel is not launched.  config.late_skip adds the four
@@ -63,7 +64,7 @@ enum Cnt {
   kNHeads0 = 16,     // band-0 items ready from the start
   kError = 17,
   kDepsDone = 18,    // CTAs of k_luma_deps that have finished (the last one scans the chain heads' weight bins)
-  kMcBadRef = 19,    // config.inter_mc: leaf corners whose vertex has a ref other than GOLD / PREV
+  kMcBadRef = 19,    // config.inter_mc: leaf corners whose vertex has a ref other than GOLD / PREV (/ NEXT: mc_next)
   kMcBeyond = 20,    //                  corner windows reaching past the reference's edge extension
   // the words the persistent kernels hammer with atomics each sit in a 128-byte line of their own
   kHeadLoL = 32,     // ticket of the luma dependency-free lists
@@ -1693,6 +1694,8 @@ struct daala_b200_kf {
   uint8_t* ref_pixels[3];
   int32_t* ref_slot;
   daala_b200_mv_pt* mv_grid;
+  int32_t* ref_slot_next;          // cfg.mc_next: each frame's NEXT slot and the mv1 grids; NULL otherwise
+  int32_t* mv1_grid;
   uint32_t* mc_leaves;
   int32_t* mc_nleaves;
   daala_b200_mc_batch mc;
@@ -1796,6 +1799,12 @@ static int kf_alloc(daala_b200_kf* kf) {
     B.nhsb = kf->nhsb;
     B.nvsb = kf->nvsb;
     B.nslots = kf->cfg.mc_refs;
+    if (kf->cfg.mc_next) {
+      KF_CHECK(dalloc(kf, &kf->ref_slot_next, (size_t)F));
+      KF_CHECK(dalloc(kf, &kf->mv1_grid, (size_t)F * (kf->nvsb * 8 + 1) * (kf->nhsb * 8 + 1) * 2));
+      B.ref_slot_next = kf->ref_slot_next;
+      B.mv1 = kf->mv1_grid;
+    }
   }
   KF_CHECK(dalloc(kf, &kf->qm, (size_t)2 * kf->cfg.qm_stride));
   KF_CHECK(dalloc(kf, &kf->qm_inv, (size_t)2 * kf->cfg.qm_stride));
@@ -2473,6 +2482,10 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
     snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: inter_mc is 0 or 1, and 1 requires inter = 1");
     return nullptr;
   }
+  if (cfg && cfg->mc_next && (cfg->mc_next != 1 || cfg->inter_mc != 1)) {
+    snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: mc_next is 0 or 1, and 1 requires inter_mc = 1");
+    return nullptr;
+  }
   if (cfg && cfg->inter_finish && (cfg->inter_finish < 0 || cfg->inter_finish > 2 || cfg->inter != 1)) {
     snprintf(g_create_err, sizeof(g_create_err),
              "daala_b200_kf_create: inter_finish is 0, 1 or 2, and 1 and 2 require inter = 1");
@@ -2518,7 +2531,7 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   kf->nhsb = (cfg->pic_w + 63) / 64;
   kf->nvsb = (cfg->pic_h + 63) / 64;
   kf->F = cfg->nframes;
-  if (kf->cfg.inter_mc && kf->cfg.mc_refs == 0) kf->cfg.mc_refs = 2 * kf->F;
+  if (kf->cfg.inter_mc && kf->cfg.mc_refs == 0) kf->cfg.mc_refs = (kf->cfg.mc_next ? 3 : 2) * kf->F;
   if (!kf->cfg.inter_mc) kf->cfg.mc_refs = 0;
   kf->slot_filled.assign((size_t)kf->cfg.mc_refs, 0);
   if (kf->cfg.sb_rows <= 0) {
@@ -2650,6 +2663,8 @@ int daala_b200_kf_device_buffers(daala_b200_kf* kf, daala_b200_kf_buffers* out) 
   out->ref_slot = kf->ref_slot;
   out->mv_grid = kf->mv_grid;
   out->mc_refs = kf->cfg.mc_refs;
+  out->ref_slot_next = kf->ref_slot_next;
+  out->mv1_grid = kf->mv1_grid;
   return 0;
 }
 
@@ -2782,6 +2797,10 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: an inter engine needs pred_pixels[0..2], luma_dc and chroma_dc");
     return (int)cudaErrorInvalidValue;
   }
+  if ((io->ref_slot_next || io->mv1_grid) && !kf->cfg.mc_next) {
+    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: ref_slot_next and mv1_grid need an engine with mc_next");
+    return (int)cudaErrorInvalidValue;
+  }
   if (io->ref_resident && !kf->cfg.inter_mc) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: ref_resident needs an engine with inter_mc");
     return (int)cudaErrorInvalidValue;
@@ -2797,11 +2816,17 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
                       : !resident && (!io->ref_pixels[0] || !io->ref_pixels[1] || !io->ref_pixels[2])
                           ? "ref_pixels[0..2] are required"
                       : !io->ref_slot ? "ref_slot is required"
+                      : kf->cfg.mc_next && !io->ref_slot_next ? "mc_next: ref_slot_next is required"
+                      : kf->cfg.mc_next && !io->mv1_grid ? "mc_next: mv1_grid is required"
                       : have_pred ? "pred_pixels is refused: the engine makes the prediction"
                       : !resident && (io->nrefs < 1 || io->nrefs > kf->cfg.mc_refs) ? "nrefs is outside [1, mc_refs]"
                                                                                     : nullptr;
-    for (int i = 0; !why && i < 2 * F; i++) {
-      const int32_t r = io->ref_slot[i];
+    // the GOLD / PREV slots, then (mc_next) the NEXT slots
+    const int nslot = (kf->cfg.mc_next ? 3 : 2) * F;
+    bool in_next = false;
+    for (int i = 0; !why && i < nslot; i++) {
+      const int32_t r = i < 2 * F ? io->ref_slot[i] : io->ref_slot_next[i - 2 * F];
+      in_next = i >= 2 * F;
       if (!resident && (r < 0 || r >= io->nrefs)) why = "a ref_slot entry is outside [0, nrefs)";
       else if (resident && (r < 0 || r >= kf->cfg.mc_refs)) why = "ref_resident: a ref_slot entry is outside [0, mc_refs)";
       else if (resident && !kf->slot_filled[r])
@@ -2809,7 +2834,7 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
               "submit or a finish with ref_slot_out writes one)";
     }
     if (why) {
-      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: inter_mc: %s", why);
+      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: inter_mc: %s%s", why, in_next ? " (ref_slot_next)" : "");
       return (int)cudaErrorInvalidValue;
     }
   }
@@ -2891,6 +2916,12 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     KF_CHECK(cudaMemcpyAsync(kf->mv_grid, io->mv_grid,
                              sizeof(daala_b200_mv_pt) * F * (kf->nvsb * 8 + 1) * (kf->nhsb * 8 + 1),
                              cudaMemcpyHostToDevice, s));
+    if (kf->cfg.mc_next) {
+      KF_CHECK(cudaMemcpyAsync(kf->ref_slot_next, io->ref_slot_next, sizeof(int32_t) * F, cudaMemcpyHostToDevice, s));
+      KF_CHECK(cudaMemcpyAsync(kf->mv1_grid, io->mv1_grid,
+                               sizeof(int32_t) * 2 * F * (kf->nvsb * 8 + 1) * (kf->nhsb * 8 + 1),
+                               cudaMemcpyHostToDevice, s));
+    }
   }
   const size_t map_bytes = (size_t)kf->nhsb * 8 * kf->nvsb * 8 * F;
   KF_CHECK(cudaMemcpyAsync(kf->bsize, io->bsize, map_bytes, cudaMemcpyHostToDevice, s));

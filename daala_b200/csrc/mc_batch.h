@@ -15,10 +15,14 @@ struct daala_b200_mc_batch {
   uint8_t* pred[3];                // [F][plane_h][plane_w]
   uint32_t* leaves;                // [F][nvsb*nhsb][64] leaf records (see mc_kernels.cu), a count per segment in
   int32_t* nleaves;                // [F][nvsb*nhsb]
-  int32_t* bad_ref;                // counter: leaf corners whose vertex has a ref other than 0 / 1
+  int32_t* bad_ref;                // counter: leaf corners whose vertex has a ref other than 0 / 1 (0 / 1 / 2 with mv1)
   int32_t* beyond;                 // counter: corner windows reaching past the reference's edge extension
   int F, nhsb, nvsb, nslots;
   int plane_w[3], plane_h[3];
+  // config.mc_next (B frames), NULL otherwise: a vertex with ref 2 (OD_FRAME_NEXT) is predicted from the frame's NEXT
+  // picture with its second vector mv1 (od_state_pred_block_from_setup, reference src/state.c:647-660)
+  const int32_t* ref_slot_next;    // [F]: pool slot of OD_FRAME_NEXT
+  const int32_t* mv1;              // [F][nvsb*8 + 1][nhsb*8 + 1][2]: each vertex's mv1 in 1/8 luma pixel
 };
 
 // od_state_pred_block's split recursion for every (frame, 64x64 MV block): its leaves and both counters.

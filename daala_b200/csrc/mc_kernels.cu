@@ -436,6 +436,10 @@ k_est_sad(const __grid_constant__ BmaPlanes P, const daala_b200_mc_block* __rest
 // log size l << 6 | oc << 8 | s << 10.  The same leaves serve all three planes.
 // k_mc_obmc: per (frame, MV block, plane) the OBMC prediction of each leaf, every corner from the pool slot of its
 // vertex's picture.
+// Both are templates on config.mc_next (B frames): kNext = false is the P-frame code as it was; kNext = true also
+// reads the NEXT slot and, for a corner whose vertex has ref 2 (OD_FRAME_NEXT), the vertex's second vector mv1
+// (od_state_pred_block_from_setup, src/state.c:647-660).  mv1 is never read on ref 0 / 1 vertices: the encoder leaves
+// stale vectors there.
 
 __constant__ int kVertD[22] = {0, 0, 1, 1, 0, 0, 1, 2, 0, 0, 2, 1, 0, -1, 1, 1, 0, -1, 0, 1, 1, -1};   // OD_VERT_D
 // offsets into OD_VERT_D of OD_VERT_SETUP_DX / _DY [oc][s] (src/state.c:593-625; OD_VERT_DY = OD_VERT_D)
@@ -446,12 +450,23 @@ __device__ __forceinline__ int div_pow2_re(int x, int shift) {   // OD_DIV_POW2_
   return shift ? (x + (((1 << shift) + ((x >> shift) & 1) - 1) >> 1)) >> shift : x;
 }
 
-// The vertex of corner k of the leaf at vertex (vx, vy) (od_state_pred_block_from_setup, src/state.c:647-651).
-__device__ __forceinline__ const daala_b200_mv_pt& leaf_corner(const daala_b200_mv_pt* g, int gstride, int vx, int vy,
-                                                               int l, int oc, int s, int k) {
-  return g[(vy + (kVertD[kSetupDY[oc][s] + k] << l)) * gstride + vx + (kVertD[kSetupDX[oc][s] + k] << l)];
+// The grid index of corner k of the leaf at vertex (vx, vy) (od_state_pred_block_from_setup, src/state.c:647-651).
+__device__ __forceinline__ int leaf_corner(int gstride, int vx, int vy, int l, int oc, int s, int k) {
+  return (vy + (kVertD[kSetupDY[oc][s] + k] << l)) * gstride + vx + (kVertD[kSetupDX[oc][s] + k] << l);
 }
 
+// The vector a corner is predicted with: mv, or (kNext) mv1 on a NEXT vertex; g1 is the frame's mv1 grid.
+template <bool kNext>
+__device__ __forceinline__ void corner_mv(const daala_b200_mv_pt& v, const int32_t* g1, int i, int& mvx, int& mvy) {
+  mvx = v.mv[0];
+  mvy = v.mv[1];
+  if (kNext && v.ref == 2) {
+    mvx = g1[2 * i];
+    mvy = g1[2 * i + 1];
+  }
+}
+
+template <bool kNext>
 __global__ void __launch_bounds__(256) k_mc_leaves(const __grid_constant__ daala_b200_mc_batch B) {
   const int lane = threadIdx.x & 31;
   const int nsb = B.nhsb * B.nvsb, gstride = B.nhsb * 8 + 1;
@@ -461,6 +476,7 @@ __global__ void __launch_bounds__(256) k_mc_leaves(const __grid_constant__ daala
     const int f = w / nsb, sb = w - f * nsb;
     const int vx0 = (sb % B.nhsb) * 8, vy0 = (sb / B.nhsb) * 8;
     const daala_b200_mv_pt* g = B.grid + f * per_frame;
+    const int32_t* g1 = kNext ? B.mv1 + 2 * f * per_frame : nullptr;
     uint32_t rec[2];
     bool emit[2];
 #pragma unroll
@@ -489,12 +505,15 @@ __global__ void __launch_bounds__(256) k_mc_leaves(const __grid_constant__ daala
       rec[h] = (uint32_t)(by * 8 + bx) | l << 6 | oc << 8 | s << 10;
       if (!emit[h]) continue;
       for (int k = 0; k < 4; k++) {
-        const daala_b200_mv_pt& v = leaf_corner(g, gstride, vx, vy, l, oc, s, k);
-        bad += v.ref > 1;
+        const int ci = leaf_corner(gstride, vx, vy, l, oc, s, k);
+        const daala_b200_mv_pt& v = g[ci];
+        bad += v.ref > (kNext ? 2 : 1);
+        int mvx, mvy;
+        corner_mv<kNext>(v, g1, ci, mvx, mvy);
         for (int p = 0; p < 3; p++) {
           const int dec = p > 0, pad = 64 >> dec, n = 1 << (l + 3 - dec);
-          const int x = (vx << (3 - dec)) + (div_pow2_re(v.mv[0], dec) >> 3);
-          const int y = (vy << (3 - dec)) + (div_pow2_re(v.mv[1], dec) >> 3);
+          const int x = (vx << (3 - dec)) + (div_pow2_re(mvx, dec) >> 3);
+          const int y = (vy << (3 - dec)) + (div_pow2_re(mvy, dec) >> 3);
           beyond += x - 2 < -pad || x + n + 2 > B.plane_w[p] - 1 + pad || y - 2 < -pad || y + n + 2 > B.plane_h[p] - 1 + pad;
         }
       }
@@ -515,6 +534,7 @@ __global__ void __launch_bounds__(256) k_mc_leaves(const __grid_constant__ daala
   if (lane == 0 && beyond) atomicAdd(B.beyond, beyond);
 }
 
+template <bool kNext>
 __global__ void __launch_bounds__(kThreads) k_mc_obmc(const __grid_constant__ daala_b200_mc_batch B) {
   __shared__ unsigned char pred[4][kMaxN * kMaxN];
   __shared__ short buf[(kMaxN + kApron) * kMaxN];
@@ -525,9 +545,11 @@ __global__ void __launch_bounds__(kThreads) k_mc_obmc(const __grid_constant__ da
     const int dec = p > 0, pw = B.plane_w[p], ph = B.plane_h[p];
     const int vx0 = (sb % B.nhsb) * 8, vy0 = (sb / B.nhsb) * 8;
     const daala_b200_mv_pt* g = B.grid + f * per_frame;
+    const int32_t* g1 = kNext ? B.mv1 + 2 * f * per_frame : nullptr;
     const size_t plane = (size_t)pw * ph;
     // submit checks the slots; a device-resident caller's are kept inside the pool
     const int gold = min(max(B.ref_slot[2 * f], 0), B.nslots - 1), prev = min(max(B.ref_slot[2 * f + 1], 0), B.nslots - 1);
+    const int next = kNext ? min(max(B.ref_slot_next[f], 0), B.nslots - 1) : 0;
     unsigned char* out = B.pred[p] + f * plane;
     const int n = B.nleaves[w];
     for (int q = 0; q < n; q++) {
@@ -536,11 +558,15 @@ __global__ void __launch_bounds__(kThreads) k_mc_obmc(const __grid_constant__ da
       daala_b200_mc_block b;
       ClampedRef refs[4];
       for (int k = 0; k < 4; k++) {
-        const daala_b200_mv_pt& v = leaf_corner(g, gstride, vx, vy, l, oc, s, k);
-        b.mvx[k] = div_pow2_re(v.mv[0], dec);
-        b.mvy[k] = div_pow2_re(v.mv[1], dec);
-        // a ref other than GOLD reads PREV (counted by k_mc_leaves)
-        refs[k] = ClampedRef{B.ref[p] + (size_t)(v.ref == 0 ? gold : prev) * plane, pw, pw, ph};
+        const int ci = leaf_corner(gstride, vx, vy, l, oc, s, k);
+        const daala_b200_mv_pt& v = g[ci];
+        int mvx, mvy;
+        corner_mv<kNext>(v, g1, ci, mvx, mvy);
+        b.mvx[k] = div_pow2_re(mvx, dec);
+        b.mvy[k] = div_pow2_re(mvy, dec);
+        // a ref other than GOLD (and NEXT) reads PREV (counted by k_mc_leaves)
+        const int slot = v.ref == 0 ? gold : kNext && v.ref == 2 ? next : prev;
+        refs[k] = ClampedRef{B.ref[p] + (size_t)slot * plane, pw, pw, ph};
       }
       b.x0 = (uint16_t)(vx << (3 - dec));
       b.y0 = (uint16_t)(vy << (3 - dec));
@@ -623,12 +649,14 @@ int daala_b200_mc_predict1fmv_batch(const uint8_t* ref, int ref_stride, uint8_t*
 }
 
 int daala_b200_launch_mc_leaves(const daala_b200_mc_batch* b, int grid, cudaStream_t stream) {
-  k_mc_leaves<<<grid, 256, 0, stream>>>(*b);
+  if (b->mv1) k_mc_leaves<true><<<grid, 256, 0, stream>>>(*b);
+  else k_mc_leaves<false><<<grid, 256, 0, stream>>>(*b);
   return (int)cudaGetLastError();
 }
 
 int daala_b200_launch_mc_obmc(const daala_b200_mc_batch* b, int grid, cudaStream_t stream) {
-  k_mc_obmc<<<grid, kThreads, 0, stream>>>(*b);
+  if (b->mv1) k_mc_obmc<true><<<grid, kThreads, 0, stream>>>(*b);
+  else k_mc_obmc<false><<<grid, kThreads, 0, stream>>>(*b);
   return (int)cudaGetLastError();
 }
 

@@ -18,6 +18,9 @@ DC record per block: qdc and the unquantised residual), and `finish_stream` take
 With inter=1 and late_skip=1 each step also returns the four late-skip distortions of every block
 (symbols.LATE_SKIP_DTYPE; `luma_late_skip` / `chroma_late_skip`, and `sym_late_skip` in stream order), from which the
 host coder takes the reference's late-skip decision (daala_b200/lateskip.py).
+With inter_mc=1 and mc_next=1 the engine predicts B frames: `ref_slot=` is [F, 3] (GOLD, PREV, NEXT) and `mv1_grid=`
+holds each vertex's second vector, which a vertex with ref 2 (NEXT) is predicted with (gop.py gives the reference's
+B-frame order and buffer rotation).
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -42,7 +45,7 @@ class Config(ctypes.Structure):
                 ("max_blocks_div", c_int), ("persist_ctas_per_sm", c_int), ("split_free", c_int), ("dering", c_int), ("noref_prepass", c_int), ("level_chains", c_int), ("stream", c_void_p),
                 ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
                 ("symbol_stream", c_int), ("inter", c_int), ("inter_mc", c_int), ("mc_refs", c_int),
-                ("inter_finish", c_int), ("late_skip", c_int)]
+                ("inter_finish", c_int), ("late_skip", c_int), ("mc_next", c_int)]
 
 
 class Totals(ctypes.Structure):
@@ -62,7 +65,7 @@ class IO(ctypes.Structure):
                 ("pred_pixels_out", c_void_p * 3), ("luma_dc_resid", c_void_p), ("chroma_dc_resid", c_void_p),
                 ("ref_resident", c_int), ("sym_dc", c_void_p), ("sym_dc_cap", c_ll),
                 ("luma_late_skip", c_void_p), ("chroma_late_skip", c_void_p), ("sym_late_skip", c_void_p),
-                ("sym_late_skip_cap", c_ll)]
+                ("sym_late_skip_cap", c_ll), ("ref_slot_next", c_void_p), ("mv1_grid", c_void_p)]
 
 
 class FinishIO(ctypes.Structure):
@@ -87,7 +90,8 @@ class Buffers(ctypes.Structure):
                 ("max_luma_blocks", c_int), ("max_chroma_blocks", c_int), ("stream", c_void_p),
                 ("bytes_allocated", c_ll), ("pred_pixels", c_void_p * 3), ("pred_coeffs", c_void_p * 3),
                 ("luma_heads_raw", c_void_p), ("luma_head_bin", c_void_p), ("ref_pixels", c_void_p * 3),
-                ("ref_slot", c_void_p), ("mv_grid", c_void_p), ("mc_refs", c_int)]
+                ("ref_slot", c_void_p), ("mv_grid", c_void_p), ("mc_refs", c_int), ("ref_slot_next", c_void_p),
+                ("mv1_grid", c_void_p)]
 
 
 def _bind():
@@ -146,7 +150,7 @@ class KeyframeEngine:
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
                  qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=0, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
                  qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0, inter_mc=0, mc_refs=0,
-                 inter_finish=0, late_skip=0):
+                 inter_finish=0, late_skip=0, mc_next=0):
         self.L = _bind()
         self.geom, self.F = geom, nframes
         if qm is None:
@@ -186,6 +190,9 @@ class KeyframeEngine:
         # late_skip: od_compute_dist with coded_quantizer, qm_is_flat and use_masking above
         cfg.late_skip = int(late_skip)
         self.late_skip = int(late_skip)
+        # mc_next: B frames, a third picture (NEXT) per frame and the mv1 grid
+        cfg.mc_next = int(mc_next)
+        self.mc_next = int(mc_next)
         self.nrefs = 0
         self.resident = False
         self._pool_src = []
@@ -266,13 +273,20 @@ class KeyframeEngine:
             raise ValueError("pred= planes are required by an inter engine and refused by a keyframe engine "
                              "and by an inter_mc engine")
 
-    def stage_mc(self, refs, ref_slot, mv_grid, resident=False):
+    def stage_mc(self, refs, ref_slot, mv_grid, resident=False, mv1_grid=None):
         """Copies one batch's prediction inputs (inter_mc engines) into the host buffers.  refs: per plane an
         array [nrefs, h, w] u8 (frame-sized reference pictures), uploaded into pool slots [0, nrefs); ref_slot: [F, 2]
-        pool slots of each frame's GOLD and PREV picture; mv_grid: [F, nvsb*8 + 1, nhsb*8 + 1] mvgrid.MV_PT_DTYPE
-        (mvgrid.pack).  resident=True: the step reads the pool as it stands (ref_resident), refs must be None and
-        every slot named must hold a picture (pool_load, an earlier upload, or a finish with ref_slot_out)."""
+        pool slots of each frame's GOLD and PREV picture ([F, 3] GOLD, PREV, NEXT on an mc_next engine); mv_grid:
+        [F, nvsb*8 + 1, nhsb*8 + 1] mvgrid.MV_PT_DTYPE (mvgrid.pack); mv1_grid (mc_next engines only, required there):
+        [F, nvsb*8 + 1, nhsb*8 + 1, 2] int32, each vertex's second vector.  resident=True: the step reads the pool as it
+        stands (ref_resident), refs must be None and every slot named must hold a picture (pool_load, an earlier upload,
+        or a finish with ref_slot_out)."""
         g = self.geom
+        nslot = 3 if self.mc_next else 2
+        if (mv1_grid is not None) != bool(self.mc_next):
+            raise ValueError("mv1_grid= goes with an mc_next engine, and it needs one")
+        if ref_slot is not None and np.shape(ref_slot) != (self.F, nslot):
+            raise ValueError("ref_slot= is [F, %d] on this engine (GOLD, PREV%s)" % (nslot, ", NEXT" if self.mc_next else ""))
         if resident:
             if not self.inter_mc or refs is not None or ref_slot is None or mv_grid is None:
                 raise ValueError("resident=True goes with an inter_mc engine, needs ref_slot= and mv_grid=, and "
@@ -286,9 +300,14 @@ class KeyframeEngine:
                 a = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8)
                 a[...] = refs[p]
         a = self._arr("slot", (self.F, 2), np.int32)
-        a[...] = ref_slot
+        a[...] = np.asarray(ref_slot)[:, :2]
         a = self._arr("grid", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1), mvgrid.MV_PT_DTYPE)
         a[...] = mv_grid
+        if self.mc_next:
+            a = self._arr("slot_next", (self.F,), np.int32)
+            a[...] = np.asarray(ref_slot)[:, 2]
+            a = self._arr("grid1", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1, 2), np.int32)
+            a[...] = mv1_grid
 
     def stage_inputs(self, planes, bsize, pred=None):
         """Copies one batch into the engine's (pinned) host input buffers.  planes: per plane an array
@@ -366,6 +385,9 @@ class KeyframeEngine:
             io.nrefs = self.nrefs
             io.ref_slot = self._arr("slot", (self.F, 2), np.int32).ctypes.data
             io.mv_grid = self._arr("grid", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1), mvgrid.MV_PT_DTYPE).ctypes.data
+            if self.mc_next:
+                io.ref_slot_next = self._arr("slot_next", (self.F,), np.int32).ctypes.data
+                io.mv1_grid = self._arr("grid1", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1, 2), np.int32).ctypes.data
         if self.inter:
             if not self.inter_mc:
                 for p in range(3):
@@ -408,6 +430,8 @@ class KeyframeEngine:
         if self.inter_mc:
             self.h2d_bytes += (px * self.nrefs + 8 * self.F
                                + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * mvgrid.MV_PT_DTYPE.itemsize)
+            if self.mc_next:   # the NEXT slot of each frame and the mv1 of each vertex
+                self.h2d_bytes += 4 * self.F + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * 8
         return out
 
     def submit(self):
@@ -430,15 +454,17 @@ class KeyframeEngine:
         return idx.nbytes + blocks * sym.BLOCK_DTYPE.itemsize + int(idx[:, 3].sum()) * 8 + int(idx[:, 5].sum()) + dc
 
     def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None, pred=None, refs=None,
-               ref_slot=None, mv_grid=None, resident=False):
+               ref_slot=None, mv_grid=None, resident=False, mv1_grid=None):
         """One batch end to end through the C ABI with host buffers; returns the result arrays (views of
         the engine's host buffers: copy what must survive the next call).  pred: see stage_inputs; refs, ref_slot,
-        mv_grid, resident (inter_mc engines, which also return the prediction as pred0..2): see stage_mc.  Raises when the
-        batch exceeded the block capacity, or (inter_mc) when a used vertex names a picture other than GOLD / PREV
-        or a vector reaches past the reference's edge extension: the reference encoder's result is undefined there."""
+        mv_grid, resident, mv1_grid (inter_mc engines, which also return the prediction as pred0..2): see stage_mc.  Raises
+        when the batch exceeded the block capacity, or (inter_mc) when a used vertex names a picture other than GOLD /
+        PREV (/ NEXT on mc_next engines) or a vector reaches past the reference's edge extension: the reference
+        encoder's result is undefined there."""
         self.stage_inputs(planes, bsize, pred)
-        if self.inter_mc or refs is not None or ref_slot is not None or mv_grid is not None or resident:
-            self.stage_mc(refs, ref_slot, mv_grid, resident)
+        if (self.inter_mc or refs is not None or ref_slot is not None or mv_grid is not None or resident
+                or mv1_grid is not None):
+            self.stage_mc(refs, ref_slot, mv_grid, resident, mv1_grid)
         if self.dering == 1:
             self.stage_dering_levels(dering_levels)
         self.prepare_io(symbols, recon, stream)
@@ -450,7 +476,8 @@ class KeyframeEngine:
             bad, beyond = int(out["counts"][CNT["mc_bad_ref"]]), int(out["counts"][CNT["mc_beyond"]])
             if bad or beyond:
                 raise RuntimeError("keyframe engine: MV grid outside the reference's definition: %d leaf corners with a "
-                                   "ref other than GOLD / PREV, %d corner windows past the edge extension" % (bad, beyond))
+                                   "ref other than GOLD / PREV%s, %d corner windows past the edge extension"
+                                   % (bad, " / NEXT" if self.mc_next else "", beyond))
         return out
 
     def prepare_finish(self, luma_skip, luma_dc, chroma_skip, chroma_dc, dering_levels=None, ref_slot_out=None):

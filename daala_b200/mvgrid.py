@@ -19,7 +19,8 @@ _DY = _D[0:4]
 _SETUP_DX = [[9, 1, 9, 1], [13, 13, 1, 1], [18, 1, 18, 1], [5, 5, 1, 1]]   # offsets into OD_VERT_D
 _SETUP_DY = [[4, 4, 0, 0], [8, 0, 8, 0], [12, 12, 0, 0], [17, 0, 17, 0]]   # offsets into OD_VERT_DY (= D)
 LOG_MVB_DELTA0 = 3   # OD_LOG_MVBSIZE_MAX - OD_LOG_MVBSIZE_MIN
-# daala_b200_mv_pt (include/daala_b200.h): one vertex as od_mv_grid_pt holds it; ref 0 = OD_FRAME_GOLD, 1 = _PREV
+# daala_b200_mv_pt (include/daala_b200.h): one vertex as od_mv_grid_pt holds it; ref 0 = OD_FRAME_GOLD, 1 = _PREV,
+# 2 = _NEXT (B frames, mc_next engines: the vertex's second vector mv1 travels beside the grid)
 MV_PT_DTYPE = np.dtype([("mv", "<i4", 2), ("valid", "u1"), ("ref", "u1"), ("pad_", "u1", 2)])
 assert MV_PT_DTYPE.itemsize == 12
 
@@ -63,6 +64,18 @@ def leaves(valid):
     return tuple(np.concatenate([o[i] for o in out]) for i in range(5))
 
 
+REF_NEXT = 2   # OD_FRAME_NEXT
+
+
+def vectors(mv, ref, mv1=None):
+    """The vector each vertex is predicted with (od_state_pred_block_from_setup, src/state.c:647-660): mv1 where
+    ref == 2 (OD_FRAME_NEXT), mv elsewhere.  mv1 is never taken on a GOLD / PREV vertex, where the encoder leaves
+    stale values; without mv1 (P frames) this is mv."""
+    if mv1 is None:
+        return np.asarray(mv)
+    return np.where((np.asarray(ref) == REF_NEXT)[..., None], mv1, mv)
+
+
 def block_list(valid, mv, xdec=0):
     """daala_b200_mc_block records (mc.MC_BLOCK_DTYPE) of one plane: `valid` bool
     [(nvmvbs+1), (nhmvbs+1)], `mv` int32 [.., .., 2] in 1/8 luma pixel."""
@@ -78,10 +91,13 @@ def corners(vx, vy, l, oc, s):
     return [(vx + (d[sdx + k] << l), vy + (d[sdy + k] << l)) for k in range(4)]
 
 
-def blocks_for(vx, vy, l, oc, s, mv, xdec=0):
+def blocks_for(vx, vy, l, oc, s, mv, xdec=0, ref=None, mv1=None):
     """Block records of given MV blocks (vertex position, log size, outside corner, split state): what
-    od_state_pred_block_from_setup (src/state.c:627) derives for one plane."""
+    od_state_pred_block_from_setup (src/state.c:627) derives for one plane.  With ref and mv1 (B frames) a corner on
+    a NEXT vertex takes mv1 (see vectors)."""
     vx, vy, l, oc, s = (np.asarray(a, np.int64) for a in (vx, vy, l, oc, s))
+    if mv1 is not None:
+        mv = vectors(mv, ref, mv1)
     blocks = np.zeros(len(vx), mc.MC_BLOCK_DTYPE)
     for k, (gx, gy) in enumerate(corners(vx, vy, l, oc, s)):
         blocks["mvx"][:, k] = _div_pow2_re(mv[gy, gx, 0].astype(np.int64), xdec)

@@ -107,3 +107,25 @@ def mv_grid(geom, seed=0, p_split=(0.6, 0.5, 0.4), p_gold=0.5, umv=32):
     mv = rng.integers(-umv * 8, umv * 8 + 1, size=(nv, nh, 2)).astype(np.int32)
     ref = (rng.random((nv, nh)) >= p_gold).astype(np.uint8)
     return valid.astype(np.uint8), mv, ref
+
+
+def mv_grid_b(geom, seed=0, p_split=(0.6, 0.5, 0.4), p_next=0.5, p_gold=0.3, umv=32):
+    """A seeded MV grid for one B frame of `geom`: (valid, mv, mv1, ref), valid / mv / split levels as mv_grid.  ref
+    is NEXT (2) with probability p_next, else GOLD (0) with probability p_gold, else PREV (1), mixed per vertex (the
+    reference's B frames use PREV and NEXT, src/encode.c:1855 rules out 3; GOLD covers the engine's third slot).  mv1 is random on every
+    vertex, as od_mv_est leaves it (stale on the vertices whose ref is not NEXT).  A stream of its own: mv_grid's
+    output for a seed does not change."""
+    rng = np.random.default_rng([seed, 2])
+    nv, nh = geom.nvsb * 8 + 1, geom.nhsb * 8 + 1
+    vy, vx = np.mgrid[0:nv, 0:nh]
+    p = np.full((nv, nh), 0.5)
+    for lvl, step in enumerate((8, 4, 2)):
+        centre = (vx % step == step // 2) & (vy % step == step // 2)
+        p[centre] = p_split[lvl]
+    valid = rng.random((nv, nh)) < p
+    valid[(vx % 8 == 0) & (vy % 8 == 0)] = True
+    mv = rng.integers(-umv * 8, umv * 8 + 1, size=(nv, nh, 2)).astype(np.int32)
+    mv1 = rng.integers(-umv * 8, umv * 8 + 1, size=(nv, nh, 2)).astype(np.int32)
+    u = rng.random((nv, nh))
+    ref = np.where(u < p_next, 2, np.where(u < p_next + (1 - p_next) * p_gold, 0, 1)).astype(np.uint8)
+    return valid.astype(np.uint8), mv, mv1, ref

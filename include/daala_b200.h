@@ -518,13 +518,22 @@ typedef struct daala_b200_kf_config {
                                   chroma_late_skip / sym_late_skip), with coded_quantizer, qm_is_flat and use_masking
                                   (enc->use_activity_masking) above.  Requires inter = 1; other values, and 1 without
                                   inter, are refused by daala_b200_kf_create */
+  int mc_next;                 /* 0 (default): nothing below exists; the engine is exactly the one without this field.
+                                  1: B frames (OD_SET_B_FRAMES).  A vertex with ref 2 (OD_FRAME_NEXT) is predicted from
+                                  the frame's NEXT picture (daala_b200_kf_io.ref_slot_next) with its second vector mv1
+                                  (daala_b200_kf_io.mv1_grid), as od_state_pred_block_from_setup does (reference
+                                  src/state.c:647-660); refs 0 and 1 work as before and their mv1 is not read (the
+                                  encoder leaves stale vectors there).  Nothing after the prediction differs from a P
+                                  frame.  mc_refs = 0 then means 3 * nframes.  Requires inter_mc = 1; other values, and
+                                  1 without inter_mc, are refused by daala_b200_kf_create */
 } daala_b200_kf_config;
 
 /* One vertex of a P frame's MV grid, as od_mv_grid_pt (reference src/mc.h:73-84) holds it after od_mv_est. */
 typedef struct daala_b200_mv_pt {  /* 12 bytes */
   int32_t mv[2];           /* x, y in 1/8 luma pixel */
   uint8_t valid;           /* the vertex is coded: the MV block with this vertex at its centre is split */
-  uint8_t ref;             /* picture the vector points into: 0 = OD_FRAME_GOLD, 1 = OD_FRAME_PREV */
+  uint8_t ref;             /* picture the vector points into: 0 = OD_FRAME_GOLD, 1 = OD_FRAME_PREV, and on
+                              config.mc_next engines 2 = OD_FRAME_NEXT (predicted with mv1, daala_b200_kf_io.mv1_grid) */
   uint8_t pad_[2];
 } daala_b200_mv_pt;
 
@@ -669,6 +678,11 @@ typedef struct daala_b200_kf_io {
      part is copied, as for sym_dc. */
   daala_b200_kf_late_skip *sym_late_skip;
   long long sym_late_skip_cap;
+  /* config.mc_next only (required there, refused otherwise).  The same submit checks as ref_slot apply to
+     ref_slot_next: within [0, nrefs) for an upload step, within [0, mc_refs) and holding a picture with ref_resident. */
+  const int32_t *ref_slot_next;         /* [nframes]: pool slot of each frame's NEXT picture */
+  const int32_t *mv1_grid;              /* [nframes][nvsb*8 + 1][nhsb*8 + 1][2]: each vertex's mv1 (od_mv_grid_pt.mv1,
+                                           src/mc.h:73-84) in 1/8 luma pixel, read only where ref == 2 */
 } daala_b200_kf_io;
 
 /* The finishing pass of a P-frame batch (config.inter_finish), daala_b200_kf_finish: the host coder's per-block
@@ -754,6 +768,8 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
   int32_t *ref_slot;                    /* the slot map ([nframes][2]) and the MV grids ([nframes][nvsb*8 + 1] */
   daala_b200_mv_pt *mv_grid;            /* [nhsb*8 + 1]) the prediction step reads; NULL otherwise */
   int mc_refs;                          /* pictures the pool holds (0 without inter_mc) */
+  int32_t *ref_slot_next;               /* config.mc_next: the NEXT slots ([nframes]) and the mv1 grids */
+  int32_t *mv1_grid;                    /* ([nframes][nvsb*8 + 1][nhsb*8 + 1][2]); NULL otherwise */
 } daala_b200_kf_buffers;
 
 #define DAALA_B200_KF_LISTS 1
@@ -792,9 +808,12 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    without symbol_stream = 2 (each with a message in daala_b200_kf_error).  With config.inter_mc it refuses, the same
    way, a NULL mv_grid, ref_pixels plane or ref_slot, pred_pixels given, nrefs outside [1, mc_refs] and a slot outside
    [0, nrefs); with ref_resident = 1 it refuses instead ref_pixels given, nrefs other than 0, a slot outside
-   [0, mc_refs) and a slot that holds no picture.  The step counts in `counts` the leaf corners whose vertex has a ref other than 0 or 1 (counts[19]) and
-   the corner windows (with the 6-tap filter's apron of -2..+3 pixels) that reach more than 64 luma / 32 chroma
-   pixels outside the plane (counts[20]), where the reference encoder's result is undefined. */
+   [0, mc_refs) and a slot that holds no picture.  With config.mc_next the same checks cover ref_slot_next, and a NULL
+   ref_slot_next or mv1_grid is refused; either given to an engine without mc_next is refused.  The step counts in
+   `counts` the leaf corners whose vertex has a ref other than 0 or 1 (counts[19]; with mc_next other than 0, 1 or 2)
+   and the corner windows (with the 6-tap filter's apron of -2..+3 pixels) that reach more than 64 luma / 32 chroma
+   pixels outside the plane (counts[20]; with mc_next the window of the vector the corner reads, mv1 on NEXT
+   vertices), where the reference encoder's result is undefined. */
 int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
 /* The finishing pass (config.inter_finish, see daala_b200_kf_finish_io) on the last submitted step: H2D of the
    decisions and levels, the pass's kernels as one CUDA graph (captured at the first call; with config.inter_finish
