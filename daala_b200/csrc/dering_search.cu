@@ -56,10 +56,13 @@ __global__ void __launch_bounds__(256) k_pack_sb_batch(const int16_t* __restrict
 // CDFs (the adaptation state is reset per frame, src/encode.c:3080).  Same operations as the host function, `coded`
 // (nullable, [F][nsb]) and `is_keyframe` included; log() is the CUDA library's, so a decision could differ from the
 // host's only where two scores agree to the last bits.
+// fq (nullable): frame f's lambda is fq[f].dering_lambda.
 __global__ void k_dering_decide(const double* __restrict__ dist, int nframes, int nhdr, int nvdr, double lambda,
-                                const uint8_t* __restrict__ coded, int is_keyframe, uint8_t* __restrict__ levels) {
+                                const uint8_t* __restrict__ coded, int is_keyframe, uint8_t* __restrict__ levels,
+                                const daala_b200_kf_frame_quant* __restrict__ fq) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= nframes) return;
+  if (fq) lambda = fq[f].dering_lambda;
   const int nsb = nhdr * nvdr;
   const size_t per_level = (size_t)nframes * nsb;
   const double* d = dist + (size_t)f * nsb;
@@ -102,6 +105,15 @@ __global__ void k_dering_decide(const double* __restrict__ dist, int nframes, in
       for (int i = best; i < kLevels; i++) m[i] = (unsigned short)(m[i] + 128);
     }
   }
+}
+
+// Per-frame thresholds (config.frame_quant): thr[gi - 1][f * nsb + sb] = frame_tbl[f][0][gi] for the five filtered
+// candidates, the per-superblock threshold maps their od_dering passes read.
+__global__ void k_cand_thresholds(const int32_t* __restrict__ frame_tbl, int n, int nsb, int32_t* __restrict__ thr) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int32_t* t = frame_tbl + (size_t)(i / nsb) * 12;
+  for (int gi = 1; gi < kLevels; gi++) thr[(size_t)(gi - 1) * n + i] = t[gi];
 }
 
 // od_encode_cdf_cost, src/generic_encoder.c:198
@@ -183,6 +195,11 @@ static int enqueue_candidates(const daala_b200_dering_search_batch* b, cudaStrea
   const int nsb = b->nhsb * b->nvsb, F = b->nframes;
   const int w = b->nhsb * 64, h = b->nvsb * 64;
   const long long filt_pitch = (long long)w * h;
+  if (b->frame_tbl) {
+    k_cand_thresholds<<<(F * nsb + 255) / 256, 256, 0, st>>>(b->frame_tbl, F * nsb, nsb, b->cand_thr);
+    cudaError_t e = cudaGetLastError();
+    if (e) return (int)e;
+  }
   for (int gi = 0; gi < kLevels; gi++) {
     const int16_t* plane = b->etmp;
     long long ppitch = b->etmp_pitch;
@@ -201,11 +218,12 @@ static int enqueue_candidates(const daala_b200_dering_search_batch* b, cudaStrea
       dp.nhsb = b->nhsb;
       dp.nvsb = b->nvsb;
       dp.threshold = b->threshold[gi];
+      dp.sb_threshold = b->frame_tbl ? b->cand_thr + (size_t)(gi - 1) * F * nsb : nullptr;
       dp.overlap = 1;
       dp.coeff_shift = 4;
       dp.dir_format = gi == 1 ? 1 : 2;
-      const int r = daala_b200_dering_plane_frames(&dp, F, filt_pitch, b->etmp_pitch, (long long)nsb * 64, 0,
-                                                   b->skip_pitch, nullptr, st);
+      const int r = daala_b200_dering_plane_frames(&dp, F, filt_pitch, b->etmp_pitch, (long long)nsb * 64,
+                                                   b->frame_tbl ? nsb : 0, b->skip_pitch, nullptr, st);
       if (r) return r;
       plane = b->filt;
       ppitch = filt_pitch;
@@ -215,8 +233,8 @@ static int enqueue_candidates(const daala_b200_dering_search_batch* b, cudaStrea
                                                   b->cand, gi == 0 ? b->orig : nullptr);
     cudaError_t e = cudaGetLastError();
     if (e) return (int)e;
-    const int r = daala_b200_compute_dist(b->orig, b->cand, F * nsb, 64, b->qm_is_flat, b->use_activity_masking,
-                                          b->coded_quantizer, b->dist + (size_t)gi * F * nsb, st);
+    const int r = daala_b200_compute_dist_frames(b->orig, b->cand, F * nsb, 64, b->qm_is_flat, b->use_activity_masking,
+                                                 b->coded_quantizer, b->fq, nsb, b->dist + (size_t)gi * F * nsb, st);
     if (r) return r;
   }
   return 0;
@@ -293,6 +311,6 @@ extern "C" int daala_b200_dering_search_enqueue(const daala_b200_dering_search_b
   const int r = enqueue_candidates(b, st);
   if (r) return r;
   k_dering_decide<<<(b->nframes + 31) / 32, 32, 0, st>>>(b->dist, b->nframes, b->nhsb, b->nvsb, b->dering_lambda,
-                                                         b->coded, b->is_keyframe, b->levels);
+                                                         b->coded, b->is_keyframe, b->levels, b->fq);
   return (int)cudaGetLastError();
 }

@@ -30,8 +30,19 @@ struct daala_b200_dering_search_batch {
   int32_t* dir;             // [F][nvsb * 8][nhsb * 8], left in the packed direction | variance << 3 format
   double* dist;             // [6][F * nsb]
   uint8_t* levels;          // out: [F][nvsb * nhsb]
+  // config.frame_quant (else NULL): per frame records (coded_quantizer and dering_lambda replace the fields above) and
+  // threshold tables ([F][2][6], replacing `threshold`), and the scratch of the filtered candidates' per-superblock
+  // thresholds, [5][F * nsb]
+  const daala_b200_kf_frame_quant* fq;
+  const int32_t* frame_tbl;
+  int32_t* cand_thr;
 };
 extern "C" int daala_b200_dering_search_enqueue(const daala_b200_dering_search_batch* b, void* stream);
+
+// daala_b200_compute_dist with each pair i scaled by the coded_quantizer of fq[i / per_frame] (fq NULL: coded_quantizer)
+int daala_b200_compute_dist_frames(const int32_t* x, const int32_t* y, int count, int n, int qm_is_flat,
+                                   int use_activity_masking, int coded_quantizer, const daala_b200_kf_frame_quant* fq,
+                                   int per_frame, double* out, void* stream);
 
 // The deringing threshold of every level at `quantizer` (src/encode.c:2697, :2822): tbl[0][g] luma,
 // (int)(OD_DERING_GAIN_TABLE[g] * quantizer^0.84182); tbl[1][g] chroma, the same product * 0.6.

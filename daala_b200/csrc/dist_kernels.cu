@@ -19,19 +19,24 @@ namespace dist {
 
 __global__ void __launch_bounds__(kDistThreads)
 k_compute_dist(const int32_t* __restrict__ xs, const int32_t* __restrict__ ys, int n, int qm_is_flat,
-               int use_activity_masking, double scale, double* __restrict__ out) {
+               int use_activity_masking, double scale, double* __restrict__ out,
+               const daala_b200_kf_frame_quant* __restrict__ fq, int per_frame) {
   extern __shared__ __align__(16) int32_t smem[];
   const size_t nn = (size_t)n * n;
   const double d = block_dist(xs + blockIdx.x * nn, n, 0, ys + blockIdx.x * nn, n, 0, __ffs(n) - 1, 1, qm_is_flat,
                               use_activity_masking, scale, smem);
-  if (threadIdx.x == 0) out[blockIdx.x] = d;
+  // fq: scale is 1.0 and the pair's frame's scale is applied here (block_dist's last multiplication; x * 1.0 is exact)
+  if (threadIdx.x == 0)
+    out[blockIdx.x] = fq && !qm_is_flat ? d * dist_scale(fq[blockIdx.x / per_frame].coded_quantizer) : d;
 }
 
 }  // namespace dist
 }  // namespace daala_b200
 
-extern "C" int daala_b200_compute_dist(const int32_t* x, const int32_t* y, int count, int n, int qm_is_flat,
-                                       int use_activity_masking, int coded_quantizer, double* out, void* stream) {
+// daala_b200_compute_dist, or (fq non-NULL) each pair i scaled by the coded_quantizer of record fq[i / per_frame]
+int daala_b200_compute_dist_frames(const int32_t* x, const int32_t* y, int count, int n, int qm_is_flat,
+                                   int use_activity_masking, int coded_quantizer, const daala_b200_kf_frame_quant* fq,
+                                   int per_frame, double* out, void* stream) {
   if (count <= 0) return 0;
   if (n != 8 && n != 16 && n != 32 && n != 64) return (int)cudaErrorInvalidValue;
   const size_t smem = daala_b200::dist::dist_scratch_bytes(n);
@@ -41,6 +46,13 @@ extern "C" int daala_b200_compute_dist(const int32_t* x, const int32_t* y, int c
     if (e != cudaSuccess) return (int)e;
   }
   daala_b200::dist::k_compute_dist<<<count, daala_b200::dist::kDistThreads, smem, (cudaStream_t)stream>>>(
-      x, y, n, qm_is_flat, use_activity_masking, daala_b200::dist::dist_scale(coded_quantizer), out);
+      x, y, n, qm_is_flat, use_activity_masking, fq ? 1.0 : daala_b200::dist::dist_scale(coded_quantizer), out, fq,
+      per_frame);
   return (int)cudaGetLastError();
+}
+
+extern "C" int daala_b200_compute_dist(const int32_t* x, const int32_t* y, int count, int n, int qm_is_flat,
+                                       int use_activity_masking, int coded_quantizer, double* out, void* stream) {
+  return daala_b200_compute_dist_frames(x, y, count, n, qm_is_flat, use_activity_masking, coded_quantizer, nullptr, 1,
+                                        out, stream);
 }

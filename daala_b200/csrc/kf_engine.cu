@@ -36,6 +36,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <mutex>
 #include <new>
 #include <vector>
@@ -528,6 +529,7 @@ struct Stage {
   long long cfl_pitch;
   int cfl_stride;
   int32_t* dc_resid;               // config.inter_finish or symbol_stream = 2: per block in[0] - ref[0], else NULL
+  const daala_b200_kf_frame_quant* fq;   // config.frame_quant: [F] the step's records (band_q), else NULL
 #ifdef DAALA_B200_CHAIN_TRACE
   struct ChainTraceRec* trace;     // luma: one record per item k_pvq_persist<true> runs, up to trace_cap
   int trace_cap;
@@ -847,7 +849,13 @@ struct ItemGeom {
   int blk, band, bn, q, beta, pli, qoff;
   size_t off;
 };
-__device__ __forceinline__ ItemGeom item_geom(const daala_b200_pvq_params& prm, uint32_t item) {
+// q0 * pvq_qm_q4[pli][qidx] >> 4 with the engine-wide quantizer, or with the record of the block's frame (fq: config.frame_quant)
+__device__ __forceinline__ int band_q(const daala_b200_pvq_params& prm, const daala_b200_kf_frame_quant* fq, int frame,
+                                      int pli, int qidx) {
+  return fq ? (fq[frame].q0 * fq[frame].pvq_qm_q4[pli][qidx]) >> 4 : (prm.q0 * prm.pvq_qm_q4[pli][qidx]) >> 4;
+}
+__device__ __forceinline__ ItemGeom item_geom(const daala_b200_pvq_params& prm, uint32_t item,
+                                              const daala_b200_kf_frame_quant* fq) {
   ItemGeom g;
   g.blk = (int)(item >> 4);
   g.band = (int)(item & 15);
@@ -858,7 +866,7 @@ __device__ __forceinline__ ItemGeom item_geom(const daala_b200_pvq_params& prm, 
   g.bn = band_start(g.band + 1) - start;
   g.off = (size_t)b.coef_off + start;
   const int qidx = bs * (bs + 1) + (g.band + 1) - (g.band + 1) / 3;
-  int q = (prm.q0 * prm.pvq_qm_q4[g.pli][qidx]) >> 4;
+  int q = band_q(prm, fq, b.frame, g.pli, qidx);
   g.q = q < 1 ? 1 : q;
   g.beta = (prm.use_masking && g.pli == 0 && bs > 0) ? kBeta15 : kBeta1;
   g.qoff = (b.xdec & 1 ? prm.qm_stride : 0) + ((((1 << (2 * bs)) - 1) << 4) / 3) + start;
@@ -866,8 +874,9 @@ __device__ __forceinline__ ItemGeom item_geom(const daala_b200_pvq_params& prm, 
 }
 
 // kPhase 0 / 1 / 2 = setup / search / finish of the items [chunk * slots, ...) of class `cls`.
-// kZeroRef: the prediction is all zero (luma bands 3 / 6).
-template <int kPhase, bool kZeroRef, int kMode>
+// kZeroRef: the prediction is all zero (luma bands 3 / 6).  kFq: the band quantisers come from the records of
+// config.frame_quant (S.fq); an instantiation of its own, so that the other engines run exactly the kernels they did.
+template <int kPhase, bool kZeroRef, int kMode, bool kFq = false>
 __global__ void __launch_bounds__(128) k_pvq_split(const __grid_constant__ Stage S, int cls, int chunk) {
   const daala_b200_pvq_params& prm = S.prm;
   const int lane = threadIdx.x & 31;
@@ -877,7 +886,7 @@ __global__ void __launch_bounds__(128) k_pvq_split(const __grid_constant__ Stage
   const int vs = cls == 2 ? 128 : 32;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < count; i += nwarps) {
-    const ItemGeom g = item_geom(prm, S.items[cls][first + i]);
+    const ItemGeom g = item_geom(prm, S.items[cls][first + i], kFq ? S.fq : nullptr);
     int16_t* vec = S.sp_vec[cls] + (size_t)i * 3 * vs;
     int32_t* lanes = S.sp_lanes[cls] + (size_t)i * kCtxLaneWords * 16;
     int32_t* uni = S.sp_uni[cls] + (size_t)i * kCtxUniWords;
@@ -928,7 +937,7 @@ __global__ void __launch_bounds__(128) k_pvq_prepass(const __grid_constant__ Sta
     const int blk = (int)(i / per), sel = (int)(i % per);
     const int band = kMode == 2 ? 7 + sel : (sel < 3 ? sel : sel + 1);
     if (band >= num_bands(prm.blocks[blk].bs)) continue;
-    const ItemGeom g = item_geom(prm, ((uint32_t)blk << 4) | band);
+    const ItemGeom g = item_geom(prm, ((uint32_t)blk << 4) | band, nullptr);
     BandCtx B;
     band_setup<kMode>(lane, B, prm.in + g.off, nullptr, g.bn, g.q, g.beta, prm.is_keyframe, g.pli, prm.qm + g.qoff,
                       prm.pvq_norm_lambda, S.rsqrt_tbl);
@@ -972,7 +981,7 @@ __global__ void __launch_bounds__(128, 4) k_pvq_levels(const __grid_constant__ S
     for (int phase = 0; phase < 3; phase++) {
       for (int i = w; i < n; i += nwarps) {
         const uint32_t item = S.lvl_items[base + i];
-        const ItemGeom g = item_geom(prm, item);
+        const ItemGeom g = item_geom(prm, item, nullptr);
         int16_t* vec = S.lv_vec + (size_t)i * 3 * vs;
         int32_t* lanes = S.lv_lanes + (size_t)i * kCtxLaneWords * 16;
         int32_t* uni = S.lv_uni + (size_t)i * kCtxUniWords;
@@ -1124,7 +1133,7 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
       if (!kInter) {
         prm.out[b.coef_off] = prm.in[b.coef_off];
       } else {
-        int dc_quant = (prm.q0 * prm.pvq_qm_q4[b.pli][b.bs * (b.bs + 1)]) >> 4;
+        int dc_quant = band_q(prm, S.fq, b.frame, b.pli, b.bs * (b.bs + 1));
         if (dc_quant < 1) dc_quant = 1;
         const int32_t r = prm.ref[b.coef_off], diff = prm.in[b.coef_off] - r;
         int qdc = 0;
@@ -1160,10 +1169,12 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
 // (the deringing kernel stores the u8 reconstruction itself).
 // thr[pl][f][sb] = table[pl][level[f][sb]].  P-frame finishing pass: `coded` (else NULL) flags the superblocks with a
 // coded 4x4 luma unit; the others are forced to level 0 (src/encode.c:2724-2738), and the level applied goes to
-// `applied`.
+// `applied`.  config.frame_quant: `frame_tbl` ([F][2][6], else NULL) holds each frame's table, the frame of superblock
+// i being i / nsb.
 __global__ void k_dering_thresholds(const uint8_t* __restrict__ level, int32_t* __restrict__ thr_luma,
                                     int32_t* __restrict__ thr_chroma, int n, int4 tl_lo, int2 tl_hi, int4 tc_lo, int2 tc_hi,
-                                    const uint8_t* __restrict__ coded = nullptr, uint8_t* __restrict__ applied = nullptr) {
+                                    const uint8_t* __restrict__ coded, uint8_t* __restrict__ applied,
+                                    const int32_t* __restrict__ frame_tbl, int nsb) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int tl[6] = {tl_lo.x, tl_lo.y, tl_lo.z, tl_lo.w, tl_hi.x, tl_hi.y};
@@ -1173,8 +1184,14 @@ __global__ void k_dering_thresholds(const uint8_t* __restrict__ level, int32_t* 
     if (!coded[i]) g = 0;
     applied[i] = (uint8_t)g;
   }
-  thr_luma[i] = tl[g];
-  thr_chroma[i] = tc[g];
+  if (frame_tbl) {
+    const int32_t* t = frame_tbl + (size_t)(i / nsb) * 12;
+    thr_luma[i] = t[g];
+    thr_chroma[i] = t[6 + g];
+  } else {
+    thr_luma[i] = tl[g];
+    thr_chroma[i] = tc[g];
+  }
 }
 
 // ---- P-frame finishing pass (config.inter_finish) ----------------------------------------------------------------
@@ -1198,6 +1215,7 @@ struct Fin {
   int nhsb, nvsb;
   int q0;
   uint8_t pvq_qm_q4[3][32];
+  const daala_b200_kf_frame_quant* fq;     // config.frame_quant: the step's records, which replace q0 / pvq_qm_q4
 };
 
 // block i of the two lists together (luma first), or false past their end
@@ -1224,7 +1242,8 @@ __global__ void __launch_bounds__(256) k_fin_patch(const __grid_constant__ Fin P
     const int32_t* src = (P.skip[list][blk] ? P.md[b.pli] : P.d[b.pli]) + o;
     const int32_t* mdp = P.md[b.pli] + o;
     int32_t* dst = P.out[b.pli] + o;
-    int dc_quant = (P.q0 * P.pvq_qm_q4[b.pli][b.bs * (b.bs + 1)]) >> 4;
+    const int qidx = b.bs * (b.bs + 1);
+    int dc_quant = P.fq ? (P.fq[b.frame].q0 * P.fq[b.frame].pvq_qm_q4[b.pli][qidx]) >> 4 : (P.q0 * P.pvq_qm_q4[b.pli][qidx]) >> 4;
     if (dc_quant < 1) dc_quant = 1;
     const int32_t dc0 = mdp[0] + P.dc[list][blk] * dc_quant;
     for (int k = lane; k < nn * nn; k += 32) {
@@ -1647,6 +1666,7 @@ struct Dering {
   const uint8_t* coded;            // nullable: superblocks with a coded luma 4x4 unit; the others get level 0 ...
   uint8_t* applied;                // ... and the level applied lands here
   int tbl[2][6];                   // luma / chroma threshold per level
+  const int32_t* frame_tbl;        // config.frame_quant: [F][2][6] tbl of each frame (replaces tbl), else NULL
   int32_t* thr[2];                 // luma / chroma threshold per superblock
   int32_t* dir;                    // [F][nvsb*8][nhsb*8]
   bool search;                     // the level search runs first, described by `sb`
@@ -1713,6 +1733,12 @@ struct daala_b200_kf {
   cudaGraphExec_t fin_exec;
   bool fin_captured;
   int fin_dc_limit;                // largest |dc| finish accepts: DAALA_B200_KF_FINISH_DC_LIMIT / the largest dc_quant
+                                   // (config.frame_quant: of the last step's records, set by submit)
+  // config.frame_quant: the step's records and the deringing threshold table of each frame ([F][2][6], computed on the
+  // host from the records' q0 as daala_b200_dering_threshold_table does), uploaded by submit
+  daala_b200_kf_frame_quant* fq;
+  int32_t* fq_tbl;
+  std::vector<int32_t> fq_tbl_host;
   // cfg.inter_mc with cfg.inter_finish: the pool slot of each frame's reconstruction (finish_io.ref_slot_out, -1 = not
   // stored) and the store that reads it
   int32_t* fin_slot_out;
@@ -1805,6 +1831,11 @@ static int kf_alloc(daala_b200_kf* kf) {
       B.ref_slot_next = kf->ref_slot_next;
       B.mv1 = kf->mv1_grid;
     }
+  }
+  if (kf->cfg.frame_quant) {
+    KF_CHECK(dalloc(kf, &kf->fq, (size_t)F));
+    KF_CHECK(dalloc(kf, &kf->fq_tbl, (size_t)F * 12));
+    kf->fq_tbl_host.assign((size_t)F * 12, 0);
   }
   KF_CHECK(dalloc(kf, &kf->qm, (size_t)2 * kf->cfg.qm_stride));
   KF_CHECK(dalloc(kf, &kf->qm_inv, (size_t)2 * kf->cfg.qm_stride));
@@ -1940,6 +1971,7 @@ static int kf_alloc(daala_b200_kf* kf) {
     p.use_masking = kf->cfg.use_masking;
     p.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
     memcpy(p.pvq_qm_q4, kf->cfg.pvq_qm_q4, sizeof(p.pvq_qm_q4));
+    S.fq = kf->fq;
     for (int c = 0; c < 3; c++) S.items[c] = chroma ? L.items_c[c] : L.items_l[c];
     S.cnt = L.cnt;
     S.rsqrt_tbl = kf->rsqrt_tbl;
@@ -2084,6 +2116,7 @@ static int kf_alloc(daala_b200_kf* kf) {
     B.qm_is_flat = kf->cfg.qm_is_flat;
     B.use_activity_masking = kf->cfg.use_masking;
     B.coded_quantizer = kf->cfg.coded_quantizer;
+    B.fq = kf->fq;
     if (kf->cfg.symbol_stream == 2) {
       Sym& Y = kf->sym;
       KF_CHECK(dalloc(kf, &Y.late_skip, (size_t)Y.cap_blocks));
@@ -2162,7 +2195,8 @@ static int kf_alloc(daala_b200_kf* kf) {
         const int dq = (P.q0 * P.pvq_qm_q4[p][bs * (bs + 1)]) >> 4;
         if (dq > dq_max) dq_max = dq;
       }
-    kf->fin_dc_limit = DAALA_B200_KF_FINISH_DC_LIMIT / dq_max;
+    kf->fin_dc_limit = DAALA_B200_KF_FINISH_DC_LIMIT / dq_max;   // config.frame_quant: replaced by each submit
+    P.fq = kf->fq;
     if (kf->cfg.inter_mc) {
       KF_CHECK(dalloc(kf, &kf->fin_slot_out, (size_t)F));
       PoolStore& W = kf->store;
@@ -2218,6 +2252,7 @@ static int kf_alloc(daala_b200_kf* kf) {
     D.coded = kf->fin_coded;
     D.applied = kf->fin_level;
     daala_b200_dering_threshold_table(kf->cfg.q0, D.tbl);
+    D.frame_tbl = kf->fq_tbl;
     D.search = dering == 2;
     if (D.search) {
       // src/encode.c:2708-2811 for every frame of the batch.  P frames (src/encode.c:2720-2811): the frame's own skip
@@ -2246,6 +2281,11 @@ static int kf_alloc(daala_b200_kf* kf) {
       KF_CHECK(dalloc(kf, &b.dist, nsb * 6));
       b.dir = D.dir;
       b.levels = D.level;   // what the thresholds read; on P frames its level 0 agrees with the forced one
+      if (kf->cfg.frame_quant) {
+        b.fq = kf->fq;
+        b.frame_tbl = kf->fq_tbl;
+        KF_CHECK(dalloc(kf, &b.cand_thr, nsb * 5));
+      }
     }
   }
   // dalloc's cudaMemset runs on the legacy default stream, asynchronously, and the engine's stream does not
@@ -2271,7 +2311,7 @@ static int enqueue_dering(daala_b200_kf* kf, const Dering& D, cudaStream_t s) {
   k_dering_thresholds<<<(kf->F * nsb + 255) / 256, 256, 0, s>>>(
       D.level, D.thr[0], D.thr[1], kf->F * nsb, make_int4(D.tbl[0][0], D.tbl[0][1], D.tbl[0][2], D.tbl[0][3]),
       make_int2(D.tbl[0][4], D.tbl[0][5]), make_int4(D.tbl[1][0], D.tbl[1][1], D.tbl[1][2], D.tbl[1][3]),
-      make_int2(D.tbl[1][4], D.tbl[1][5]), D.coded, D.applied);
+      make_int2(D.tbl[1][4], D.tbl[1][5]), D.coded, D.applied, D.frame_tbl, nsb);
   for (int p = 0; p < 3; p++) {
     const long long per = (long long)kf->plane_w[p] * kf->plane_h[p];
     daala_b200_dering_params dp;
@@ -2306,19 +2346,19 @@ static int dering_launches(const Dering& D) { return 1 + 1 + (D.search ? 5 + 6 +
 
 // Everything between "inputs are in HBM" and "results are in HBM", on kf->stream.
 // the three phase kernels over every chunk of every class of a stage's dependency-free lists
-template <bool kZeroRef>
+template <bool kZeroRef, bool kFq = false>
 static void enqueue_split(daala_b200_kf* kf, const Stage& S, cudaStream_t s) {
   const int grid = kf->sms * 16;
   for (int cls = 2; cls >= 0; cls--) {
     for (int chunk = 0; chunk < S.sp_chunks[cls]; chunk++) {
       if (cls == 2) {
-        k_pvq_split<0, kZeroRef, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
-        k_pvq_split<1, kZeroRef, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
-        k_pvq_split<2, kZeroRef, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<0, kZeroRef, 2, kFq><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<1, kZeroRef, 2><<<grid, 128, 0, s>>>(S, cls, chunk);   // the search reads no quantiser
+        k_pvq_split<2, kZeroRef, 2, kFq><<<grid, 128, 0, s>>>(S, cls, chunk);
       } else {
-        k_pvq_split<0, kZeroRef, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<0, kZeroRef, 1, kFq><<<grid, 128, 0, s>>>(S, cls, chunk);
         k_pvq_split<1, kZeroRef, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
-        k_pvq_split<2, kZeroRef, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<2, kZeroRef, 1, kFq><<<grid, 128, 0, s>>>(S, cls, chunk);
       }
     }
   }
@@ -2373,7 +2413,8 @@ static int kf_enqueue_step_inter(daala_b200_kf* kf, int phases) {
   for (const Stage* S : {&kf->luma, &kf->chroma}) {
     if (!(phases & (S == &kf->luma ? DAALA_B200_KF_PVQ_LUMA : DAALA_B200_KF_PVQ_CHROMA))) continue;
     if (!core) k_gather<kGatherInter><<<wide, 256, 0, s>>>(*S);
-    enqueue_split<false>(kf, *S, s);
+    if (S->fq) enqueue_split<false, true>(kf, *S, s);
+    else enqueue_split<false>(kf, *S, s);
     if (!core) k_finish_scatter<true><<<wide, 256, 0, s>>>(*S);
   }
   if (!core && (phases & DAALA_B200_KF_PVQ_CHROMA) && kf->cfg.late_skip) {
@@ -2500,6 +2541,11 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   if (cfg && cfg->late_skip && (cfg->late_skip != 1 || cfg->inter != 1)) {
     snprintf(g_create_err, sizeof(g_create_err),
              "daala_b200_kf_create: late_skip is 0 or 1, and 1 requires inter = 1 (keyframes have no late skip)");
+    return nullptr;
+  }
+  if (cfg && cfg->frame_quant && (cfg->frame_quant != 1 || cfg->inter != 1)) {
+    snprintf(g_create_err, sizeof(g_create_err),
+             "daala_b200_kf_create: frame_quant is 0 or 1, and 1 requires inter = 1 (a keyframe batch shares one quantizer)");
     return nullptr;
   }
   if (cfg && cfg->mc_refs < 0) {
@@ -2665,6 +2711,7 @@ int daala_b200_kf_device_buffers(daala_b200_kf* kf, daala_b200_kf_buffers* out) 
   out->mc_refs = kf->cfg.mc_refs;
   out->ref_slot_next = kf->ref_slot_next;
   out->mv1_grid = kf->mv1_grid;
+  out->frame_quant = kf->fq;
   return 0;
 }
 
@@ -2848,6 +2895,32 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", ls_why);
     return (int)cudaErrorInvalidValue;
   }
+  // per-frame quantizers: every record in range; then each frame's deringing thresholds and the finishing pass's DC
+  // limit of this step (daala_b200_kf_frame_quant_derive)
+  int fq_dc_limit = 0;
+  if (io->frame_quant || kf->cfg.frame_quant) {
+    const char* why = !kf->cfg.frame_quant ? "frame_quant needs an engine with frame_quant = 1"
+                      : !io->frame_quant  ? "frame_quant: the records ([nframes]) are required"
+                                          : nullptr;
+    for (int f = 0; !why && f < F; f++) {
+      const daala_b200_kf_frame_quant& r = io->frame_quant[f];
+      if (r.q0 < 1 || r.q0 > DAALA_B200_KF_MAX_Q0) why = "a record's q0 is outside [1, 8191]";
+      else if (r.coded_quantizer < 1 || r.coded_quantizer > 63) why = "a record's coded_quantizer is outside [1, 63]";
+      else if (!std::isfinite(r.dering_lambda) || r.dering_lambda < 0) why = "a record's dering_lambda is negative or not finite";
+      for (int p = 0; !why && p < 3; p++)
+        for (int i = 0; i < 30; i++)   // OD_QM_SIZE entries are read
+          if (r.pvq_qm_q4[p][i] < 1) {
+            why = "a record's pvq_qm_q4 entry is 0";
+            break;
+          }
+    }
+    if (why) {
+      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", why);
+      return (int)cudaErrorInvalidValue;
+    }
+    fq_dc_limit = daala_b200_kf_frame_quant_derive(io->frame_quant, F,
+                                                   reinterpret_cast<int32_t(*)[2][6]>(kf->fq_tbl_host.data()));
+  }
   // symbol stream: the engine must produce it, and every requested buffer must hold the worst case and be pinned
   SymCopy sc;
   memset(&sc, 0, sizeof(sc));
@@ -2923,6 +2996,10 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
                                cudaMemcpyHostToDevice, s));
     }
   }
+  if (kf->cfg.frame_quant) {
+    KF_CHECK(cudaMemcpyAsync(kf->fq, io->frame_quant, sizeof(daala_b200_kf_frame_quant) * F, cudaMemcpyHostToDevice, s));
+    KF_CHECK(cudaMemcpyAsync(kf->fq_tbl, kf->fq_tbl_host.data(), sizeof(int32_t) * 12 * F, cudaMemcpyHostToDevice, s));
+  }
   const size_t map_bytes = (size_t)kf->nhsb * 8 * kf->nvsb * 8 * F;
   KF_CHECK(cudaMemcpyAsync(kf->bsize, io->bsize, map_bytes, cudaMemcpyHostToDevice, s));
   if (kf->cfg.dering == 1) {
@@ -2940,6 +3017,7 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   }
   kf->have_step = true;
   kf->last_tot = tot;
+  if (kf->cfg.frame_quant) kf->fin_dc_limit = fq_dc_limit;
   for (int p = 0; p < 3; p++)
     if (io->pixels_out[p])
       KF_CHECK(cudaMemcpyAsync(io->pixels_out[p], kf->pixels_out[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
@@ -2979,6 +3057,19 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     KF_CHECK(cudaGetLastError());
   }
   return 0;
+}
+
+int daala_b200_kf_frame_quant_derive(const daala_b200_kf_frame_quant* rec, int n, int32_t (*tbl)[2][6]) {
+  int dq_max = 1;
+  for (int f = 0; f < n; f++) {
+    for (int p = 0; p < 3; p++)
+      for (int bs = 0; bs < 5; bs++) {
+        const int dq = (rec[f].q0 * rec[f].pvq_qm_q4[p][bs * (bs + 1)]) >> 4;
+        if (dq > dq_max) dq_max = dq;
+      }
+    if (tbl) daala_b200_dering_threshold_table(rec[f].q0, tbl[f]);
+  }
+  return DAALA_B200_KF_FINISH_DC_LIMIT / dq_max;
 }
 
 int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {

@@ -21,6 +21,9 @@ host coder takes the reference's late-skip decision (daala_b200/lateskip.py).
 With inter_mc=1 and mc_next=1 the engine predicts B frames: `ref_slot=` is [F, 3] (GOLD, PREV, NEXT) and `mv1_grid=`
 holds each vertex's second vector, which a vertex with ref 2 (NEXT) is predicted with (gop.py gives the reference's
 B-frame order and buffer rotation).
+With inter=1 and frame_quant=1 every frame of a batch has its own quantizer: `encode(..., frame_quant=)` takes one
+FRAME_QUANT_DTYPE record per frame (frame_quant_records builds them) in place of the engine-wide q0, coded_quantizer,
+dering_lambda and pvq_qm_q4, so P and B frames of different types or streams share one batch.
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -45,7 +48,28 @@ class Config(ctypes.Structure):
                 ("max_blocks_div", c_int), ("persist_ctas_per_sm", c_int), ("split_free", c_int), ("dering", c_int), ("noref_prepass", c_int), ("level_chains", c_int), ("stream", c_void_p),
                 ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
                 ("symbol_stream", c_int), ("inter", c_int), ("inter_mc", c_int), ("mc_refs", c_int),
-                ("inter_finish", c_int), ("late_skip", c_int), ("mc_next", c_int)]
+                ("inter_finish", c_int), ("late_skip", c_int), ("mc_next", c_int), ("frame_quant", c_int)]
+
+
+# daala_b200_kf_frame_quant: one frame's quantizer on a frame_quant engine
+FRAME_QUANT_DTYPE = np.dtype([("q0", "<i4"), ("coded_quantizer", "<i4"), ("dering_lambda", "<f8"),
+                              ("pvq_qm_q4", "u1", (3, 32))])
+MAX_Q0 = 8191   # od_codedquantizer_to_quantizer(63), the largest quantizer a record may carry
+
+
+def frame_quant_records(q0, coded_quantizer, dering_lambda=None, pvq_qm_q4=None):
+    """[F] FRAME_QUANT_DTYPE records from per-frame values: q0 and coded_quantizer [F]; dering_lambda [F] (None: each
+    frame's 0.67 * OD_PVQ_LAMBDA * q0^2, the engine's default, src/rate.c:1086); pvq_qm_q4 [F, 3, 30] or one [3, 30]
+    table for every frame (None: all 16)."""
+    q0 = np.atleast_1d(np.asarray(q0, np.int64))
+    rec = np.zeros(q0.shape[0], FRAME_QUANT_DTYPE)
+    rec["q0"] = q0
+    rec["coded_quantizer"] = np.broadcast_to(np.asarray(coded_quantizer, np.int64), q0.shape)
+    lam = 0.67 * pvq.PVQ_LAMBDA * q0.astype(np.float64) ** 2 if dering_lambda is None else dering_lambda
+    rec["dering_lambda"] = np.broadcast_to(np.asarray(lam, np.float64), q0.shape)
+    q4 = np.full((3, 30), 16, np.uint8) if pvq_qm_q4 is None else np.asarray(pvq_qm_q4, np.uint8)
+    rec["pvq_qm_q4"][:, :, :30] = np.broadcast_to(q4[..., :30], (q0.shape[0], 3, 30))
+    return rec
 
 
 class Totals(ctypes.Structure):
@@ -65,7 +89,8 @@ class IO(ctypes.Structure):
                 ("pred_pixels_out", c_void_p * 3), ("luma_dc_resid", c_void_p), ("chroma_dc_resid", c_void_p),
                 ("ref_resident", c_int), ("sym_dc", c_void_p), ("sym_dc_cap", c_ll),
                 ("luma_late_skip", c_void_p), ("chroma_late_skip", c_void_p), ("sym_late_skip", c_void_p),
-                ("sym_late_skip_cap", c_ll), ("ref_slot_next", c_void_p), ("mv1_grid", c_void_p)]
+                ("sym_late_skip_cap", c_ll), ("ref_slot_next", c_void_p), ("mv1_grid", c_void_p),
+                ("frame_quant", c_void_p)]
 
 
 class FinishIO(ctypes.Structure):
@@ -91,7 +116,7 @@ class Buffers(ctypes.Structure):
                 ("bytes_allocated", c_ll), ("pred_pixels", c_void_p * 3), ("pred_coeffs", c_void_p * 3),
                 ("luma_heads_raw", c_void_p), ("luma_head_bin", c_void_p), ("ref_pixels", c_void_p * 3),
                 ("ref_slot", c_void_p), ("mv_grid", c_void_p), ("mc_refs", c_int), ("ref_slot_next", c_void_p),
-                ("mv1_grid", c_void_p)]
+                ("mv1_grid", c_void_p), ("frame_quant", c_void_p)]
 
 
 def _bind():
@@ -115,6 +140,7 @@ def _bind():
     L.daala_b200_kf_finish.argtypes = [c_void_p, ctypes.POINTER(FinishIO)]
     L.daala_b200_kf_pool_load.argtypes = [c_void_p, c_int, ctypes.POINTER(c_void_p)]
     L.daala_b200_kf_symbol_bounds.argtypes = [ctypes.POINTER(Totals), c_int, ctypes.POINTER(SymBounds)]
+    L.daala_b200_kf_frame_quant_derive.argtypes = [c_void_p, c_int, c_void_p]
     L.daala_b200_kf_wait.argtypes = [c_void_p]
     L.daala_b200_device_copy.argtypes = [c_void_p, c_void_p, ctypes.c_size_t, c_int]
     L.daala_b200_host_alloc.argtypes = [ctypes.c_size_t]
@@ -123,6 +149,15 @@ def _bind():
     L.daala_b200_host_free.restype = None
     L._kf_bound = True
     return L
+
+
+def frame_quant_derive(records):
+    """What submit derives from a frame_quant step's records (daala_b200_kf_frame_quant_derive): each frame's
+    deringing thresholds [F, 2, 6] int32 (luma, chroma per level) and the finishing pass's DC limit."""
+    r = np.ascontiguousarray(records, FRAME_QUANT_DTYPE)
+    tbl = np.zeros((r.shape[0], 2, 6), np.int32)
+    limit = _bind().daala_b200_kf_frame_quant_derive(r.ctypes.data, r.shape[0], tbl.ctypes.data)
+    return tbl, int(limit)
 
 
 class Pinned:
@@ -150,7 +185,7 @@ class KeyframeEngine:
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
                  qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=0, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
                  qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0, inter_mc=0, mc_refs=0,
-                 inter_finish=0, late_skip=0, mc_next=0):
+                 inter_finish=0, late_skip=0, mc_next=0, frame_quant=0):
         self.L = _bind()
         self.geom, self.F = geom, nframes
         if qm is None:
@@ -193,6 +228,11 @@ class KeyframeEngine:
         # mc_next: B frames, a third picture (NEXT) per frame and the mv1 grid
         cfg.mc_next = int(mc_next)
         self.mc_next = int(mc_next)
+        # frame_quant: each step takes one FRAME_QUANT_DTYPE record per frame (encode(..., frame_quant=)); the config's
+        # q0, coded_quantizer, dering_lambda and pvq_qm_q4 are then not read
+        cfg.frame_quant = int(frame_quant)
+        self.frame_quant = int(frame_quant)
+        self._fq = None
         self.nrefs = 0
         self.resident = False
         self._pool_src = []
@@ -309,6 +349,18 @@ class KeyframeEngine:
             a = self._arr("grid1", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1, 2), np.int32)
             a[...] = mv1_grid
 
+    def stage_frame_quant(self, records):
+        """Copies the [F] FRAME_QUANT_DTYPE records of one batch into the host buffers (frame_quant engines; the C call
+        refuses them elsewhere).  None: the next step is submitted without records."""
+        if records is None:
+            self._fq = None
+            return
+        r = np.asarray(records)
+        if r.dtype != FRAME_QUANT_DTYPE or r.shape != (self.F,):
+            raise ValueError("frame_quant= is [%d] FRAME_QUANT_DTYPE records (frame_quant_records builds them)" % self.F)
+        self._fq = self._arr("fq", (self.F,), FRAME_QUANT_DTYPE)
+        self._fq[...] = r
+
     def stage_inputs(self, planes, bsize, pred=None):
         """Copies one batch into the engine's (pinned) host input buffers.  planes: per plane an array
         [F, h, w] u8 (padded geometry); bsize: [F, nvsb*8, nhsb*8]; pred (inter engines): the
@@ -401,6 +453,8 @@ class KeyframeEngine:
             out["luma_dc_resid"] = self._arr("ldr", (int(t.n_luma),), np.int32)
             out["chroma_dc_resid"] = self._arr("cdr", (int(t.n_chroma),), np.int32)
             io.luma_dc_resid, io.chroma_dc_resid = out["luma_dc_resid"].ctypes.data, out["chroma_dc_resid"].ctypes.data
+        if self._fq is not None:
+            io.frame_quant = self._fq.ctypes.data
         out["counts"] = self._arr("cnt", (32,), np.int32)
         io.counts = out["counts"].ctypes.data
         if self.dering:
@@ -432,6 +486,8 @@ class KeyframeEngine:
                                + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * mvgrid.MV_PT_DTYPE.itemsize)
             if self.mc_next:   # the NEXT slot of each frame and the mv1 of each vertex
                 self.h2d_bytes += 4 * self.F + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * 8
+        if self._fq is not None:   # the records and each frame's deringing threshold table (int32 [2][6])
+            self.h2d_bytes += self.F * (FRAME_QUANT_DTYPE.itemsize + 48)
         return out
 
     def submit(self):
@@ -454,10 +510,11 @@ class KeyframeEngine:
         return idx.nbytes + blocks * sym.BLOCK_DTYPE.itemsize + int(idx[:, 3].sum()) * 8 + int(idx[:, 5].sum()) + dc
 
     def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None, pred=None, refs=None,
-               ref_slot=None, mv_grid=None, resident=False, mv1_grid=None):
+               ref_slot=None, mv_grid=None, resident=False, mv1_grid=None, frame_quant=None):
         """One batch end to end through the C ABI with host buffers; returns the result arrays (views of
         the engine's host buffers: copy what must survive the next call).  pred: see stage_inputs; refs, ref_slot,
-        mv_grid, resident, mv1_grid (inter_mc engines, which also return the prediction as pred0..2): see stage_mc.  Raises
+        mv_grid, resident, mv1_grid (inter_mc engines, which also return the prediction as pred0..2): see stage_mc;
+        frame_quant (frame_quant engines, required there): [F] FRAME_QUANT_DTYPE records, see stage_frame_quant.  Raises
         when the batch exceeded the block capacity, or (inter_mc) when a used vertex names a picture other than GOLD /
         PREV (/ NEXT on mc_next engines) or a vector reaches past the reference's edge extension: the reference
         encoder's result is undefined there."""
@@ -467,6 +524,7 @@ class KeyframeEngine:
             self.stage_mc(refs, ref_slot, mv_grid, resident, mv1_grid)
         if self.dering == 1:
             self.stage_dering_levels(dering_levels)
+        self.stage_frame_quant(frame_quant)
         self.prepare_io(symbols, recon, stream)
         self.submit()
         out = self.wait()
@@ -591,9 +649,17 @@ class KeyframeEngine:
                     "kf_time_device")
         return float(ms.value)
 
-    def upload(self, planes, bsize, pred=None):
+    def upload(self, planes, bsize, pred=None, frame_quant=None):
+        """Copies one batch straight into the engine's device buffers for run_device; frame_quant (frame_quant
+        engines): the [F] FRAME_QUANT_DTYPE records the step's kernels read."""
         g = self.geom
         self._check_pred(pred)
+        if frame_quant is not None:
+            if not self.frame_quant:
+                raise ValueError("frame_quant= needs an engine created with frame_quant=1")
+            r = np.ascontiguousarray(frame_quant, FRAME_QUANT_DTYPE)
+            assert r.shape == (self.F,)
+            self._check(self.L.daala_b200_device_copy(self.buf.frame_quant, r.ctypes.data, r.nbytes, 0), "upload")
         for p in range(3):
             for dst, src in ((self.buf.pixels[p], planes[p]),) + (((self.buf.pred_pixels[p], pred[p]),) if pred is not None else ()):
                 a = np.ascontiguousarray(src, np.uint8)

@@ -14,6 +14,11 @@ goes to.  The reference decides this in three places, restated here:
 The encoder runs with OD_CLOSED_GOP = 0 and without rate control dropping frames (a dropped frame keeps the same
 rotation).  The buffer indices serve directly as pool slots of a device-resident sequence: sequence s uses slots
 4*s .. 4*s + 3.
+
+pipelined_steps groups one sequence's coded frames into engine steps, so that one sequence fills a batch (new
+scheduling, not the reference's): each step holds the next I / P anchor and the B frames coded just before it, which
+depend only on pictures finished in earlier steps.  The frames of such a step differ in type, so their quantizers differ
+too: the engine takes one quantizer record per frame (config.frame_quant).
 """
 from collections import namedtuple
 
@@ -89,3 +94,37 @@ def coding_order(nframes, b_frames, keyframe_rate=256):
         if kind != B_FRAME:
             ip_count += 1
     return out
+
+
+def pipelined_steps(frames):
+    """The coded frames of coding_order(...) as engine steps, in the order they run: [[Frame, ...], ...].
+
+    A P frame forms a step with the B frames coded just before it (the B frames between the two anchors before it),
+    all of which read only pictures that earlier steps finished.  An I frame is a step of its own (the keyframe engine,
+    whose picture the P-frame engine's pool takes with pool_load); the B frames coded before it form a step of their
+    own ahead of it, and so do B frames left at the end of the stream.  Inside a step every frame reads the pool before
+    any frame's reconstruction is stored, which is what lets an anchor's SELF buffer be one that the step's B frames
+    still read."""
+    steps, pending = [], []
+    for fr in frames:
+        if fr.type == B_FRAME:
+            pending.append(fr)
+        elif fr.type == I_FRAME:
+            if pending:
+                steps.append(pending)
+            steps.append([fr])
+            pending = []
+        else:
+            steps.append([fr] + pending)
+            pending = []
+    if pending:
+        steps.append(pending)
+    return steps
+
+
+def pool_slots(fr, base=0):
+    """The pool slots (GOLD, PREV, NEXT) an mc_next engine reads frame `fr` from, its sequence's buffers starting at
+    slot `base`.  A frame without a NEXT picture (every frame when b_frames = 0, and I / P frames, which never predict
+    from NEXT) names its PREV slot there."""
+    gold, prev, nxt = fr.refs[GOLD], fr.refs[PREV], fr.refs[NEXT]
+    return base + gold, base + prev, base + (nxt if nxt >= 0 and fr.type == B_FRAME else prev)

@@ -526,7 +526,27 @@ typedef struct daala_b200_kf_config {
                                   encoder leaves stale vectors there).  Nothing after the prediction differs from a P
                                   frame.  mc_refs = 0 then means 3 * nframes.  Requires inter_mc = 1; other values, and
                                   1 without inter_mc, are refused by daala_b200_kf_create */
+  int frame_quant;             /* 0 (default): nothing below exists; the engine is exactly the one without this field.
+                                  1: every frame of a step has its own quantizer: daala_b200_kf_io.frame_quant gives one
+                                  daala_b200_kf_frame_quant per frame, and the step and the finishing pass read no
+                                  per-frame field of this config (q0, coded_quantizer, dering_lambda, pvq_qm_q4).  The
+                                  stream settings use_masking, qm / qm_inv, qm_is_flat and pvq_norm_lambda stay
+                                  engine-wide: the frames of one batch must share them.  Requires inter = 1; other
+                                  values, and 1 without inter, are refused by daala_b200_kf_create */
 } daala_b200_kf_config;
+
+/* config.frame_quant = 1: the quantizer of one frame of a batch, what od_enc_rc_select_quantizers_and_lambdas
+   (reference src/rate.c:727-835, :1086) left in state / enc for that frame, and the pvq_qm_q4 table in force
+   (src/encode.c:3050-3075).  Submit refuses a record with q0 outside [1, 8191] (8191 = od_codedquantizer_to_quantizer(63):
+   lossless frames are not coded by the engine), coded_quantizer outside [1, 63], a dering_lambda that is negative or
+   not finite, or a pvq_qm_q4 entry of 0. */
+typedef struct daala_b200_kf_frame_quant {   /* 112 bytes, 8-byte aligned */
+  int32_t q0;                 /* max(1, state->quantizer) of this frame */
+  int32_t coded_quantizer;    /* state->coded_quantizer: od_compute_dist's scale */
+  double dering_lambda;       /* enc->dering_lambda of this frame */
+  uint8_t pvq_qm_q4[3][32];   /* state->pvq_qm_q4 in force for this frame */
+} daala_b200_kf_frame_quant;
+#define DAALA_B200_KF_MAX_Q0 8191
 
 /* One vertex of a P frame's MV grid, as od_mv_grid_pt (reference src/mc.h:73-84) holds it after od_mv_est. */
 typedef struct daala_b200_mv_pt {  /* 12 bytes */
@@ -683,6 +703,10 @@ typedef struct daala_b200_kf_io {
   const int32_t *ref_slot_next;         /* [nframes]: pool slot of each frame's NEXT picture */
   const int32_t *mv1_grid;              /* [nframes][nvsb*8 + 1][nhsb*8 + 1][2]: each vertex's mv1 (od_mv_grid_pt.mv1,
                                            src/mc.h:73-84) in 1/8 luma pixel, read only where ref == 2 */
+  /* config.frame_quant = 1 only (required there, refused otherwise): [nframes] records, frame f coded at
+     frame_quant[f].  They go to the device with the step's other inputs; the finishing pass after the step uses the
+     same records. */
+  const daala_b200_kf_frame_quant *frame_quant;
 } daala_b200_kf_io;
 
 /* The finishing pass of a P-frame batch (config.inter_finish), daala_b200_kf_finish: the host coder's per-block
@@ -691,13 +715,15 @@ typedef struct daala_b200_kf_io {
      skip = 0: the block's coefficients are those the step coded, with d[0] = md[0] + dc * dc_quant;
      skip = 1: d = md over the whole block (the PVQ skip of src/pvq_encoder.c:951-977, AC = prediction; the late
                skip of src/encode.c:1412-1450 is skip = 1 with dc = 0), then d[0] = md[0] + dc * dc_quant.
-   dc_quant = max(1, q0 * pvq_qm_q4[pli][bs * (bs + 1)] >> 4), the step's band-0 quantiser.  A block counts as
+   dc_quant = max(1, q0 * pvq_qm_q4[pli][bs * (bs + 1)] >> 4), the step's band-0 quantiser (config.frame_quant: the
+   block's frame's record).  A block counts as
    skipped in bskip when skip && dc == 0 (od_pvq_encode's return value with has_dc_skip, src/encode.c:1364-1371,
    :1690-1691).  Then the inverse, the split and superblock-edge postfilters (they ignore the skip flags without
    OD_DEBLOCKING, src/filter.c:1505-1509, :1596-1598) and the deringing of src/encode.c:2695-2842 with the given
    levels: a superblock none of whose 4x4 luma units is coded is forced to level 0 (:2724-2738), chroma thresholds
    are x0.6, od_dering reads the real skip map (src/dering.c:297-325).  |dc| must not exceed
-   DAALA_B200_KF_FINISH_DC_LIMIT / DQ, DQ the largest dc_quant of the engine over planes and block sizes, so that
+   DAALA_B200_KF_FINISH_DC_LIMIT / DQ, DQ the largest dc_quant of the engine over planes and block sizes (with
+   config.frame_quant: of the last step, over its records, planes and block sizes), so that
    dc * dc_quant stays within 2^30 and md[0] + dc * dc_quant within od_coeff.  The pass equals the reference bit for
    bit while every sample of the reconstruction before deringing (state->ctmp, after the superblock-edge postfilter)
    fits int16, as it always does for 8-bit content with decisions near the step's own DC indices: the pass keeps that
@@ -770,6 +796,7 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
   int mc_refs;                          /* pictures the pool holds (0 without inter_mc) */
   int32_t *ref_slot_next;               /* config.mc_next: the NEXT slots ([nframes]) and the mv1 grids */
   int32_t *mv1_grid;                    /* ([nframes][nvsb*8 + 1][nhsb*8 + 1][2]); NULL otherwise */
+  daala_b200_kf_frame_quant *frame_quant;   /* config.frame_quant: the step's records ([nframes]); NULL otherwise */
 } daala_b200_kf_buffers;
 
 #define DAALA_B200_KF_LISTS 1
@@ -813,8 +840,16 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    `counts` the leaf corners whose vertex has a ref other than 0 or 1 (counts[19]; with mc_next other than 0, 1 or 2)
    and the corner windows (with the 6-tap filter's apron of -2..+3 pixels) that reach more than 64 luma / 32 chroma
    pixels outside the plane (counts[20]; with mc_next the window of the vector the corner reads, mv1 on NEXT
-   vertices), where the reference encoder's result is undefined. */
+   vertices), where the reference encoder's result is undefined.  With config.frame_quant it refuses a NULL
+   frame_quant and a record out of range (see daala_b200_kf_frame_quant); frame_quant given to an engine without
+   config.frame_quant is refused. */
 int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
+/* What submit derives on the host from the n records of a config.frame_quant step (no GPU involved, no validation):
+   tbl[f][0][g] / tbl[f][1][g] (nullable) the luma / chroma deringing threshold of level g for frame f,
+   (int)(OD_DERING_GAIN_TABLE[g] * q0^0.84182) and the same times 0.6 (reference src/encode.c:2694, :2822) with that
+   frame's q0; the return value is the finishing pass's DC limit for the step, DAALA_B200_KF_FINISH_DC_LIMIT / the
+   largest dc_quant over the records, planes and block sizes. */
+int daala_b200_kf_frame_quant_derive(const daala_b200_kf_frame_quant *rec, int n, int32_t (*tbl)[2][6]);
 /* The finishing pass (config.inter_finish, see daala_b200_kf_finish_io) on the last submitted step: H2D of the
    decisions and levels, the pass's kernels as one CUDA graph (captured at the first call; with config.inter_finish
    = 2 it includes the level search), D2H of the requested outputs; enqueued on the engine's stream like submit,
