@@ -26,8 +26,8 @@ extern "C" {
 int daala_b200_launch_forward(const FrameXformParams* prm, int nplanes, cudaStream_t stream);
 int daala_b200_launch_forward_no_tma(const FrameXformParams* prm, int nplanes, cudaStream_t stream);
 int daala_b200_launch_inverse(const FrameXformParams* prm, int nplanes, cudaStream_t stream);
-int daala_b200_launch_inverse_lapped_only(const FrameXformParams* prm, int nplanes, cudaStream_t stream);
-int daala_b200_launch_sb_postfilter_store(const FrameXformParams* prm, int nplanes, cudaStream_t stream);
+int daala_b200_launch_inverse_lapped_only(const FrameXformParams* prm, int plane0, int nplanes, cudaStream_t stream);
+int daala_b200_launch_sb_postfilter_store(const FrameXformParams* prm, int plane0, int nplanes, cudaStream_t stream);
 int daala_b200_launch_plane_sb_filter(int32_t* c, int stride, int nhsb, int nvsb, int xdec, int ydec,
                                       int post, cudaStream_t stream);
 int daala_b200_launch_block_transform(int32_t* blocks, int count, int ln, int mode, cudaStream_t stream);
@@ -489,10 +489,10 @@ int daala_b200_inverse_frame(const daala_b200_frame* f, int nplanes, void* strea
   return daala_b200_launch_inverse(f, nplanes, (cudaStream_t)stream);
 }
 int daala_b200_inverse_frame_lapped(const daala_b200_frame* f, int nplanes, void* stream) {
-  return daala_b200_launch_inverse_lapped_only(f, nplanes, (cudaStream_t)stream);
+  return daala_b200_launch_inverse_lapped_only(f, 0, nplanes, (cudaStream_t)stream);
 }
 int daala_b200_sb_postfilter_store_frame(const daala_b200_frame* f, int nplanes, void* stream) {
-  return daala_b200_launch_sb_postfilter_store(f, nplanes, (cudaStream_t)stream);
+  return daala_b200_launch_sb_postfilter_store(f, 0, nplanes, (cudaStream_t)stream);
 }
 int daala_b200_plane_sb_filter(int32_t* c, int stride, int nhsb, int nvsb, int xdec, int ydec, int post,
                                void* stream) {

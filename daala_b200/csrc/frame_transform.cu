@@ -883,15 +883,28 @@ int daala_b200_launch_inverse(const FrameXformParams* prm, int nplanes, cudaStre
   return (int)cudaGetLastError();
 }
 
-int daala_b200_launch_inverse_lapped_only(const FrameXformParams* prm, int nplanes, cudaStream_t stream) {
+// The kernels take their plane from blockIdx.y: planes [plane0, plane0 + nplanes) of prm become planes
+// [0, nplanes) of the launch's copy.
+static FrameXformParams plane_range(const FrameXformParams* prm, int plane0) {
+  FrameXformParams q = *prm;
+  for (int p = 0; p + plane0 < 3; p++) {
+    q.plane[p] = prm->plane[plane0 + p];
+    q.post16[p] = prm->post16[plane0 + p];
+  }
+  return q;
+}
+
+int daala_b200_launch_inverse_lapped_only(const FrameXformParams* prm, int plane0, int nplanes, cudaStream_t stream) {
+  if (plane0 < 0 || nplanes < 1 || plane0 + nplanes > 3) return (int)cudaErrorInvalidValue;
   dim3 grid(prm->nhsb * prm->sb_rows, nplanes, prm->nframes);
-  k_inverse_sb<<<grid, kThreads, 0, stream>>>(*prm);
+  k_inverse_sb<<<grid, kThreads, 0, stream>>>(plane_range(prm, plane0));
   return (int)cudaGetLastError();
 }
 
-int daala_b200_launch_sb_postfilter_store(const FrameXformParams* prm, int nplanes, cudaStream_t stream) {
+int daala_b200_launch_sb_postfilter_store(const FrameXformParams* prm, int plane0, int nplanes, cudaStream_t stream) {
+  if (plane0 < 0 || nplanes < 1 || plane0 + nplanes > 3) return (int)cudaErrorInvalidValue;
   dim3 grid(prm->nhsb * prm->sb_rows, nplanes, prm->nframes);
-  k_sb_postfilter_store<<<grid, kPostThreads, 0, stream>>>(*prm);
+  k_sb_postfilter_store<<<grid, kPostThreads, 0, stream>>>(plane_range(prm, plane0));
   return (int)cudaGetLastError();
 }
 

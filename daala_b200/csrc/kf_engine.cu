@@ -92,6 +92,9 @@ struct Lists {
   int ntiles;
   int4* tile_sum;                  // [ntiles] then exclusive prefixes in place
   int32_t* unit_lbase;             // [F*UH*UW] index of the first luma block whose origin is in the unit
+  // keyframes: [F*UH*UW] coding offset of the first luma block of a unit with block origins (the CfL source of its
+  // chroma blocks); kept from the last step that listed them, zero before; NULL on inter engines
+  int32_t* unit_loff;
   daala_b200_pvq_block* luma;
   daala_b200_pvq_block* chroma;
   int32_t* dep_top;                // same-size neighbour above / to the left (od_hv_intra_pred), or -1
@@ -243,6 +246,7 @@ __global__ void __launch_bounds__(kTile) k_unit_emit(const __grid_constant__ Lis
   L.unit_lbase[((long long)f * L.UH + uy) * L.UW + ux] = pre.x;
   if (v.x == 0) return;
   if (pre.x + v.x > L.max_luma || 2 * (pre.z + v.z) > L.max_chroma) return;   // flagged by k_tile_scan
+  if (L.unit_loff) L.unit_loff[((long long)f * L.UH + uy) * L.UW + ux] = pre.y;
   if (b == 0) {
     for (int q = 0; q < 4; q++)
       put_block(L.luma + pre.x + q, pre.y + 16 * q, ux * 8 + (q & 1) * 4, uy * 8 + (q >> 1) * 4, 0, 0, 0, f);
@@ -525,9 +529,11 @@ struct Stage {
   int skip_lo;                     // the persistent kernel leaves the dependency-free lists to the split path
   const double* rsqrt_tbl;         // [kTableDoubles] the reference's 1/sqrt(i) and theta-rate terms (pvq_fill_rsqrt_table)
   int16_t* res_pack;               // [nblocks*9][4]: gain, itheta, max_theta, k (what the coder reads)
-  const int32_t* cfl_plane;        // chroma: prediction plane (chroma geometry), else NULL
-  long long cfl_pitch;
-  int cfl_stride;
+  // keyframe chroma: the CfL source, the luma stage's coding-order input (its DC) and output (the quantised
+  // coefficients), and Lists::unit_loff; NULL otherwise
+  const int32_t* cfl_in;
+  const int32_t* cfl_out;
+  const int32_t* cfl_loff;
   int32_t* dc_resid;               // config.inter_finish or symbol_stream = 2: per block in[0] - ref[0], else NULL
   const daala_b200_kf_frame_quant* fq;   // config.frame_quant: [F] the step's records (band_q), else NULL
 #ifdef DAALA_B200_CHAIN_TRACE
@@ -576,6 +582,36 @@ __device__ __noinline__ void trace_item(const Stage& S, uint32_t item, int kind,
 }
 #endif
 
+// OD_CFL_SCALING4 (src/intra.c), indexed [column][row]
+__constant__ int kCflScaling4[4][4] = {{128, 128, 100, 36}, {128, 80, 71, 35}, {100, 71, 35, 31}, {36, 35, 31, 18}};
+
+// Chroma-from-luma reference of coefficient i (coding order) of keyframe chroma block b (od_resample_luma_coeffs,
+// src/intra.c:72), read from the luma stage's coding-order buffers; `lo` is the coding offset of the co-located luma.
+// Every block size codes the same nested layout (scan_rc does not depend on it) and a chroma block codes no more
+// coefficients than its luma block (512 at most), so chroma index i is luma index i.  Position 0 is the luma DC of
+// the plane k_finish_scatter writes on keyframes, the unquantised Haar DC in[0].
+__device__ __forceinline__ int32_t cfl_ref(const Stage& S, const daala_b200_pvq_block& b, int lo, int i) {
+  if (!(b.xdec & 0x80)) return i == 0 ? S.cfl_in[lo] : S.cfl_out[lo + i];
+  // four 4x4 luma blocks (k_unit_emit: block q = 2 row + column, coefficients at lo + 16 q) -> one 4x4 chroma
+  // prediction: od_tf_up_hv_lp (src/tf.c:82) + OD_CFL_SCALING4.  Output (r, c) comes from sample (r >> 1, c >> 1)
+  // of each luma block; kScan4 lists rasters 4, 1, 5 first, so sample (y, x) of a 4x4 block is coefficient y + 2 x.
+  int r = 0, c = 0;
+  if (i) scan_rc(i, &r, &c);
+  const int y = r >> 1, x = c >> 1, at = y + 2 * x;
+  int ll = at ? S.cfl_out[lo + at] : S.cfl_in[lo];
+  int lh = at ? S.cfl_out[lo + 16 + at] : S.cfl_in[lo + 16];
+  int hl = at ? S.cfl_out[lo + 32 + at] : S.cfl_in[lo + 32];
+  int hh = at ? S.cfl_out[lo + 48 + at] : S.cfl_in[lo + 48];
+  ll += lh; hh -= hl;
+  const int t = (ll - hh) >> 1;
+  hl = t - hl; lh = t - lh;
+  ll -= hl; hh += lh;
+  // (2y + vs, 2x + hs) <- ll, (2y + vs, 2x + 1 - hs) <- lh, (2y + 1 - vs, 2x + hs) <- hl, the rest <- hh, with
+  // vs = y, hs = x: the first kind of row is r = 3y, of column c = 3x
+  const int v = r == 3 * y ? (c == 3 * x ? ll : lh) : (c == 3 * x ? hl : hh);
+  return (kCflScaling4[c][r] * v + 64) >> 7;
+}
+
 // raster -> coding order of every block (od_raster_to_coding_order, src/partition.c:123); keyframe chroma:
 // also the CfL prediction and its sign flip (src/pvq_encoder.c:847-871); inter frames, all planes alike: the
 // reference vector is the transformed prediction md (prm.pred_plane), never flipped.  One warp per block.
@@ -604,13 +640,15 @@ __global__ void __launch_bounds__(256) k_gather(const __grid_constant__ Stage S)
         vref[i] = psrc[at];
       }
     } else {
-      const int32_t* psrc = S.cfl_plane + b.frame * S.cfl_pitch + (size_t)b.y0 * S.cfl_stride + b.x0;
+      // the co-located luma at (2 x0, 2 y0): the unit of the block's origin (4x4 chroma samples) has its offset
+      const int lo = S.cfl_loff[b.frame * (prm.plane_frame_pitch[b.pli] >> 4) + (long long)(b.y0 >> 2) * (stride >> 2) +
+                                (b.x0 >> 2)];
       int32_t* vref = prm.ref + b.coef_off;
       const int qoff = prm.qm_stride + ((((1 << (2 * b.bs)) - 1) << 4) / 3);
       int32_t xy = 0;
       for (int i = lane; i < len; i += 32) {
         const int32_t vi = i == 0 ? src[0] : src[scan_to_raster(i, ln, stride)];
-        const int32_t vr = i == 0 ? psrc[0] : psrc[scan_to_raster(i, ln, S.cfl_stride)];
+        const int32_t vr = cfl_ref(S, b, lo, i);
         vin[i] = vi;
         vref[i] = vr;
         if (i >= 1 && i < 16) {
@@ -627,50 +665,6 @@ __global__ void __launch_bounds__(256) k_gather(const __grid_constant__ Stage S)
         for (int i = 1 + lane; i < end; i += 32) vref[i] = -vref[i];
       }
       if (lane == 0) prm.res_flip[blk] = flip;
-    }
-  }
-}
-
-// Chroma-from-luma prediction planes (od_resample_luma_coeffs, src/intra.c:72): see k_cfl_pred of
-// pvq_kernels.cu; here with the block count on the device.  One warp per chroma block of plane 1
-// (plane 2 shares the prediction).
-__global__ void __launch_bounds__(256) k_cfl_plane(const __grid_constant__ Stage S, int32_t* pred_plane) {
-  const daala_b200_pvq_params& prm = S.prm;
-  const int n = min(S.cnt[S.n_blocks_at], S.max_blocks);
-  const int lane = threadIdx.x & 31;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (int blk = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; blk < n; blk += nwarps) {
-    const daala_b200_pvq_block b = prm.blocks[blk];
-    if (b.pli != 1) continue;
-    const int nn = 4 << b.bs;
-    const int lstride = prm.plane_stride[0];
-    const int32_t* luma = prm.coef_plane[0] + b.frame * prm.plane_frame_pitch[0] + (size_t)(2 * b.y0) * lstride + 2 * b.x0;
-    int32_t* dst = pred_plane + b.frame * S.cfl_pitch + (size_t)b.y0 * S.cfl_stride + b.x0;
-    if (b.xdec & 0x80) {
-      // four 4x4 luma blocks -> one 4x4 chroma prediction: od_tf_up_hv_lp (src/tf.c:82) + OD_CFL_SCALING4
-      const int scaling4[4][4] = {{128, 128, 100, 36}, {128, 80, 71, 35}, {100, 71, 35, 31}, {36, 35, 31, 18}};
-      if (lane < 4) {
-        const int x = lane & 1, y = lane >> 1;
-        int ll = luma[(size_t)y * lstride + x], lh = luma[(size_t)y * lstride + x + 4];
-        int hl = luma[(size_t)(y + 4) * lstride + x], hh = luma[(size_t)(y + 4) * lstride + x + 4];
-        ll += lh; hh -= hl;
-        const int t = (ll - hh) >> 1;
-        hl = t - hl; lh = t - lh;
-        ll -= hl; hh += lh;
-        const int hs = x & 1, vs = y & 1;
-        int r, c;
-        r = 2 * y + vs; c = 2 * x + hs;         dst[(size_t)r * S.cfl_stride + c] = (scaling4[c][r] * ll + 64) >> 7;
-        r = 2 * y + vs; c = 2 * x + 1 - hs;     dst[(size_t)r * S.cfl_stride + c] = (scaling4[c][r] * lh + 64) >> 7;
-        r = 2 * y + 1 - vs; c = 2 * x + hs;     dst[(size_t)r * S.cfl_stride + c] = (scaling4[c][r] * hl + 64) >> 7;
-        r = 2 * y + 1 - vs; c = 2 * x + 1 - hs; dst[(size_t)r * S.cfl_stride + c] = (scaling4[c][r] * hh + 64) >> 7;
-      }
-    } else {
-      // only the coded prefix is ever read; copying the whole low-frequency quarter keeps this simple
-      const int lim = nn > 32 ? 32 : nn;
-      for (int i = lane; i < lim * lim; i += 32) {
-        const int r = i / lim, c = i % lim;
-        dst[(size_t)r * S.cfl_stride + c] = luma[(size_t)r * lstride + c];
-      }
     }
   }
 }
@@ -1086,10 +1080,12 @@ __global__ void k_fill_rsqrt(double* tbl) {
   if (i < kTableDoubles) pvq_fill_rsqrt_table(tbl, i);
 }
 
-// Start of a PVQ stage: the tickets; the chain queue starts with the heads.
-__global__ void k_begin_pvq(int32_t* cnt, int luma) {
+// Start of the PVQ stages in `stages` (kBeginLuma | kBeginChroma): the tickets; the chain queue starts with the
+// heads.  Neither stage touches the other's tickets, so the whole step starts both at once.
+enum { kBeginLuma = 1, kBeginChroma = 2 };
+__global__ void k_begin_pvq(int32_t* cnt, int stages) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
-    if (luma) {
+    if (stages & kBeginLuma) {
       cnt[kHeadLoL] = 0;
       cnt[kHeadHi] = 0;
       cnt[kTailHi] = cnt[kNHeads0];
@@ -1099,9 +1095,8 @@ __global__ void k_begin_pvq(int32_t* cnt, int luma) {
 #ifdef DAALA_B200_CHAIN_TRACE
       cnt[kTraceN] = 0;
 #endif
-    } else {
-      cnt[kHeadLoC] = 0;
     }
+    if (stages & kBeginChroma) cnt[kHeadLoC] = 0;
   }
 }
 
@@ -1651,8 +1646,10 @@ using namespace daala_b200::kf;
 
 extern "C" int daala_b200_launch_forward(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
 extern "C" int daala_b200_launch_inverse(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
-extern "C" int daala_b200_launch_inverse_lapped_only(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
-extern "C" int daala_b200_launch_sb_postfilter_store(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
+extern "C" int daala_b200_launch_inverse_lapped_only(const daala_b200_frame* prm, int plane0, int nplanes,
+                                                     cudaStream_t stream);
+extern "C" int daala_b200_launch_sb_postfilter_store(const daala_b200_frame* prm, int plane0, int nplanes,
+                                                     cudaStream_t stream);
 
 // One deringing pass over the batch (od_encode_coefficients' final application, src/encode.c:2812-2842): the step's on
 // keyframes (config.dering) or the finishing pass's on P frames (config.inter_finish).  The two differ only in the data
@@ -1673,12 +1670,17 @@ struct Dering {
   daala_b200_dering_search_batch sb;
 };
 
+// The events of kf_enqueue_step_forked, one per fork or join.
+enum { kEvLists, kEvForward, kEvLumaBands, kEvLumaScatter, kEvChroma, kNumEvents };
+
 struct daala_b200_kf {
   daala_b200_kf_config cfg;
   int nhsb, nvsb, F;
   int plane_w[3], plane_h[3];
   cudaStream_t stream;
   bool own_stream;
+  cudaStream_t side;               // keyframe engines: the second branch of the forked step (engine-owned, highest priority)
+  cudaEvent_t ev[kNumEvents];
   cudaGraph_t graph;
   cudaGraphExec_t exec;
   bool captured;
@@ -1690,7 +1692,6 @@ struct daala_b200_kf {
   uint8_t* pred_pixels[3];         // cfg.inter: the prediction planes and their transform md
   int32_t* pred_coeffs[3];
   uint8_t* bsize;
-  int32_t* cfl_plane;
   int16_t *qm, *qm_inv;
   double* rsqrt_tbl;
   int16_t* sp_vec[3];
@@ -1802,7 +1803,6 @@ static int kf_alloc(daala_b200_kf* kf) {
   }
   const int UW = kf->nhsb * 8, UH = kf->nvsb * 8;
   KF_CHECK(dalloc(kf, &kf->bsize, (size_t)F * UW * UH));
-  if (!inter) KF_CHECK(dalloc(kf, &kf->cfl_plane, (size_t)kf->plane_w[1] * kf->plane_h[1] * F));
   if (kf->cfg.inter_mc) {
     daala_b200_mc_batch& B = kf->mc;
     const size_t nsb = (size_t)kf->nhsb * kf->nvsb;
@@ -1862,6 +1862,7 @@ static int kf_alloc(daala_b200_kf* kf) {
   L.max_chroma = (int)(nunits * 2 / div) + 64;
   KF_CHECK(dalloc(kf, &L.tile_sum, (size_t)L.ntiles));
   KF_CHECK(dalloc(kf, &L.unit_lbase, (size_t)F * UW * UH));
+  if (!inter) KF_CHECK(dalloc(kf, &L.unit_loff, (size_t)F * UW * UH));
   KF_CHECK(dalloc(kf, &L.luma, (size_t)L.max_luma));
   KF_CHECK(dalloc(kf, &L.chroma, (size_t)L.max_chroma));
   // the intra dependency structure (neighbours, chain heads, ring) is a keyframe matter
@@ -2020,10 +2021,6 @@ static int kf_alloc(daala_b200_kf* kf) {
       S.heads0 = L.heads0;
       KF_CHECK(dalloc(kf, &S.ring, inter ? 0 : kf->chain_cap));
       KF_CHECK(dalloc(kf, &S.join0, ndep));
-    } else {
-      S.cfl_plane = kf->cfl_plane;
-      S.cfl_pitch = (long long)kf->plane_w[1] * kf->plane_h[1];
-      S.cfl_stride = kf->plane_w[1];
     }
     return 0;
   };
@@ -2031,6 +2028,12 @@ static int kf_alloc(daala_b200_kf* kf) {
   if (rc) return rc;
   rc = setup_stage(kf->chroma, true);
   if (rc) return rc;
+  if (!inter) {
+    Stage& C = kf->chroma;
+    C.cfl_in = kf->luma.prm.in;
+    C.cfl_out = kf->luma.prm.out;
+    C.cfl_loff = L.unit_loff;
+  }
   (void)luma_px;
   // the unquantised DC residual per block: what the host's od_rdo_quant needs, returned classically (inter_finish) or
   // in the stream's DC records (symbol_stream = 2)
@@ -2298,51 +2301,68 @@ static int kf_alloc(daala_b200_kf* kf) {
   return 0;
 }
 
-// The deringing pass D over the whole batch: iDCT + split postfilters -> lapped planes; SB-edge postfilter -> etmp
-// (int16, the fused kernel's optional output); [the level search -> D.level]; thresholds per superblock; od_dering of
-// all frames per plane in one launch, luma first (it writes the direction map chroma reads), storing the u8
-// reconstruction.
-static int enqueue_dering(daala_b200_kf* kf, const Dering& D, cudaStream_t s) {
-  int rc = daala_b200_launch_inverse_lapped_only(&D.frame, 3, s);
-  if (!rc) rc = daala_b200_launch_sb_postfilter_store(&D.frame, 3, s);
-  if (!rc && D.search) rc = daala_b200_dering_search_enqueue(&D.sb, s);
-  if (rc) return rc;
+// Inverse of planes [p0, p0 + n): iDCT + split postfilters -> lapped planes; SB-edge postfilter -> the u8 planes, or
+// etmp (int16) when frame.post16 is set (the deringing stage's input).
+static int enqueue_recon(const daala_b200_frame& frame, int p0, int n, cudaStream_t s) {
+  const int rc = daala_b200_launch_inverse_lapped_only(&frame, p0, n, s);
+  return rc ? rc : daala_b200_launch_sb_postfilter_store(&frame, p0, n, s);
+}
+
+// od_dering of all frames of plane p in one launch, storing the u8 reconstruction.
+static int enqueue_dering_plane(daala_b200_kf* kf, const Dering& D, int p, cudaStream_t s) {
+  const int nsb = kf->nhsb * kf->nvsb;
+  const long long per = (long long)kf->plane_w[p] * kf->plane_h[p];
+  daala_b200_dering_params dp;
+  memset(&dp, 0, sizeof(dp));
+  dp.y = nullptr;   // u8 output only
+  dp.x = D.frame.post16[p];
+  dp.dir = D.dir;
+  dp.bskip = D.skip[p];
+  dp.sb_threshold = D.thr[p ? 1 : 0];
+  dp.ystride = dp.xstride = kf->plane_w[p];
+  dp.dir_stride = kf->nhsb * 8;
+  dp.skip_stride = D.skip_stride;
+  dp.nhsb = kf->nhsb;
+  dp.nvsb = kf->nvsb;
+  dp.xdec = p ? 1 : 0;
+  dp.pli = p;
+  dp.overlap = 1;      // OD_DERING_CHECK_OVERLAP
+  dp.coeff_shift = 4;  // OD_COEFF_SHIFT
+  // after a search the direction map is already there, packed with the variance; neither depends on the skip map
+  // (src/dering.c:280-287)
+  dp.dir_format = D.search ? 2 : 0;
+  return daala_b200_dering_plane_frames(&dp, kf->F, per, per, (long long)nsb * 64, nsb, D.skip_pitch[p],
+                                        D.frame.plane[p].pixels_out, s);
+}
+
+// The deringing pass D after the inverse: [the level search -> D.level]; thresholds per superblock (both plane
+// kinds); od_dering of plane 0, which writes the direction map the chroma planes read.
+static int enqueue_dering_luma(daala_b200_kf* kf, const Dering& D, cudaStream_t s) {
+  if (D.search) {
+    const int rc = daala_b200_dering_search_enqueue(&D.sb, s);
+    if (rc) return rc;
+  }
   const int nsb = kf->nhsb * kf->nvsb;
   k_dering_thresholds<<<(kf->F * nsb + 255) / 256, 256, 0, s>>>(
       D.level, D.thr[0], D.thr[1], kf->F * nsb, make_int4(D.tbl[0][0], D.tbl[0][1], D.tbl[0][2], D.tbl[0][3]),
       make_int2(D.tbl[0][4], D.tbl[0][5]), make_int4(D.tbl[1][0], D.tbl[1][1], D.tbl[1][2], D.tbl[1][3]),
       make_int2(D.tbl[1][4], D.tbl[1][5]), D.coded, D.applied, D.frame_tbl, nsb);
-  for (int p = 0; p < 3; p++) {
-    const long long per = (long long)kf->plane_w[p] * kf->plane_h[p];
-    daala_b200_dering_params dp;
-    memset(&dp, 0, sizeof(dp));
-    dp.y = nullptr;   // u8 output only
-    dp.x = D.frame.post16[p];
-    dp.dir = D.dir;
-    dp.bskip = D.skip[p];
-    dp.sb_threshold = D.thr[p ? 1 : 0];
-    dp.ystride = dp.xstride = kf->plane_w[p];
-    dp.dir_stride = kf->nhsb * 8;
-    dp.skip_stride = D.skip_stride;
-    dp.nhsb = kf->nhsb;
-    dp.nvsb = kf->nvsb;
-    dp.xdec = p ? 1 : 0;
-    dp.pli = p;
-    dp.overlap = 1;      // OD_DERING_CHECK_OVERLAP
-    dp.coeff_shift = 4;  // OD_COEFF_SHIFT
-    // after a search the direction map is already there, packed with the variance; neither depends on the skip map
-    // (src/dering.c:280-287)
-    dp.dir_format = D.search ? 2 : 0;
-    rc = daala_b200_dering_plane_frames(&dp, kf->F, per, per, (long long)nsb * 64, nsb, D.skip_pitch[p],
-                                        D.frame.plane[p].pixels_out, s);
-    if (rc) return rc;
-  }
-  return 0;
+  return enqueue_dering_plane(kf, D, 0, s);
 }
 
-// Kernel launches of enqueue_dering: inverse, SB postfilter -> int16, [level search: 5 filtered candidates, 6 packs,
-// 6 distortion passes, decision], thresholds, dering + u8 store per plane.
-static int dering_launches(const Dering& D) { return 1 + 1 + (D.search ? 5 + 6 + 6 + 1 : 0) + 1 + 3; }
+// The deringing pass D over the whole batch on one stream: inverse of all planes, then enqueue_dering_luma, then
+// od_dering of the chroma planes.
+static int enqueue_dering(daala_b200_kf* kf, const Dering& D, cudaStream_t s) {
+  int rc = enqueue_recon(D.frame, 0, 3, s);
+  if (!rc) rc = enqueue_dering_luma(kf, D, s);
+  for (int p = 1; !rc && p < 3; p++) rc = enqueue_dering_plane(kf, D, p, s);
+  return rc;
+}
+
+// Kernel launches of enqueue_dering with the inverse in `parts` plane ranges: inverse, SB postfilter -> int16 per
+// range, [level search: 5 filtered candidates, 6 packs, 6 distortion passes, decision], thresholds, dering + u8
+// store per plane.
+static int dering_launches(const Dering& D, int parts) { return 2 * parts + (D.search ? 5 + 6 + 6 + 1 : 0) + 1 + 3; }
 
 // Everything between "inputs are in HBM" and "results are in HBM", on kf->stream.
 // the three phase kernels over every chunk of every class of a stage's dependency-free lists
@@ -2429,62 +2449,128 @@ static int kf_enqueue_step_inter(daala_b200_kf* kf, int phases) {
   return (int)cudaGetLastError();
 }
 
-static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
-  if (kf->cfg.inter) return kf_enqueue_step_inter(kf, phases);
-  cudaStream_t s = kf->stream;
+// Keyframe work lists from the block-size maps.
+static int enqueue_lists(daala_b200_kf* kf, cudaStream_t s) {
   const Lists& L = kf->lists;
   const int wide = kf->sms * 8;
-  if (phases & DAALA_B200_KF_LISTS) {
-    k_unit_tile_sums<<<L.ntiles, kTile, 0, s>>>(L);
-    k_tile_scan<<<1, 1024, 0, s>>>(L);
-    k_unit_emit<<<L.ntiles, kTile, 0, s>>>(L);
-    const size_t nl = (size_t)L.max_luma * sizeof(int32_t);
-    if (cudaMemsetAsync(L.succ_bottom, 0xff, nl, s) != cudaSuccess || cudaMemsetAsync(L.succ_right, 0xff, nl, s) != cudaSuccess)
-      return (int)cudaGetLastError();
-    if (L.lvl_hist && cudaMemsetAsync(L.lvl_hist, 0, sizeof(int32_t) * kLevelBins, s) != cudaSuccess) return (int)cudaGetLastError();
-    if (cudaMemsetAsync(L.head_hist, 0, sizeof(int32_t) * kLevelBins, s) != cudaSuccess) return (int)cudaGetLastError();
-    k_luma_deps<<<wide, 256, 0, s>>>(L);
-    if (L.lvl_hist) {
-      k_level_scan<<<1, 1024, 0, s>>>(L);
-      k_level_scatter<<<wide, 256, 0, s>>>(L);
-    }
-    k_chroma_items<<<wide, 256, 0, s>>>(L);
+  k_unit_tile_sums<<<L.ntiles, kTile, 0, s>>>(L);
+  k_tile_scan<<<1, 1024, 0, s>>>(L);
+  k_unit_emit<<<L.ntiles, kTile, 0, s>>>(L);
+  const size_t nl = (size_t)L.max_luma * sizeof(int32_t);
+  if (cudaMemsetAsync(L.succ_bottom, 0xff, nl, s) != cudaSuccess || cudaMemsetAsync(L.succ_right, 0xff, nl, s) != cudaSuccess)
+    return (int)cudaGetLastError();
+  if (L.lvl_hist && cudaMemsetAsync(L.lvl_hist, 0, sizeof(int32_t) * kLevelBins, s) != cudaSuccess) return (int)cudaGetLastError();
+  if (cudaMemsetAsync(L.head_hist, 0, sizeof(int32_t) * kLevelBins, s) != cudaSuccess) return (int)cudaGetLastError();
+  k_luma_deps<<<wide, 256, 0, s>>>(L);
+  if (L.lvl_hist) {
+    k_level_scan<<<1, 1024, 0, s>>>(L);
+    k_level_scatter<<<wide, 256, 0, s>>>(L);
   }
-  if (phases & DAALA_B200_KF_FORWARD) {
-    int rc = daala_b200_launch_forward(&kf->frame, 3, s);
+  k_chroma_items<<<wide, 256, 0, s>>>(L);
+  return 0;
+}
+
+// The luma PVQ stage up to its last band: the tickets of the stages in `begin`, gather, [luma split bands, prepass], the chain kernel.  `core`
+// (_SEARCH_ONLY, measurement): just the search kernels, on the coding-order buffers a previous full pass left behind
+// (same inputs, same results).
+static int enqueue_luma_bands(daala_b200_kf* kf, bool core, int begin, cudaStream_t s) {
+  const int wide = kf->sms * 8;
+  const int persist = kf->sms * (kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas);
+  if (cudaMemsetAsync(kf->luma.ring, 0xff, kf->chain_cap * sizeof(uint32_t), s) != cudaSuccess ||
+      cudaMemsetAsync(kf->luma.join0, 0, (size_t)kf->luma.max_blocks * sizeof(int32_t), s) != cudaSuccess)
+    return (int)cudaGetLastError();
+  k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, begin);
+  if (!core) k_gather<kGatherLuma><<<wide, 256, 0, s>>>(kf->luma);
+  if (kf->cfg.split_free > 1) enqueue_split<true>(kf, kf->luma, s);
+  if (kf->luma.pre_ev) {
+    k_pvq_prepass<2><<<kf->sms * 16, 128, 0, s>>>(kf->luma);
+    k_pvq_prepass<1><<<kf->sms * 16, 128, 0, s>>>(kf->luma);
+  }
+  if (kf->cfg.level_chains) {
+    if (cudaMemsetAsync(kf->lv_bar, 0, sizeof(int32_t) * 32, s) != cudaSuccess) return (int)cudaGetLastError();
+    k_pvq_levels<<<kf->lvl_grid, 128, 0, s>>>(kf->luma);
+  } else {
+    k_pvq_persist<true><<<persist, kPersistThreads, 0, s>>>(kf->luma);
+  }
+  return 0;
+}
+
+// The chroma PVQ stage: [its tickets], gather with the CfL reference (it reads the luma stage's coding-order buffers, so it needs
+// the luma bands, not the luma scatter), the bands, the scatter into the coefficient planes.
+static void enqueue_chroma(daala_b200_kf* kf, bool core, bool begin, cudaStream_t s) {
+  const int wide = kf->sms * 8;
+  if (begin) k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, kBeginChroma);
+  if (!core) k_gather<kGatherChroma><<<wide, 256, 0, s>>>(kf->chroma);
+  if (kf->cfg.split_free > 0) enqueue_split<false>(kf, kf->chroma, s);
+  else k_pvq_persist<false><<<kf->sms * (kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas),
+                              kPersistThreads, 0, s>>>(kf->chroma);
+  if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->chroma);
+}
+
+// The whole keyframe step (DAALA_B200_KF_ALL) as two branches, kf->stream and kf->side, forked and joined with
+// events (captured into the step graph as parallel branches; live launches order the same way):
+//   lists on kf->stream beside the forward transform on kf->side; join;
+//   both stages' tickets, luma bands (the chain kernel) on kf->stream; fork;
+//   kf->side: chroma stage, [symbol stream, after the luma scatter], inverse + SB postfilter of planes 1-2;
+//   kf->stream: luma scatter, inverse + SB postfilter of plane 0, [level search, thresholds, od_dering of plane 0];
+//   join; [od_dering of planes 1-2: they read the direction map plane 0 writes].
+// The branches write disjoint buffers; only the order of independent work differs from the phase-by-phase path.
+static int kf_enqueue_step_forked(daala_b200_kf* kf) {
+  cudaStream_t s = kf->stream, c = kf->side;
+  const daala_b200_frame& fr = kf->cfg.dering ? kf->dering.frame : kf->frame;
+  auto fork = [](cudaEvent_t e, cudaStream_t from, cudaStream_t to) {
+    return cudaEventRecord(e, from) == cudaSuccess && cudaStreamWaitEvent(to, e, 0) == cudaSuccess;
+  };
+  if (!fork(kf->ev[kEvLists], s, c)) return (int)cudaGetLastError();
+  int rc = daala_b200_launch_forward(&kf->frame, 3, c);
+  if (!rc) rc = enqueue_lists(kf, s);
+  if (rc) return rc;
+  if (!fork(kf->ev[kEvForward], c, s)) return (int)cudaGetLastError();
+  rc = enqueue_luma_bands(kf, false, kBeginLuma | kBeginChroma, s);
+  if (rc) return rc;
+  if (!fork(kf->ev[kEvLumaBands], s, c)) return (int)cudaGetLastError();
+  enqueue_chroma(kf, false, false, c);
+  // 16 waves of short CTAs instead of one resident wave: priority only orders CTAs that are still waiting, so a grid
+  // that fits the GPU at once would hold every SM until it is done and stall the chroma gather behind it
+  k_finish_scatter<false><<<kf->sms * 128, 256, 0, s>>>(kf->luma);
+  if (kf->cfg.symbol_stream) {
+    if (!fork(kf->ev[kEvLumaScatter], s, c)) return (int)cudaGetLastError();
+    enqueue_sym<false>(kf->sym, kf->sms * 8, c);
+  }
+  rc = enqueue_recon(fr, 1, 2, c);
+  if (!rc) rc = enqueue_recon(fr, 0, 1, s);
+  if (!rc && kf->cfg.dering) rc = enqueue_dering_luma(kf, kf->dering, s);
+  if (rc) return rc;
+  if (!fork(kf->ev[kEvChroma], c, s)) return (int)cudaGetLastError();
+  for (int p = 1; kf->cfg.dering && p < 3; p++) {
+    rc = enqueue_dering_plane(kf, kf->dering, p, s);
     if (rc) return rc;
   }
-  const int persist = kf->sms * (kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas);
-  // _SEARCH_ONLY (measurement): just the persistent search kernels, on the coding-order buffers a
-  // previous full pass left behind (same inputs, same results)
+  return (int)cudaGetLastError();
+}
+
+// One step on kf->stream phase by phase (a partial phase mask: per-phase timings), or the whole step forked.
+static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
+  if (kf->cfg.inter) return kf_enqueue_step_inter(kf, phases);
+  if (phases == DAALA_B200_KF_ALL) return kf_enqueue_step_forked(kf);
+  cudaStream_t s = kf->stream;
+  if (phases & DAALA_B200_KF_LISTS) {
+    const int rc = enqueue_lists(kf, s);
+    if (rc) return rc;
+  }
+  if (phases & DAALA_B200_KF_FORWARD) {
+    const int rc = daala_b200_launch_forward(&kf->frame, 3, s);
+    if (rc) return rc;
+  }
   const bool core = (phases & DAALA_B200_KF_SEARCH_ONLY) != 0;
   if (phases & DAALA_B200_KF_PVQ_LUMA) {
-    if (cudaMemsetAsync(kf->luma.ring, 0xff, kf->chain_cap * sizeof(uint32_t), s) != cudaSuccess ||
-        cudaMemsetAsync(kf->luma.join0, 0, (size_t)kf->luma.max_blocks * sizeof(int32_t), s) != cudaSuccess)
-      return (int)cudaGetLastError();
-    k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, 1);
-    if (!core) k_gather<kGatherLuma><<<wide, 256, 0, s>>>(kf->luma);
-    if (kf->cfg.split_free > 1) enqueue_split<true>(kf, kf->luma, s);
-    if (kf->luma.pre_ev) {
-      k_pvq_prepass<2><<<kf->sms * 16, 128, 0, s>>>(kf->luma);
-      k_pvq_prepass<1><<<kf->sms * 16, 128, 0, s>>>(kf->luma);
-    }
-    if (kf->cfg.level_chains) {
-      if (cudaMemsetAsync(kf->lv_bar, 0, sizeof(int32_t) * 32, s) != cudaSuccess) return (int)cudaGetLastError();
-      k_pvq_levels<<<kf->lvl_grid, 128, 0, s>>>(kf->luma);
-    } else {
-      k_pvq_persist<true><<<persist, kPersistThreads, 0, s>>>(kf->luma);
-    }
-    if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->luma);
+    const int rc = enqueue_luma_bands(kf, core, kBeginLuma, s);
+    if (rc) return rc;
+    if (!core) k_finish_scatter<false><<<kf->sms * 8, 256, 0, s>>>(kf->luma);
   }
   if (phases & DAALA_B200_KF_PVQ_CHROMA) {
-    k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, 0);
-    if (!core) k_cfl_plane<<<wide, 256, 0, s>>>(kf->chroma, kf->cfl_plane);
-    if (!core) k_gather<kGatherChroma><<<wide, 256, 0, s>>>(kf->chroma);
-    if (kf->cfg.split_free > 0) enqueue_split<false>(kf, kf->chroma, s);
-    else k_pvq_persist<false><<<persist, kPersistThreads, 0, s>>>(kf->chroma);
-    if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->chroma);
-    if (!core && kf->cfg.symbol_stream) enqueue_sym<false>(kf->sym, wide, s);
+    enqueue_chroma(kf, core, true, s);
+    if (!core && kf->cfg.symbol_stream) enqueue_sym<false>(kf->sym, kf->sms * 8, s);
   }
   if (phases & DAALA_B200_KF_INVERSE) {
     int rc = kf->cfg.dering ? enqueue_dering(kf, kf->dering, s) : daala_b200_launch_inverse(&kf->frame, 3, s);
@@ -2609,6 +2695,19 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
     }
     kf->own_stream = true;
   }
+  if (!cfg->inter) {
+    // the side branch carries the longer chain (the chroma stage) at the highest priority: the luma branch's CTAs
+    // then take the SMs the chroma kernels leave idle instead of delaying them
+    int least = 0, greatest = 0;
+    bool ok = cudaDeviceGetStreamPriorityRange(&least, &greatest) == cudaSuccess &&
+              cudaStreamCreateWithPriority(&kf->side, cudaStreamNonBlocking, greatest) == cudaSuccess;
+    for (int i = 0; ok && i < kNumEvents; i++) ok = cudaEventCreateWithFlags(&kf->ev[i], cudaEventDisableTiming) == cudaSuccess;
+    if (!ok) {
+      snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: cannot create the second stream and its events");
+      daala_b200_kf_destroy(kf);
+      return nullptr;
+    }
+  }
   if (kf_alloc(kf) != 0) {
     fprintf(stderr, "daala_b200_kf_create: %s\n", kf->err);
     snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: %s", kf->err);
@@ -2627,6 +2726,9 @@ void daala_b200_kf_destroy(daala_b200_kf* kf) {
   if (kf->fin_exec) cudaGraphExecDestroy(kf->fin_exec);
   if (kf->fin_graph) cudaGraphDestroy(kf->fin_graph);
   for (void* p : kf->allocs) cudaFree(p);
+  for (cudaEvent_t e : kf->ev)
+    if (e) cudaEventDestroy(e);
+  if (kf->side) cudaStreamDestroy(kf->side);
   if (kf->own_stream) cudaStreamDestroy(kf->stream);
   delete kf;
 }
@@ -2656,9 +2758,10 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
            (kf->cfg.symbol_stream ? 8 : 0) + (kf->cfg.late_skip ? kLateSkipLaunches : 0);
   int n = 5 + (kf->cfg.level_chains ? 2 : 0);                                    // work lists
   n += 1;                                                                         // forward
-  n += 3 + 1 + (kf->cfg.split_free > 1 ? split(kf->luma) : 0) + (kf->luma.pre_ev ? 2 : 0);   // luma: begin, gather, [prepass], chains, finish
-  n += 4 + (kf->cfg.split_free > 0 ? split(kf->chroma) : 1);                      // chroma: begin, cfl, gather, bands, finish
-  n += kf->cfg.dering ? dering_launches(kf->dering) : 2;                          // [deringing pass | inverse, SB postfilter + store]
+  n += 3 + 1 + (kf->cfg.split_free > 1 ? split(kf->luma) : 0) + (kf->luma.pre_ev ? 2 : 0);   // luma: begin (both stages), gather, [prepass], chains, finish
+  n += 2 + (kf->cfg.split_free > 0 ? split(kf->chroma) : 1);                      // chroma: gather, bands, finish
+  // inverse + SB postfilter of plane 0 and of planes 1-2, [the rest of the deringing pass]
+  n += kf->cfg.dering ? dering_launches(kf->dering, 2) : 4;
   if (kf->cfg.symbol_stream) n += 8;             // symbol stream: rank, superblock scan, place, 3 scan kernels, pack, index
   return n;
 }
@@ -2728,7 +2831,8 @@ int daala_b200_kf_run_device(daala_b200_kf* kf, int phases, int use_graph) {
     cudaError_t e = cudaStreamEndCapture(kf->stream, &kf->graph);
     if (rc) return rc;
     KF_CHECK(e);
-    KF_CHECK(cudaGraphInstantiate(&kf->exec, kf->graph, 0));
+    // the captured nodes keep their stream's priority (kf->side's branch first)
+    KF_CHECK(cudaGraphInstantiate(&kf->exec, kf->graph, cudaGraphInstantiateFlagUseNodePriority));
     kf->captured = true;
   }
   KF_CHECK(cudaGraphLaunch(kf->exec, kf->stream));
