@@ -32,6 +32,7 @@
 #include "gen/dct_lifting.cuh"
 #include "lapped_filter.cuh"
 #include "frame_transform.h"
+#include "haar.cuh"
 
 namespace daala_b200 {
 
@@ -747,11 +748,7 @@ __global__ void k_split_filter_batch(int32_t* blocks, int n, int post, int hfilt
 using namespace daala_b200;
 
 // od_haar / od_haar_inv (src/dct.c:4822 / :4861): the multi-level 2-D Haar wavelet of the lossless
-// path, one CTA per packed n x n block, in place.  Every level is "read all 2x2 groups, then write":
-// the reference's serial loop order only makes its in-place update equal to that (forward: LL(i,j) is
-// consumed by group (i/2, j/2), visited earlier; inverse: groups are visited in descending order).
-// Sub-band placement as the reference: lh -> (i, j + np), hl -> (i + np, j), hh -> (i + np, j + np),
-// with OD_HAAR_KERNEL(a, b, c, d) taking b = the sample BELOW a and c = the one to its RIGHT.
+// path, one CTA per packed n x n block, in place (the level loops: haar.cuh).
 template <bool kInverse>
 __global__ void __launch_bounds__(256) k_haar_blocks(int32_t* __restrict__ blocks, int ln) {
   __shared__ int t[64 * 64];
@@ -760,65 +757,9 @@ __global__ void __launch_bounds__(256) k_haar_blocks(int32_t* __restrict__ block
   if (!kInverse) {
     for (int i = threadIdx.x; i < n * n; i += 256) t[i] = g[i];
     __syncthreads();
-    for (int level = 0; level < ln; level++) {
-      const int np = n >> level >> 1;
-      int keep[4];   // np * np <= 1024 groups, 256 threads
-      int q = 0;
-      for (int idx = threadIdx.x; idx < np * np; idx += 256, q++) {
-        const int i = idx / np, j = idx - i * np;
-        int ll = t[2 * i * n + 2 * j], lh = t[(2 * i + 1) * n + 2 * j];
-        int hl = t[2 * i * n + 2 * j + 1], hh = t[(2 * i + 1) * n + 2 * j + 1];
-        ll += hl;
-        hh -= lh;
-        const int m = (ll - hh) >> 1;
-        lh = m - lh;
-        hl = m - hl;
-        ll -= lh;
-        hh += hl;
-        keep[q] = ll;
-        g[i * n + j + np] = lh;
-        g[(i + np) * n + j] = hl;
-        g[(i + np) * n + j + np] = hh;
-      }
-      __syncthreads();
-      q = 0;
-      for (int idx = threadIdx.x; idx < np * np; idx += 256, q++) {
-        const int i = idx / np, j = idx - i * np;
-        t[i * n + j] = keep[q];
-      }
-      __syncthreads();
-    }
-    if (threadIdx.x == 0) g[0] = t[0];
+    haar_forward_levels<256>(t, g, n, ln);
   } else {
-    if (threadIdx.x == 0) t[0] = g[0];
-    __syncthreads();
-    for (int level = ln - 1; level >= 0; level--) {
-      const int np = 1 << (ln - 1 - level);
-      int a4[4], b4[4], c4[4], d4[4];
-      int q = 0;
-      for (int idx = threadIdx.x; idx < np * np; idx += 256, q++) {
-        const int i = idx / np, j = idx - i * np;
-        int ll = t[i * n + j], lh = g[i * n + j + np], hl = g[(i + np) * n + j], hh = g[(i + np) * n + j + np];
-        ll += hl;
-        hh -= lh;
-        const int m = (ll - hh) >> 1;
-        lh = m - lh;
-        hl = m - hl;
-        ll -= lh;
-        hh += hl;
-        a4[q] = ll; b4[q] = lh; c4[q] = hl; d4[q] = hh;
-      }
-      __syncthreads();
-      q = 0;
-      for (int idx = threadIdx.x; idx < np * np; idx += 256, q++) {
-        const int i = idx / np, j = idx - i * np;
-        t[2 * i * n + 2 * j] = a4[q];
-        t[(2 * i + 1) * n + 2 * j] = b4[q];
-        t[2 * i * n + 2 * j + 1] = c4[q];
-        t[(2 * i + 1) * n + 2 * j + 1] = d4[q];
-      }
-      __syncthreads();
-    }
+    haar_inverse_levels<256>(t, g, n, ln);
     for (int i = threadIdx.x; i < n * n; i += 256) g[i] = t[i];
   }
 }

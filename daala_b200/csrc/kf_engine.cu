@@ -44,6 +44,7 @@
 #include "daala_b200.h"
 #include "dering_search.h"
 #include "late_skip.h"
+#include "lossless.h"
 #include "mc_batch.h"
 #include "gen/coding_order.inc"
 #include "pvq_math.cuh"
@@ -1755,6 +1756,13 @@ struct daala_b200_kf {
   int32_t* d_orig[3];
   daala_b200_kf_late_skip* late_skip[2];
   daala_b200_late_skip_batch lsb;
+  // cfg.lossless: the residual planes, the root-sum records, the keyframe DCs, the slot table of ll_ref_slot_out and the
+  // parameters of the step (csrc/lossless.cu)
+  int16_t* ll_coeffs[3];
+  int32_t* ll_blocks;
+  int32_t* ll_dc;
+  int32_t* ll_slot_out;
+  daala_b200_lossless_batch ll;
   std::vector<uint8_t> slot_filled;  // cfg.inter_mc, per pool slot: something has written a picture there
   bool have_step;                  // a step has been submitted; last_tot are its totals
   daala_b200_kf_totals last_tot;
@@ -1786,7 +1794,86 @@ static cudaError_t dalloc(daala_b200_kf* kf, T** p, size_t n) {
   return e;
 }
 
+// cfg.inter_mc: the reference-picture pool, the slot map, the MV grids and the leaf segments of the prediction step
+// (kf->pred_pixels must exist: the prediction's destination).
+static int mc_alloc(daala_b200_kf* kf) {
+  const int F = kf->F;
+  daala_b200_mc_batch& B = kf->mc;
+  const size_t nsb = (size_t)kf->nhsb * kf->nvsb;
+  for (int p = 0; p < 3; p++) {
+    KF_CHECK(dalloc(kf, &kf->ref_pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * kf->cfg.mc_refs));
+    B.ref[p] = kf->ref_pixels[p];
+    B.pred[p] = kf->pred_pixels[p];
+    B.plane_w[p] = kf->plane_w[p];
+    B.plane_h[p] = kf->plane_h[p];
+  }
+  KF_CHECK(dalloc(kf, &kf->ref_slot, (size_t)2 * F));
+  KF_CHECK(dalloc(kf, &kf->mv_grid, (size_t)F * (kf->nvsb * 8 + 1) * (kf->nhsb * 8 + 1)));
+  KF_CHECK(dalloc(kf, &kf->mc_leaves, (size_t)F * nsb * 64));
+  KF_CHECK(dalloc(kf, &kf->mc_nleaves, (size_t)F * nsb));
+  B.grid = kf->mv_grid;
+  B.ref_slot = kf->ref_slot;
+  B.leaves = kf->mc_leaves;
+  B.nleaves = kf->mc_nleaves;
+  B.F = F;
+  B.nhsb = kf->nhsb;
+  B.nvsb = kf->nvsb;
+  B.nslots = kf->cfg.mc_refs;
+  if (kf->cfg.mc_next) {
+    KF_CHECK(dalloc(kf, &kf->ref_slot_next, (size_t)F));
+    KF_CHECK(dalloc(kf, &kf->mv1_grid, (size_t)F * (kf->nvsb * 8 + 1) * (kf->nhsb * 8 + 1) * 2));
+    B.ref_slot_next = kf->ref_slot_next;
+    B.mv1 = kf->mv1_grid;
+  }
+  return 0;
+}
+
+// cfg.lossless: the input, prediction and reconstruction planes, [inter_mc: the pool], the counters and the lossless
+// step's own buffers; nothing of the PVQ step.
+static int ll_alloc(daala_b200_kf* kf) {
+  const int F = kf->F;
+  daala_b200_lossless_batch& B = kf->ll;
+  memset(&B, 0, sizeof(B));
+  for (int p = 0; p < 3; p++) {
+    const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
+    KF_CHECK(dalloc(kf, &kf->pixels[p], n));
+    KF_CHECK(dalloc(kf, &kf->pixels_out[p], n));
+    KF_CHECK(dalloc(kf, &kf->ll_coeffs[p], n));
+    if (kf->cfg.inter) KF_CHECK(dalloc(kf, &kf->pred_pixels[p], n));
+    B.src[p] = kf->pixels[p];
+    B.pred[p] = kf->pred_pixels[p];
+    B.coeffs[p] = kf->ll_coeffs[p];
+    B.out[p] = kf->pixels_out[p];
+    B.plane_w[p] = kf->plane_w[p];
+    B.plane_h[p] = kf->plane_h[p];
+  }
+  const size_t nrec = (size_t)F * kf->nhsb * kf->nvsb * 3;
+  KF_CHECK(dalloc(kf, &kf->ll_blocks, nrec * 4));
+  KF_CHECK(dalloc(kf, &kf->ll_dc, nrec));
+  KF_CHECK(dalloc(kf, &kf->lists.cnt, (size_t)kCntWords));
+  kf->mc.bad_ref = kf->lists.cnt + kMcBadRef;
+  kf->mc.beyond = kf->lists.cnt + kMcBeyond;
+  if (kf->cfg.inter_mc) {
+    int rc = mc_alloc(kf);
+    if (rc) return rc;
+    KF_CHECK(dalloc(kf, &kf->ll_slot_out, (size_t)F));
+    for (int p = 0; p < 3; p++) B.pool[p] = kf->ref_pixels[p];
+    B.slot_out = kf->ll_slot_out;
+  }
+  B.blocks = kf->ll_blocks;
+  B.dc = kf->ll_dc;
+  B.F = F;
+  B.nhsb = kf->nhsb;
+  B.nvsb = kf->nvsb;
+  B.pic_w = kf->cfg.pic_w;
+  B.pic_h = kf->cfg.pic_h;
+  // dalloc's clears run on the legacy default stream (see the end of kf_alloc)
+  KF_CHECK(cudaDeviceSynchronize());
+  return 0;
+}
+
 static int kf_alloc(daala_b200_kf* kf) {
+  if (kf->cfg.lossless) return ll_alloc(kf);
   const int F = kf->F;
   const bool inter = kf->cfg.inter != 0;
   const long long luma_px = (long long)kf->plane_w[0] * kf->plane_h[0];
@@ -1804,33 +1891,8 @@ static int kf_alloc(daala_b200_kf* kf) {
   const int UW = kf->nhsb * 8, UH = kf->nvsb * 8;
   KF_CHECK(dalloc(kf, &kf->bsize, (size_t)F * UW * UH));
   if (kf->cfg.inter_mc) {
-    daala_b200_mc_batch& B = kf->mc;
-    const size_t nsb = (size_t)kf->nhsb * kf->nvsb;
-    for (int p = 0; p < 3; p++) {
-      KF_CHECK(dalloc(kf, &kf->ref_pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * kf->cfg.mc_refs));
-      B.ref[p] = kf->ref_pixels[p];
-      B.pred[p] = kf->pred_pixels[p];
-      B.plane_w[p] = kf->plane_w[p];
-      B.plane_h[p] = kf->plane_h[p];
-    }
-    KF_CHECK(dalloc(kf, &kf->ref_slot, (size_t)2 * F));
-    KF_CHECK(dalloc(kf, &kf->mv_grid, (size_t)F * (kf->nvsb * 8 + 1) * (kf->nhsb * 8 + 1)));
-    KF_CHECK(dalloc(kf, &kf->mc_leaves, (size_t)F * nsb * 64));
-    KF_CHECK(dalloc(kf, &kf->mc_nleaves, (size_t)F * nsb));
-    B.grid = kf->mv_grid;
-    B.ref_slot = kf->ref_slot;
-    B.leaves = kf->mc_leaves;
-    B.nleaves = kf->mc_nleaves;
-    B.F = F;
-    B.nhsb = kf->nhsb;
-    B.nvsb = kf->nvsb;
-    B.nslots = kf->cfg.mc_refs;
-    if (kf->cfg.mc_next) {
-      KF_CHECK(dalloc(kf, &kf->ref_slot_next, (size_t)F));
-      KF_CHECK(dalloc(kf, &kf->mv1_grid, (size_t)F * (kf->nvsb * 8 + 1) * (kf->nhsb * 8 + 1) * 2));
-      B.ref_slot_next = kf->ref_slot_next;
-      B.mv1 = kf->mv1_grid;
-    }
+    const int rc = mc_alloc(kf);
+    if (rc) return rc;
   }
   if (kf->cfg.frame_quant) {
     KF_CHECK(dalloc(kf, &kf->fq, (size_t)F));
@@ -2549,8 +2611,26 @@ static int kf_enqueue_step_forked(daala_b200_kf* kf) {
   return (int)cudaGetLastError();
 }
 
+// config.lossless: the whole step, one phase.  [inter_mc: leaf enumeration and OBMC, unchanged], the lossless kernels.
+static int kf_enqueue_step_lossless(daala_b200_kf* kf, int phases) {
+  if (phases != DAALA_B200_KF_ALL) {
+    snprintf(kf->err, sizeof(kf->err), "a lossless step runs whole (DAALA_B200_KF_ALL)");
+    return (int)cudaErrorInvalidValue;
+  }
+  cudaStream_t s = kf->stream;
+  const int wide = kf->sms * 8;
+  if (kf->cfg.inter_mc) {
+    if (cudaMemsetAsync(kf->lists.cnt + kMcBadRef, 0, 2 * sizeof(int32_t), s) != cudaSuccess) return (int)cudaGetLastError();
+    int rc = daala_b200_launch_mc_leaves(&kf->mc, wide, s);
+    if (!rc) rc = daala_b200_launch_mc_obmc(&kf->mc, wide, s);
+    if (rc) return rc;
+  }
+  return daala_b200_launch_lossless(&kf->ll, s);
+}
+
 // One step on kf->stream phase by phase (a partial phase mask: per-phase timings), or the whole step forked.
 static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
+  if (kf->cfg.lossless) return kf_enqueue_step_lossless(kf, phases);
   if (kf->cfg.inter) return kf_enqueue_step_inter(kf, phases);
   if (phases == DAALA_B200_KF_ALL) return kf_enqueue_step_forked(kf);
   cudaStream_t s = kf->stream;
@@ -2634,6 +2714,22 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
              "daala_b200_kf_create: frame_quant is 0 or 1, and 1 requires inter = 1 (a keyframe batch shares one quantizer)");
     return nullptr;
   }
+  if (cfg && cfg->lossless) {
+    // the lossless path has no PVQ, no deringing and no coder-side state: none of these stages exists for it
+    const char* with = cfg->lossless != 1 ? "a value other than 0 or 1"
+                       : cfg->dering ? "dering (lossless frames skip deringing)"
+                       : cfg->symbol_stream ? "symbol_stream (the stream is the PVQ symbols)"
+                       : cfg->late_skip ? "late_skip"
+                       : cfg->inter_finish ? "inter_finish"
+                       : cfg->frame_quant ? "frame_quant (every frame is at quantizer 0)"
+                       : cfg->noref_prepass ? "noref_prepass"
+                       : cfg->level_chains ? "level_chains"
+                       : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
+    if (with) {
+      snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: lossless is not defined with %s", with);
+      return nullptr;
+    }
+  }
   if (cfg && cfg->mc_refs < 0) {
     snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: mc_refs < 0");
     return nullptr;
@@ -2695,7 +2791,7 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
     }
     kf->own_stream = true;
   }
-  if (!cfg->inter) {
+  if (!cfg->inter && !cfg->lossless) {
     // the side branch carries the longer chain (the chroma stage) at the highest priority: the luma branch's CTAs
     // then take the SMs the chroma kernels leave idle instead of delaying them
     int least = 0, greatest = 0;
@@ -2749,6 +2845,8 @@ int daala_b200_kf_chain_trace(daala_b200_kf* kf, void** recs, int* cap) {
 // Kernel launches of one whole step (kf_enqueue_step with DAALA_B200_KF_ALL), memset nodes not counted.
 int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   if (!kf) return 0;
+  // lossless: [leaves + OBMC], the forward kernel, [keyframes: the DC + reconstruction kernel]
+  if (kf->cfg.lossless) return (kf->cfg.inter_mc ? 2 : 0) + (kf->cfg.inter ? 1 : 2);
   auto split = [](const Stage& S) { return 3 * (S.sp_chunks[0] + S.sp_chunks[1] + S.sp_chunks[2]); };
   // inter: work lists, two forward launches, per stage gather + phase kernels + finish, inverse + SB postfilter;
   // inter_mc: leaf enumeration and OBMC
@@ -2932,17 +3030,41 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   if (!kf || !io) return (int)cudaErrorInvalidValue;
   cudaStream_t s = kf->stream;
   const int F = kf->F;
-  if (!io->bsize) return (int)cudaErrorInvalidValue;
+  const bool lossless = kf->cfg.lossless != 0;
+  if (!io->bsize && !lossless) return (int)cudaErrorInvalidValue;
   // refuse a batch with more blocks than the work lists hold before anything is copied or launched: the
-  // step would otherwise run on truncated lists
+  // step would otherwise run on truncated lists (a lossless step has no block lists)
   daala_b200_kf_totals tot;
-  if (io->totals) tot = *io->totals;
-  else daala_b200_kf_count_blocks(io->bsize, F, (long long)kf->nhsb * 8 * kf->nvsb * 8, kf->nhsb * 8, kf->nhsb, kf->nvsb,
-                                  kf->cfg.sb_row0, kf->cfg.sb_rows, &tot);
+  memset(&tot, 0, sizeof(tot));
+  if (lossless) {
+  } else if (io->totals) {
+    tot = *io->totals;
+  } else {
+    daala_b200_kf_count_blocks(io->bsize, F, (long long)kf->nhsb * 8 * kf->nvsb * 8, kf->nhsb * 8, kf->nhsb, kf->nvsb,
+                               kf->cfg.sb_row0, kf->cfg.sb_rows, &tot);
+  }
   if (tot.n_luma > kf->lists.max_luma || tot.n_chroma > kf->lists.max_chroma) return (int)cudaErrorInvalidValue;
   const bool have_pred = io->pred_pixels[0] || io->pred_pixels[1] || io->pred_pixels[2];
-  // symbol_stream = 2: the stream's DC records carry the DC indices, so the classic arrays are optional
-  const bool need_dc = kf->cfg.symbol_stream != 2 && (!io->luma_dc || !io->chroma_dc);
+  // symbol_stream = 2: the stream's DC records carry the DC indices, so the classic arrays are optional; a lossless
+  // step has no scalar DC index
+  const bool need_dc = !lossless && kf->cfg.symbol_stream != 2 && (!io->luma_dc || !io->chroma_dc);
+  // the lossless outputs: only a lossless engine has them, and only one with the pool stores into it
+  const bool want_ll = io->ll_coeffs[0] || io->ll_coeffs[1] || io->ll_coeffs[2] || io->ll_blocks;
+  const char* ll_why = (want_ll || io->ll_ref_slot_out) && !lossless
+                           ? "ll_coeffs / ll_blocks / ll_ref_slot_out need an engine with lossless = 1"
+                       : io->ll_ref_slot_out && !kf->cfg.inter_mc
+                           ? "ll_ref_slot_out needs an engine with inter_mc (the reference-picture pool)"
+                           : nullptr;
+  for (int f = 0; !ll_why && io->ll_ref_slot_out && f < F; f++) {
+    const int32_t r = io->ll_ref_slot_out[f];
+    if (r < -1 || r >= kf->cfg.mc_refs) ll_why = "an ll_ref_slot_out entry is outside [-1, mc_refs)";
+    for (int g = 0; !ll_why && r >= 0 && g < f; g++)
+      if (io->ll_ref_slot_out[g] == r) ll_why = "two frames name the same ll_ref_slot_out slot";
+  }
+  if (ll_why) {
+    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", ll_why);
+    return (int)cudaErrorInvalidValue;
+  }
   if (kf->cfg.inter && !kf->cfg.inter_mc &&
       (!io->pred_pixels[0] || !io->pred_pixels[1] || !io->pred_pixels[2] || need_dc)) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: an inter engine needs pred_pixels[0..2], luma_dc and chroma_dc");
@@ -3105,7 +3227,10 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     KF_CHECK(cudaMemcpyAsync(kf->fq_tbl, kf->fq_tbl_host.data(), sizeof(int32_t) * 12 * F, cudaMemcpyHostToDevice, s));
   }
   const size_t map_bytes = (size_t)kf->nhsb * 8 * kf->nvsb * 8 * F;
-  KF_CHECK(cudaMemcpyAsync(kf->bsize, io->bsize, map_bytes, cudaMemcpyHostToDevice, s));
+  if (!lossless) KF_CHECK(cudaMemcpyAsync(kf->bsize, io->bsize, map_bytes, cudaMemcpyHostToDevice, s));
+  // the graph's lossless kernels read the slot table: NULL stores nothing (every entry -1)
+  if (io->ll_ref_slot_out) KF_CHECK(cudaMemcpyAsync(kf->ll_slot_out, io->ll_ref_slot_out, 4 * (size_t)F, cudaMemcpyHostToDevice, s));
+  else if (kf->ll_slot_out) KF_CHECK(cudaMemsetAsync(kf->ll_slot_out, 0xFF, 4 * (size_t)F, s));
   if (kf->cfg.dering == 1) {
     if (!io->dering_level) return (int)cudaErrorInvalidValue;
     KF_CHECK(cudaMemcpyAsync(kf->dering.level, io->dering_level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyHostToDevice, s));
@@ -3126,6 +3251,21 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     if (io->pixels_out[p])
       KF_CHECK(cudaMemcpyAsync(io->pixels_out[p], kf->pixels_out[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
                                cudaMemcpyDeviceToHost, s));
+  if (lossless) {
+    for (int f = 0; io->ll_ref_slot_out && f < F; f++)
+      if (io->ll_ref_slot_out[f] >= 0) kf->slot_filled[io->ll_ref_slot_out[f]] = 1;
+    for (int p = 0; p < 3; p++) {
+      const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
+      if (io->ll_coeffs[p]) KF_CHECK(cudaMemcpyAsync(io->ll_coeffs[p], kf->ll_coeffs[p], 2 * n, cudaMemcpyDeviceToHost, s));
+      if (kf->cfg.inter_mc && io->pred_pixels_out[p])
+        KF_CHECK(cudaMemcpyAsync(io->pred_pixels_out[p], kf->pred_pixels[p], n, cudaMemcpyDeviceToHost, s));
+    }
+    if (io->ll_blocks)
+      KF_CHECK(cudaMemcpyAsync(io->ll_blocks, kf->ll_blocks, sizeof(daala_b200_kf_ll_block) * F * kf->nhsb * kf->nvsb * 3,
+                               cudaMemcpyDeviceToHost, s));
+    if (io->counts) KF_CHECK(cudaMemcpyAsync(io->counts, kf->lists.cnt, sizeof(int32_t) * 32, cudaMemcpyDeviceToHost, s));
+    return 0;
+  }
   if (io->luma_blocks) KF_CHECK(cudaMemcpyAsync(io->luma_blocks, kf->lists.luma, sizeof(daala_b200_pvq_block) * tot.n_luma, cudaMemcpyDeviceToHost, s));
   if (io->chroma_blocks) KF_CHECK(cudaMemcpyAsync(io->chroma_blocks, kf->lists.chroma, sizeof(daala_b200_pvq_block) * tot.n_chroma, cudaMemcpyDeviceToHost, s));
   if (io->luma_res) KF_CHECK(cudaMemcpyAsync(io->luma_res, kf->luma.res_pack, 8 * 9 * (size_t)tot.n_luma, cudaMemcpyDeviceToHost, s));

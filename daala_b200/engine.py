@@ -24,6 +24,11 @@ B-frame order and buffer rotation).
 With inter=1 and frame_quant=1 every frame of a batch has its own quantizer: `encode(..., frame_quant=)` takes one
 FRAME_QUANT_DTYPE record per frame (frame_quant_records builds them) in place of the engine-wide q0, coded_quantizer,
 dering_lambda and pvq_qm_q4, so P and B frames of different types or streams share one batch.
+With lossless=1 every frame is coded at quantizer 0, the reference's Haar-wavelet path (keyframes, or P / B frames with
+inter=1 and host or inter_mc prediction): `encode` takes no block-size map and returns each block's residual
+(`ll_coeffs0..2`, int16 planes), the three root tree sums of every block (`ll_blocks`, [F, nvsb, nhsb, 3, 4] int32) and
+the reconstruction; `encode(..., ll_ref_slot_out=)` stores each frame's reconstruction into a pool slot (inter_mc).
+daala_b200/lossless.py restates the path in numpy.
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -48,7 +53,8 @@ class Config(ctypes.Structure):
                 ("max_blocks_div", c_int), ("persist_ctas_per_sm", c_int), ("split_free", c_int), ("dering", c_int), ("noref_prepass", c_int), ("level_chains", c_int), ("stream", c_void_p),
                 ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
                 ("symbol_stream", c_int), ("inter", c_int), ("inter_mc", c_int), ("mc_refs", c_int),
-                ("inter_finish", c_int), ("late_skip", c_int), ("mc_next", c_int), ("frame_quant", c_int)]
+                ("inter_finish", c_int), ("late_skip", c_int), ("mc_next", c_int), ("frame_quant", c_int),
+                ("lossless", c_int)]
 
 
 # daala_b200_kf_frame_quant: one frame's quantizer on a frame_quant engine
@@ -90,7 +96,8 @@ class IO(ctypes.Structure):
                 ("ref_resident", c_int), ("sym_dc", c_void_p), ("sym_dc_cap", c_ll),
                 ("luma_late_skip", c_void_p), ("chroma_late_skip", c_void_p), ("sym_late_skip", c_void_p),
                 ("sym_late_skip_cap", c_ll), ("ref_slot_next", c_void_p), ("mv1_grid", c_void_p),
-                ("frame_quant", c_void_p)]
+                ("frame_quant", c_void_p), ("ll_coeffs", c_void_p * 3), ("ll_blocks", c_void_p),
+                ("ll_ref_slot_out", c_void_p)]
 
 
 class FinishIO(ctypes.Structure):
@@ -185,7 +192,7 @@ class KeyframeEngine:
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
                  qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=0, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
                  qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0, inter_mc=0, mc_refs=0,
-                 inter_finish=0, late_skip=0, mc_next=0, frame_quant=0):
+                 inter_finish=0, late_skip=0, mc_next=0, frame_quant=0, lossless=0):
         self.L = _bind()
         self.geom, self.F = geom, nframes
         if qm is None:
@@ -233,6 +240,10 @@ class KeyframeEngine:
         cfg.frame_quant = int(frame_quant)
         self.frame_quant = int(frame_quant)
         self._fq = None
+        # lossless: quantizer 0 (the Haar-wavelet path); q0, pvq_qm_q4 and the block-size maps are not read
+        cfg.lossless = int(lossless)
+        self.lossless = int(lossless)
+        self._ll_slot = None
         self.nrefs = 0
         self.resident = False
         self._pool_src = []
@@ -373,6 +384,9 @@ class KeyframeEngine:
             if self.inter and not self.inter_mc:
                 a = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
                 a[...] = pred[p]
+        if self.lossless:   # every block is 64x64: no map, no block lists
+            self.totals = None
+            return
         b = self._arr("bsize", (self.F,) + tuple(g.bsize_shape), np.uint8)
         b[...] = bsize
         self.totals = self.count_blocks(b)
@@ -394,6 +408,8 @@ class KeyframeEngine:
         (symbols.LATE_SKIP_DTYPE per block, block order) with the symbols.  On a
         symbol_stream=2 engine symbols=False also leaves out the classic DC arrays (the stream carries them).
         pred=False (inter_mc engines): the prediction planes are not copied back."""
+        if self.lossless:
+            return self._prepare_io_lossless(recon, pred)
         g, t = self.geom, self.totals
         io = IO()
         for p in range(3):
@@ -455,6 +471,8 @@ class KeyframeEngine:
             io.luma_dc_resid, io.chroma_dc_resid = out["luma_dc_resid"].ctypes.data, out["chroma_dc_resid"].ctypes.data
         if self._fq is not None:
             io.frame_quant = self._fq.ctypes.data
+        if self._ll_slot is not None:   # refused by the C call: a lossy engine has no lossless step
+            io.ll_ref_slot_out = self._ll_slot.ctypes.data
         out["counts"] = self._arr("cnt", (32,), np.int32)
         io.counts = out["counts"].ctypes.data
         if self.dering:
@@ -490,6 +508,64 @@ class KeyframeEngine:
             self.h2d_bytes += self.F * (FRAME_QUANT_DTYPE.itemsize + 48)
         return out
 
+    def stage_ll_ref_slot_out(self, slots):
+        """[F] int32 pool slots that receive each frame's lossless reconstruction (-1 = not stored), or None: nothing
+        stored (lossless engines with inter_mc; the C call refuses the table elsewhere)."""
+        if slots is None:
+            self._ll_slot = None
+            return
+        self._ll_slot = self._arr("llslot", (self.F,), np.int32)
+        self._ll_slot[...] = slots
+
+    def _prepare_io_lossless(self, recon, pred):
+        """prepare_io of a lossless engine: the inputs, [the prediction inputs], and as outputs the reconstruction
+        (recon0..2), the residual planes ll_coeffs0..2 ([F, h, w] int16), the root sums ll_blocks ([F, nvsb, nhsb, 3, 4]
+        int32: tree_sum[0][1], [1][0], [1][1], 0 per plane), [pred0..2] and the counters."""
+        g = self.geom
+        io = IO()
+        out = {}
+        for p in range(3):
+            io.pixels[p] = self._arr("in%d" % p, (self.F,) + g.plane_shape(p), np.uint8).ctypes.data
+            if recon:
+                out["recon%d" % p] = self._arr("out%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
+                io.pixels_out[p] = out["recon%d" % p].ctypes.data
+            out["ll_coeffs%d" % p] = self._arr("llc%d" % p, (self.F,) + g.plane_shape(p), np.int16)
+            io.ll_coeffs[p] = out["ll_coeffs%d" % p].ctypes.data
+            if self.inter and not self.inter_mc:
+                io.pred_pixels[p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8).ctypes.data
+        out["ll_blocks"] = self._arr("llb", (self.F, g.nvsb, g.nhsb, 3, 4), np.int32)
+        io.ll_blocks = out["ll_blocks"].ctypes.data
+        if self.inter_mc:
+            io.ref_resident = int(self.resident)
+            for p in range(3):
+                if not self.resident:
+                    io.ref_pixels[p] = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8).ctypes.data
+                if pred:
+                    out["pred%d" % p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
+                    io.pred_pixels_out[p] = out["pred%d" % p].ctypes.data
+            io.nrefs = self.nrefs
+            io.ref_slot = self._arr("slot", (self.F, 2), np.int32).ctypes.data
+            io.mv_grid = self._arr("grid", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1), mvgrid.MV_PT_DTYPE).ctypes.data
+            if self.mc_next:
+                io.ref_slot_next = self._arr("slot_next", (self.F,), np.int32).ctypes.data
+                io.mv1_grid = self._arr("grid1", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1, 2), np.int32).ctypes.data
+        if self._ll_slot is not None:
+            io.ll_ref_slot_out = self._ll_slot.ctypes.data
+        out["counts"] = self._arr("cnt", (32,), np.int32)
+        io.counts = out["counts"].ctypes.data
+        self.d2h_bytes = sum(v.nbytes for v in out.values())
+        self._io, self._out = io, out
+        px = sum(int(np.prod(g.plane_shape(p))) for p in range(3))
+        self.h2d_bytes = px * self.F * (2 if self.inter and not self.inter_mc else 1)
+        if self.inter_mc:
+            self.h2d_bytes += (px * self.nrefs + 8 * self.F
+                               + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * mvgrid.MV_PT_DTYPE.itemsize)
+            if self.mc_next:
+                self.h2d_bytes += 4 * self.F + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * 8
+        if self._ll_slot is not None:
+            self.h2d_bytes += 4 * self.F
+        return out
+
     def submit(self):
         self._check(self.L.daala_b200_kf_submit(self.kf, ctypes.byref(self._io)), "kf_submit")
 
@@ -510,11 +586,13 @@ class KeyframeEngine:
         return idx.nbytes + blocks * sym.BLOCK_DTYPE.itemsize + int(idx[:, 3].sum()) * 8 + int(idx[:, 5].sum()) + dc
 
     def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None, pred=None, refs=None,
-               ref_slot=None, mv_grid=None, resident=False, mv1_grid=None, frame_quant=None):
+               ref_slot=None, mv_grid=None, resident=False, mv1_grid=None, frame_quant=None, ll_ref_slot_out=None):
         """One batch end to end through the C ABI with host buffers; returns the result arrays (views of
         the engine's host buffers: copy what must survive the next call).  pred: see stage_inputs; refs, ref_slot,
         mv_grid, resident, mv1_grid (inter_mc engines, which also return the prediction as pred0..2): see stage_mc;
-        frame_quant (frame_quant engines, required there): [F] FRAME_QUANT_DTYPE records, see stage_frame_quant.  Raises
+        frame_quant (frame_quant engines, required there): [F] FRAME_QUANT_DTYPE records, see stage_frame_quant;
+        ll_ref_slot_out (lossless engines with inter_mc): see stage_ll_ref_slot_out.  On a lossless engine bsize is not
+        read (None is fine) and the results are those of _prepare_io_lossless.  Raises
         when the batch exceeded the block capacity, or (inter_mc) when a used vertex names a picture other than GOLD /
         PREV (/ NEXT on mc_next engines) or a vector reaches past the reference's edge extension: the reference
         encoder's result is undefined there."""
@@ -525,6 +603,7 @@ class KeyframeEngine:
         if self.dering == 1:
             self.stage_dering_levels(dering_levels)
         self.stage_frame_quant(frame_quant)
+        self.stage_ll_ref_slot_out(ll_ref_slot_out)
         self.prepare_io(symbols, recon, stream)
         self.submit()
         out = self.wait()

@@ -533,12 +533,37 @@ typedef struct daala_b200_kf_config {
                                   stream settings use_masking, qm / qm_inv, qm_is_flat and pvq_norm_lambda stay
                                   engine-wide: the frames of one batch must share them.  Requires inter = 1; other
                                   values, and 1 without inter, are refused by daala_b200_kf_create */
+  int lossless;                /* 0 (default): nothing below exists; the engine is exactly the one without this field.
+                                  1: every frame is coded at quantizer 0 (OD_SET_QUANT 0), the reference's lossless
+                                  Haar-wavelet path (OD_LOSSLESS, src/internal.h:131): every superblock is one 64x64 block
+                                  (32x32 in 4:2:0 chroma), c = pixel - 128, d = od_haar(c), no lapping, no deringing,
+                                  a quantizer of 1 everywhere.  The step returns each block's residual
+                                  (daala_b200_kf_io.ll_coeffs), the three root sums the host's tree coder starts from
+                                  (daala_b200_kf_ll_block) and the reconstruction the decoder makes, which equals the
+                                  (padded) input.  Keyframes (inter = 0): the residual is d, its DC the difference to the
+                                  superblock DC predictor of od_quantize_haar_dc_sb (src/encode.c:1537-1590).  P and B
+                                  frames (inter = 1, prediction planes from the host or made by inter_mc [+ mc_next]):
+                                  outside the picture the input is replaced by the prediction (src/encode.c:2589-2602),
+                                  the residual is d - od_haar(prediction), DC included.  q0, pvq_qm_q4, the other
+                                  quantizer fields and io.bsize are not read.  Refused by daala_b200_kf_create with a
+                                  value other than 0 or 1, and 1 together with dering, symbol_stream, late_skip,
+                                  inter_finish, frame_quant, noref_prepass, level_chains or a row shard (sb_rows > 0) */
 } daala_b200_kf_config;
+
+/* config.lossless: the root sums of one block (od_compute_max_tree, src/encode.c:899-919, over the residual of
+   daala_b200_kf_io.ll_coeffs): what od_wavelet_quantize codes first (src/encode.c:1029-1049).  tree[0] is the tree of
+   the horizontal root (x, y) = (1, 0) (tree_sum[0][1]: every sub-band at column offset 1 << level, row offset 0),
+   tree[1] that of (0, 1) (tree_sum[1][0]), tree[2] that of (1, 1) (tree_sum[1][1]); each is the sum of |residual| over
+   its sub-bands.  The DC is in no tree. */
+typedef struct daala_b200_kf_ll_block {   /* 16 bytes */
+  int32_t tree[3];
+  int32_t reserved;        /* 0 */
+} daala_b200_kf_ll_block;
 
 /* config.frame_quant = 1: the quantizer of one frame of a batch, what od_enc_rc_select_quantizers_and_lambdas
    (reference src/rate.c:727-835, :1086) left in state / enc for that frame, and the pvq_qm_q4 table in force
-   (src/encode.c:3050-3075).  Submit refuses a record with q0 outside [1, 8191] (8191 = od_codedquantizer_to_quantizer(63):
-   lossless frames are not coded by the engine), coded_quantizer outside [1, 63], a dering_lambda that is negative or
+   (src/encode.c:3050-3075).  Submit refuses a record with q0 outside [1, 8191] (8191 = od_codedquantizer_to_quantizer(63);
+   lossless frames, quantizer 0, are coded by an engine with config.lossless), coded_quantizer outside [1, 63], a dering_lambda that is negative or
    not finite, or a pvq_qm_q4 entry of 0. */
 typedef struct daala_b200_kf_frame_quant {   /* 112 bytes, 8-byte aligned */
   int32_t q0;                 /* max(1, state->quantizer) of this frame */
@@ -707,6 +732,18 @@ typedef struct daala_b200_kf_io {
      frame_quant[f].  They go to the device with the step's other inputs; the finishing pass after the step uses the
      same records. */
   const daala_b200_kf_frame_quant *frame_quant;
+  /* config.lossless only (refused otherwise; each optional, NULL = not copied).  ll_coeffs[p]: [nframes][plane_h][plane_w]
+     int16, each block's residual in raster order at the block's own place (the layout of the `d` planes); the DC slot
+     holds the coded DC: d[0] minus the superblock DC predictor on keyframes, d[0] - md[0] on P and B frames.  Every
+     value fits int16 (the bound is derived in DESIGN.md).  ll_blocks: [nframes][nvsb][nhsb][3] records, one per
+     superblock and plane.  The reconstruction goes to pixels_out. */
+  int16_t *ll_coeffs[3];
+  daala_b200_kf_ll_block *ll_blocks;
+  /* config.lossless with inter_mc only (refused otherwise; optional): [nframes] the pool slot that receives frame f's
+     reconstruction, -1 = not stored, as daala_b200_kf_finish_io.ref_slot_out does for a lossy step; entries must lie
+     in [-1, mc_refs) and name distinct slots.  The stored slots then hold a picture (ref_resident).  The step's own
+     prediction is made before the store, so a frame may name its own PREV slot. */
+  const int32_t *ll_ref_slot_out;
 } daala_b200_kf_io;
 
 /* The finishing pass of a P-frame batch (config.inter_finish), daala_b200_kf_finish: the host coder's per-block
@@ -842,7 +879,9 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    pixels outside the plane (counts[20]; with mc_next the window of the vector the corner reads, mv1 on NEXT
    vertices), where the reference encoder's result is undefined.  With config.frame_quant it refuses a NULL
    frame_quant and a record out of range (see daala_b200_kf_frame_quant); frame_quant given to an engine without
-   config.frame_quant is refused. */
+   config.frame_quant is refused.  ll_coeffs, ll_blocks and ll_ref_slot_out are refused on an engine without
+   config.lossless, and ll_ref_slot_out also without inter_mc, with an entry outside [-1, mc_refs) or with two frames
+   naming one slot.  A lossless engine reads neither bsize nor totals, and returns none of the PVQ outputs. */
 int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
 /* What submit derives on the host from the n records of a config.frame_quant step (no GPU involved, no validation):
    tbl[f][0][g] / tbl[f][1][g] (nullable) the luma / chroma deringing threshold of level g for frame f,
