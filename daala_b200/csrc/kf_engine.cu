@@ -45,6 +45,7 @@
 #include "dering_search.h"
 #include "late_skip.h"
 #include "lossless.h"
+#include "haar_dc.h"
 #include "mc_batch.h"
 #include "gen/coding_order.inc"
 #include "pvq_math.cuh"
@@ -531,7 +532,8 @@ struct Stage {
   const double* rsqrt_tbl;         // [kTableDoubles] the reference's 1/sqrt(i) and theta-rate terms (pvq_fill_rsqrt_table)
   int16_t* res_pack;               // [nblocks*9][4]: gain, itheta, max_theta, k (what the coder reads)
   // keyframe chroma: the CfL source, the luma stage's coding-order input (its DC) and output (the quantised
-  // coefficients), and Lists::unit_loff; NULL otherwise
+  // coefficients), and Lists::unit_loff; NULL otherwise.  config.haar_dc_quant: cfl_in is, in both keyframe stages,
+  // the DC chain's grids of reconstructed DCs (hdc_grid), which the kHdc instantiations read in place of in[0]
   const int32_t* cfl_in;
   const int32_t* cfl_out;
   const int32_t* cfl_loff;
@@ -583,6 +585,13 @@ __device__ __noinline__ void trace_item(const Stage& S, uint32_t item, int kind,
 }
 #endif
 
+// config.haar_dc_quant: the DC chain's grid of plane `pli` of frame `frame` (one entry per 4x4 unit, the leaf DCs at the
+// leaf origins).  The grids of a frame lie together, planes 0, 1, 2: daala_b200_haar_dc_batch.grid_frame_pitch.
+__device__ __forceinline__ const int32_t* hdc_grid(const Stage& S, int frame, int pli) {
+  const long long g0 = S.prm.plane_frame_pitch[0] >> 4, g1 = S.prm.plane_frame_pitch[1] >> 4;
+  return S.cfl_in + frame * (g0 + 2 * g1) + (pli ? g0 + (pli - 1) * g1 : 0);
+}
+
 // OD_CFL_SCALING4 (src/intra.c), indexed [column][row]
 __constant__ int kCflScaling4[4][4] = {{128, 128, 100, 36}, {128, 80, 71, 35}, {100, 71, 35, 31}, {36, 35, 31, 18}};
 
@@ -590,19 +599,25 @@ __constant__ int kCflScaling4[4][4] = {{128, 128, 100, 36}, {128, 80, 71, 35}, {
 // src/intra.c:72), read from the luma stage's coding-order buffers; `lo` is the coding offset of the co-located luma.
 // Every block size codes the same nested layout (scan_rc does not depend on it) and a chroma block codes no more
 // coefficients than its luma block (512 at most), so chroma index i is luma index i.  Position 0 is the luma DC of
-// the plane k_finish_scatter writes on keyframes, the unquantised Haar DC in[0].
+// the plane k_finish_scatter writes on keyframes, the unquantised Haar DC in[0]; kHdc (config.haar_dc_quant): the
+// quantised DC of the luma block at that place, from the DC chain's luma grid.
+template <bool kHdc = false>
 __device__ __forceinline__ int32_t cfl_ref(const Stage& S, const daala_b200_pvq_block& b, int lo, int i) {
-  if (!(b.xdec & 0x80)) return i == 0 ? S.cfl_in[lo] : S.cfl_out[lo + i];
+  // luma 4x4 unit (u, v) of the block's co-located luma, in the luma grid of the block's frame
+  auto ldc = [&](int u, int v) {
+    return hdc_grid(S, b.frame, 0)[(long long)((b.y0 >> 1) + v) * (S.prm.plane_stride[0] >> 2) + (b.x0 >> 1) + u];
+  };
+  if (!(b.xdec & 0x80)) return i == 0 ? (kHdc ? ldc(0, 0) : S.cfl_in[lo]) : S.cfl_out[lo + i];
   // four 4x4 luma blocks (k_unit_emit: block q = 2 row + column, coefficients at lo + 16 q) -> one 4x4 chroma
   // prediction: od_tf_up_hv_lp (src/tf.c:82) + OD_CFL_SCALING4.  Output (r, c) comes from sample (r >> 1, c >> 1)
   // of each luma block; kScan4 lists rasters 4, 1, 5 first, so sample (y, x) of a 4x4 block is coefficient y + 2 x.
   int r = 0, c = 0;
   if (i) scan_rc(i, &r, &c);
   const int y = r >> 1, x = c >> 1, at = y + 2 * x;
-  int ll = at ? S.cfl_out[lo + at] : S.cfl_in[lo];
-  int lh = at ? S.cfl_out[lo + 16 + at] : S.cfl_in[lo + 16];
-  int hl = at ? S.cfl_out[lo + 32 + at] : S.cfl_in[lo + 32];
-  int hh = at ? S.cfl_out[lo + 48 + at] : S.cfl_in[lo + 48];
+  int ll = at ? S.cfl_out[lo + at] : kHdc ? ldc(0, 0) : S.cfl_in[lo];
+  int lh = at ? S.cfl_out[lo + 16 + at] : kHdc ? ldc(1, 0) : S.cfl_in[lo + 16];
+  int hl = at ? S.cfl_out[lo + 32 + at] : kHdc ? ldc(0, 1) : S.cfl_in[lo + 32];
+  int hh = at ? S.cfl_out[lo + 48 + at] : kHdc ? ldc(1, 1) : S.cfl_in[lo + 48];
   ll += lh; hh -= hl;
   const int t = (ll - hh) >> 1;
   hl = t - hl; lh = t - lh;
@@ -617,7 +632,7 @@ __device__ __forceinline__ int32_t cfl_ref(const Stage& S, const daala_b200_pvq_
 // also the CfL prediction and its sign flip (src/pvq_encoder.c:847-871); inter frames, all planes alike: the
 // reference vector is the transformed prediction md (prm.pred_plane), never flipped.  One warp per block.
 enum { kGatherLuma = 0, kGatherChroma = 1, kGatherInter = 2 };
-template <int kKind>
+template <int kKind, bool kHdc = false>
 __global__ void __launch_bounds__(256) k_gather(const __grid_constant__ Stage S) {
   const daala_b200_pvq_params& prm = S.prm;
   const int n = min(S.cnt[S.n_blocks_at], S.max_blocks);
@@ -649,7 +664,7 @@ __global__ void __launch_bounds__(256) k_gather(const __grid_constant__ Stage S)
       int32_t xy = 0;
       for (int i = lane; i < len; i += 32) {
         const int32_t vi = i == 0 ? src[0] : src[scan_to_raster(i, ln, stride)];
-        const int32_t vr = cfl_ref(S, b, lo, i);
+        const int32_t vr = cfl_ref<kHdc>(S, b, lo, i);
         vin[i] = vi;
         vref[i] = vr;
         if (i >= 1 && i < 16) {
@@ -1108,7 +1123,9 @@ __global__ void k_begin_pvq(int32_t* cnt, int stages) {
 // kInter: DC is the scalar quantisation of in[0] - ref[0] with the band-0 quantiser (od_block_encode's
 // non-keyframe branch; the index goes to prm.res_dc), and the uncoded tail of 32x32 / 64x64 blocks is the
 // transformed prediction (od_init_skipped_coeffs for inter frames).
-template <bool kInter>
+// kHdc (keyframes with config.haar_dc_quant): the DC is the quantised one the DC chain left in its grid, into out[0]
+// and the coefficient plane.
+template <bool kInter, bool kHdc = false>
 __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ Stage S) {
   const daala_b200_pvq_params& prm = S.prm;
   const int n = min(S.cnt[S.n_blocks_at], S.max_blocks);
@@ -1126,7 +1143,9 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
       double sd = 0;
       for (int i = 0; i < nb; i++) sd += prm.res_skip_term[(size_t)blk * 9 + i];
       prm.res_skip_diff[blk] = sd;
-      if (!kInter) {
+      if (kHdc) {
+        prm.out[b.coef_off] = dst[0] = hdc_grid(S, b.frame, b.pli)[(long long)(b.y0 >> 2) * (stride >> 2) + (b.x0 >> 2)];
+      } else if (!kInter) {
         prm.out[b.coef_off] = prm.in[b.coef_off];
       } else {
         int dc_quant = band_q(prm, S.fq, b.frame, b.pli, b.bs * (b.bs + 1));
@@ -1672,7 +1691,7 @@ struct Dering {
 };
 
 // The events of kf_enqueue_step_forked, one per fork or join.
-enum { kEvLists, kEvForward, kEvLumaBands, kEvLumaScatter, kEvChroma, kNumEvents };
+enum { kEvLists, kEvForward, kEvLumaBands, kEvLumaScatter, kEvChroma, kEvHaarDc, kNumEvents };
 
 struct daala_b200_kf {
   daala_b200_kf_config cfg;
@@ -1711,6 +1730,7 @@ struct daala_b200_kf {
   Stage luma, chroma;
   Sym sym;                         // symbol stream (cfg.symbol_stream); zero otherwise
   daala_b200_frame frame;
+  daala_b200_frame frame_fwd;      // keyframes: `frame` for the forward transform, which always builds the DC pyramid
   daala_b200_frame frame_pred;     // cfg.inter: `frame` with the prediction planes as the forward transform's input / output
   // cfg.inter_mc: the reference-picture pool, slot map, MV grids and per-MV-block leaf segments
   uint8_t* ref_pixels[3];
@@ -1763,6 +1783,11 @@ struct daala_b200_kf {
   int32_t* ll_dc;
   int32_t* ll_slot_out;
   daala_b200_lossless_batch ll;
+  // cfg.haar_dc_quant: the DC chain's grids (reconstructed DCs of all planes, frame by frame; signed indices per plane)
+  // and its launch parameters
+  int32_t* hdc;
+  int32_t* hdc_index[3];
+  daala_b200_haar_dc_batch hdcb;
   std::vector<uint8_t> slot_filled;  // cfg.inter_mc, per pool slot: something has written a picture there
   bool have_step;                  // a step has been submitted; last_tot are its totals
   daala_b200_kf_totals last_tot;
@@ -2096,6 +2121,29 @@ static int kf_alloc(daala_b200_kf* kf) {
     C.cfl_out = kf->luma.prm.out;
     C.cfl_loff = L.unit_loff;
   }
+  if (kf->cfg.haar_dc_quant) {
+    daala_b200_haar_dc_batch& H = kf->hdcb;
+    memset(&H, 0, sizeof(H));
+    const size_t g0 = (size_t)(kf->plane_w[0] >> 2) * (kf->plane_h[0] >> 2), g1 = (size_t)(kf->plane_w[1] >> 2) * (kf->plane_h[1] >> 2);
+    KF_CHECK(dalloc(kf, &kf->hdc, (g0 + 2 * g1) * F));
+    H.grid_frame_pitch = (long long)(g0 + 2 * g1);
+    kf->luma.cfl_in = kf->chroma.cfl_in = kf->hdc;
+    for (int p = 0; p < 3; p++) {
+      KF_CHECK(dalloc(kf, &kf->hdc_index[p], (p ? g1 : g0) * F));
+      H.coeffs[p] = kf->coeffs[p];
+      H.dc[p] = kf->hdc + (p ? g0 + (p - 1) * g1 : 0);
+      H.index[p] = kf->hdc_index[p];
+      H.plane_w[p] = kf->plane_w[p];
+      H.plane_h[p] = kf->plane_h[p];
+      // od_quantize_haar_dc_sb / _level: max(1, quantizer * pvq_qm_q4[pli][od_qm_get_index(OD_NBSIZES - 1, 0)] >> 4)
+      H.dc_quant[p] = std::max(1, kf->cfg.q0 * kf->cfg.pvq_qm_q4[p][20] >> 4);
+    }
+    H.bsize = kf->bsize;
+    H.F = F;
+    H.nhsb = kf->nhsb;
+    H.nvsb = kf->nvsb;
+    H.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
+  }
   (void)luma_px;
   // the unquantised DC residual per block: what the host's od_rdo_quant needs, returned classically (inter_finish) or
   // in the stream's DC records (symbol_stream = 2)
@@ -2210,11 +2258,15 @@ static int kf_alloc(daala_b200_kf* kf) {
   f.nvsb = kf->nvsb;
   f.pic_w = kf->cfg.pic_w;
   f.pic_h = kf->cfg.pic_h;
-  f.haar_dc = inter ? 0 : 1;
+  // haar_dc_quant: the leaf DCs the finishing scatter stores are final, as on P frames, so the inverse skips the
+  // pyramid; the forward (frame_fwd) still builds it for the DC chain
+  f.haar_dc = inter || kf->cfg.haar_dc_quant ? 0 : 1;
   f.nframes = F;
   f.sb_row0 = kf->cfg.sb_row0;
   f.sb_rows = kf->cfg.sb_rows;
   kf->frame_pred = f;
+  kf->frame_fwd = f;
+  kf->frame_fwd.haar_dc = inter ? 0 : 1;
   for (int p = 0; p < 3; p++) {
     kf->frame_pred.plane[p].pixels = kf->pred_pixels[p];
     kf->frame_pred.plane[p].coeffs = kf->pred_coeffs[p];
@@ -2561,12 +2613,15 @@ static int enqueue_luma_bands(daala_b200_kf* kf, bool core, int begin, cudaStrea
 // the luma bands, not the luma scatter), the bands, the scatter into the coefficient planes.
 static void enqueue_chroma(daala_b200_kf* kf, bool core, bool begin, cudaStream_t s) {
   const int wide = kf->sms * 8;
+  const bool hdc = kf->cfg.haar_dc_quant != 0;
   if (begin) k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, kBeginChroma);
-  if (!core) k_gather<kGatherChroma><<<wide, 256, 0, s>>>(kf->chroma);
+  if (!core && hdc) k_gather<kGatherChroma, true><<<wide, 256, 0, s>>>(kf->chroma);
+  else if (!core) k_gather<kGatherChroma><<<wide, 256, 0, s>>>(kf->chroma);
   if (kf->cfg.split_free > 0) enqueue_split<false>(kf, kf->chroma, s);
   else k_pvq_persist<false><<<kf->sms * (kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas),
                               kPersistThreads, 0, s>>>(kf->chroma);
-  if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->chroma);
+  if (!core && hdc) k_finish_scatter<false, true><<<wide, 256, 0, s>>>(kf->chroma);
+  else if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->chroma);
 }
 
 // The whole keyframe step (DAALA_B200_KF_ALL) as two branches, kf->stream and kf->side, forked and joined with
@@ -2576,6 +2631,8 @@ static void enqueue_chroma(daala_b200_kf* kf, bool core, bool begin, cudaStream_
 //   kf->side: chroma stage, [symbol stream, after the luma scatter], inverse + SB postfilter of planes 1-2;
 //   kf->stream: luma scatter, inverse + SB postfilter of plane 0, [level search, thresholds, od_dering of plane 0];
 //   join; [od_dering of planes 1-2: they read the direction map plane 0 writes].
+// haar_dc_quant: the DC chain runs on kf->side right after the forward transform, after kEvForward is recorded, so the
+// luma bands do not wait for it; the chroma stage follows it by stream order and the luma scatter waits for kEvHaarDc.
 // The branches write disjoint buffers; only the order of independent work differs from the phase-by-phase path.
 static int kf_enqueue_step_forked(daala_b200_kf* kf) {
   cudaStream_t s = kf->stream, c = kf->side;
@@ -2584,17 +2641,28 @@ static int kf_enqueue_step_forked(daala_b200_kf* kf) {
     return cudaEventRecord(e, from) == cudaSuccess && cudaStreamWaitEvent(to, e, 0) == cudaSuccess;
   };
   if (!fork(kf->ev[kEvLists], s, c)) return (int)cudaGetLastError();
-  int rc = daala_b200_launch_forward(&kf->frame, 3, c);
+  int rc = daala_b200_launch_forward(&kf->frame_fwd, 3, c);
   if (!rc) rc = enqueue_lists(kf, s);
   if (rc) return rc;
   if (!fork(kf->ev[kEvForward], c, s)) return (int)cudaGetLastError();
+  const bool hdc = kf->cfg.haar_dc_quant != 0;
+  if (hdc) {
+    rc = daala_b200_launch_haar_dc(&kf->hdcb, c);
+    if (rc) return rc;
+    if (cudaEventRecord(kf->ev[kEvHaarDc], c) != cudaSuccess) return (int)cudaGetLastError();
+  }
   rc = enqueue_luma_bands(kf, false, kBeginLuma | kBeginChroma, s);
   if (rc) return rc;
   if (!fork(kf->ev[kEvLumaBands], s, c)) return (int)cudaGetLastError();
   enqueue_chroma(kf, false, false, c);
   // 16 waves of short CTAs instead of one resident wave: priority only orders CTAs that are still waiting, so a grid
   // that fits the GPU at once would hold every SM until it is done and stall the chroma gather behind it
-  k_finish_scatter<false><<<kf->sms * 128, 256, 0, s>>>(kf->luma);
+  if (hdc) {
+    if (cudaStreamWaitEvent(s, kf->ev[kEvHaarDc], 0) != cudaSuccess) return (int)cudaGetLastError();
+    k_finish_scatter<false, true><<<kf->sms * 128, 256, 0, s>>>(kf->luma);
+  } else {
+    k_finish_scatter<false><<<kf->sms * 128, 256, 0, s>>>(kf->luma);
+  }
   if (kf->cfg.symbol_stream) {
     if (!fork(kf->ev[kEvLumaScatter], s, c)) return (int)cudaGetLastError();
     enqueue_sym<false>(kf->sym, kf->sms * 8, c);
@@ -2639,14 +2707,16 @@ static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
     if (rc) return rc;
   }
   if (phases & DAALA_B200_KF_FORWARD) {
-    const int rc = daala_b200_launch_forward(&kf->frame, 3, s);
+    int rc = daala_b200_launch_forward(&kf->frame_fwd, 3, s);
+    if (!rc && kf->cfg.haar_dc_quant) rc = daala_b200_launch_haar_dc(&kf->hdcb, s);
     if (rc) return rc;
   }
   const bool core = (phases & DAALA_B200_KF_SEARCH_ONLY) != 0;
   if (phases & DAALA_B200_KF_PVQ_LUMA) {
     const int rc = enqueue_luma_bands(kf, core, kBeginLuma, s);
     if (rc) return rc;
-    if (!core) k_finish_scatter<false><<<kf->sms * 8, 256, 0, s>>>(kf->luma);
+    if (!core && kf->cfg.haar_dc_quant) k_finish_scatter<false, true><<<kf->sms * 8, 256, 0, s>>>(kf->luma);
+    else if (!core) k_finish_scatter<false><<<kf->sms * 8, 256, 0, s>>>(kf->luma);
   }
   if (phases & DAALA_B200_KF_PVQ_CHROMA) {
     enqueue_chroma(kf, core, true, s);
@@ -2727,6 +2797,18 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
                        : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
     if (with) {
       snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: lossless is not defined with %s", with);
+      return nullptr;
+    }
+  }
+  if (cfg && cfg->haar_dc_quant) {
+    // the chain quantises the Haar DC pyramid of lossy keyframes; the superblock predictor reads the superblocks above,
+    // across any row shard
+    const char* with = cfg->haar_dc_quant != 1 ? "a value other than 0 or 1"
+                       : cfg->inter ? "inter (P and B frames code a scalar DC per block)"
+                       : cfg->lossless ? "lossless (its keyframe DCs are coded exactly)"
+                       : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
+    if (with) {
+      snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: haar_dc_quant is not defined with %s", with);
       return nullptr;
     }
   }
@@ -2855,7 +2937,7 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
     return 5 + 2 + (2 + split(kf->luma)) + (2 + split(kf->chroma)) + 2 + (kf->cfg.inter_mc ? 2 : 0) +
            (kf->cfg.symbol_stream ? 8 : 0) + (kf->cfg.late_skip ? kLateSkipLaunches : 0);
   int n = 5 + (kf->cfg.level_chains ? 2 : 0);                                    // work lists
-  n += 1;                                                                         // forward
+  n += 1 + (kf->cfg.haar_dc_quant ? 1 : 0);                                       // forward, [DC chain]
   n += 3 + 1 + (kf->cfg.split_free > 1 ? split(kf->luma) : 0) + (kf->luma.pre_ev ? 2 : 0);   // luma: begin (both stages), gather, [prepass], chains, finish
   n += 2 + (kf->cfg.split_free > 0 ? split(kf->chroma) : 1);                      // chroma: gather, bands, finish
   // inverse + SB postfilter of plane 0 and of planes 1-2, [the rest of the deringing pass]
@@ -2913,6 +2995,10 @@ int daala_b200_kf_device_buffers(daala_b200_kf* kf, daala_b200_kf_buffers* out) 
   out->ref_slot_next = kf->ref_slot_next;
   out->mv1_grid = kf->mv1_grid;
   out->frame_quant = kf->fq;
+  for (int p = 0; p < 3; p++) {
+    out->haar_dc[p] = kf->hdcb.dc[p];
+    out->dc_index[p] = kf->hdc_index[p];
+  }
   return 0;
 }
 
@@ -3063,6 +3149,10 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   }
   if (ll_why) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", ll_why);
+    return (int)cudaErrorInvalidValue;
+  }
+  if ((io->dc_index[0] || io->dc_index[1] || io->dc_index[2]) && !kf->cfg.haar_dc_quant) {
+    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: dc_index needs an engine with haar_dc_quant = 1");
     return (int)cudaErrorInvalidValue;
   }
   if (kf->cfg.inter && !kf->cfg.inter_mc &&
@@ -3294,6 +3384,10 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     KF_CHECK(cudaMemcpyAsync(io->chroma_late_skip, kf->late_skip[1], sizeof(daala_b200_kf_late_skip) * tot.n_chroma,
                              cudaMemcpyDeviceToHost, s));
   if (io->counts) KF_CHECK(cudaMemcpyAsync(io->counts, kf->lists.cnt, sizeof(int32_t) * 32, cudaMemcpyDeviceToHost, s));
+  for (int p = 0; p < 3; p++)
+    if (io->dc_index[p])
+      KF_CHECK(cudaMemcpyAsync(io->dc_index[p], kf->hdc_index[p],
+                               sizeof(int32_t) * (kf->plane_w[p] >> 2) * (kf->plane_h[p] >> 2) * F, cudaMemcpyDeviceToHost, s));
   if (io->dering_level_out && kf->cfg.dering)
     KF_CHECK(cudaMemcpyAsync(io->dering_level_out, kf->dering.level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyDeviceToHost, s));
   if (want_sym) {

@@ -29,6 +29,10 @@ inter=1 and host or inter_mc prediction): `encode` takes no block-size map and r
 (`ll_coeffs0..2`, int16 planes), the three root tree sums of every block (`ll_blocks`, [F, nvsb, nhsb, 3, 4] int32) and
 the reconstruction; `encode(..., ll_ref_slot_out=)` stores each frame's reconstruction into a pool slot (inter_mc).
 daala_b200/lossless.py restates the path in numpy.
+With haar_dc_quant=1 (keyframes) the step quantises the keyframe DCs as the reference encoder does (its superblock DC
+predictor and Haar-level quantiser, with the adaptive DC rate): the reconstruction, the coefficient planes and the CfL
+reference carry the quantised DCs, and `encode` returns the coded indices as dc_index0..2 ([F, h / 4, w / 4] int32 per
+plane).  daala_b200/haardc.py restates the chain in numpy.
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -54,7 +58,7 @@ class Config(ctypes.Structure):
                 ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
                 ("symbol_stream", c_int), ("inter", c_int), ("inter_mc", c_int), ("mc_refs", c_int),
                 ("inter_finish", c_int), ("late_skip", c_int), ("mc_next", c_int), ("frame_quant", c_int),
-                ("lossless", c_int)]
+                ("lossless", c_int), ("haar_dc_quant", c_int)]
 
 
 # daala_b200_kf_frame_quant: one frame's quantizer on a frame_quant engine
@@ -97,7 +101,7 @@ class IO(ctypes.Structure):
                 ("luma_late_skip", c_void_p), ("chroma_late_skip", c_void_p), ("sym_late_skip", c_void_p),
                 ("sym_late_skip_cap", c_ll), ("ref_slot_next", c_void_p), ("mv1_grid", c_void_p),
                 ("frame_quant", c_void_p), ("ll_coeffs", c_void_p * 3), ("ll_blocks", c_void_p),
-                ("ll_ref_slot_out", c_void_p)]
+                ("ll_ref_slot_out", c_void_p), ("dc_index", c_void_p * 3)]
 
 
 class FinishIO(ctypes.Structure):
@@ -123,7 +127,8 @@ class Buffers(ctypes.Structure):
                 ("bytes_allocated", c_ll), ("pred_pixels", c_void_p * 3), ("pred_coeffs", c_void_p * 3),
                 ("luma_heads_raw", c_void_p), ("luma_head_bin", c_void_p), ("ref_pixels", c_void_p * 3),
                 ("ref_slot", c_void_p), ("mv_grid", c_void_p), ("mc_refs", c_int), ("ref_slot_next", c_void_p),
-                ("mv1_grid", c_void_p), ("frame_quant", c_void_p)]
+                ("mv1_grid", c_void_p), ("frame_quant", c_void_p), ("haar_dc", c_void_p * 3),
+                ("dc_index", c_void_p * 3)]
 
 
 def _bind():
@@ -192,7 +197,7 @@ class KeyframeEngine:
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
                  qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=0, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
                  qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0, inter_mc=0, mc_refs=0,
-                 inter_finish=0, late_skip=0, mc_next=0, frame_quant=0, lossless=0):
+                 inter_finish=0, late_skip=0, mc_next=0, frame_quant=0, lossless=0, haar_dc_quant=0):
         self.L = _bind()
         self.geom, self.F = geom, nframes
         if qm is None:
@@ -243,6 +248,9 @@ class KeyframeEngine:
         # lossless: quantizer 0 (the Haar-wavelet path); q0, pvq_qm_q4 and the block-size maps are not read
         cfg.lossless = int(lossless)
         self.lossless = int(lossless)
+        # haar_dc_quant: keyframe DCs quantised on the device, indices returned as dc_index0..2
+        cfg.haar_dc_quant = int(haar_dc_quant)
+        self.haar_dc_quant = int(haar_dc_quant)
         self._ll_slot = None
         self.nrefs = 0
         self.resident = False
@@ -473,6 +481,11 @@ class KeyframeEngine:
             io.frame_quant = self._fq.ctypes.data
         if self._ll_slot is not None:   # refused by the C call: a lossy engine has no lossless step
             io.ll_ref_slot_out = self._ll_slot.ctypes.data
+        if self.haar_dc_quant:
+            for p in range(3):
+                h, w = g.plane_shape(p)
+                out["dc_index%d" % p] = self._arr("dci%d" % p, (self.F, h >> 2, w >> 2), np.int32)
+                io.dc_index[p] = out["dc_index%d" % p].ctypes.data
         out["counts"] = self._arr("cnt", (32,), np.int32)
         io.counts = out["counts"].ctypes.data
         if self.dering:

@@ -548,6 +548,17 @@ typedef struct daala_b200_kf_config {
                                   quantizer fields and io.bsize are not read.  Refused by daala_b200_kf_create with a
                                   value other than 0 or 1, and 1 together with dering, symbol_stream, late_skip,
                                   inter_finish, frame_quant, noref_prepass, level_chains or a row shard (sb_rows > 0) */
+  int haar_dc_quant;           /* 0 (default): keyframes are reconstructed with their unquantised DCs (the inverse
+                                  undoes the forward transform's Haar DC pyramid); nothing below exists.
+                                  1: the step quantises the keyframe DCs as the reference encoder does: per plane,
+                                  od_quantize_haar_dc_sb and od_quantize_haar_dc_level (src/encode.c:1537-1657, with the
+                                  RDO increment rated on the adapting DC model) in od_encode_recursive's order, one warp
+                                  per (frame, plane) beside the luma chain kernel.  The coefficient planes, out[0] of
+                                  every block, the 4x4-chroma CfL reference and the reconstruction then carry the
+                                  quantised DCs; daala_b200_kf_io.dc_index returns the coded indices.  q0, pvq_qm_q4 and
+                                  pvq_norm_lambda are the chain's quantizer and lambda.  Refused by daala_b200_kf_create
+                                  with a value other than 0 or 1, and 1 together with inter, lossless or a row shard
+                                  (sb_rows > 0: the superblock predictor reads the row above) */
 } daala_b200_kf_config;
 
 /* config.lossless: the root sums of one block (od_compute_max_tree, src/encode.c:899-919, over the residual of
@@ -744,6 +755,12 @@ typedef struct daala_b200_kf_io {
      in [-1, mc_refs) and name distinct slots.  The stored slots then hold a picture (ref_resident).  The step's own
      prediction is made before the store, so a frame may name its own PREV slot. */
   const int32_t *ll_ref_slot_out;
+  /* config.haar_dc_quant only (refused otherwise; each optional, NULL = not copied): [nframes][plane_h / 4][plane_w / 4]
+     int32, plane p's signed keyframe DC indices at 4x4 granularity: a superblock's DC index at the superblock's origin,
+     the three indices of a split node (its children's Haar coefficients x[1], x[2], x[3]) at the origins of its
+     children 1, 2, 3 (top right, bottom left, bottom right), 0 everywhere else.  INTEGRATION.md describes the order
+     the coder reads them in. */
+  int32_t *dc_index[3];
 } daala_b200_kf_io;
 
 /* The finishing pass of a P-frame batch (config.inter_finish), daala_b200_kf_finish: the host coder's per-block
@@ -834,6 +851,10 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
   int32_t *ref_slot_next;               /* config.mc_next: the NEXT slots ([nframes]) and the mv1 grids */
   int32_t *mv1_grid;                    /* ([nframes][nvsb*8 + 1][nhsb*8 + 1][2]); NULL otherwise */
   daala_b200_kf_frame_quant *frame_quant;   /* config.frame_quant: the step's records ([nframes]); NULL otherwise */
+  int32_t *haar_dc[3];                  /* config.haar_dc_quant: the DC chain's reconstructed DCs per plane, one entry per
+                                           4x4 unit (leaf DCs at leaf origins), the three planes of a frame together
+                                           (frame f of plane p at haar_dc[p] + f * (g0 + 2 g1), g = plane grid size) */
+  int32_t *dc_index[3];                 /* and the index grids ([nframes][plane_h / 4][plane_w / 4]); else NULL */
 } daala_b200_kf_buffers;
 
 #define DAALA_B200_KF_LISTS 1
