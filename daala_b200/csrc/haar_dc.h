@@ -18,6 +18,9 @@ struct daala_b200_haar_dc_batch {
   long long grid_frame_pitch;  // entries between the DC grids of consecutive frames
   int dc_quant[3];            // max(1, q0 * pvq_qm_q4[pli][od_qm_get_index(4, 0)] >> 4)
   double pvq_norm_lambda;
+  // config.keyframe_quant: each frame's band quantisers ([F][3][32], max(1, q0 * pvq_qm_q4[pli][i] >> 4) of its
+  // record); frame f's dc_quant of plane p is entry [f][p][20], and dc_quant[] is not read.  NULL otherwise.
+  const int32_t* fq_bq;
 };
 
 // One warp per (frame, plane): grid F * 3.

@@ -537,8 +537,15 @@ struct Stage {
   const int32_t* cfl_in;
   const int32_t* cfl_out;
   const int32_t* cfl_loff;
-  int32_t* dc_resid;               // config.inter_finish or symbol_stream = 2: per block in[0] - ref[0], else NULL
-  const daala_b200_kf_frame_quant* fq;   // config.frame_quant: [F] the step's records (band_q), else NULL
+  // Two modes that never meet share one slot, so that the parameter block of the kernels that read neither keeps its
+  // layout: inter engines have no keyframe_quant, and keyframe engines neither inter_finish nor symbol_stream = 2.
+  union {
+    int32_t* dc_resid;             // config.inter_finish or symbol_stream = 2: per block in[0] - ref[0], else NULL
+    // config.keyframe_quant: [F][3][32] each frame's band quantisers max(1, q0 * pvq_qm_q4[pli][i] >> 4), filled on the
+    // host from the records (what k_pvq_persist_fq reads: one load per item)
+    const int32_t* fq_bq;
+  };
+  const daala_b200_kf_frame_quant* fq;   // config.frame_quant / keyframe_quant: [F] the step's records (band_q), else NULL
 #ifdef DAALA_B200_CHAIN_TRACE
   struct ChainTraceRec* trace;     // luma: one record per item k_pvq_persist<true> runs, up to trace_cap
   int trace_cap;
@@ -814,8 +821,9 @@ __device__ __forceinline__ void intra_band_ref(const Stage& S, int blk, int band
 }
 
 // One (block, band) item by one warp.  kIntra: the band's prediction is built from the quantised
-// neighbours first (od_hv_intra_pred, src/intra.c:37-62).
-template <bool kIntra>
+// neighbours first (od_hv_intra_pred, src/intra.c:37-62).  kFq (config.keyframe_quant): the band quantiser is the
+// block's frame's entry of S.fq_bq.
+template <bool kIntra, bool kFq = false>
 __device__ __forceinline__ void run_item(const Stage& S, uint32_t item, int lane, int16_t* snap) {
   const daala_b200_pvq_params& prm = S.prm;
   const int blk = (int)(item >> 4), band = (int)(item & 15);
@@ -826,8 +834,13 @@ __device__ __forceinline__ void run_item(const Stage& S, uint32_t item, int lane
   const size_t off = (size_t)b.coef_off + start;
   if (kIntra) intra_band_ref(S, blk, band, b.coef_off, lane);
   int qidx = bs * (bs + 1) + (band + 1) - (band + 1) / 3;
-  int q = (prm.q0 * prm.pvq_qm_q4[pli][qidx]) >> 4;
-  if (q < 1) q = 1;
+  int q;
+  if (kFq) {
+    q = S.fq_bq[(b.frame * 3 + pli) * 32 + qidx];
+  } else {
+    q = (prm.q0 * prm.pvq_qm_q4[pli][qidx]) >> 4;
+    if (q < 1) q = 1;
+  }
   const int beta = (prm.use_masking && pli == 0 && bs > 0) ? kBeta15 : kBeta1;
   const int qoff = (b.xdec & 1 ? prm.qm_stride : 0) + ((((1 << (2 * bs)) - 1) << 4) / 3) + start;
   int itheta, max_theta, k;
@@ -885,7 +898,7 @@ __device__ __forceinline__ ItemGeom item_geom(const daala_b200_pvq_params& prm, 
 
 // kPhase 0 / 1 / 2 = setup / search / finish of the items [chunk * slots, ...) of class `cls`.
 // kZeroRef: the prediction is all zero (luma bands 3 / 6).  kFq: the band quantisers come from the records of
-// config.frame_quant (S.fq); an instantiation of its own, so that the other engines run exactly the kernels they did.
+// config.frame_quant / keyframe_quant (S.fq); an instantiation of its own, so that the other engines run exactly the kernels they did.
 template <int kPhase, bool kZeroRef, int kMode, bool kFq = false>
 __global__ void __launch_bounds__(128) k_pvq_split(const __grid_constant__ Stage S, int cls, int chunk) {
   const daala_b200_pvq_params& prm = S.prm;
@@ -1031,13 +1044,11 @@ __global__ void __launch_bounds__(128, 4) k_pvq_levels(const __grid_constant__ S
 // intra predictor form a dependency graph (per size class: band 0 a 2-D wavefront, bands 1/4/7 columns,
 // bands 2/5/8 rows).  A warp that finishes a chain item CONTINUES with a successor it made ready -- a
 // column or row is walked by one warp without touching the queue -- and pushes a second ready
-// successor (band 0 forks) into the chain queue.
-template <bool kIntra>
-__global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(const __grid_constant__ Stage S) {
-  // per warp: the pulses of every search event of a band and the band's parked context (quantise_band_warp)
-  __shared__ __align__(16) int16_t snap_all[kPersistThreads / 32][kSnapEntries];
+// successor (band 0 forks) into the chain queue.  The body of k_pvq_persist and k_pvq_persist_fq; `snap` is the
+// warp's shared scratch.
+template <bool kIntra, bool kFq>
+__device__ __forceinline__ void persist_items(const Stage& S, int16_t* snap) {
   const int lane = threadIdx.x & 31;
-  int16_t* snap = snap_all[threadIdx.x >> 5];
   int done = 0;
   bool waiter = false;
   for (;;) {
@@ -1051,7 +1062,7 @@ __global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(c
 #ifdef DAALA_B200_CHAIN_TRACE
       const unsigned long long t0 = globaltimer();
 #endif
-      run_item<kIntra>(S, item, lane, snap);
+      run_item<kIntra, kFq>(S, item, lane, snap);
 #ifdef DAALA_B200_CHAIN_TRACE
       if (kIntra) trace_item(S, item, kind, t0, lane);
       kind = 3;
@@ -1089,6 +1100,21 @@ __global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(c
       item = next;
     }
   }
+}
+
+template <bool kIntra>
+__global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(const __grid_constant__ Stage S) {
+  // per warp: the pulses of every search event of a band and the band's parked context (quantise_band_warp)
+  __shared__ __align__(16) int16_t snap_all[kPersistThreads / 32][kSnapEntries];
+  persist_items<kIntra, false>(S, snap_all[threadIdx.x >> 5]);
+}
+
+// config.keyframe_quant: the same walk with each band's quantiser from its frame's record (S.fq_bq).  A kernel of its
+// own, so that the other engines run exactly the kernel they did.
+template <bool kIntra>
+__global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist_fq(const __grid_constant__ Stage S) {
+  __shared__ __align__(16) int16_t snap_all[kPersistThreads / 32][kSnapEntries];
+  persist_items<kIntra, true>(S, snap_all[threadIdx.x >> 5]);
 }
 
 __global__ void k_fill_rsqrt(double* tbl) {
@@ -1184,7 +1210,7 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
 // (the deringing kernel stores the u8 reconstruction itself).
 // thr[pl][f][sb] = table[pl][level[f][sb]].  P-frame finishing pass: `coded` (else NULL) flags the superblocks with a
 // coded 4x4 luma unit; the others are forced to level 0 (src/encode.c:2724-2738), and the level applied goes to
-// `applied`.  config.frame_quant: `frame_tbl` ([F][2][6], else NULL) holds each frame's table, the frame of superblock
+// `applied`.  config.frame_quant / keyframe_quant: `frame_tbl` ([F][2][6], else NULL) holds each frame's table, the frame of superblock
 // i being i / nsb.
 __global__ void k_dering_thresholds(const uint8_t* __restrict__ level, int32_t* __restrict__ thr_luma,
                                     int32_t* __restrict__ thr_chroma, int n, int4 tl_lo, int2 tl_hi, int4 tc_lo, int2 tc_hi,
@@ -1683,7 +1709,7 @@ struct Dering {
   const uint8_t* coded;            // nullable: superblocks with a coded luma 4x4 unit; the others get level 0 ...
   uint8_t* applied;                // ... and the level applied lands here
   int tbl[2][6];                   // luma / chroma threshold per level
-  const int32_t* frame_tbl;        // config.frame_quant: [F][2][6] tbl of each frame (replaces tbl), else NULL
+  const int32_t* frame_tbl;        // frame_quant / keyframe_quant: [F][2][6] tbl of each frame (replaces tbl), else NULL
   int32_t* thr[2];                 // luma / chroma threshold per superblock
   int32_t* dir;                    // [F][nvsb*8][nhsb*8]
   bool search;                     // the level search runs first, described by `sb`
@@ -1756,11 +1782,14 @@ struct daala_b200_kf {
   bool fin_captured;
   int fin_dc_limit;                // largest |dc| finish accepts: DAALA_B200_KF_FINISH_DC_LIMIT / the largest dc_quant
                                    // (config.frame_quant: of the last step's records, set by submit)
-  // config.frame_quant: the step's records and the deringing threshold table of each frame ([F][2][6], computed on the
+  // frame_quant / keyframe_quant: the step's records and the deringing threshold table of each frame ([F][2][6], computed on the
   // host from the records' q0 as daala_b200_dering_threshold_table does), uploaded by submit
   daala_b200_kf_frame_quant* fq;
   int32_t* fq_tbl;
   std::vector<int32_t> fq_tbl_host;
+  // config.keyframe_quant: each frame's band quantisers ([F][3][32], Stage::fq_bq), computed on the host by submit
+  int32_t* fq_bq;
+  std::vector<int32_t> fq_bq_host;
   // cfg.inter_mc with cfg.inter_finish: the pool slot of each frame's reconstruction (finish_io.ref_slot_out, -1 = not
   // stored) and the store that reads it
   int32_t* fin_slot_out;
@@ -1919,10 +1948,14 @@ static int kf_alloc(daala_b200_kf* kf) {
     const int rc = mc_alloc(kf);
     if (rc) return rc;
   }
-  if (kf->cfg.frame_quant) {
+  if (kf->cfg.frame_quant || kf->cfg.keyframe_quant) {
     KF_CHECK(dalloc(kf, &kf->fq, (size_t)F));
     KF_CHECK(dalloc(kf, &kf->fq_tbl, (size_t)F * 12));
     kf->fq_tbl_host.assign((size_t)F * 12, 0);
+  }
+  if (kf->cfg.keyframe_quant) {
+    KF_CHECK(dalloc(kf, &kf->fq_bq, (size_t)F * 96));
+    kf->fq_bq_host.assign((size_t)F * 96, 1);
   }
   KF_CHECK(dalloc(kf, &kf->qm, (size_t)2 * kf->cfg.qm_stride));
   KF_CHECK(dalloc(kf, &kf->qm_inv, (size_t)2 * kf->cfg.qm_stride));
@@ -2016,6 +2049,19 @@ static int kf_alloc(daala_b200_kf* kf) {
                per_sm[1], want);
       return (int)cudaErrorLaunchOutOfResources;
     }
+    if (kf->cfg.keyframe_quant) {
+      KF_CHECK(cudaFuncSetAttribute(k_pvq_persist_fq<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                    cudaSharedmemCarveoutMaxShared));
+      KF_CHECK(cudaFuncSetAttribute(k_pvq_persist_fq<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                    cudaSharedmemCarveoutMaxShared));
+      KF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[0], k_pvq_persist_fq<true>, kPersistThreads, 0));
+      KF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[1], k_pvq_persist_fq<false>, kPersistThreads, 0));
+      if (per_sm[0] < want || per_sm[1] < want) {
+        snprintf(kf->err, sizeof(kf->err), "k_pvq_persist_fq: %d / %d CTAs per SM resident, %d wanted", per_sm[0],
+                 per_sm[1], want);
+        return (int)cudaErrorLaunchOutOfResources;
+      }
+    }
   }
   KF_CHECK(dalloc(kf, &L.heads, inter ? 0 : kf->chain_cap));
   KF_CHECK(dalloc(kf, &L.heads_raw, inter ? 0 : kf->chain_cap));
@@ -2060,6 +2106,7 @@ static int kf_alloc(daala_b200_kf* kf) {
     p.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
     memcpy(p.pvq_qm_q4, kf->cfg.pvq_qm_q4, sizeof(p.pvq_qm_q4));
     S.fq = kf->fq;
+    if (kf->cfg.keyframe_quant) S.fq_bq = kf->fq_bq;
     for (int c = 0; c < 3; c++) S.items[c] = chroma ? L.items_c[c] : L.items_l[c];
     S.cnt = L.cnt;
     S.rsqrt_tbl = kf->rsqrt_tbl;
@@ -2143,6 +2190,7 @@ static int kf_alloc(daala_b200_kf* kf) {
     H.nhsb = kf->nhsb;
     H.nvsb = kf->nvsb;
     H.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
+    H.fq_bq = kf->fq_bq;   // keyframe_quant: each frame's dc_quant is its entry [f][pli][20], dc_quant[] is not read
   }
   (void)luma_px;
   // the unquantised DC residual per block: what the host's od_rdo_quant needs, returned classically (inter_finish) or
@@ -2398,7 +2446,7 @@ static int kf_alloc(daala_b200_kf* kf) {
       KF_CHECK(dalloc(kf, &b.dist, nsb * 6));
       b.dir = D.dir;
       b.levels = D.level;   // what the thresholds read; on P frames its level 0 agrees with the forced one
-      if (kf->cfg.frame_quant) {
+      if (kf->cfg.frame_quant || kf->cfg.keyframe_quant) {
         b.fq = kf->fq;
         b.frame_tbl = kf->fq_tbl;
         KF_CHECK(dalloc(kf, &b.cand_thr, nsb * 5));
@@ -2475,8 +2523,10 @@ static int enqueue_dering(daala_b200_kf* kf, const Dering& D, cudaStream_t s) {
 
 // Kernel launches of enqueue_dering with the inverse in `parts` plane ranges: inverse, SB postfilter -> int16 per
 // range, [level search: 5 filtered candidates, 6 packs, 6 distortion passes, decision], thresholds, dering + u8
-// store per plane.
-static int dering_launches(const Dering& D, int parts) { return 2 * parts + (D.search ? 5 + 6 + 6 + 1 : 0) + 1 + 3; }
+// store per plane; per-frame quantizers add the candidates' thresholds to the search.
+static int dering_launches(const Dering& D, int parts) {
+  return 2 * parts + (D.search ? 5 + 6 + 6 + 1 + (D.sb.frame_tbl ? 1 : 0) : 0) + 1 + 3;
+}
 
 // Everything between "inputs are in HBM" and "results are in HBM", on kf->stream.
 // the three phase kernels over every chunk of every class of a stage's dependency-free lists
@@ -2595,7 +2645,9 @@ static int enqueue_luma_bands(daala_b200_kf* kf, bool core, int begin, cudaStrea
     return (int)cudaGetLastError();
   k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, begin);
   if (!core) k_gather<kGatherLuma><<<wide, 256, 0, s>>>(kf->luma);
-  if (kf->cfg.split_free > 1) enqueue_split<true>(kf, kf->luma, s);
+  const bool kfq = kf->cfg.keyframe_quant != 0;
+  if (kf->cfg.split_free > 1 && kfq) enqueue_split<true, true>(kf, kf->luma, s);
+  else if (kf->cfg.split_free > 1) enqueue_split<true>(kf, kf->luma, s);
   if (kf->luma.pre_ev) {
     k_pvq_prepass<2><<<kf->sms * 16, 128, 0, s>>>(kf->luma);
     k_pvq_prepass<1><<<kf->sms * 16, 128, 0, s>>>(kf->luma);
@@ -2603,6 +2655,8 @@ static int enqueue_luma_bands(daala_b200_kf* kf, bool core, int begin, cudaStrea
   if (kf->cfg.level_chains) {
     if (cudaMemsetAsync(kf->lv_bar, 0, sizeof(int32_t) * 32, s) != cudaSuccess) return (int)cudaGetLastError();
     k_pvq_levels<<<kf->lvl_grid, 128, 0, s>>>(kf->luma);
+  } else if (kfq) {
+    k_pvq_persist_fq<true><<<persist, kPersistThreads, 0, s>>>(kf->luma);
   } else {
     k_pvq_persist<true><<<persist, kPersistThreads, 0, s>>>(kf->luma);
   }
@@ -2617,9 +2671,12 @@ static void enqueue_chroma(daala_b200_kf* kf, bool core, bool begin, cudaStream_
   if (begin) k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, kBeginChroma);
   if (!core && hdc) k_gather<kGatherChroma, true><<<wide, 256, 0, s>>>(kf->chroma);
   else if (!core) k_gather<kGatherChroma><<<wide, 256, 0, s>>>(kf->chroma);
-  if (kf->cfg.split_free > 0) enqueue_split<false>(kf, kf->chroma, s);
-  else k_pvq_persist<false><<<kf->sms * (kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas),
-                              kPersistThreads, 0, s>>>(kf->chroma);
+  const bool kfq = kf->cfg.keyframe_quant != 0;
+  const int persist = kf->sms * (kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas);
+  if (kf->cfg.split_free > 0 && kfq) enqueue_split<false, true>(kf, kf->chroma, s);
+  else if (kf->cfg.split_free > 0) enqueue_split<false>(kf, kf->chroma, s);
+  else if (kfq) k_pvq_persist_fq<false><<<persist, kPersistThreads, 0, s>>>(kf->chroma);
+  else k_pvq_persist<false><<<persist, kPersistThreads, 0, s>>>(kf->chroma);
   if (!core && hdc) k_finish_scatter<false, true><<<wide, 256, 0, s>>>(kf->chroma);
   else if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->chroma);
 }
@@ -2781,8 +2838,21 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   }
   if (cfg && cfg->frame_quant && (cfg->frame_quant != 1 || cfg->inter != 1)) {
     snprintf(g_create_err, sizeof(g_create_err),
-             "daala_b200_kf_create: frame_quant is 0 or 1, and 1 requires inter = 1 (a keyframe batch shares one quantizer)");
+             "daala_b200_kf_create: frame_quant is 0 or 1, and 1 requires inter = 1 (keyframes: keyframe_quant = 1)");
     return nullptr;
+  }
+  if (cfg && cfg->keyframe_quant) {
+    // the kernels that read the quantizer in these modes have no per-frame form
+    const char* with = cfg->keyframe_quant != 1 ? "a value other than 0 or 1"
+                       : cfg->inter ? "inter (P and B frames take their records with frame_quant = 1)"
+                       : cfg->lossless ? "lossless (every frame is at quantizer 0)"
+                       : cfg->noref_prepass ? "noref_prepass"
+                       : cfg->level_chains ? "level_chains"
+                       : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
+    if (with) {
+      snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: keyframe_quant is not defined with %s", with);
+      return nullptr;
+    }
   }
   if (cfg && cfg->lossless) {
     // the lossless path has no PVQ, no deringing and no coder-side state: none of these stages exists for it
@@ -3112,6 +3182,55 @@ static int sym_target(const void* p, long long cap, long long need, uint8_t** de
 static std::mutex g_compute_mu;
 static cudaEvent_t g_last_compute = nullptr;
 
+// The records of a frame_quant / keyframe_quant step: why they are refused, or nullptr when every one is in range; then
+// the host tables hold each frame's deringing thresholds (daala_b200_kf_frame_quant_derive) and, with keyframe_quant,
+// its band quantisers, and *dc_limit is the finishing pass's DC limit.
+static const char* fq_derive_host(daala_b200_kf* kf, const daala_b200_kf_frame_quant* rec, int* dc_limit) {
+  if (!rec) return "frame_quant: the records ([nframes]) are required";
+  const int F = kf->F;
+  for (int f = 0; f < F; f++) {
+    const daala_b200_kf_frame_quant& r = rec[f];
+    if (r.q0 < 1 || r.q0 > DAALA_B200_KF_MAX_Q0) return "a record's q0 is outside [1, 8191]";
+    if (r.coded_quantizer < 1 || r.coded_quantizer > 63) return "a record's coded_quantizer is outside [1, 63]";
+    if (!std::isfinite(r.dering_lambda) || r.dering_lambda < 0) return "a record's dering_lambda is negative or not finite";
+    for (int p = 0; p < 3; p++)
+      for (int i = 0; i < 30; i++)   // OD_QM_SIZE entries are read
+        if (r.pvq_qm_q4[p][i] < 1) return "a record's pvq_qm_q4 entry is 0";
+  }
+  *dc_limit = daala_b200_kf_frame_quant_derive(rec, F, reinterpret_cast<int32_t(*)[2][6]>(kf->fq_tbl_host.data()));
+  if (kf->cfg.keyframe_quant)
+    for (int f = 0; f < F; f++)
+      for (int p = 0; p < 3; p++)
+        for (int i = 0; i < 30; i++)
+          kf->fq_bq_host[(size_t)(f * 3 + p) * 32 + i] = std::max(1, (rec[f].q0 * rec[f].pvq_qm_q4[p][i]) >> 4);
+  return nullptr;
+}
+
+// The H2D of the records fq_derive_host accepted and of its tables, on `s`.
+static cudaError_t fq_copy(daala_b200_kf* kf, const daala_b200_kf_frame_quant* rec, cudaStream_t s) {
+  const int F = kf->F;
+  cudaError_t e = cudaMemcpyAsync(kf->fq, rec, sizeof(daala_b200_kf_frame_quant) * F, cudaMemcpyHostToDevice, s);
+  if (!e) e = cudaMemcpyAsync(kf->fq_tbl, kf->fq_tbl_host.data(), sizeof(int32_t) * 12 * F, cudaMemcpyHostToDevice, s);
+  if (!e && kf->fq_bq)
+    e = cudaMemcpyAsync(kf->fq_bq, kf->fq_bq_host.data(), sizeof(int32_t) * 96 * F, cudaMemcpyHostToDevice, s);
+  return e;
+}
+
+int daala_b200_kf_load_frame_quant(daala_b200_kf* kf, const daala_b200_kf_frame_quant* rec) {
+  if (!kf) return (int)cudaErrorInvalidValue;
+  int dc_limit = 0;
+  const char* why = !kf->cfg.frame_quant && !kf->cfg.keyframe_quant
+                        ? "needs an engine with frame_quant = 1 or keyframe_quant = 1"
+                        : fq_derive_host(kf, rec, &dc_limit);
+  if (why) {
+    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_load_frame_quant: %s", why);
+    return (int)cudaErrorInvalidValue;
+  }
+  KF_CHECK(fq_copy(kf, rec, kf->stream));
+  KF_CHECK(cudaStreamSynchronize(kf->stream));   // the host tables are reused by the next call
+  return 0;
+}
+
 int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   if (!kf || !io) return (int)cudaErrorInvalidValue;
   cudaStream_t s = kf->stream;
@@ -3211,31 +3330,17 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", ls_why);
     return (int)cudaErrorInvalidValue;
   }
-  // per-frame quantizers: every record in range; then each frame's deringing thresholds and the finishing pass's DC
-  // limit of this step (daala_b200_kf_frame_quant_derive)
+  // per-frame quantizers: every record in range; then each frame's deringing thresholds [and band quantisers] and the
+  // finishing pass's DC limit of this step
   int fq_dc_limit = 0;
-  if (io->frame_quant || kf->cfg.frame_quant) {
-    const char* why = !kf->cfg.frame_quant ? "frame_quant needs an engine with frame_quant = 1"
-                      : !io->frame_quant  ? "frame_quant: the records ([nframes]) are required"
-                                          : nullptr;
-    for (int f = 0; !why && f < F; f++) {
-      const daala_b200_kf_frame_quant& r = io->frame_quant[f];
-      if (r.q0 < 1 || r.q0 > DAALA_B200_KF_MAX_Q0) why = "a record's q0 is outside [1, 8191]";
-      else if (r.coded_quantizer < 1 || r.coded_quantizer > 63) why = "a record's coded_quantizer is outside [1, 63]";
-      else if (!std::isfinite(r.dering_lambda) || r.dering_lambda < 0) why = "a record's dering_lambda is negative or not finite";
-      for (int p = 0; !why && p < 3; p++)
-        for (int i = 0; i < 30; i++)   // OD_QM_SIZE entries are read
-          if (r.pvq_qm_q4[p][i] < 1) {
-            why = "a record's pvq_qm_q4 entry is 0";
-            break;
-          }
-    }
+  const bool fq_mode = kf->cfg.frame_quant || kf->cfg.keyframe_quant;
+  if (io->frame_quant || fq_mode) {
+    const char* why = !fq_mode ? "frame_quant needs an engine with frame_quant = 1 or keyframe_quant = 1"
+                               : fq_derive_host(kf, io->frame_quant, &fq_dc_limit);
     if (why) {
       snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", why);
       return (int)cudaErrorInvalidValue;
     }
-    fq_dc_limit = daala_b200_kf_frame_quant_derive(io->frame_quant, F,
-                                                   reinterpret_cast<int32_t(*)[2][6]>(kf->fq_tbl_host.data()));
   }
   // symbol stream: the engine must produce it, and every requested buffer must hold the worst case and be pinned
   SymCopy sc;
@@ -3312,10 +3417,7 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
                                cudaMemcpyHostToDevice, s));
     }
   }
-  if (kf->cfg.frame_quant) {
-    KF_CHECK(cudaMemcpyAsync(kf->fq, io->frame_quant, sizeof(daala_b200_kf_frame_quant) * F, cudaMemcpyHostToDevice, s));
-    KF_CHECK(cudaMemcpyAsync(kf->fq_tbl, kf->fq_tbl_host.data(), sizeof(int32_t) * 12 * F, cudaMemcpyHostToDevice, s));
-  }
+  if (fq_mode) KF_CHECK(fq_copy(kf, io->frame_quant, s));
   const size_t map_bytes = (size_t)kf->nhsb * 8 * kf->nvsb * 8 * F;
   if (!lossless) KF_CHECK(cudaMemcpyAsync(kf->bsize, io->bsize, map_bytes, cudaMemcpyHostToDevice, s));
   // the graph's lossless kernels read the slot table: NULL stores nothing (every entry -1)

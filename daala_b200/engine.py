@@ -24,6 +24,9 @@ B-frame order and buffer rotation).
 With inter=1 and frame_quant=1 every frame of a batch has its own quantizer: `encode(..., frame_quant=)` takes one
 FRAME_QUANT_DTYPE record per frame (frame_quant_records builds them) in place of the engine-wide q0, coded_quantizer,
 dering_lambda and pvq_qm_q4, so P and B frames of different types or streams share one batch.
+With keyframe_quant=1 (keyframes) the same records code every keyframe of a batch at its own quantizer: the keyframes
+of several streams, or several sweep points of one, share one step.  use_masking, qm and pvq_norm_lambda stay
+engine-wide (stream settings).
 With lossless=1 every frame is coded at quantizer 0, the reference's Haar-wavelet path (keyframes, or P / B frames with
 inter=1 and host or inter_mc prediction): `encode` takes no block-size map and returns each block's residual
 (`ll_coeffs0..2`, int16 planes), the three root tree sums of every block (`ll_blocks`, [F, nvsb, nhsb, 3, 4] int32) and
@@ -58,10 +61,11 @@ class Config(ctypes.Structure):
                 ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
                 ("symbol_stream", c_int), ("inter", c_int), ("inter_mc", c_int), ("mc_refs", c_int),
                 ("inter_finish", c_int), ("late_skip", c_int), ("mc_next", c_int), ("frame_quant", c_int),
-                ("lossless", c_int), ("haar_dc_quant", c_int)]
+                ("lossless", c_int), ("haar_dc_quant", c_int), ("keyframe_quant", c_int)]
 
 
-# daala_b200_kf_frame_quant: one frame's quantizer on a frame_quant engine
+# daala_b200_kf_frame_quant: one frame's quantizer on a frame_quant or keyframe_quant engine.  A keyframe's record:
+# q0 = max(1, state->quantizer), state->coded_quantizer, enc->dering_lambda and the pvq_qm_q4 od_interp_qm set for it
 FRAME_QUANT_DTYPE = np.dtype([("q0", "<i4"), ("coded_quantizer", "<i4"), ("dering_lambda", "<f8"),
                               ("pvq_qm_q4", "u1", (3, 32))])
 MAX_Q0 = 8191   # od_codedquantizer_to_quantizer(63), the largest quantizer a record may carry
@@ -153,6 +157,7 @@ def _bind():
     L.daala_b200_kf_pool_load.argtypes = [c_void_p, c_int, ctypes.POINTER(c_void_p)]
     L.daala_b200_kf_symbol_bounds.argtypes = [ctypes.POINTER(Totals), c_int, ctypes.POINTER(SymBounds)]
     L.daala_b200_kf_frame_quant_derive.argtypes = [c_void_p, c_int, c_void_p]
+    L.daala_b200_kf_load_frame_quant.argtypes = [c_void_p, c_void_p]
     L.daala_b200_kf_wait.argtypes = [c_void_p]
     L.daala_b200_device_copy.argtypes = [c_void_p, c_void_p, ctypes.c_size_t, c_int]
     L.daala_b200_host_alloc.argtypes = [ctypes.c_size_t]
@@ -197,7 +202,7 @@ class KeyframeEngine:
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
                  qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=0, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
                  qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0, inter_mc=0, mc_refs=0,
-                 inter_finish=0, late_skip=0, mc_next=0, frame_quant=0, lossless=0, haar_dc_quant=0):
+                 inter_finish=0, late_skip=0, mc_next=0, frame_quant=0, lossless=0, haar_dc_quant=0, keyframe_quant=0):
         self.L = _bind()
         self.geom, self.F = geom, nframes
         if qm is None:
@@ -251,6 +256,9 @@ class KeyframeEngine:
         # haar_dc_quant: keyframe DCs quantised on the device, indices returned as dc_index0..2
         cfg.haar_dc_quant = int(haar_dc_quant)
         self.haar_dc_quant = int(haar_dc_quant)
+        # keyframe_quant: keyframes take one FRAME_QUANT_DTYPE record per frame, as frame_quant engines do
+        cfg.keyframe_quant = int(keyframe_quant)
+        self.keyframe_quant = int(keyframe_quant)
         self._ll_slot = None
         self.nrefs = 0
         self.resident = False
@@ -369,8 +377,8 @@ class KeyframeEngine:
             a[...] = mv1_grid
 
     def stage_frame_quant(self, records):
-        """Copies the [F] FRAME_QUANT_DTYPE records of one batch into the host buffers (frame_quant engines; the C call
-        refuses them elsewhere).  None: the next step is submitted without records."""
+        """Copies the [F] FRAME_QUANT_DTYPE records of one batch into the host buffers (frame_quant and keyframe_quant
+        engines; the C call refuses them elsewhere).  None: the next step is submitted without records."""
         if records is None:
             self._fq = None
             return
@@ -519,6 +527,8 @@ class KeyframeEngine:
                 self.h2d_bytes += 4 * self.F + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * 8
         if self._fq is not None:   # the records and each frame's deringing threshold table (int32 [2][6])
             self.h2d_bytes += self.F * (FRAME_QUANT_DTYPE.itemsize + 48)
+            if self.keyframe_quant:   # and its band quantisers (int32 [3][32])
+                self.h2d_bytes += self.F * 384
         return out
 
     def stage_ll_ref_slot_out(self, slots):
@@ -603,7 +613,8 @@ class KeyframeEngine:
         """One batch end to end through the C ABI with host buffers; returns the result arrays (views of
         the engine's host buffers: copy what must survive the next call).  pred: see stage_inputs; refs, ref_slot,
         mv_grid, resident, mv1_grid (inter_mc engines, which also return the prediction as pred0..2): see stage_mc;
-        frame_quant (frame_quant engines, required there): [F] FRAME_QUANT_DTYPE records, see stage_frame_quant;
+        frame_quant (frame_quant and keyframe_quant engines, required there): [F] FRAME_QUANT_DTYPE records, see
+        stage_frame_quant;
         ll_ref_slot_out (lossless engines with inter_mc): see stage_ll_ref_slot_out.  On a lossless engine bsize is not
         read (None is fine) and the results are those of _prepare_io_lossless.  Raises
         when the batch exceeded the block capacity, or (inter_mc) when a used vertex names a picture other than GOLD /
@@ -742,16 +753,20 @@ class KeyframeEngine:
         return float(ms.value)
 
     def upload(self, planes, bsize, pred=None, frame_quant=None):
-        """Copies one batch straight into the engine's device buffers for run_device; frame_quant (frame_quant
-        engines): the [F] FRAME_QUANT_DTYPE records the step's kernels read."""
+        """Copies one batch straight into the engine's device buffers for run_device; frame_quant (frame_quant and
+        keyframe_quant engines): the [F] FRAME_QUANT_DTYPE records the step's kernels read (keyframe_quant: checked and
+        loaded with the tables submit derives from them, daala_b200_kf_load_frame_quant)."""
         g = self.geom
         self._check_pred(pred)
         if frame_quant is not None:
-            if not self.frame_quant:
-                raise ValueError("frame_quant= needs an engine created with frame_quant=1")
+            if not (self.frame_quant or self.keyframe_quant):
+                raise ValueError("frame_quant= needs an engine created with frame_quant=1 or keyframe_quant=1")
             r = np.ascontiguousarray(frame_quant, FRAME_QUANT_DTYPE)
             assert r.shape == (self.F,)
-            self._check(self.L.daala_b200_device_copy(self.buf.frame_quant, r.ctypes.data, r.nbytes, 0), "upload")
+            if self.keyframe_quant:
+                self._check(self.L.daala_b200_kf_load_frame_quant(self.kf, r.ctypes.data), "upload")
+            else:
+                self._check(self.L.daala_b200_device_copy(self.buf.frame_quant, r.ctypes.data, r.nbytes, 0), "upload")
         for p in range(3):
             for dst, src in ((self.buf.pixels[p], planes[p]),) + (((self.buf.pred_pixels[p], pred[p]),) if pred is not None else ()):
                 a = np.ascontiguousarray(src, np.uint8)

@@ -104,7 +104,9 @@ def pipelined_steps(frames):
     whose picture the P-frame engine's pool takes with pool_load); the B frames coded before it form a step of their
     own ahead of it, and so do B frames left at the end of the stream.  Inside a step every frame reads the pool before
     any frame's reconstruction is stored, which is what lets an anchor's SELF buffer be one that the step's B frames
-    still read."""
+    still read.  The I frames of several sequences may share one step of a keyframe engine with keyframe_quant = 1, each
+    at its own record; pool_load from that engine's reconstruction seeds each sequence's P engine as it does for a
+    keyframe coded alone."""
     steps, pending = [], []
     for fr in frames:
         if fr.type == B_FRAME:

@@ -559,6 +559,20 @@ typedef struct daala_b200_kf_config {
                                   pvq_norm_lambda are the chain's quantizer and lambda.  Refused by daala_b200_kf_create
                                   with a value other than 0 or 1, and 1 together with inter, lossless or a row shard
                                   (sb_rows > 0: the superblock predictor reads the row above) */
+  int keyframe_quant;          /* 0 (default): nothing below exists; the engine is exactly the one without this field.
+                                  1: the keyframe counterpart of frame_quant: every keyframe of a step has its own
+                                  quantizer, one daala_b200_kf_frame_quant per frame in daala_b200_kf_io.frame_quant.
+                                  The luma chain kernel, the phase kernels, the DC chain (haar_dc_quant) and the
+                                  deringing stage (its thresholds and, with dering = 2, the level search's distortion
+                                  scale and lambda) read the block's or superblock's frame's record, and the step reads
+                                  no per-frame field of this config (q0, coded_quantizer, dering_lambda, pvq_qm_q4).
+                                  use_masking, qm / qm_inv, qm_is_flat and pvq_norm_lambda stay engine-wide: they are
+                                  stream settings, and the frames of one batch must share them.  A host encoder fills
+                                  a keyframe's record with q0 = max(1, state->quantizer), state->coded_quantizer,
+                                  enc->dering_lambda and the pvq_qm_q4 od_interp_qm set for that keyframe (reference
+                                  src/encode.c:3050-3075).  Refused by daala_b200_kf_create with a value other than 0
+                                  or 1, and 1 together with inter (P and B frames have frame_quant), lossless,
+                                  noref_prepass, level_chains or a row shard (sb_rows > 0) */
 } daala_b200_kf_config;
 
 /* config.lossless: the root sums of one block (od_compute_max_tree, src/encode.c:899-919, over the residual of
@@ -571,7 +585,7 @@ typedef struct daala_b200_kf_ll_block {   /* 16 bytes */
   int32_t reserved;        /* 0 */
 } daala_b200_kf_ll_block;
 
-/* config.frame_quant = 1: the quantizer of one frame of a batch, what od_enc_rc_select_quantizers_and_lambdas
+/* config.frame_quant = 1 or config.keyframe_quant = 1: the quantizer of one frame of a batch, what od_enc_rc_select_quantizers_and_lambdas
    (reference src/rate.c:727-835, :1086) left in state / enc for that frame, and the pvq_qm_q4 table in force
    (src/encode.c:3050-3075).  Submit refuses a record with q0 outside [1, 8191] (8191 = od_codedquantizer_to_quantizer(63);
    lossless frames, quantizer 0, are coded by an engine with config.lossless), coded_quantizer outside [1, 63], a dering_lambda that is negative or
@@ -739,9 +753,9 @@ typedef struct daala_b200_kf_io {
   const int32_t *ref_slot_next;         /* [nframes]: pool slot of each frame's NEXT picture */
   const int32_t *mv1_grid;              /* [nframes][nvsb*8 + 1][nhsb*8 + 1][2]: each vertex's mv1 (od_mv_grid_pt.mv1,
                                            src/mc.h:73-84) in 1/8 luma pixel, read only where ref == 2 */
-  /* config.frame_quant = 1 only (required there, refused otherwise): [nframes] records, frame f coded at
-     frame_quant[f].  They go to the device with the step's other inputs; the finishing pass after the step uses the
-     same records. */
+  /* config.frame_quant = 1 or config.keyframe_quant = 1 only (required there, refused otherwise): [nframes] records,
+     frame f coded at frame_quant[f].  They go to the device with the step's other inputs; the finishing pass after the
+     step uses the same records. */
   const daala_b200_kf_frame_quant *frame_quant;
   /* config.lossless only (refused otherwise; each optional, NULL = not copied).  ll_coeffs[p]: [nframes][plane_h][plane_w]
      int16, each block's residual in raster order at the block's own place (the layout of the `d` planes); the DC slot
@@ -850,7 +864,8 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
   int mc_refs;                          /* pictures the pool holds (0 without inter_mc) */
   int32_t *ref_slot_next;               /* config.mc_next: the NEXT slots ([nframes]) and the mv1 grids */
   int32_t *mv1_grid;                    /* ([nframes][nvsb*8 + 1][nhsb*8 + 1][2]); NULL otherwise */
-  daala_b200_kf_frame_quant *frame_quant;   /* config.frame_quant: the step's records ([nframes]); NULL otherwise */
+  daala_b200_kf_frame_quant *frame_quant;   /* config.frame_quant or keyframe_quant: the step's records ([nframes]);
+                                               NULL otherwise */
   int32_t *haar_dc[3];                  /* config.haar_dc_quant: the DC chain's reconstructed DCs per plane, one entry per
                                            4x4 unit (leaf DCs at leaf origins), the three planes of a frame together
                                            (frame f of plane p at haar_dc[p] + f * (g0 + 2 g1), g = plane grid size) */
@@ -898,9 +913,9 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    `counts` the leaf corners whose vertex has a ref other than 0 or 1 (counts[19]; with mc_next other than 0, 1 or 2)
    and the corner windows (with the 6-tap filter's apron of -2..+3 pixels) that reach more than 64 luma / 32 chroma
    pixels outside the plane (counts[20]; with mc_next the window of the vector the corner reads, mv1 on NEXT
-   vertices), where the reference encoder's result is undefined.  With config.frame_quant it refuses a NULL
-   frame_quant and a record out of range (see daala_b200_kf_frame_quant); frame_quant given to an engine without
-   config.frame_quant is refused.  ll_coeffs, ll_blocks and ll_ref_slot_out are refused on an engine without
+   vertices), where the reference encoder's result is undefined.  With config.frame_quant or keyframe_quant it
+   refuses a NULL frame_quant and a record out of range (see daala_b200_kf_frame_quant); frame_quant given to an engine
+   with neither is refused.  ll_coeffs, ll_blocks and ll_ref_slot_out are refused on an engine without
    config.lossless, and ll_ref_slot_out also without inter_mc, with an entry outside [-1, mc_refs) or with two frames
    naming one slot.  A lossless engine reads neither bsize nor totals, and returns none of the PVQ outputs. */
 int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
@@ -910,6 +925,12 @@ int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
    frame's q0; the return value is the finishing pass's DC limit for the step, DAALA_B200_KF_FINISH_DC_LIMIT / the
    largest dc_quant over the records, planes and block sizes. */
 int daala_b200_kf_frame_quant_derive(const daala_b200_kf_frame_quant *rec, int n, int32_t (*tbl)[2][6]);
+/* config.frame_quant or keyframe_quant, for run_device without a submit: checks the [nframes] records as submit does
+   and copies them into the engine's device buffers with what submit derives from them (each frame's deringing
+   thresholds; keyframe_quant: each frame's band quantisers max(1, q0 * pvq_qm_q4[pli][i] >> 4), which the luma chain
+   kernel and the DC chain read), on the engine's stream, and waits for the copies.  The finishing pass's DC limit is
+   not changed (a submit sets it). */
+int daala_b200_kf_load_frame_quant(daala_b200_kf *kf, const daala_b200_kf_frame_quant *rec);
 /* The finishing pass (config.inter_finish, see daala_b200_kf_finish_io) on the last submitted step: H2D of the
    decisions and levels, the pass's kernels as one CUDA graph (captured at the first call; with config.inter_finish
    = 2 it includes the level search), D2H of the requested outputs; enqueued on the engine's stream like submit,
