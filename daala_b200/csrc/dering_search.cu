@@ -107,7 +107,7 @@ __global__ void k_dering_decide(const double* __restrict__ dist, int nframes, in
   }
 }
 
-// Per-frame thresholds (frame_quant / keyframe_quant): thr[gi - 1][f * nsb + sb] = frame_tbl[f][0][gi] for the five filtered
+// Per-frame thresholds (the engine's search): thr[gi - 1][f * nsb + sb] = frame_tbl[f][0][gi] for the five filtered
 // candidates, the per-superblock threshold maps their od_dering passes read.
 __global__ void k_cand_thresholds(const int32_t* __restrict__ frame_tbl, int n, int nsb, int32_t* __restrict__ thr) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -30,9 +30,9 @@ struct daala_b200_dering_search_batch {
   int32_t* dir;             // [F][nvsb * 8][nhsb * 8], left in the packed direction | variance << 3 format
   double* dist;             // [6][F * nsb]
   uint8_t* levels;          // out: [F][nvsb * nhsb]
-  // frame_quant / keyframe_quant (else NULL): per frame records (coded_quantizer and dering_lambda replace the fields above) and
-  // threshold tables ([F][2][6], replacing `threshold`), and the scratch of the filtered candidates' per-superblock
-  // thresholds, [5][F * nsb]
+  // the engine's (NULL in daala_b200_dering_search): per frame records (coded_quantizer and dering_lambda replace the
+  // fields above) and threshold tables ([F][2][6], replacing `threshold`), and the scratch of the filtered candidates'
+  // per-superblock thresholds, [5][F * nsb]
   const daala_b200_kf_frame_quant* fq;
   const int32_t* frame_tbl;
   int32_t* cand_thr;

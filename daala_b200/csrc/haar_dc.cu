@@ -63,9 +63,7 @@ struct Node {
   int hgrad, vgrad;
 };
 
-// kFq (config.keyframe_quant): the quantiser is that of the warp's frame, B.fq_bq; an instantiation of its own, so that
-// the other engines run exactly the kernel they did.
-template <bool kFq = false>
+// The quantiser is that of the warp's frame, B.fq_bq.
 __global__ void __launch_bounds__(32) k_haar_dc(const __grid_constant__ daala_b200_haar_dc_batch B) {
   extern __shared__ int sb_mem[];                 // [2][nhsb]: quantised SB DCs of the row above and of this row
   __shared__ int cdfs[kTables * 16];
@@ -87,7 +85,7 @@ __global__ void __launch_bounds__(32) k_haar_dc(const __grid_constant__ daala_b2
   int ex_dc[5][3];
   for (int i = 0; i < 5; i++)
     for (int j = 0; j < 3; j++) ex_dc[i][j] = ex0;
-  const int dq = kFq ? B.fq_bq[(f * 3 + pli) * 32 + 20] : B.dc_quant[pli];
+  const int dq = B.fq_bq[(f * 3 + pli) * 32 + 20];
   const double lam = B.pvq_norm_lambda;
   const int nhsb = B.nhsb;
   const int lsb = 6 - xdec;                       // log2 of the superblock edge in this plane
@@ -182,7 +180,6 @@ __global__ void __launch_bounds__(32) k_haar_dc(const __grid_constant__ daala_b2
 
 extern "C" int daala_b200_launch_haar_dc(const daala_b200_haar_dc_batch* b, cudaStream_t stream) {
   using namespace daala_b200::haar_dc;
-  if (b->fq_bq) k_haar_dc<true><<<b->F * 3, 32, sizeof(int) * 2 * b->nhsb, stream>>>(*b);
-  else k_haar_dc<<<b->F * 3, 32, sizeof(int) * 2 * b->nhsb, stream>>>(*b);
+  k_haar_dc<<<b->F * 3, 32, sizeof(int) * 2 * b->nhsb, stream>>>(*b);
   return (int)cudaGetLastError();
 }

@@ -16,10 +16,9 @@ struct daala_b200_haar_dc_batch {
   int F, nhsb, nvsb;
   int plane_w[3], plane_h[3];
   long long grid_frame_pitch;  // entries between the DC grids of consecutive frames
-  int dc_quant[3];            // max(1, q0 * pvq_qm_q4[pli][od_qm_get_index(4, 0)] >> 4)
   double pvq_norm_lambda;
-  // config.keyframe_quant: each frame's band quantisers ([F][3][32], max(1, q0 * pvq_qm_q4[pli][i] >> 4) of its
-  // record); frame f's dc_quant of plane p is entry [f][p][20], and dc_quant[] is not read.  NULL otherwise.
+  // each frame's band quantisers ([F][3][32], max(1, q0 * pvq_qm_q4[pli][i] >> 4) of its record); frame f's dc_quant of
+  // plane p is entry [f][p][20] (od_qm_get_index(OD_NBSIZES - 1, 0))
   const int32_t* fq_bq;
 };
 

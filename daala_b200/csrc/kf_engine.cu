@@ -537,15 +537,10 @@ struct Stage {
   const int32_t* cfl_in;
   const int32_t* cfl_out;
   const int32_t* cfl_loff;
-  // Two modes that never meet share one slot, so that the parameter block of the kernels that read neither keeps its
-  // layout: inter engines have no keyframe_quant, and keyframe engines neither inter_finish nor symbol_stream = 2.
-  union {
-    int32_t* dc_resid;             // config.inter_finish or symbol_stream = 2: per block in[0] - ref[0], else NULL
-    // config.keyframe_quant: [F][3][32] each frame's band quantisers max(1, q0 * pvq_qm_q4[pli][i] >> 4), filled on the
-    // host from the records (what k_pvq_persist_fq reads: one load per item)
-    const int32_t* fq_bq;
-  };
-  const daala_b200_kf_frame_quant* fq;   // config.frame_quant / keyframe_quant: [F] the step's records (band_q), else NULL
+  int32_t* dc_resid;               // config.inter_finish or symbol_stream = 2: per block in[0] - ref[0], else NULL
+  // [F][3][32] each frame's band quantisers max(1, q0 * pvq_qm_q4[pli][i] >> 4), filled on the host from the records
+  // (one load per item)
+  const int32_t* fq_bq;
 #ifdef DAALA_B200_CHAIN_TRACE
   struct ChainTraceRec* trace;     // luma: one record per item k_pvq_persist<true> runs, up to trace_cap
   int trace_cap;
@@ -821,9 +816,8 @@ __device__ __forceinline__ void intra_band_ref(const Stage& S, int blk, int band
 }
 
 // One (block, band) item by one warp.  kIntra: the band's prediction is built from the quantised
-// neighbours first (od_hv_intra_pred, src/intra.c:37-62).  kFq (config.keyframe_quant): the band quantiser is the
-// block's frame's entry of S.fq_bq.
-template <bool kIntra, bool kFq = false>
+// neighbours first (od_hv_intra_pred, src/intra.c:37-62).  The band quantiser is the block's frame's entry of S.fq_bq.
+template <bool kIntra>
 __device__ __forceinline__ void run_item(const Stage& S, uint32_t item, int lane, int16_t* snap) {
   const daala_b200_pvq_params& prm = S.prm;
   const int blk = (int)(item >> 4), band = (int)(item & 15);
@@ -833,14 +827,8 @@ __device__ __forceinline__ void run_item(const Stage& S, uint32_t item, int lane
   const int bn = band_start(band + 1) - start;
   const size_t off = (size_t)b.coef_off + start;
   if (kIntra) intra_band_ref(S, blk, band, b.coef_off, lane);
-  int qidx = bs * (bs + 1) + (band + 1) - (band + 1) / 3;
-  int q;
-  if (kFq) {
-    q = S.fq_bq[(b.frame * 3 + pli) * 32 + qidx];
-  } else {
-    q = (prm.q0 * prm.pvq_qm_q4[pli][qidx]) >> 4;
-    if (q < 1) q = 1;
-  }
+  const int qidx = bs * (bs + 1) + (band + 1) - (band + 1) / 3;
+  const int q = S.fq_bq[(b.frame * 3 + pli) * 32 + qidx];
   const int beta = (prm.use_masking && pli == 0 && bs > 0) ? kBeta15 : kBeta1;
   const int qoff = (b.xdec & 1 ? prm.qm_stride : 0) + ((((1 << (2 * bs)) - 1) << 4) / 3) + start;
   int itheta, max_theta, k;
@@ -872,13 +860,8 @@ struct ItemGeom {
   int blk, band, bn, q, beta, pli, qoff;
   size_t off;
 };
-// q0 * pvq_qm_q4[pli][qidx] >> 4 with the engine-wide quantizer, or with the record of the block's frame (fq: config.frame_quant)
-__device__ __forceinline__ int band_q(const daala_b200_pvq_params& prm, const daala_b200_kf_frame_quant* fq, int frame,
-                                      int pli, int qidx) {
-  return fq ? (fq[frame].q0 * fq[frame].pvq_qm_q4[pli][qidx]) >> 4 : (prm.q0 * prm.pvq_qm_q4[pli][qidx]) >> 4;
-}
-__device__ __forceinline__ ItemGeom item_geom(const daala_b200_pvq_params& prm, uint32_t item,
-                                              const daala_b200_kf_frame_quant* fq) {
+__device__ __forceinline__ ItemGeom item_geom(const Stage& S, uint32_t item) {
+  const daala_b200_pvq_params& prm = S.prm;
   ItemGeom g;
   g.blk = (int)(item >> 4);
   g.band = (int)(item & 15);
@@ -889,17 +872,15 @@ __device__ __forceinline__ ItemGeom item_geom(const daala_b200_pvq_params& prm, 
   g.bn = band_start(g.band + 1) - start;
   g.off = (size_t)b.coef_off + start;
   const int qidx = bs * (bs + 1) + (g.band + 1) - (g.band + 1) / 3;
-  int q = band_q(prm, fq, b.frame, g.pli, qidx);
-  g.q = q < 1 ? 1 : q;
+  g.q = S.fq_bq[(b.frame * 3 + g.pli) * 32 + qidx];
   g.beta = (prm.use_masking && g.pli == 0 && bs > 0) ? kBeta15 : kBeta1;
   g.qoff = (b.xdec & 1 ? prm.qm_stride : 0) + ((((1 << (2 * bs)) - 1) << 4) / 3) + start;
   return g;
 }
 
 // kPhase 0 / 1 / 2 = setup / search / finish of the items [chunk * slots, ...) of class `cls`.
-// kZeroRef: the prediction is all zero (luma bands 3 / 6).  kFq: the band quantisers come from the records of
-// config.frame_quant / keyframe_quant (S.fq); an instantiation of its own, so that the other engines run exactly the kernels they did.
-template <int kPhase, bool kZeroRef, int kMode, bool kFq = false>
+// kZeroRef: the prediction is all zero (luma bands 3 / 6).
+template <int kPhase, bool kZeroRef, int kMode>
 __global__ void __launch_bounds__(128) k_pvq_split(const __grid_constant__ Stage S, int cls, int chunk) {
   const daala_b200_pvq_params& prm = S.prm;
   const int lane = threadIdx.x & 31;
@@ -909,7 +890,7 @@ __global__ void __launch_bounds__(128) k_pvq_split(const __grid_constant__ Stage
   const int vs = cls == 2 ? 128 : 32;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < count; i += nwarps) {
-    const ItemGeom g = item_geom(prm, S.items[cls][first + i], kFq ? S.fq : nullptr);
+    const ItemGeom g = item_geom(S, S.items[cls][first + i]);
     int16_t* vec = S.sp_vec[cls] + (size_t)i * 3 * vs;
     int32_t* lanes = S.sp_lanes[cls] + (size_t)i * kCtxLaneWords * 16;
     int32_t* uni = S.sp_uni[cls] + (size_t)i * kCtxUniWords;
@@ -960,7 +941,7 @@ __global__ void __launch_bounds__(128) k_pvq_prepass(const __grid_constant__ Sta
     const int blk = (int)(i / per), sel = (int)(i % per);
     const int band = kMode == 2 ? 7 + sel : (sel < 3 ? sel : sel + 1);
     if (band >= num_bands(prm.blocks[blk].bs)) continue;
-    const ItemGeom g = item_geom(prm, ((uint32_t)blk << 4) | band, nullptr);
+    const ItemGeom g = item_geom(S, ((uint32_t)blk << 4) | band);
     BandCtx B;
     band_setup<kMode>(lane, B, prm.in + g.off, nullptr, g.bn, g.q, g.beta, prm.is_keyframe, g.pli, prm.qm + g.qoff,
                       prm.pvq_norm_lambda, S.rsqrt_tbl);
@@ -1004,7 +985,7 @@ __global__ void __launch_bounds__(128, 4) k_pvq_levels(const __grid_constant__ S
     for (int phase = 0; phase < 3; phase++) {
       for (int i = w; i < n; i += nwarps) {
         const uint32_t item = S.lvl_items[base + i];
-        const ItemGeom g = item_geom(prm, item, nullptr);
+        const ItemGeom g = item_geom(S, item);
         int16_t* vec = S.lv_vec + (size_t)i * 3 * vs;
         int32_t* lanes = S.lv_lanes + (size_t)i * kCtxLaneWords * 16;
         int32_t* uni = S.lv_uni + (size_t)i * kCtxUniWords;
@@ -1044,11 +1025,13 @@ __global__ void __launch_bounds__(128, 4) k_pvq_levels(const __grid_constant__ S
 // intra predictor form a dependency graph (per size class: band 0 a 2-D wavefront, bands 1/4/7 columns,
 // bands 2/5/8 rows).  A warp that finishes a chain item CONTINUES with a successor it made ready -- a
 // column or row is walked by one warp without touching the queue -- and pushes a second ready
-// successor (band 0 forks) into the chain queue.  The body of k_pvq_persist and k_pvq_persist_fq; `snap` is the
-// warp's shared scratch.
-template <bool kIntra, bool kFq>
-__device__ __forceinline__ void persist_items(const Stage& S, int16_t* snap) {
+// successor (band 0 forks) into the chain queue.
+template <bool kIntra>
+__global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(const __grid_constant__ Stage S) {
+  // per warp: the pulses of every search event of a band and the band's parked context (quantise_band_warp)
+  __shared__ __align__(16) int16_t snap_all[kPersistThreads / 32][kSnapEntries];
   const int lane = threadIdx.x & 31;
+  int16_t* snap = snap_all[threadIdx.x >> 5];
   int done = 0;
   bool waiter = false;
   for (;;) {
@@ -1062,7 +1045,7 @@ __device__ __forceinline__ void persist_items(const Stage& S, int16_t* snap) {
 #ifdef DAALA_B200_CHAIN_TRACE
       const unsigned long long t0 = globaltimer();
 #endif
-      run_item<kIntra, kFq>(S, item, lane, snap);
+      run_item<kIntra>(S, item, lane, snap);
 #ifdef DAALA_B200_CHAIN_TRACE
       if (kIntra) trace_item(S, item, kind, t0, lane);
       kind = 3;
@@ -1100,21 +1083,6 @@ __device__ __forceinline__ void persist_items(const Stage& S, int16_t* snap) {
       item = next;
     }
   }
-}
-
-template <bool kIntra>
-__global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(const __grid_constant__ Stage S) {
-  // per warp: the pulses of every search event of a band and the band's parked context (quantise_band_warp)
-  __shared__ __align__(16) int16_t snap_all[kPersistThreads / 32][kSnapEntries];
-  persist_items<kIntra, false>(S, snap_all[threadIdx.x >> 5]);
-}
-
-// config.keyframe_quant: the same walk with each band's quantiser from its frame's record (S.fq_bq).  A kernel of its
-// own, so that the other engines run exactly the kernel they did.
-template <bool kIntra>
-__global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist_fq(const __grid_constant__ Stage S) {
-  __shared__ __align__(16) int16_t snap_all[kPersistThreads / 32][kSnapEntries];
-  persist_items<kIntra, true>(S, snap_all[threadIdx.x >> 5]);
 }
 
 __global__ void k_fill_rsqrt(double* tbl) {
@@ -1174,8 +1142,7 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
       } else if (!kInter) {
         prm.out[b.coef_off] = prm.in[b.coef_off];
       } else {
-        int dc_quant = band_q(prm, S.fq, b.frame, b.pli, b.bs * (b.bs + 1));
-        if (dc_quant < 1) dc_quant = 1;
+        const int dc_quant = S.fq_bq[(b.frame * 3 + b.pli) * 32 + b.bs * (b.bs + 1)];
         const int32_t r = prm.ref[b.coef_off], diff = prm.in[b.coef_off] - r;
         int qdc = 0;
         if (abs(diff) >= dc_quant * 141 / 256) {
@@ -1210,29 +1177,20 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
 // (the deringing kernel stores the u8 reconstruction itself).
 // thr[pl][f][sb] = table[pl][level[f][sb]].  P-frame finishing pass: `coded` (else NULL) flags the superblocks with a
 // coded 4x4 luma unit; the others are forced to level 0 (src/encode.c:2724-2738), and the level applied goes to
-// `applied`.  config.frame_quant / keyframe_quant: `frame_tbl` ([F][2][6], else NULL) holds each frame's table, the frame of superblock
-// i being i / nsb.
+// `applied`.  `frame_tbl` ([F][2][6]) holds each frame's table, the frame of superblock i being i / nsb.
 __global__ void k_dering_thresholds(const uint8_t* __restrict__ level, int32_t* __restrict__ thr_luma,
-                                    int32_t* __restrict__ thr_chroma, int n, int4 tl_lo, int2 tl_hi, int4 tc_lo, int2 tc_hi,
-                                    const uint8_t* __restrict__ coded, uint8_t* __restrict__ applied,
-                                    const int32_t* __restrict__ frame_tbl, int nsb) {
+                                    int32_t* __restrict__ thr_chroma, int n, const uint8_t* __restrict__ coded,
+                                    uint8_t* __restrict__ applied, const int32_t* __restrict__ frame_tbl, int nsb) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const int tl[6] = {tl_lo.x, tl_lo.y, tl_lo.z, tl_lo.w, tl_hi.x, tl_hi.y};
-  const int tc[6] = {tc_lo.x, tc_lo.y, tc_lo.z, tc_lo.w, tc_hi.x, tc_hi.y};
   int g = level[i] < 6 ? level[i] : 5;
   if (coded) {
     if (!coded[i]) g = 0;
     applied[i] = (uint8_t)g;
   }
-  if (frame_tbl) {
-    const int32_t* t = frame_tbl + (size_t)(i / nsb) * 12;
-    thr_luma[i] = t[g];
-    thr_chroma[i] = t[6 + g];
-  } else {
-    thr_luma[i] = tl[g];
-    thr_chroma[i] = tc[g];
-  }
+  const int32_t* t = frame_tbl + (size_t)(i / nsb) * 12;
+  thr_luma[i] = t[g];
+  thr_chroma[i] = t[6 + g];
 }
 
 // ---- P-frame finishing pass (config.inter_finish) ----------------------------------------------------------------
@@ -1254,9 +1212,7 @@ struct Fin {
   int skip_stride;                         // state->skip_stride = nhsb * 16
   uint8_t* coded;                          // [F][nvsb][nhsb]: a luma 4x4 unit of the superblock is coded (preset 0)
   int nhsb, nvsb;
-  int q0;
-  uint8_t pvq_qm_q4[3][32];
-  const daala_b200_kf_frame_quant* fq;     // config.frame_quant: the step's records, which replace q0 / pvq_qm_q4
+  const int32_t* fq_bq;                    // [F][3][32] each frame's band quantisers (Stage::fq_bq)
 };
 
 // block i of the two lists together (luma first), or false past their end
@@ -1283,9 +1239,7 @@ __global__ void __launch_bounds__(256) k_fin_patch(const __grid_constant__ Fin P
     const int32_t* src = (P.skip[list][blk] ? P.md[b.pli] : P.d[b.pli]) + o;
     const int32_t* mdp = P.md[b.pli] + o;
     int32_t* dst = P.out[b.pli] + o;
-    const int qidx = b.bs * (b.bs + 1);
-    int dc_quant = P.fq ? (P.fq[b.frame].q0 * P.fq[b.frame].pvq_qm_q4[b.pli][qidx]) >> 4 : (P.q0 * P.pvq_qm_q4[b.pli][qidx]) >> 4;
-    if (dc_quant < 1) dc_quant = 1;
+    const int dc_quant = P.fq_bq[(b.frame * 3 + b.pli) * 32 + b.bs * (b.bs + 1)];
     const int32_t dc0 = mdp[0] + P.dc[list][blk] * dc_quant;
     for (int k = lane; k < nn * nn; k += 32) {
       const size_t at = (size_t)(k >> ln) * stride + (k & (nn - 1));
@@ -1708,8 +1662,7 @@ struct Dering {
   uint8_t* level;                  // [F][nvsb][nhsb]: what the thresholds read and the search writes
   const uint8_t* coded;            // nullable: superblocks with a coded luma 4x4 unit; the others get level 0 ...
   uint8_t* applied;                // ... and the level applied lands here
-  int tbl[2][6];                   // luma / chroma threshold per level
-  const int32_t* frame_tbl;        // frame_quant / keyframe_quant: [F][2][6] tbl of each frame (replaces tbl), else NULL
+  const int32_t* frame_tbl;        // [F][2][6] luma / chroma threshold per level of each frame
   int32_t* thr[2];                 // luma / chroma threshold per superblock
   int32_t* dir;                    // [F][nvsb*8][nhsb*8]
   bool search;                     // the level search runs first, described by `sb`
@@ -1781,13 +1734,13 @@ struct daala_b200_kf {
   cudaGraphExec_t fin_exec;
   bool fin_captured;
   int fin_dc_limit;                // largest |dc| finish accepts: DAALA_B200_KF_FINISH_DC_LIMIT / the largest dc_quant
-                                   // (config.frame_quant: of the last step's records, set by submit)
-  // frame_quant / keyframe_quant: the step's records and the deringing threshold table of each frame ([F][2][6], computed on the
-  // host from the records' q0 as daala_b200_dering_threshold_table does), uploaded by submit
+                                   // of the last step's records
+  // Lossy engines: each frame's record, its deringing threshold table ([F][2][6], daala_b200_dering_threshold_table of
+  // its q0) and its band quantisers ([F][3][32], Stage::fq_bq).  The tables are computed on the host by fq_derive_host:
+  // once at create from the config, or per step with frame_quant / keyframe_quant.
   daala_b200_kf_frame_quant* fq;
   int32_t* fq_tbl;
   std::vector<int32_t> fq_tbl_host;
-  // config.keyframe_quant: each frame's band quantisers ([F][3][32], Stage::fq_bq), computed on the host by submit
   int32_t* fq_bq;
   std::vector<int32_t> fq_bq_host;
   // cfg.inter_mc with cfg.inter_finish: the pool slot of each frame's reconstruction (finish_io.ref_slot_out, -1 = not
@@ -1926,6 +1879,39 @@ static int ll_alloc(daala_b200_kf* kf) {
   return 0;
 }
 
+// The records of a step ([F]): why they are refused, or nullptr when every one is in range; then the host tables hold
+// each frame's deringing thresholds (daala_b200_kf_frame_quant_derive) and band quantisers, and *dc_limit is the
+// finishing pass's DC limit.  check = false: records made from the config, whose fields a mode that does not read them
+// may leave out of range (coded_quantizer = 0 without dering = 2); create has checked q0.
+static const char* fq_derive_host(daala_b200_kf* kf, const daala_b200_kf_frame_quant* rec, bool check, int* dc_limit) {
+  if (!rec) return "frame_quant: the records ([nframes]) are required";
+  const int F = kf->F;
+  for (int f = 0; check && f < F; f++) {
+    const daala_b200_kf_frame_quant& r = rec[f];
+    if (r.q0 < 1 || r.q0 > DAALA_B200_KF_MAX_Q0) return "a record's q0 is outside [1, 8191]";
+    if (r.coded_quantizer < 1 || r.coded_quantizer > 63) return "a record's coded_quantizer is outside [1, 63]";
+    if (!std::isfinite(r.dering_lambda) || r.dering_lambda < 0) return "a record's dering_lambda is negative or not finite";
+    for (int p = 0; p < 3; p++)
+      for (int i = 0; i < 30; i++)   // OD_QM_SIZE entries are read
+        if (r.pvq_qm_q4[p][i] < 1) return "a record's pvq_qm_q4 entry is 0";
+  }
+  *dc_limit = daala_b200_kf_frame_quant_derive(rec, F, reinterpret_cast<int32_t(*)[2][6]>(kf->fq_tbl_host.data()));
+  for (int f = 0; f < F; f++)
+    for (int p = 0; p < 3; p++)
+      for (int i = 0; i < 30; i++)
+        kf->fq_bq_host[(size_t)(f * 3 + p) * 32 + i] = std::max(1, (rec[f].q0 * rec[f].pvq_qm_q4[p][i]) >> 4);
+  return nullptr;
+}
+
+// The H2D of the records fq_derive_host accepted and of its tables, on `s`.
+static cudaError_t fq_copy(daala_b200_kf* kf, const daala_b200_kf_frame_quant* rec, cudaStream_t s) {
+  const int F = kf->F;
+  cudaError_t e = cudaMemcpyAsync(kf->fq, rec, sizeof(daala_b200_kf_frame_quant) * F, cudaMemcpyHostToDevice, s);
+  if (!e) e = cudaMemcpyAsync(kf->fq_tbl, kf->fq_tbl_host.data(), sizeof(int32_t) * 12 * F, cudaMemcpyHostToDevice, s);
+  if (!e) e = cudaMemcpyAsync(kf->fq_bq, kf->fq_bq_host.data(), sizeof(int32_t) * 96 * F, cudaMemcpyHostToDevice, s);
+  return e;
+}
+
 static int kf_alloc(daala_b200_kf* kf) {
   if (kf->cfg.lossless) return ll_alloc(kf);
   const int F = kf->F;
@@ -1948,15 +1934,11 @@ static int kf_alloc(daala_b200_kf* kf) {
     const int rc = mc_alloc(kf);
     if (rc) return rc;
   }
-  if (kf->cfg.frame_quant || kf->cfg.keyframe_quant) {
-    KF_CHECK(dalloc(kf, &kf->fq, (size_t)F));
-    KF_CHECK(dalloc(kf, &kf->fq_tbl, (size_t)F * 12));
-    kf->fq_tbl_host.assign((size_t)F * 12, 0);
-  }
-  if (kf->cfg.keyframe_quant) {
-    KF_CHECK(dalloc(kf, &kf->fq_bq, (size_t)F * 96));
-    kf->fq_bq_host.assign((size_t)F * 96, 1);
-  }
+  KF_CHECK(dalloc(kf, &kf->fq, (size_t)F));
+  KF_CHECK(dalloc(kf, &kf->fq_tbl, (size_t)F * 12));
+  KF_CHECK(dalloc(kf, &kf->fq_bq, (size_t)F * 96));
+  kf->fq_tbl_host.assign((size_t)F * 12, 0);
+  kf->fq_bq_host.assign((size_t)F * 96, 1);
   KF_CHECK(dalloc(kf, &kf->qm, (size_t)2 * kf->cfg.qm_stride));
   KF_CHECK(dalloc(kf, &kf->qm_inv, (size_t)2 * kf->cfg.qm_stride));
   KF_CHECK(dalloc(kf, &kf->rsqrt_tbl, (size_t)kTableDoubles));
@@ -2049,19 +2031,6 @@ static int kf_alloc(daala_b200_kf* kf) {
                per_sm[1], want);
       return (int)cudaErrorLaunchOutOfResources;
     }
-    if (kf->cfg.keyframe_quant) {
-      KF_CHECK(cudaFuncSetAttribute(k_pvq_persist_fq<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                    cudaSharedmemCarveoutMaxShared));
-      KF_CHECK(cudaFuncSetAttribute(k_pvq_persist_fq<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                    cudaSharedmemCarveoutMaxShared));
-      KF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[0], k_pvq_persist_fq<true>, kPersistThreads, 0));
-      KF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[1], k_pvq_persist_fq<false>, kPersistThreads, 0));
-      if (per_sm[0] < want || per_sm[1] < want) {
-        snprintf(kf->err, sizeof(kf->err), "k_pvq_persist_fq: %d / %d CTAs per SM resident, %d wanted", per_sm[0],
-                 per_sm[1], want);
-        return (int)cudaErrorLaunchOutOfResources;
-      }
-    }
   }
   KF_CHECK(dalloc(kf, &L.heads, inter ? 0 : kf->chain_cap));
   KF_CHECK(dalloc(kf, &L.heads_raw, inter ? 0 : kf->chain_cap));
@@ -2100,13 +2069,10 @@ static int kf_alloc(daala_b200_kf* kf) {
       p.plane_stride[i] = kf->plane_w[i];
     }
     p.qm_stride = kf->cfg.qm_stride;
-    p.q0 = kf->cfg.q0 > 1 ? kf->cfg.q0 : 1;
     p.is_keyframe = inter ? 0 : 1;
     p.use_masking = kf->cfg.use_masking;
     p.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
-    memcpy(p.pvq_qm_q4, kf->cfg.pvq_qm_q4, sizeof(p.pvq_qm_q4));
-    S.fq = kf->fq;
-    if (kf->cfg.keyframe_quant) S.fq_bq = kf->fq_bq;
+    S.fq_bq = kf->fq_bq;
     for (int c = 0; c < 3; c++) S.items[c] = chroma ? L.items_c[c] : L.items_l[c];
     S.cnt = L.cnt;
     S.rsqrt_tbl = kf->rsqrt_tbl;
@@ -2182,15 +2148,13 @@ static int kf_alloc(daala_b200_kf* kf) {
       H.index[p] = kf->hdc_index[p];
       H.plane_w[p] = kf->plane_w[p];
       H.plane_h[p] = kf->plane_h[p];
-      // od_quantize_haar_dc_sb / _level: max(1, quantizer * pvq_qm_q4[pli][od_qm_get_index(OD_NBSIZES - 1, 0)] >> 4)
-      H.dc_quant[p] = std::max(1, kf->cfg.q0 * kf->cfg.pvq_qm_q4[p][20] >> 4);
     }
     H.bsize = kf->bsize;
     H.F = F;
     H.nhsb = kf->nhsb;
     H.nvsb = kf->nvsb;
     H.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
-    H.fq_bq = kf->fq_bq;   // keyframe_quant: each frame's dc_quant is its entry [f][pli][20], dc_quant[] is not read
+    H.fq_bq = kf->fq_bq;
   }
   (void)luma_px;
   // the unquantised DC residual per block: what the host's od_rdo_quant needs, returned classically (inter_finish) or
@@ -2272,12 +2236,10 @@ static int kf_alloc(daala_b200_kf* kf) {
     }
     KF_CHECK(dalloc(kf, &B.cls_items, (size_t)daala_b200_late_skip_class_caps(px, B.cls_off, B.cls_cap)));
     KF_CHECK(dalloc(kf, &B.cls_n, (size_t)4));
-    B.q0 = kf->luma.prm.q0;
-    memcpy(B.pvq_qm_q4, kf->cfg.pvq_qm_q4, sizeof(B.pvq_qm_q4));
     B.qm_is_flat = kf->cfg.qm_is_flat;
     B.use_activity_masking = kf->cfg.use_masking;
-    B.coded_quantizer = kf->cfg.coded_quantizer;
     B.fq = kf->fq;
+    B.fq_bq = kf->fq_bq;
     if (kf->cfg.symbol_stream == 2) {
       Sym& Y = kf->sym;
       KF_CHECK(dalloc(kf, &Y.late_skip, (size_t)Y.cap_blocks));
@@ -2352,16 +2314,7 @@ static int kf_alloc(daala_b200_kf* kf) {
     P.coded = kf->fin_coded;
     P.nhsb = kf->nhsb;
     P.nvsb = kf->nvsb;
-    P.q0 = kf->luma.prm.q0;
-    memcpy(P.pvq_qm_q4, kf->cfg.pvq_qm_q4, sizeof(P.pvq_qm_q4));
-    int dq_max = 1;
-    for (int p = 0; p < 3; p++)
-      for (int bs = 0; bs < 5; bs++) {
-        const int dq = (P.q0 * P.pvq_qm_q4[p][bs * (bs + 1)]) >> 4;
-        if (dq > dq_max) dq_max = dq;
-      }
-    kf->fin_dc_limit = DAALA_B200_KF_FINISH_DC_LIMIT / dq_max;   // config.frame_quant: replaced by each submit
-    P.fq = kf->fq;
+    P.fq_bq = kf->fq_bq;
     if (kf->cfg.inter_mc) {
       KF_CHECK(dalloc(kf, &kf->fin_slot_out, (size_t)F));
       PoolStore& W = kf->store;
@@ -2416,7 +2369,6 @@ static int kf_alloc(daala_b200_kf* kf) {
     KF_CHECK(dalloc(kf, &D.dir, nsb * 64));
     D.coded = kf->fin_coded;
     D.applied = kf->fin_level;
-    daala_b200_dering_threshold_table(kf->cfg.q0, D.tbl);
     D.frame_tbl = kf->fq_tbl;
     D.search = dering == 2;
     if (D.search) {
@@ -2430,11 +2382,8 @@ static int kf_alloc(daala_b200_kf* kf) {
       b.nframes = F;
       b.nhsb = kf->nhsb;
       b.nvsb = kf->nvsb;
-      memcpy(b.threshold, D.tbl[0], sizeof(b.threshold));
-      b.coded_quantizer = kf->cfg.coded_quantizer;
       b.qm_is_flat = kf->cfg.qm_is_flat;
       b.use_activity_masking = kf->cfg.use_masking;
-      b.dering_lambda = kf->cfg.dering_lambda;
       b.bskip = D.skip[0];
       b.skip_stride = D.skip_stride;
       b.skip_pitch = D.skip_pitch[0];
@@ -2446,11 +2395,9 @@ static int kf_alloc(daala_b200_kf* kf) {
       KF_CHECK(dalloc(kf, &b.dist, nsb * 6));
       b.dir = D.dir;
       b.levels = D.level;   // what the thresholds read; on P frames its level 0 agrees with the forced one
-      if (kf->cfg.frame_quant || kf->cfg.keyframe_quant) {
-        b.fq = kf->fq;
-        b.frame_tbl = kf->fq_tbl;
-        KF_CHECK(dalloc(kf, &b.cand_thr, nsb * 5));
-      }
+      b.fq = kf->fq;
+      b.frame_tbl = kf->fq_tbl;
+      KF_CHECK(dalloc(kf, &b.cand_thr, nsb * 5));
     }
   }
   // dalloc's cudaMemset runs on the legacy default stream, asynchronously, and the engine's stream does not
@@ -2459,6 +2406,16 @@ static int kf_alloc(daala_b200_kf* kf) {
   KF_CHECK(cudaDeviceSynchronize());
   k_fill_rsqrt<<<(kTableDoubles + 255) / 256, 256, 0, kf->stream>>>(kf->rsqrt_tbl);
   KF_CHECK(cudaGetLastError());
+  // every frame at the config's quantizer; frame_quant / keyframe_quant replace the records with each step's
+  std::vector<daala_b200_kf_frame_quant> rec((size_t)F);
+  for (daala_b200_kf_frame_quant& r : rec) {
+    r.q0 = kf->cfg.q0;
+    r.coded_quantizer = kf->cfg.coded_quantizer;
+    r.dering_lambda = kf->cfg.dering_lambda;
+    memcpy(r.pvq_qm_q4, kf->cfg.pvq_qm_q4, sizeof(r.pvq_qm_q4));
+  }
+  fq_derive_host(kf, rec.data(), false, &kf->fin_dc_limit);
+  KF_CHECK(fq_copy(kf, rec.data(), kf->stream));
   KF_CHECK(cudaStreamSynchronize(kf->stream));
   return 0;
 }
@@ -2505,10 +2462,8 @@ static int enqueue_dering_luma(daala_b200_kf* kf, const Dering& D, cudaStream_t 
     if (rc) return rc;
   }
   const int nsb = kf->nhsb * kf->nvsb;
-  k_dering_thresholds<<<(kf->F * nsb + 255) / 256, 256, 0, s>>>(
-      D.level, D.thr[0], D.thr[1], kf->F * nsb, make_int4(D.tbl[0][0], D.tbl[0][1], D.tbl[0][2], D.tbl[0][3]),
-      make_int2(D.tbl[0][4], D.tbl[0][5]), make_int4(D.tbl[1][0], D.tbl[1][1], D.tbl[1][2], D.tbl[1][3]),
-      make_int2(D.tbl[1][4], D.tbl[1][5]), D.coded, D.applied, D.frame_tbl, nsb);
+  k_dering_thresholds<<<(kf->F * nsb + 255) / 256, 256, 0, s>>>(D.level, D.thr[0], D.thr[1], kf->F * nsb, D.coded,
+                                                                   D.applied, D.frame_tbl, nsb);
   return enqueue_dering_plane(kf, D, 0, s);
 }
 
@@ -2522,27 +2477,27 @@ static int enqueue_dering(daala_b200_kf* kf, const Dering& D, cudaStream_t s) {
 }
 
 // Kernel launches of enqueue_dering with the inverse in `parts` plane ranges: inverse, SB postfilter -> int16 per
-// range, [level search: 5 filtered candidates, 6 packs, 6 distortion passes, decision], thresholds, dering + u8
-// store per plane; per-frame quantizers add the candidates' thresholds to the search.
+// range, [level search: the candidates' thresholds, 5 filtered candidates, 6 packs, 6 distortion passes, decision],
+// thresholds, dering + u8 store per plane.
 static int dering_launches(const Dering& D, int parts) {
-  return 2 * parts + (D.search ? 5 + 6 + 6 + 1 + (D.sb.frame_tbl ? 1 : 0) : 0) + 1 + 3;
+  return 2 * parts + (D.search ? 1 + 5 + 6 + 6 + 1 : 0) + 1 + 3;
 }
 
 // Everything between "inputs are in HBM" and "results are in HBM", on kf->stream.
 // the three phase kernels over every chunk of every class of a stage's dependency-free lists
-template <bool kZeroRef, bool kFq = false>
+template <bool kZeroRef>
 static void enqueue_split(daala_b200_kf* kf, const Stage& S, cudaStream_t s) {
   const int grid = kf->sms * 16;
   for (int cls = 2; cls >= 0; cls--) {
     for (int chunk = 0; chunk < S.sp_chunks[cls]; chunk++) {
       if (cls == 2) {
-        k_pvq_split<0, kZeroRef, 2, kFq><<<grid, 128, 0, s>>>(S, cls, chunk);
-        k_pvq_split<1, kZeroRef, 2><<<grid, 128, 0, s>>>(S, cls, chunk);   // the search reads no quantiser
-        k_pvq_split<2, kZeroRef, 2, kFq><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<0, kZeroRef, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<1, kZeroRef, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<2, kZeroRef, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
       } else {
-        k_pvq_split<0, kZeroRef, 1, kFq><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<0, kZeroRef, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
         k_pvq_split<1, kZeroRef, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
-        k_pvq_split<2, kZeroRef, 1, kFq><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<2, kZeroRef, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
       }
     }
   }
@@ -2597,8 +2552,7 @@ static int kf_enqueue_step_inter(daala_b200_kf* kf, int phases) {
   for (const Stage* S : {&kf->luma, &kf->chroma}) {
     if (!(phases & (S == &kf->luma ? DAALA_B200_KF_PVQ_LUMA : DAALA_B200_KF_PVQ_CHROMA))) continue;
     if (!core) k_gather<kGatherInter><<<wide, 256, 0, s>>>(*S);
-    if (S->fq) enqueue_split<false, true>(kf, *S, s);
-    else enqueue_split<false>(kf, *S, s);
+    enqueue_split<false>(kf, *S, s);
     if (!core) k_finish_scatter<true><<<wide, 256, 0, s>>>(*S);
   }
   if (!core && (phases & DAALA_B200_KF_PVQ_CHROMA) && kf->cfg.late_skip) {
@@ -2645,9 +2599,7 @@ static int enqueue_luma_bands(daala_b200_kf* kf, bool core, int begin, cudaStrea
     return (int)cudaGetLastError();
   k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, begin);
   if (!core) k_gather<kGatherLuma><<<wide, 256, 0, s>>>(kf->luma);
-  const bool kfq = kf->cfg.keyframe_quant != 0;
-  if (kf->cfg.split_free > 1 && kfq) enqueue_split<true, true>(kf, kf->luma, s);
-  else if (kf->cfg.split_free > 1) enqueue_split<true>(kf, kf->luma, s);
+  if (kf->cfg.split_free > 1) enqueue_split<true>(kf, kf->luma, s);
   if (kf->luma.pre_ev) {
     k_pvq_prepass<2><<<kf->sms * 16, 128, 0, s>>>(kf->luma);
     k_pvq_prepass<1><<<kf->sms * 16, 128, 0, s>>>(kf->luma);
@@ -2655,8 +2607,6 @@ static int enqueue_luma_bands(daala_b200_kf* kf, bool core, int begin, cudaStrea
   if (kf->cfg.level_chains) {
     if (cudaMemsetAsync(kf->lv_bar, 0, sizeof(int32_t) * 32, s) != cudaSuccess) return (int)cudaGetLastError();
     k_pvq_levels<<<kf->lvl_grid, 128, 0, s>>>(kf->luma);
-  } else if (kfq) {
-    k_pvq_persist_fq<true><<<persist, kPersistThreads, 0, s>>>(kf->luma);
   } else {
     k_pvq_persist<true><<<persist, kPersistThreads, 0, s>>>(kf->luma);
   }
@@ -2671,11 +2621,8 @@ static void enqueue_chroma(daala_b200_kf* kf, bool core, bool begin, cudaStream_
   if (begin) k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, kBeginChroma);
   if (!core && hdc) k_gather<kGatherChroma, true><<<wide, 256, 0, s>>>(kf->chroma);
   else if (!core) k_gather<kGatherChroma><<<wide, 256, 0, s>>>(kf->chroma);
-  const bool kfq = kf->cfg.keyframe_quant != 0;
   const int persist = kf->sms * (kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas);
-  if (kf->cfg.split_free > 0 && kfq) enqueue_split<false, true>(kf, kf->chroma, s);
-  else if (kf->cfg.split_free > 0) enqueue_split<false>(kf, kf->chroma, s);
-  else if (kfq) k_pvq_persist_fq<false><<<persist, kPersistThreads, 0, s>>>(kf->chroma);
+  if (kf->cfg.split_free > 0) enqueue_split<false>(kf, kf->chroma, s);
   else k_pvq_persist<false><<<persist, kPersistThreads, 0, s>>>(kf->chroma);
   if (!core && hdc) k_finish_scatter<false, true><<<wide, 256, 0, s>>>(kf->chroma);
   else if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->chroma);
@@ -2882,6 +2829,12 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
       return nullptr;
     }
   }
+  if (cfg && !cfg->lossless && (cfg->q0 < 1 || cfg->q0 > DAALA_B200_KF_MAX_Q0)) {
+    // the records made from the config follow the records' rule (quantizer 0 is the lossless engine's)
+    snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: q0 is outside [1, %d] (lossless = 1 codes quantizer 0)",
+             DAALA_B200_KF_MAX_Q0);
+    return nullptr;
+  }
   if (cfg && cfg->mc_refs < 0) {
     snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: mc_refs < 0");
     return nullptr;
@@ -3064,7 +3017,7 @@ int daala_b200_kf_device_buffers(daala_b200_kf* kf, daala_b200_kf_buffers* out) 
   out->mc_refs = kf->cfg.mc_refs;
   out->ref_slot_next = kf->ref_slot_next;
   out->mv1_grid = kf->mv1_grid;
-  out->frame_quant = kf->fq;
+  out->frame_quant = kf->cfg.frame_quant || kf->cfg.keyframe_quant ? kf->fq : nullptr;
   for (int p = 0; p < 3; p++) {
     out->haar_dc[p] = kf->hdcb.dc[p];
     out->dc_index[p] = kf->hdc_index[p];
@@ -3182,46 +3135,12 @@ static int sym_target(const void* p, long long cap, long long need, uint8_t** de
 static std::mutex g_compute_mu;
 static cudaEvent_t g_last_compute = nullptr;
 
-// The records of a frame_quant / keyframe_quant step: why they are refused, or nullptr when every one is in range; then
-// the host tables hold each frame's deringing thresholds (daala_b200_kf_frame_quant_derive) and, with keyframe_quant,
-// its band quantisers, and *dc_limit is the finishing pass's DC limit.
-static const char* fq_derive_host(daala_b200_kf* kf, const daala_b200_kf_frame_quant* rec, int* dc_limit) {
-  if (!rec) return "frame_quant: the records ([nframes]) are required";
-  const int F = kf->F;
-  for (int f = 0; f < F; f++) {
-    const daala_b200_kf_frame_quant& r = rec[f];
-    if (r.q0 < 1 || r.q0 > DAALA_B200_KF_MAX_Q0) return "a record's q0 is outside [1, 8191]";
-    if (r.coded_quantizer < 1 || r.coded_quantizer > 63) return "a record's coded_quantizer is outside [1, 63]";
-    if (!std::isfinite(r.dering_lambda) || r.dering_lambda < 0) return "a record's dering_lambda is negative or not finite";
-    for (int p = 0; p < 3; p++)
-      for (int i = 0; i < 30; i++)   // OD_QM_SIZE entries are read
-        if (r.pvq_qm_q4[p][i] < 1) return "a record's pvq_qm_q4 entry is 0";
-  }
-  *dc_limit = daala_b200_kf_frame_quant_derive(rec, F, reinterpret_cast<int32_t(*)[2][6]>(kf->fq_tbl_host.data()));
-  if (kf->cfg.keyframe_quant)
-    for (int f = 0; f < F; f++)
-      for (int p = 0; p < 3; p++)
-        for (int i = 0; i < 30; i++)
-          kf->fq_bq_host[(size_t)(f * 3 + p) * 32 + i] = std::max(1, (rec[f].q0 * rec[f].pvq_qm_q4[p][i]) >> 4);
-  return nullptr;
-}
-
-// The H2D of the records fq_derive_host accepted and of its tables, on `s`.
-static cudaError_t fq_copy(daala_b200_kf* kf, const daala_b200_kf_frame_quant* rec, cudaStream_t s) {
-  const int F = kf->F;
-  cudaError_t e = cudaMemcpyAsync(kf->fq, rec, sizeof(daala_b200_kf_frame_quant) * F, cudaMemcpyHostToDevice, s);
-  if (!e) e = cudaMemcpyAsync(kf->fq_tbl, kf->fq_tbl_host.data(), sizeof(int32_t) * 12 * F, cudaMemcpyHostToDevice, s);
-  if (!e && kf->fq_bq)
-    e = cudaMemcpyAsync(kf->fq_bq, kf->fq_bq_host.data(), sizeof(int32_t) * 96 * F, cudaMemcpyHostToDevice, s);
-  return e;
-}
-
 int daala_b200_kf_load_frame_quant(daala_b200_kf* kf, const daala_b200_kf_frame_quant* rec) {
   if (!kf) return (int)cudaErrorInvalidValue;
   int dc_limit = 0;
   const char* why = !kf->cfg.frame_quant && !kf->cfg.keyframe_quant
                         ? "needs an engine with frame_quant = 1 or keyframe_quant = 1"
-                        : fq_derive_host(kf, rec, &dc_limit);
+                        : fq_derive_host(kf, rec, true, &dc_limit);
   if (why) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_load_frame_quant: %s", why);
     return (int)cudaErrorInvalidValue;
@@ -3330,13 +3249,13 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", ls_why);
     return (int)cudaErrorInvalidValue;
   }
-  // per-frame quantizers: every record in range; then each frame's deringing thresholds [and band quantisers] and the
+  // per-frame quantizers: every record in range; then each frame's deringing thresholds and band quantisers and the
   // finishing pass's DC limit of this step
   int fq_dc_limit = 0;
   const bool fq_mode = kf->cfg.frame_quant || kf->cfg.keyframe_quant;
   if (io->frame_quant || fq_mode) {
     const char* why = !fq_mode ? "frame_quant needs an engine with frame_quant = 1 or keyframe_quant = 1"
-                               : fq_derive_host(kf, io->frame_quant, &fq_dc_limit);
+                               : fq_derive_host(kf, io->frame_quant, true, &fq_dc_limit);
     if (why) {
       snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", why);
       return (int)cudaErrorInvalidValue;
@@ -3438,7 +3357,7 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   }
   kf->have_step = true;
   kf->last_tot = tot;
-  if (kf->cfg.frame_quant) kf->fin_dc_limit = fq_dc_limit;
+  if (fq_mode) kf->fin_dc_limit = fq_dc_limit;
   for (int p = 0; p < 3; p++)
     if (io->pixels_out[p])
       KF_CHECK(cudaMemcpyAsync(io->pixels_out[p], kf->pixels_out[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,

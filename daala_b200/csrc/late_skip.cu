@@ -94,7 +94,7 @@ __global__ void __launch_bounds__(kDistThreads) k_late_skip(const __grid_constan
   __shared__ const int32_t* s_md[G];
   __shared__ int s_stride[G];
   __shared__ int32_t s_dc[G][2];                                       // md[0], md[0] + q1 * dc_quant
-  __shared__ double s_scale[G];                                        // fq: the slot's frame's dist_scale
+  __shared__ double s_scale[G];                                        // the slot's frame's dist_scale
   const int c = LN - 3;
   const int n = min(P.cls_n[c], (int)P.cls_cap[c]);
   const uint32_t* items = P.cls_items + P.cls_off[c];
@@ -111,16 +111,13 @@ __global__ void __launch_bounds__(kDistThreads) k_late_skip(const __grid_constan
         s_d[t] = P.d[b.pli] + o;
         s_md[t] = P.md[b.pli] + o;
         s_stride[t] = stride;
-        const int qidx = b.bs * (b.bs + 1);
-        int dc_quant = P.fq ? (P.fq[b.frame].q0 * P.fq[b.frame].pvq_qm_q4[b.pli][qidx]) >> 4
-                            : (P.q0 * P.pvq_qm_q4[b.pli][qidx]) >> 4;
-        if (dc_quant < 1) dc_quant = 1;
+        const int dc_quant = P.fq_bq[(b.frame * 3 + b.pli) * 32 + b.bs * (b.bs + 1)];
         const int32_t md0 = s_md[t][0], resid = s_dor[t][0] - md0;
         const int half = ((dc_quant + 1) >> 1) - 1;
         const int32_t q1 = (resid + (resid < 0 ? -half : half)) / dc_quant;   // OD_DIV_R0 (src/odintrin.h:123)
         s_dc[t][0] = md0;
         s_dc[t][1] = md0 + q1 * dc_quant;
-        if (P.fq) s_scale[t] = dist::dist_scale(P.fq[b.frame].coded_quantizer);
+        s_scale[t] = dist::dist_scale(P.fq[b.frame].coded_quantizer);
       }
     }
     __syncthreads();
@@ -141,10 +138,10 @@ __global__ void __launch_bounds__(kDistThreads) k_late_skip(const __grid_constan
       __syncthreads();
       idct_tile<LN>(dst, G);
       if (cand >= 0) {
-        // fq: the HVS totals are scaled per slot at the end (the scale is block_dist's last multiplication; x * 1.0 is
+        // the HVS totals are scaled per slot at the end (the scale is block_dist's last multiplication; x * 1.0 is
         // exact)
-        const double d = dist::block_dist(A, N + 1, NP, B, N + 1, NP, LN, G, P.qm_is_flat, P.use_activity_masking,
-                                          P.fq ? 1.0 : dist::dist_scale(P.coded_quantizer), scratch);
+        const double d = dist::block_dist(A, N + 1, NP, B, N + 1, NP, LN, G, P.qm_is_flat, P.use_activity_masking, 1.0,
+                                          scratch);
         if (cand == 0) rec.dist_skip = d;
         else if (cand == 1) rec.noskip_coded_dc0 = d;
         else if (cand == 2) rec.noskip_coded_dcq = d;
@@ -152,7 +149,7 @@ __global__ void __launch_bounds__(kDistThreads) k_late_skip(const __grid_constan
       }
     }
     if (t < G && b0 + t < n) {
-      if (P.fq && !P.qm_is_flat) {
+      if (!P.qm_is_flat) {
         const double sc = s_scale[t];
         rec.dist_skip *= sc;
         rec.noskip_coded_dc0 *= sc;

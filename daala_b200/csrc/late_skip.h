@@ -16,10 +16,9 @@ struct daala_b200_late_skip_batch {
   const int32_t* md[3];                    // the transformed prediction
   long long plane_pitch[3];                // elements between frames
   int plane_stride[3];
-  int q0;
-  uint8_t pvq_qm_q4[3][32];
-  int qm_is_flat, use_activity_masking, coded_quantizer;   // od_compute_dist's parameters
-  const daala_b200_kf_frame_quant* fq;     // config.frame_quant: per frame q0 / pvq_qm_q4 / coded_quantizer, else NULL
+  int qm_is_flat, use_activity_masking;    // od_compute_dist's parameters, with each frame's coded_quantizer
+  const daala_b200_kf_frame_quant* fq;     // [F] each frame's record (its coded_quantizer)
+  const int32_t* fq_bq;                    // [F][3][32] each frame's band quantisers (the DC's: [bs * (bs + 1)])
   daala_b200_kf_late_skip* out[2];         // per block of each list
   // scratch: the blocks of each size class 8x8 .. 64x64 (list << 31 | block), cls_cap[c] entries from cls_off[c] of
   // cls_items, and their counts cls_n[4] (cleared by the enqueue)

@@ -525,10 +525,8 @@ class KeyframeEngine:
                                + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * mvgrid.MV_PT_DTYPE.itemsize)
             if self.mc_next:   # the NEXT slot of each frame and the mv1 of each vertex
                 self.h2d_bytes += 4 * self.F + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * 8
-        if self._fq is not None:   # the records and each frame's deringing threshold table (int32 [2][6])
-            self.h2d_bytes += self.F * (FRAME_QUANT_DTYPE.itemsize + 48)
-            if self.keyframe_quant:   # and its band quantisers (int32 [3][32])
-                self.h2d_bytes += self.F * 384
+        if self._fq is not None:   # the records, each frame's deringing thresholds (int32 [2][6]) and band quantisers ([3][32])
+            self.h2d_bytes += self.F * (FRAME_QUANT_DTYPE.itemsize + 48 + 384)
         return out
 
     def stage_ll_ref_slot_out(self, slots):
@@ -754,8 +752,8 @@ class KeyframeEngine:
 
     def upload(self, planes, bsize, pred=None, frame_quant=None):
         """Copies one batch straight into the engine's device buffers for run_device; frame_quant (frame_quant and
-        keyframe_quant engines): the [F] FRAME_QUANT_DTYPE records the step's kernels read (keyframe_quant: checked and
-        loaded with the tables submit derives from them, daala_b200_kf_load_frame_quant)."""
+        keyframe_quant engines): the [F] FRAME_QUANT_DTYPE records the step's kernels read, checked and loaded with the
+        tables submit derives from them (daala_b200_kf_load_frame_quant)."""
         g = self.geom
         self._check_pred(pred)
         if frame_quant is not None:
@@ -763,10 +761,7 @@ class KeyframeEngine:
                 raise ValueError("frame_quant= needs an engine created with frame_quant=1 or keyframe_quant=1")
             r = np.ascontiguousarray(frame_quant, FRAME_QUANT_DTYPE)
             assert r.shape == (self.F,)
-            if self.keyframe_quant:
-                self._check(self.L.daala_b200_kf_load_frame_quant(self.kf, r.ctypes.data), "upload")
-            else:
-                self._check(self.L.daala_b200_device_copy(self.buf.frame_quant, r.ctypes.data, r.nbytes, 0), "upload")
+            self._check(self.L.daala_b200_kf_load_frame_quant(self.kf, r.ctypes.data), "upload")
         for p in range(3):
             for dst, src in ((self.buf.pixels[p], planes[p]),) + (((self.buf.pred_pixels[p], pred[p]),) if pred is not None else ()):
                 a = np.ascontiguousarray(src, np.uint8)

@@ -438,7 +438,8 @@ typedef struct daala_b200_kf daala_b200_kf;
 typedef struct daala_b200_kf_config {
   int pic_w, pic_h;            /* luma picture size; frames are padded to whole 64x64 superblocks */
   int nframes;                 /* frames per batch (1..255), independent keyframes of one geometry */
-  int q0;                      /* state->quantizer */
+  int q0;                      /* state->quantizer; lossy engines (lossless = 0) refuse it outside [1,
+                                  DAALA_B200_KF_MAX_Q0], the range of a daala_b200_kf_frame_quant record's */
   int use_masking;             /* activity masking (OD_PVQ_BETA, src/pvq.c:205) */
   int qm_stride;               /* OD_QM_STRIDE = 5456 */
   double pvq_norm_lambda;      /* enc->pvq_norm_lambda */
@@ -526,7 +527,9 @@ typedef struct daala_b200_kf_config {
                                   encoder leaves stale vectors there).  Nothing after the prediction differs from a P
                                   frame.  mc_refs = 0 then means 3 * nframes.  Requires inter_mc = 1; other values, and
                                   1 without inter_mc, are refused by daala_b200_kf_create */
-  int frame_quant;             /* 0 (default): nothing below exists; the engine is exactly the one without this field.
+  int frame_quant;             /* 0 (default): every frame is coded at this config's quantizer: the engine makes one
+                                  daala_b200_kf_frame_quant record per frame from q0, coded_quantizer, dering_lambda
+                                  and pvq_qm_q4 at create, and its kernels read those records.
                                   1: every frame of a step has its own quantizer: daala_b200_kf_io.frame_quant gives one
                                   daala_b200_kf_frame_quant per frame, and the step and the finishing pass read no
                                   per-frame field of this config (q0, coded_quantizer, dering_lambda, pvq_qm_q4).  The
@@ -559,7 +562,8 @@ typedef struct daala_b200_kf_config {
                                   pvq_norm_lambda are the chain's quantizer and lambda.  Refused by daala_b200_kf_create
                                   with a value other than 0 or 1, and 1 together with inter, lossless or a row shard
                                   (sb_rows > 0: the superblock predictor reads the row above) */
-  int keyframe_quant;          /* 0 (default): nothing below exists; the engine is exactly the one without this field.
+  int keyframe_quant;          /* 0 (default): every keyframe is coded at this config's quantizer, through records
+                                  made from it as with frame_quant = 0.
                                   1: the keyframe counterpart of frame_quant: every keyframe of a step has its own
                                   quantizer, one daala_b200_kf_frame_quant per frame in daala_b200_kf_io.frame_quant.
                                   The luma chain kernel, the phase kernels, the DC chain (haar_dc_quant) and the
@@ -585,7 +589,8 @@ typedef struct daala_b200_kf_ll_block {   /* 16 bytes */
   int32_t reserved;        /* 0 */
 } daala_b200_kf_ll_block;
 
-/* config.frame_quant = 1 or config.keyframe_quant = 1: the quantizer of one frame of a batch, what od_enc_rc_select_quantizers_and_lambdas
+/* The quantizer of one frame of a batch (config.frame_quant = 1 or config.keyframe_quant = 1; other lossy engines make
+   theirs from the config), what od_enc_rc_select_quantizers_and_lambdas
    (reference src/rate.c:727-835, :1086) left in state / enc for that frame, and the pvq_qm_q4 table in force
    (src/encode.c:3050-3075).  Submit refuses a record with q0 outside [1, 8191] (8191 = od_codedquantizer_to_quantizer(63);
    lossless frames, quantizer 0, are coded by an engine with config.lossless), coded_quantizer outside [1, 63], a dering_lambda that is negative or
@@ -865,7 +870,8 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
   int32_t *ref_slot_next;               /* config.mc_next: the NEXT slots ([nframes]) and the mv1 grids */
   int32_t *mv1_grid;                    /* ([nframes][nvsb*8 + 1][nhsb*8 + 1][2]); NULL otherwise */
   daala_b200_kf_frame_quant *frame_quant;   /* config.frame_quant or keyframe_quant: the step's records ([nframes]);
-                                               NULL otherwise */
+                                               NULL otherwise.  Replace them with daala_b200_kf_load_frame_quant,
+                                               which also loads the tables derived from them */
   int32_t *haar_dc[3];                  /* config.haar_dc_quant: the DC chain's reconstructed DCs per plane, one entry per
                                            4x4 unit (leaf DCs at leaf origins), the three planes of a frame together
                                            (frame f of plane p at haar_dc[p] + f * (g0 + 2 g1), g = plane grid size) */
@@ -927,8 +933,8 @@ int daala_b200_kf_submit(daala_b200_kf *kf, const daala_b200_kf_io *io);
 int daala_b200_kf_frame_quant_derive(const daala_b200_kf_frame_quant *rec, int n, int32_t (*tbl)[2][6]);
 /* config.frame_quant or keyframe_quant, for run_device without a submit: checks the [nframes] records as submit does
    and copies them into the engine's device buffers with what submit derives from them (each frame's deringing
-   thresholds; keyframe_quant: each frame's band quantisers max(1, q0 * pvq_qm_q4[pli][i] >> 4), which the luma chain
-   kernel and the DC chain read), on the engine's stream, and waits for the copies.  The finishing pass's DC limit is
+   thresholds and its band quantisers max(1, q0 * pvq_qm_q4[pli][i] >> 4), which the PVQ kernels, the DC quantisers
+   and the finishing pass read), on the engine's stream, and waits for the copies.  The finishing pass's DC limit is
    not changed (a submit sets it). */
 int daala_b200_kf_load_frame_quant(daala_b200_kf *kf, const daala_b200_kf_frame_quant *rec);
 /* The finishing pass (config.inter_finish, see daala_b200_kf_finish_io) on the last submitted step: H2D of the

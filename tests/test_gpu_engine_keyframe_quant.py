@@ -13,7 +13,7 @@ created with per-frame config fields far from every record (q0 999, coded quanti
   settings.
 - Nothing is baked at create: batch A then batch B on one engine, live and replayed, equals a fresh engine's B; a
   permuted batch permutes the outputs.
-- Uniform records equal the engine without the mode; the schedules (split_free 0 / 1 / 2, forked graph / phase by phase,
+- Uniform records equal the engine without the mode, launches included; the schedules (split_free 0 / 1 / 2, forked graph / phase by phase,
   dering 1 / 2, haar_dc_quant on / off) agree; submit refuses missing and out-of-range records before any copy."""
 import os
 
@@ -255,7 +255,9 @@ def test_nothing_baked_at_create():
 
 
 @pytest.mark.parametrize("point", (0, 4, 7))
-def test_uniform_records_equal_the_engine_without_the_mode(point):
+def test_uniform_records_run_as_the_engine_without_the_mode(point):
+    """Records that all equal the config: the outputs of the engine without the mode, and the same kernel launches (both
+    read their quantizers from per-frame records)."""
     geom, config, F = Geometry(200, 130), 0, 3
     planes, maps = _frames(geom, F, seed=61 + point)
     base = _uniform(geom, point, config, F=F, **FULL)
@@ -269,8 +271,7 @@ def test_uniform_records_equal_the_engine_without_the_mode(point):
                                 dering_lambda=s["dering_lambda"], **_stream_kw(config), **FULL)
     try:
         got = _run(eng, planes, maps, _records((point,) * F, config))
-        # the level search adds the candidates' per-frame thresholds
-        assert eng.launches_per_step() == n_base + 1
+        assert eng.launches_per_step() == n_base
     finally:
         eng.close()
     _assert_steps_equal(got, want, geom, F, "uniform records")
