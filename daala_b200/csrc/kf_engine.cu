@@ -1329,6 +1329,10 @@ struct Sym {
   // with config.late_skip: the late-skip record of each slot, from the block-order records (else NULL)
   daala_b200_kf_late_skip* late_skip;   // [cap_blocks]
   const daala_b200_kf_late_skip* ls_block[2];
+  // symbol_stream = 1 with haar_dc_quant: the keyframe DC record of each slot, from the DC chain's index grids (else NULL)
+  daala_b200_kf_sym_hdc* hdc;      // [cap_blocks]
+  const int32_t* hdc_index[3];     // [F][gh][gw] per plane
+  int gw[3], gh[3];                // index grid width / height (4x4 units of the plane)
 };
 
 // Bytes the band's pulses take in the stream: the n - (itheta != -1) values pvq_encode_partition hands to
@@ -1398,6 +1402,90 @@ __global__ void __launch_bounds__(1024) k_sym_sb_scan(const __grid_constant__ Sy
     __syncthreads();
   }
   if (t == 0) S.tot[0] = min(carry, S.cap_blocks);
+}
+
+// symbol_stream = 1 with haar_dc_quant: the keyframe DC records (daala_b200_kf_sym_hdc), one warp per (frame, superblock,
+// plane).  od_encode_recursive (src/encode.c:1660-1787) codes the superblock DC, then at every split node, before its
+// children, the node's three indices: a quadtree with L leaves gives 1 + 3 (L - 1) / 3 = L records, which fill the slots
+// of the (superblock, plane)'s L block records.  Pre-order is the Z order of the nodes' origins, coarser nodes first at
+// a shared origin, so a node's place among the split nodes is a warp scan over the superblock's 64 units in Z order
+// (lane l: units 2l and 2l + 1, as k_sym_rank) of the split nodes whose origin each unit is.  A node is split when it and
+// every ancestor read a size below their own at their origin (max(obs, xdec) < bsi, the map at the node's 8x8 unit);
+// its first leaf is the leaf at its origin unit, whose slot k_sym_rank / k_sym_sb_scan already give.
+__global__ void __launch_bounds__(256) k_sym_hdc(const __grid_constant__ Sym S) {
+  const int lane = threadIdx.x & 31;
+  const int item = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (item >= S.F * S.nsb * 3) return;   // whole warps
+  const int sb = item / 3, pli = item - 3 * sb;
+  const int f = sb / S.nsb, r = sb % S.nsb;
+  const int sby = r / S.nhsb, sbx = r % S.nhsb;
+  const int uw = S.nhsb * 8, xdec = pli ? 1 : 0;
+  int b[2], ux[2], uy[2];
+  for (int h = 0; h < 2; h++) {
+    const int m = 2 * lane + h;
+    ux[h] = sbx * 8 + ((m & 1) | ((m >> 1) & 2) | ((m >> 2) & 4));
+    uy[h] = S.u_row0 + sby * 8 + (((m >> 1) & 1) | ((m >> 2) & 2) | ((m >> 3) & 4));
+    b[h] = max((int)S.bsize[f * S.bsize_pitch + (long long)uy[h] * S.bstride + ux[h]], xdec);
+  }
+  // the sizes at the origins of the unit's 16x16, 32x32 and 64x64 luma ancestors (Z codes multiple of 4, 16, 64: even)
+  const int b2 = __shfl_sync(0xffffffffu, b[0], lane & ~1);
+  const int b3 = __shfl_sync(0xffffffffu, b[0], lane & ~7);
+  const int b4 = __shfl_sync(0xffffffffu, b[0], 0);
+  const bool s4 = b4 < 4, s3 = s4 && b3 < 3, s2 = s3 && b2 < 2;
+  // the split nodes whose origin is each of the lane's units: bit 4 - bsi of the mask, so the coarsest is the lowest bit
+  int mask[2];
+  for (int h = 0; h < 2; h++) {
+    const int m = 2 * lane + h;
+    mask[h] = (m == 0 && s4 ? 1 : 0) | ((m & 15) == 0 && s3 ? 2 : 0) | ((m & 3) == 0 && s2 ? 4 : 0) |
+              (s2 && b[h] < 1 ? 8 : 0);
+  }
+  const int n = __popc(mask[0]) + __popc(mask[1]);
+  int inc = n;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int a = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += a;
+  }
+  const uint32_t sc = S.sb_cnt[sb];
+  const int plane_off = pli ? (int)(sc & 0xffff) + (pli - 1) * (int)(sc >> 16) : 0;
+  const long long base = (long long)S.sb_base[sb] + plane_off;            // the (superblock, plane)'s first slot
+  const long long first = S.sb_base[f * S.nsb];                           // the frame's first slot
+  const int32_t* grid = S.hdc_index[pli] + (long long)f * S.gw[pli] * S.gh[pli];
+  const int gsh = pli ? 0 : 1;   // 4x4 units of the plane per 8x8 luma unit: log2 2 (luma) or 1 (4:2:0 chroma)
+  if (lane == 0 && base < S.cap_blocks) {
+    daala_b200_kf_sym_hdc d;
+    d.value = grid[(long long)(uy[0] << gsh) * S.gw[pli] + (ux[0] << gsh)];
+    d.block = (uint32_t)(base - first);
+    d.pli = (uint8_t)pli;
+    d.bsi = 4;
+    d.child = 0;
+    d.reserved = 0;
+    S.hdc[base] = d;
+  }
+  int k = inc - n;   // split nodes before the lane's first unit, in pre-order
+  for (int h = 0; h < 2; h++) {
+    if (!mask[h]) continue;
+    const uint32_t rk = S.unit_rank[((long long)f * S.sb_rows * 8 + (uy[h] - S.u_row0)) * uw + ux[h]];
+    const uint32_t block = (uint32_t)(base - first) + (pli ? rk >> 16 : rk & 0xffff);
+    const int gx = ux[h] << gsh, gy = uy[h] << gsh;
+    for (int bsi = 4; bsi >= 1; bsi--) {
+      if (!(mask[h] & (1 << (4 - bsi)))) continue;
+      const int half = 1 << (bsi - 1 - xdec);   // child offset in 4x4 units of the plane
+      for (int c = 1; c <= 3; c++) {
+        const long long slot = base + 1 + 3 * k + (c - 1);
+        if (slot >= S.cap_blocks) break;
+        daala_b200_kf_sym_hdc d;
+        d.value = grid[(long long)(gy + (c >> 1) * half) * S.gw[pli] + gx + (c & 1) * half];
+        d.block = block;
+        d.pli = (uint8_t)pli;
+        d.bsi = (uint8_t)(bsi - 1);
+        d.child = (uint8_t)c;
+        d.reserved = 0;
+        S.hdc[slot] = d;
+      }
+      k++;
+    }
+  }
 }
 
 // Per block (luma list, then chroma list): its slot, and the slot's band count and pulse bytes.
@@ -1578,9 +1666,9 @@ __global__ void k_sym_index(const __grid_constant__ Sym S) {
 }
 
 // Copy of the used part of each stream array into the caller's pinned host buffers (device-addressable):
-// the lengths are only known on the device.  Segment 0 index, 1 block records, 2 band records, 3 pulses, 4 DC records
-// and 5 late-skip records (one per block record each).
-constexpr int kSymSegs = 6;
+// the lengths are only known on the device.  Segment 0 index, 1 block records, 2 band records, 3 pulses, 4 DC records,
+// 5 late-skip records and 6 keyframe DC records (one per block record each).
+constexpr int kSymSegs = 7;
 struct SymCopy {
   const uint8_t* src[kSymSegs];
   uint8_t* dst[kSymSegs];
@@ -2211,6 +2299,14 @@ static int kf_alloc(daala_b200_kf* kf) {
         Y.dc_resid[c] = kf->dc_resid[c];
       }
     }
+    if (kf->cfg.haar_dc_quant) {
+      KF_CHECK(dalloc(kf, &Y.hdc, (size_t)Y.cap_blocks));
+      for (int p = 0; p < 3; p++) {
+        Y.hdc_index[p] = kf->hdc_index[p];
+        Y.gw[p] = kf->plane_w[p] >> 2;
+        Y.gh[p] = kf->plane_h[p] >> 2;
+      }
+    }
   }
   if (kf->cfg.late_skip) {
     daala_b200_late_skip_batch& B = kf->lsb;
@@ -2504,11 +2600,13 @@ static void enqueue_split(daala_b200_kf* kf, const Stage& S, cudaStream_t s) {
 }
 
 // The symbol stream of the step (cfg.symbol_stream), after both stages' k_finish_scatter: rank, superblock scan,
-// place, the three scan kernels, pack (kInter: with the DC records), index.
+// [haar_dc_quant: the keyframe DC records, after the DC chain], place, the three scan kernels, pack (kInter: with the DC
+// records), index.
 template <bool kInter>
 static void enqueue_sym(const Sym& Y, int wide, cudaStream_t s) {
   k_sym_rank<<<(Y.F * Y.nsb + 7) / 8, 256, 0, s>>>(Y);
   k_sym_sb_scan<<<1, 1024, 0, s>>>(Y);
+  if (!kInter && Y.hdc) k_sym_hdc<<<(Y.F * Y.nsb * 3 + 7) / 8, 256, 0, s>>>(Y);
   k_sym_place<<<wide, 256, 0, s>>>(Y);
   k_sym_tile_sums<<<Y.ntiles, kTile, 0, s>>>(Y);
   k_sym_tile_scan<<<1, 1024, 0, s>>>(Y);
@@ -2965,7 +3063,8 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   n += 2 + (kf->cfg.split_free > 0 ? split(kf->chroma) : 1);                      // chroma: gather, bands, finish
   // inverse + SB postfilter of plane 0 and of planes 1-2, [the rest of the deringing pass]
   n += kf->cfg.dering ? dering_launches(kf->dering, 2) : 4;
-  if (kf->cfg.symbol_stream) n += 8;             // symbol stream: rank, superblock scan, place, 3 scan kernels, pack, index
+  // symbol stream: rank, superblock scan, [haar_dc_quant: DC records], place, 3 scan kernels, pack, index
+  if (kf->cfg.symbol_stream) n += 8 + (kf->cfg.haar_dc_quant ? 1 : 0);
   return n;
 }
 
@@ -3022,6 +3121,7 @@ int daala_b200_kf_device_buffers(daala_b200_kf* kf, daala_b200_kf_buffers* out) 
     out->haar_dc[p] = kf->hdcb.dc[p];
     out->dc_index[p] = kf->hdc_index[p];
   }
+  out->sym_hdc = kf->sym.hdc;
   return 0;
 }
 
@@ -3265,8 +3365,12 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   SymCopy sc;
   memset(&sc, 0, sizeof(sc));
   const bool want_sym = io->sym_index || io->sym_blocks || io->sym_bands || io->sym_pulses || io->sym_dc ||
-                        io->sym_late_skip;
+                        io->sym_late_skip || io->sym_hdc;
   if (want_sym) {
+    if (io->sym_hdc && !(kf->cfg.symbol_stream == 1 && kf->cfg.haar_dc_quant)) {
+      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: sym_hdc needs an engine with symbol_stream = 1 and haar_dc_quant = 1");
+      return (int)cudaErrorInvalidValue;
+    }
     if (!kf->cfg.symbol_stream) return (int)cudaErrorInvalidValue;
     if (io->sym_dc && kf->cfg.symbol_stream != 2) {
       snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: sym_dc needs an engine with symbol_stream = 2");
@@ -3286,6 +3390,12 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
                "daala_b200_kf_symbol_bounds(...).blocks records");
       return (int)cudaErrorInvalidValue;
     }
+    if (sym_target(io->sym_hdc, io->sym_hdc_cap, bd.blocks, &sc.dst[6])) {
+      snprintf(kf->err, sizeof(kf->err),
+               "daala_b200_kf_submit: sym_hdc must be pinned host memory of at least "
+               "daala_b200_kf_symbol_bounds(...).blocks records");
+      return (int)cudaErrorInvalidValue;
+    }
     const Sym& Y = kf->sym;
     sc.src[0] = (const uint8_t*)Y.index;
     sc.src[1] = (const uint8_t*)Y.blocks;
@@ -3293,22 +3403,26 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     sc.src[3] = Y.pulses;
     sc.src[4] = (const uint8_t*)Y.dc;
     sc.src[5] = (const uint8_t*)Y.late_skip;
+    sc.src[6] = (const uint8_t*)Y.hdc;
     sc.unit[1] = sizeof(daala_b200_kf_sym_block);
     sc.unit[2] = 4 * sizeof(int16_t);
     sc.unit[3] = 1;
     sc.unit[4] = sizeof(daala_b200_kf_sym_dc);
     sc.unit[5] = sizeof(daala_b200_kf_late_skip);
+    sc.unit[6] = sizeof(daala_b200_kf_sym_hdc);
     sc.index_bytes = (long long)F * sizeof(daala_b200_kf_sym_frame);
     sc.tot = Y.tot;
     const long long host[kSymSegs] = {io->sym_index_cap * (long long)sizeof(daala_b200_kf_sym_frame),
                                       io->sym_blocks_cap * (long long)sizeof(daala_b200_kf_sym_block),
                                       io->sym_bands_cap * 8, io->sym_pulses_cap,
                                       io->sym_dc_cap * (long long)sizeof(daala_b200_kf_sym_dc),
-                                      io->sym_late_skip_cap * (long long)sizeof(daala_b200_kf_late_skip)};
+                                      io->sym_late_skip_cap * (long long)sizeof(daala_b200_kf_late_skip),
+                                      io->sym_hdc_cap * (long long)sizeof(daala_b200_kf_sym_hdc)};
     const long long dev[kSymSegs] = {sc.index_bytes, (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_block),
                                      Y.cap_bands * 8, Y.cap_bytes,
                                      Y.dc ? (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_dc) : 0,
-                                     Y.late_skip ? (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_late_skip) : 0};
+                                     Y.late_skip ? (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_late_skip) : 0,
+                                     Y.hdc ? (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_hdc) : 0};
     for (int i = 0; i < kSymSegs; i++) sc.cap[i] = host[i] < dev[i] ? host[i] : dev[i];
   }
   for (int p = 0; p < 3; p++) {

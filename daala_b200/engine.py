@@ -35,7 +35,9 @@ daala_b200/lossless.py restates the path in numpy.
 With haar_dc_quant=1 (keyframes) the step quantises the keyframe DCs as the reference encoder does (its superblock DC
 predictor and Haar-level quantiser, with the adaptive DC rate): the reconstruction, the coefficient planes and the CfL
 reference carry the quantised DCs, and `encode` returns the coded indices as dc_index0..2 ([F, h / 4, w / 4] int32 per
-plane).  daala_b200/haardc.py restates the chain in numpy.
+plane).  daala_b200/haardc.py restates the chain in numpy.  With symbol_stream=1 too the stream carries the same
+indices in coding order, one symbols.HDC_DTYPE record per block record (`sym_hdc`), and `encode(..., dc_grids=False)`
+leaves the grids out.
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -105,7 +107,8 @@ class IO(ctypes.Structure):
                 ("luma_late_skip", c_void_p), ("chroma_late_skip", c_void_p), ("sym_late_skip", c_void_p),
                 ("sym_late_skip_cap", c_ll), ("ref_slot_next", c_void_p), ("mv1_grid", c_void_p),
                 ("frame_quant", c_void_p), ("ll_coeffs", c_void_p * 3), ("ll_blocks", c_void_p),
-                ("ll_ref_slot_out", c_void_p), ("dc_index", c_void_p * 3)]
+                ("ll_ref_slot_out", c_void_p), ("dc_index", c_void_p * 3), ("sym_hdc", c_void_p),
+                ("sym_hdc_cap", c_ll)]
 
 
 class FinishIO(ctypes.Structure):
@@ -132,7 +135,7 @@ class Buffers(ctypes.Structure):
                 ("luma_heads_raw", c_void_p), ("luma_head_bin", c_void_p), ("ref_pixels", c_void_p * 3),
                 ("ref_slot", c_void_p), ("mv_grid", c_void_p), ("mc_refs", c_int), ("ref_slot_next", c_void_p),
                 ("mv1_grid", c_void_p), ("frame_quant", c_void_p), ("haar_dc", c_void_p * 3),
-                ("dc_index", c_void_p * 3)]
+                ("dc_index", c_void_p * 3), ("sym_hdc", c_void_p)]
 
 
 def _bind():
@@ -415,15 +418,16 @@ class KeyframeEngine:
                     "symbol_bounds")
         return b
 
-    def prepare_io(self, symbols=True, recon=True, stream=None, pred=True):
+    def prepare_io(self, symbols=True, recon=True, stream=None, pred=True, dc_grids=True):
         """Builds the daala_b200_kf_io record over the staged inputs and result buffers sized for them.
         stream (default: whether the engine was created with symbol_stream) adds the symbol stream buffers
         sym_index, sym_blocks, sym_bands and sym_pulses (daala_b200/symbols.py), and sym_dc on a symbol_stream=2
-        engine (and sym_late_skip on one with late_skip too), pinned and sized by daala_b200_kf_symbol_bounds; only
-        their used part is copied back.  late_skip engines return luma_late_skip / chroma_late_skip
-        (symbols.LATE_SKIP_DTYPE per block, block order) with the symbols.  On a
-        symbol_stream=2 engine symbols=False also leaves out the classic DC arrays (the stream carries them).
-        pred=False (inter_mc engines): the prediction planes are not copied back."""
+        engine (and sym_late_skip on one with late_skip too), or sym_hdc on a symbol_stream=1 engine with
+        haar_dc_quant, pinned and sized by daala_b200_kf_symbol_bounds; only their used part is copied back.
+        late_skip engines return luma_late_skip / chroma_late_skip (symbols.LATE_SKIP_DTYPE per block, block order)
+        with the symbols.  On a symbol_stream=2 engine symbols=False also leaves out the classic DC arrays (the stream
+        carries them).  pred=False (inter_mc engines): the prediction planes are not copied back.  dc_grids=False
+        (haar_dc_quant engines): the index grids dc_index0..2 are not copied back (sym_hdc carries the same indices)."""
         if self.lossless:
             return self._prepare_io_lossless(recon, pred)
         g, t = self.geom, self.totals
@@ -489,7 +493,7 @@ class KeyframeEngine:
             io.frame_quant = self._fq.ctypes.data
         if self._ll_slot is not None:   # refused by the C call: a lossy engine has no lossless step
             io.ll_ref_slot_out = self._ll_slot.ctypes.data
-        if self.haar_dc_quant:
+        if self.haar_dc_quant and dc_grids:
             for p in range(3):
                 h, w = g.plane_shape(p)
                 out["dc_index%d" % p] = self._arr("dci%d" % p, (self.F, h >> 2, w >> 2), np.int32)
@@ -517,6 +521,9 @@ class KeyframeEngine:
                 if self.late_skip:
                     out["sym_late_skip"] = self._arr("sls", (int(b.blocks),), sym.LATE_SKIP_DTYPE, pinned=True)
                     io.sym_late_skip, io.sym_late_skip_cap = out["sym_late_skip"].ctypes.data, int(b.blocks)
+            elif self.haar_dc_quant:
+                out["sym_hdc"] = self._arr("shdc", (int(b.blocks),), sym.HDC_DTYPE, pinned=True)
+                io.sym_hdc, io.sym_hdc_cap = out["sym_hdc"].ctypes.data, int(b.blocks)
         self._io, self._out = io, out
         px = sum(int(np.prod(g.plane_shape(p))) for p in range(3))
         self.h2d_bytes = px * self.F * (2 if self.inter and not self.inter_mc else 1) + int(np.prod(g.bsize_shape)) * self.F
@@ -598,22 +605,24 @@ class KeyframeEngine:
     def stream_d2h_bytes(self):
         """Bytes the last submit copied of the symbol stream (after wait): the index and the used part of the
         other arrays (block records, band records, pulses and, on symbol_stream=2 engines, DC records and, with
-        late_skip, late-skip records)."""
+        late_skip, late-skip records; with haar_dc_quant, the keyframe DC records)."""
         from . import symbols as sym
         idx = self._out["sym_index"]
         blocks = int(idx[:, 1].sum())
         dc = blocks * sym.DC_DTYPE.itemsize if "sym_dc" in self._out else 0
         dc += blocks * sym.LATE_SKIP_DTYPE.itemsize if "sym_late_skip" in self._out else 0
+        dc += blocks * sym.HDC_DTYPE.itemsize if "sym_hdc" in self._out else 0
         return idx.nbytes + blocks * sym.BLOCK_DTYPE.itemsize + int(idx[:, 3].sum()) * 8 + int(idx[:, 5].sum()) + dc
 
     def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None, pred=None, refs=None,
-               ref_slot=None, mv_grid=None, resident=False, mv1_grid=None, frame_quant=None, ll_ref_slot_out=None):
+               ref_slot=None, mv_grid=None, resident=False, mv1_grid=None, frame_quant=None, ll_ref_slot_out=None,
+               dc_grids=True):
         """One batch end to end through the C ABI with host buffers; returns the result arrays (views of
         the engine's host buffers: copy what must survive the next call).  pred: see stage_inputs; refs, ref_slot,
         mv_grid, resident, mv1_grid (inter_mc engines, which also return the prediction as pred0..2): see stage_mc;
         frame_quant (frame_quant and keyframe_quant engines, required there): [F] FRAME_QUANT_DTYPE records, see
         stage_frame_quant;
-        ll_ref_slot_out (lossless engines with inter_mc): see stage_ll_ref_slot_out.  On a lossless engine bsize is not
+        ll_ref_slot_out (lossless engines with inter_mc): see stage_ll_ref_slot_out; dc_grids: see prepare_io.  On a lossless engine bsize is not
         read (None is fine) and the results are those of _prepare_io_lossless.  Raises
         when the batch exceeded the block capacity, or (inter_mc) when a used vertex names a picture other than GOLD /
         PREV (/ NEXT on mc_next engines) or a vector reaches past the reference's edge extension: the reference
@@ -626,7 +635,7 @@ class KeyframeEngine:
             self.stage_dering_levels(dering_levels)
         self.stage_frame_quant(frame_quant)
         self.stage_ll_ref_slot_out(ll_ref_slot_out)
-        self.prepare_io(symbols, recon, stream)
+        self.prepare_io(symbols, recon, stream, dc_grids=dc_grids)
         self.submit()
         out = self.wait()
         if int(out["counts"][CNT["error"]]):

@@ -22,6 +22,8 @@ import math
 
 import numpy as np
 
+from .symbols import HDC_DTYPE
+
 GENERIC_TABLES = 12
 OD_DC_QM = ((21, 25), (18, 20), (17, 18), (17, 17))   # src/state.c:48
 M_LOG2E = 1.4426950408889634074
@@ -203,3 +205,69 @@ def quantize_frame(geom, d_planes, bsize, q0, pvq_qm_q4, lam):
         out["idx"].append(idx)
         out["stats"].append(st)
     return out
+
+
+# What a host coder reads of the chain (config.symbol_stream = 1 with haar_dc_quant = 1; include/daala_b200.h,
+# daala_b200_kf_sym_hdc): per superblock in raster order, planes 0, 1, 2, the superblock DC and then every split node's
+# three indices in od_encode_recursive's pre-order, each record naming the block record the coder emits it before.
+# The records are symbols.HDC_DTYPE.
+
+
+def _walk_records(bsize, geom, visit):
+    """The DC symbols of one frame in coding order: visit(pli, gy, gx, bsi, child, block) per symbol, with (gy, gx) the
+    index grid position of the symbol (4x4 units of the plane), bsi the record's size index and block the frame-relative
+    index of the leaf the symbol precedes.  Returns the frame's leaf count."""
+    bsize = np.asarray(bsize)
+    leaves = [0]
+
+    def recurse(pli, xdec, bx, by, bsi):
+        obs = int(bsize[(by << bsi) >> 1, (bx << bsi) >> 1])
+        if max(obs, xdec) >= bsi:
+            leaves[0] += 1
+            return
+        first = leaves[0]
+        sh = bsi - 1 - xdec             # child edge in 4x4 units of the plane: 2 ** sh
+        gx, gy = (2 * bx) << sh, (2 * by) << sh
+        half = 1 << sh
+        for c in (1, 2, 3):
+            visit(pli, gy + (c >> 1) * half, gx + (c & 1) * half, bsi - 1, c, first)
+        for cy in (0, 1):
+            for cx in (0, 1):
+                recurse(pli, xdec, 2 * bx + cx, 2 * by + cy, bsi - 1)
+
+    for sby in range(geom.nvsb):
+        for sbx in range(geom.nhsb):
+            for pli in range(3):
+                xdec = geom.xdec[pli]
+                g = 16 >> xdec                   # superblock edge in 4x4 units of the plane
+                visit(pli, sby * g, sbx * g, 4, 0, leaves[0])
+                recurse(pli, xdec, sbx, sby, 4)
+    return leaves[0]
+
+
+def stream_records(idx_planes, bsize, geom):
+    """One frame's keyframe DC records (HDC_DTYPE, one per leaf block, in coding order) from its index grids
+    (idx_planes: 3 x [h / 4, w / 4], what quantize_frame returns as idx and the engine as dc_index0..2) and its
+    block-size map."""
+    out = []
+    _walk_records(bsize, geom, lambda pli, gy, gx, bsi, c, blk: out.append(
+        (int(idx_planes[pli][gy, gx]), blk, pli, bsi, c, 0)))
+    return np.array(out, HDC_DTYPE)
+
+
+def grids_from_records(records, bsize, geom):
+    """The inverse of stream_records: the three index grids (int32, 0 where no symbol is coded) from one frame's
+    records.  Asserts that the records are those of the map (count, order, sizes and blocks)."""
+    idx = [np.zeros((h >> 2, w >> 2), np.int32) for h, w in (geom.plane_shape(p) for p in range(3))]
+    it = iter(np.asarray(records, HDC_DTYPE))
+
+    def visit(pli, gy, gx, bsi, c, blk):
+        r = next(it, None)
+        assert r is not None, "fewer records than the map's symbols"
+        assert (int(r["pli"]), int(r["bsi"]), int(r["child"]), int(r["block"])) == (pli, bsi, c, blk), \
+            "record does not fit the map: %r against %r" % (r, (pli, bsi, c, blk))
+        idx[pli][gy, gx] = r["value"]
+
+    n = _walk_records(bsize, geom, visit)
+    assert len(records) == n, "%d records for %d leaves" % (len(records), n)
+    return idx

@@ -26,6 +26,11 @@ BAND_EDGES = np.array([1, 16, 24, 32, 64, 96, 128, 256, 384, 512])   # OD_BAND_O
 ORDER_DTYPE = np.dtype([("pli", "u1"), ("x0", "<u2"), ("y0", "<u2"), ("bs", "u1")])
 DC_DTYPE = np.dtype([("qdc", "<i4"), ("dc_resid", "<i4")])
 assert DC_DTYPE.itemsize == 8
+# symbol_stream = 1 with haar_dc_quant = 1: daala_b200_kf_sym_hdc, the keyframe's DC symbols in coding order, one per
+# block record (sym_hdc, same index range; haardc.stream_records)
+HDC_DTYPE = np.dtype([("value", "<i4"), ("block", "<u4"), ("pli", "u1"), ("bsi", "u1"), ("child", "u1"),
+                      ("reserved", "u1")])
+assert HDC_DTYPE.itemsize == 12
 # config.late_skip: daala_b200_kf_late_skip, one per block (block order) or per block record (sym_late_skip)
 LATE_SKIP_DTYPE = np.dtype([("dist_skip", "<f8"), ("noskip_coded_dc0", "<f8"), ("noskip_coded_dcq", "<f8"),
                             ("noskip_pred_dcq", "<f8")])
@@ -55,10 +60,11 @@ def _band_numbers(bs):
 
 
 def read_frame(out, f):
-    """Frame f of a submit's stream outputs (sym_index, sym_blocks, sym_bands, sym_pulses[, sym_dc]): dict with
-    `blocks` (BLOCK_DTYPE), `bands` (int16[B, 4]), `band_block` (block of each band), `band_no` (band number inside
-    its block), `pulses` (per band an int32 vector of its coded values; empty when K = 0) and, when the outputs have
-    sym_dc, `dc` (DC_DTYPE, one record per block)."""
+    """Frame f of a submit's stream outputs (sym_index, sym_blocks, sym_bands, sym_pulses[, sym_dc][, sym_hdc]): dict
+    with `blocks` (BLOCK_DTYPE), `bands` (int16[B, 4]), `band_block` (block of each band), `band_no` (band number
+    inside its block), `pulses` (per band an int32 vector of its coded values; empty when K = 0) and, when the outputs
+    have sym_dc, `dc` (DC_DTYPE, one record per block), when they have sym_hdc, `hdc` (HDC_DTYPE, one record per
+    block)."""
     idx = out["sym_index"][f]
     b0, nb, n0, nn, y0, ny = (int(v) for v in idx)
     blocks = out["sym_blocks"][b0:b0 + nb]
@@ -86,6 +92,8 @@ def read_frame(out, f):
     r = dict(blocks=blocks, bands=bands, band_block=band_block, band_no=band_no, pulses=pulses)
     if "sym_dc" in out:
         r["dc"] = out["sym_dc"][b0:b0 + nb]
+    if "sym_hdc" in out:
+        r["hdc"] = out["sym_hdc"][b0:b0 + nb]
     return r
 
 
@@ -183,9 +191,11 @@ def pack_reference(out, frames):
     put in bitstream order by sorting on (superblock, plane, Z order of the origin), independently of how the
     device ranks them.  Returns dict(sym_index, sym_blocks, sym_bands, sym_pulses) over those frames.  The outputs of
     a P-frame step (they have luma_dc / chroma_dc, and luma_dc_resid / chroma_dc_resid must be there too) give the
-    P-frame stream: flip 0 and sym_dc from *_dc and *_dc_resid."""
+    P-frame stream: flip 0 and sym_dc from *_dc and *_dc_resid.  Those of a haar_dc_quant keyframe step with the index
+    grids (dc_index0..2) give sym_hdc too (haardc.stream_records over the map the luma blocks tile)."""
     frames = list(range(frames)) if np.isscalar(frames) else list(frames)
     inter = "luma_dc" in out
+    hdc = not inter and "dc_index0" in out
     lb, cb = out["luma_blocks"], out["chroma_blocks"]
     nl_coefs = len(out["luma_y16"])
     y = np.concatenate([out["luma_y16"], out["chroma_y16"]])
@@ -208,7 +218,26 @@ def pack_reference(out, frames):
                 dc[k] = np.concatenate([out["luma_" + k][sl], out["chroma_" + k][sc]])[o]
         parts.append(pack_blocks(blk["x0"][o], blk["y0"][o], blk["bs"][o], pli[o], flip[o], skip[o], res[o], y,
                                  y_off[o], dc.get("dc"), dc.get("dc_resid")))
-    return concat_frames(parts)
+        if hdc:
+            parts[-1] = parts[-1][:3] + (_hdc_reference(out, lb[sl], f),)
+    r = concat_frames(parts)
+    if hdc:
+        r["sym_hdc"] = r.pop("sym_dc")
+    return r
+
+
+def _hdc_reference(out, luma, f):
+    """Frame f's keyframe DC records from the index grids dc_index0..2 and the map its luma blocks tile."""
+    from . import haardc
+    from .frame import Geometry
+    idx = [np.asarray(out["dc_index%d" % p][f]) for p in range(3)]
+    gh, gw = idx[0].shape
+    geom = Geometry(gw * 4, gh * 4)
+    bsize = np.zeros(geom.bsize_shape, np.uint8)
+    for x0, y0, bs in zip(luma["x0"].astype(np.int64), luma["y0"].astype(np.int64), luma["bs"].astype(np.int64)):
+        n = max(1, 1 << (bs - 1))            # 8x8 units the block spans (a 4x4 block: its unit, value 0)
+        bsize[y0 >> 3:(y0 >> 3) + n, x0 >> 3:(x0 >> 3) + n] = bs
+    return haardc.stream_records(idx, bsize, geom)
 
 
 def stream_to_classic(out):
@@ -247,6 +276,8 @@ def stream_equal(got, want, frames_got, frames_want=None):
         parts = (("sym_blocks", 0, 1), ("sym_bands", 2, 3), ("sym_pulses", 4, 5))
         if "sym_dc" in got or "sym_dc" in want:
             parts += (("sym_dc", 0, 1),)
+        if "sym_hdc" in got or "sym_hdc" in want:
+            parts += (("sym_hdc", 0, 1),)
         for key, c0, c1 in parts:
             if key not in got or key not in want:
                 bad.append((fg, key, "missing"))

@@ -674,6 +674,26 @@ typedef struct daala_b200_kf_late_skip {   /* 32 bytes */
   double noskip_pred_dcq;   /* ... AC = md (PVQ skip), d[0] = md[0] + q1 * dc_quant */
 } daala_b200_kf_late_skip;
 
+/* Engines with symbol_stream = 1 and haar_dc_quant = 1: the keyframe's DC symbols in the order od_encode_coefficients
+   codes them (reference src/encode.c:2605-2656, :1765-1787), one record per block record, so a frame's part is
+   first_block / n_blocks of the index as for the block records.  A quadtree with L leaves has (L - 1) / 3 split nodes,
+   and the reference codes one superblock DC per (superblock, plane) and three indices per split node: L symbols.  Per
+   (superblock, plane) the records fill the index range of its block records: the superblock DC first, then each split
+   node's three (child 1, 2, 3) in pre-order with the children top-left, top-right, bottom-left, bottom-right.  A host
+   coder emits record j just before block record `block` (after, on luma with child == 1, the node's split symbol,
+   src/encode.c:1765-1769): generic_encode of |value| on the plane's DC model with ex_sb_dc[pli] (child 0) or
+   ex_dc[pli][bsi][child - 1], then the sign bit when value != 0 (od_ec_enc_bits(ec, value < 0, 1)). */
+typedef struct daala_b200_kf_sym_hdc {     /* 12 bytes */
+  int32_t value;           /* the signed coded index (what daala_b200_kf_io.dc_index holds at the node's position) */
+  uint32_t block;          /* frame-relative index of the block record the coder emits this symbol before: the first
+                              leaf, in coding order, of the superblock (child 0) or of the split node (1..3) */
+  uint8_t pli;
+  uint8_t bsi;             /* child 0: 4 (the superblock).  1..3: the bsi od_quantize_haar_dc_level is called with
+                              (od_encode_recursive's bsi - 1, the luma size index also for chroma): ex_dc[pli][bsi] */
+  uint8_t child;           /* 0: the superblock DC; 1..3: x[child] of the split node */
+  uint8_t reserved;        /* 0 */
+} daala_b200_kf_sym_hdc;
+
 typedef struct daala_b200_kf_sym_frame {   /* one frame's part of the batch-wide arrays (indices, not bytes, */
   int64_t first_block, n_blocks;           /* except for the pulses) */
   int64_t first_band, n_bands;
@@ -780,6 +800,11 @@ typedef struct daala_b200_kf_io {
      children 1, 2, 3 (top right, bottom left, bottom right), 0 everywhere else.  INTEGRATION.md describes the order
      the coder reads them in. */
   int32_t *dc_index[3];
+  /* config.symbol_stream = 1 with haar_dc_quant = 1 only (refused otherwise): the keyframe DC records of the stream
+     (daala_b200_kf_sym_hdc), a pinned host buffer with its capacity in records, at least
+     daala_b200_kf_symbol_bounds(...).blocks; NULL = not copied.  Only the used part is copied, as for sym_dc. */
+  daala_b200_kf_sym_hdc *sym_hdc;
+  long long sym_hdc_cap;
 } daala_b200_kf_io;
 
 /* The finishing pass of a P-frame batch (config.inter_finish), daala_b200_kf_finish: the host coder's per-block
@@ -876,6 +901,9 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
                                            4x4 unit (leaf DCs at leaf origins), the three planes of a frame together
                                            (frame f of plane p at haar_dc[p] + f * (g0 + 2 g1), g = plane grid size) */
   int32_t *dc_index[3];                 /* and the index grids ([nframes][plane_h / 4][plane_w / 4]); else NULL */
+  daala_b200_kf_sym_hdc *sym_hdc;       /* config.symbol_stream = 1 with haar_dc_quant: the step's keyframe DC records,
+                                           the frames one after the other from index 0 (what io.sym_hdc receives,
+                                           max_luma_blocks + max_chroma_blocks entries); else NULL */
 } daala_b200_kf_buffers;
 
 #define DAALA_B200_KF_LISTS 1
@@ -910,8 +938,9 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    anything is copied or launched; so does a request for symbol stream outputs from an engine created without
    symbol_stream (sym_dc: without symbol_stream = 2), a stream capacity below daala_b200_kf_symbol_bounds, a stream
    buffer that is not pinned host memory, or (config.inter) a NULL pred_pixels plane, luma_dc or chroma_dc (the last
-   two are optional with symbol_stream = 2), a late-skip output on an engine without late_skip, and sym_late_skip
-   without symbol_stream = 2 (each with a message in daala_b200_kf_error).  With config.inter_mc it refuses, the same
+   two are optional with symbol_stream = 2), a late-skip output on an engine without late_skip, sym_late_skip
+   without symbol_stream = 2, and sym_hdc on an engine without both symbol_stream = 1 and haar_dc_quant = 1, below
+   daala_b200_kf_symbol_bounds(...).blocks records or not pinned (each with a message in daala_b200_kf_error).  With config.inter_mc it refuses, the same
    way, a NULL mv_grid, ref_pixels plane or ref_slot, pred_pixels given, nrefs outside [1, mc_refs] and a slot outside
    [0, nrefs); with ref_resident = 1 it refuses instead ref_pixels given, nrefs other than 0, a slot outside
    [0, mc_refs) and a slot that holds no picture.  With config.mc_next the same checks cover ref_slot_next, and a NULL

@@ -8,9 +8,12 @@ process, alternating the two configurations round by round, it measures:
     bench.py's e2e loop does) for (a) reconstruction + the classic symbol arrays and (b) reconstruction + the
     symbol stream;
   - the bytes copied device -> host per step in (a) and (b).
+With --haar-dc both configurations quantise the keyframe DCs (haar_dc_quant = 1): (a) returns the classic arrays and
+the DC index grids, (b) the stream with its keyframe DC records (sym_hdc) and no grids; the device step of (b) also
+times the DC record kernel alone (k_sym_hdc, torch.profiler).
 Prints the GPU's name and power limit with the numbers, and one JSON line at the end.
 
-    python tools/bench_symbol_stream.py [--steps 10] [--rounds 3]
+    python tools/bench_symbol_stream.py [--steps 10] [--rounds 3] [--haar-dc]
 """
 import argparse
 import json
@@ -27,6 +30,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--haar-dc", action="store_true")
     args = ap.parse_args()
 
     import numpy as np
@@ -47,10 +51,10 @@ def main():
         eng = engine.KeyframeEngine(geom, nframes=F, q0=bench.Q0, use_masking=1, pvq_qm_q4=q4, dering=1,
                                     coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA,
                                     persist_ctas_per_sm=0, split_free=1, level_chains=0, noref_prepass=0,
-                                    max_blocks_div=2, symbol_stream=stream)
+                                    max_blocks_div=2, symbol_stream=stream, haar_dc_quant=int(args.haar_dc))
         eng.stage_inputs([np.stack([f[0][p] for f in hf]) for p in range(3)], np.stack([f[1] for f in hf]))
         eng.stage_dering_levels(np.stack([f[2] for f in hf]))
-        eng.prepare_io(symbols=not stream, recon=True, stream=bool(stream))
+        eng.prepare_io(symbols=not stream, recon=True, stream=bool(stream), dc_grids=not stream)
         return eng
 
     # (a): two engines without the stream, classic symbols; (b): two with the stream, no classic symbols
@@ -91,7 +95,7 @@ def main():
               % (r, dev["a"][-1], dev["b"][-1], rate["a"][-1], rate["b"][-1]), flush=True)
     bytes_a, bytes_b = d2h(cfg["a"][0]), d2h(cfg["b"][0])
     res = {
-        "gpu": gpu, "frames_per_step": F, "steps": args.steps, "rounds": args.rounds,
+        "gpu": gpu, "frames_per_step": F, "steps": args.steps, "rounds": args.rounds, "haar_dc_quant": int(args.haar_dc),
         "device_step_ms": {"symbol_stream_0": [round(v, 3) for v in dev["a"]],
                            "symbol_stream_1": [round(v, 3) for v in dev["b"]],
                            "stream_extra_ms_median": round(statistics.median(dev["b"]) - statistics.median(dev["a"]), 3)},
@@ -107,10 +111,25 @@ def main():
     nk = int((lb["luma_res"][..., 3] > 0).sum() + (lb["chroma_res"][..., 3] > 0).sum())
     res["stream_per_step"] = {"blocks": int(idx[:, 1].sum()), "bands": int(idx[:, 3].sum()),
                               "pulse_bytes": int(idx[:, 5].sum()), "bands_with_k_gt_0": nk}
+    if args.haar_dc:
+        res["stream_per_step"]["hdc_records"] = int(idx[:, 1].sum())
+        res["k_sym_hdc_us"] = kernel_us(cfg["b"][0], "k_sym_hdc")
     print(json.dumps(res), flush=True)
     for engs in cfg.values():
         for e in engs:
             e.close()
+
+
+def kernel_us(eng, name, reps=5):
+    """Mean device time of the kernels whose name contains `name` over `reps` graph replays (torch.profiler)."""
+    from torch.profiler import ProfilerActivity, profile
+    from daala_b200 import engine
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            eng.run_device(engine.PH_ALL, True)
+        eng.wait()
+    us = [e.device_time_total for e in prof.key_averages() if name in e.key]
+    return round(sum(us) / reps, 2) if us else None
 
 
 if __name__ == "__main__":
