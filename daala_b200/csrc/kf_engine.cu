@@ -37,7 +37,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <mutex>
 #include <new>
 #include <vector>
 
@@ -77,13 +76,13 @@ enum Cnt {
   kDoneHi = 160,     // band-0 items finished (flushed by warps when they go idle)
   kHeadCh = 192,     // ticket of the row / column chain heads
   kWaiters = 224,    // warps parked on a future band-0 slot
-  kTraceN = 240,     // DAALA_B200_CHAIN_TRACE: records written by k_pvq_persist<true>
+  kTraceN = 240,     // DAALA_B200_CHAIN_TRACE: records written by k_pvq_persist
   kCntWords = 256
 };
 
 constexpr int kTile = 1024;        // units per scan tile
-constexpr int kMaxLevels = 4096;   // (plane width + height) / 4 of an 8K frame is 3008
-constexpr int kLevelBins = kMaxLevels * 3;
+// weight bins of the chain heads (weight_bin); the count sets how finely k_chroma_items orders the heads
+constexpr int kHeadBins = 12288;
 
 struct Lists {
   const uint8_t* bsize;            // [F][UH][bstride]
@@ -111,15 +110,9 @@ struct Lists {
   // counts the bins and its last CTA scans them, k_chroma_items scatters the heads into `heads`
   uint32_t* heads_raw;
   int32_t* head_bin;
-  int32_t* head_hist;              // [kLevelBins] counts, then exclusive offsets
-  int32_t* head_cursor;            // [kLevelBins]
+  int32_t* head_hist;              // [kHeadBins] counts, then exclusive offsets
+  int32_t* head_cursor;            // [kHeadBins]
   int32_t* cnt;                    // [kCntWords]
-  // level path: chain items counting-sorted by dependency level (position along the chain in units of the
-  // block size; larger bands first inside a level)
-  int32_t* lvl_hist;               // [kLevelBins] counts, then exclusive offsets
-  int32_t* lvl_cursor;             // [kLevelBins]
-  uint32_t* lvl_items;             // sorted chain items
-  int nlevels;
   int max_luma, max_chroma;        // capacities (blocks)
 };
 
@@ -265,16 +258,6 @@ __global__ void __launch_bounds__(kTile) k_unit_emit(const __grid_constant__ Lis
 
 __device__ __forceinline__ int band_class(int band) { return band < 3 ? 0 : band < 6 ? 1 : 2; }
 
-// Dependency level of a chain item: its position along the chain in units of its own block size (band 0:
-// the anti-diagonal).  Items only depend on same-size neighbours, whose level is smaller by one; bin =
-// level * 3 + (2 - class) so that the 128-coefficient bands of a level come first.
-__device__ __forceinline__ int level_bin(int band, int bs, int x0, int y0, int y_first) {
-  const int sh = bs + 2, bx = x0 >> sh, by = (y0 - y_first) >> sh;
-  const int r = band % 3;
-  const int lvl = band == 0 ? bx + by : r == 1 ? by : bx;
-  return lvl * 3 + (2 - band_class(band));
-}
-
 // warp-aggregated append of `v` to list[*counter] by the lanes with `pred`; the index written, or -1
 __device__ __forceinline__ int append(uint32_t* list, int32_t* counter, bool pred, uint32_t v) {
   const unsigned m = __ballot_sync(__activemask(), pred);
@@ -298,14 +281,14 @@ __device__ __forceinline__ int count_key(int32_t* ctr, int key) {
 }
 
 // Cost of one chain item per band class (n <= 16, 32, 128 coefficients) in units of 10 us: the mean duration of an
-// item of the class in k_pvq_persist<intra> while every warp is busy, 73 / 89 / 178 us on bench.py's workload (one
+// item of the class in k_pvq_persist while every warp is busy, 73 / 89 / 178 us on bench.py's workload (one
 // H100 80GB HBM3 at 700 W, tools/chain_timeline.py, DESIGN.md section 5).  A chain's weight is its length in blocks
 // times this; the bin of the weight orders the chain heads.
 constexpr int kChainCost0 = 7, kChainCost1 = 9, kChainCost2 = 18;
 __device__ __forceinline__ int weight_bin(int len, int band) {
   const int c = band_class(band);
   const int w = len * (c == 0 ? kChainCost0 : c == 1 ? kChainCost1 : kChainCost2);
-  return kLevelBins - 1 - min(w, kLevelBins - 1);   // heaviest first
+  return kHeadBins - 1 - min(w, kHeadBins - 1);   // heaviest first
 }
 
 // Length in blocks of the column (down) or row chain that starts at the block (x0, y0, bs) of `map`: its
@@ -322,12 +305,12 @@ __device__ int chain_length(const Lists& L, const uint8_t* map, int x0, int y0, 
   return len;
 }
 
-// One CTA of kThreads: exclusive scan of kLevelBins counts in place (+ a copy as scatter cursors).  The counts are
+// One CTA of kThreads: exclusive scan of kHeadBins counts in place (+ a copy as scatter cursors).  The counts are
 // read past L1: the last CTA of k_luma_deps scans what the other CTAs of that launch counted.
 template <int kThreads>
 __device__ __forceinline__ void scan_bins(int32_t* hist, int32_t* cursor) {
   __shared__ int part[kThreads];
-  constexpr int kPer = kLevelBins / kThreads;
+  constexpr int kPer = kHeadBins / kThreads;
   const int t = threadIdx.x;
   int v[kPer], sum = 0;
 #pragma unroll
@@ -414,10 +397,6 @@ __global__ void __launch_bounds__(256) k_luma_deps(const __grid_constant__ Lists
         }
       }
       chain += has && !is_free;
-      if (has && !is_free && L.lvl_hist) {
-        const daala_b200_pvq_block b = L.luma[blk];
-        atomicAdd(&L.lvl_hist[level_bin(band, bs, b.x0, b.y0, L.u_row0 * 8)], 1);
-      }
     }
     // total number of chain items
 #pragma unroll
@@ -433,24 +412,6 @@ __global__ void __launch_bounds__(256) k_luma_deps(const __grid_constant__ Lists
   if (last) {
     __threadfence();
     scan_bins<256>(L.head_hist, L.head_cursor);
-  }
-}
-
-// One CTA: exclusive scan of the level bins in place (+ a copy as scatter cursors).
-__global__ void __launch_bounds__(1024) k_level_scan(const __grid_constant__ Lists L) {
-  scan_bins<1024>(L.lvl_hist, L.lvl_cursor);
-}
-
-__global__ void __launch_bounds__(256) k_level_scatter(const __grid_constant__ Lists L) {
-  const int n = min(L.cnt[kNLuma], L.max_luma);
-  for (int blk = blockIdx.x * blockDim.x + threadIdx.x; blk < n; blk += gridDim.x * blockDim.x) {
-    const daala_b200_pvq_block b = L.luma[blk];
-    const int nb = num_bands(b.bs);
-    for (int band = 0; band < nb; band++) {
-      if (band == 3 || band == 6) continue;
-      const int pos = atomicAdd(&L.lvl_cursor[level_bin(band, b.bs, b.x0, b.y0, L.u_row0 * 8)], 1);
-      L.lvl_items[pos] = ((uint32_t)blk << 4) | band;
-    }
   }
 }
 
@@ -518,17 +479,7 @@ struct Stage {
   int16_t* sp_snap[3];             // [slots][kMaxEvents][vstride]
   int sp_slots[3];                 // slots per chunk
   int sp_chunks[3];                // chunks that cover the list capacity of the class
-  // level path: chain items sorted by level; one record of context per position inside a level
-  const int32_t* lvl_off;          // [kLevelBins] exclusive offsets of the bins
-  const uint32_t* lvl_items;
-  int nlevels, lvl_slots;
-  int16_t* lv_vec; int32_t* lv_lanes; int32_t* lv_uni; int16_t* lv_snap;
-  int32_t* lv_bar;                 // grid barrier counter
-  // luma: the no-reference events of every chain band, searched ahead of the chains (k_pvq_prepass)
-  int32_t* pre_ev;                 // [coefs / 8][kPreEvWords], record of a band at (coef_off + band start) >> 3
-  int16_t* pre_snap;               // [2 * coefs]: the events' pulses at 2 * (coef_off + band start)
   int max_waiters;                 // warps that may park on future band-0 slots; the others exit when idle
-  int skip_lo;                     // the persistent kernel leaves the dependency-free lists to the split path
   const double* rsqrt_tbl;         // [kTableDoubles] the reference's 1/sqrt(i) and theta-rate terms (pvq_fill_rsqrt_table)
   int16_t* res_pack;               // [nblocks*9][4]: gain, itheta, max_theta, k (what the coder reads)
   // keyframe chroma: the CfL source, the luma stage's coding-order input (its DC) and output (the quantised
@@ -542,7 +493,7 @@ struct Stage {
   // (one load per item)
   const int32_t* fq_bq;
 #ifdef DAALA_B200_CHAIN_TRACE
-  struct ChainTraceRec* trace;     // luma: one record per item k_pvq_persist<true> runs, up to trace_cap
+  struct ChainTraceRec* trace;     // luma: one record per item k_pvq_persist runs, up to trace_cap
   int trace_cap;
 #endif
 };
@@ -711,39 +662,35 @@ __device__ __forceinline__ void push_chain(const Stage& S, int blk, int band) {
   st_release((int*)&S.ring[pos], (int)(((uint32_t)blk << 4) | band));
 }
 
-// Next item for an idle warp (uniform), or kNoItem when the stage has nothing left for it.
-//  chroma (kIntra = false): a ticket into the item lists, largest bands first.
-//  luma, in this order: (1) a filled slot of the band-0 queue -- band 0 is a 2-D wavefront over each
+// Next item for an idle warp of the luma stage (uniform), or kNoItem when the stage has nothing left for it.
+// In this order: (1) a filled slot of the band-0 queue -- band 0 is a 2-D wavefront over each
 //  same-size region, the deepest dependency structure of a frame, so it goes first; (2) the head of a row
 //  or column chain; (3) a dependency-free item; (4) a ticket for a FUTURE band-0 slot, waited for on the
 //  slot itself (distinct addresses: no hot spot).  `done` = band-0 items this warp finished since it was
 //  last here; the warp whose flush completes the count releases every waiter with kExit.
-template <bool kIntra>
 __device__ __forceinline__ uint32_t next_item(const Stage& S, int lane, int* done, bool* waiter) {
   int slot = -1, head = -1, lo = -1, nheads0 = 0, fin = -1;
   if (lane == 0) {
     const int n2 = S.cnt[S.n_items_at + 2], n1 = S.cnt[S.n_items_at + 1], n0 = S.cnt[S.n_items_at];
-    const int nlo = S.skip_lo ? 0 : n0 + n1 + n2;
-    if (kIntra) {
-      nheads0 = S.cnt[kNHeads0];
-      if (*done) {
-        const int d = atomicAdd(&S.cnt[kDoneHi], *done) + *done;
-        if (d == S.cnt[kNLuma]) {   // every luma block has a band 0
-          __threadfence();
-          fin = ld_relaxed(&S.cnt[kTailHi]) - nheads0;   // final: every push happened before its item finished
-        }
+    const int nlo = n0 + n1 + n2;
+    nheads0 = S.cnt[kNHeads0];
+    if (*done) {
+      const int d = atomicAdd(&S.cnt[kDoneHi], *done) + *done;
+      if (d == S.cnt[kNLuma]) {   // every luma block has a band 0
+        __threadfence();
+        fin = ld_relaxed(&S.cnt[kTailHi]) - nheads0;   // final: every push happened before its item finished
       }
-      if (ld_relaxed(&S.cnt[kHeadHi]) < ld_relaxed(&S.cnt[kTailHi])) slot = atomicAdd(&S.cnt[kHeadHi], 1);
-      if (slot < 0 && ld_relaxed(&S.cnt[kHeadCh]) < S.cnt[kNHeads]) {
-        const int h = atomicAdd(&S.cnt[kHeadCh], 1);
-        if (h < S.cnt[kNHeads]) head = h;
-      }
+    }
+    if (ld_relaxed(&S.cnt[kHeadHi]) < ld_relaxed(&S.cnt[kTailHi])) slot = atomicAdd(&S.cnt[kHeadHi], 1);
+    if (slot < 0 && ld_relaxed(&S.cnt[kHeadCh]) < S.cnt[kNHeads]) {
+      const int h = atomicAdd(&S.cnt[kHeadCh], 1);
+      if (h < S.cnt[kNHeads]) head = h;
     }
     if (slot < 0 && head < 0 && ld_relaxed(&S.cnt[S.head_lo_at]) < nlo) {
       const int l = atomicAdd(&S.cnt[S.head_lo_at], 1);
       if (l < nlo) lo = l;
     }
-    if (kIntra && slot < 0 && head < 0 && lo < 0) {
+    if (slot < 0 && head < 0 && lo < 0) {
       // nothing to do right now: park on the next band-0 slot -- unless enough warps already do; the rest
       // leave and free their SM resources for whatever kernel comes next (another engine's batch)
       if (!*waiter && atomicAdd(&S.cnt[kWaiters], 1) < S.max_waiters) *waiter = true;
@@ -751,17 +698,15 @@ __device__ __forceinline__ uint32_t next_item(const Stage& S, int lane, int* don
     }
   }
   *done = 0;
-  if (kIntra) {
-    fin = __shfl_sync(0xffffffffu, fin, 0);
-    if (fin >= 0) {
-      // every warp holds at most one ticket: slots [fin, fin + #warps] cover all of them, now and later
-      const int nw = (gridDim.x * blockDim.x) >> 5;
+  fin = __shfl_sync(0xffffffffu, fin, 0);
+  if (fin >= 0) {
+    // every warp holds at most one ticket: slots [fin, fin + #warps] cover all of them, now and later
+    const int nw = (gridDim.x * blockDim.x) >> 5;
 #pragma unroll 1
-      for (int i = lane; i <= nw; i += 32) st_release((int*)&S.ring[fin + i], (int)kExit);
-    }
-    head = __shfl_sync(0xffffffffu, head, 0);
-    if (head >= 0) return S.heads[head];
+    for (int i = lane; i <= nw; i += 32) st_release((int*)&S.ring[fin + i], (int)kExit);
   }
+  head = __shfl_sync(0xffffffffu, head, 0);
+  if (head >= 0) return S.heads[head];
   slot = __shfl_sync(0xffffffffu, slot, 0);
   lo = __shfl_sync(0xffffffffu, lo, 0);
   if (slot >= 0) {
@@ -815,9 +760,8 @@ __device__ __forceinline__ void intra_band_ref(const Stage& S, int blk, int band
   }
 }
 
-// One (block, band) item by one warp.  kIntra: the band's prediction is built from the quantised
-// neighbours first (od_hv_intra_pred, src/intra.c:37-62).  The band quantiser is the block's frame's entry of S.fq_bq.
-template <bool kIntra>
+// One luma (block, band) item by one warp: the band's prediction is built from the quantised neighbours first
+// (od_hv_intra_pred, src/intra.c:37-62).  The band quantiser is the block's frame's entry of S.fq_bq.
 __device__ __forceinline__ void run_item(const Stage& S, uint32_t item, int lane, int16_t* snap) {
   const daala_b200_pvq_params& prm = S.prm;
   const int blk = (int)(item >> 4), band = (int)(item & 15);
@@ -826,19 +770,16 @@ __device__ __forceinline__ void run_item(const Stage& S, uint32_t item, int lane
   const int start = band_start(band);
   const int bn = band_start(band + 1) - start;
   const size_t off = (size_t)b.coef_off + start;
-  if (kIntra) intra_band_ref(S, blk, band, b.coef_off, lane);
+  intra_band_ref(S, blk, band, b.coef_off, lane);
   const int qidx = bs * (bs + 1) + (band + 1) - (band + 1) / 3;
   const int q = S.fq_bq[(b.frame * 3 + pli) * 32 + qidx];
   const int beta = (prm.use_masking && pli == 0 && bs > 0) ? kBeta15 : kBeta1;
   const int qoff = (b.xdec & 1 ? prm.qm_stride : 0) + ((((1 << (2 * bs)) - 1) << 4) / 3) + start;
   int itheta, max_theta, k;
   double skip_term;
-  const bool pre = kIntra && S.pre_ev && band != 3 && band != 6;
-  const int32_t* pev = pre ? S.pre_ev + (off >> 3) * kPreEvWords : nullptr;
-  const int16_t* psn = pre ? S.pre_snap + 2 * off : nullptr;
   const int gain = quantise_band_warp<0>(lane, snap, S.rsqrt_tbl, prm.out + off, prm.in + off, prm.ref + off, bn, q,
                                          prm.y + off, &itheta, &max_theta, &k, beta, &skip_term, prm.is_keyframe, pli,
-                                         prm.qm + qoff, prm.qm_inv + qoff, prm.pvq_norm_lambda, pev, psn);
+                                         prm.qm + qoff, prm.qm_inv + qoff, prm.pvq_norm_lambda);
   if (lane == 0) {
     const size_t r = (size_t)blk * 9 + band;
     prm.res_skip_term[r] = skip_term;
@@ -855,7 +796,7 @@ __device__ __forceinline__ void run_item(const Stage& S, uint32_t item, int lane
 // instruction cache; the persistent kernel spends most of its issue slots waiting for instruction fetch
 // (no_instruction is the first stall reason).  One phase at a
 // time on the whole GPU keeps the resident code small.  Only items without dependencies can go this way
-// (chroma; luma bands 3 / 6); the intra chains stay in the persistent kernel.
+// (keyframe chroma, every band of an inter frame); keyframe luma stays in the persistent kernel.
 struct ItemGeom {
   int blk, band, bn, q, beta, pli, qoff;
   size_t off;
@@ -879,8 +820,7 @@ __device__ __forceinline__ ItemGeom item_geom(const Stage& S, uint32_t item) {
 }
 
 // kPhase 0 / 1 / 2 = setup / search / finish of the items [chunk * slots, ...) of class `cls`.
-// kZeroRef: the prediction is all zero (luma bands 3 / 6).
-template <int kPhase, bool kZeroRef, int kMode>
+template <int kPhase, int kMode>
 __global__ void __launch_bounds__(128) k_pvq_split(const __grid_constant__ Stage S, int cls, int chunk) {
   const daala_b200_pvq_params& prm = S.prm;
   const int lane = threadIdx.x & 31;
@@ -895,7 +835,7 @@ __global__ void __launch_bounds__(128) k_pvq_split(const __grid_constant__ Stage
     int32_t* lanes = S.sp_lanes[cls] + (size_t)i * kCtxLaneWords * 16;
     int32_t* uni = S.sp_uni[cls] + (size_t)i * kCtxUniWords;
     int16_t* snap = S.sp_snap[cls] + (size_t)i * kMaxEvents * vs;
-    const int32_t* r0 = kZeroRef ? nullptr : prm.ref + g.off;
+    const int32_t* r0 = prm.ref + g.off;
     BandCtx B;
     if (kPhase == 0) {
       band_setup<kMode>(lane, B, prm.in + g.off, r0, g.bn, g.q, g.beta, prm.is_keyframe, g.pli, prm.qm + g.qoff,
@@ -922,111 +862,11 @@ __global__ void __launch_bounds__(128) k_pvq_split(const __grid_constant__ Stage
   }
 }
 
-// ---- prepass ---------------------------------------------------------------------------------------------
-// Keyframe luma always evaluates the no-reference candidates of pvq_theta (src/pvq_encoder.c:573-606), and
-// they depend on the input vector alone: their searches (two from scratch per band, the larger half of a
-// chain band's work) run here for every chain band at once, fully parallel, and the chain walk imports the
-// results (band_noref_export / band_search's pre_ev) -- that work leaves the dependency-bound kernel.
-template <int kMode>
-__global__ void __launch_bounds__(128) k_pvq_prepass(const __grid_constant__ Stage S) {
-  const daala_b200_pvq_params& prm = S.prm;
-  __shared__ int16_t snap_all[4][2 * kMaxN];
-  const int lane = threadIdx.x & 31;
-  int16_t* snap = snap_all[threadIdx.x >> 5];
-  const int nblk = min(S.cnt[S.n_blocks_at], S.max_blocks);
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  // kMode 1: bands 0, 1, 2, 4, 5 (n <= 32); kMode 2: bands 7, 8 (n = 128)
-  const int per = kMode == 2 ? 2 : 5;
-  for (long long i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < (long long)nblk * per; i += nwarps) {
-    const int blk = (int)(i / per), sel = (int)(i % per);
-    const int band = kMode == 2 ? 7 + sel : (sel < 3 ? sel : sel + 1);
-    if (band >= num_bands(prm.blocks[blk].bs)) continue;
-    const ItemGeom g = item_geom(S, ((uint32_t)blk << 4) | band);
-    BandCtx B;
-    band_setup<kMode>(lane, B, prm.in + g.off, nullptr, g.bn, g.q, g.beta, prm.is_keyframe, g.pli, prm.qm + g.qoff,
-                      prm.pvq_norm_lambda, S.rsqrt_tbl);
-    band_search<kMode>(lane, B, g.bn, snap, kMaxN, S.rsqrt_tbl);
-    band_noref_export(lane, B, g.bn, snap, kMaxN, S.pre_ev + (g.off >> 3) * kPreEvWords, S.pre_snap + 2 * g.off);
-  }
-}
-
-// ---- level path -----------------------------------------------------------------------------------------
-// The luma intra chains, level-synchronously: all chain items of one dependency level are independent, so
-// the whole GPU runs phase A (prediction from the neighbours + band_setup) for the level, then phase B
-// (searches), then phase C (costs, fold, synthesis), with a grid-wide barrier in between -- at any time
-// only one phase's code is being executed anywhere (see "split path" above for why that matters), and
-// nobody ever waits on a flag.  One persistent launch, all CTAs resident (the host sizes the grid).
-__device__ __forceinline__ void grid_barrier(int32_t* bar, int* target, int nctas) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    *target += nctas;
-    __threadfence();
-    atomicAdd(bar, 1);
-    while (ld_acquire(bar) < *target) {}
-  }
-  __syncthreads();
-}
-
-__global__ void __launch_bounds__(128, 4) k_pvq_levels(const __grid_constant__ Stage S) {
-  const daala_b200_pvq_params& prm = S.prm;
-  __shared__ int bar_target;
-  if (threadIdx.x == 0) bar_target = 0;
-  const int lane = threadIdx.x & 31;
-  const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  const int total = S.cnt[kTotalHi];
-  constexpr int vs = 128;
-  for (int lvl = 0; lvl < S.nlevels; lvl++) {
-    const int base = S.lvl_off[lvl * 3];
-    const int end = lvl + 1 < kMaxLevels ? S.lvl_off[(lvl + 1) * 3] : total;
-    if (end - base > S.lvl_slots && threadIdx.x == 0 && blockIdx.x == 0) S.cnt[kError] = 2;
-    const int n = min(end - base, S.lvl_slots);
-    if (n <= 0) continue;   // uniform: every CTA reads the same offsets
-    for (int phase = 0; phase < 3; phase++) {
-      for (int i = w; i < n; i += nwarps) {
-        const uint32_t item = S.lvl_items[base + i];
-        const ItemGeom g = item_geom(S, item);
-        int16_t* vec = S.lv_vec + (size_t)i * 3 * vs;
-        int32_t* lanes = S.lv_lanes + (size_t)i * kCtxLaneWords * 16;
-        int32_t* uni = S.lv_uni + (size_t)i * kCtxUniWords;
-        int16_t* snap = S.lv_snap + (size_t)i * kMaxEvents * vs;
-        BandCtx B;
-        if (phase == 0) {
-          intra_band_ref(S, g.blk, g.band, (int)(g.off - band_start(g.band)), lane);
-          band_setup<0>(lane, B, prm.in + g.off, prm.ref + g.off, g.bn, g.q, g.beta, prm.is_keyframe, g.pli,
-                        prm.qm + g.qoff, prm.pvq_norm_lambda, S.rsqrt_tbl);
-          band_ctx_store_setup(lane, B, g.bn, vec, vs, lanes, uni);
-        } else if (phase == 1) {
-          band_ctx_load_search(lane, B, g.bn, vec, vs, lanes);
-          band_search<0>(lane, B, g.bn, snap, vs, S.rsqrt_tbl);
-          band_ctx_store_search(lane, B, lanes);
-        } else {
-          band_ctx_load_finish(lane, B, g.bn, vec, vs, lanes, uni);
-          int itheta, max_theta, k;
-          double skip_term;
-          const int gain = band_finish<0>(lane, B, snap, vs, prm.out + g.off, prm.ref + g.off, g.bn, g.q, prm.y + g.off,
-                                          &itheta, &max_theta, &k, g.beta, &skip_term, prm.is_keyframe, g.pli,
-                                          prm.qm_inv + g.qoff, prm.pvq_norm_lambda);
-          if (lane == 0) {
-            const size_t r = (size_t)g.blk * 9 + g.band;
-            prm.res_skip_term[r] = skip_term;
-            short4 pk;
-            pk.x = (short)gain; pk.y = (short)itheta; pk.z = (short)max_theta; pk.w = (short)k;
-            reinterpret_cast<short4*>(S.res_pack)[r] = pk;
-          }
-        }
-      }
-      grid_barrier(S.lv_bar, &bar_target, gridDim.x);
-    }
-  }
-}
-
-// Persistent PVQ kernel: one warp = one band at a time.  Luma (kIntra): the chain items of the H/V
+// Persistent PVQ kernel of the keyframe luma stage: one warp = one band at a time.  The chain items of the H/V
 // intra predictor form a dependency graph (per size class: band 0 a 2-D wavefront, bands 1/4/7 columns,
 // bands 2/5/8 rows).  A warp that finishes a chain item CONTINUES with a successor it made ready -- a
 // column or row is walked by one warp without touching the queue -- and pushes a second ready
 // successor (band 0 forks) into the chain queue.
-template <bool kIntra>
 __global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(const __grid_constant__ Stage S) {
   // per warp: the pulses of every search event of a band and the band's parked context (quantise_band_warp)
   __shared__ __align__(16) int16_t snap_all[kPersistThreads / 32][kSnapEntries];
@@ -1035,7 +875,7 @@ __global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(c
   int done = 0;
   bool waiter = false;
   for (;;) {
-    uint32_t item = next_item<kIntra>(S, lane, &done, &waiter);
+    uint32_t item = next_item(S, lane, &done, &waiter);
     if (item == kNoItem) return;
 #ifdef DAALA_B200_CHAIN_TRACE
     int kind = (item & 15) == 0 ? 0 : (item & 15) == 3 || (item & 15) == 6 ? 2 : 1;
@@ -1045,12 +885,12 @@ __global__ void __launch_bounds__(kPersistThreads, kPersistCtas) k_pvq_persist(c
 #ifdef DAALA_B200_CHAIN_TRACE
       const unsigned long long t0 = globaltimer();
 #endif
-      run_item<kIntra>(S, item, lane, snap);
+      run_item(S, item, lane, snap);
 #ifdef DAALA_B200_CHAIN_TRACE
-      if (kIntra) trace_item(S, item, kind, t0, lane);
+      trace_item(S, item, kind, t0, lane);
       kind = 3;
 #endif
-      if (!kIntra || band == 3 || band == 6) break;
+      if (band == 3 || band == 6) break;
       done += band == 0;
       // results of this item -> visible to whoever runs a successor (this warp included: other lanes)
       __threadfence();
@@ -1786,12 +1626,6 @@ struct daala_b200_kf {
   int32_t* sp_uni[3];
   int16_t* sp_snap[3];
   int sp_slots[3];
-  int16_t* lv_vec;
-  int32_t* lv_lanes;
-  int32_t* lv_uni;
-  int16_t* lv_snap;
-  int32_t* lv_bar;
-  int lvl_slots, lvl_grid;
   Dering dering;                   // cfg.dering or cfg.inter_finish
   Lists lists;
   Stage luma, chroma;
@@ -2074,7 +1908,7 @@ static int kf_alloc(daala_b200_kf* kf) {
     KF_CHECK(dalloc(kf, &L.items_l[c], cap_l[c]));
     KF_CHECK(dalloc(kf, &L.items_c[c], cap_c[c]));
   }
-  if (kf->cfg.split_free > 0 || inter) {
+  {
     // context records of one chunk of items per class (pvq_warp.cuh: band_ctx_*)
     const int slots[3] = {1 << 19, 1 << 19, 3 << 15};
     for (int c = 0; c < 3; c++) {
@@ -2086,45 +1920,24 @@ static int kf_alloc(daala_b200_kf* kf) {
       KF_CHECK(dalloc(kf, &kf->sp_snap[c], (size_t)slots[c] * kMaxEvents * vs));
     }
   }
-  if (kf->cfg.level_chains) {
-    KF_CHECK(dalloc(kf, &L.lvl_hist, (size_t)kLevelBins));
-    KF_CHECK(dalloc(kf, &L.lvl_cursor, (size_t)kLevelBins));
-    KF_CHECK(dalloc(kf, &L.lvl_items, kf->chain_cap));
-    L.nlevels = (kf->plane_w[0] + L.u_rows * 8) / 4 + 2;
-    if (L.nlevels >= kMaxLevels) return (int)cudaErrorInvalidValue;
-    kf->lvl_slots = 2048 * F;
-    KF_CHECK(dalloc(kf, &kf->lv_vec, (size_t)kf->lvl_slots * 3 * 128));
-    KF_CHECK(dalloc(kf, &kf->lv_lanes, (size_t)kf->lvl_slots * kCtxLaneWords * 16));
-    KF_CHECK(dalloc(kf, &kf->lv_uni, (size_t)kf->lvl_slots * kCtxUniWords));
-    KF_CHECK(dalloc(kf, &kf->lv_snap, (size_t)kf->lvl_slots * kMaxEvents * 128));
-    KF_CHECK(dalloc(kf, &kf->lv_bar, (size_t)32));
-    int per_sm = 0;
-    KF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pvq_levels, 128, 0));
-    if (per_sm < 1) return (int)cudaErrorLaunchOutOfResources;
-    kf->lvl_grid = per_sm * kf->sms;   // all CTAs resident: the kernel synchronises the whole grid
-  }
   {
     // the persistent grid is sized to be resident at once: 32 one-warp CTAs with kSnapEntries of shared
     // scratch each (plus the 1 KB the SM reserves per CTA) need 223 of the SM's 228 KB
     const int want = kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas;
-    int per_sm[2] = {0, 0};
-    KF_CHECK(cudaFuncSetAttribute(k_pvq_persist<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
+    int per_sm = 0;
+    KF_CHECK(cudaFuncSetAttribute(k_pvq_persist, cudaFuncAttributePreferredSharedMemoryCarveout,
                                   cudaSharedmemCarveoutMaxShared));
-    KF_CHECK(cudaFuncSetAttribute(k_pvq_persist<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                  cudaSharedmemCarveoutMaxShared));
-    KF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[0], k_pvq_persist<true>, kPersistThreads, 0));
-    KF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[1], k_pvq_persist<false>, kPersistThreads, 0));
-    if (per_sm[0] < want || per_sm[1] < want) {
-      snprintf(kf->err, sizeof(kf->err), "k_pvq_persist: %d / %d CTAs per SM resident, %d wanted", per_sm[0],
-               per_sm[1], want);
+    KF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pvq_persist, kPersistThreads, 0));
+    if (per_sm < want) {
+      snprintf(kf->err, sizeof(kf->err), "k_pvq_persist: %d CTAs per SM resident, %d wanted", per_sm, want);
       return (int)cudaErrorLaunchOutOfResources;
     }
   }
   KF_CHECK(dalloc(kf, &L.heads, inter ? 0 : kf->chain_cap));
   KF_CHECK(dalloc(kf, &L.heads_raw, inter ? 0 : kf->chain_cap));
   KF_CHECK(dalloc(kf, &L.head_bin, inter ? 0 : kf->chain_cap));
-  KF_CHECK(dalloc(kf, &L.head_hist, inter ? 0 : (size_t)kLevelBins));
-  KF_CHECK(dalloc(kf, &L.head_cursor, inter ? 0 : (size_t)kLevelBins));
+  KF_CHECK(dalloc(kf, &L.head_hist, inter ? 0 : (size_t)kHeadBins));
+  KF_CHECK(dalloc(kf, &L.head_cursor, inter ? 0 : (size_t)kHeadBins));
   KF_CHECK(dalloc(kf, &L.heads0, ndep));
   KF_CHECK(dalloc(kf, &L.cnt, (size_t)kCntWords));
   kf->mc.bad_ref = L.cnt + kMcBadRef;
@@ -2173,23 +1986,7 @@ static int kf_alloc(daala_b200_kf* kf) {
       const size_t cap = chroma ? cap_c[c] : cap_l[c];
       S.sp_chunks[c] = kf->sp_slots[c] > 0 ? (int)((cap + kf->sp_slots[c] - 1) / kf->sp_slots[c]) : 0;
     }
-    S.skip_lo = chroma ? 0 : kf->cfg.split_free > 1;
-    S.max_waiters = getenv("DAALA_B200_MAX_WAITERS") ? atoi(getenv("DAALA_B200_MAX_WAITERS")) : kf->sms * 8;
-    if (!chroma && kf->cfg.noref_prepass) {
-      KF_CHECK(dalloc(kf, &S.pre_ev, (ncoef / 8 + 2) * kPreEvWords));
-      KF_CHECK(dalloc(kf, &S.pre_snap, 2 * ncoef));
-    }
-    if (!chroma) {
-      S.lvl_off = L.lvl_hist;
-      S.lvl_items = L.lvl_items;
-      S.nlevels = L.nlevels;
-      S.lvl_slots = kf->lvl_slots;
-      S.lv_vec = kf->lv_vec;
-      S.lv_lanes = kf->lv_lanes;
-      S.lv_uni = kf->lv_uni;
-      S.lv_snap = kf->lv_snap;
-      S.lv_bar = kf->lv_bar;
-    }
+    S.max_waiters = kf->sms * 8;
     S.n_items_at = chroma ? kNItemsC : kNItemsL;
     S.head_lo_at = chroma ? kHeadLoC : kHeadLoL;
     S.n_blocks_at = chroma ? kNChroma : kNLuma;
@@ -2581,19 +2378,18 @@ static int dering_launches(const Dering& D, int parts) {
 
 // Everything between "inputs are in HBM" and "results are in HBM", on kf->stream.
 // the three phase kernels over every chunk of every class of a stage's dependency-free lists
-template <bool kZeroRef>
 static void enqueue_split(daala_b200_kf* kf, const Stage& S, cudaStream_t s) {
   const int grid = kf->sms * 16;
   for (int cls = 2; cls >= 0; cls--) {
     for (int chunk = 0; chunk < S.sp_chunks[cls]; chunk++) {
       if (cls == 2) {
-        k_pvq_split<0, kZeroRef, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
-        k_pvq_split<1, kZeroRef, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
-        k_pvq_split<2, kZeroRef, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<0, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<1, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<2, 2><<<grid, 128, 0, s>>>(S, cls, chunk);
       } else {
-        k_pvq_split<0, kZeroRef, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
-        k_pvq_split<1, kZeroRef, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
-        k_pvq_split<2, kZeroRef, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<0, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<1, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
+        k_pvq_split<2, 1><<<grid, 128, 0, s>>>(S, cls, chunk);
       }
     }
   }
@@ -2650,7 +2446,7 @@ static int kf_enqueue_step_inter(daala_b200_kf* kf, int phases) {
   for (const Stage* S : {&kf->luma, &kf->chroma}) {
     if (!(phases & (S == &kf->luma ? DAALA_B200_KF_PVQ_LUMA : DAALA_B200_KF_PVQ_CHROMA))) continue;
     if (!core) k_gather<kGatherInter><<<wide, 256, 0, s>>>(*S);
-    enqueue_split<false>(kf, *S, s);
+    enqueue_split(kf, *S, s);
     if (!core) k_finish_scatter<true><<<wide, 256, 0, s>>>(*S);
   }
   if (!core && (phases & DAALA_B200_KF_PVQ_CHROMA) && kf->cfg.late_skip) {
@@ -2675,18 +2471,13 @@ static int enqueue_lists(daala_b200_kf* kf, cudaStream_t s) {
   const size_t nl = (size_t)L.max_luma * sizeof(int32_t);
   if (cudaMemsetAsync(L.succ_bottom, 0xff, nl, s) != cudaSuccess || cudaMemsetAsync(L.succ_right, 0xff, nl, s) != cudaSuccess)
     return (int)cudaGetLastError();
-  if (L.lvl_hist && cudaMemsetAsync(L.lvl_hist, 0, sizeof(int32_t) * kLevelBins, s) != cudaSuccess) return (int)cudaGetLastError();
-  if (cudaMemsetAsync(L.head_hist, 0, sizeof(int32_t) * kLevelBins, s) != cudaSuccess) return (int)cudaGetLastError();
+  if (cudaMemsetAsync(L.head_hist, 0, sizeof(int32_t) * kHeadBins, s) != cudaSuccess) return (int)cudaGetLastError();
   k_luma_deps<<<wide, 256, 0, s>>>(L);
-  if (L.lvl_hist) {
-    k_level_scan<<<1, 1024, 0, s>>>(L);
-    k_level_scatter<<<wide, 256, 0, s>>>(L);
-  }
   k_chroma_items<<<wide, 256, 0, s>>>(L);
   return 0;
 }
 
-// The luma PVQ stage up to its last band: the tickets of the stages in `begin`, gather, [luma split bands, prepass], the chain kernel.  `core`
+// The luma PVQ stage up to its last band: the tickets of the stages in `begin`, gather, the chain kernel.  `core`
 // (_SEARCH_ONLY, measurement): just the search kernels, on the coding-order buffers a previous full pass left behind
 // (same inputs, same results).
 static int enqueue_luma_bands(daala_b200_kf* kf, bool core, int begin, cudaStream_t s) {
@@ -2697,17 +2488,7 @@ static int enqueue_luma_bands(daala_b200_kf* kf, bool core, int begin, cudaStrea
     return (int)cudaGetLastError();
   k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, begin);
   if (!core) k_gather<kGatherLuma><<<wide, 256, 0, s>>>(kf->luma);
-  if (kf->cfg.split_free > 1) enqueue_split<true>(kf, kf->luma, s);
-  if (kf->luma.pre_ev) {
-    k_pvq_prepass<2><<<kf->sms * 16, 128, 0, s>>>(kf->luma);
-    k_pvq_prepass<1><<<kf->sms * 16, 128, 0, s>>>(kf->luma);
-  }
-  if (kf->cfg.level_chains) {
-    if (cudaMemsetAsync(kf->lv_bar, 0, sizeof(int32_t) * 32, s) != cudaSuccess) return (int)cudaGetLastError();
-    k_pvq_levels<<<kf->lvl_grid, 128, 0, s>>>(kf->luma);
-  } else {
-    k_pvq_persist<true><<<persist, kPersistThreads, 0, s>>>(kf->luma);
-  }
+  k_pvq_persist<<<persist, kPersistThreads, 0, s>>>(kf->luma);
   return 0;
 }
 
@@ -2719,9 +2500,7 @@ static void enqueue_chroma(daala_b200_kf* kf, bool core, bool begin, cudaStream_
   if (begin) k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, kBeginChroma);
   if (!core && hdc) k_gather<kGatherChroma, true><<<wide, 256, 0, s>>>(kf->chroma);
   else if (!core) k_gather<kGatherChroma><<<wide, 256, 0, s>>>(kf->chroma);
-  const int persist = kf->sms * (kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas);
-  if (kf->cfg.split_free > 0) enqueue_split<false>(kf, kf->chroma, s);
-  else k_pvq_persist<false><<<persist, kPersistThreads, 0, s>>>(kf->chroma);
+  enqueue_split(kf, kf->chroma, s);
   if (!core && hdc) k_finish_scatter<false, true><<<wide, 256, 0, s>>>(kf->chroma);
   else if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->chroma);
 }
@@ -2891,8 +2670,6 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
     const char* with = cfg->keyframe_quant != 1 ? "a value other than 0 or 1"
                        : cfg->inter ? "inter (P and B frames take their records with frame_quant = 1)"
                        : cfg->lossless ? "lossless (every frame is at quantizer 0)"
-                       : cfg->noref_prepass ? "noref_prepass"
-                       : cfg->level_chains ? "level_chains"
                        : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
     if (with) {
       snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: keyframe_quant is not defined with %s", with);
@@ -2907,8 +2684,6 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
                        : cfg->late_skip ? "late_skip"
                        : cfg->inter_finish ? "inter_finish"
                        : cfg->frame_quant ? "frame_quant (every frame is at quantizer 0)"
-                       : cfg->noref_prepass ? "noref_prepass"
-                       : cfg->level_chains ? "level_chains"
                        : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
     if (with) {
       snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: lossless is not defined with %s", with);
@@ -2944,8 +2719,6 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
                        : cfg->dering ? "dering (the all-zero skip map of the deringing stage is a keyframe property)"
                        : cfg->symbol_stream == 1 ? "symbol_stream = 1 (its block record has no DC field; "
                                                    "symbol_stream = 2 is the P-frame stream)"
-                       : cfg->noref_prepass ? "noref_prepass"
-                       : cfg->level_chains ? "level_chains"
                        : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
     if (with) {
       snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: inter is not defined with %s", with);
@@ -2958,7 +2731,6 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   daala_b200_kf* kf = new (std::nothrow) daala_b200_kf();   // value-initialised: every field zero
   if (!kf) return nullptr;
   kf->cfg = *cfg;
-  if (kf->cfg.level_chains && kf->cfg.split_free < 2) kf->cfg.split_free = 2;   // the level kernel only walks the chains
   kf->nhsb = (cfg->pic_w + 63) / 64;
   kf->nvsb = (cfg->pic_h + 63) / 64;
   kf->F = cfg->nframes;
@@ -3057,10 +2829,10 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   if (kf->cfg.inter)
     return 5 + 2 + (2 + split(kf->luma)) + (2 + split(kf->chroma)) + 2 + (kf->cfg.inter_mc ? 2 : 0) +
            (kf->cfg.symbol_stream ? 8 : 0) + (kf->cfg.late_skip ? kLateSkipLaunches : 0);
-  int n = 5 + (kf->cfg.level_chains ? 2 : 0);                                    // work lists
+  int n = 5;                                                                      // work lists
   n += 1 + (kf->cfg.haar_dc_quant ? 1 : 0);                                       // forward, [DC chain]
-  n += 3 + 1 + (kf->cfg.split_free > 1 ? split(kf->luma) : 0) + (kf->luma.pre_ev ? 2 : 0);   // luma: begin (both stages), gather, [prepass], chains, finish
-  n += 2 + (kf->cfg.split_free > 0 ? split(kf->chroma) : 1);                      // chroma: gather, bands, finish
+  n += 3 + 1;                                                                     // luma: begin (both stages), gather, chains, finish
+  n += 2 + split(kf->chroma);                                                     // chroma: gather, phase kernels, finish
   // inverse + SB postfilter of plane 0 and of planes 1-2, [the rest of the deringing pass]
   n += kf->cfg.dering ? dering_launches(kf->dering, 2) : 4;
   // symbol stream: rank, superblock scan, [haar_dc_quant: DC records], place, 3 scan kernels, pack, index
@@ -3227,13 +2999,6 @@ static int sym_target(const void* p, long long cap, long long need, uint8_t** de
   *dev = (uint8_t*)a.devicePointer;
   return 0;
 }
-
-// With level_chains the compute phases of different engines never overlap on the device: the level kernel
-// synchronises its whole grid and needs every CTA resident, which two such kernels in flight could deny
-// each other.  Copies of one
-// engine still overlap the compute of another (that is what double buffering is for).
-static std::mutex g_compute_mu;
-static cudaEvent_t g_last_compute = nullptr;
 
 int daala_b200_kf_load_frame_quant(daala_b200_kf* kf, const daala_b200_kf_frame_quant* rec) {
   if (!kf) return (int)cudaErrorInvalidValue;
@@ -3460,15 +3225,8 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     if (!io->dering_level) return (int)cudaErrorInvalidValue;
     KF_CHECK(cudaMemcpyAsync(kf->dering.level, io->dering_level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyHostToDevice, s));
   }
-  int rc;
-  {
-    std::lock_guard<std::mutex> lock(g_compute_mu);
-    if (!g_last_compute) KF_CHECK(cudaEventCreateWithFlags(&g_last_compute, cudaEventDisableTiming));
-    else if (kf->cfg.level_chains) KF_CHECK(cudaStreamWaitEvent(s, g_last_compute, 0));
-    rc = daala_b200_kf_run_device(kf, DAALA_B200_KF_ALL, 1);
-    if (rc) return rc;
-    KF_CHECK(cudaEventRecord(g_last_compute, s));
-  }
+  const int rc = daala_b200_kf_run_device(kf, DAALA_B200_KF_ALL, 1);
+  if (rc) return rc;
   kf->have_step = true;
   kf->last_tot = tot;
   if (fq_mode) kf->fin_dc_limit = fq_dc_limit;

@@ -698,8 +698,7 @@ __device__ __forceinline__ void band_setup(int lane, BandCtx& B, const int32_t* 
 // Phase B: the searches of all events.  `snap`: kMaxEvents rows of snap_stride int16, private to the band.
 template <int kMode>
 __device__ __forceinline__ void band_search(int lane, BandCtx& B, int n, int16_t* snap, int snap_stride,
-                                            const double* rsq, const int32_t* pre_ev = nullptr,
-                                            const int16_t* pre_snap = nullptr) {
+                                            const double* rsq) {
   const bool big = kMode == 0 ? n > 32 : kMode == 2;
   const int (&x16)[4] = B.x16; const int (&xr)[4] = B.xr;
   const int &c_k = B.c_k, &c_alive = B.c_alive;
@@ -709,7 +708,6 @@ __device__ __forceinline__ void band_search(int lane, BandCtx& B, int n, int16_t
   int &e_sum = B.e_sum, &e_k = B.e_k, &e_zero = B.e_zero;
   unsigned alive_w = __ballot_sync(kFull, c_alive && lane < 12);
   unsigned alive_n = __ballot_sync(kFull, c_alive && lane >= 12);
-  if (pre_ev) alive_n = 0;   // the no-reference events were searched ahead of time (band_noref_export)
 
   // ---- events: the searches ---------------------------------------------------------------------------
   int ya[4];  // pulses of the running search, magnitudes (the reference's y_tmp without signs)
@@ -784,30 +782,6 @@ __device__ __forceinline__ void band_search(int lane, BandCtx& B, int n, int16_t
     if ((grp >> lane) & 1) c_ev = nev;
     nev++;
   }
-  if (pre_ev) {
-    // import the no-reference events: they follow the with-reference ones in the reference's candidate order
-    const int cev = (lane == 12 || lane == 13) ? pre_ev[lane - 12] : -1;
-    const int nimp = wmax(cev) + 1;
-    if (cev >= 0) c_ev = nev + cev;
-    if (lane >= nev && lane < nev + nimp) {
-      const int32_t* r = pre_ev + 2 + (lane - nev) * 9;
-      e_xy = __hiloint2double(r[1], r[0]);
-      e_yy = __hiloint2double(r[3], r[2]);
-      e_xx = __hiloint2double(r[5], r[4]);
-      e_sum = r[6];
-      e_k = r[7];
-      e_zero = r[8];
-    }
-    for (int ev = 0; ev < nimp; ev++) {
-#pragma unroll
-      for (int e = 0; e < 4; e++) {
-        if (e && !big) break;
-        const int j = e * 32 + lane;
-        if (j < n) snap[(nev + ev) * snap_stride + j] = pre_snap[ev * n + j];
-      }
-    }
-  }
-
 }
 
 // Phase C: costs, the reference's fold, synthesis of the winner (od_pvq_synthesis_partial, src/pvq.c:1037).
@@ -989,27 +963,6 @@ __device__ __forceinline__ int band_finish(int lane, const BandCtx& B, const int
   }
 }
 
-// No-reference events searched ahead of time (keyframe luma: they depend on the input vector alone, while
-// the with-reference half of pvq_theta has to wait for the neighbours the prediction comes from).  After
-// band_setup with r0 = NULL and band_search: pre_ev = {c_ev of lanes 12, 13; per event xy, yy, xx, sum, k,
-// zero} (20 words), pre_snap = the events' pulses, n int16 each.
-constexpr int kPreEvWords = 20;
-__device__ __forceinline__ void band_noref_export(int lane, const BandCtx& B, int n, const int16_t* snap,
-                                                  int snap_stride, int32_t* pre_ev, int16_t* pre_snap) {
-  const int cev = (lane == 12 || lane == 13) ? B.c_ev : -1;
-  const int nev = wmax(cev) + 1;
-  if (lane == 12 || lane == 13) pre_ev[lane - 12] = B.c_ev;
-  if (lane < nev) {
-    int32_t* r = pre_ev + 2 + lane * 9;
-    r[0] = __double2loint(B.e_xy); r[1] = __double2hiint(B.e_xy);
-    r[2] = __double2loint(B.e_yy); r[3] = __double2hiint(B.e_yy);
-    r[4] = __double2loint(B.e_xx); r[5] = __double2hiint(B.e_xx);
-    r[6] = B.e_sum; r[7] = B.e_k; r[8] = B.e_zero;
-  }
-  for (int ev = 0; ev < nev; ev++)
-    for (int j = lane; j < n; j += 32) pre_snap[ev * n + j] = snap[ev * snap_stride + j];
-}
-
 // One band by one warp, the three phases back to back.  `snap`: kSnapEntries int16 of scratch private to
 // the warp (shared memory); `rsq`: kTableDoubles doubles filled by pvq_fill_rsqrt_table.
 // The context is parked in the scratch between the phases, so that only what the search reads is live
@@ -1020,8 +973,7 @@ __device__ __forceinline__ int quantise_band_warp(int lane, int16_t* snap, const
                                                   const int32_t* r0, int n, int q0, int32_t* yout, int* itheta,
                                                   int* max_theta, int* vk, int beta, double* skip_term, int is_keyframe,
                                                   int pli, const int16_t* qm, const int16_t* qm_inv,
-                                                  double pvq_norm_lambda, const int32_t* pre_ev = nullptr,
-                                                  const int16_t* pre_snap = nullptr) {
+                                                  double pvq_norm_lambda) {
   int16_t* vec = snap + kMaxEvents * kMaxN;
   int32_t* lanes = reinterpret_cast<int32_t*>(vec + 3 * kMaxN);
   int32_t* uni = lanes + kCtxLaneWords * 16;
@@ -1035,7 +987,7 @@ __device__ __forceinline__ int quantise_band_warp(int lane, int16_t* snap, const
   {
     BandCtx B;
     band_ctx_load_search(lane, B, n, vec, kMaxN, lanes);
-    band_search<kMode>(lane, B, n, snap, kMaxN, rsq, pre_ev, pre_snap);
+    band_search<kMode>(lane, B, n, snap, kMaxN, rsq);
     band_ctx_store_search(lane, B, lanes);
   }
   ctx_sync();

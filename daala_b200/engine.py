@@ -59,7 +59,7 @@ class Config(ctypes.Structure):
     _fields_ = [("pic_w", c_int), ("pic_h", c_int), ("nframes", c_int), ("q0", c_int), ("use_masking", c_int),
                 ("qm_stride", c_int), ("pvq_norm_lambda", ctypes.c_double), ("pvq_qm_q4", (ctypes.c_ubyte * 32) * 3),
                 ("qm", c_void_p), ("qm_inv", c_void_p), ("sb_row0", c_int), ("sb_rows", c_int),
-                ("max_blocks_div", c_int), ("persist_ctas_per_sm", c_int), ("split_free", c_int), ("dering", c_int), ("noref_prepass", c_int), ("level_chains", c_int), ("stream", c_void_p),
+                ("max_blocks_div", c_int), ("persist_ctas_per_sm", c_int), ("dering", c_int), ("stream", c_void_p),
                 ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
                 ("symbol_stream", c_int), ("inter", c_int), ("inter_mc", c_int), ("mc_refs", c_int),
                 ("inter_finish", c_int), ("late_skip", c_int), ("mc_next", c_int), ("frame_quant", c_int),
@@ -203,9 +203,17 @@ class KeyframeEngine:
     """One engine = one set of device buffers + one CUDA graph for batches of `nframes` keyframes."""
 
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
-                 qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=0, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
+                 qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=1, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
                  qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0, inter_mc=0, mc_refs=0,
                  inter_finish=0, late_skip=0, mc_next=0, frame_quant=0, lossless=0, haar_dc_quant=0, keyframe_quant=0):
+        # split_free, level_chains and noref_prepass exist only for bench.py, which passes them: one schedule is left
+        retired = ("split_free=%r (chroma through the persistent kernel)" % split_free if split_free == 0 else
+                   "split_free=%r (luma bands 3 / 6 through the phase kernels)" % split_free if split_free != 1 else
+                   "level_chains=%r (level-synchronous luma chains)" % level_chains if level_chains != 0 else
+                   "noref_prepass=%r (the no-reference prepass)" % noref_prepass if noref_prepass != 0 else None)
+        if retired:
+            raise ValueError("KeyframeEngine: %s is a retired PVQ schedule; split_free=1, level_chains=0, noref_prepass=0 "
+                             "is the one the engine has" % retired)
         self.L = _bind()
         self.geom, self.F = geom, nframes
         if qm is None:
@@ -223,9 +231,6 @@ class KeyframeEngine:
         cfg.qm, cfg.qm_inv = self._qm.ctypes.data, self._qm_inv.ctypes.data
         cfg.sb_row0, cfg.sb_rows = int(sb_row0), int(sb_rows)
         cfg.max_blocks_div, cfg.persist_ctas_per_sm = int(max_blocks_div), int(persist_ctas_per_sm)
-        cfg.split_free = int(split_free)
-        cfg.level_chains = int(level_chains)
-        cfg.noref_prepass = int(noref_prepass)
         cfg.dering = int(dering)
         # dering == 2 or inter_finish == 2 (level search): scale of od_compute_dist and enc->dering_lambda =
         # 0.67 * OD_PVQ_LAMBDA * q^2 (src/rate.c:1086; the target quantizer is this engine's q0)

@@ -430,7 +430,8 @@ void daala_b200_host_keyframe_lists_free(daala_b200_keyframe_lists *lists);
    reconstruction + PVQ symbols out.  Inside (csrc/kf_engine.cu): work lists built on the device from
    the block-size maps EVERY step (leaf descriptors by prefix scan, od_hv_intra_pred neighbours,
    dependency-ordered band items), fused lapped prefilter + fDCT, luma PVQ with H/V intra prediction as
-   one persistent kernel with per-band acquire / release flags, chroma CfL + PVQ, iDCT + postfilters;
+   one persistent kernel with per-band acquire / release flags, chroma CfL + PVQ as three phase kernels
+   (setup / search / finish), iDCT + postfilters;
    one CUDA graph per engine.  Two engines give a double-buffered pipeline (submit one, wait for the
    other). */
 typedef struct daala_b200_kf daala_b200_kf;
@@ -448,9 +449,6 @@ typedef struct daala_b200_kf_config {
   int sb_row0, sb_rows;        /* superblock rows of this rank's shard (sb_rows <= 0: whole frames) */
   int max_blocks_div;          /* 0/1: capacity for all-4x4 maps; d > 1: 1/d of that (saves HBM) */
   int persist_ctas_per_sm;     /* 0 = default */
-  int split_free;              /* dependency-free bands as three phase kernels (setup / search / finish) with
-                                  the band context in HBM records instead of the persistent kernel:
-                                  0 = no, 1 = chroma, 2 = chroma and luma bands 3 / 6 */
   int dering;                  /* 1: the reconstruction goes through od_dering with the per-superblock levels of
                                   daala_b200_kf_io.dering_level (the final application of src/encode.c:2812-2842).
                                   2: the engine also SEARCHES the levels (src/encode.c:2708-2811: five filtered
@@ -458,11 +456,6 @@ typedef struct daala_b200_kf_config {
                                   rate, decision per frame on the device) and returns them in
                                   daala_b200_kf_io.dering_level_out; needs coded_quantizer / qm_is_flat /
                                   dering_lambda below */
-  int noref_prepass;           /* 1: the no-reference searches of every luma chain band run ahead of the chains in a
-                                  fully parallel kernel (they do not depend on the prediction) */
-  int level_chains;            /* luma intra chains: 0 = persistent kernel with a dependency queue, 1 = one
-                                  level-synchronous kernel (phases separated by grid barriers); implies
-                                  split_free = 2 */
   void *stream;                /* cudaStream_t to run on, or NULL: the engine creates its own */
   int coded_quantizer;         /* state->coded_quantizer (scale of od_compute_dist, src/encode.c:1221); dering == 2 or
                                   inter_finish == 2 */
@@ -484,14 +477,13 @@ typedef struct daala_b200_kf_config {
                                   goes through the same prefilters + fDCT as the source (no DC Haar pyramid on either)
                                   and is the reference vector of every band of every plane (pvq_theta with
                                   is_keyframe = 0: no H/V intra prediction, no CfL, no flip).  No band depends on
-                                  another block, so luma and chroma both run as the three phase kernels of
-                                  split_free and the persistent chain kernel is not launched.  DC is the scalar
+                                  another block, so luma and chroma both run as the three phase kernels (setup /
+                                  search / finish) of keyframe chroma and the persistent chain kernel is not launched.  DC is the scalar
                                   quantisation of in[0] - ref[0] with the band-0 quantiser (index in
                                   daala_b200_kf_io.luma_dc / chroma_dc); the uncoded tail of 32x32 / 64x64 blocks is
                                   the transformed prediction (od_init_skipped_coeffs for inter frames).
                                   Not defined, and refused by daala_b200_kf_create, together with dering,
-                                  symbol_stream = 1 (2 is its stream), noref_prepass, level_chains or a row shard
-                                  (sb_rows > 0) */
+                                  symbol_stream = 1 (2 is its stream) or a row shard (sb_rows > 0) */
   int inter_mc;                /* 0 (default): with inter, the prediction planes are the host input pred_pixels.
                                   1: the engine makes the prediction itself, as od_state_mc_predict does
                                   (reference src/state.c:932), from each frame's MV grid
@@ -550,7 +542,7 @@ typedef struct daala_b200_kf_config {
                                   the residual is d - od_haar(prediction), DC included.  q0, pvq_qm_q4, the other
                                   quantizer fields and io.bsize are not read.  Refused by daala_b200_kf_create with a
                                   value other than 0 or 1, and 1 together with dering, symbol_stream, late_skip,
-                                  inter_finish, frame_quant, noref_prepass, level_chains or a row shard (sb_rows > 0) */
+                                  inter_finish, frame_quant or a row shard (sb_rows > 0) */
   int haar_dc_quant;           /* 0 (default): keyframes are reconstructed with their unquantised DCs (the inverse
                                   undoes the forward transform's Haar DC pyramid); nothing below exists.
                                   1: the step quantises the keyframe DCs as the reference encoder does: per plane,
@@ -575,8 +567,8 @@ typedef struct daala_b200_kf_config {
                                   a keyframe's record with q0 = max(1, state->quantizer), state->coded_quantizer,
                                   enc->dering_lambda and the pvq_qm_q4 od_interp_qm set for that keyframe (reference
                                   src/encode.c:3050-3075).  Refused by daala_b200_kf_create with a value other than 0
-                                  or 1, and 1 together with inter (P and B frames have frame_quant), lossless,
-                                  noref_prepass, level_chains or a row shard (sb_rows > 0) */
+                                  or 1, and 1 together with inter (P and B frames have frame_quant), lossless or a
+                                  row shard (sb_rows > 0) */
 } daala_b200_kf_config;
 
 /* config.lossless: the root sums of one block (od_compute_max_tree, src/encode.c:899-919, over the residual of

@@ -26,22 +26,7 @@ extern "C" int emu_quantise_band(int32_t* out, const int32_t* x0, const int32_t*
     gain[lane] = quantise_band_warp(lane, snap, rsq, out, x0, r0, n, q0, y, &it[lane], &mt[lane], &k[lane], beta, &sd[lane],
                                     is_keyframe, pli, qm, qm_inv, lambda);
   });
-  if (getenv("DAALA_B200_EMU_PREPASS") && is_keyframe && pli == 0) {
-    // keyframe luma: the no-reference events searched ahead of time without the prediction, then imported
-    static int32_t pre_ev[kPreEvWords];
-    static int16_t pre_snap[2 * kMaxN];
-    static int16_t psnap[kSnapEntries];
-    simt_emu::run_warp([&](int lane) {
-      BandCtx B;
-      band_setup<0>(lane, B, x0, nullptr, n, q0, beta, is_keyframe, pli, qm, lambda, rsq);
-      band_search<0>(lane, B, n, psnap, kMaxN, rsq);
-      band_noref_export(lane, B, n, psnap, kMaxN, pre_ev, pre_snap);
-    });
-    simt_emu::run_warp([&](int lane) {
-      gain[lane] = quantise_band_warp(lane, snap, rsq, out, x0, r0, n, q0, y, &it[lane], &mt[lane], &k[lane], beta,
-                                      &sd[lane], is_keyframe, pli, qm, qm_inv, lambda, pre_ev, pre_snap);
-    });
-  } else if (getenv("DAALA_B200_EMU_SPLIT")) {
+  if (getenv("DAALA_B200_EMU_SPLIT")) {
     // the same band through the three phases with the context parked in a record in between
     static int16_t vec[3 * kMaxN];
     static int32_t lanes[kCtxLaneWords * 16], uni[kCtxUniWords];

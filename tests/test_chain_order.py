@@ -115,7 +115,7 @@ def test_weight_bins_order_heaviest_first():
 def _check_sorted_heads(geom, maps):
     from daala_b200 import engine, pvq, synth
     F = len(maps)
-    eng = engine.KeyframeEngine(geom, nframes=F, q0=72, pvq_qm_q4=np.full((3, 30), 16, np.uint8), split_free=1,
+    eng = engine.KeyframeEngine(geom, nframes=F, q0=72, pvq_qm_q4=np.full((3, 30), 16, np.uint8),
                                 max_blocks_div=2 if geom.pic_w == 3840 else 0)
     planes = []
     seed = 12345

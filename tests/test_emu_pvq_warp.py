@@ -71,21 +71,15 @@ def _check_case_set(emu, name, qm, qm_inv):
 
 # the second build lowers the "products are exact" bound so that the literal-scan path of the plain
 # pulses (taken on the device only when a product could exceed 2^53) runs on ordinary inputs
-# fourth run: keyframe luma with the no-reference half searched ahead of time (the engine's prepass);
 # third run: the same bands through the three phases with the band context parked in a record in between
 # (the split kernels of the engine), size-class specialised instantiations
-@pytest.mark.parametrize("name,extra,seeds,split", [("libpvq_warp_emu.so", [], (1, 2, 3), False),
+@pytest.mark.parametrize("name,extra,seeds,split", [("libpvq_warp_emu.so", [], (1, 2, 3, 5), False),
                                                     ("libpvq_warp_emu_scan.so", ["-DDAALA_B200_PVQ_EXACT_BOUND=1e12"], (1,), False),
-                                                    ("libpvq_warp_emu.so", [], (4,), True),
-                                                    ("libpvq_warp_emu.so", [], (5,), "prepass")])
+                                                    ("libpvq_warp_emu.so", [], (4,), True)])
 def test_warp_quantiser_matches_reference(name, extra, seeds, split, monkeypatch):
     emu = _build(name, extra)
-    # "prepass": keyframe luma bands with their no-reference events searched ahead of time and imported
     monkeypatch.delenv("DAALA_B200_EMU_SPLIT", raising=False)
-    monkeypatch.delenv("DAALA_B200_EMU_PREPASS", raising=False)
-    if split == "prepass":
-        monkeypatch.setenv("DAALA_B200_EMU_PREPASS", "1")
-    elif split:
+    if split:
         monkeypatch.setenv("DAALA_B200_EMU_SPLIT", "1")
     qm, qm_inv = _reference_qm()
     stats = (ctypes.c_longlong * 4).in_dll(emu, "daala_b200_pvq_warp_stats")

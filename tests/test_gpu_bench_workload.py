@@ -1,6 +1,6 @@
 """The workload bench.py measures, checked whole against the oracle: 16 frames of 3840x2160 per batch, the
 reference encoder's block-size maps and deringing levels, q0 72, the engine configured exactly as bench.py
-configures it (max_blocks_div = 2, split_free = 1, dering = 1).  Every frame, every plane and every output the
+configures it (max_blocks_div = 2, dering = 1).  Every frame, every plane and every output the
 host reads is compared -- reconstruction, band records, pulses, quantised coefficient planes, per-block
 skip_diff and CfL flip -- after the first submit, after the bench's timing sequence, and across two engines
 used alternately.  The batch cycles 4 distinct frames, so the oracle runs once per distinct frame."""
@@ -28,8 +28,7 @@ def _engine(geom, nframes=F, dering=1):
     from daala_b200 import engine
     return engine.KeyframeEngine(geom, nframes=nframes, q0=bench.Q0, use_masking=1, pvq_qm_q4=Q4, dering=dering,
                                  coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA,
-                                 persist_ctas_per_sm=0, split_free=1, level_chains=0, noref_prepass=0,
-                                 max_blocks_div=2)
+                                 persist_ctas_per_sm=0, max_blocks_div=2)
 
 
 def _stage(eng, hf, dering_levels=True):

@@ -123,7 +123,7 @@ def test_engine_block_capacity_boundary(binding):
         sizes = [1] * 128 + [2] * 32
         over = [1] * 132 + [2] * 31                   # one 16x16 block split into 8x8 blocks: 6 chroma blocks more
     q0, q4 = 72, np.full((3, 30), 16, np.uint8)
-    eng = engine.KeyframeEngine(geom, nframes=F, q0=q0, pvq_qm_q4=q4, split_free=1, max_blocks_div=2)
+    eng = engine.KeyframeEngine(geom, nframes=F, q0=q0, pvq_qm_q4=q4, max_blocks_div=2)
     cap = {"luma": eng.buf.max_luma_blocks, "chroma": eng.buf.max_chroma_blocks}
     nunits = F * geom.bsize_shape[0] * geom.bsize_shape[1]
     assert cap == {"luma": nunits * 2 + 64, "chroma": nunits + 64}
@@ -245,31 +245,14 @@ def test_engine_keyframe_chain_matches_oracle(size, q0, nf):
     eng.close()
 
 
-def test_engine_noref_prepass_matches_oracle():
-    """The no-reference searches of the luma chain bands ahead of the chains (daala_b200_kf_config.noref_prepass),
-    imported by the persistent kernel: same results, on mixed and on uniform maps, two batches per engine."""
+def test_engine_split_phase_kernels_match_oracle():
+    """Chroma through the three phase kernels with the band context parked in HBM records, on a mixed map and on an
+    all-64x64 one: same results as the oracle, bit for bit."""
     from daala_b200 import engine
     from daala_b200.frame import Geometry
     geom = Geometry(328, 200)
     q4 = np.full((3, 30), 16, np.uint8)
-    eng = engine.KeyframeEngine(geom, nframes=2, q0=72, pvq_qm_q4=q4, split_free=1, noref_prepass=1)
-    _check_batch(eng, geom, _frames(geom, 2), 72, q4)
-    _check_batch(eng, geom, _frames(geom, 2, q_seed=5, mode="32"), 72, q4)
-    _check_batch(eng, geom, _frames(geom, 2, q_seed=6, mode="4"), 72, q4)
-    eng.close()
-
-
-@pytest.mark.parametrize("split", [1, 2, 3])
-def test_engine_split_phase_kernels_match_oracle(split):
-    """The dependency-free bands (chroma; with split = 2 also luma bands 3 / 6) through the three phase
-    kernels with the band context parked in HBM records (daala_b200_kf_config.split_free) instead of the
-    persistent kernel: same results, bit for bit."""
-    from daala_b200 import engine
-    from daala_b200.frame import Geometry
-    geom = Geometry(328, 200)
-    q4 = np.full((3, 30), 16, np.uint8)
-    # split 3: additionally the luma intra chains level-synchronously (daala_b200_kf_config.level_chains)
-    eng = engine.KeyframeEngine(geom, nframes=2, q0=72, pvq_qm_q4=q4, split_free=min(split, 2), level_chains=int(split == 3))
+    eng = engine.KeyframeEngine(geom, nframes=2, q0=72, pvq_qm_q4=q4)
     _check_batch(eng, geom, _frames(geom, 2), 72, q4)
     _check_batch(eng, geom, _frames(geom, 2, q_seed=3, mode="64"), 72, q4)
     eng.close()
@@ -346,7 +329,7 @@ def test_engine_dering_stage_matches_oracle():
     rng = np.random.default_rng(3)
     levels = rng.integers(0, 6, size=(F, geom.nvsb, geom.nhsb)).astype(np.uint8)
     levels[0, 0, 0] = 0
-    eng = engine.KeyframeEngine(geom, nframes=F, q0=q0, pvq_qm_q4=q4, split_free=1, dering=1)
+    eng = engine.KeyframeEngine(geom, nframes=F, q0=q0, pvq_qm_q4=q4, dering=1)
     out = eng.encode([np.stack([f[0][p] for f in frames]) for p in range(3)], np.stack([f[1] for f in frames]),
                      dering_levels=levels)
     gain = [0, 0.5, 0.707, 1, 1.41, 2]
@@ -407,7 +390,7 @@ def test_engine_dering_search_matches_reference(q0):
     q4 = np.full((3, 30), 16, np.uint8)
     F = 3
     frames = _frames(geom, F, q_seed=q0)
-    eng = engine.KeyframeEngine(geom, nframes=F, q0=q0, pvq_qm_q4=q4, split_free=1, dering=2, coded_quantizer=q0)
+    eng = engine.KeyframeEngine(geom, nframes=F, q0=q0, pvq_qm_q4=q4, dering=2, coded_quantizer=q0)
     out = eng.encode([np.stack([f[0][p] for f in frames]) for p in range(3)], np.stack([f[1] for f in frames]))
     got_levels = out["dering_levels"].copy()
     a = oracle_lib.addr

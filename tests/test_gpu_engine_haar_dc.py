@@ -35,7 +35,7 @@ def _frames(geom, nframes):
 
 
 def _encode(geom, frames, maps, q0, q4, lam, **kw):
-    eng = engine.KeyframeEngine(geom, nframes=len(frames), q0=q0, pvq_qm_q4=q4, lam=lam, split_free=1, haar_dc_quant=1,
+    eng = engine.KeyframeEngine(geom, nframes=len(frames), q0=q0, pvq_qm_q4=q4, lam=lam, haar_dc_quant=1,
                                 **kw)
     try:
         out = eng.encode([np.stack([fr[p] for fr in frames]) for p in range(3)], np.stack(maps))
@@ -84,7 +84,7 @@ def test_quantised_dcs_change_the_reconstruction():
     frames, maps = _frames(geom, 2), _maps(geom, 2)
     q0, q4, lam = _settings(7, 0)
     got = _encode(geom, frames, maps, q0, q4, lam, dering=2)
-    eng = engine.KeyframeEngine(geom, nframes=2, q0=q0, pvq_qm_q4=q4, lam=lam, split_free=1, dering=2)
+    eng = engine.KeyframeEngine(geom, nframes=2, q0=q0, pvq_qm_q4=q4, lam=lam, dering=2)
     try:
         base = eng.encode([np.stack([fr[p] for fr in frames]) for p in range(3)], np.stack(maps))
         assert any(not np.array_equal(base["recon%d" % p], got["recon%d" % p]) for p in range(3))
@@ -97,7 +97,7 @@ def test_quantised_dcs_change_the_reconstruction():
 def test_submit_refuses_dc_index_without_the_mode():
     geom = Geometry(200, 130)
     frames, maps = _frames(geom, 1), _maps(geom, 1)
-    eng = engine.KeyframeEngine(geom, nframes=1, q0=45, pvq_qm_q4=np.full((3, 30), 20, np.uint8), split_free=1)
+    eng = engine.KeyframeEngine(geom, nframes=1, q0=45, pvq_qm_q4=np.full((3, 30), 20, np.uint8))
     try:
         eng.stage_inputs([fr[None] for fr in frames[0]], maps[0][None])
         eng.prepare_io()
@@ -181,7 +181,7 @@ def test_forked_step_equals_phase_by_phase(dering):
     geom = Geometry(1920, 1080)
     frames, maps = _frames(geom, 2), _maps(geom, 2)
     q0, q4, lam = _settings(5, 0)
-    eng = engine.KeyframeEngine(geom, nframes=2, q0=q0, pvq_qm_q4=q4, lam=lam, dering=dering, split_free=1,
+    eng = engine.KeyframeEngine(geom, nframes=2, q0=q0, pvq_qm_q4=q4, lam=lam, dering=dering,
                                 coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA, haar_dc_quant=1)
     try:
         eng.stage_inputs([np.stack([fr[p] for fr in frames]) for p in range(3)], np.stack(maps))

@@ -270,14 +270,13 @@ def test_inter_engine_refusals():
     from daala_b200.frame import Geometry
     geom = Geometry(128, 64)
     for kw, word in ((dict(dering=1), "dering"), (dict(symbol_stream=1), "symbol_stream"),
-                     (dict(noref_prepass=1), "noref_prepass"), (dict(level_chains=1), "level_chains"),
                      (dict(sb_row0=0, sb_rows=1), "shard"), (dict(inter=2), "0 or 1")):
         args = dict(inter=1)
         args.update(kw)
         with pytest.raises(RuntimeError, match=word):
             engine.KeyframeEngine(geom, nframes=1, q0=45, pvq_qm_q4=Q4, **args)
     # a keyframe engine refuses pred=, an inter engine a batch without it
-    kf = engine.KeyframeEngine(geom, nframes=1, q0=45, pvq_qm_q4=Q4, split_free=1)
+    kf = engine.KeyframeEngine(geom, nframes=1, q0=45, pvq_qm_q4=Q4)
     frames = _frames(geom, 1)
     planes, pred, bsize = ([a[None] for a in frames[0][0]], [a[None] for a in frames[0][1]], frames[0][2][None])
     with pytest.raises(ValueError):

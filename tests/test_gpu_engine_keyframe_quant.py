@@ -13,8 +13,8 @@ created with per-frame config fields far from every record (q0 999, coded quanti
   settings.
 - Nothing is baked at create: batch A then batch B on one engine, live and replayed, equals a fresh engine's B; a
   permuted batch permutes the outputs.
-- Uniform records equal the engine without the mode, launches included; the schedules (split_free 0 / 1 / 2, forked graph / phase by phase,
-  dering 1 / 2, haar_dc_quant on / off) agree; submit refuses missing and out-of-range records before any copy."""
+- Uniform records equal the engine without the mode, launches included; the forked graph and the phase-by-phase path
+  agree (dering 1 / 2, haar_dc_quant on / off); submit refuses missing and out-of-range records before any copy."""
 import os
 
 import numpy as np
@@ -31,7 +31,7 @@ CONFIGS = ("hvs-masking", "hvs", "flat-masking")
 ALL = tuple(range(NPOINTS))
 # the per-frame config fields of the engine under test: none of them is any record's
 OFF = dict(q0=999, pvq_qm_q4=np.full((3, 30), 9, np.uint8), coded_quantizer=33, dering_lambda=7.0)
-FULL = dict(split_free=1, dering=2, symbol_stream=1, haar_dc_quant=1)
+FULL = dict(dering=2, symbol_stream=1, haar_dc_quant=1)
 
 
 def _records(points, config):
@@ -161,7 +161,7 @@ def test_4k_two_points_on_bench_maps():
     frames = bench.make_host_frames(geom, 2)
     planes, maps = [fr[0] for fr in frames], [fr[1] for fr in frames]
     levels = np.stack([fr[2] for fr in frames])
-    _against_uniform(geom, 0, (1, 6), planes, maps, levels, split_free=1, dering=1, max_blocks_div=2, symbol_stream=1,
+    _against_uniform(geom, 0, (1, 6), planes, maps, levels, dering=1, max_blocks_div=2, symbol_stream=1,
                      haar_dc_quant=1)
 
 
@@ -173,7 +173,7 @@ def test_mixed_batch_matches_pipeline_oracle():
         pytest.skip("needs the reference build (the level search of keyframe_chain)")
     geom, config, points = Geometry(200, 130), 0, (0, 3, 7)
     planes, maps = _frames(geom, len(points), seed=31)
-    eng = _mixed(geom, len(points), config, split_free=1, dering=2)
+    eng = _mixed(geom, len(points), config, dering=2)
     try:
         got = _run(eng, planes, maps, _records(points, config))
     finally:
@@ -200,7 +200,7 @@ def test_mixed_batch_matches_haar_dc_driver():
         pytest.skip("needs oracle/_ref/libdaala_ref_haar_dc.so")
     geom, config, points = Geometry(200, 130), 1, (1, 5, 7)
     planes, maps = _frames(geom, len(points), seed=41)
-    eng = _mixed(geom, len(points), config, split_free=1, haar_dc_quant=1)
+    eng = _mixed(geom, len(points), config, haar_dc_quant=1)
     try:
         got = _run(eng, planes, maps, _records(points, config))
     finally:
@@ -277,28 +277,20 @@ def test_uniform_records_run_as_the_engine_without_the_mode(point):
     _assert_steps_equal(got, want, geom, F, "uniform records")
 
 
-SCHEDULES = [dict(split_free=sf, dering=d, haar_dc_quant=h) for sf in (0, 1, 2) for d in (1, 2) for h in (0, 1)]
+SCHEDULES = [dict(dering=d, haar_dc_quant=h) for d in (1, 2) for h in (0, 1)]
 
 
-@pytest.mark.parametrize("opts", SCHEDULES, ids=lambda o: "split%d-dering%d-hdc%d" % (o["split_free"], o["dering"],
-                                                                                        o["haar_dc_quant"]))
+@pytest.mark.parametrize("opts", SCHEDULES, ids=lambda o: "dering%d-hdc%d" % (o["dering"], o["haar_dc_quant"]))
 def test_schedules_agree(opts):
-    """Every schedule of the mode against split_free = 1 with the same dering and DC options, and the forked graph
-    against the phase-by-phase path on the device."""
+    """The forked graph against the phase-by-phase path on the device, with each dering and DC option."""
     geom, config, points = Geometry(200, 130), 0, (0, 4, 7)
     F = len(points)
     planes, maps = _frames(geom, F, seed=71)
     rec = _records(points, config)
     levels = _levels(geom, F, 72) if opts["dering"] == 1 else None
-    base = _mixed(geom, F, config, **dict(opts, split_free=1))
-    try:
-        want = _run(base, planes, maps, rec, levels)
-    finally:
-        base.close()
     eng = _mixed(geom, F, config, **opts)
     try:
-        got = _run(eng, planes, maps, rec, levels)
-        _assert_steps_equal(got, want, geom, F, "schedule %s" % opts)
+        want = _run(eng, planes, maps, rec, levels)
         # the phase-by-phase path (each phase enqueued on its own) on the inputs the submit left on the device
         eng.run_device(phases=engine.PH_LISTS | engine.PH_FORWARD, graph=False)
         eng.run_device(phases=engine.PH_PVQ_LUMA, graph=False)
@@ -314,7 +306,7 @@ def test_schedules_agree(opts):
 def test_submit_refusals_before_any_copy():
     geom, config, F = Geometry(200, 130), 0, 2
     planes, maps = _frames(geom, F, seed=81)
-    eng = _mixed(geom, F, config, split_free=1)
+    eng = _mixed(geom, F, config)
     try:
         _run(eng, planes, maps, _records((2, 5), config))
         before = [eng.coeff_plane(p) for p in range(3)]
@@ -335,7 +327,7 @@ def test_submit_refusals_before_any_copy():
     finally:
         eng.close()
     # records on an engine with neither mode
-    plain = _uniform(geom, 2, config, F=F, split_free=1)
+    plain = _uniform(geom, 2, config, F=F)
     try:
         with pytest.raises(Exception, match="needs an engine with frame_quant = 1 or keyframe_quant = 1"):
             _run(plain, planes, maps, _records((2, 5), config))

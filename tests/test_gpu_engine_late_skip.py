@@ -235,7 +235,7 @@ def test_refusals():
     F = 2
     for kw in (dict(late_skip=1), dict(inter=1, late_skip=2), dict(inter=1, late_skip=-1)):
         with pytest.raises(RuntimeError, match="late_skip"):
-            engine.KeyframeEngine(geom, nframes=F, q0=45, pvq_qm_q4=Q4, split_free=1, **kw)
+            engine.KeyframeEngine(geom, nframes=F, q0=45, pvq_qm_q4=Q4, **kw)
     planes, pred, bsize = _stack(_frames(geom, F, seed=5))
     recs = engine.Pinned((4096,), symbols.LATE_SKIP_DTYPE)
 

@@ -186,8 +186,8 @@ def test_launches_and_refusals():
     from daala_b200.frame import Geometry
     geom = Geometry(200, 130)
     q4 = np.full((3, 30), 20, np.uint8)
-    a = engine.KeyframeEngine(geom, nframes=1, q0=45, pvq_qm_q4=q4, split_free=1)
-    b = engine.KeyframeEngine(geom, nframes=1, q0=45, pvq_qm_q4=q4, split_free=1, lossless=0)
+    a = engine.KeyframeEngine(geom, nframes=1, q0=45, pvq_qm_q4=q4)
+    b = engine.KeyframeEngine(geom, nframes=1, q0=45, pvq_qm_q4=q4, lossless=0)
     assert a.launches_per_step() == b.launches_per_step()
     planes = [a_[None] for a_ in content(geom, "random", seed=1)]
     bsize = synth.block_size_map(geom, "mixed", seed=2)[None]

@@ -146,7 +146,7 @@ def _run_keyframes(geom, F, point, config, seed, noise=False):
         pytest.skip("needs the reference build (the level search of keyframe_chain)")
     s = settings(point, config, 0)
     frames = _kf_frames(geom, F, seed, noise)
-    eng = _engine(geom, F, s, split_free=1, dering=2, symbol_stream=1)
+    eng = _engine(geom, F, s, dering=2, symbol_stream=1)
     try:
         out = eng.encode([np.stack([fr[0][p] for fr in frames]) for p in range(3)], np.stack([fr[1] for fr in frames]),
                          stream=True)

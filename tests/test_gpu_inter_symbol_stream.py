@@ -329,7 +329,7 @@ def test_submit_refusals():
     F = 2
     planes, pred, bsize = _stack(_frames(geom, F, seed=5))
     # a keyframe engine with the keyframe stream
-    kf = engine.KeyframeEngine(geom, nframes=F, q0=45, pvq_qm_q4=Q4, split_free=1, symbol_stream=1)
+    kf = engine.KeyframeEngine(geom, nframes=F, q0=45, pvq_qm_q4=Q4, symbol_stream=1)
     kf.stage_inputs(planes, bsize)
     kf.prepare_io(stream=True)
     b = kf.symbol_bounds()

@@ -53,7 +53,7 @@ def test_forked_step_equals_phase_by_phase(size, dering):
     frames = _frames(geom)
     F = len(frames)
     eng = engine.KeyframeEngine(geom, nframes=F, q0=bench.Q0, use_masking=1, pvq_qm_q4=Q4, dering=dering,
-                                coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA, split_free=1,
+                                coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA,
                                 symbol_stream=1)
     try:
         eng.stage_inputs([np.stack([f[0][p] for f in frames]) for p in range(3)], np.stack([f[1] for f in frames]))

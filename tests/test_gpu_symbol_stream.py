@@ -19,8 +19,7 @@ Q4 = np.full((3, 30), bench.PVQ_QM_Q4, np.uint8)
 def _engine(geom, nframes, symbol_stream=1, dering=1, q0=bench.Q0, q4=Q4, **kw):
     from daala_b200 import engine
     args = dict(nframes=nframes, q0=q0, use_masking=1, pvq_qm_q4=q4, dering=dering, coded_quantizer=bench.CODED_Q,
-                dering_lambda=bench.DERING_LAMBDA, persist_ctas_per_sm=0, split_free=1, level_chains=0,
-                noref_prepass=0, max_blocks_div=2, symbol_stream=symbol_stream)
+                dering_lambda=bench.DERING_LAMBDA, persist_ctas_per_sm=0, max_blocks_div=2, symbol_stream=symbol_stream)
     args.update(kw)
     return engine.KeyframeEngine(geom, **args)
 

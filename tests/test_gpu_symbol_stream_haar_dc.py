@@ -42,7 +42,7 @@ def _frames(geom, n, seed=3):
 
 def _engine(geom, F, setting=5, **kw):
     q0, q4, lam = _settings(setting)
-    opts = dict(q0=q0, pvq_qm_q4=q4, lam=lam, split_free=1, symbol_stream=1, haar_dc_quant=1)
+    opts = dict(q0=q0, pvq_qm_q4=q4, lam=lam, symbol_stream=1, haar_dc_quant=1)
     opts.update(kw)
     return engine.KeyframeEngine(geom, nframes=F, **opts)
 
@@ -89,7 +89,7 @@ def test_records_match_the_grids_4k_bench_workload():
     hf = bench.make_host_frames(geom, 4)
     eng = engine.KeyframeEngine(geom, nframes=4, q0=bench.Q0, use_masking=1,
                                 pvq_qm_q4=np.full((3, 30), bench.PVQ_QM_Q4, np.uint8), dering=1,
-                                coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA, split_free=1,
+                                coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA,
                                 max_blocks_div=2, symbol_stream=1, haar_dc_quant=1)
     try:
         out = _run(eng, [f[0] for f in hf], [f[1] for f in hf], dering_levels=np.stack([f[2] for f in hf]))
@@ -103,7 +103,7 @@ def test_keyframe_quant_batch_over_the_sweep():
     from tests.test_gpu_engine_keyframe_quant import ALL, _frames as kq_frames, _mixed, _records
     geom = Geometry(200, 130)
     planes, maps = kq_frames(geom, len(ALL), seed=31)
-    eng = _mixed(geom, len(ALL), 0, split_free=1, dering=2, symbol_stream=1, haar_dc_quant=1)
+    eng = _mixed(geom, len(ALL), 0, dering=2, symbol_stream=1, haar_dc_quant=1)
     try:
         out = _run(eng, planes, maps, frame_quant=_records(ALL, 0))
     finally:

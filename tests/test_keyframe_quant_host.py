@@ -38,8 +38,6 @@ REFUSED = (
     (dict(keyframe_quant=-1), KQ + "a value other than 0 or 1"),
     (dict(inter=1), KQ + "inter"),
     (dict(lossless=1), KQ + "lossless"),
-    (dict(noref_prepass=1), KQ + "noref_prepass"),
-    (dict(level_chains=1), KQ + "level_chains"),
     (dict(sb_row0=0, sb_rows=1), KQ + r"a row shard \(sb_rows > 0\)"),
     (dict(q0=0), Q0),
     (dict(keyframe_quant=0, q0=0), Q0),

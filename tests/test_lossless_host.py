@@ -140,8 +140,7 @@ def test_struct_layout(tmp_path):
 
 
 REFUSED = (dict(lossless=2), dict(lossless=-1), dict(dering=1), dict(symbol_stream=1), dict(inter=1, symbol_stream=2),
-           dict(inter=1, late_skip=1), dict(inter=1, inter_finish=1), dict(inter=1, frame_quant=1),
-           dict(noref_prepass=1), dict(level_chains=1), dict(sb_rows=1))
+           dict(inter=1, late_skip=1), dict(inter=1, inter_finish=1), dict(inter=1, frame_quant=1), dict(sb_rows=1))
 
 
 @pytest.mark.parametrize("kw", REFUSED, ids=lambda kw: ",".join("%s=%d" % i for i in kw.items()))

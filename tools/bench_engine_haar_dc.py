@@ -4,7 +4,7 @@ synthetic 3840x2160 4:2:0 frames with the reference encoder's block-size maps, q
 Two engines, timed in alternating rounds (CUDA events on the engine's stream, inputs resident in HBM, one graph replay
 per step).  Reported: ms per step of each; the DC chain's own device time and its place in the step (the median node
 timeline of tools/profile_step.py under torch.profiler: start and end of k_haar_dc against the luma chain kernel
-k_pvq_persist<true> and the luma finishing scatter that waits for it); the index grids' D2H bytes per step; the card's
+k_pvq_persist and the luma finishing scatter that waits for it); the index grids' D2H bytes per step; the card's
 name and power limit.  Needs a CUDA device; prints one JSON line.
 
     python tools/bench_engine_haar_dc.py [--rounds 3] [--steps 10] [--reps 10]
@@ -43,7 +43,7 @@ def main():
     engines, d2h = {}, {}
     for mode in (0, 1):
         eng = engine.KeyframeEngine(geom, nframes=F, q0=bench.Q0, use_masking=1, pvq_qm_q4=q4, dering=1,
-                                    coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA, split_free=1,
+                                    coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA,
                                     max_blocks_div=2, haar_dc_quant=mode)
         eng.stage_inputs([np.stack([f[0][p] for f in hf]) for p in range(3)], np.stack([f[1] for f in hf]))
         eng.stage_dering_levels(np.stack([f[2] for f in hf]))
@@ -68,7 +68,7 @@ def main():
         return next((r for r in s["nodes"] if r["node"].startswith(prefix)), None)
 
     chain = node(tl, "daala_b200::haar_dc::k_haar_dc") or node(tl, "k_haar_dc")
-    persist = node(tl, "daala_b200::kf::k_pvq_persist<true>") or node(tl, "k_pvq_persist<true>")
+    persist = node(tl, "daala_b200::kf::k_pvq_persist") or node(tl, "k_pvq_persist")
     scatter = node(tl, "daala_b200::kf::k_finish_scatter<false, true>") or node(tl, "k_finish_scatter<false, true>")
     m0, m1 = statistics.median(ms[0]), statistics.median(ms[1])
     res = dict(gpu=bench.gpu_identity(torch.cuda.current_device()), frames=F, size="%dx%d" % (bench.PIC_W, bench.PIC_H),

@@ -43,7 +43,7 @@ def main():
     pred = [np.roll(planes[p], 1, axis=0) for p in range(3)]
     bsize = np.stack([f[1] for f in hf])
     common = dict(nframes=F, q0=bench.Q0, use_masking=1, pvq_qm_q4=q4, max_blocks_div=2)
-    engines = {"keyframe": engine.KeyframeEngine(geom, split_free=1, **common),
+    engines = {"keyframe": engine.KeyframeEngine(geom, **common),
                "inter": engine.KeyframeEngine(geom, inter=1, **common)}
     outs = {}
     for name, eng in engines.items():

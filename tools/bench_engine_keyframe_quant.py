@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Keyframe batches with a quantizer per frame (keyframe_quant = 1) against the default keyframe step: bench.py's 16
 synthetic 3840x2160 4:2:0 frames with the reference encoder's block-size maps and deringing levels (dering = 1,
-split_free = 1, max_blocks_div = 2).  Arms, each its own engine, timed in alternating rounds (CUDA events on the
+max_blocks_div = 2).  Arms, each its own engine, timed in alternating rounds (CUDA events on the
 engine's stream, inputs resident in HBM, one graph replay per step):
 
   default       bench.py's engine: q0 72, flat pvq_qm_q4 16
@@ -60,7 +60,7 @@ def main():
     engines, outs = {}, {}
     for arm in ARMS:
         eng = engine.KeyframeEngine(geom, nframes=F, q0=bench.Q0, use_masking=1, pvq_qm_q4=q4, dering=1,
-                                    coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA, split_free=1,
+                                    coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA,
                                     max_blocks_div=2, keyframe_quant=int(records[arm] is not None),
                                     haar_dc_quant=int(arm.startswith("hdc")))
         eng.stage_inputs([np.stack([f[0][p] for f in hf]) for p in range(3)], np.stack([f[1] for f in hf]))

@@ -1,7 +1,7 @@
 """What the keyframe engine's symbol stream (config.symbol_stream = 1) costs and saves on the benchmark workload.
 
 The workload is bench.py's (16 x 3840x2160 per batch, the reference encoder's block-size maps and deringing
-levels, q0 72, max_blocks_div = 2, split_free = 1, dering = 1), built with bench.py's own helpers.  In one
+levels, q0 72, max_blocks_div = 2, dering = 1), built with bench.py's own helpers.  In one
 process, alternating the two configurations round by round, it measures:
   - the device step time (graph replay, CUDA events on the engine's stream) with symbol_stream 0 and 1;
   - end-to-end Mpixels/s through two double-buffered engines (submit one batch while the other one runs, as
@@ -49,8 +49,7 @@ def main():
     def make(stream, rotate):
         hf = bench.make_host_frames(geom, F, rotate=rotate)
         eng = engine.KeyframeEngine(geom, nframes=F, q0=bench.Q0, use_masking=1, pvq_qm_q4=q4, dering=1,
-                                    coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA,
-                                    persist_ctas_per_sm=0, split_free=1, level_chains=0, noref_prepass=0,
+                                    coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA, persist_ctas_per_sm=0,
                                     max_blocks_div=2, symbol_stream=stream, haar_dc_quant=int(args.haar_dc))
         eng.stage_inputs([np.stack([f[0][p] for f in hf]) for p in range(3)], np.stack([f[1] for f in hf]))
         eng.stage_dering_levels(np.stack([f[2] for f in hf]))

@@ -1,4 +1,4 @@
-"""Timeline of the luma chain kernel k_pvq_persist<intra> on bench.py's workload.
+"""Timeline of the luma chain kernel k_pvq_persist on bench.py's workload.
 
 Builds a copy of the library whose chain kernel records every item it runs (kf_engine.cu compiled with
 -DDAALA_B200_CHAIN_TRACE, in a temporary directory; the in-tree library and its kernel are untouched), runs
@@ -11,7 +11,7 @@ one luma stage:
 
 Needs a GPU and a prior build() (the other objects of the library are linked from daala_b200/_obj).
 
-    python tools/chain_timeline.py [--json out.json] [--ctas-per-sm 0] [--split-free 1]
+    python tools/chain_timeline.py [--json out.json] [--ctas-per-sm 0]
 """
 import argparse
 import ctypes
@@ -93,7 +93,6 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--json", help="write the report here as well")
     ap.add_argument("--ctas-per-sm", type=int, default=0)
-    ap.add_argument("--split-free", type=int, default=1)
     ap.add_argument("--runs", type=int, default=3, help="luma stages to run; the last one is reported")
     args = ap.parse_args()
     with tempfile.TemporaryDirectory() as tmp:
@@ -110,7 +109,7 @@ def main():
         hf = bench.make_host_frames(geom, 16)
         q4 = np.full((3, 30), bench.PVQ_QM_Q4, np.uint8)
         eng = engine.KeyframeEngine(geom, nframes=16, q0=bench.Q0, use_masking=1, pvq_qm_q4=q4,
-                                    persist_ctas_per_sm=args.ctas_per_sm, split_free=args.split_free, max_blocks_div=2)
+                                    persist_ctas_per_sm=args.ctas_per_sm, max_blocks_div=2)
         eng.upload([np.stack([f[0][p] for f in hf]) for p in range(3)], np.stack([f[1] for f in hf]))
         eng.run_device(engine.PH_ALL, graph=False)
         for _ in range(args.runs):

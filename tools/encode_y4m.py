@@ -45,7 +45,7 @@ def main():
     maps = np.load(args.bsize_npz) if args.bsize_npz else None
     F = min(args.batch, len(frames))
     q4 = np.full((3, 30), 16, np.uint8)
-    eng = engine.KeyframeEngine(geom, nframes=F, q0=args.q0, pvq_qm_q4=q4, split_free=1, dering=args.dering,
+    eng = engine.KeyframeEngine(geom, nframes=F, q0=args.q0, pvq_qm_q4=q4, dering=args.dering,
                                 coded_quantizer=args.coded_quantizer, symbol_stream=1,
                                 haar_dc_quant=int(args.haar_dc))
     if args.symbols:

@@ -4,7 +4,7 @@ SB-edge postfilter, deringing, u8 store) on the workload bench.py measures, unde
 activities.
 
 The workload is built with bench.py's own helpers and constants (16 frames of 3840x2160 4:2:0, the reference
-encoder's block-size maps and deringing levels, q0 72, max_blocks_div 2, split_free 1).  One full step runs first
+encoder's block-size maps and deringing levels, q0 72, max_blocks_div 2).  One full step runs first
 so that the inverse phase has its inputs, then PH_INVERSE is launched `--reps` times without a graph under the
 profiler, then PH_ALL once more in a trace of its own.  For every kernel of the phase the script prints its mean
 device time per step, the bytes it has to move (computed from the plane shapes: every sample read and written
@@ -82,7 +82,7 @@ def main():
     hf = bench.make_host_frames(geom, F)
     eng = engine.KeyframeEngine(geom, nframes=F, q0=bench.Q0, use_masking=1, pvq_qm_q4=q4, dering=args.dering,
                                 coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA, persist_ctas_per_sm=0,
-                                split_free=1, level_chains=0, noref_prepass=0, max_blocks_div=2)
+                                max_blocks_div=2)
     eng.stage_inputs([np.stack([f[0][p] for f in hf]) for p in range(3)], np.stack([f[1] for f in hf]))
     if args.dering == 1:
         eng.stage_dering_levels(np.stack([f[2] for f in hf]))

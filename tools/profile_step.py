@@ -3,7 +3,7 @@
 start / end offset within the step, and the idle gaps between nodes, under torch.profiler with CUDA activities.
 
 The workload is bench.py's (built with its own helpers and constants): 16 frames of 3840x2160 4:2:0, the reference
-encoder's block-size maps and deringing levels, q0 72, max_blocks_div 2, split_free 1, symbol stream on.  After one
+encoder's block-size maps and deringing levels, q0 72, max_blocks_div 2, symbol stream on.  After one
 end-to-end pass and a few warm-up steps, `--reps` replays of the whole-step graph run under the profiler, each
 followed by a device synchronise and a short host pause, so that the trace falls apart into one segment per step.
 The same is done with live launches (no graph) unless --graph-only is given.  Per node the script reports the
@@ -150,7 +150,7 @@ def main():
     hf = bench.make_host_frames(geom, F)
     eng = engine.KeyframeEngine(geom, nframes=F, q0=bench.Q0, use_masking=1, pvq_qm_q4=q4, dering=args.dering,
                                 coded_quantizer=bench.CODED_Q, dering_lambda=bench.DERING_LAMBDA, persist_ctas_per_sm=0,
-                                split_free=1, level_chains=0, noref_prepass=0, max_blocks_div=2)
+                                max_blocks_div=2)
     eng.stage_inputs([np.stack([f[0][p] for f in hf]) for p in range(3)], np.stack([f[1] for f in hf]))
     if args.dering == 1:
         eng.stage_dering_levels(np.stack([f[2] for f in hf]))

@@ -3,7 +3,7 @@
 Compiles daala_b200/csrc/kf_engine.cu to a cubin with the library's flags (daala_b200/build.py, which
 include -lineinfo) and prints, per PVQ kernel: SASS bytes, registers, stack frame, spill bytes and the
 STL / LDL / BRA / BSSY / CALL counts.  For one kernel (by default the luma chain kernel
-k_pvq_persist<true>) it also splits the bytes by source region, from the line info of every instruction:
+k_pvq_persist) it also splits the bytes by source region, from the line info of every instruction:
 
   * out-of-line <fn>: the body of a subroutine the kernel calls (a __noinline__ function, or a slow path of
     the CUDA math library), whatever it inlines, found by the subroutine's label;
@@ -29,7 +29,7 @@ from daala_b200 import build as _build  # noqa: E402
 
 SRC = os.path.join(_build.CSRC, "kf_engine.cu")
 CUDA_BIN = os.path.dirname(_build.NVCC)
-PVQ_KERNELS = ("k_pvq_persist", "k_pvq_split", "k_pvq_prepass", "k_pvq_levels")
+PVQ_KERNELS = ("k_pvq_persist", "k_pvq_split")
 COUNTED = ("STL", "LDL", "BRA", "BSSY", "CALL", "WARPSYNC")
 
 def pretty(mangled):
@@ -185,7 +185,7 @@ def footprint(kernel_filter=None):
             row[op] = sum(1 for o, _, _ in instrs if o == op)
         rows.append(row)
     rows.sort(key=lambda r: -r["sass_bytes"])
-    detail_name = kernel_filter or "k_pvq_persist<true>"
+    detail_name = kernel_filter or "k_pvq_persist"
     detail = None
     for mangled, instrs in code.items():
         if pretty(mangled) == detail_name:
@@ -200,7 +200,7 @@ def footprint(kernel_filter=None):
 
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
-    ap.add_argument("--kernel", help="kernel whose bytes are split by region (default k_pvq_persist<true>)")
+    ap.add_argument("--kernel", help="kernel whose bytes are split by region (default k_pvq_persist)")
     ap.add_argument("--json", action="store_true", help="print one JSON object instead of tables")
     a = ap.parse_args()
     rows, detail = footprint(a.kernel)
