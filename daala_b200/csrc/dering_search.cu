@@ -59,9 +59,10 @@ __global__ void __launch_bounds__(256) k_pack_sb_batch(const int16_t* __restrict
 // fq (nullable): frame f's lambda is fq[f].dering_lambda.
 __global__ void k_dering_decide(const double* __restrict__ dist, int nframes, int nhdr, int nvdr, double lambda,
                                 const uint8_t* __restrict__ coded, int is_keyframe, uint8_t* __restrict__ levels,
-                                const daala_b200_kf_frame_quant* __restrict__ fq) {
+                                const daala_b200_kf_frame_quant* __restrict__ fq, const uint8_t* __restrict__ frame_type) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= nframes) return;
+  if (frame_type) is_keyframe = frame_type[f];
   if (fq) lambda = fq[f].dering_lambda;
   const int nsb = nhdr * nvdr;
   const size_t per_level = (size_t)nframes * nsb;
@@ -311,6 +312,6 @@ extern "C" int daala_b200_dering_search_enqueue(const daala_b200_dering_search_b
   const int r = enqueue_candidates(b, st);
   if (r) return r;
   k_dering_decide<<<(b->nframes + 31) / 32, 32, 0, st>>>(b->dist, b->nframes, b->nhsb, b->nvsb, b->dering_lambda,
-                                                         b->coded, b->is_keyframe, b->levels, b->fq);
+                                                         b->coded, b->is_keyframe, b->levels, b->fq, b->frame_type);
   return (int)cudaGetLastError();
 }

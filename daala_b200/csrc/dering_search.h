@@ -24,6 +24,7 @@ struct daala_b200_dering_search_batch {
   // do not adapt the CDF (src/encode.c:2724-2738)
   const uint8_t* coded;
   int is_keyframe;          // context up + left (keyframes), else 0 (src/encode.c:2753-2769)
+  const uint8_t* frame_type; // nullable [F]: frame f's is_keyframe (the engine's frame_types), replacing the field above
   // scratch / outputs (device)
   int16_t* filt;            // [F] filtered planes (same geometry as etmp, pitch = width * height)
   int32_t *orig, *cand;     // [F * nsb][64 * 64]

@@ -351,12 +351,20 @@ __device__ __forceinline__ bool rows_aligned16(const void* p, long long stride_e
 }
 
 // ---------------------------------------------------------------------------
+// Per-frame forms of the forward transform's frame-wide settings (device tables of [nframes], each nullable): haar[f]
+// replaces prm.haar_dc for frame f (the engine's batches of keyframes and P frames build the DC pyramid on keyframes
+// only), and a frame with skip[f] set is not transformed at all (the prediction planes of those batches' keyframes).
+struct FrameMasks {
+  const uint8_t* haar;
+  const uint8_t* skip;
+};
+
 // Forward kernel.  grid = (nhsb*sb_rows, nplanes, nframes).
 // ---------------------------------------------------------------------------
 template <int XDEC, bool kTma>
 __device__ __forceinline__ void forward_sb_body(const FrameXformParams& prm, const PlaneXform& pl,
                                                 int* tile_s, SbLists& lists, const CUtensorMap* map,
-                                                unsigned char* raw, uint64_t* bar) {
+                                                unsigned char* raw, uint64_t* bar, const FrameMasks& fm) {
   constexpr int B = kMaxB >> XDEC;
   constexpr int T = B + 2 * kHalo;
   // one pitch (69 = 5 mod 32) for luma AND chroma tiles: the transform / filter code is then
@@ -365,6 +373,8 @@ __device__ __forceinline__ void forward_sb_body(const FrameXformParams& prm, con
   using Sb = SbCtxT<B, P>;
   const int sbx = blockIdx.x % prm.nhsb, sby = prm.sb_row0 + blockIdx.x / prm.nhsb;
   const int fr = blockIdx.z;
+  if (fm.skip && fm.skip[fr]) return;   // the whole CTA: nothing below is written for this frame
+  const bool haar_dc = fm.haar ? fm.haar[fr] != 0 : prm.haar_dc != 0;
   Sb s;
   s.x0 = sbx * B;
   s.y0 = sby * B;
@@ -446,7 +456,7 @@ __device__ __forceinline__ void forward_sb_body(const FrameXformParams& prm, con
   }
 #endif
   transform_all_leaves<true, P>(tile, lists);
-  if (prm.haar_dc) {
+  if (haar_dc) {
 #pragma unroll 1
     for (int l = 0; l <= Sb::logB - 3; l++) {
       if (lists.nnode[l] == 0) continue;
@@ -466,19 +476,20 @@ __device__ __forceinline__ void forward_sb_body(const FrameXformParams& prm, con
 }
 
 __global__ void __launch_bounds__(kThreads, kCtasPerSm)
-k_forward_sb(const __grid_constant__ FrameXformParams prm) {
+k_forward_sb(const __grid_constant__ FrameXformParams prm, const __grid_constant__ FrameMasks fm) {
   __shared__ int tile_s[kMaxT * kMaxPitch];
   __shared__ SbLists lists;
   const PlaneXform& pl = prm.plane[blockIdx.y];
-  if (pl.xdec == 0) forward_sb_body<0, false>(prm, pl, tile_s, lists, nullptr, nullptr, nullptr);
-  else forward_sb_body<1, false>(prm, pl, tile_s, lists, nullptr, nullptr, nullptr);
+  if (pl.xdec == 0) forward_sb_body<0, false>(prm, pl, tile_s, lists, nullptr, nullptr, nullptr, fm);
+  else forward_sb_body<1, false>(prm, pl, tile_s, lists, nullptr, nullptr, nullptr, fm);
 }
 
 // Same with the input window staged by TMA (the default when the planes meet
 // the 16-byte alignment rules of tensor maps).
 __global__ void __launch_bounds__(kThreads, kCtasPerSm)
 k_forward_sb_tma(const __grid_constant__ FrameXformParams prm, const __grid_constant__ CUtensorMap map0,
-                 const __grid_constant__ CUtensorMap map1, const __grid_constant__ CUtensorMap map2) {
+                 const __grid_constant__ CUtensorMap map1, const __grid_constant__ CUtensorMap map2,
+                 const __grid_constant__ FrameMasks fm) {
   __shared__ int tile_s[kMaxT * kMaxPitch];
   __shared__ __align__(128) unsigned char raw[RawTile<0>::bytes];
   __shared__ __align__(8) uint64_t bar;
@@ -487,8 +498,8 @@ k_forward_sb_tma(const __grid_constant__ FrameXformParams prm, const __grid_cons
   // the descriptor must stay in parameter space: select between the three
   // kernel parameters, never index an array of them (that would copy to local)
   const CUtensorMap* map = blockIdx.y == 0 ? &map0 : (blockIdx.y == 1 ? &map1 : &map2);
-  if (pl.xdec == 0) forward_sb_body<0, true>(prm, pl, tile_s, lists, map, raw, &bar);
-  else forward_sb_body<1, true>(prm, pl, tile_s, lists, map, raw, &bar);
+  if (pl.xdec == 0) forward_sb_body<0, true>(prm, pl, tile_s, lists, map, raw, &bar, fm);
+  else forward_sb_body<1, true>(prm, pl, tile_s, lists, map, raw, &bar, fm);
 }
 
 // ---------------------------------------------------------------------------
@@ -801,19 +812,25 @@ static bool encode_input_maps(const FrameXformParams* prm, int nplanes, TmaMaps*
   return true;
 }
 
-int daala_b200_launch_forward(const FrameXformParams* prm, int nplanes, cudaStream_t stream) {
+int daala_b200_launch_forward_masked(const FrameXformParams* prm, int nplanes, const uint8_t* haar_frames,
+                                     const uint8_t* skip_frames, cudaStream_t stream) {
   dim3 grid(prm->nhsb * prm->sb_rows, nplanes, prm->nframes);
+  const FrameMasks fm = {haar_frames, skip_frames};
   TmaMaps maps;
   if (encode_input_maps(prm, nplanes, &maps))
-    k_forward_sb_tma<<<grid, kThreads, 0, stream>>>(*prm, maps.plane[0], maps.plane[1], maps.plane[2]);
-  else k_forward_sb<<<grid, kThreads, 0, stream>>>(*prm);
+    k_forward_sb_tma<<<grid, kThreads, 0, stream>>>(*prm, maps.plane[0], maps.plane[1], maps.plane[2], fm);
+  else k_forward_sb<<<grid, kThreads, 0, stream>>>(*prm, fm);
   return (int)cudaGetLastError();
+}
+
+int daala_b200_launch_forward(const FrameXformParams* prm, int nplanes, cudaStream_t stream) {
+  return daala_b200_launch_forward_masked(prm, nplanes, nullptr, nullptr, stream);
 }
 
 // Test hook: force the plain-load variant.
 int daala_b200_launch_forward_no_tma(const FrameXformParams* prm, int nplanes, cudaStream_t stream) {
   dim3 grid(prm->nhsb * prm->sb_rows, nplanes, prm->nframes);
-  k_forward_sb<<<grid, kThreads, 0, stream>>>(*prm);
+  k_forward_sb<<<grid, kThreads, 0, stream>>>(*prm, FrameMasks{nullptr, nullptr});
   return (int)cudaGetLastError();
 }
 

@@ -79,7 +79,7 @@ __global__ void __launch_bounds__(32) k_haar_dc(const __grid_constant__ daala_b2
   for (size_t i = threadIdx.x; i < gn; i += 32) idx[i] = 0;
   for (int i = threadIdx.x; i < kTables * 16; i += 32) cdfs[i] = ((i & 15) + 1) * 64;   // generic_model_init
   __syncwarp();
-  if (threadIdx.x != 0) return;
+  if (threadIdx.x != 0 || (B.frame_type && !B.frame_type[f])) return;
   const int ex0 = pli ? 8 : 32768;
   int ex_sb = ex0;
   int ex_dc[5][3];

@@ -20,6 +20,9 @@ struct daala_b200_haar_dc_batch {
   // each frame's band quantisers ([F][3][32], max(1, q0 * pvq_qm_q4[pli][i] >> 4) of its record); frame f's dc_quant of
   // plane p is entry [f][p][20] (od_qm_get_index(OD_NBSIZES - 1, 0))
   const int32_t* fq_bq;
+  // nullable [F]: with the engine's frame_types, 1 on keyframes; the other frames' index grids are cleared and nothing
+  // else of them is read or written
+  const uint8_t* frame_type;
 };
 
 // One warp per (frame, plane): grid F * 3.

@@ -114,6 +114,11 @@ struct Lists {
   int32_t* head_cursor;            // [kHeadBins]
   int32_t* cnt;                    // [kCntWords]
   int max_luma, max_chroma;        // capacities (blocks)
+  // config.frame_types: the step's type per frame (1 = keyframe), and the counters and dependency-free item lists of
+  // the keyframe luma chains, apart from those of the P-frame luma phase kernels.  Other engines: NULL, cnt, items_l
+  const uint8_t* ftype;
+  int32_t* kcnt;
+  uint32_t* kitems_l[3];
 };
 
 __device__ __forceinline__ int4 add4(int4 a, int4 b) { return make_int4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
@@ -201,6 +206,15 @@ __global__ void __launch_bounds__(1024) k_tile_scan(const __grid_constant__ List
     L.cnt[kNHeads] = 0;
     L.cnt[kNHeads0] = 0;
     L.cnt[kDepsDone] = 0;
+    if (L.kcnt != L.cnt) {
+      // frame_types: k_luma_deps counts the keyframe luma blocks, the band-0 items the chain kernel waits for
+      L.kcnt[kNLuma] = 0;
+      for (int c = 0; c < 3; c++) L.kcnt[kNItemsL + c] = 0;
+      L.kcnt[kTotalHi] = 0;
+      L.kcnt[kNHeads] = 0;
+      L.kcnt[kNHeads0] = 0;
+      L.kcnt[kDepsDone] = 0;
+    }
     // set on every step, so that an over-capacity batch does not flag the batches after it
     L.cnt[kError] = tot.x > L.max_luma || 2 * tot.z > L.max_chroma ? 1 : 0;
   }
@@ -340,12 +354,18 @@ __device__ __forceinline__ void scan_bins(int32_t* hist, int32_t* cursor) {
 // nothing (bands 3/6).  Per block: the two neighbours and, inverted, the blocks that wait for this one;
 // per (block, band): a dependency-free item, a chain head (ready now) or a chain link (made ready by the
 // persistent kernel when its neighbours are done).  Row / column chain heads also get the weight bin of their chain.
+// frame_types: keyframe blocks only, into the keyframe counters and lists (L.kcnt, L.kitems_l), which also count them.
+// A block's neighbours lie in its own frame, so a P-frame block is never a keyframe block's neighbour or successor.
 __global__ void __launch_bounds__(256) k_luma_deps(const __grid_constant__ Lists L) {
   const int n = min(L.cnt[kNLuma], L.max_luma);
   const int nth = gridDim.x * blockDim.x;
   for (int base = blockIdx.x * blockDim.x; base < n; base += nth) {
     const int blk = base + threadIdx.x;
-    const bool in = blk < n;
+    const bool in = blk < n && (!L.ftype || L.ftype[L.luma[blk].frame]);
+    if (L.ftype) {
+      const int nk = __popc(__ballot_sync(0xffffffffu, in));
+      if ((threadIdx.x & 31) == 0 && nk) atomicAdd(&L.kcnt[kNLuma], nk);
+    }
     int bs = 0, top = -1, left = -1;
     if (in) {
       const daala_b200_pvq_block b = L.luma[blk];
@@ -385,11 +405,11 @@ __global__ void __launch_bounds__(256) k_luma_deps(const __grid_constant__ Lists
       const bool waits = band == 0 ? (top >= 0 || left >= 0) : r == 1 ? top >= 0 : left >= 0;
       const uint32_t item = ((uint32_t)blk << 4) | band;
       if (band == 3 || band == 6) {
-        append(L.items_l[band_class(band)], &L.cnt[kNItemsL + band_class(band)], has, item);
+        append(L.kitems_l[band_class(band)], &L.kcnt[kNItemsL + band_class(band)], has, item);
       } else if (band == 0) {
-        append(L.heads0, &L.cnt[kNHeads0], has && !waits, item);
+        append(L.heads0, &L.kcnt[kNHeads0], has && !waits, item);
       } else {
-        const int pos = append(L.heads_raw, &L.cnt[kNHeads], has && !waits, item);
+        const int pos = append(L.heads_raw, &L.kcnt[kNHeads], has && !waits, item);
         if (pos >= 0) {
           const int bin = weight_bin(r == 1 ? len_down : len_across, band);
           L.head_bin[pos] = bin;
@@ -401,13 +421,13 @@ __global__ void __launch_bounds__(256) k_luma_deps(const __grid_constant__ Lists
     // total number of chain items
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) chain += __shfl_xor_sync(0xffffffffu, chain, o);
-    if ((threadIdx.x & 31) == 0 && chain) atomicAdd(&L.cnt[kTotalHi], chain);
+    if ((threadIdx.x & 31) == 0 && chain) atomicAdd(&L.kcnt[kTotalHi], chain);
   }
   // the last CTA to finish scans the weight bins of the chain heads; k_chroma_items sorts them
   __shared__ bool last;
   __threadfence();
   __syncthreads();
-  if (threadIdx.x == 0) last = atomicAdd(&L.cnt[kDepsDone], 1) == (int)gridDim.x - 1;
+  if (threadIdx.x == 0) last = atomicAdd(&L.kcnt[kDepsDone], 1) == (int)gridDim.x - 1;
   __syncthreads();
   if (last) {
     __threadfence();
@@ -418,7 +438,7 @@ __global__ void __launch_bounds__(256) k_luma_deps(const __grid_constant__ Lists
 // Chroma items: no dependencies between blocks; compaction per class (order is free).  Keyframes: first the luma
 // chain heads into `heads` by the weight bins k_luma_deps scanned, heaviest first (the order inside a bin is free).
 __global__ void __launch_bounds__(256) k_chroma_items(const __grid_constant__ Lists L) {
-  const int nh = L.cnt[kNHeads];   // 0 in inter mode
+  const int nh = L.kcnt[kNHeads];   // 0 in inter mode
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nh; i += gridDim.x * blockDim.x)
     L.heads[count_key(L.head_cursor, L.head_bin[i])] = L.heads_raw[i];
   const int n = min(L.cnt[kNChroma], L.max_chroma);
@@ -440,13 +460,14 @@ __global__ void __launch_bounds__(256) k_chroma_items(const __grid_constant__ Li
 }
 
 // Inter frames: no intra predictor, so every luma (block, band) is a dependency-free item as well; item
-// encoding and classes of k_chroma_items, in place of k_luma_deps.
+// encoding and classes of k_chroma_items, in place of k_luma_deps.  frame_types: the P-frame blocks, beside k_luma_deps.
 __global__ void __launch_bounds__(256) k_luma_items(const __grid_constant__ Lists L) {
   const int n = min(L.cnt[kNLuma], L.max_luma);
   const int nth = gridDim.x * blockDim.x;
   for (int base = blockIdx.x * blockDim.x; base < n; base += nth) {   // whole warps: append() is warp-aggregated
     const int blk = base + threadIdx.x;
-    const int nb = blk < n ? num_bands(L.luma[blk].bs) : 0;
+    const bool in = blk < n && (!L.ftype || !L.ftype[L.luma[blk].frame]);
+    const int nb = in ? num_bands(L.luma[blk].bs) : 0;
     for (int band = 0; band < 9; band++) {
       const int c = band_class(band);
       append(L.items_l[c], &L.cnt[kNItemsL + c], band < nb, ((uint32_t)blk << 4) | band);
@@ -492,6 +513,9 @@ struct Stage {
   // [F][3][32] each frame's band quantisers max(1, q0 * pvq_qm_q4[pli][i] >> 4), filled on the host from the records
   // (one load per item)
   const int32_t* fq_bq;
+  // config.frame_types: the step's type per frame (1 = keyframe); the phase kernels, gather and scatter then take the
+  // block's kind from its frame (the chain kernel's items are all keyframe items and read prm.is_keyframe); else NULL
+  const uint8_t* ftype;
 #ifdef DAALA_B200_CHAIN_TRACE
   struct ChainTraceRec* trace;     // luma: one record per item k_pvq_persist runs, up to trace_cap
   int trace_cap;
@@ -584,8 +608,10 @@ __device__ __forceinline__ int32_t cfl_ref(const Stage& S, const daala_b200_pvq_
 // raster -> coding order of every block (od_raster_to_coding_order, src/partition.c:123); keyframe chroma:
 // also the CfL prediction and its sign flip (src/pvq_encoder.c:847-871); inter frames, all planes alike: the
 // reference vector is the transformed prediction md (prm.pred_plane), never flipped.  One warp per block.
+// kMixed (config.frame_types): kKind on keyframe blocks, kGatherInter on the others, chosen per warp from the block's
+// frame; a P-frame chroma block's flip is 0.
 enum { kGatherLuma = 0, kGatherChroma = 1, kGatherInter = 2 };
-template <int kKind, bool kHdc = false>
+template <int kKind, bool kHdc = false, bool kMixed = false>
 __global__ void __launch_bounds__(256) k_gather(const __grid_constant__ Stage S) {
   const daala_b200_pvq_params& prm = S.prm;
   const int n = min(S.cnt[S.n_blocks_at], S.max_blocks);
@@ -593,14 +619,15 @@ __global__ void __launch_bounds__(256) k_gather(const __grid_constant__ Stage S)
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int blk = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; blk < n; blk += nwarps) {
     const daala_b200_pvq_block b = prm.blocks[blk];
+    const int kind = kMixed && !S.ftype[b.frame] ? kGatherInter : kKind;
     const int ln = b.bs + 2;
     const int len = ln >= 5 ? 512 : 1 << (2 * ln);
     const int stride = prm.plane_stride[b.pli];
     const int32_t* src = prm.coef_plane[b.pli] + b.frame * prm.plane_frame_pitch[b.pli] + (size_t)b.y0 * stride + b.x0;
     int32_t* vin = prm.in + b.coef_off;
-    if (kKind == kGatherLuma) {
+    if (kind == kGatherLuma) {
       for (int i = lane; i < len; i += 32) vin[i] = i == 0 ? src[0] : src[scan_to_raster(i, ln, stride)];
-    } else if (kKind == kGatherInter) {
+    } else if (kind == kGatherInter) {
       const int32_t* psrc = prm.pred_plane[b.pli] + b.frame * prm.plane_frame_pitch[b.pli] + (size_t)b.y0 * stride + b.x0;
       int32_t* vref = prm.ref + b.coef_off;
       for (int i = lane; i < len; i += 32) {
@@ -608,6 +635,7 @@ __global__ void __launch_bounds__(256) k_gather(const __grid_constant__ Stage S)
         vin[i] = src[at];
         vref[i] = psrc[at];
       }
+      if (kMixed && kKind == kGatherChroma && lane == 0) prm.res_flip[blk] = 0;
     } else {
       // the co-located luma at (2 x0, 2 y0): the unit of the block's origin (4x4 chroma samples) has its offset
       const int lo = S.cfl_loff[b.frame * (prm.plane_frame_pitch[b.pli] >> 4) + (long long)(b.y0 >> 2) * (stride >> 2) +
@@ -798,7 +826,7 @@ __device__ __forceinline__ void run_item(const Stage& S, uint32_t item, int lane
 // time on the whole GPU keeps the resident code small.  Only items without dependencies can go this way
 // (keyframe chroma, every band of an inter frame); keyframe luma stays in the persistent kernel.
 struct ItemGeom {
-  int blk, band, bn, q, beta, pli, qoff;
+  int blk, band, bn, q, beta, pli, qoff, is_keyframe;
   size_t off;
 };
 __device__ __forceinline__ ItemGeom item_geom(const Stage& S, uint32_t item) {
@@ -816,6 +844,7 @@ __device__ __forceinline__ ItemGeom item_geom(const Stage& S, uint32_t item) {
   g.q = S.fq_bq[(b.frame * 3 + g.pli) * 32 + qidx];
   g.beta = (prm.use_masking && g.pli == 0 && bs > 0) ? kBeta15 : kBeta1;
   g.qoff = (b.xdec & 1 ? prm.qm_stride : 0) + ((((1 << (2 * bs)) - 1) << 4) / 3) + start;
+  g.is_keyframe = S.ftype ? S.ftype[b.frame] : prm.is_keyframe;
   return g;
 }
 
@@ -838,7 +867,7 @@ __global__ void __launch_bounds__(128) k_pvq_split(const __grid_constant__ Stage
     const int32_t* r0 = prm.ref + g.off;
     BandCtx B;
     if (kPhase == 0) {
-      band_setup<kMode>(lane, B, prm.in + g.off, r0, g.bn, g.q, g.beta, prm.is_keyframe, g.pli, prm.qm + g.qoff,
+      band_setup<kMode>(lane, B, prm.in + g.off, r0, g.bn, g.q, g.beta, g.is_keyframe, g.pli, prm.qm + g.qoff,
                  prm.pvq_norm_lambda, S.rsqrt_tbl);
       band_ctx_store_setup(lane, B, g.bn, vec, vs, lanes, uni);
     } else if (kPhase == 1) {
@@ -850,7 +879,7 @@ __global__ void __launch_bounds__(128) k_pvq_split(const __grid_constant__ Stage
       int itheta, max_theta, k;
       double skip_term;
       const int gain = band_finish<kMode>(lane, B, snap, vs, prm.out + g.off, r0, g.bn, g.q, prm.y + g.off, &itheta, &max_theta, &k,
-                                   g.beta, &skip_term, prm.is_keyframe, g.pli, prm.qm_inv + g.qoff, prm.pvq_norm_lambda);
+                                   g.beta, &skip_term, g.is_keyframe, g.pli, prm.qm_inv + g.qoff, prm.pvq_norm_lambda);
       if (lane == 0) {
         const size_t r = (size_t)g.blk * 9 + g.band;
         prm.res_skip_term[r] = skip_term;
@@ -932,8 +961,13 @@ __global__ void k_fill_rsqrt(double* tbl) {
 
 // Start of the PVQ stages in `stages` (kBeginLuma | kBeginChroma): the tickets; the chain queue starts with the
 // heads.  Neither stage touches the other's tickets, so the whole step starts both at once.
+// ring (frame_types, else NULL): a step without keyframe luma blocks has no band-0 item whose completion would release
+// the chain kernel's parked warps, so their slots [0, nwarps] are released (kExit) from the start, as the last band-0
+// item does on a step with keyframes.
 enum { kBeginLuma = 1, kBeginChroma = 2 };
-__global__ void k_begin_pvq(int32_t* cnt, int stages) {
+__global__ void k_begin_pvq(int32_t* cnt, int stages, uint32_t* ring = nullptr, int nwarps = 0) {
+  if (ring && cnt[kNLuma] == 0)
+    for (int i = threadIdx.x; i <= nwarps; i += blockDim.x) ring[i] = kExit;
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     if (stages & kBeginLuma) {
       cnt[kHeadLoL] = 0;
@@ -959,7 +993,9 @@ __global__ void k_begin_pvq(int32_t* cnt, int stages) {
 // transformed prediction (od_init_skipped_coeffs for inter frames).
 // kHdc (keyframes with config.haar_dc_quant): the DC is the quantised one the DC chain left in its grid, into out[0]
 // and the coefficient plane.
-template <bool kInter, bool kHdc = false>
+// kMixed (config.frame_types): per warp from the block's frame, keyframe blocks as <false, true> and the others as
+// <true>; a keyframe block's DC index and residual are 0.
+template <bool kInter, bool kHdc = false, bool kMixed = false>
 __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ Stage S) {
   const daala_b200_pvq_params& prm = S.prm;
   const int n = min(S.cnt[S.n_blocks_at], S.max_blocks);
@@ -967,6 +1003,8 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int blk = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; blk < n; blk += nwarps) {
     const daala_b200_pvq_block b = prm.blocks[blk];
+    const bool key = kMixed && S.ftype[b.frame];
+    const bool inter = kMixed ? !key : kInter, hdc = kMixed ? key : kHdc;
     const int ln = b.bs + 2, nn = 1 << ln;
     const int len = ln >= 5 ? 512 : 1 << (2 * ln);
     const int stride = prm.plane_stride[b.pli];
@@ -977,9 +1015,13 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
       double sd = 0;
       for (int i = 0; i < nb; i++) sd += prm.res_skip_term[(size_t)blk * 9 + i];
       prm.res_skip_diff[blk] = sd;
-      if (kHdc) {
+      if (hdc) {
         prm.out[b.coef_off] = dst[0] = hdc_grid(S, b.frame, b.pli)[(long long)(b.y0 >> 2) * (stride >> 2) + (b.x0 >> 2)];
-      } else if (!kInter) {
+        if (kMixed) {
+          prm.res_dc[blk] = 0;
+          if (S.dc_resid) S.dc_resid[blk] = 0;
+        }
+      } else if (!inter) {
         prm.out[b.coef_off] = prm.in[b.coef_off];
       } else {
         const int dc_quant = S.fq_bq[(b.frame * 3 + b.pli) * 32 + b.bs * (b.bs + 1)];
@@ -995,11 +1037,11 @@ __global__ void __launch_bounds__(256) k_finish_scatter(const __grid_constant__ 
       }
     }
     if (ln >= 5) {
-      const int32_t* mdp = kInter ? prm.pred_plane[b.pli] + b.frame * prm.plane_frame_pitch[b.pli] + (size_t)b.y0 * stride + b.x0
-                                  : nullptr;
+      const int32_t* mdp = inter ? prm.pred_plane[b.pli] + b.frame * prm.plane_frame_pitch[b.pli] + (size_t)b.y0 * stride + b.x0
+                                 : nullptr;
       for (int i = lane; i < nn * nn; i += 32) {
         const size_t at = (size_t)(i >> ln) * stride + (i & (nn - 1));
-        if (i) dst[at] = kInter ? mdp[at] : 0;
+        if (i) dst[at] = inter ? mdp[at] : 0;
       }
       __syncwarp();
     }
@@ -1053,6 +1095,7 @@ struct Fin {
   uint8_t* coded;                          // [F][nvsb][nhsb]: a luma 4x4 unit of the superblock is coded (preset 0)
   int nhsb, nvsb;
   const int32_t* fq_bq;                    // [F][3][32] each frame's band quantisers (Stage::fq_bq)
+  const uint8_t* ftype;                    // config.frame_types: 1 on keyframes, whose decisions are not read; else NULL
 };
 
 // block i of the two lists together (luma first), or false past their end
@@ -1066,7 +1109,8 @@ __device__ __forceinline__ bool fin_block(const Fin& P, int i, int* list, int* b
 
 // One warp per block.  skip = 0: the step's coefficients; skip = 1: md over the whole block (AC = prediction,
 // src/pvq_encoder.c:975; the late skip's d = md, src/encode.c:1444-1448); either way DC = md[0] + dc * dc_quant
-// (src/encode.c:1373-1374 with the band-0 quantiser of :1333-1334).
+// (src/encode.c:1373-1374 with the band-0 quantiser of :1333-1334).  A keyframe block (frame_types) keeps the step's
+// coefficients, its quantised DC included.
 __global__ void __launch_bounds__(256) k_fin_patch(const __grid_constant__ Fin P) {
   const int lane = threadIdx.x & 31;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -1079,6 +1123,13 @@ __global__ void __launch_bounds__(256) k_fin_patch(const __grid_constant__ Fin P
     const int32_t* src = (P.skip[list][blk] ? P.md[b.pli] : P.d[b.pli]) + o;
     const int32_t* mdp = P.md[b.pli] + o;
     int32_t* dst = P.out[b.pli] + o;
+    if (P.ftype && P.ftype[b.frame]) {
+      for (int k = lane; k < nn * nn; k += 32) {
+        const size_t at = (size_t)(k >> ln) * stride + (k & (nn - 1));
+        dst[at] = P.d[b.pli][o + at];
+      }
+      continue;
+    }
     const int dc_quant = P.fq_bq[(b.frame * 3 + b.pli) * 32 + b.bs * (b.bs + 1)];
     const int32_t dc0 = mdp[0] + P.dc[list][blk] * dc_quant;
     for (int k = lane; k < nn * nn; k += 32) {
@@ -1089,14 +1140,15 @@ __global__ void __launch_bounds__(256) k_fin_patch(const __grid_constant__ Fin P
 }
 
 // One warp per block: bskip = skip && dc == 0 over the block's 4x4 units (src/encode.c:1690-1691, :1821-1825), and
-// the coded flag of the superblock of a luma block that is not skipped.
+// the coded flag of the superblock of a luma block that is not skipped.  Keyframe blocks (frame_types) are never
+// skipped (skip && !is_keyframe, src/encode.c:1691, :1824).
 __global__ void __launch_bounds__(256) k_fin_skip_map(const __grid_constant__ Fin P) {
   const int lane = threadIdx.x & 31;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   int list, blk;
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; fin_block(P, i, &list, &blk); i += nwarps) {
     const daala_b200_pvq_block b = P.blocks[list][blk];
-    const uint8_t s = P.skip[list][blk] && P.dc[list][blk] == 0;
+    const uint8_t s = P.skip[list][blk] && P.dc[list][blk] == 0 && !(P.ftype && P.ftype[b.frame]);
     const int nu = 1 << b.bs;   // 4x4 units per side
     uint8_t* m = P.bskip[b.pli] + b.frame * P.skip_pitch[b.pli] + (size_t)(b.y0 >> 2) * P.skip_stride + (b.x0 >> 2);
     for (int k = lane; k < nu * nu; k += 32) m[(size_t)(k >> b.bs) * P.skip_stride + (k & (nu - 1))] = s;
@@ -1573,6 +1625,8 @@ __global__ void __launch_bounds__(256) k_fin_unstream(const __grid_constant__ Un
 using namespace daala_b200::kf;
 
 extern "C" int daala_b200_launch_forward(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
+extern "C" int daala_b200_launch_forward_masked(const daala_b200_frame* prm, int nplanes, const uint8_t* haar_frames,
+                                                const uint8_t* skip_frames, cudaStream_t stream);
 extern "C" int daala_b200_launch_inverse(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
 extern "C" int daala_b200_launch_inverse_lapped_only(const daala_b200_frame* prm, int plane0, int nplanes,
                                                      cudaStream_t stream);
@@ -1597,8 +1651,8 @@ struct Dering {
   daala_b200_dering_search_batch sb;
 };
 
-// The events of kf_enqueue_step_forked, one per fork or join.
-enum { kEvLists, kEvForward, kEvLumaBands, kEvLumaScatter, kEvChroma, kEvHaarDc, kNumEvents };
+// The events of kf_enqueue_step_forked and kf_enqueue_step_mixed, one per fork or join.
+enum { kEvLists, kEvForward, kEvLumaBands, kEvLumaScatter, kEvChroma, kEvHaarDc, kEvLumaGather, kEvInterLuma, kNumEvents };
 
 struct daala_b200_kf {
   daala_b200_kf_config cfg;
@@ -1629,6 +1683,11 @@ struct daala_b200_kf {
   Dering dering;                   // cfg.dering or cfg.inter_finish
   Lists lists;
   Stage luma, chroma;
+  // cfg.frame_types: the step's type per frame on the device ([F], 1 = keyframe), and the luma stage of the keyframe
+  // chains (kf->luma with the keyframe counters and item lists, is_keyframe = 1) beside kf->luma, which then runs the
+  // P-frame luma bands
+  uint8_t* ftype;
+  Stage luma_kf;
   Sym sym;                         // symbol stream (cfg.symbol_stream); zero otherwise
   daala_b200_frame frame;
   daala_b200_frame frame_fwd;      // keyframes: `frame` for the forward transform, which always builds the DC pyramid
@@ -1838,6 +1897,9 @@ static int kf_alloc(daala_b200_kf* kf) {
   if (kf->cfg.lossless) return ll_alloc(kf);
   const int F = kf->F;
   const bool inter = kf->cfg.inter != 0;
+  // frame_types: an inter engine that also has everything the keyframe chains, CfL and the DC chain need
+  const bool mixed = kf->cfg.frame_types != 0;
+  if (mixed) KF_CHECK(dalloc(kf, &kf->ftype, (size_t)F));
   const long long luma_px = (long long)kf->plane_w[0] * kf->plane_h[0];
   for (int p = 0; p < 3; p++) {
     const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
@@ -1855,6 +1917,7 @@ static int kf_alloc(daala_b200_kf* kf) {
   if (kf->cfg.inter_mc) {
     const int rc = mc_alloc(kf);
     if (rc) return rc;
+    kf->mc.frame_type = kf->ftype;
   }
   KF_CHECK(dalloc(kf, &kf->fq, (size_t)F));
   KF_CHECK(dalloc(kf, &kf->fq_tbl, (size_t)F * 12));
@@ -1886,11 +1949,12 @@ static int kf_alloc(daala_b200_kf* kf) {
   L.max_chroma = (int)(nunits * 2 / div) + 64;
   KF_CHECK(dalloc(kf, &L.tile_sum, (size_t)L.ntiles));
   KF_CHECK(dalloc(kf, &L.unit_lbase, (size_t)F * UW * UH));
-  if (!inter) KF_CHECK(dalloc(kf, &L.unit_loff, (size_t)F * UW * UH));
+  if (!inter || mixed) KF_CHECK(dalloc(kf, &L.unit_loff, (size_t)F * UW * UH));
   KF_CHECK(dalloc(kf, &L.luma, (size_t)L.max_luma));
   KF_CHECK(dalloc(kf, &L.chroma, (size_t)L.max_chroma));
   // the intra dependency structure (neighbours, chain heads, ring) is a keyframe matter
-  const size_t ndep = inter ? 0 : (size_t)L.max_luma;
+  const size_t ndep = inter && !mixed ? 0 : (size_t)L.max_luma;
+  const bool chains = ndep != 0;
   KF_CHECK(dalloc(kf, &L.dep_top, ndep));
   KF_CHECK(dalloc(kf, &L.dep_left, ndep));
   KF_CHECK(dalloc(kf, &L.succ_bottom, ndep));
@@ -1907,7 +1971,11 @@ static int kf_alloc(daala_b200_kf* kf) {
   for (int c = 0; c < 3; c++) {
     KF_CHECK(dalloc(kf, &L.items_l[c], cap_l[c]));
     KF_CHECK(dalloc(kf, &L.items_c[c], cap_c[c]));
+    L.kitems_l[c] = L.items_l[c];
   }
+  // frame_types: the keyframe chains' bands 3 / 6, at the capacities of a keyframe engine
+  const size_t cap_k[3] = {64, cap_l[1], cap_l[2]};
+  for (int c = 0; mixed && c < 3; c++) KF_CHECK(dalloc(kf, &L.kitems_l[c], cap_k[c]));
   {
     // context records of one chunk of items per class (pvq_warp.cuh: band_ctx_*)
     const int slots[3] = {1 << 19, 1 << 19, 3 << 15};
@@ -1933,13 +2001,16 @@ static int kf_alloc(daala_b200_kf* kf) {
       return (int)cudaErrorLaunchOutOfResources;
     }
   }
-  KF_CHECK(dalloc(kf, &L.heads, inter ? 0 : kf->chain_cap));
-  KF_CHECK(dalloc(kf, &L.heads_raw, inter ? 0 : kf->chain_cap));
-  KF_CHECK(dalloc(kf, &L.head_bin, inter ? 0 : kf->chain_cap));
-  KF_CHECK(dalloc(kf, &L.head_hist, inter ? 0 : (size_t)kHeadBins));
-  KF_CHECK(dalloc(kf, &L.head_cursor, inter ? 0 : (size_t)kHeadBins));
+  KF_CHECK(dalloc(kf, &L.heads, chains ? kf->chain_cap : 0));
+  KF_CHECK(dalloc(kf, &L.heads_raw, chains ? kf->chain_cap : 0));
+  KF_CHECK(dalloc(kf, &L.head_bin, chains ? kf->chain_cap : 0));
+  KF_CHECK(dalloc(kf, &L.head_hist, chains ? (size_t)kHeadBins : 0));
+  KF_CHECK(dalloc(kf, &L.head_cursor, chains ? (size_t)kHeadBins : 0));
   KF_CHECK(dalloc(kf, &L.heads0, ndep));
   KF_CHECK(dalloc(kf, &L.cnt, (size_t)kCntWords));
+  L.kcnt = L.cnt;
+  if (mixed) KF_CHECK(dalloc(kf, &L.kcnt, (size_t)kCntWords));
+  L.ftype = kf->ftype;
   kf->mc.bad_ref = L.cnt + kMcBadRef;
   kf->mc.beyond = L.cnt + kMcBeyond;
 
@@ -2004,7 +2075,7 @@ static int kf_alloc(daala_b200_kf* kf) {
       S.succ_right = L.succ_right;
       S.heads = L.heads;
       S.heads0 = L.heads0;
-      KF_CHECK(dalloc(kf, &S.ring, inter ? 0 : kf->chain_cap));
+      KF_CHECK(dalloc(kf, &S.ring, chains ? kf->chain_cap : 0));
       KF_CHECK(dalloc(kf, &S.join0, ndep));
     }
     return 0;
@@ -2013,7 +2084,8 @@ static int kf_alloc(daala_b200_kf* kf) {
   if (rc) return rc;
   rc = setup_stage(kf->chroma, true);
   if (rc) return rc;
-  if (!inter) {
+  kf->luma.ftype = kf->chroma.ftype = kf->ftype;
+  if (!inter || mixed) {
     Stage& C = kf->chroma;
     C.cfl_in = kf->luma.prm.in;
     C.cfl_out = kf->luma.prm.out;
@@ -2040,6 +2112,16 @@ static int kf_alloc(daala_b200_kf* kf) {
     H.nvsb = kf->nvsb;
     H.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
     H.fq_bq = kf->fq_bq;
+    H.frame_type = kf->ftype;
+  }
+  if (mixed) {
+    // the chain kernel walks the keyframe luma items; its Stage reads no frame type
+    Stage& K = kf->luma_kf;
+    K = kf->luma;
+    K.prm.is_keyframe = 1;
+    K.cnt = L.kcnt;
+    for (int c = 0; c < 3; c++) K.items[c] = L.kitems_l[c];
+    K.ftype = nullptr;
   }
   (void)luma_px;
   // the unquantised DC residual per block: what the host's od_rdo_quant needs, returned classically (inter_finish) or
@@ -2208,6 +2290,7 @@ static int kf_alloc(daala_b200_kf* kf) {
     P.nhsb = kf->nhsb;
     P.nvsb = kf->nvsb;
     P.fq_bq = kf->fq_bq;
+    P.ftype = kf->ftype;
     if (kf->cfg.inter_mc) {
       KF_CHECK(dalloc(kf, &kf->fin_slot_out, (size_t)F));
       PoolStore& W = kf->store;
@@ -2282,6 +2365,7 @@ static int kf_alloc(daala_b200_kf* kf) {
       b.skip_pitch = D.skip_pitch[0];
       b.coded = D.coded;
       b.is_keyframe = inter ? 0 : 1;
+      b.frame_type = kf->ftype;   // frame_types: the keyframe rule (up / left context) on keyframes
       KF_CHECK(dalloc(kf, &b.filt, (size_t)kf->plane_w[0] * kf->plane_h[0] * F));
       KF_CHECK(dalloc(kf, &b.orig, nsb * 4096));
       KF_CHECK(dalloc(kf, &b.cand, nsb * 4096));
@@ -2560,6 +2644,76 @@ static int kf_enqueue_step_forked(daala_b200_kf* kf) {
   return (int)cudaGetLastError();
 }
 
+// config.frame_types: keyframes and P / B frames in one step, as two branches (kf->stream and kf->side) forked and joined
+// with events:
+//   kf->side: [inter_mc: the P / B frames' leaves and OBMC], the source transform (DC pyramid on keyframes only), the
+//             prediction's transform (P / B frames only);  kf->stream: the work lists (keyframe luma through
+//             k_luma_deps, P-frame luma through k_luma_items, chroma of both kinds through k_chroma_items); join;
+//   kf->side: the keyframes' DC chain;  kf->stream: the chain tickets and the luma gather (per block by its kind); fork;
+//   kf->stream: the keyframe luma chains (k_pvq_persist);  kf->side: the P-frame luma bands through the phase kernels
+//             beside them, on the SMs the chains leave idle;
+//   kf->side, after the chains: the chroma stage (gather per block by its kind: CfL from the coded luma or md), scatter,
+//             inverse + SB postfilter of planes 1-2;  kf->stream, after the P-frame luma bands and the DC chain: the
+//             luma scatter, inverse + SB postfilter of plane 0; join.
+static int kf_enqueue_step_mixed(daala_b200_kf* kf, int phases) {
+  if (phases != DAALA_B200_KF_ALL) {
+    snprintf(kf->err, sizeof(kf->err), "a frame_types step runs whole (DAALA_B200_KF_ALL)");
+    return (int)cudaErrorInvalidValue;
+  }
+  cudaStream_t s = kf->stream, c = kf->side;
+  const Lists& L = kf->lists;
+  const int wide = kf->sms * 8;
+  auto fork = [](cudaEvent_t e, cudaStream_t from, cudaStream_t to) {
+    return cudaEventRecord(e, from) == cudaSuccess && cudaStreamWaitEvent(to, e, 0) == cudaSuccess;
+  };
+  if (!fork(kf->ev[kEvLists], s, c)) return (int)cudaGetLastError();
+  int rc = 0;
+  if (kf->cfg.inter_mc) {
+    if (cudaMemsetAsync(L.cnt + kMcBadRef, 0, 2 * sizeof(int32_t), c) != cudaSuccess) return (int)cudaGetLastError();
+    rc = daala_b200_launch_mc_leaves(&kf->mc, wide, c);
+    if (!rc) rc = daala_b200_launch_mc_obmc(&kf->mc, wide, c);
+  }
+  if (!rc) rc = daala_b200_launch_forward_masked(&kf->frame_fwd, 3, kf->ftype, nullptr, c);
+  if (!rc) rc = daala_b200_launch_forward_masked(&kf->frame_pred, 3, nullptr, kf->ftype, c);
+  if (rc) return rc;
+  k_unit_tile_sums<<<L.ntiles, kTile, 0, s>>>(L);
+  k_tile_scan<<<1, 1024, 0, s>>>(L);
+  k_unit_emit<<<L.ntiles, kTile, 0, s>>>(L);
+  const size_t nl = (size_t)L.max_luma * sizeof(int32_t);
+  if (cudaMemsetAsync(L.succ_bottom, 0xff, nl, s) != cudaSuccess || cudaMemsetAsync(L.succ_right, 0xff, nl, s) != cudaSuccess ||
+      cudaMemsetAsync(L.head_hist, 0, sizeof(int32_t) * kHeadBins, s) != cudaSuccess)
+    return (int)cudaGetLastError();
+  k_luma_deps<<<wide, 256, 0, s>>>(L);
+  k_luma_items<<<wide, 256, 0, s>>>(L);
+  k_chroma_items<<<wide, 256, 0, s>>>(L);
+  if (!fork(kf->ev[kEvForward], c, s)) return (int)cudaGetLastError();
+  rc = daala_b200_launch_haar_dc(&kf->hdcb, c);
+  if (rc) return rc;
+  const Stage& K = kf->luma_kf;
+  if (cudaMemsetAsync(K.ring, 0xff, kf->chain_cap * sizeof(uint32_t), s) != cudaSuccess ||
+      cudaMemsetAsync(K.join0, 0, (size_t)K.max_blocks * sizeof(int32_t), s) != cudaSuccess)
+    return (int)cudaGetLastError();
+  const int persist = kf->sms * (kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas);
+  k_begin_pvq<<<1, 256, 0, s>>>(L.kcnt, kBeginLuma, K.ring, persist * kPersistThreads / 32);
+  k_gather<kGatherLuma, false, true><<<wide, 256, 0, s>>>(kf->luma);
+  if (!fork(kf->ev[kEvLumaGather], s, c)) return (int)cudaGetLastError();
+  k_pvq_persist<<<persist, kPersistThreads, 0, s>>>(K);
+  enqueue_split(kf, kf->luma, c);
+  if (cudaEventRecord(kf->ev[kEvInterLuma], c) != cudaSuccess) return (int)cudaGetLastError();
+  if (!fork(kf->ev[kEvLumaBands], s, c)) return (int)cudaGetLastError();
+  k_gather<kGatherChroma, true, true><<<wide, 256, 0, c>>>(kf->chroma);
+  enqueue_split(kf, kf->chroma, c);
+  k_finish_scatter<false, true, true><<<wide, 256, 0, c>>>(kf->chroma);
+  rc = enqueue_recon(kf->frame, 1, 2, c);
+  if (rc) return rc;
+  if (cudaStreamWaitEvent(s, kf->ev[kEvInterLuma], 0) != cudaSuccess) return (int)cudaGetLastError();
+  k_finish_scatter<false, true, true><<<wide, 256, 0, s>>>(kf->luma);
+  rc = enqueue_recon(kf->frame, 0, 1, s);
+  if (rc) return rc;
+  if (!fork(kf->ev[kEvChroma], c, s)) return (int)cudaGetLastError();
+  return (int)cudaGetLastError();
+}
+
 // config.lossless: the whole step, one phase.  [inter_mc: leaf enumeration and OBMC, unchanged], the lossless kernels.
 static int kf_enqueue_step_lossless(daala_b200_kf* kf, int phases) {
   if (phases != DAALA_B200_KF_ALL) {
@@ -2580,6 +2734,7 @@ static int kf_enqueue_step_lossless(daala_b200_kf* kf, int phases) {
 // One step on kf->stream phase by phase (a partial phase mask: per-phase timings), or the whole step forked.
 static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
   if (kf->cfg.lossless) return kf_enqueue_step_lossless(kf, phases);
+  if (kf->cfg.frame_types) return kf_enqueue_step_mixed(kf, phases);
   if (kf->cfg.inter) return kf_enqueue_step_inter(kf, phases);
   if (phases == DAALA_B200_KF_ALL) return kf_enqueue_step_forked(kf);
   cudaStream_t s = kf->stream;
@@ -2636,6 +2791,24 @@ static thread_local char g_create_err[256] = "null engine";
 
 daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: invalid configuration");
+  if (cfg && cfg->frame_types) {
+    // the mixed step is the keyframe path of keyframe_quant + haar_dc_quant beside the P-frame path of frame_quant, with
+    // keyframe deringing in the finishing pass; the stages below have no mixed form
+    const char* why = cfg->frame_types != 1 ? "frame_types is 0 or 1"
+                      : cfg->inter != 1 || cfg->frame_quant != 1 || cfg->haar_dc_quant != 1 ||
+                                (cfg->inter_finish != 1 && cfg->inter_finish != 2)
+                          ? "frame_types = 1 requires inter = 1, frame_quant = 1, haar_dc_quant = 1 and inter_finish 1 or 2"
+                      : cfg->symbol_stream ? "frame_types is not defined with symbol_stream (keyframes and P frames have "
+                                             "streams of different formats)"
+                      : cfg->late_skip ? "frame_types is not defined with late_skip"
+                      : cfg->lossless ? "frame_types is not defined with lossless"
+                      : cfg->dering ? "frame_types is not defined with dering (keyframes are deringed in the finishing pass)"
+                      : cfg->sb_rows > 0 ? "frame_types is not defined with a row shard (sb_rows > 0)" : nullptr;
+    if (why) {
+      snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: %s", why);
+      return nullptr;
+    }
+  }
   if (cfg && cfg->inter_mc && (cfg->inter_mc != 1 || cfg->inter != 1)) {
     snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: inter_mc is 0 or 1, and 1 requires inter = 1");
     return nullptr;
@@ -2694,7 +2867,7 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
     // the chain quantises the Haar DC pyramid of lossy keyframes; the superblock predictor reads the superblocks above,
     // across any row shard
     const char* with = cfg->haar_dc_quant != 1 ? "a value other than 0 or 1"
-                       : cfg->inter ? "inter (P and B frames code a scalar DC per block)"
+                       : cfg->inter && !cfg->frame_types ? "inter (P and B frames code a scalar DC per block)"
                        : cfg->lossless ? "lossless (its keyframe DCs are coded exactly)"
                        : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
     if (with) {
@@ -2766,7 +2939,7 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
     }
     kf->own_stream = true;
   }
-  if (!cfg->inter && !cfg->lossless) {
+  if ((!cfg->inter && !cfg->lossless) || cfg->frame_types) {
     // the side branch carries the longer chain (the chroma stage) at the highest priority: the luma branch's CTAs
     // then take the SMs the chroma kernels leave idle instead of delaying them
     int least = 0, greatest = 0;
@@ -2823,6 +2996,10 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   // lossless: [leaves + OBMC], the forward kernel, [keyframes: the DC + reconstruction kernel]
   if (kf->cfg.lossless) return (kf->cfg.inter_mc ? 2 : 0) + (kf->cfg.inter ? 1 : 2);
   auto split = [](const Stage& S) { return 3 * (S.sp_chunks[0] + S.sp_chunks[1] + S.sp_chunks[2]); };
+  // frame_types: work lists (6), [leaves + OBMC], two forward launches, DC chain, begin, luma gather, chains, P-frame luma
+  // phase kernels, luma scatter, chroma gather + phase kernels + scatter, inverse + SB postfilter of plane 0 and 1-2
+  if (kf->cfg.frame_types)
+    return 6 + (kf->cfg.inter_mc ? 2 : 0) + 2 + 1 + 1 + 1 + 1 + split(kf->luma) + 1 + (2 + split(kf->chroma)) + 4;
   // inter: work lists, two forward launches, per stage gather + phase kernels + finish, inverse + SB postfilter;
   // inter_mc: leaf enumeration and OBMC
   // [symbol_stream = 2: the 8 stream kernels]; [late_skip: the size-class split and one launch per class]
@@ -3054,6 +3231,16 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", ll_why);
     return (int)cudaErrorInvalidValue;
   }
+  // frame_types: a type per frame, 1 (keyframe) or 0 (P or B frame); refused by the other engines
+  const char* ft_why = !kf->cfg.frame_types ? (io->frame_type ? "frame_type needs an engine with frame_types = 1" : nullptr)
+                       : !io->frame_type ? "frame_types: frame_type ([nframes], 1 = keyframe, 0 = P or B frame) is required"
+                                         : nullptr;
+  for (int f = 0; !ft_why && kf->cfg.frame_types && f < F; f++)
+    if (io->frame_type[f] > 1) ft_why = "frame_types: a frame_type entry is neither 0 nor 1";
+  if (ft_why) {
+    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", ft_why);
+    return (int)cudaErrorInvalidValue;
+  }
   if ((io->dc_index[0] || io->dc_index[1] || io->dc_index[2]) && !kf->cfg.haar_dc_quant) {
     snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: dc_index needs an engine with haar_dc_quant = 1");
     return (int)cudaErrorInvalidValue;
@@ -3093,6 +3280,7 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     for (int i = 0; !why && i < nslot; i++) {
       const int32_t r = i < 2 * F ? io->ref_slot[i] : io->ref_slot_next[i - 2 * F];
       in_next = i >= 2 * F;
+      if (kf->cfg.frame_types && io->frame_type[i < 2 * F ? i / 2 : i - 2 * F]) continue;   // a keyframe reads no picture
       if (!resident && (r < 0 || r >= io->nrefs)) why = "a ref_slot entry is outside [0, nrefs)";
       else if (resident && (r < 0 || r >= kf->cfg.mc_refs)) why = "ref_resident: a ref_slot entry is outside [0, mc_refs)";
       else if (resident && !kf->slot_filled[r])
@@ -3216,6 +3404,7 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     }
   }
   if (fq_mode) KF_CHECK(fq_copy(kf, io->frame_quant, s));
+  if (kf->cfg.frame_types) KF_CHECK(cudaMemcpyAsync(kf->ftype, io->frame_type, (size_t)F, cudaMemcpyHostToDevice, s));
   const size_t map_bytes = (size_t)kf->nhsb * 8 * kf->nvsb * 8 * F;
   if (!lossless) KF_CHECK(cudaMemcpyAsync(kf->bsize, io->bsize, map_bytes, cudaMemcpyHostToDevice, s));
   // the graph's lossless kernels read the slot table: NULL stores nothing (every entry -1)

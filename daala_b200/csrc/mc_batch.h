@@ -23,6 +23,8 @@ struct daala_b200_mc_batch {
   // picture with its second vector mv1 (od_state_pred_block_from_setup, reference src/state.c:647-660)
   const int32_t* ref_slot_next;    // [F]: pool slot of OD_FRAME_NEXT
   const int32_t* mv1;              // [F][nvsb*8 + 1][nhsb*8 + 1][2]: each vertex's mv1 in 1/8 luma pixel
+  // nullable [F]: the engine's frame_types, 1 on keyframes, which have no leaves and a prediction of 0
+  const uint8_t* frame_type;
 };
 
 // od_state_pred_block's split recursion for every (frame, 64x64 MV block): its leaves and both counters.

@@ -474,6 +474,10 @@ __global__ void __launch_bounds__(256) k_mc_leaves(const __grid_constant__ daala
   int bad = 0, beyond = 0;
   for (int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < B.F * nsb; w += (gridDim.x * blockDim.x) >> 5) {
     const int f = w / nsb, sb = w - f * nsb;
+    if (B.frame_type && B.frame_type[f]) {   // a keyframe: no prediction, its grid is not read
+      if (lane == 0) B.nleaves[w] = 0;
+      continue;
+    }
     const int vx0 = (sb % B.nhsb) * 8, vy0 = (sb / B.nhsb) * 8;
     const daala_b200_mv_pt* g = B.grid + f * per_frame;
     const int32_t* g1 = kNext ? B.mv1 + 2 * f * per_frame : nullptr;
@@ -551,6 +555,12 @@ __global__ void __launch_bounds__(kThreads) k_mc_obmc(const __grid_constant__ da
     const int gold = min(max(B.ref_slot[2 * f], 0), B.nslots - 1), prev = min(max(B.ref_slot[2 * f + 1], 0), B.nslots - 1);
     const int next = kNext ? min(max(B.ref_slot_next[f], 0), B.nslots - 1) : 0;
     unsigned char* out = B.pred[p] + f * plane;
+    if (B.frame_type && B.frame_type[f]) {   // a keyframe's prediction planes are 0
+      const int sbw = 64 >> dec;
+      unsigned char* o = out + (size_t)vy0 * 8 / (1 + dec) * pw + (size_t)vx0 * 8 / (1 + dec);
+      for (int i = threadIdx.x; i < sbw * sbw; i += blockDim.x) o[(size_t)(i / sbw) * pw + i % sbw] = 0;
+      continue;
+    }
     const int n = B.nleaves[w];
     for (int q = 0; q < n; q++) {
       const uint32_t r = B.leaves[(size_t)w * 64 + q];

@@ -38,6 +38,11 @@ reference carry the quantised DCs, and `encode` returns the coded indices as dc_
 plane).  daala_b200/haardc.py restates the chain in numpy.  With symbol_stream=1 too the stream carries the same
 indices in coding order, one symbols.HDC_DTYPE record per block record (`sym_hdc`), and `encode(..., dc_grids=False)`
 leaves the grids out.
+With frame_types=1 (on an inter=1, frame_quant=1, haar_dc_quant=1 engine with inter_finish) one batch holds keyframes
+and P / B frames: `encode(..., frame_type=)` takes one type per frame (1 = keyframe, 0 = P or B frame), each keyframe is
+coded as a keyframe_quant=1, haar_dc_quant=1 engine codes it and each P / B frame as the frame_quant=1 inter engine
+does, and the results are those of both kinds.  The finishing pass deringes the keyframes too, and ref_slot_out stores
+them in the pool, so one engine codes a whole GOP.
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -63,7 +68,7 @@ class Config(ctypes.Structure):
                 ("coded_quantizer", c_int), ("qm_is_flat", c_int), ("dering_lambda", ctypes.c_double),
                 ("symbol_stream", c_int), ("inter", c_int), ("inter_mc", c_int), ("mc_refs", c_int),
                 ("inter_finish", c_int), ("late_skip", c_int), ("mc_next", c_int), ("frame_quant", c_int),
-                ("lossless", c_int), ("haar_dc_quant", c_int), ("keyframe_quant", c_int)]
+                ("lossless", c_int), ("haar_dc_quant", c_int), ("keyframe_quant", c_int), ("frame_types", c_int)]
 
 
 # daala_b200_kf_frame_quant: one frame's quantizer on a frame_quant or keyframe_quant engine.  A keyframe's record:
@@ -108,7 +113,7 @@ class IO(ctypes.Structure):
                 ("sym_late_skip_cap", c_ll), ("ref_slot_next", c_void_p), ("mv1_grid", c_void_p),
                 ("frame_quant", c_void_p), ("ll_coeffs", c_void_p * 3), ("ll_blocks", c_void_p),
                 ("ll_ref_slot_out", c_void_p), ("dc_index", c_void_p * 3), ("sym_hdc", c_void_p),
-                ("sym_hdc_cap", c_ll)]
+                ("sym_hdc_cap", c_ll), ("frame_type", c_void_p)]
 
 
 class FinishIO(ctypes.Structure):
@@ -205,7 +210,8 @@ class KeyframeEngine:
     def __init__(self, geom, nframes=1, q0=38, use_masking=1, lam=pvq.PVQ_LAMBDA, pvq_qm_q4=None, qm=None,
                  qm_inv=None, sb_row0=0, sb_rows=0, max_blocks_div=0, persist_ctas_per_sm=0, split_free=1, level_chains=0, noref_prepass=0, dering=0, coded_quantizer=0,
                  qm_is_flat=0, dering_lambda=None, pinned=True, symbol_stream=0, inter=0, inter_mc=0, mc_refs=0,
-                 inter_finish=0, late_skip=0, mc_next=0, frame_quant=0, lossless=0, haar_dc_quant=0, keyframe_quant=0):
+                 inter_finish=0, late_skip=0, mc_next=0, frame_quant=0, lossless=0, haar_dc_quant=0, keyframe_quant=0,
+                 frame_types=0):
         # split_free, level_chains and noref_prepass exist only for bench.py, which passes them: one schedule is left
         retired = ("split_free=%r (chroma through the persistent kernel)" % split_free if split_free == 0 else
                    "split_free=%r (luma bands 3 / 6 through the phase kernels)" % split_free if split_free != 1 else
@@ -267,6 +273,10 @@ class KeyframeEngine:
         # keyframe_quant: keyframes take one FRAME_QUANT_DTYPE record per frame, as frame_quant engines do
         cfg.keyframe_quant = int(keyframe_quant)
         self.keyframe_quant = int(keyframe_quant)
+        # frame_types: keyframes and P / B frames in one batch, one type per frame (encode(..., frame_type=))
+        cfg.frame_types = int(frame_types)
+        self.frame_types = int(frame_types)
+        self._ftype = None
         self._ll_slot = None
         self.nrefs = 0
         self.resident = False
@@ -396,6 +406,20 @@ class KeyframeEngine:
         self._fq = self._arr("fq", (self.F,), FRAME_QUANT_DTYPE)
         self._fq[...] = r
 
+    def stage_frame_type(self, frame_type):
+        """Copies the [F] frame types of one batch (1 = keyframe, 0 = P or B frame) into the host buffers: required by a
+        frame_types engine and refused by any other with a ValueError.  The C call refuses values other than 0 and 1."""
+        if bool(self.frame_types) != (frame_type is not None):
+            raise ValueError("frame_type= is required by an engine created with frame_types=1 and refused by any other")
+        if frame_type is None:
+            self._ftype = None
+            return
+        t = np.asarray(frame_type)
+        if t.shape != (self.F,):
+            raise ValueError("frame_type= is [%d] values, 1 = keyframe, 0 = P or B frame" % self.F)
+        self._ftype = self._arr("ftype", (self.F,), np.uint8)
+        self._ftype[...] = t
+
     def stage_inputs(self, planes, bsize, pred=None):
         """Copies one batch into the engine's (pinned) host input buffers.  planes: per plane an array
         [F, h, w] u8 (padded geometry); bsize: [F, nvsb*8, nhsb*8]; pred (inter engines): the
@@ -496,6 +520,8 @@ class KeyframeEngine:
             io.luma_dc_resid, io.chroma_dc_resid = out["luma_dc_resid"].ctypes.data, out["chroma_dc_resid"].ctypes.data
         if self._fq is not None:
             io.frame_quant = self._fq.ctypes.data
+        if self._ftype is not None:
+            io.frame_type = self._ftype.ctypes.data
         if self._ll_slot is not None:   # refused by the C call: a lossy engine has no lossless step
             io.ll_ref_slot_out = self._ll_slot.ctypes.data
         if self.haar_dc_quant and dc_grids:
@@ -539,6 +565,8 @@ class KeyframeEngine:
                 self.h2d_bytes += 4 * self.F + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * 8
         if self._fq is not None:   # the records, each frame's deringing thresholds (int32 [2][6]) and band quantisers ([3][32])
             self.h2d_bytes += self.F * (FRAME_QUANT_DTYPE.itemsize + 48 + 384)
+        if self._ftype is not None:
+            self.h2d_bytes += self.F
         return out
 
     def stage_ll_ref_slot_out(self, slots):
@@ -621,17 +649,20 @@ class KeyframeEngine:
 
     def encode(self, planes, bsize, symbols=True, recon=True, dering_levels=None, stream=None, pred=None, refs=None,
                ref_slot=None, mv_grid=None, resident=False, mv1_grid=None, frame_quant=None, ll_ref_slot_out=None,
-               dc_grids=True):
+               dc_grids=True, frame_type=None):
         """One batch end to end through the C ABI with host buffers; returns the result arrays (views of
         the engine's host buffers: copy what must survive the next call).  pred: see stage_inputs; refs, ref_slot,
         mv_grid, resident, mv1_grid (inter_mc engines, which also return the prediction as pred0..2): see stage_mc;
         frame_quant (frame_quant and keyframe_quant engines, required there): [F] FRAME_QUANT_DTYPE records, see
         stage_frame_quant;
+        frame_type (frame_types engines, required there and refused elsewhere): see stage_frame_type; such an engine
+        returns the outputs of both kinds, each 0 on the blocks and frames of the other kind (include/daala_b200.h);
         ll_ref_slot_out (lossless engines with inter_mc): see stage_ll_ref_slot_out; dc_grids: see prepare_io.  On a lossless engine bsize is not
         read (None is fine) and the results are those of _prepare_io_lossless.  Raises
         when the batch exceeded the block capacity, or (inter_mc) when a used vertex names a picture other than GOLD /
         PREV (/ NEXT on mc_next engines) or a vector reaches past the reference's edge extension: the reference
         encoder's result is undefined there."""
+        self.stage_frame_type(frame_type)
         self.stage_inputs(planes, bsize, pred)
         if (self.inter_mc or refs is not None or ref_slot is not None or mv_grid is not None or resident
                 or mv1_grid is not None):

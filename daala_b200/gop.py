@@ -18,7 +18,8 @@ rotation).  The buffer indices serve directly as pool slots of a device-resident
 pipelined_steps groups one sequence's coded frames into engine steps, so that one sequence fills a batch (new
 scheduling, not the reference's): each step holds the next I / P anchor and the B frames coded just before it, which
 depend only on pictures finished in earlier steps.  The frames of such a step differ in type, so their quantizers differ
-too: the engine takes one quantizer record per frame (config.frame_quant).
+too: the engine takes one quantizer record per frame (config.frame_quant).  With keyframes_inline an I frame joins
+such a step too, on an engine with config.frame_types that codes keyframes and P / B frames in one batch.
 """
 from collections import namedtuple
 
@@ -96,7 +97,7 @@ def coding_order(nframes, b_frames, keyframe_rate=256):
     return out
 
 
-def pipelined_steps(frames):
+def pipelined_steps(frames, keyframes_inline=False):
     """The coded frames of coding_order(...) as engine steps, in the order they run: [[Frame, ...], ...].
 
     A P frame forms a step with the B frames coded just before it (the B frames between the two anchors before it),
@@ -106,12 +107,16 @@ def pipelined_steps(frames):
     any frame's reconstruction is stored, which is what lets an anchor's SELF buffer be one that the step's B frames
     still read.  The I frames of several sequences may share one step of a keyframe engine with keyframe_quant = 1, each
     at its own record; pool_load from that engine's reconstruction seeds each sequence's P engine as it does for a
-    keyframe coded alone."""
+    keyframe coded alone.
+
+    keyframes_inline=True: an I frame forms a step with the B frames coded just before it, exactly as a P frame does;
+    the steps are those of an engine with frame_types = 1, which codes the keyframe beside them and stores it in the
+    pool with ref_slot_out like any other frame."""
     steps, pending = [], []
     for fr in frames:
         if fr.type == B_FRAME:
             pending.append(fr)
-        elif fr.type == I_FRAME:
+        elif fr.type == I_FRAME and not keyframes_inline:
             if pending:
                 steps.append(pending)
             steps.append([fr])

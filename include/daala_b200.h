@@ -552,8 +552,8 @@ typedef struct daala_b200_kf_config {
                                   every block, the 4x4-chroma CfL reference and the reconstruction then carry the
                                   quantised DCs; daala_b200_kf_io.dc_index returns the coded indices.  q0, pvq_qm_q4 and
                                   pvq_norm_lambda are the chain's quantizer and lambda.  Refused by daala_b200_kf_create
-                                  with a value other than 0 or 1, and 1 together with inter, lossless or a row shard
-                                  (sb_rows > 0: the superblock predictor reads the row above) */
+                                  with a value other than 0 or 1, and 1 together with inter (unless frame_types = 1),
+                                  lossless or a row shard (sb_rows > 0: the superblock predictor reads the row above) */
   int keyframe_quant;          /* 0 (default): every keyframe is coded at this config's quantizer, through records
                                   made from it as with frame_quant = 0.
                                   1: the keyframe counterpart of frame_quant: every keyframe of a step has its own
@@ -569,6 +569,22 @@ typedef struct daala_b200_kf_config {
                                   src/encode.c:3050-3075).  Refused by daala_b200_kf_create with a value other than 0
                                   or 1, and 1 together with inter (P and B frames have frame_quant), lossless or a
                                   row shard (sb_rows > 0) */
+  int frame_types;             /* 0 (default): nothing below exists; the engine is exactly the one without this field.
+                                  1: keyframes and P / B frames in one batch.  Every step takes one type per frame
+                                  (daala_b200_kf_io.frame_type: 1 = keyframe, 0 = P or B frame).  A keyframe is coded
+                                  exactly as an engine with keyframe_quant = 1 and haar_dc_quant = 1 codes it (DC Haar
+                                  pyramid and DC chain, luma through the chain kernel, CfL chroma), a P or B frame exactly
+                                  as the frame_quant = 1 inter engine codes it; each frame reads its own
+                                  daala_b200_kf_frame_quant record.  One captured graph serves every mix of types: the
+                                  type table goes to the device with the records.  The finishing pass leaves a keyframe's
+                                  coefficients as the step coded them (its skip and DC entries are not read, its bskip is
+                                  all zero) and deringes it at its given level (inter_finish = 1) or at the level the
+                                  keyframe rule searches (inter_finish = 2: every superblock, up / left CDF context);
+                                  ref_slot_out stores keyframes like any other frame.  Requires inter = 1, frame_quant = 1,
+                                  haar_dc_quant = 1 and inter_finish 1 or 2 (inter_mc and mc_next are allowed); refused by
+                                  daala_b200_kf_create with a value other than 0 or 1, and 1 together with symbol_stream,
+                                  late_skip, lossless, dering (a keyframe is deringed in the finishing pass) or a row
+                                  shard (sb_rows > 0) */
 } daala_b200_kf_config;
 
 /* config.lossless: the root sums of one block (od_compute_max_tree, src/encode.c:899-919, over the residual of
@@ -797,6 +813,12 @@ typedef struct daala_b200_kf_io {
      daala_b200_kf_symbol_bounds(...).blocks; NULL = not copied.  Only the used part is copied, as for sym_dc. */
   daala_b200_kf_sym_hdc *sym_hdc;
   long long sym_hdc_cap;
+  /* config.frame_types = 1 only (required there, refused otherwise): [nframes] 1 = keyframe, 0 = P or B frame; any other
+     value is refused.  Outputs of one kind are 0 for the blocks and frames of the other: chroma_flip and dc_index[0..2]
+     for P / B frames; luma_dc / chroma_dc, luma_dc_resid / chroma_dc_resid and pred_pixels_out (inter_mc) for keyframes.
+     With inter_mc a keyframe has no prediction: its ref_slot / ref_slot_next entries and its MV grid are not read or
+     checked, and it adds nothing to counts[19] / counts[20]. */
+  const uint8_t *frame_type;
 } daala_b200_kf_io;
 
 /* The finishing pass of a P-frame batch (config.inter_finish), daala_b200_kf_finish: the host coder's per-block
