@@ -70,7 +70,6 @@ enum Cnt {
   kMcBeyond = 20,    //                  corner windows reaching past the reference's edge extension
   // the words the persistent kernels hammer with atomics each sit in a 128-byte line of their own
   kHeadLoL = 32,     // ticket of the luma dependency-free lists
-  kHeadLoC = 64,     // ticket of the chroma lists
   kHeadHi = 96,      // luma chain queue: next slot to claim
   kTailHi = 128,     //                   next slot to fill
   kDoneHi = 160,     // band-0 items finished (flushed by warps when they go idle)
@@ -490,7 +489,7 @@ struct Stage {
   const int32_t* succ_right;
   int32_t* join0;                  // [nblocks] band 0: neighbours finished so far (it may wait for two)
   int32_t* cnt;
-  int n_items_at, head_lo_at, n_blocks_at;
+  int n_items_at, head_lo_at, n_blocks_at;   // head_lo_at: luma only (next_item)
   int max_blocks;
   // split path (phases as separate kernels over the dependency-free item lists): context records of one
   // chunk of items per class
@@ -959,28 +958,23 @@ __global__ void k_fill_rsqrt(double* tbl) {
   if (i < kTableDoubles) pvq_fill_rsqrt_table(tbl, i);
 }
 
-// Start of the PVQ stages in `stages` (kBeginLuma | kBeginChroma): the tickets; the chain queue starts with the
-// heads.  Neither stage touches the other's tickets, so the whole step starts both at once.
+// Start of the luma chain kernel: its tickets; the chain queue starts with the heads.
 // ring (frame_types, else NULL): a step without keyframe luma blocks has no band-0 item whose completion would release
 // the chain kernel's parked warps, so their slots [0, nwarps] are released (kExit) from the start, as the last band-0
 // item does on a step with keyframes.
-enum { kBeginLuma = 1, kBeginChroma = 2 };
-__global__ void k_begin_pvq(int32_t* cnt, int stages, uint32_t* ring = nullptr, int nwarps = 0) {
+__global__ void k_begin_pvq(int32_t* cnt, uint32_t* ring = nullptr, int nwarps = 0) {
   if (ring && cnt[kNLuma] == 0)
     for (int i = threadIdx.x; i <= nwarps; i += blockDim.x) ring[i] = kExit;
   if (threadIdx.x == 0 && blockIdx.x == 0) {
-    if (stages & kBeginLuma) {
-      cnt[kHeadLoL] = 0;
-      cnt[kHeadHi] = 0;
-      cnt[kTailHi] = cnt[kNHeads0];
-      cnt[kDoneHi] = 0;
-      cnt[kHeadCh] = 0;
-      cnt[kWaiters] = 0;
+    cnt[kHeadLoL] = 0;
+    cnt[kHeadHi] = 0;
+    cnt[kTailHi] = cnt[kNHeads0];
+    cnt[kDoneHi] = 0;
+    cnt[kHeadCh] = 0;
+    cnt[kWaiters] = 0;
 #ifdef DAALA_B200_CHAIN_TRACE
-      cnt[kTraceN] = 0;
+    cnt[kTraceN] = 0;
 #endif
-    }
-    if (stages & kBeginChroma) cnt[kHeadLoC] = 0;
   }
 }
 
@@ -1624,10 +1618,8 @@ __global__ void __launch_bounds__(256) k_fin_unstream(const __grid_constant__ Un
 // =====================================================================================================
 using namespace daala_b200::kf;
 
-extern "C" int daala_b200_launch_forward(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
 extern "C" int daala_b200_launch_forward_masked(const daala_b200_frame* prm, int nplanes, const uint8_t* haar_frames,
                                                 const uint8_t* skip_frames, cudaStream_t stream);
-extern "C" int daala_b200_launch_inverse(const daala_b200_frame* prm, int nplanes, cudaStream_t stream);
 extern "C" int daala_b200_launch_inverse_lapped_only(const daala_b200_frame* prm, int plane0, int nplanes,
                                                      cudaStream_t stream);
 extern "C" int daala_b200_launch_sb_postfilter_store(const daala_b200_frame* prm, int plane0, int nplanes,
@@ -1651,7 +1643,7 @@ struct Dering {
   daala_b200_dering_search_batch sb;
 };
 
-// The events of kf_enqueue_step_forked and kf_enqueue_step_mixed, one per fork or join.
+// The events of enqueue_step's two-stream form, one per fork or join.
 enum { kEvLists, kEvForward, kEvLumaBands, kEvLumaScatter, kEvChroma, kEvHaarDc, kEvLumaGather, kEvInterLuma, kNumEvents };
 
 struct daala_b200_kf {
@@ -2059,7 +2051,6 @@ static int kf_alloc(daala_b200_kf* kf) {
     }
     S.max_waiters = kf->sms * 8;
     S.n_items_at = chroma ? kNItemsC : kNItemsL;
-    S.head_lo_at = chroma ? kHeadLoC : kHeadLoL;
     S.n_blocks_at = chroma ? kNChroma : kNLuma;
     S.max_blocks = (int)nblk;
 #ifdef DAALA_B200_CHAIN_TRACE
@@ -2069,6 +2060,7 @@ static int kf_alloc(daala_b200_kf* kf) {
     }
 #endif
     if (!chroma) {
+      S.head_lo_at = kHeadLoL;
       S.dep_top = L.dep_top;
       S.dep_left = L.dep_left;
       S.succ_bottom = L.succ_bottom;
@@ -2460,8 +2452,7 @@ static int dering_launches(const Dering& D, int parts) {
   return 2 * parts + (D.search ? 1 + 5 + 6 + 6 + 1 : 0) + 1 + 3;
 }
 
-// Everything between "inputs are in HBM" and "results are in HBM", on kf->stream.
-// the three phase kernels over every chunk of every class of a stage's dependency-free lists
+// The three phase kernels over every chunk of every class of a stage's dependency-free lists
 static void enqueue_split(daala_b200_kf* kf, const Stage& S, cudaStream_t s) {
   const int grid = kf->sms * 16;
   for (int cls = 2; cls >= 0; cls--) {
@@ -2495,224 +2486,152 @@ static void enqueue_sym(const Sym& Y, int wide, cudaStream_t s) {
   k_sym_index<<<1, 256, 0, s>>>(Y);
 }
 
-// config.inter: the same step for P-frame residuals.  Both plane sets through the forward transform (two
-// launches: the kernel's tensor maps describe one pixel allocation each), every band of both stages through
-// the phase kernels with the transformed prediction as reference.
-static int kf_enqueue_step_inter(daala_b200_kf* kf, int phases) {
-  cudaStream_t s = kf->stream;
-  const Lists& L = kf->lists;
+// config.inter_mc: the bad-ref counters cleared and the leaves of the MV grids (DAALA_B200_KF_LISTS), then OBMC into the
+// prediction planes (DAALA_B200_KF_FORWARD).
+static int enqueue_mc(daala_b200_kf* kf, int phases, cudaStream_t s) {
+  if (!kf->cfg.inter_mc) return 0;
   const int wide = kf->sms * 8;
+  if (phases & DAALA_B200_KF_LISTS) {
+    const cudaError_t e = cudaMemsetAsync(kf->lists.cnt + kMcBadRef, 0, 2 * sizeof(int32_t), s);
+    if (e != cudaSuccess) return (int)e;
+    const int rc = daala_b200_launch_mc_leaves(&kf->mc, wide, s);
+    if (rc) return rc;
+  }
+  return phases & DAALA_B200_KF_FORWARD ? daala_b200_launch_mc_obmc(&kf->mc, wide, s) : 0;
+}
+
+#define STEP_TRY(x)           \
+  do {                        \
+    const int rc_ = (int)(x); \
+    if (rc_) return rc_;      \
+  } while (0)
+
+// Everything between "inputs are in HBM" and "results are in HBM" for every lossy engine, each piece under its phase
+// bit.  The engine has keyframes (`key`: !inter, or frame_types) and / or P / B frames (`pb`: inter).  The whole step of
+// an engine with a side stream (keyframe and frame_types engines) runs as two branches, s = kf->stream and c = kf->side,
+// forked and joined with events (captured into the step graph as parallel branches; live launches order the same way).
+// A partial phase mask (per-phase timings) or an inter-only engine runs every piece on s, in the same order.  `core`
+// (DAALA_B200_KF_SEARCH_ONLY, measurement): only the band kernels of the PVQ phases, on the coding-order buffers a
+// previous full pass left behind (same inputs, same results).  The pieces, in order:
+//   c: [inter_mc: leaves, OBMC], the source transform (frame_types: the DC pyramid on keyframes only), [late_skip: the
+//      unquantised coefficients], [pb: the prediction's transform];  s: the work lists (key: k_luma_deps, pb:
+//      k_luma_items, k_chroma_items); join;
+//   c: [haar_dc_quant: the keyframes' DC chain];  s: [key: the chain tickets], the luma gather, [key: the chain kernel];
+//      c, after the gather: [pb: the P / B luma phase kernels];
+//   c, after the chains: the chroma stage (gather -- CfL reads the luma bands in coding order, not the luma scatter --
+//      phase kernels, scatter);  s, after the DC chain and the P / B luma bands: the luma scatter;
+//   c, after the luma scatter: [late skip], [symbol stream];
+//   c: inverse + SB postfilter of planes 1-2;  s: of plane 0, [level search, thresholds, od_dering of plane 0]; join;
+//   s: [od_dering of planes 1-2: they read the direction map plane 0 writes].
+// The side stream has the highest priority: its chroma kernels take the SMs first and the luma branch fills what they
+// leave idle.  The branches write disjoint buffers; only the order of independent work differs between the two forms.
+static int enqueue_step(daala_b200_kf* kf, int phases) {
+  const daala_b200_kf_config& cfg = kf->cfg;
+  const bool key = !cfg.inter || cfg.frame_types, pb = cfg.inter != 0, mixed = cfg.frame_types != 0;
+  const bool hdc = cfg.haar_dc_quant != 0, core = (phases & DAALA_B200_KF_SEARCH_ONLY) != 0;
+  cudaStream_t s = kf->stream, c = phases == DAALA_B200_KF_ALL && kf->side ? kf->side : s;
+  const Lists& L = kf->lists;
+  const Stage& K = mixed ? kf->luma_kf : kf->luma;   // the chain kernel's stage
+  const uint8_t* ftype = mixed ? kf->ftype : nullptr;
+  const int wide = kf->sms * 8;
+  const int persist = kf->sms * (cfg.persist_ctas_per_sm > 0 ? cfg.persist_ctas_per_sm : kPersistCtas);
+  // event e recorded on `from` / waited for on `to`: only when the step forks
+  auto record = [&](int e, cudaStream_t from) { return c == s ? cudaSuccess : cudaEventRecord(kf->ev[e], from); };
+  auto wait = [&](int e, cudaStream_t to) { return c == s ? cudaSuccess : cudaStreamWaitEvent(to, kf->ev[e], 0); };
+  auto join = [&](int e, cudaStream_t from, cudaStream_t to) {
+    const cudaError_t r = record(e, from);
+    return r != cudaSuccess ? r : wait(e, to);
+  };
+
+  STEP_TRY(join(kEvLists, s, c));
+  STEP_TRY(enqueue_mc(kf, phases, c));
+  if (phases & DAALA_B200_KF_FORWARD) {
+    STEP_TRY(daala_b200_launch_forward_masked(&kf->frame_fwd, 3, ftype, nullptr, c));
+    // late_skip: the unquantised coefficients, before k_finish_scatter<true> overwrites them with the coded ones
+    for (int p = 0; cfg.late_skip && p < 3; p++)
+      STEP_TRY(cudaMemcpyAsync(kf->d_orig[p], kf->coeffs[p], sizeof(int32_t) * kf->plane_w[p] * kf->plane_h[p] * kf->F,
+                               cudaMemcpyDeviceToDevice, c));
+    // a launch of its own: the kernel's tensor maps describe one pixel allocation each
+    if (pb) STEP_TRY(daala_b200_launch_forward_masked(&kf->frame_pred, 3, nullptr, ftype, c));
+  }
   if (phases & DAALA_B200_KF_LISTS) {
     k_unit_tile_sums<<<L.ntiles, kTile, 0, s>>>(L);
     k_tile_scan<<<1, 1024, 0, s>>>(L);
     k_unit_emit<<<L.ntiles, kTile, 0, s>>>(L);
-    k_luma_items<<<wide, 256, 0, s>>>(L);
+    if (key) {
+      const size_t nl = (size_t)L.max_luma * sizeof(int32_t);
+      STEP_TRY(cudaMemsetAsync(L.succ_bottom, 0xff, nl, s));
+      STEP_TRY(cudaMemsetAsync(L.succ_right, 0xff, nl, s));
+      STEP_TRY(cudaMemsetAsync(L.head_hist, 0, sizeof(int32_t) * kHeadBins, s));
+      k_luma_deps<<<wide, 256, 0, s>>>(L);
+    }
+    if (pb) k_luma_items<<<wide, 256, 0, s>>>(L);
     k_chroma_items<<<wide, 256, 0, s>>>(L);
-    if (kf->cfg.inter_mc) {
-      if (cudaMemsetAsync(L.cnt + kMcBadRef, 0, 2 * sizeof(int32_t), s) != cudaSuccess) return (int)cudaGetLastError();
-      int rc = daala_b200_launch_mc_leaves(&kf->mc, wide, s);
-      if (rc) return rc;
+  }
+  STEP_TRY(join(kEvForward, c, s));
+  if (hdc && (phases & DAALA_B200_KF_FORWARD)) {
+    STEP_TRY(daala_b200_launch_haar_dc(&kf->hdcb, c));
+    STEP_TRY(record(kEvHaarDc, c));
+  }
+
+  if (phases & DAALA_B200_KF_PVQ_LUMA) {
+    if (key) {
+      STEP_TRY(cudaMemsetAsync(K.ring, 0xff, kf->chain_cap * sizeof(uint32_t), s));
+      STEP_TRY(cudaMemsetAsync(K.join0, 0, (size_t)K.max_blocks * sizeof(int32_t), s));
+      if (mixed) k_begin_pvq<<<1, 256, 0, s>>>(K.cnt, K.ring, persist * kPersistThreads / 32);
+      else k_begin_pvq<<<1, 32, 0, s>>>(K.cnt);
+    }
+    if (!core && mixed) k_gather<kGatherLuma, false, true><<<wide, 256, 0, s>>>(kf->luma);
+    else if (!core && pb) k_gather<kGatherInter><<<wide, 256, 0, s>>>(kf->luma);
+    else if (!core) k_gather<kGatherLuma><<<wide, 256, 0, s>>>(kf->luma);
+    if (pb) STEP_TRY(join(kEvLumaGather, s, c));
+    if (key) k_pvq_persist<<<persist, kPersistThreads, 0, s>>>(K);
+    if (pb) {
+      enqueue_split(kf, kf->luma, c);
+      STEP_TRY(record(kEvInterLuma, c));
     }
   }
-  if (phases & DAALA_B200_KF_FORWARD) {
-    int rc = kf->cfg.inter_mc ? daala_b200_launch_mc_obmc(&kf->mc, wide, s) : 0;
-    if (!rc) rc = daala_b200_launch_forward(&kf->frame, 3, s);
-    if (rc) return rc;
-    // late_skip: the unquantised coefficients, before k_finish_scatter<true> overwrites them with the coded ones
-    for (int p = 0; kf->cfg.late_skip && p < 3; p++)
-      if (cudaMemcpyAsync(kf->d_orig[p], kf->coeffs[p], sizeof(int32_t) * kf->plane_w[p] * kf->plane_h[p] * kf->F,
-                          cudaMemcpyDeviceToDevice, s) != cudaSuccess)
-        return (int)cudaGetLastError();
-    rc = daala_b200_launch_forward(&kf->frame_pred, 3, s);
-    if (rc) return rc;
+  STEP_TRY(join(kEvLumaBands, s, c));
+  if (phases & DAALA_B200_KF_PVQ_CHROMA) {
+    if (!core && mixed) k_gather<kGatherChroma, true, true><<<wide, 256, 0, c>>>(kf->chroma);
+    else if (!core && pb) k_gather<kGatherInter><<<wide, 256, 0, c>>>(kf->chroma);
+    else if (!core && hdc) k_gather<kGatherChroma, true><<<wide, 256, 0, c>>>(kf->chroma);
+    else if (!core) k_gather<kGatherChroma><<<wide, 256, 0, c>>>(kf->chroma);
+    enqueue_split(kf, kf->chroma, c);
+    if (!core && mixed) k_finish_scatter<false, true, true><<<wide, 256, 0, c>>>(kf->chroma);
+    else if (!core && pb) k_finish_scatter<true><<<wide, 256, 0, c>>>(kf->chroma);
+    else if (!core && hdc) k_finish_scatter<false, true><<<wide, 256, 0, c>>>(kf->chroma);
+    else if (!core) k_finish_scatter<false><<<wide, 256, 0, c>>>(kf->chroma);
   }
-  const bool core = (phases & DAALA_B200_KF_SEARCH_ONLY) != 0;
-  for (const Stage* S : {&kf->luma, &kf->chroma}) {
-    if (!(phases & (S == &kf->luma ? DAALA_B200_KF_PVQ_LUMA : DAALA_B200_KF_PVQ_CHROMA))) continue;
-    if (!core) k_gather<kGatherInter><<<wide, 256, 0, s>>>(*S);
-    enqueue_split(kf, *S, s);
-    if (!core) k_finish_scatter<true><<<wide, 256, 0, s>>>(*S);
+  if (!core && (phases & DAALA_B200_KF_PVQ_LUMA)) {
+    if (hdc) STEP_TRY(wait(kEvHaarDc, s));
+    if (pb) STEP_TRY(wait(kEvInterLuma, s));
+    // forked: 16 waves of short CTAs instead of one resident wave: priority only orders CTAs that are still waiting, so
+    // a grid that fits the GPU at once would hold every SM until it is done and stall the chroma gather behind it
+    const int grid = c != s ? kf->sms * 128 : wide;
+    if (mixed) k_finish_scatter<false, true, true><<<grid, 256, 0, s>>>(kf->luma);
+    else if (pb) k_finish_scatter<true><<<grid, 256, 0, s>>>(kf->luma);
+    else if (hdc) k_finish_scatter<false, true><<<grid, 256, 0, s>>>(kf->luma);
+    else k_finish_scatter<false><<<grid, 256, 0, s>>>(kf->luma);
   }
-  if (!core && (phases & DAALA_B200_KF_PVQ_CHROMA) && kf->cfg.late_skip) {
-    const int rc = daala_b200_late_skip_enqueue(&kf->lsb, kf->sms * 3, s);
-    if (rc) return rc;
+  if (!core && (phases & DAALA_B200_KF_PVQ_CHROMA) && (cfg.late_skip || cfg.symbol_stream)) {
+    STEP_TRY(join(kEvLumaScatter, s, c));
+    if (cfg.late_skip) STEP_TRY(daala_b200_late_skip_enqueue(&kf->lsb, kf->sms * 3, c));
+    if (cfg.symbol_stream && pb) enqueue_sym<true>(kf->sym, wide, c);
+    else if (cfg.symbol_stream) enqueue_sym<false>(kf->sym, wide, c);
   }
-  if (!core && (phases & DAALA_B200_KF_PVQ_CHROMA) && kf->cfg.symbol_stream) enqueue_sym<true>(kf->sym, wide, s);
+
   if (phases & DAALA_B200_KF_INVERSE) {
-    int rc = daala_b200_launch_inverse(&kf->frame, 3, s);
-    if (rc) return rc;
+    const daala_b200_frame& fr = cfg.dering ? kf->dering.frame : kf->frame;
+    if (c != s) STEP_TRY(enqueue_recon(fr, 1, 2, c));
+    STEP_TRY(enqueue_recon(fr, 0, c != s ? 1 : 3, s));
+    if (cfg.dering) STEP_TRY(enqueue_dering_luma(kf, kf->dering, s));
+    STEP_TRY(join(kEvChroma, c, s));
+    for (int p = 1; cfg.dering && p < 3; p++) STEP_TRY(enqueue_dering_plane(kf, kf->dering, p, s));
   }
   return (int)cudaGetLastError();
 }
-
-// Keyframe work lists from the block-size maps.
-static int enqueue_lists(daala_b200_kf* kf, cudaStream_t s) {
-  const Lists& L = kf->lists;
-  const int wide = kf->sms * 8;
-  k_unit_tile_sums<<<L.ntiles, kTile, 0, s>>>(L);
-  k_tile_scan<<<1, 1024, 0, s>>>(L);
-  k_unit_emit<<<L.ntiles, kTile, 0, s>>>(L);
-  const size_t nl = (size_t)L.max_luma * sizeof(int32_t);
-  if (cudaMemsetAsync(L.succ_bottom, 0xff, nl, s) != cudaSuccess || cudaMemsetAsync(L.succ_right, 0xff, nl, s) != cudaSuccess)
-    return (int)cudaGetLastError();
-  if (cudaMemsetAsync(L.head_hist, 0, sizeof(int32_t) * kHeadBins, s) != cudaSuccess) return (int)cudaGetLastError();
-  k_luma_deps<<<wide, 256, 0, s>>>(L);
-  k_chroma_items<<<wide, 256, 0, s>>>(L);
-  return 0;
-}
-
-// The luma PVQ stage up to its last band: the tickets of the stages in `begin`, gather, the chain kernel.  `core`
-// (_SEARCH_ONLY, measurement): just the search kernels, on the coding-order buffers a previous full pass left behind
-// (same inputs, same results).
-static int enqueue_luma_bands(daala_b200_kf* kf, bool core, int begin, cudaStream_t s) {
-  const int wide = kf->sms * 8;
-  const int persist = kf->sms * (kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas);
-  if (cudaMemsetAsync(kf->luma.ring, 0xff, kf->chain_cap * sizeof(uint32_t), s) != cudaSuccess ||
-      cudaMemsetAsync(kf->luma.join0, 0, (size_t)kf->luma.max_blocks * sizeof(int32_t), s) != cudaSuccess)
-    return (int)cudaGetLastError();
-  k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, begin);
-  if (!core) k_gather<kGatherLuma><<<wide, 256, 0, s>>>(kf->luma);
-  k_pvq_persist<<<persist, kPersistThreads, 0, s>>>(kf->luma);
-  return 0;
-}
-
-// The chroma PVQ stage: [its tickets], gather with the CfL reference (it reads the luma stage's coding-order buffers, so it needs
-// the luma bands, not the luma scatter), the bands, the scatter into the coefficient planes.
-static void enqueue_chroma(daala_b200_kf* kf, bool core, bool begin, cudaStream_t s) {
-  const int wide = kf->sms * 8;
-  const bool hdc = kf->cfg.haar_dc_quant != 0;
-  if (begin) k_begin_pvq<<<1, 32, 0, s>>>(kf->lists.cnt, kBeginChroma);
-  if (!core && hdc) k_gather<kGatherChroma, true><<<wide, 256, 0, s>>>(kf->chroma);
-  else if (!core) k_gather<kGatherChroma><<<wide, 256, 0, s>>>(kf->chroma);
-  enqueue_split(kf, kf->chroma, s);
-  if (!core && hdc) k_finish_scatter<false, true><<<wide, 256, 0, s>>>(kf->chroma);
-  else if (!core) k_finish_scatter<false><<<wide, 256, 0, s>>>(kf->chroma);
-}
-
-// The whole keyframe step (DAALA_B200_KF_ALL) as two branches, kf->stream and kf->side, forked and joined with
-// events (captured into the step graph as parallel branches; live launches order the same way):
-//   lists on kf->stream beside the forward transform on kf->side; join;
-//   both stages' tickets, luma bands (the chain kernel) on kf->stream; fork;
-//   kf->side: chroma stage, [symbol stream, after the luma scatter], inverse + SB postfilter of planes 1-2;
-//   kf->stream: luma scatter, inverse + SB postfilter of plane 0, [level search, thresholds, od_dering of plane 0];
-//   join; [od_dering of planes 1-2: they read the direction map plane 0 writes].
-// haar_dc_quant: the DC chain runs on kf->side right after the forward transform, after kEvForward is recorded, so the
-// luma bands do not wait for it; the chroma stage follows it by stream order and the luma scatter waits for kEvHaarDc.
-// The branches write disjoint buffers; only the order of independent work differs from the phase-by-phase path.
-static int kf_enqueue_step_forked(daala_b200_kf* kf) {
-  cudaStream_t s = kf->stream, c = kf->side;
-  const daala_b200_frame& fr = kf->cfg.dering ? kf->dering.frame : kf->frame;
-  auto fork = [](cudaEvent_t e, cudaStream_t from, cudaStream_t to) {
-    return cudaEventRecord(e, from) == cudaSuccess && cudaStreamWaitEvent(to, e, 0) == cudaSuccess;
-  };
-  if (!fork(kf->ev[kEvLists], s, c)) return (int)cudaGetLastError();
-  int rc = daala_b200_launch_forward(&kf->frame_fwd, 3, c);
-  if (!rc) rc = enqueue_lists(kf, s);
-  if (rc) return rc;
-  if (!fork(kf->ev[kEvForward], c, s)) return (int)cudaGetLastError();
-  const bool hdc = kf->cfg.haar_dc_quant != 0;
-  if (hdc) {
-    rc = daala_b200_launch_haar_dc(&kf->hdcb, c);
-    if (rc) return rc;
-    if (cudaEventRecord(kf->ev[kEvHaarDc], c) != cudaSuccess) return (int)cudaGetLastError();
-  }
-  rc = enqueue_luma_bands(kf, false, kBeginLuma | kBeginChroma, s);
-  if (rc) return rc;
-  if (!fork(kf->ev[kEvLumaBands], s, c)) return (int)cudaGetLastError();
-  enqueue_chroma(kf, false, false, c);
-  // 16 waves of short CTAs instead of one resident wave: priority only orders CTAs that are still waiting, so a grid
-  // that fits the GPU at once would hold every SM until it is done and stall the chroma gather behind it
-  if (hdc) {
-    if (cudaStreamWaitEvent(s, kf->ev[kEvHaarDc], 0) != cudaSuccess) return (int)cudaGetLastError();
-    k_finish_scatter<false, true><<<kf->sms * 128, 256, 0, s>>>(kf->luma);
-  } else {
-    k_finish_scatter<false><<<kf->sms * 128, 256, 0, s>>>(kf->luma);
-  }
-  if (kf->cfg.symbol_stream) {
-    if (!fork(kf->ev[kEvLumaScatter], s, c)) return (int)cudaGetLastError();
-    enqueue_sym<false>(kf->sym, kf->sms * 8, c);
-  }
-  rc = enqueue_recon(fr, 1, 2, c);
-  if (!rc) rc = enqueue_recon(fr, 0, 1, s);
-  if (!rc && kf->cfg.dering) rc = enqueue_dering_luma(kf, kf->dering, s);
-  if (rc) return rc;
-  if (!fork(kf->ev[kEvChroma], c, s)) return (int)cudaGetLastError();
-  for (int p = 1; kf->cfg.dering && p < 3; p++) {
-    rc = enqueue_dering_plane(kf, kf->dering, p, s);
-    if (rc) return rc;
-  }
-  return (int)cudaGetLastError();
-}
-
-// config.frame_types: keyframes and P / B frames in one step, as two branches (kf->stream and kf->side) forked and joined
-// with events:
-//   kf->side: [inter_mc: the P / B frames' leaves and OBMC], the source transform (DC pyramid on keyframes only), the
-//             prediction's transform (P / B frames only);  kf->stream: the work lists (keyframe luma through
-//             k_luma_deps, P-frame luma through k_luma_items, chroma of both kinds through k_chroma_items); join;
-//   kf->side: the keyframes' DC chain;  kf->stream: the chain tickets and the luma gather (per block by its kind); fork;
-//   kf->stream: the keyframe luma chains (k_pvq_persist);  kf->side: the P-frame luma bands through the phase kernels
-//             beside them, on the SMs the chains leave idle;
-//   kf->side, after the chains: the chroma stage (gather per block by its kind: CfL from the coded luma or md), scatter,
-//             inverse + SB postfilter of planes 1-2;  kf->stream, after the P-frame luma bands and the DC chain: the
-//             luma scatter, inverse + SB postfilter of plane 0; join.
-static int kf_enqueue_step_mixed(daala_b200_kf* kf, int phases) {
-  if (phases != DAALA_B200_KF_ALL) {
-    snprintf(kf->err, sizeof(kf->err), "a frame_types step runs whole (DAALA_B200_KF_ALL)");
-    return (int)cudaErrorInvalidValue;
-  }
-  cudaStream_t s = kf->stream, c = kf->side;
-  const Lists& L = kf->lists;
-  const int wide = kf->sms * 8;
-  auto fork = [](cudaEvent_t e, cudaStream_t from, cudaStream_t to) {
-    return cudaEventRecord(e, from) == cudaSuccess && cudaStreamWaitEvent(to, e, 0) == cudaSuccess;
-  };
-  if (!fork(kf->ev[kEvLists], s, c)) return (int)cudaGetLastError();
-  int rc = 0;
-  if (kf->cfg.inter_mc) {
-    if (cudaMemsetAsync(L.cnt + kMcBadRef, 0, 2 * sizeof(int32_t), c) != cudaSuccess) return (int)cudaGetLastError();
-    rc = daala_b200_launch_mc_leaves(&kf->mc, wide, c);
-    if (!rc) rc = daala_b200_launch_mc_obmc(&kf->mc, wide, c);
-  }
-  if (!rc) rc = daala_b200_launch_forward_masked(&kf->frame_fwd, 3, kf->ftype, nullptr, c);
-  if (!rc) rc = daala_b200_launch_forward_masked(&kf->frame_pred, 3, nullptr, kf->ftype, c);
-  if (rc) return rc;
-  k_unit_tile_sums<<<L.ntiles, kTile, 0, s>>>(L);
-  k_tile_scan<<<1, 1024, 0, s>>>(L);
-  k_unit_emit<<<L.ntiles, kTile, 0, s>>>(L);
-  const size_t nl = (size_t)L.max_luma * sizeof(int32_t);
-  if (cudaMemsetAsync(L.succ_bottom, 0xff, nl, s) != cudaSuccess || cudaMemsetAsync(L.succ_right, 0xff, nl, s) != cudaSuccess ||
-      cudaMemsetAsync(L.head_hist, 0, sizeof(int32_t) * kHeadBins, s) != cudaSuccess)
-    return (int)cudaGetLastError();
-  k_luma_deps<<<wide, 256, 0, s>>>(L);
-  k_luma_items<<<wide, 256, 0, s>>>(L);
-  k_chroma_items<<<wide, 256, 0, s>>>(L);
-  if (!fork(kf->ev[kEvForward], c, s)) return (int)cudaGetLastError();
-  rc = daala_b200_launch_haar_dc(&kf->hdcb, c);
-  if (rc) return rc;
-  const Stage& K = kf->luma_kf;
-  if (cudaMemsetAsync(K.ring, 0xff, kf->chain_cap * sizeof(uint32_t), s) != cudaSuccess ||
-      cudaMemsetAsync(K.join0, 0, (size_t)K.max_blocks * sizeof(int32_t), s) != cudaSuccess)
-    return (int)cudaGetLastError();
-  const int persist = kf->sms * (kf->cfg.persist_ctas_per_sm > 0 ? kf->cfg.persist_ctas_per_sm : kPersistCtas);
-  k_begin_pvq<<<1, 256, 0, s>>>(L.kcnt, kBeginLuma, K.ring, persist * kPersistThreads / 32);
-  k_gather<kGatherLuma, false, true><<<wide, 256, 0, s>>>(kf->luma);
-  if (!fork(kf->ev[kEvLumaGather], s, c)) return (int)cudaGetLastError();
-  k_pvq_persist<<<persist, kPersistThreads, 0, s>>>(K);
-  enqueue_split(kf, kf->luma, c);
-  if (cudaEventRecord(kf->ev[kEvInterLuma], c) != cudaSuccess) return (int)cudaGetLastError();
-  if (!fork(kf->ev[kEvLumaBands], s, c)) return (int)cudaGetLastError();
-  k_gather<kGatherChroma, true, true><<<wide, 256, 0, c>>>(kf->chroma);
-  enqueue_split(kf, kf->chroma, c);
-  k_finish_scatter<false, true, true><<<wide, 256, 0, c>>>(kf->chroma);
-  rc = enqueue_recon(kf->frame, 1, 2, c);
-  if (rc) return rc;
-  if (cudaStreamWaitEvent(s, kf->ev[kEvInterLuma], 0) != cudaSuccess) return (int)cudaGetLastError();
-  k_finish_scatter<false, true, true><<<wide, 256, 0, s>>>(kf->luma);
-  rc = enqueue_recon(kf->frame, 0, 1, s);
-  if (rc) return rc;
-  if (!fork(kf->ev[kEvChroma], c, s)) return (int)cudaGetLastError();
-  return (int)cudaGetLastError();
-}
+#undef STEP_TRY
 
 // config.lossless: the whole step, one phase.  [inter_mc: leaf enumeration and OBMC, unchanged], the lossless kernels.
 static int kf_enqueue_step_lossless(daala_b200_kf* kf, int phases) {
@@ -2720,49 +2639,8 @@ static int kf_enqueue_step_lossless(daala_b200_kf* kf, int phases) {
     snprintf(kf->err, sizeof(kf->err), "a lossless step runs whole (DAALA_B200_KF_ALL)");
     return (int)cudaErrorInvalidValue;
   }
-  cudaStream_t s = kf->stream;
-  const int wide = kf->sms * 8;
-  if (kf->cfg.inter_mc) {
-    if (cudaMemsetAsync(kf->lists.cnt + kMcBadRef, 0, 2 * sizeof(int32_t), s) != cudaSuccess) return (int)cudaGetLastError();
-    int rc = daala_b200_launch_mc_leaves(&kf->mc, wide, s);
-    if (!rc) rc = daala_b200_launch_mc_obmc(&kf->mc, wide, s);
-    if (rc) return rc;
-  }
-  return daala_b200_launch_lossless(&kf->ll, s);
-}
-
-// One step on kf->stream phase by phase (a partial phase mask: per-phase timings), or the whole step forked.
-static int kf_enqueue_step(daala_b200_kf* kf, int phases) {
-  if (kf->cfg.lossless) return kf_enqueue_step_lossless(kf, phases);
-  if (kf->cfg.frame_types) return kf_enqueue_step_mixed(kf, phases);
-  if (kf->cfg.inter) return kf_enqueue_step_inter(kf, phases);
-  if (phases == DAALA_B200_KF_ALL) return kf_enqueue_step_forked(kf);
-  cudaStream_t s = kf->stream;
-  if (phases & DAALA_B200_KF_LISTS) {
-    const int rc = enqueue_lists(kf, s);
-    if (rc) return rc;
-  }
-  if (phases & DAALA_B200_KF_FORWARD) {
-    int rc = daala_b200_launch_forward(&kf->frame_fwd, 3, s);
-    if (!rc && kf->cfg.haar_dc_quant) rc = daala_b200_launch_haar_dc(&kf->hdcb, s);
-    if (rc) return rc;
-  }
-  const bool core = (phases & DAALA_B200_KF_SEARCH_ONLY) != 0;
-  if (phases & DAALA_B200_KF_PVQ_LUMA) {
-    const int rc = enqueue_luma_bands(kf, core, kBeginLuma, s);
-    if (rc) return rc;
-    if (!core && kf->cfg.haar_dc_quant) k_finish_scatter<false, true><<<kf->sms * 8, 256, 0, s>>>(kf->luma);
-    else if (!core) k_finish_scatter<false><<<kf->sms * 8, 256, 0, s>>>(kf->luma);
-  }
-  if (phases & DAALA_B200_KF_PVQ_CHROMA) {
-    enqueue_chroma(kf, core, true, s);
-    if (!core && kf->cfg.symbol_stream) enqueue_sym<false>(kf->sym, kf->sms * 8, s);
-  }
-  if (phases & DAALA_B200_KF_INVERSE) {
-    int rc = kf->cfg.dering ? enqueue_dering(kf, kf->dering, s) : daala_b200_launch_inverse(&kf->frame, 3, s);
-    if (rc) return rc;
-  }
-  return (int)cudaGetLastError();
+  const int rc = enqueue_mc(kf, phases, kf->stream);
+  return rc ? rc : daala_b200_launch_lossless(&kf->ll, kf->stream);
 }
 
 // config.inter_finish: the kernels of the finishing pass, between the H2D of the decisions / levels and the D2H of
@@ -2990,31 +2868,26 @@ int daala_b200_kf_chain_trace(daala_b200_kf* kf, void** recs, int* cap) {
 }
 #endif
 
-// Kernel launches of one whole step (kf_enqueue_step with DAALA_B200_KF_ALL), memset nodes not counted.
+// Kernel launches of one whole step (DAALA_B200_KF_ALL), memset nodes not counted: enqueue_step's pieces in its order.
 int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   if (!kf) return 0;
+  const daala_b200_kf_config& cfg = kf->cfg;
   // lossless: [leaves + OBMC], the forward kernel, [keyframes: the DC + reconstruction kernel]
-  if (kf->cfg.lossless) return (kf->cfg.inter_mc ? 2 : 0) + (kf->cfg.inter ? 1 : 2);
+  if (cfg.lossless) return (cfg.inter_mc ? 2 : 0) + (cfg.inter ? 1 : 2);
+  const bool key = !cfg.inter || cfg.frame_types, pb = cfg.inter != 0;
   auto split = [](const Stage& S) { return 3 * (S.sp_chunks[0] + S.sp_chunks[1] + S.sp_chunks[2]); };
-  // frame_types: work lists (6), [leaves + OBMC], two forward launches, DC chain, begin, luma gather, chains, P-frame luma
-  // phase kernels, luma scatter, chroma gather + phase kernels + scatter, inverse + SB postfilter of plane 0 and 1-2
-  if (kf->cfg.frame_types)
-    return 6 + (kf->cfg.inter_mc ? 2 : 0) + 2 + 1 + 1 + 1 + 1 + split(kf->luma) + 1 + (2 + split(kf->chroma)) + 4;
-  // inter: work lists, two forward launches, per stage gather + phase kernels + finish, inverse + SB postfilter;
-  // inter_mc: leaf enumeration and OBMC
-  // [symbol_stream = 2: the 8 stream kernels]; [late_skip: the size-class split and one launch per class]
-  if (kf->cfg.inter)
-    return 5 + 2 + (2 + split(kf->luma)) + (2 + split(kf->chroma)) + 2 + (kf->cfg.inter_mc ? 2 : 0) +
-           (kf->cfg.symbol_stream ? 8 : 0) + (kf->cfg.late_skip ? kLateSkipLaunches : 0);
-  int n = 5;                                                                      // work lists
-  n += 1 + (kf->cfg.haar_dc_quant ? 1 : 0);                                       // forward, [DC chain]
-  n += 3 + 1;                                                                     // luma: begin (both stages), gather, chains, finish
-  n += 2 + split(kf->chroma);                                                     // chroma: gather, phase kernels, finish
-  // inverse + SB postfilter of plane 0 and of planes 1-2, [the rest of the deringing pass]
-  n += kf->cfg.dering ? dering_launches(kf->dering, 2) : 4;
+  int n = (cfg.inter_mc ? 2 : 0) + 1 + (pb ? 1 : 0);               // [leaves, OBMC], source transform, [prediction's]
+  n += 3 + (key ? 1 : 0) + (pb ? 1 : 0) + 1;                          // work lists: scan, [deps], [luma items], chroma items
+  n += cfg.haar_dc_quant ? 1 : 0;                                     // DC chain
+  n += (key ? 2 : 0) + 1 + (pb ? split(kf->luma) : 0);                // luma: [tickets, chains], gather, [phase kernels]
+  n += 2 + split(kf->chroma);                                         // chroma: gather, phase kernels, scatter
+  n += 1;                                                             // luma scatter
+  n += cfg.late_skip ? kLateSkipLaunches : 0;                         // late skip: size-class split, one launch per class
   // symbol stream: rank, superblock scan, [haar_dc_quant: DC records], place, 3 scan kernels, pack, index
-  if (kf->cfg.symbol_stream) n += 8 + (kf->cfg.haar_dc_quant ? 1 : 0);
-  return n;
+  n += cfg.symbol_stream ? 8 + (cfg.haar_dc_quant ? 1 : 0) : 0;
+  // inverse + SB postfilter of planes 0-2 (forked: plane 0 and planes 1-2), [the rest of the deringing pass]
+  const int parts = kf->side ? 2 : 1;
+  return n + (cfg.dering ? dering_launches(kf->dering, parts) : 2 * parts);
 }
 
 int daala_b200_kf_device_buffers(daala_b200_kf* kf, daala_b200_kf_buffers* out) {
@@ -3076,14 +2949,15 @@ int daala_b200_kf_device_buffers(daala_b200_kf* kf, daala_b200_kf_buffers* out) 
 
 int daala_b200_kf_run_device(daala_b200_kf* kf, int phases, int use_graph) {
   if (!kf) return (int)cudaErrorInvalidValue;
-  if (!use_graph || phases != DAALA_B200_KF_ALL) return kf_enqueue_step(kf, phases);
+  auto enqueue = [&] { return kf->cfg.lossless ? kf_enqueue_step_lossless(kf, phases) : enqueue_step(kf, phases); };
+  if (!use_graph || phases != DAALA_B200_KF_ALL) return enqueue();
   if (!kf->captured) {
     // warm-up outside the capture: module loading and the TMA descriptor encode are not capturable
-    int rc = kf_enqueue_step(kf, phases);
+    int rc = enqueue();
     if (rc) return rc;
     KF_CHECK(cudaStreamSynchronize(kf->stream));
     KF_CHECK(cudaStreamBeginCapture(kf->stream, cudaStreamCaptureModeThreadLocal));
-    rc = kf_enqueue_step(kf, phases);
+    rc = enqueue();
     cudaError_t e = cudaStreamEndCapture(kf->stream, &kf->graph);
     if (rc) return rc;
     KF_CHECK(e);

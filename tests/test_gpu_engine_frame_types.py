@@ -316,6 +316,43 @@ def test_4k_mixed_batch_on_the_bench_maps():
     eng.close()
 
 
+def test_phase_by_phase_equals_the_forked_step():
+    """A mixed batch (keyframes, P and B frames, inter_mc, a record per frame) run phase by phase on one stream, the
+    forked step as live launches and a graph replay all leave the device state of the submitted step graph: the
+    reconstruction, the coefficient planes of the source and of the prediction, the band records, pulses, skip_diff,
+    CfL flips and the keyframe DC indices.  The P / B frames' DC indices reach the coefficient planes."""
+    from tests.test_gpu_step_fork import _assert_same, _state
+    geom = Geometry(200, 130)
+    types = (1, 0, 2, 1)
+    planes, bsize, rec, pool, grids, slots = _inputs(geom, types, seed=31)
+    eng = _mixed(geom, len(types))
+
+    def state():
+        st = _state(eng)
+        for p in range(3):
+            st["pred_coeffs%d" % p] = eng.pred_coeff_plane(p)
+            st["dc_index%d" % p] = eng.download(eng.buf.dc_index[p], (eng.F,) + tuple(s >> 2 for s in geom.plane_shape(p)),
+                                                np.int32)
+        return st
+
+    try:
+        got = _step(eng, planes, bsize, rec, types, pool, grids, slots)   # the forked step graph
+        forked = state()
+        for p in range(3):
+            assert np.array_equal(forked["recon%d" % p], got["recon%d" % p])
+            assert np.array_equal(forked["dc_index%d" % p], got["dc_index%d" % p])
+        assert np.array_equal(forked["chroma_flip"], got["chroma_flip"])
+        for ph in (engine.PH_LISTS, engine.PH_FORWARD, engine.PH_PVQ_LUMA, engine.PH_PVQ_CHROMA, engine.PH_INVERSE):
+            eng.run_device(ph, False)
+        _assert_same(state(), forked, "phase by phase")
+        eng.run_device(engine.PH_ALL, False)   # the forked step as live launches
+        _assert_same(state(), forked, "live launches")
+        eng.run_device(engine.PH_ALL, True)    # and a graph replay
+        _assert_same(state(), forked, "graph replay")
+    finally:
+        eng.close()
+
+
 def test_replay_is_identical_and_refusals_come_with_messages():
     geom = Geometry(200, 130)
     types = (0, 1, 2)
