@@ -508,7 +508,7 @@ struct Stage {
   const int32_t* cfl_in;
   const int32_t* cfl_out;
   const int32_t* cfl_loff;
-  int32_t* dc_resid;               // config.inter_finish or symbol_stream = 2: per block in[0] - ref[0], else NULL
+  int32_t* dc_resid;               // config.inter_finish or symbol_stream 2 / 3: per block in[0] - ref[0], else NULL
   // [F][3][32] each frame's band quantisers max(1, q0 * pvq_qm_q4[pli][i] >> 4), filled on the host from the records
   // (one load per item)
   const int32_t* fq_bq;
@@ -1208,18 +1208,24 @@ struct Sym {
   const int32_t* flip;
   const int32_t* cnt;
   int max_luma, max_chroma;
-  // symbol_stream = 2 (P frames): the DC record of each slot, from the step's DC index and unquantised residual
+  // symbol_stream = 2 (P frames) or 3: the DC record of each slot, from the step's DC index and unquantised residual
   daala_b200_kf_sym_dc* dc;        // [cap_blocks]
   const int32_t* qdc[2];
   const int32_t* dc_resid[2];
   // with config.late_skip: the late-skip record of each slot, from the block-order records (else NULL)
   daala_b200_kf_late_skip* late_skip;   // [cap_blocks]
   const daala_b200_kf_late_skip* ls_block[2];
-  // symbol_stream = 1 with haar_dc_quant: the keyframe DC record of each slot, from the DC chain's index grids (else NULL)
+  // symbol_stream = 1 with haar_dc_quant, or 3: the keyframe DC record of each slot, from the DC chain's index grids
+  // (else NULL)
   daala_b200_kf_sym_hdc* hdc;      // [cap_blocks]
   const int32_t* hdc_index[3];     // [F][gh][gw] per plane
   int gw[3], gh[3];                // index grid width / height (4x4 units of the plane)
+  const uint8_t* ftype;            // symbol_stream = 3: the step's type per frame (1 = keyframe); else NULL
 };
+
+// The forms of the stream: symbol_stream = 1 (keyframes: CfL flips), 2 (P / B frames: DC records) and 3 (mixed
+// batches, config.frame_types: both, each block record in the kind of its frame).
+enum SymForm { kSymKey, kSymInter, kSymMixed };
 
 // Bytes the band's pulses take in the stream: the n - (itheta != -1) values pvq_encode_partition hands to
 // od_encode_pvq_codeword (src/pvq_encoder.c:719-720), one byte each for K <= 127, two above.
@@ -1298,12 +1304,28 @@ __global__ void __launch_bounds__(1024) k_sym_sb_scan(const __grid_constant__ Sy
 // (lane l: units 2l and 2l + 1, as k_sym_rank) of the split nodes whose origin each unit is.  A node is split when it and
 // every ancestor read a size below their own at their origin (max(obs, xdec) < bsi, the map at the node's 8x8 unit);
 // its first leaf is the leaf at its origin unit, whose slot k_sym_rank / k_sym_sb_scan already give.
+// kMixed (symbol_stream = 3): on a P / B frame (S.ftype[f] == 0) the warp zeroes the (superblock, plane)'s L slots
+// instead, so every record of a P / B frame is all zero, a value no keyframe record has (bsi = 4 or child >= 1).
+template <bool kMixed>
 __global__ void __launch_bounds__(256) k_sym_hdc(const __grid_constant__ Sym S) {
   const int lane = threadIdx.x & 31;
   const int item = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (item >= S.F * S.nsb * 3) return;   // whole warps
   const int sb = item / 3, pli = item - 3 * sb;
   const int f = sb / S.nsb, r = sb % S.nsb;
+  if (kMixed && !S.ftype[f]) {   // warp-uniform
+    const uint32_t sc = S.sb_cnt[sb];
+    const int nleaf = pli ? (int)(sc >> 16) : (int)(sc & 0xffff);
+    const long long base = (long long)S.sb_base[sb] + (pli ? (int)(sc & 0xffff) + (pli - 1) * (int)(sc >> 16) : 0);
+    for (int i = lane; i < nleaf && base + i < S.cap_blocks; i += 32) {
+      daala_b200_kf_sym_hdc d;
+      d.value = 0;
+      d.block = 0;
+      d.pli = d.bsi = d.child = d.reserved = 0;
+      S.hdc[base + i] = d;
+    }
+    return;
+  }
   const int sby = r / S.nhsb, sbx = r % S.nhsb;
   const int uw = S.nhsb * 8, xdec = pli ? 1 : 0;
   int b[2], ux[2], uy[2];
@@ -1470,10 +1492,13 @@ __global__ void __launch_bounds__(kTile) k_sym_offsets(const __grid_constant__ S
   if (valid) S.off[i] = make_longlong2(pre.x + s.x - v.x, pre.y + s.y - v.y);
 }
 
-// One warp per slot: the block record, its band records and the pulses of its bands with K > 0.  kInter (symbol_stream
-// = 2): flip is 0 (P frames have no CfL; res_flip is never written) and the slot's DC record is written too, and with
-// config.late_skip its late-skip record.
-template <bool kInter>
+// One warp per slot: the block record, its band records and the pulses of its bands with K > 0.  kSymInter
+// (symbol_stream = 2): flip is 0 (P frames have no CfL; res_flip is never written) and the slot's DC record is written
+// too, and with config.late_skip its late-skip record.  kSymMixed (symbol_stream = 3): the flip from res_flip and the
+// DC record from res_dc / dc_resid for every slot, with no type test: the mixed gather writes res_flip = 0 on the
+// chroma blocks of P / B frames and the mixed scatter res_dc = dc_resid = 0 on keyframe blocks, so each record is that
+// of its frame's kind with the other kind's fields 0.
+template <int kForm>
 __global__ void __launch_bounds__(256) k_sym_pack(const __grid_constant__ Sym S) {
   const int lane = threadIdx.x & 31;
   const long long n = S.tot[0];
@@ -1499,10 +1524,10 @@ __global__ void __launch_bounds__(256) k_sym_pack(const __grid_constant__ Sym S)
       rec.y0 = b.y0;
       rec.bs = b.bs;
       rec.pli = b.pli;
-      rec.flip = !kInter && ch ? (uint8_t)S.flip[blk] : 0;
+      rec.flip = kForm != kSymInter && ch ? (uint8_t)S.flip[blk] : 0;
       rec.reserved = 0;
       S.blocks[slot] = rec;
-      if (kInter) {
+      if (kForm != kSymKey) {
         daala_b200_kf_sym_dc d;
         d.qdc = S.qdc[ch][blk];
         d.dc_resid = S.dc_resid[ch][blk];
@@ -1584,7 +1609,7 @@ __global__ void __launch_bounds__(256) k_sym_copy(const __grid_constant__ SymCop
   }
 }
 
-// symbol_stream = 2 with inter_finish: the finishing pass's decisions given in stream order (finish_io.stream_skip /
+// symbol_stream 2 or 3 with inter_finish: the finishing pass's decisions given in stream order (finish_io.stream_skip /
 // stream_dc, staged in skip / dc) scattered into the block order the pass reads, through the step's slot -> block map.
 // The first node of the finishing graph; `form` (set by each finish call) is 0 for the classic form, which the call
 // copied into fin_skip / fin_dc itself.
@@ -1720,7 +1745,7 @@ struct daala_b200_kf {
   // stored) and the store that reads it
   int32_t* fin_slot_out;
   PoolStore store;
-  // cfg.symbol_stream = 2 with cfg.inter_finish: the decisions of a stream-order finish (staged), the form flag
+  // cfg.symbol_stream 2 or 3 with cfg.inter_finish: the decisions of a stream-order finish (staged), the form flag
   // k_fin_unstream reads, and its parameters
   uint8_t* fin_stream_skip;
   int32_t* fin_stream_dc;
@@ -2117,8 +2142,8 @@ static int kf_alloc(daala_b200_kf* kf) {
   }
   (void)luma_px;
   // the unquantised DC residual per block: what the host's od_rdo_quant needs, returned classically (inter_finish) or
-  // in the stream's DC records (symbol_stream = 2)
-  if (kf->cfg.inter_finish || kf->cfg.symbol_stream == 2)
+  // in the stream's DC records (symbol_stream = 2 or 3)
+  if (kf->cfg.inter_finish || kf->cfg.symbol_stream >= 2)
     for (int c = 0; c < 2; c++) {
       Stage& S = c ? kf->chroma : kf->luma;
       KF_CHECK(dalloc(kf, &kf->dc_resid[c], (size_t)S.max_blocks));
@@ -2163,7 +2188,7 @@ static int kf_alloc(daala_b200_kf* kf) {
     Y.cnt = L.cnt;
     Y.max_luma = L.max_luma;
     Y.max_chroma = L.max_chroma;
-    if (kf->cfg.symbol_stream == 2) {
+    if (kf->cfg.symbol_stream >= 2) {
       KF_CHECK(dalloc(kf, &Y.dc, (size_t)Y.cap_blocks));
       for (int c = 0; c < 2; c++) {
         Y.qdc[c] = (c ? kf->chroma : kf->luma).prm.res_dc;
@@ -2178,6 +2203,7 @@ static int kf_alloc(daala_b200_kf* kf) {
         Y.gh[p] = kf->plane_h[p] >> 2;
       }
     }
+    if (mixed) Y.ftype = kf->ftype;
   }
   if (kf->cfg.late_skip) {
     daala_b200_late_skip_batch& B = kf->lsb;
@@ -2293,7 +2319,7 @@ static int kf_alloc(daala_b200_kf* kf) {
       }
       W.slot = kf->fin_slot_out;
     }
-    if (kf->cfg.symbol_stream == 2) {
+    if (kf->cfg.symbol_stream >= 2) {
       Unstream& U = kf->unstream;
       KF_CHECK(dalloc(kf, &kf->fin_stream_skip, (size_t)kf->sym.cap_blocks));
       KF_CHECK(dalloc(kf, &kf->fin_stream_dc, (size_t)kf->sym.cap_blocks));
@@ -2471,18 +2497,18 @@ static void enqueue_split(daala_b200_kf* kf, const Stage& S, cudaStream_t s) {
 }
 
 // The symbol stream of the step (cfg.symbol_stream), after both stages' k_finish_scatter: rank, superblock scan,
-// [haar_dc_quant: the keyframe DC records, after the DC chain], place, the three scan kernels, pack (kInter: with the DC
-// records), index.
-template <bool kInter>
+// [haar_dc_quant: the keyframe DC records, after the DC chain], place, the three scan kernels, pack (kSymInter /
+// kSymMixed: with the DC records), index.
+template <int kForm>
 static void enqueue_sym(const Sym& Y, int wide, cudaStream_t s) {
   k_sym_rank<<<(Y.F * Y.nsb + 7) / 8, 256, 0, s>>>(Y);
   k_sym_sb_scan<<<1, 1024, 0, s>>>(Y);
-  if (!kInter && Y.hdc) k_sym_hdc<<<(Y.F * Y.nsb * 3 + 7) / 8, 256, 0, s>>>(Y);
+  if (kForm != kSymInter && Y.hdc) k_sym_hdc<kForm == kSymMixed><<<(Y.F * Y.nsb * 3 + 7) / 8, 256, 0, s>>>(Y);
   k_sym_place<<<wide, 256, 0, s>>>(Y);
   k_sym_tile_sums<<<Y.ntiles, kTile, 0, s>>>(Y);
   k_sym_tile_scan<<<1, 1024, 0, s>>>(Y);
   k_sym_offsets<<<Y.ntiles, kTile, 0, s>>>(Y);
-  k_sym_pack<kInter><<<wide, 256, 0, s>>>(Y);
+  k_sym_pack<kForm><<<wide, 256, 0, s>>>(Y);
   k_sym_index<<<1, 256, 0, s>>>(Y);
 }
 
@@ -2520,7 +2546,8 @@ static int enqueue_mc(daala_b200_kf* kf, int phases, cudaStream_t s) {
 //      c, after the gather: [pb: the P / B luma phase kernels];
 //   c, after the chains: the chroma stage (gather -- CfL reads the luma bands in coding order, not the luma scatter --
 //      phase kernels, scatter);  s, after the DC chain and the P / B luma bands: the luma scatter;
-//   c, after the luma scatter: [late skip], [symbol stream];
+//   c, after the luma scatter: [late skip], [symbol stream: its keyframe DC records (k_sym_hdc, haar_dc_quant) read
+//      the DC chain's index grids, which c itself wrote, and the luma scatter it waits for waited for kEvHaarDc];
 //   c: inverse + SB postfilter of planes 1-2;  s: of plane 0, [level search, thresholds, od_dering of plane 0]; join;
 //   s: [od_dering of planes 1-2: they read the direction map plane 0 writes].
 // The side stream has the highest priority: its chroma kernels take the SMs first and the luma branch fills what they
@@ -2615,10 +2642,12 @@ static int enqueue_step(daala_b200_kf* kf, int phases) {
     else k_finish_scatter<false><<<grid, 256, 0, s>>>(kf->luma);
   }
   if (!core && (phases & DAALA_B200_KF_PVQ_CHROMA) && (cfg.late_skip || cfg.symbol_stream)) {
+    // after the luma scatter, and so (hdc) after kEvHaarDc too: the stream's DC records need the DC chain's grids
     STEP_TRY(join(kEvLumaScatter, s, c));
     if (cfg.late_skip) STEP_TRY(daala_b200_late_skip_enqueue(&kf->lsb, kf->sms * 3, c));
-    if (cfg.symbol_stream && pb) enqueue_sym<true>(kf->sym, wide, c);
-    else if (cfg.symbol_stream) enqueue_sym<false>(kf->sym, wide, c);
+    if (cfg.symbol_stream == 3) enqueue_sym<kSymMixed>(kf->sym, wide, c);
+    else if (cfg.symbol_stream && pb) enqueue_sym<kSymInter>(kf->sym, wide, c);
+    else if (cfg.symbol_stream) enqueue_sym<kSymKey>(kf->sym, wide, c);
   }
 
   if (phases & DAALA_B200_KF_INVERSE) {
@@ -2644,7 +2673,7 @@ static int kf_enqueue_step_lossless(daala_b200_kf* kf, int phases) {
 }
 
 // config.inter_finish: the kernels of the finishing pass, between the H2D of the decisions / levels and the D2H of
-// the results.  [symbol_stream = 2: the stream-order decisions into block order], patch and skip map, then the
+// the results.  [symbol_stream 2 / 3: the stream-order decisions into block order], patch and skip map, then the
 // deringing pass with the real skip maps (enqueue_dering: the inverse in place on the patched plane, [inter_finish = 2:
 // the level search], thresholds with the forced level 0, od_dering), [inter_mc: the store of the reconstruction into
 // the pool slots of fin_slot_out].
@@ -2676,8 +2705,9 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
                       : cfg->inter != 1 || cfg->frame_quant != 1 || cfg->haar_dc_quant != 1 ||
                                 (cfg->inter_finish != 1 && cfg->inter_finish != 2)
                           ? "frame_types = 1 requires inter = 1, frame_quant = 1, haar_dc_quant = 1 and inter_finish 1 or 2"
-                      : cfg->symbol_stream ? "frame_types is not defined with symbol_stream (keyframes and P frames have "
-                                             "streams of different formats)"
+                      : cfg->symbol_stream && cfg->symbol_stream != 3
+                          ? "frame_types takes symbol_stream 0 or 3 (3 is the mixed stream; 1 and 2 are the keyframe "
+                            "and P-frame streams)"
                       : cfg->late_skip ? "frame_types is not defined with late_skip"
                       : cfg->lossless ? "frame_types is not defined with lossless"
                       : cfg->dering ? "frame_types is not defined with dering (keyframes are deringed in the finishing pass)"
@@ -2700,10 +2730,11 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
              "daala_b200_kf_create: inter_finish is 0, 1 or 2, and 1 and 2 require inter = 1");
     return nullptr;
   }
-  if (cfg && (cfg->symbol_stream < 0 || cfg->symbol_stream > 2 || (cfg->symbol_stream == 2 && cfg->inter != 1))) {
+  if (cfg && (cfg->symbol_stream < 0 || cfg->symbol_stream > 3 || (cfg->symbol_stream == 2 && cfg->inter != 1) ||
+              (cfg->symbol_stream == 3 && cfg->frame_types != 1))) {
     snprintf(g_create_err, sizeof(g_create_err),
-             "daala_b200_kf_create: symbol_stream is 0, 1 or 2, and 2 requires inter = 1 (a keyframe's DC goes through "
-             "the Haar pyramid and has no scalar index)");
+             "daala_b200_kf_create: symbol_stream is 0, 1, 2 or 3; 2 requires inter = 1 (a keyframe's DC goes through "
+             "the Haar pyramid and has no scalar index) and 3 (the mixed stream) frame_types = 1");
     return nullptr;
   }
   if (cfg && cfg->late_skip && (cfg->late_skip != 1 || cfg->inter != 1)) {
@@ -2883,7 +2914,8 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   n += 2 + split(kf->chroma);                                         // chroma: gather, phase kernels, scatter
   n += 1;                                                             // luma scatter
   n += cfg.late_skip ? kLateSkipLaunches : 0;                         // late skip: size-class split, one launch per class
-  // symbol stream: rank, superblock scan, [haar_dc_quant: DC records], place, 3 scan kernels, pack, index
+  // symbol stream: rank, superblock scan, [haar_dc_quant (symbol_stream 1 or 3): DC records], place, 3 scan kernels,
+  // pack, index
   n += cfg.symbol_stream ? 8 + (cfg.haar_dc_quant ? 1 : 0) : 0;
   // inverse + SB postfilter of planes 0-2 (forked: plane 0 and planes 1-2), [the rest of the deringing pass]
   const int parts = kf->side ? 2 : 1;
@@ -3085,9 +3117,9 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   }
   if (tot.n_luma > kf->lists.max_luma || tot.n_chroma > kf->lists.max_chroma) return (int)cudaErrorInvalidValue;
   const bool have_pred = io->pred_pixels[0] || io->pred_pixels[1] || io->pred_pixels[2];
-  // symbol_stream = 2: the stream's DC records carry the DC indices, so the classic arrays are optional; a lossless
-  // step has no scalar DC index
-  const bool need_dc = !lossless && kf->cfg.symbol_stream != 2 && (!io->luma_dc || !io->chroma_dc);
+  // symbol_stream = 2 or 3: the stream's DC records carry the DC indices, so the classic arrays are optional; a
+  // lossless step has no scalar DC index
+  const bool need_dc = !lossless && kf->cfg.symbol_stream < 2 && (!io->luma_dc || !io->chroma_dc);
   // the lossless outputs: only a lossless engine has them, and only one with the pool stores into it
   const bool want_ll = io->ll_coeffs[0] || io->ll_coeffs[1] || io->ll_coeffs[2] || io->ll_blocks;
   const char* ll_why = (want_ll || io->ll_ref_slot_out) && !lossless
@@ -3194,13 +3226,15 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
   const bool want_sym = io->sym_index || io->sym_blocks || io->sym_bands || io->sym_pulses || io->sym_dc ||
                         io->sym_late_skip || io->sym_hdc;
   if (want_sym) {
-    if (io->sym_hdc && !(kf->cfg.symbol_stream == 1 && kf->cfg.haar_dc_quant)) {
-      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: sym_hdc needs an engine with symbol_stream = 1 and haar_dc_quant = 1");
+    if (io->sym_hdc && !((kf->cfg.symbol_stream == 1 && kf->cfg.haar_dc_quant) || kf->cfg.symbol_stream == 3)) {
+      snprintf(kf->err, sizeof(kf->err),
+               "daala_b200_kf_submit: sym_hdc needs an engine with symbol_stream = 1 and haar_dc_quant = 1, or "
+               "symbol_stream = 3");
       return (int)cudaErrorInvalidValue;
     }
     if (!kf->cfg.symbol_stream) return (int)cudaErrorInvalidValue;
-    if (io->sym_dc && kf->cfg.symbol_stream != 2) {
-      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: sym_dc needs an engine with symbol_stream = 2");
+    if (io->sym_dc && kf->cfg.symbol_stream < 2) {
+      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: sym_dc needs an engine with symbol_stream = 2 or 3");
       return (int)cudaErrorInvalidValue;
     }
     daala_b200_kf_sym_bounds bd;
@@ -3209,8 +3243,13 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     if (!e) e = sym_target(io->sym_blocks, io->sym_blocks_cap, bd.blocks, &sc.dst[1]);
     if (!e) e = sym_target(io->sym_bands, io->sym_bands_cap, bd.bands, &sc.dst[2]);
     if (!e) e = sym_target(io->sym_pulses, io->sym_pulses_cap, bd.pulse_bytes, &sc.dst[3]);
-    if (!e) e = sym_target(io->sym_dc, io->sym_dc_cap, bd.blocks, &sc.dst[4]);
     if (e) return e;
+    if (sym_target(io->sym_dc, io->sym_dc_cap, bd.blocks, &sc.dst[4])) {
+      snprintf(kf->err, sizeof(kf->err),
+               "daala_b200_kf_submit: sym_dc must be pinned host memory of at least "
+               "daala_b200_kf_symbol_bounds(...).blocks records");
+      return (int)cudaErrorInvalidValue;
+    }
     if (sym_target(io->sym_late_skip, io->sym_late_skip_cap, bd.blocks, &sc.dst[5])) {
       snprintf(kf->err, sizeof(kf->err),
                "daala_b200_kf_submit: sym_late_skip must be pinned host memory of at least "
@@ -3384,7 +3423,7 @@ int daala_b200_kf_finish(daala_b200_kf* kf, const daala_b200_kf_finish_io* io) {
                     : stream && classic
                         ? "both forms of the decisions are given (luma_skip / chroma_skip / luma_dc / chroma_dc and "
                           "stream_skip / stream_dc): give one"
-                    : stream && !kf->fin_form ? "stream_skip / stream_dc need an engine with symbol_stream = 2"
+                    : stream && !kf->fin_form ? "stream_skip / stream_dc need an engine with symbol_stream = 2 or 3"
                     : stream && (!io->stream_skip || !io->stream_dc) ? "stream_skip and stream_dc are required together"
                     : !stream && (!skip[0] || !skip[1] || !dc[0] || !dc[1])
                         ? "luma_skip, chroma_skip, luma_dc and chroma_dc are required"
@@ -3491,10 +3530,15 @@ int daala_b200_kf_encode(daala_b200_kf* kf, const daala_b200_kf_io* io) {
 }
 
 // Synchronous copy helper for tests / device-resident callers without a CUDA binding of their own:
-// kind 0 = host -> device, 1 = device -> host, 2 = device -> device.
+// kind 0 = host -> device, 1 = device -> host, 2 = device -> device.  cudaMemcpy alone returns before the data has
+// landed for a pageable host -> device or a device -> device copy, and the engines' streams are non-blocking, so they
+// do not wait for it: a step launched right after an upload could read half of a new block-size map, build work lists
+// that disagree with each other, and leave the luma chain kernel waiting for band-0 items that never come.  The copy
+// is complete when this returns.
 int daala_b200_device_copy(void* dst, const void* src, size_t bytes, int kind) {
   const cudaMemcpyKind k = kind == 0 ? cudaMemcpyHostToDevice : kind == 1 ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
   cudaError_t e = cudaMemcpy(dst, src, bytes, k);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(cudaStreamLegacy);
   return (int)e;
 }
 

@@ -42,7 +42,9 @@ With frame_types=1 (on an inter=1, frame_quant=1, haar_dc_quant=1 engine with in
 and P / B frames: `encode(..., frame_type=)` takes one type per frame (1 = keyframe, 0 = P or B frame), each keyframe is
 coded as a keyframe_quant=1, haar_dc_quant=1 engine codes it and each P / B frame as the frame_quant=1 inter engine
 does, and the results are those of both kinds.  The finishing pass deringes the keyframes too, and ref_slot_out stores
-them in the pool, so one engine codes a whole GOP.
+them in the pool, so one engine codes a whole GOP.  With symbol_stream=3 too each step returns the mixed stream: every
+frame's block records in the kind of its frame (a keyframe's with its CfL flips and sym_hdc records, a P / B frame's
+with its sym_dc records; the other kind's records are zero), and `finish_stream` takes the decisions in its order.
 
 No torch here: device memory, streams and the CUDA graph belong to the engine."""
 import ctypes
@@ -451,11 +453,12 @@ class KeyframeEngine:
         """Builds the daala_b200_kf_io record over the staged inputs and result buffers sized for them.
         stream (default: whether the engine was created with symbol_stream) adds the symbol stream buffers
         sym_index, sym_blocks, sym_bands and sym_pulses (daala_b200/symbols.py), and sym_dc on a symbol_stream=2
-        engine (and sym_late_skip on one with late_skip too), or sym_hdc on a symbol_stream=1 engine with
-        haar_dc_quant, pinned and sized by daala_b200_kf_symbol_bounds; only their used part is copied back.
+        engine (and sym_late_skip on one with late_skip too), sym_hdc on a symbol_stream=1 engine with
+        haar_dc_quant, or both sym_dc and sym_hdc on a symbol_stream=3 engine, pinned and sized by
+        daala_b200_kf_symbol_bounds; only their used part is copied back.
         late_skip engines return luma_late_skip / chroma_late_skip (symbols.LATE_SKIP_DTYPE per block, block order)
-        with the symbols.  On a symbol_stream=2 engine symbols=False also leaves out the classic DC arrays (the stream
-        carries them).  pred=False (inter_mc engines): the prediction planes are not copied back.  dc_grids=False
+        with the symbols.  On a symbol_stream=2 or 3 engine symbols=False also leaves out the classic DC arrays (the
+        stream carries them).  pred=False (inter_mc engines): the prediction planes are not copied back.  dc_grids=False
         (haar_dc_quant engines): the index grids dc_index0..2 are not copied back (sym_hdc carries the same indices)."""
         if self.lossless:
             return self._prepare_io_lossless(recon, pred)
@@ -509,12 +512,12 @@ class KeyframeEngine:
             if not self.inter_mc:
                 for p in range(3):
                     io.pred_pixels[p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8).ctypes.data
-        classic_dc = symbols or self.symbol_stream != 2
+        classic_dc = symbols or self.symbol_stream < 2
         if self.inter and classic_dc:
             out["luma_dc"] = self._arr("ld", (int(t.n_luma),), np.int32)
             out["chroma_dc"] = self._arr("cd", (int(t.n_chroma),), np.int32)
             io.luma_dc, io.chroma_dc = out["luma_dc"].ctypes.data, out["chroma_dc"].ctypes.data
-        if (self.inter_finish or self.symbol_stream == 2) and classic_dc:
+        if (self.inter_finish or self.symbol_stream >= 2) and classic_dc:
             out["luma_dc_resid"] = self._arr("ldr", (int(t.n_luma),), np.int32)
             out["chroma_dc_resid"] = self._arr("cdr", (int(t.n_chroma),), np.int32)
             io.luma_dc_resid, io.chroma_dc_resid = out["luma_dc_resid"].ctypes.data, out["chroma_dc_resid"].ctypes.data
@@ -546,13 +549,13 @@ class KeyframeEngine:
                            ("sym_pulses", b.pulse_bytes)):
                 setattr(io, k, out[k].ctypes.data)
                 setattr(io, k + "_cap", int(cap))
-            if self.symbol_stream == 2:
+            if self.symbol_stream >= 2:
                 out["sym_dc"] = self._arr("sd", (int(b.blocks),), sym.DC_DTYPE, pinned=True)
                 io.sym_dc, io.sym_dc_cap = out["sym_dc"].ctypes.data, int(b.blocks)
                 if self.late_skip:
                     out["sym_late_skip"] = self._arr("sls", (int(b.blocks),), sym.LATE_SKIP_DTYPE, pinned=True)
                     io.sym_late_skip, io.sym_late_skip_cap = out["sym_late_skip"].ctypes.data, int(b.blocks)
-            elif self.haar_dc_quant:
+            if self.haar_dc_quant:
                 out["sym_hdc"] = self._arr("shdc", (int(b.blocks),), sym.HDC_DTYPE, pinned=True)
                 io.sym_hdc, io.sym_hdc_cap = out["sym_hdc"].ctypes.data, int(b.blocks)
         self._io, self._out = io, out
@@ -638,7 +641,8 @@ class KeyframeEngine:
     def stream_d2h_bytes(self):
         """Bytes the last submit copied of the symbol stream (after wait): the index and the used part of the
         other arrays (block records, band records, pulses and, on symbol_stream=2 engines, DC records and, with
-        late_skip, late-skip records; with haar_dc_quant, the keyframe DC records)."""
+        late_skip, late-skip records; with haar_dc_quant, the keyframe DC records; on symbol_stream=3 engines both the
+        DC records and the keyframe DC records)."""
         from . import symbols as sym
         idx = self._out["sym_index"]
         blocks = int(idx[:, 1].sum())
@@ -705,9 +709,10 @@ class KeyframeEngine:
         return self._prepare_finish_rest(fio, sum(n.values()), dering_levels, ref_slot_out)
 
     def prepare_finish_stream(self, skip, dc, dering_levels=None, ref_slot_out=None):
-        """prepare_finish with the decisions in stream order (symbol_stream=2 engines with inter_finish): skip and dc
-        have one entry per block record of the last step's stream, frames one after the other (the order of its
-        sym_blocks).  symbols.stream_to_classic gives each record's index in the classic block order."""
+        """prepare_finish with the decisions in stream order (symbol_stream=2 or 3 engines with inter_finish): skip
+        and dc have one entry per block record of the last step's stream, frames one after the other (the order of its
+        sym_blocks).  symbols.stream_to_classic gives each record's index in the classic block order.  On a
+        symbol_stream=3 engine the keyframes' entries are checked as any other and otherwise not read."""
         t = self.totals
         fio = FinishIO()
         n = int(t.n_luma) + int(t.n_chroma)

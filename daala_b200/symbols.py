@@ -1,7 +1,10 @@
 """The keyframe engine's symbol stream (include/daala_b200.h, "Symbol stream"; config.symbol_stream = 1): per
 frame the PVQ symbols the serial entropy coder reads, in bitstream order.  The P-frame stream (symbol_stream = 2,
 inter = 1) is the same with flip = 0 and a DC_DTYPE record per block record (sym_dc, same index): the step's scalar
-DC index and the unquantised DC residual; with late_skip = 1 also a LATE_SKIP_DTYPE record (sym_late_skip).
+DC index and the unquantised DC residual; with late_skip = 1 also a LATE_SKIP_DTYPE record (sym_late_skip).  The
+mixed stream (symbol_stream = 3, frame_types = 1) has both record kinds: each frame's block records in the kind of its
+frame, a keyframe's with its CfL flips, HDC_DTYPE records and zero DC_DTYPE records, a P / B frame's with flip 0,
+DC_DTYPE records and zero HDC_DTYPE records (no keyframe record is all zero: bsi = 4 or child >= 1).
 
 For each frame of a batch the index (int64[6]: first block, block count, first band, band count, first pulse
 byte, pulse byte count) locates three parts inside batch-wide arrays:
@@ -185,28 +188,32 @@ def concat_frames(parts):
     return r
 
 
-def pack_reference(out, frames):
+def pack_reference(out, frames, frame_type=None):
     """The stream the engine must produce, built from a submit's classic outputs (luma_/chroma_blocks, _res,
     _y16, _skip_diff, chroma_flip) for the frames `frames` (list, or a count = frames 0 .. count-1).  Blocks are
     put in bitstream order by sorting on (superblock, plane, Z order of the origin), independently of how the
     device ranks them.  Returns dict(sym_index, sym_blocks, sym_bands, sym_pulses) over those frames.  The outputs of
     a P-frame step (they have luma_dc / chroma_dc, and luma_dc_resid / chroma_dc_resid must be there too) give the
     P-frame stream: flip 0 and sym_dc from *_dc and *_dc_resid.  Those of a haar_dc_quant keyframe step with the index
-    grids (dc_index0..2) give sym_hdc too (haardc.stream_records over the map the luma blocks tile)."""
+    grids (dc_index0..2) give sym_hdc too (haardc.stream_records over the map the luma blocks tile).
+    frame_type (the type of every frame of the step, 1 = keyframe) gives the mixed stream (symbol_stream = 3) from a
+    frame_types step's outputs, which have both: each keyframe's records as the keyframe stream has them with a zero
+    sym_dc record, each P / B frame's as the P-frame stream has them with a zero sym_hdc record."""
     frames = list(range(frames)) if np.isscalar(frames) else list(frames)
     inter = "luma_dc" in out
-    hdc = not inter and "dc_index0" in out
+    hdc = (frame_type is not None or not inter) and "dc_index0" in out
     lb, cb = out["luma_blocks"], out["chroma_blocks"]
     nl_coefs = len(out["luma_y16"])
     y = np.concatenate([out["luma_y16"], out["chroma_y16"]])
-    parts = []
+    parts, hdcs = [], []
     for f in frames:
+        key = not inter if frame_type is None else bool(frame_type[f])
         sl, sc = np.nonzero(lb["frame"] == f)[0], np.nonzero(cb["frame"] == f)[0]
         blk = np.concatenate([lb[sl], cb[sc]])
         res = np.concatenate([out["luma_res"][sl], out["chroma_res"][sc]])
         skip = np.concatenate([out["luma_skip_diff"][sl], out["chroma_skip_diff"][sc]])
         flip = np.zeros(len(blk), np.int64)
-        if not inter:
+        if key:
             flip[len(sl):] = out["chroma_flip"][sc]
         y_off = np.concatenate([lb["coef_off"][sl].astype(np.int64), cb["coef_off"][sc].astype(np.int64) + nl_coefs])
         pli = blk["pli"].astype(np.int64)
@@ -215,14 +222,15 @@ def pack_reference(out, frames):
         dc = {}
         if inter:
             for k in ("dc", "dc_resid"):
-                dc[k] = np.concatenate([out["luma_" + k][sl], out["chroma_" + k][sc]])[o]
+                v = np.concatenate([out["luma_" + k][sl], out["chroma_" + k][sc]])[o]
+                dc[k] = np.zeros_like(v) if key else v
         parts.append(pack_blocks(blk["x0"][o], blk["y0"][o], blk["bs"][o], pli[o], flip[o], skip[o], res[o], y,
                                  y_off[o], dc.get("dc"), dc.get("dc_resid")))
         if hdc:
-            parts[-1] = parts[-1][:3] + (_hdc_reference(out, lb[sl], f),)
+            hdcs.append(_hdc_reference(out, lb[sl], f) if key else np.zeros(len(blk), HDC_DTYPE))
     r = concat_frames(parts)
     if hdc:
-        r["sym_hdc"] = r.pop("sym_dc")
+        r["sym_hdc"] = np.concatenate(hdcs) if hdcs else np.zeros(0, HDC_DTYPE)
     return r
 
 

@@ -468,8 +468,15 @@ typedef struct daala_b200_kf_config {
                                   2: the P-frame stream (requires inter = 1): the stream of 1 with flip = 0 and one
                                   daala_b200_kf_sym_dc record per block (daala_b200_kf_io.sym_dc); with inter_finish
                                   the finishing pass also takes its decisions in stream order
-                                  (daala_b200_kf_finish_io.stream_skip / stream_dc).  1 is refused with inter (a
-                                  keyframe block has no scalar DC), 2 without it; other values are refused */
+                                  (daala_b200_kf_finish_io.stream_skip / stream_dc).
+                                  3: the mixed stream of a frame_types = 1 engine: each frame's block records in the
+                                  kind of its frame, a keyframe's as 1 with haar_dc_quant writes them (CfL flip,
+                                  daala_b200_kf_sym_hdc records; its daala_b200_kf_sym_dc records are {0, 0}), a P / B
+                                  frame's as 2 does (flip 0, daala_b200_kf_sym_dc records; its daala_b200_kf_sym_hdc
+                                  records are all zero, which no keyframe record is); with inter_finish the finishing
+                                  pass takes its decisions in stream order as with 2.
+                                  1 is refused with inter (a keyframe block has no scalar DC), 2 without it, 3 without
+                                  frame_types and 1 and 2 with it; other values are refused */
   int inter;                   /* 0 (default): keyframes, exactly the engine described above.
                                   1: P-frame residual mode.  Every frame is coded as od_encode_coefficients codes a
                                   non-key frame, entropy coding and the coder-state skip decision left to the host:
@@ -582,9 +589,9 @@ typedef struct daala_b200_kf_config {
                                   keyframe rule searches (inter_finish = 2: every superblock, up / left CDF context);
                                   ref_slot_out stores keyframes like any other frame.  Requires inter = 1, frame_quant = 1,
                                   haar_dc_quant = 1 and inter_finish 1 or 2 (inter_mc and mc_next are allowed); refused by
-                                  daala_b200_kf_create with a value other than 0 or 1, and 1 together with symbol_stream,
-                                  late_skip, lossless, dering (a keyframe is deringed in the finishing pass) or a row
-                                  shard (sb_rows > 0) */
+                                  daala_b200_kf_create with a value other than 0 or 1, and 1 together with symbol_stream
+                                  1 or 2 (3 is the mixed stream), late_skip, lossless, dering (a keyframe is deringed in
+                                  the finishing pass) or a row shard (sb_rows > 0) */
 } daala_b200_kf_config;
 
 /* config.lossless: the root sums of one block (od_compute_max_tree, src/encode.c:899-919, over the residual of
@@ -647,8 +654,9 @@ typedef struct daala_b200_kf_sym_block {   /* 24 bytes, 8-byte aligned */
   uint8_t reserved;        /* 0 */
 } daala_b200_kf_sym_block;
 
-/* symbol_stream = 2 (P frames): one record per block record, at the same index as the daala_b200_kf_sym_block it
-   belongs to (a frame's part is first_block / n_blocks of the index, as for the block records). */
+/* symbol_stream = 2 (P frames) and 3 (mixed batches; {0, 0} on a keyframe's block records): one record per block
+   record, at the same index as the daala_b200_kf_sym_block it belongs to (a frame's part is first_block / n_blocks of
+   the index, as for the block records). */
 typedef struct daala_b200_kf_sym_dc {      /* 8 bytes */
   int32_t qdc;             /* the step's scalar DC index (as daala_b200_kf_io.luma_dc / chroma_dc) */
   int32_t dc_resid;        /* the unquantised DC residual in[0] - ref[0] (as daala_b200_kf_io.*_dc_resid), what the
@@ -682,7 +690,9 @@ typedef struct daala_b200_kf_late_skip {   /* 32 bytes */
   double noskip_pred_dcq;   /* ... AC = md (PVQ skip), d[0] = md[0] + q1 * dc_quant */
 } daala_b200_kf_late_skip;
 
-/* Engines with symbol_stream = 1 and haar_dc_quant = 1: the keyframe's DC symbols in the order od_encode_coefficients
+/* Engines with symbol_stream = 1 and haar_dc_quant = 1, and keyframes in the mixed stream (symbol_stream = 3, where a
+   P / B frame's records are all zero: no keyframe record is, since the superblock DC has bsi = 4 and every other record
+   child >= 1, so an all-zero record marks a P / B frame): the keyframe's DC symbols in the order od_encode_coefficients
    codes them (reference src/encode.c:2605-2656, :1765-1787), one record per block record, so a frame's part is
    first_block / n_blocks of the index as for the block records.  A quadtree with L leaves has (L - 1) / 3 split nodes,
    and the reference codes one superblock DC per (superblock, plane) and three indices per split node: L symbols.  Per
@@ -744,7 +754,7 @@ typedef struct daala_b200_kf_io {
   long long sym_bands_cap;
   uint8_t *sym_pulses;
   long long sym_pulses_cap;
-  /* config.inter only (required there, ignored otherwise; luma_dc / chroma_dc are optional with symbol_stream = 2,
+  /* config.inter only (required there, ignored otherwise; luma_dc / chroma_dc are optional with symbol_stream = 2 or 3,
      whose sym_dc carries the same indices). */
   const uint8_t *pred_pixels[3];        /* motion-compensated prediction planes, shapes and padding of `pixels` */
   int32_t *luma_dc, *chroma_dc;         /* [n_blocks]: the scalar-quantised DC index qdc of each block (keyframes code
@@ -757,7 +767,7 @@ typedef struct daala_b200_kf_io {
                                            when the frame predicts from one picture) */
   const daala_b200_mv_pt *mv_grid;      /* [nframes][nvsb*8 + 1][nhsb*8 + 1]: each frame's state->mv_grid */
   uint8_t *pred_pixels_out[3];          /* optional: the prediction planes the engine made, layout of pixels */
-  /* config.inter_finish or symbol_stream = 2 only (optional, NULL = not copied). */
+  /* config.inter_finish or symbol_stream = 2 / 3 only (optional, NULL = not copied). */
   int32_t *luma_dc_resid, *chroma_dc_resid; /* [n_blocks]: each block's unquantised DC residual in[0] - ref[0] (what the
                                            host's od_rdo_quant quantises, src/pvq_encoder.c:886 / :956), block order
                                            of luma_dc / chroma_dc */
@@ -768,9 +778,9 @@ typedef struct daala_b200_kf_io {
      daala_b200_kf_finish_io.ref_slot_out has written it.  Everything is ordered by call order on the engine's
      stream: a step submitted before the finish that rewrites its PREV slot reads the old picture. */
   int ref_resident;
-  /* config.symbol_stream = 2 only: the DC records of the stream (daala_b200_kf_sym_dc), a pinned host buffer with its
-     capacity in records, at least daala_b200_kf_symbol_bounds(...).blocks; NULL = not copied.  Only the used part is
-     copied, as for the other stream arrays. */
+  /* config.symbol_stream = 2 or 3 only: the DC records of the stream (daala_b200_kf_sym_dc), a pinned host buffer with
+     its capacity in records, at least daala_b200_kf_symbol_bounds(...).blocks; NULL = not copied.  Only the used part
+     is copied, as for the other stream arrays. */
   daala_b200_kf_sym_dc *sym_dc;
   long long sym_dc_cap;
   /* config.late_skip = 1 only (optional, NULL = not copied): the late-skip records (daala_b200_kf_late_skip) in the
@@ -808,9 +818,10 @@ typedef struct daala_b200_kf_io {
      children 1, 2, 3 (top right, bottom left, bottom right), 0 everywhere else.  INTEGRATION.md describes the order
      the coder reads them in. */
   int32_t *dc_index[3];
-  /* config.symbol_stream = 1 with haar_dc_quant = 1 only (refused otherwise): the keyframe DC records of the stream
-     (daala_b200_kf_sym_hdc), a pinned host buffer with its capacity in records, at least
-     daala_b200_kf_symbol_bounds(...).blocks; NULL = not copied.  Only the used part is copied, as for sym_dc. */
+  /* config.symbol_stream = 1 with haar_dc_quant = 1, or symbol_stream = 3, only (refused otherwise): the keyframe DC
+     records of the stream (daala_b200_kf_sym_hdc; all zero on a P / B frame's block records of the mixed stream), a
+     pinned host buffer with its capacity in records, at least daala_b200_kf_symbol_bounds(...).blocks; NULL = not
+     copied.  Only the used part is copied, as for sym_dc.  With them the index grids dc_index are optional. */
   daala_b200_kf_sym_hdc *sym_hdc;
   long long sym_hdc_cap;
   /* config.frame_types = 1 only (required there, refused otherwise): [nframes] 1 = keyframe, 0 = P or B frame; any other
@@ -869,9 +880,11 @@ typedef struct daala_b200_kf_finish_io {
                                               Rewriting a slot the last step read (a frame's own PREV slot) is legal:
                                               the step's prediction and md are already made, and a repeated finish
                                               reads md, never the pool; the last finish wins. */
-  /* The decisions in stream order (engines with config.symbol_stream = 2): one entry per block of the last submitted
-     step, in the order of that step's sym_blocks, frames one after the other (n_luma + n_chroma entries).  A call
-     gives either these two or the four classic arrays above, never both; the same checks apply to either form. */
+  /* The decisions in stream order (engines with config.symbol_stream = 2 or 3): one entry per block of the last
+     submitted step, in the order of that step's sym_blocks, frames one after the other (n_luma + n_chroma entries).  A
+     call gives either these two or the four classic arrays above, never both; the same checks apply to either form.
+     With symbol_stream = 3 a keyframe's entries are checked like the others and otherwise not read, as in the classic
+     form. */
   const uint8_t *stream_skip;              /* 0 or 1 */
   const int32_t *stream_dc;                /* the final DC index */
 } daala_b200_kf_finish_io;
@@ -915,9 +928,9 @@ typedef struct daala_b200_kf_buffers {  /* device pointers of an engine (tests, 
                                            4x4 unit (leaf DCs at leaf origins), the three planes of a frame together
                                            (frame f of plane p at haar_dc[p] + f * (g0 + 2 g1), g = plane grid size) */
   int32_t *dc_index[3];                 /* and the index grids ([nframes][plane_h / 4][plane_w / 4]); else NULL */
-  daala_b200_kf_sym_hdc *sym_hdc;       /* config.symbol_stream = 1 with haar_dc_quant: the step's keyframe DC records,
-                                           the frames one after the other from index 0 (what io.sym_hdc receives,
-                                           max_luma_blocks + max_chroma_blocks entries); else NULL */
+  daala_b200_kf_sym_hdc *sym_hdc;       /* config.symbol_stream = 1 with haar_dc_quant, or 3: the step's keyframe DC
+                                           records, the frames one after the other from index 0 (what io.sym_hdc
+                                           receives, max_luma_blocks + max_chroma_blocks entries); else NULL */
 } daala_b200_kf_buffers;
 
 #define DAALA_B200_KF_LISTS 1
@@ -950,10 +963,11 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daal
    H2D of the inputs, the whole step, D2H of the requested outputs: enqueued, not waited for.  A batch with more
    luma or chroma blocks than the engine's capacity (see max_blocks_div) returns cudaErrorInvalidValue before
    anything is copied or launched; so does a request for symbol stream outputs from an engine created without
-   symbol_stream (sym_dc: without symbol_stream = 2), a stream capacity below daala_b200_kf_symbol_bounds, a stream
+   symbol_stream (sym_dc: without symbol_stream 2 or 3), a stream capacity below daala_b200_kf_symbol_bounds, a stream
    buffer that is not pinned host memory, or (config.inter) a NULL pred_pixels plane, luma_dc or chroma_dc (the last
-   two are optional with symbol_stream = 2), a late-skip output on an engine without late_skip, sym_late_skip
-   without symbol_stream = 2, and sym_hdc on an engine without both symbol_stream = 1 and haar_dc_quant = 1, below
+   two are optional with symbol_stream 2 or 3), a late-skip output on an engine without late_skip, sym_late_skip
+   without symbol_stream = 2, sym_dc below daala_b200_kf_symbol_bounds(...).blocks records or not pinned, and sym_hdc
+   on an engine without both symbol_stream = 1 and haar_dc_quant = 1 or symbol_stream = 3, below
    daala_b200_kf_symbol_bounds(...).blocks records or not pinned (each with a message in daala_b200_kf_error).  With config.inter_mc it refuses, the same
    way, a NULL mv_grid, ref_pixels plane or ref_slot, pred_pixels given, nrefs outside [1, mc_refs] and a slot outside
    [0, nrefs); with ref_resident = 1 it refuses instead ref_pixels given, nrefs other than 0, a slot outside
@@ -987,7 +1001,7 @@ int daala_b200_kf_load_frame_quant(daala_b200_kf *kf, const daala_b200_kf_frame_
    applied to a plane of their own), so the pass may run any number of times after one step.  Refused with
    cudaErrorInvalidValue and a message in daala_b200_kf_error, before anything is copied or launched: an engine
    without inter_finish, no step submitted yet, a NULL decision array (neither form complete), both forms given, the
-   stream form on an engine without symbol_stream = 2, a skip value other than 0 or 1, a level above
+   stream form on an engine without symbol_stream 2 or 3, a skip value other than 0 or 1, a level above
    5, a |dc| above DAALA_B200_KF_FINISH_DC_LIMIT / DQ, (config.inter_finish = 2) a non-NULL dering_level, and a
    ref_slot_out on an engine without inter_mc, with an entry outside [-1, mc_refs) or with two frames naming one slot.
    With ref_slot_out the pass's last kernel copies each stored frame's reconstruction into its pool slot.  With the

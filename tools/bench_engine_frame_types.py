@@ -14,7 +14,14 @@ around --steps replays, daala_b200_kf_time_device) of an all-P batch on the mixe
 inter engine: the cost of carrying the mode.  Reports bytes_allocated of every engine and the card's name and power
 limit.  Needs a CUDA device; prints one JSON line.
 
-    python tools/bench_engine_frame_types.py [--rounds 3] [--steps 5]
+--stream measures the mixed symbol stream (symbol_stream = 3) instead, on the same 1 keyframe + 15 P frame step: the
+step graph's device time on the mixed engine with symbol_stream 0 and 3 (CUDA events around --steps replays,
+daala_b200_kf_time_device, the two engines alternated over --rounds rounds, same inputs and pool contents), and the
+step's D2H bytes of the stream route (encode(..., symbols=False, dc_grids=False): reconstruction, prediction, counters
+and the used part of the stream with its DC and keyframe DC records) against the classic route (the same outputs with
+the block-order arrays and the DC index grids in place of the stream).
+
+    python tools/bench_engine_frame_types.py [--rounds 3] [--steps 5] [--stream]
 """
 import argparse
 import json
@@ -45,6 +52,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--stream", action="store_true", help="the mixed symbol stream (symbol_stream = 3) instead")
     args = ap.parse_args()
     geom, F = Geometry(3840, 2160), 16
     real = np.load(os.path.join(ROOT, "daala_b200", "data", "bench_bsize_4k.npz"))
@@ -60,6 +68,9 @@ def main():
     types = np.array([1] + [0] * (F - 1), np.uint8)
     slot = np.zeros((F, 2), np.int32)
     slot[:, 1] = 1
+    if args.stream:
+        print(json.dumps(stream_result(args, geom, planes, bsize, pool, grid, rec, types, slot)))
+        return
 
     def finish_inputs(eng, out):
         return (np.zeros(len(out["luma_blocks"]), np.uint8), np.array(out["luma_dc"]),
@@ -124,6 +135,40 @@ def main():
     plain.close()
     mixed.close()
     print(json.dumps(result))
+
+
+def stream_result(args, geom, planes, bsize, pool, grid, rec, types, slot):
+    """--stream: the step graph with and without the mixed stream, and the step's D2H bytes by route."""
+    from daala_b200 import engine
+    F = len(types)
+    engines = {s: engine.KeyframeEngine(geom, nframes=F, inter=1, inter_mc=1, mc_refs=F + 2, frame_quant=1,
+                                        haar_dc_quant=1, inter_finish=1, frame_types=1, symbol_stream=s) for s in (0, 3)}
+    kw = dict(frame_quant=rec, frame_type=types, refs=pool, ref_slot=slot, mv_grid=grid)
+    try:
+        engines[0].encode(planes, bsize, **kw)
+        classic = engines[0].d2h_bytes
+        out = engines[3].encode(planes, bsize, symbols=False, dc_grids=False, **kw)
+        fixed, stream = engines[3].d2h_bytes, engines[3].stream_d2h_bytes()
+        blocks = int(out["sym_index"][:, 1].sum())
+        step = {"symbol_stream_0": [], "symbol_stream_3": []}
+        for s, eng in engines.items():
+            eng.time_device(reps=1)   # warm-up of the graph as it is timed
+        for _ in range(args.rounds):
+            for s, eng in engines.items():
+                step["symbol_stream_%d" % s].append(eng.time_device(reps=args.steps) / args.steps)
+        med = {k: statistics.median(v) for k, v in step.items()}
+        return {"metric": "frame_types_stream", "card": card(), "geometry": "%dx%d" % (geom.pic_w, geom.pic_h),
+                "frames": F, "keyframes": int(types.sum()),
+                "step_graph_ms": {k: {"median": med[k], "all": v} for k, v in step.items()},
+                "stream_cost_ms": med["symbol_stream_3"] - med["symbol_stream_0"],
+                "d2h_bytes": {"classic_route": classic, "stream_route": fixed + stream,
+                              "stream_route_stream_part": stream, "stream_route_other_part": fixed},
+                "stream_blocks": blocks,
+                "launches_per_step": {k: e.launches_per_step() for k, e in (("symbol_stream_0", engines[0]),
+                                                                             ("symbol_stream_3", engines[3]))}}
+    finally:
+        for eng in engines.values():
+            eng.close()
 
 
 if __name__ == "__main__":
