@@ -1671,8 +1671,15 @@ struct Dering {
 // The events of enqueue_step's two-stream form, one per fork or join.
 enum { kEvLists, kEvForward, kEvLumaBands, kEvLumaScatter, kEvChroma, kEvHaarDc, kEvLumaGather, kEvInterLuma, kNumEvents };
 
+// The kernel form of a lossy step: which k_gather, k_finish_scatter and enqueue_sym instantiation it launches.
+enum StepForm { kFormKey, kFormKeyHdc, kFormInter, kFormMixed };
+
 struct daala_b200_kf {
   daala_b200_kf_config cfg;
+  // the engine's mode, fixed at create: the batch can hold keyframes (!inter, or frame_types) and / or P / B frames
+  // (inter); mixed: both (frame_types)
+  bool key, pb, mixed;
+  StepForm form;
   int nhsb, nvsb, F;
   int plane_w[3], plane_h[3];
   cudaStream_t stream;
@@ -1692,11 +1699,6 @@ struct daala_b200_kf {
   uint8_t* bsize;
   int16_t *qm, *qm_inv;
   double* rsqrt_tbl;
-  int16_t* sp_vec[3];
-  int32_t* sp_lanes[3];
-  int32_t* sp_uni[3];
-  int16_t* sp_snap[3];
-  int sp_slots[3];
   Dering dering;                   // cfg.dering or cfg.inter_finish
   Lists lists;
   Stage luma, chroma;
@@ -1787,6 +1789,12 @@ struct daala_b200_kf {
     }                                                                                     \
   } while (0)
 
+#define STEP_TRY(x)           \
+  do {                        \
+    const int rc_ = (int)(x); \
+    if (rc_) return rc_;      \
+  } while (0)
+
 template <class T>
 static cudaError_t dalloc(daala_b200_kf* kf, T** p, size_t n) {
   const size_t bytes = (n ? n : 1) * sizeof(T);
@@ -1838,7 +1846,6 @@ static int mc_alloc(daala_b200_kf* kf) {
 static int ll_alloc(daala_b200_kf* kf) {
   const int F = kf->F;
   daala_b200_lossless_batch& B = kf->ll;
-  memset(&B, 0, sizeof(B));
   for (int p = 0; p < 3; p++) {
     const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
     KF_CHECK(dalloc(kf, &kf->pixels[p], n));
@@ -1859,8 +1866,7 @@ static int ll_alloc(daala_b200_kf* kf) {
   kf->mc.bad_ref = kf->lists.cnt + kMcBadRef;
   kf->mc.beyond = kf->lists.cnt + kMcBeyond;
   if (kf->cfg.inter_mc) {
-    int rc = mc_alloc(kf);
-    if (rc) return rc;
+    STEP_TRY(mc_alloc(kf));
     KF_CHECK(dalloc(kf, &kf->ll_slot_out, (size_t)F));
     for (int p = 0; p < 3; p++) B.pool[p] = kf->ref_pixels[p];
     B.slot_out = kf->ll_slot_out;
@@ -1910,45 +1916,15 @@ static cudaError_t fq_copy(daala_b200_kf* kf, const daala_b200_kf_frame_quant* r
   return e;
 }
 
-static int kf_alloc(daala_b200_kf* kf) {
-  if (kf->cfg.lossless) return ll_alloc(kf);
-  const int F = kf->F;
-  const bool inter = kf->cfg.inter != 0;
-  // frame_types: an inter engine that also has everything the keyframe chains, CfL and the DC chain need
-  const bool mixed = kf->cfg.frame_types != 0;
-  if (mixed) KF_CHECK(dalloc(kf, &kf->ftype, (size_t)F));
-  const long long luma_px = (long long)kf->plane_w[0] * kf->plane_h[0];
-  for (int p = 0; p < 3; p++) {
-    const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
-    KF_CHECK(dalloc(kf, &kf->pixels[p], n));
-    KF_CHECK(dalloc(kf, &kf->coeffs[p], n));
-    KF_CHECK(dalloc(kf, &kf->lapped[p], n));
-    KF_CHECK(dalloc(kf, &kf->pixels_out[p], n));
-    if (inter) {
-      KF_CHECK(dalloc(kf, &kf->pred_pixels[p], n));
-      KF_CHECK(dalloc(kf, &kf->pred_coeffs[p], n));
-    }
-  }
-  const int UW = kf->nhsb * 8, UH = kf->nvsb * 8;
-  KF_CHECK(dalloc(kf, &kf->bsize, (size_t)F * UW * UH));
-  if (kf->cfg.inter_mc) {
-    const int rc = mc_alloc(kf);
-    if (rc) return rc;
-    kf->mc.frame_type = kf->ftype;
-  }
-  KF_CHECK(dalloc(kf, &kf->fq, (size_t)F));
-  KF_CHECK(dalloc(kf, &kf->fq_tbl, (size_t)F * 12));
-  KF_CHECK(dalloc(kf, &kf->fq_bq, (size_t)F * 96));
-  kf->fq_tbl_host.assign((size_t)F * 12, 0);
-  kf->fq_bq_host.assign((size_t)F * 96, 1);
-  KF_CHECK(dalloc(kf, &kf->qm, (size_t)2 * kf->cfg.qm_stride));
-  KF_CHECK(dalloc(kf, &kf->qm_inv, (size_t)2 * kf->cfg.qm_stride));
-  KF_CHECK(dalloc(kf, &kf->rsqrt_tbl, (size_t)kTableDoubles));
-  KF_CHECK(cudaMemcpy(kf->qm, kf->cfg.qm, sizeof(int16_t) * 2 * kf->cfg.qm_stride, cudaMemcpyHostToDevice));
-  KF_CHECK(cudaMemcpy(kf->qm_inv, kf->cfg.qm_inv, sizeof(int16_t) * 2 * kf->cfg.qm_stride, cudaMemcpyHostToDevice));
+// Luma pixels of the batch rows the work lists cover.
+static size_t shard_px(const Lists& L) { return (size_t)L.F * L.u_rows * L.UW * 64; }
 
+// The work lists, the PVQ items of both stages (frame_types: and the keyframe chains' own), the band contexts the two
+// stages share and (keyframes) the luma chain queue.
+static int lists_alloc(daala_b200_kf* kf) {
+  const int F = kf->F;
+  const int UW = kf->nhsb * 8, UH = kf->nvsb * 8;
   Lists& L = kf->lists;
-  memset(&L, 0, sizeof(L));
   L.bsize = kf->bsize;
   L.bstride = UW;
   L.bsize_pitch = (long long)UW * UH;
@@ -1966,23 +1942,22 @@ static int kf_alloc(daala_b200_kf* kf) {
   L.max_chroma = (int)(nunits * 2 / div) + 64;
   KF_CHECK(dalloc(kf, &L.tile_sum, (size_t)L.ntiles));
   KF_CHECK(dalloc(kf, &L.unit_lbase, (size_t)F * UW * UH));
-  if (!inter || mixed) KF_CHECK(dalloc(kf, &L.unit_loff, (size_t)F * UW * UH));
+  if (kf->key) KF_CHECK(dalloc(kf, &L.unit_loff, (size_t)F * UW * UH));
   KF_CHECK(dalloc(kf, &L.luma, (size_t)L.max_luma));
   KF_CHECK(dalloc(kf, &L.chroma, (size_t)L.max_chroma));
   // the intra dependency structure (neighbours, chain heads, ring) is a keyframe matter
-  const size_t ndep = inter && !mixed ? 0 : (size_t)L.max_luma;
-  const bool chains = ndep != 0;
+  const size_t ndep = kf->key ? (size_t)L.max_luma : 0;
   KF_CHECK(dalloc(kf, &L.dep_top, ndep));
   KF_CHECK(dalloc(kf, &L.dep_left, ndep));
   KF_CHECK(dalloc(kf, &L.succ_bottom, ndep));
   KF_CHECK(dalloc(kf, &L.succ_right, ndep));
   // item capacities follow from the pixel count alone: one band per 4x4 block is the densest case
-  const size_t luma_shard_px = (size_t)F * L.u_rows * UW * 64;
+  const size_t luma_shard_px = shard_px(L);
   kf->chain_cap = luma_shard_px / 16 + 64 + (size_t)kf->sms * 64;   // + one exit slot per persistent warp
   // keyframes: bands 3 / 6 only.  inter: every band; class 0 (bands 0..2) is densest on an all-4x4 map (one item
   // per block) or an all-8x8 one (three per block), classes 1 / 2 on all-8x8 / all-16x16 maps, one item per block
   const size_t cap_l0 = (size_t)L.max_luma * 3 < luma_shard_px / 16 ? (size_t)L.max_luma * 3 : luma_shard_px / 16;
-  const size_t cap_l[3] = {inter ? cap_l0 + 64 : 64, luma_shard_px / 64 + 64, luma_shard_px / 256 + 64};
+  const size_t cap_l[3] = {kf->pb ? cap_l0 + 64 : 64, luma_shard_px / 64 + 64, luma_shard_px / 256 + 64};
   const size_t cap_c[3] = {(size_t)L.max_chroma * 3 / 2 + 64, luma_shard_px / 4 * 2 * 3 / 64 + 64,
                            luma_shard_px / 4 * 2 * 3 / 256 + 64};
   for (int c = 0; c < 3; c++) {
@@ -1992,18 +1967,23 @@ static int kf_alloc(daala_b200_kf* kf) {
   }
   // frame_types: the keyframe chains' bands 3 / 6, at the capacities of a keyframe engine
   const size_t cap_k[3] = {64, cap_l[1], cap_l[2]};
-  for (int c = 0; mixed && c < 3; c++) KF_CHECK(dalloc(kf, &L.kitems_l[c], cap_k[c]));
-  {
-    // context records of one chunk of items per class (pvq_warp.cuh: band_ctx_*)
-    const int slots[3] = {1 << 19, 1 << 19, 3 << 15};
-    for (int c = 0; c < 3; c++) {
-      const int vs = c == 2 ? 128 : 32;
-      kf->sp_slots[c] = slots[c];
-      KF_CHECK(dalloc(kf, &kf->sp_vec[c], (size_t)slots[c] * 3 * vs));
-      KF_CHECK(dalloc(kf, &kf->sp_lanes[c], (size_t)slots[c] * kCtxLaneWords * 16));
-      KF_CHECK(dalloc(kf, &kf->sp_uni[c], (size_t)slots[c] * kCtxUniWords));
-      KF_CHECK(dalloc(kf, &kf->sp_snap[c], (size_t)slots[c] * kMaxEvents * vs));
-    }
+  for (int c = 0; kf->mixed && c < 3; c++) KF_CHECK(dalloc(kf, &L.kitems_l[c], cap_k[c]));
+  // context records of one chunk of items per class (pvq_warp.cuh: band_ctx_*), written into both stages
+  const int slots[3] = {1 << 19, 1 << 19, 3 << 15};
+  Stage &Y = kf->luma, &C = kf->chroma;
+  for (int c = 0; c < 3; c++) {
+    const int vs = c == 2 ? 128 : 32;
+    KF_CHECK(dalloc(kf, &Y.sp_vec[c], (size_t)slots[c] * 3 * vs));
+    KF_CHECK(dalloc(kf, &Y.sp_lanes[c], (size_t)slots[c] * kCtxLaneWords * 16));
+    KF_CHECK(dalloc(kf, &Y.sp_uni[c], (size_t)slots[c] * kCtxUniWords));
+    KF_CHECK(dalloc(kf, &Y.sp_snap[c], (size_t)slots[c] * kMaxEvents * vs));
+    C.sp_vec[c] = Y.sp_vec[c];
+    C.sp_lanes[c] = Y.sp_lanes[c];
+    C.sp_uni[c] = Y.sp_uni[c];
+    C.sp_snap[c] = Y.sp_snap[c];
+    Y.sp_slots[c] = C.sp_slots[c] = slots[c];
+    Y.sp_chunks[c] = (int)((cap_l[c] + slots[c] - 1) / slots[c]);
+    C.sp_chunks[c] = (int)((cap_c[c] + slots[c] - 1) / slots[c]);
   }
   {
     // the persistent grid is sized to be resident at once: 32 one-warp CTAs with kSnapEntries of shared
@@ -2018,231 +1998,222 @@ static int kf_alloc(daala_b200_kf* kf) {
       return (int)cudaErrorLaunchOutOfResources;
     }
   }
-  KF_CHECK(dalloc(kf, &L.heads, chains ? kf->chain_cap : 0));
-  KF_CHECK(dalloc(kf, &L.heads_raw, chains ? kf->chain_cap : 0));
-  KF_CHECK(dalloc(kf, &L.head_bin, chains ? kf->chain_cap : 0));
-  KF_CHECK(dalloc(kf, &L.head_hist, chains ? (size_t)kHeadBins : 0));
-  KF_CHECK(dalloc(kf, &L.head_cursor, chains ? (size_t)kHeadBins : 0));
+  const size_t nchain = kf->key ? kf->chain_cap : 0;
+  KF_CHECK(dalloc(kf, &L.heads, nchain));
+  KF_CHECK(dalloc(kf, &L.heads_raw, nchain));
+  KF_CHECK(dalloc(kf, &L.head_bin, nchain));
+  KF_CHECK(dalloc(kf, &L.head_hist, kf->key ? (size_t)kHeadBins : 0));
+  KF_CHECK(dalloc(kf, &L.head_cursor, kf->key ? (size_t)kHeadBins : 0));
   KF_CHECK(dalloc(kf, &L.heads0, ndep));
   KF_CHECK(dalloc(kf, &L.cnt, (size_t)kCntWords));
   L.kcnt = L.cnt;
-  if (mixed) KF_CHECK(dalloc(kf, &L.kcnt, (size_t)kCntWords));
+  if (kf->mixed) KF_CHECK(dalloc(kf, &L.kcnt, (size_t)kCntWords));
   L.ftype = kf->ftype;
   kf->mc.bad_ref = L.cnt + kMcBadRef;
   kf->mc.beyond = L.cnt + kMcBeyond;
+  return 0;
+}
 
-  auto setup_stage = [&](Stage& S, bool chroma) -> int {
-    memset(&S, 0, sizeof(S));
-    daala_b200_pvq_params& p = S.prm;
-    const size_t ncoef = chroma ? luma_shard_px / 2 + 1024 : luma_shard_px + 1024;
-    const size_t nblk = chroma ? L.max_chroma : L.max_luma;
-    p.blocks = chroma ? L.chroma : L.luma;
-    KF_CHECK(dalloc(kf, &p.in, ncoef));
-    KF_CHECK(dalloc(kf, &p.ref, ncoef));
-    KF_CHECK(dalloc(kf, &p.out, ncoef));
-    KF_CHECK(dalloc(kf, &p.y, ncoef));
-    KF_CHECK(dalloc(kf, &p.y16, ncoef));
-    KF_CHECK(dalloc(kf, &p.res_skip_term, nblk * 9));
-    KF_CHECK(dalloc(kf, &p.res_skip_diff, nblk));
-    KF_CHECK(dalloc(kf, &p.res_flip, nblk));
-    KF_CHECK(dalloc(kf, &S.res_pack, nblk * 9 * 4));
-    p.res_gain = p.res_theta = p.res_max_theta = p.res_k = nullptr;   // packed into res_pack here
-    p.res_dc = nullptr;
-    if (inter) KF_CHECK(dalloc(kf, &p.res_dc, nblk));
-    p.qm = kf->qm;
-    p.qm_inv = kf->qm_inv;
-    for (int i = 0; i < 3; i++) {
-      p.coef_plane[i] = kf->coeffs[i];
-      p.pred_plane[i] = kf->pred_coeffs[i];
-      p.plane_frame_pitch[i] = (long long)kf->plane_w[i] * kf->plane_h[i];
-      p.plane_stride[i] = kf->plane_w[i];
-    }
-    p.qm_stride = kf->cfg.qm_stride;
-    p.is_keyframe = inter ? 0 : 1;
-    p.use_masking = kf->cfg.use_masking;
-    p.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
-    S.fq_bq = kf->fq_bq;
-    for (int c = 0; c < 3; c++) S.items[c] = chroma ? L.items_c[c] : L.items_l[c];
-    S.cnt = L.cnt;
-    S.rsqrt_tbl = kf->rsqrt_tbl;
-    for (int c = 0; c < 3; c++) {
-      S.sp_vec[c] = kf->sp_vec[c];
-      S.sp_lanes[c] = kf->sp_lanes[c];
-      S.sp_uni[c] = kf->sp_uni[c];
-      S.sp_snap[c] = kf->sp_snap[c];
-      S.sp_slots[c] = kf->sp_slots[c];
-      const size_t cap = chroma ? cap_c[c] : cap_l[c];
-      S.sp_chunks[c] = kf->sp_slots[c] > 0 ? (int)((cap + kf->sp_slots[c] - 1) / kf->sp_slots[c]) : 0;
-    }
-    S.max_waiters = kf->sms * 8;
-    S.n_items_at = chroma ? kNItemsC : kNItemsL;
-    S.n_blocks_at = chroma ? kNChroma : kNLuma;
-    S.max_blocks = (int)nblk;
+// One PVQ stage (luma or chroma) over the work lists: its coefficient buffers in coding order, its per-block results
+// and (luma) the chain kernel's view of the dependency structure.  lists_alloc has set its band contexts.
+static int stage_alloc(daala_b200_kf* kf, Stage& S, bool chroma) {
+  const Lists& L = kf->lists;
+  const size_t luma_shard_px = shard_px(L);
+  daala_b200_pvq_params& p = S.prm;
+  const size_t ncoef = chroma ? luma_shard_px / 2 + 1024 : luma_shard_px + 1024;
+  const size_t nblk = chroma ? L.max_chroma : L.max_luma;
+  p.blocks = chroma ? L.chroma : L.luma;
+  KF_CHECK(dalloc(kf, &p.in, ncoef));
+  KF_CHECK(dalloc(kf, &p.ref, ncoef));
+  KF_CHECK(dalloc(kf, &p.out, ncoef));
+  KF_CHECK(dalloc(kf, &p.y, ncoef));
+  KF_CHECK(dalloc(kf, &p.y16, ncoef));
+  KF_CHECK(dalloc(kf, &p.res_skip_term, nblk * 9));
+  KF_CHECK(dalloc(kf, &p.res_skip_diff, nblk));
+  KF_CHECK(dalloc(kf, &p.res_flip, nblk));
+  KF_CHECK(dalloc(kf, &S.res_pack, nblk * 9 * 4));
+  p.res_gain = p.res_theta = p.res_max_theta = p.res_k = nullptr;   // packed into res_pack here
+  p.res_dc = nullptr;
+  if (kf->pb) KF_CHECK(dalloc(kf, &p.res_dc, nblk));
+  p.qm = kf->qm;
+  p.qm_inv = kf->qm_inv;
+  for (int i = 0; i < 3; i++) {
+    p.coef_plane[i] = kf->coeffs[i];
+    p.pred_plane[i] = kf->pred_coeffs[i];
+    p.plane_frame_pitch[i] = (long long)kf->plane_w[i] * kf->plane_h[i];
+    p.plane_stride[i] = kf->plane_w[i];
+  }
+  p.qm_stride = kf->cfg.qm_stride;
+  p.is_keyframe = kf->pb ? 0 : 1;
+  p.use_masking = kf->cfg.use_masking;
+  p.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
+  S.fq_bq = kf->fq_bq;
+  for (int c = 0; c < 3; c++) S.items[c] = chroma ? L.items_c[c] : L.items_l[c];
+  S.cnt = L.cnt;
+  S.rsqrt_tbl = kf->rsqrt_tbl;
+  S.max_waiters = kf->sms * 8;
+  S.n_items_at = chroma ? kNItemsC : kNItemsL;
+  S.n_blocks_at = chroma ? kNChroma : kNLuma;
+  S.max_blocks = (int)nblk;
+  S.ftype = kf->ftype;
 #ifdef DAALA_B200_CHAIN_TRACE
-    if (!chroma && !inter) {
-      S.trace_cap = (int)(luma_shard_px / 16);   // one band per 16 pixels at most
-      KF_CHECK(dalloc(kf, &S.trace, (size_t)S.trace_cap));
-    }
+  if (!chroma && !kf->pb) {
+    S.trace_cap = (int)(luma_shard_px / 16);   // one band per 16 pixels at most
+    KF_CHECK(dalloc(kf, &S.trace, (size_t)S.trace_cap));
+  }
 #endif
-    if (!chroma) {
-      S.head_lo_at = kHeadLoL;
-      S.dep_top = L.dep_top;
-      S.dep_left = L.dep_left;
-      S.succ_bottom = L.succ_bottom;
-      S.succ_right = L.succ_right;
-      S.heads = L.heads;
-      S.heads0 = L.heads0;
-      KF_CHECK(dalloc(kf, &S.ring, chains ? kf->chain_cap : 0));
-      KF_CHECK(dalloc(kf, &S.join0, ndep));
+  if (chroma && kf->key) {   // keyframe CfL: the luma stage's coding-order input and output
+    S.cfl_in = kf->luma.prm.in;
+    S.cfl_out = kf->luma.prm.out;
+    S.cfl_loff = L.unit_loff;
+  }
+  if (!chroma) {
+    const size_t ndep = kf->key ? (size_t)L.max_luma : 0;
+    S.head_lo_at = kHeadLoL;
+    S.dep_top = L.dep_top;
+    S.dep_left = L.dep_left;
+    S.succ_bottom = L.succ_bottom;
+    S.succ_right = L.succ_right;
+    S.heads = L.heads;
+    S.heads0 = L.heads0;
+    KF_CHECK(dalloc(kf, &S.ring, kf->key ? kf->chain_cap : 0));
+    KF_CHECK(dalloc(kf, &S.join0, ndep));
+  }
+  return 0;
+}
+
+// cfg.haar_dc_quant: the DC chain's grids (reconstructed DCs of all planes, frame by frame; signed indices per plane),
+// which the keyframe stages' CfL reads, and its launch parameters.
+static int hdc_alloc(daala_b200_kf* kf) {
+  const int F = kf->F;
+  daala_b200_haar_dc_batch& H = kf->hdcb;
+  const size_t g0 = (size_t)(kf->plane_w[0] >> 2) * (kf->plane_h[0] >> 2), g1 = (size_t)(kf->plane_w[1] >> 2) * (kf->plane_h[1] >> 2);
+  KF_CHECK(dalloc(kf, &kf->hdc, (g0 + 2 * g1) * F));
+  H.grid_frame_pitch = (long long)(g0 + 2 * g1);
+  kf->luma.cfl_in = kf->chroma.cfl_in = kf->hdc;
+  for (int p = 0; p < 3; p++) {
+    KF_CHECK(dalloc(kf, &kf->hdc_index[p], (p ? g1 : g0) * F));
+    H.coeffs[p] = kf->coeffs[p];
+    H.dc[p] = kf->hdc + (p ? g0 + (p - 1) * g1 : 0);
+    H.index[p] = kf->hdc_index[p];
+    H.plane_w[p] = kf->plane_w[p];
+    H.plane_h[p] = kf->plane_h[p];
+  }
+  H.bsize = kf->bsize;
+  H.F = F;
+  H.nhsb = kf->nhsb;
+  H.nvsb = kf->nvsb;
+  H.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
+  H.fq_bq = kf->fq_bq;
+  H.frame_type = kf->ftype;
+  return 0;
+}
+
+// cfg.symbol_stream: the stream arrays at the worst case of the engine's capacity, and the stages' results they read.
+static int sym_alloc(daala_b200_kf* kf) {
+  const int F = kf->F;
+  const Lists& L = kf->lists;
+  const int UW = kf->nhsb * 8, UH = kf->nvsb * 8;
+  Sym& Y = kf->sym;
+  Y.bsize = kf->bsize;
+  Y.bstride = UW;
+  Y.bsize_pitch = (long long)UW * UH;
+  Y.F = F;
+  Y.nhsb = kf->nhsb;
+  Y.sb_rows = kf->cfg.sb_rows;
+  Y.u_row0 = L.u_row0;
+  Y.nsb = kf->nhsb * kf->cfg.sb_rows;
+  Y.cap_blocks = L.max_luma + L.max_chroma;
+  Y.ntiles = (Y.cap_blocks + kTile - 1) / kTile;
+  // every band has at least 8 coefficients and 4x4 / 8x8 blocks have one band per 16: bands <= coefficients / 16
+  const size_t luma_shard_px = shard_px(L);
+  const size_t ncoef = (luma_shard_px + 1024) + (luma_shard_px / 2 + 1024);
+  KF_CHECK(dalloc(kf, &Y.unit_rank, (size_t)F * L.u_rows * UW));
+  KF_CHECK(dalloc(kf, &Y.sb_cnt, (size_t)F * Y.nsb));
+  KF_CHECK(dalloc(kf, &Y.sb_base, (size_t)F * Y.nsb));
+  KF_CHECK(dalloc(kf, &Y.order, (size_t)Y.cap_blocks));
+  KF_CHECK(dalloc(kf, &Y.off, (size_t)Y.cap_blocks));
+  KF_CHECK(dalloc(kf, &Y.tile, (size_t)Y.ntiles));
+  KF_CHECK(dalloc(kf, &Y.tot, (size_t)4));
+  KF_CHECK(dalloc(kf, &Y.index, (size_t)F));
+  KF_CHECK(dalloc(kf, &Y.blocks, (size_t)Y.cap_blocks));
+  Y.cap_bands = (long long)(ncoef / 16);
+  Y.cap_bytes = (long long)(2 * ncoef);
+  KF_CHECK(dalloc(kf, &Y.bands, ncoef / 16));
+  KF_CHECK(dalloc(kf, &Y.pulses, 2 * ncoef));
+  for (int c = 0; c < 2; c++) {
+    const Stage& S = c ? kf->chroma : kf->luma;
+    Y.list[c] = S.prm.blocks;
+    Y.res[c] = reinterpret_cast<const short4*>(S.res_pack);
+    Y.y[c] = S.prm.y;
+    Y.skip_diff[c] = S.prm.res_skip_diff;
+  }
+  Y.flip = kf->chroma.prm.res_flip;
+  Y.cnt = L.cnt;
+  Y.max_luma = L.max_luma;
+  Y.max_chroma = L.max_chroma;
+  if (kf->cfg.symbol_stream >= 2) {
+    KF_CHECK(dalloc(kf, &Y.dc, (size_t)Y.cap_blocks));
+    for (int c = 0; c < 2; c++) {
+      Y.qdc[c] = (c ? kf->chroma : kf->luma).prm.res_dc;
+      Y.dc_resid[c] = kf->dc_resid[c];
     }
-    return 0;
-  };
-  int rc = setup_stage(kf->luma, false);
-  if (rc) return rc;
-  rc = setup_stage(kf->chroma, true);
-  if (rc) return rc;
-  kf->luma.ftype = kf->chroma.ftype = kf->ftype;
-  if (!inter || mixed) {
-    Stage& C = kf->chroma;
-    C.cfl_in = kf->luma.prm.in;
-    C.cfl_out = kf->luma.prm.out;
-    C.cfl_loff = L.unit_loff;
   }
   if (kf->cfg.haar_dc_quant) {
-    daala_b200_haar_dc_batch& H = kf->hdcb;
-    memset(&H, 0, sizeof(H));
-    const size_t g0 = (size_t)(kf->plane_w[0] >> 2) * (kf->plane_h[0] >> 2), g1 = (size_t)(kf->plane_w[1] >> 2) * (kf->plane_h[1] >> 2);
-    KF_CHECK(dalloc(kf, &kf->hdc, (g0 + 2 * g1) * F));
-    H.grid_frame_pitch = (long long)(g0 + 2 * g1);
-    kf->luma.cfl_in = kf->chroma.cfl_in = kf->hdc;
+    KF_CHECK(dalloc(kf, &Y.hdc, (size_t)Y.cap_blocks));
     for (int p = 0; p < 3; p++) {
-      KF_CHECK(dalloc(kf, &kf->hdc_index[p], (p ? g1 : g0) * F));
-      H.coeffs[p] = kf->coeffs[p];
-      H.dc[p] = kf->hdc + (p ? g0 + (p - 1) * g1 : 0);
-      H.index[p] = kf->hdc_index[p];
-      H.plane_w[p] = kf->plane_w[p];
-      H.plane_h[p] = kf->plane_h[p];
-    }
-    H.bsize = kf->bsize;
-    H.F = F;
-    H.nhsb = kf->nhsb;
-    H.nvsb = kf->nvsb;
-    H.pvq_norm_lambda = kf->cfg.pvq_norm_lambda;
-    H.fq_bq = kf->fq_bq;
-    H.frame_type = kf->ftype;
-  }
-  if (mixed) {
-    // the chain kernel walks the keyframe luma items; its Stage reads no frame type
-    Stage& K = kf->luma_kf;
-    K = kf->luma;
-    K.prm.is_keyframe = 1;
-    K.cnt = L.kcnt;
-    for (int c = 0; c < 3; c++) K.items[c] = L.kitems_l[c];
-    K.ftype = nullptr;
-  }
-  (void)luma_px;
-  // the unquantised DC residual per block: what the host's od_rdo_quant needs, returned classically (inter_finish) or
-  // in the stream's DC records (symbol_stream = 2 or 3)
-  if (kf->cfg.inter_finish || kf->cfg.symbol_stream >= 2)
-    for (int c = 0; c < 2; c++) {
-      Stage& S = c ? kf->chroma : kf->luma;
-      KF_CHECK(dalloc(kf, &kf->dc_resid[c], (size_t)S.max_blocks));
-      S.dc_resid = kf->dc_resid[c];
-    }
-  if (kf->cfg.symbol_stream) {
-    Sym& Y = kf->sym;
-    memset(&Y, 0, sizeof(Y));
-    Y.bsize = kf->bsize;
-    Y.bstride = UW;
-    Y.bsize_pitch = (long long)UW * UH;
-    Y.F = F;
-    Y.nhsb = kf->nhsb;
-    Y.sb_rows = kf->cfg.sb_rows;
-    Y.u_row0 = L.u_row0;
-    Y.nsb = kf->nhsb * kf->cfg.sb_rows;
-    Y.cap_blocks = L.max_luma + L.max_chroma;
-    Y.ntiles = (Y.cap_blocks + kTile - 1) / kTile;
-    // every band has at least 8 coefficients and 4x4 / 8x8 blocks have one band per 16: bands <= coefficients / 16
-    const size_t ncoef = (luma_shard_px + 1024) + (luma_shard_px / 2 + 1024);
-    KF_CHECK(dalloc(kf, &Y.unit_rank, (size_t)F * L.u_rows * UW));
-    KF_CHECK(dalloc(kf, &Y.sb_cnt, (size_t)F * Y.nsb));
-    KF_CHECK(dalloc(kf, &Y.sb_base, (size_t)F * Y.nsb));
-    KF_CHECK(dalloc(kf, &Y.order, (size_t)Y.cap_blocks));
-    KF_CHECK(dalloc(kf, &Y.off, (size_t)Y.cap_blocks));
-    KF_CHECK(dalloc(kf, &Y.tile, (size_t)Y.ntiles));
-    KF_CHECK(dalloc(kf, &Y.tot, (size_t)4));
-    KF_CHECK(dalloc(kf, &Y.index, (size_t)F));
-    KF_CHECK(dalloc(kf, &Y.blocks, (size_t)Y.cap_blocks));
-    Y.cap_bands = (long long)(ncoef / 16);
-    Y.cap_bytes = (long long)(2 * ncoef);
-    KF_CHECK(dalloc(kf, &Y.bands, ncoef / 16));
-    KF_CHECK(dalloc(kf, &Y.pulses, 2 * ncoef));
-    for (int c = 0; c < 2; c++) {
-      const Stage& S = c ? kf->chroma : kf->luma;
-      Y.list[c] = S.prm.blocks;
-      Y.res[c] = reinterpret_cast<const short4*>(S.res_pack);
-      Y.y[c] = S.prm.y;
-      Y.skip_diff[c] = S.prm.res_skip_diff;
-    }
-    Y.flip = kf->chroma.prm.res_flip;
-    Y.cnt = L.cnt;
-    Y.max_luma = L.max_luma;
-    Y.max_chroma = L.max_chroma;
-    if (kf->cfg.symbol_stream >= 2) {
-      KF_CHECK(dalloc(kf, &Y.dc, (size_t)Y.cap_blocks));
-      for (int c = 0; c < 2; c++) {
-        Y.qdc[c] = (c ? kf->chroma : kf->luma).prm.res_dc;
-        Y.dc_resid[c] = kf->dc_resid[c];
-      }
-    }
-    if (kf->cfg.haar_dc_quant) {
-      KF_CHECK(dalloc(kf, &Y.hdc, (size_t)Y.cap_blocks));
-      for (int p = 0; p < 3; p++) {
-        Y.hdc_index[p] = kf->hdc_index[p];
-        Y.gw[p] = kf->plane_w[p] >> 2;
-        Y.gh[p] = kf->plane_h[p] >> 2;
-      }
-    }
-    if (mixed) Y.ftype = kf->ftype;
-  }
-  if (kf->cfg.late_skip) {
-    daala_b200_late_skip_batch& B = kf->lsb;
-    memset(&B, 0, sizeof(B));
-    long long px = 0;
-    for (int p = 0; p < 3; p++) {
-      const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
-      KF_CHECK(dalloc(kf, &kf->d_orig[p], n));
-      px += (long long)n;
-      B.d_orig[p] = kf->d_orig[p];
-      B.d[p] = kf->coeffs[p];
-      B.md[p] = kf->pred_coeffs[p];
-      B.plane_pitch[p] = (long long)kf->plane_w[p] * kf->plane_h[p];
-      B.plane_stride[p] = kf->plane_w[p];
-    }
-    for (int c = 0; c < 2; c++) {
-      const Stage& S = c ? kf->chroma : kf->luma;
-      KF_CHECK(dalloc(kf, &kf->late_skip[c], (size_t)S.max_blocks));
-      B.blocks[c] = S.prm.blocks;
-      B.count[c] = L.cnt + S.n_blocks_at;
-      B.max_blocks[c] = S.max_blocks;
-      B.out[c] = kf->late_skip[c];
-    }
-    KF_CHECK(dalloc(kf, &B.cls_items, (size_t)daala_b200_late_skip_class_caps(px, B.cls_off, B.cls_cap)));
-    KF_CHECK(dalloc(kf, &B.cls_n, (size_t)4));
-    B.qm_is_flat = kf->cfg.qm_is_flat;
-    B.use_activity_masking = kf->cfg.use_masking;
-    B.fq = kf->fq;
-    B.fq_bq = kf->fq_bq;
-    if (kf->cfg.symbol_stream == 2) {
-      Sym& Y = kf->sym;
-      KF_CHECK(dalloc(kf, &Y.late_skip, (size_t)Y.cap_blocks));
-      Y.ls_block[0] = kf->late_skip[0];
-      Y.ls_block[1] = kf->late_skip[1];
+      Y.hdc_index[p] = kf->hdc_index[p];
+      Y.gw[p] = kf->plane_w[p] >> 2;
+      Y.gh[p] = kf->plane_h[p] >> 2;
     }
   }
+  if (kf->mixed) Y.ftype = kf->ftype;
+  return 0;
+}
 
+// cfg.late_skip: the unquantised coefficients (a copy of `coeffs` taken before the finishing scatter), the records per
+// block of each list (symbol_stream = 2: and in stream order), and the parameters of the late-skip launches.
+static int late_skip_alloc(daala_b200_kf* kf) {
+  const int F = kf->F;
+  daala_b200_late_skip_batch& B = kf->lsb;
+  long long px = 0;
+  for (int p = 0; p < 3; p++) {
+    const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
+    KF_CHECK(dalloc(kf, &kf->d_orig[p], n));
+    px += (long long)n;
+    B.d_orig[p] = kf->d_orig[p];
+    B.d[p] = kf->coeffs[p];
+    B.md[p] = kf->pred_coeffs[p];
+    B.plane_pitch[p] = (long long)kf->plane_w[p] * kf->plane_h[p];
+    B.plane_stride[p] = kf->plane_w[p];
+  }
+  for (int c = 0; c < 2; c++) {
+    const Stage& S = c ? kf->chroma : kf->luma;
+    KF_CHECK(dalloc(kf, &kf->late_skip[c], (size_t)S.max_blocks));
+    B.blocks[c] = S.prm.blocks;
+    B.count[c] = kf->lists.cnt + S.n_blocks_at;
+    B.max_blocks[c] = S.max_blocks;
+    B.out[c] = kf->late_skip[c];
+  }
+  KF_CHECK(dalloc(kf, &B.cls_items, (size_t)daala_b200_late_skip_class_caps(px, B.cls_off, B.cls_cap)));
+  KF_CHECK(dalloc(kf, &B.cls_n, (size_t)4));
+  B.qm_is_flat = kf->cfg.qm_is_flat;
+  B.use_activity_masking = kf->cfg.use_masking;
+  B.fq = kf->fq;
+  B.fq_bq = kf->fq_bq;
+  if (kf->cfg.symbol_stream == 2) {
+    Sym& Y = kf->sym;
+    KF_CHECK(dalloc(kf, &Y.late_skip, (size_t)Y.cap_blocks));
+    Y.ls_block[0] = kf->late_skip[0];
+    Y.ls_block[1] = kf->late_skip[1];
+  }
+  return 0;
+}
+
+// The transforms' frame descriptions: `frame`, `frame_fwd` (the forward's) and `frame_pred` (inter: the prediction's).
+static void frames_setup(daala_b200_kf* kf) {
+  const int UW = kf->nhsb * 8, UH = kf->nvsb * 8;
   daala_b200_frame& f = kf->frame;
-  memset(&f, 0, sizeof(f));
   for (int p = 0; p < 3; p++) {
     daala_b200_plane& pl = f.plane[p];
     pl.pixels = kf->pixels[p];
@@ -2263,138 +2234,205 @@ static int kf_alloc(daala_b200_kf* kf) {
   f.pic_h = kf->cfg.pic_h;
   // haar_dc_quant: the leaf DCs the finishing scatter stores are final, as on P frames, so the inverse skips the
   // pyramid; the forward (frame_fwd) still builds it for the DC chain
-  f.haar_dc = inter || kf->cfg.haar_dc_quant ? 0 : 1;
-  f.nframes = F;
+  f.haar_dc = kf->pb || kf->cfg.haar_dc_quant ? 0 : 1;
+  f.nframes = kf->F;
   f.sb_row0 = kf->cfg.sb_row0;
   f.sb_rows = kf->cfg.sb_rows;
   kf->frame_pred = f;
   kf->frame_fwd = f;
-  kf->frame_fwd.haar_dc = inter ? 0 : 1;
+  kf->frame_fwd.haar_dc = kf->pb ? 0 : 1;
   for (int p = 0; p < 3; p++) {
     kf->frame_pred.plane[p].pixels = kf->pred_pixels[p];
     kf->frame_pred.plane[p].coeffs = kf->pred_coeffs[p];
   }
-  if (kf->cfg.inter_finish) {
-    const size_t nsb = (size_t)F * kf->nhsb * kf->nvsb;
-    Fin& P = kf->fin;
-    memset(&P, 0, sizeof(P));
+}
+
+// cfg.inter_finish: the finishing pass's decisions per block, its planes and skip maps, the superblock flags,
+// [inter_mc: the pool store's slot table], [symbol_stream 2 / 3: the stream-order decisions and their scatter].
+static int fin_alloc(daala_b200_kf* kf) {
+  const int F = kf->F;
+  const size_t nsb = (size_t)F * kf->nhsb * kf->nvsb;
+  Fin& P = kf->fin;
+  for (int c = 0; c < 2; c++) {
+    const Stage& S = c ? kf->chroma : kf->luma;
+    KF_CHECK(dalloc(kf, &kf->fin_skip[c], (size_t)S.max_blocks));
+    KF_CHECK(dalloc(kf, &kf->fin_dc[c], (size_t)S.max_blocks));
+    P.blocks[c] = S.prm.blocks;
+    P.skip[c] = kf->fin_skip[c];
+    P.dc[c] = kf->fin_dc[c];
+    P.max_blocks[c] = S.max_blocks;
+  }
+  P.cnt = kf->lists.cnt;
+  P.skip_stride = kf->nhsb * 16;
+  for (int p = 0; p < 3; p++) {
+    const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
+    KF_CHECK(dalloc(kf, &kf->fin_coeffs[p], n));
+    KF_CHECK(dalloc(kf, &kf->fin_pixels[p], n));
+    P.skip_pitch[p] = (long long)(kf->plane_h[p] / 4) * P.skip_stride;
+    KF_CHECK(dalloc(kf, &kf->fin_bskip[p], (size_t)P.skip_pitch[p] * F));
+    P.d[p] = kf->coeffs[p];
+    P.md[p] = kf->pred_coeffs[p];
+    P.out[p] = kf->fin_coeffs[p];
+    P.plane_pitch[p] = (long long)kf->plane_w[p] * kf->plane_h[p];
+    P.plane_stride[p] = kf->plane_w[p];
+    P.bskip[p] = kf->fin_bskip[p];
+  }
+  KF_CHECK(dalloc(kf, &kf->fin_level, nsb));
+  KF_CHECK(dalloc(kf, &kf->fin_coded, nsb));
+  P.coded = kf->fin_coded;
+  P.nhsb = kf->nhsb;
+  P.nvsb = kf->nvsb;
+  P.fq_bq = kf->fq_bq;
+  P.ftype = kf->ftype;
+  if (kf->cfg.inter_mc) {
+    KF_CHECK(dalloc(kf, &kf->fin_slot_out, (size_t)F));
+    PoolStore& W = kf->store;
+    for (int p = 0; p < 3; p++) {
+      W.src[p] = kf->fin_pixels[p];
+      W.pool[p] = kf->ref_pixels[p];
+      W.plane_bytes[p] = (long long)kf->plane_w[p] * kf->plane_h[p];
+    }
+    W.slot = kf->fin_slot_out;
+  }
+  if (kf->cfg.symbol_stream >= 2) {
+    Unstream& U = kf->unstream;
+    KF_CHECK(dalloc(kf, &kf->fin_stream_skip, (size_t)kf->sym.cap_blocks));
+    KF_CHECK(dalloc(kf, &kf->fin_stream_dc, (size_t)kf->sym.cap_blocks));
+    KF_CHECK(dalloc(kf, &kf->fin_form, (size_t)1));
+    U.order = kf->sym.order;
+    U.tot = kf->sym.tot;
+    U.skip = kf->fin_stream_skip;
+    U.dc = kf->fin_stream_dc;
     for (int c = 0; c < 2; c++) {
-      const Stage& S = c ? kf->chroma : kf->luma;
-      KF_CHECK(dalloc(kf, &kf->fin_skip[c], (size_t)S.max_blocks));
-      KF_CHECK(dalloc(kf, &kf->fin_dc[c], (size_t)S.max_blocks));
-      P.blocks[c] = S.prm.blocks;
-      P.skip[c] = kf->fin_skip[c];
-      P.dc[c] = kf->fin_dc[c];
-      P.max_blocks[c] = S.max_blocks;
+      U.fin_skip[c] = kf->fin_skip[c];
+      U.fin_dc[c] = kf->fin_dc[c];
     }
-    P.cnt = L.cnt;
-    P.skip_stride = kf->nhsb * 16;
-    for (int p = 0; p < 3; p++) {
-      const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
-      KF_CHECK(dalloc(kf, &kf->fin_coeffs[p], n));
-      KF_CHECK(dalloc(kf, &kf->fin_pixels[p], n));
-      P.skip_pitch[p] = (long long)(kf->plane_h[p] / 4) * P.skip_stride;
-      KF_CHECK(dalloc(kf, &kf->fin_bskip[p], (size_t)P.skip_pitch[p] * F));
-      P.d[p] = kf->coeffs[p];
-      P.md[p] = kf->pred_coeffs[p];
-      P.out[p] = kf->fin_coeffs[p];
-      P.plane_pitch[p] = (long long)kf->plane_w[p] * kf->plane_h[p];
-      P.plane_stride[p] = kf->plane_w[p];
-      P.bskip[p] = kf->fin_bskip[p];
-    }
-    KF_CHECK(dalloc(kf, &kf->fin_level, nsb));
-    KF_CHECK(dalloc(kf, &kf->fin_coded, nsb));
-    P.coded = kf->fin_coded;
-    P.nhsb = kf->nhsb;
-    P.nvsb = kf->nvsb;
-    P.fq_bq = kf->fq_bq;
-    P.ftype = kf->ftype;
-    if (kf->cfg.inter_mc) {
-      KF_CHECK(dalloc(kf, &kf->fin_slot_out, (size_t)F));
-      PoolStore& W = kf->store;
-      for (int p = 0; p < 3; p++) {
-        W.src[p] = kf->fin_pixels[p];
-        W.pool[p] = kf->ref_pixels[p];
-        W.plane_bytes[p] = (long long)kf->plane_w[p] * kf->plane_h[p];
-      }
-      W.slot = kf->fin_slot_out;
-    }
-    if (kf->cfg.symbol_stream >= 2) {
-      Unstream& U = kf->unstream;
-      KF_CHECK(dalloc(kf, &kf->fin_stream_skip, (size_t)kf->sym.cap_blocks));
-      KF_CHECK(dalloc(kf, &kf->fin_stream_dc, (size_t)kf->sym.cap_blocks));
-      KF_CHECK(dalloc(kf, &kf->fin_form, (size_t)1));
-      U.order = kf->sym.order;
-      U.tot = kf->sym.tot;
-      U.skip = kf->fin_stream_skip;
-      U.dc = kf->fin_stream_dc;
-      for (int c = 0; c < 2; c++) {
-        U.fin_skip[c] = kf->fin_skip[c];
-        U.fin_dc[c] = kf->fin_dc[c];
-      }
-      U.form = kf->fin_form;
+    U.form = kf->fin_form;
+  }
+  return 0;
+}
+
+// The deringing pass: the step's on keyframes (cfg.dering) or the finishing pass's (cfg.inter_finish); inter refuses
+// dering, so an engine has at most one.  Level 2 of either searches the levels first.
+static int dering_alloc(daala_b200_kf* kf, int level) {
+  const int F = kf->F;
+  const size_t nsb = (size_t)F * kf->nhsb * kf->nvsb;
+  Dering& D = kf->dering;
+  D.frame = kf->frame;
+  D.skip_stride = kf->nhsb * 16;
+  uint8_t* zero_skip = nullptr;   // keyframes never mark a block skipped (src/encode.c:1690): one map for all frames
+  if (!kf->cfg.inter_finish) KF_CHECK(dalloc(kf, &zero_skip, nsb * 256 + 64));
+  for (int p = 0; p < 3; p++) {
+    KF_CHECK(dalloc(kf, &D.frame.post16[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F));
+    if (kf->cfg.inter_finish) {
+      // the patched coefficients, inverted in place (k_inverse_sb only touches its own superblock)
+      D.frame.plane[p].coeffs = D.frame.plane[p].lapped = kf->fin_coeffs[p];
+      D.frame.plane[p].pixels_out = kf->fin_pixels[p];
+      D.skip[p] = kf->fin_bskip[p];
+      D.skip_pitch[p] = kf->fin.skip_pitch[p];
+    } else {
+      D.skip[p] = zero_skip;
     }
   }
-  // the deringing pass: the step's on keyframes (cfg.dering) or the finishing pass's (cfg.inter_finish); inter refuses
-  // dering, so an engine has at most one.  Level 2 of either searches the levels first.
+  KF_CHECK(dalloc(kf, &D.level, nsb));
+  KF_CHECK(dalloc(kf, &D.thr[0], nsb));
+  KF_CHECK(dalloc(kf, &D.thr[1], nsb));
+  KF_CHECK(dalloc(kf, &D.dir, nsb * 64));
+  D.coded = kf->fin_coded;
+  D.applied = kf->fin_level;
+  D.frame_tbl = kf->fq_tbl;
+  D.search = level == 2;
+  if (D.search) {
+    // src/encode.c:2708-2811 for every frame of the batch.  P frames (src/encode.c:2720-2811): the frame's own skip
+    // map under every candidate, superblocks without a coded luma 4x4 unit neither scored nor adapted, context 0
+    daala_b200_dering_search_batch& b = D.sb;
+    b.etmp = D.frame.post16[0];
+    b.src = kf->pixels[0];
+    b.etmp_pitch = b.src_pitch = (long long)kf->plane_w[0] * kf->plane_h[0];
+    b.etmp_stride = b.src_stride = kf->plane_w[0];
+    b.nframes = F;
+    b.nhsb = kf->nhsb;
+    b.nvsb = kf->nvsb;
+    b.qm_is_flat = kf->cfg.qm_is_flat;
+    b.use_activity_masking = kf->cfg.use_masking;
+    b.bskip = D.skip[0];
+    b.skip_stride = D.skip_stride;
+    b.skip_pitch = D.skip_pitch[0];
+    b.coded = D.coded;
+    b.is_keyframe = kf->pb ? 0 : 1;
+    b.frame_type = kf->ftype;   // frame_types: the keyframe rule (up / left context) on keyframes
+    KF_CHECK(dalloc(kf, &b.filt, (size_t)kf->plane_w[0] * kf->plane_h[0] * F));
+    KF_CHECK(dalloc(kf, &b.orig, nsb * 4096));
+    KF_CHECK(dalloc(kf, &b.cand, nsb * 4096));
+    KF_CHECK(dalloc(kf, &b.dist, nsb * 6));
+    b.dir = D.dir;
+    b.levels = D.level;   // what the thresholds read; on P frames its level 0 agrees with the forced one
+    b.fq = kf->fq;
+    b.frame_tbl = kf->fq_tbl;
+    KF_CHECK(dalloc(kf, &b.cand_thr, nsb * 5));
+  }
+  return 0;
+}
+
+// Every buffer of a lossy engine, part by part.  The engine is value-initialised: what no part sets stays zero.
+static int kf_alloc(daala_b200_kf* kf) {
+  if (kf->cfg.lossless) return ll_alloc(kf);
+  const int F = kf->F;
+  if (kf->mixed) KF_CHECK(dalloc(kf, &kf->ftype, (size_t)F));
+  for (int p = 0; p < 3; p++) {
+    const size_t n = (size_t)kf->plane_w[p] * kf->plane_h[p] * F;
+    KF_CHECK(dalloc(kf, &kf->pixels[p], n));
+    KF_CHECK(dalloc(kf, &kf->coeffs[p], n));
+    KF_CHECK(dalloc(kf, &kf->lapped[p], n));
+    KF_CHECK(dalloc(kf, &kf->pixels_out[p], n));
+    if (kf->pb) {
+      KF_CHECK(dalloc(kf, &kf->pred_pixels[p], n));
+      KF_CHECK(dalloc(kf, &kf->pred_coeffs[p], n));
+    }
+  }
+  KF_CHECK(dalloc(kf, &kf->bsize, (size_t)F * kf->nhsb * 8 * kf->nvsb * 8));
+  if (kf->cfg.inter_mc) {
+    STEP_TRY(mc_alloc(kf));
+    kf->mc.frame_type = kf->ftype;
+  }
+  KF_CHECK(dalloc(kf, &kf->fq, (size_t)F));
+  KF_CHECK(dalloc(kf, &kf->fq_tbl, (size_t)F * 12));
+  KF_CHECK(dalloc(kf, &kf->fq_bq, (size_t)F * 96));
+  kf->fq_tbl_host.assign((size_t)F * 12, 0);
+  kf->fq_bq_host.assign((size_t)F * 96, 1);
+  KF_CHECK(dalloc(kf, &kf->qm, (size_t)2 * kf->cfg.qm_stride));
+  KF_CHECK(dalloc(kf, &kf->qm_inv, (size_t)2 * kf->cfg.qm_stride));
+  KF_CHECK(dalloc(kf, &kf->rsqrt_tbl, (size_t)kTableDoubles));
+  KF_CHECK(cudaMemcpy(kf->qm, kf->cfg.qm, sizeof(int16_t) * 2 * kf->cfg.qm_stride, cudaMemcpyHostToDevice));
+  KF_CHECK(cudaMemcpy(kf->qm_inv, kf->cfg.qm_inv, sizeof(int16_t) * 2 * kf->cfg.qm_stride, cudaMemcpyHostToDevice));
+
+  STEP_TRY(lists_alloc(kf));
+  STEP_TRY(stage_alloc(kf, kf->luma, false));
+  STEP_TRY(stage_alloc(kf, kf->chroma, true));
+  if (kf->cfg.haar_dc_quant) STEP_TRY(hdc_alloc(kf));
+  if (kf->mixed) {
+    // the chain kernel walks the keyframe luma items; its Stage reads no frame type
+    Stage& K = kf->luma_kf;
+    K = kf->luma;
+    K.prm.is_keyframe = 1;
+    K.cnt = kf->lists.kcnt;
+    for (int c = 0; c < 3; c++) K.items[c] = kf->lists.kitems_l[c];
+    K.ftype = nullptr;
+  }
+  // the unquantised DC residual per block: what the host's od_rdo_quant needs, returned classically (inter_finish) or
+  // in the stream's DC records (symbol_stream = 2 or 3)
+  if (kf->cfg.inter_finish || kf->cfg.symbol_stream >= 2)
+    for (int c = 0; c < 2; c++) {
+      Stage& S = c ? kf->chroma : kf->luma;
+      KF_CHECK(dalloc(kf, &kf->dc_resid[c], (size_t)S.max_blocks));
+      S.dc_resid = kf->dc_resid[c];
+    }
+  if (kf->cfg.symbol_stream) STEP_TRY(sym_alloc(kf));
+  if (kf->cfg.late_skip) STEP_TRY(late_skip_alloc(kf));
+  frames_setup(kf);
+  if (kf->cfg.inter_finish) STEP_TRY(fin_alloc(kf));
   const int dering = kf->cfg.dering ? kf->cfg.dering : kf->cfg.inter_finish;
-  if (dering) {
-    const size_t nsb = (size_t)F * kf->nhsb * kf->nvsb;
-    Dering& D = kf->dering;
-    D.frame = kf->frame;
-    D.skip_stride = kf->nhsb * 16;
-    uint8_t* zero_skip = nullptr;   // keyframes never mark a block skipped (src/encode.c:1690): one map for all frames
-    if (!kf->cfg.inter_finish) KF_CHECK(dalloc(kf, &zero_skip, nsb * 256 + 64));
-    for (int p = 0; p < 3; p++) {
-      KF_CHECK(dalloc(kf, &D.frame.post16[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F));
-      if (kf->cfg.inter_finish) {
-        // the patched coefficients, inverted in place (k_inverse_sb only touches its own superblock)
-        D.frame.plane[p].coeffs = D.frame.plane[p].lapped = kf->fin_coeffs[p];
-        D.frame.plane[p].pixels_out = kf->fin_pixels[p];
-        D.skip[p] = kf->fin_bskip[p];
-        D.skip_pitch[p] = kf->fin.skip_pitch[p];
-      } else {
-        D.skip[p] = zero_skip;
-      }
-    }
-    KF_CHECK(dalloc(kf, &D.level, nsb));
-    KF_CHECK(dalloc(kf, &D.thr[0], nsb));
-    KF_CHECK(dalloc(kf, &D.thr[1], nsb));
-    KF_CHECK(dalloc(kf, &D.dir, nsb * 64));
-    D.coded = kf->fin_coded;
-    D.applied = kf->fin_level;
-    D.frame_tbl = kf->fq_tbl;
-    D.search = dering == 2;
-    if (D.search) {
-      // src/encode.c:2708-2811 for every frame of the batch.  P frames (src/encode.c:2720-2811): the frame's own skip
-      // map under every candidate, superblocks without a coded luma 4x4 unit neither scored nor adapted, context 0
-      daala_b200_dering_search_batch& b = D.sb;
-      b.etmp = D.frame.post16[0];
-      b.src = kf->pixels[0];
-      b.etmp_pitch = b.src_pitch = (long long)kf->plane_w[0] * kf->plane_h[0];
-      b.etmp_stride = b.src_stride = kf->plane_w[0];
-      b.nframes = F;
-      b.nhsb = kf->nhsb;
-      b.nvsb = kf->nvsb;
-      b.qm_is_flat = kf->cfg.qm_is_flat;
-      b.use_activity_masking = kf->cfg.use_masking;
-      b.bskip = D.skip[0];
-      b.skip_stride = D.skip_stride;
-      b.skip_pitch = D.skip_pitch[0];
-      b.coded = D.coded;
-      b.is_keyframe = inter ? 0 : 1;
-      b.frame_type = kf->ftype;   // frame_types: the keyframe rule (up / left context) on keyframes
-      KF_CHECK(dalloc(kf, &b.filt, (size_t)kf->plane_w[0] * kf->plane_h[0] * F));
-      KF_CHECK(dalloc(kf, &b.orig, nsb * 4096));
-      KF_CHECK(dalloc(kf, &b.cand, nsb * 4096));
-      KF_CHECK(dalloc(kf, &b.dist, nsb * 6));
-      b.dir = D.dir;
-      b.levels = D.level;   // what the thresholds read; on P frames its level 0 agrees with the forced one
-      b.fq = kf->fq;
-      b.frame_tbl = kf->fq_tbl;
-      KF_CHECK(dalloc(kf, &b.cand_thr, nsb * 5));
-    }
-  }
+  if (dering) STEP_TRY(dering_alloc(kf, dering));
   // dalloc's cudaMemset runs on the legacy default stream, asynchronously, and the engine's stream does not
   // synchronise with it (cudaStreamNonBlocking): wait for every clear before anything is launched -- the table
   // fill below used to race with the clear of its own buffer (intermittently all-zero 1/sqrt table)
@@ -2512,6 +2550,31 @@ static void enqueue_sym(const Sym& Y, int wide, cudaStream_t s) {
   k_sym_index<<<1, 256, 0, s>>>(Y);
 }
 
+// The gather of the luma or chroma stage S in the step's kernel form (haar_dc_quant: only chroma reads the DC grids).
+static void enqueue_gather(StepForm form, const Stage& S, bool chroma, int grid, cudaStream_t s) {
+  if (!chroma) switch (form) {
+    case kFormMixed: k_gather<kGatherLuma, false, true><<<grid, 256, 0, s>>>(S); break;
+    case kFormInter: k_gather<kGatherInter><<<grid, 256, 0, s>>>(S); break;
+    case kFormKeyHdc: case kFormKey: k_gather<kGatherLuma><<<grid, 256, 0, s>>>(S); break;
+  }
+  else switch (form) {
+    case kFormMixed: k_gather<kGatherChroma, true, true><<<grid, 256, 0, s>>>(S); break;
+    case kFormInter: k_gather<kGatherInter><<<grid, 256, 0, s>>>(S); break;
+    case kFormKeyHdc: k_gather<kGatherChroma, true><<<grid, 256, 0, s>>>(S); break;
+    case kFormKey: k_gather<kGatherChroma><<<grid, 256, 0, s>>>(S); break;
+  }
+}
+
+// The finishing scatter of stage S in the step's kernel form.
+static void enqueue_finish_scatter(StepForm form, const Stage& S, int grid, cudaStream_t s) {
+  switch (form) {
+    case kFormMixed: k_finish_scatter<false, true, true><<<grid, 256, 0, s>>>(S); break;
+    case kFormInter: k_finish_scatter<true><<<grid, 256, 0, s>>>(S); break;
+    case kFormKeyHdc: k_finish_scatter<false, true><<<grid, 256, 0, s>>>(S); break;
+    case kFormKey: k_finish_scatter<false><<<grid, 256, 0, s>>>(S); break;
+  }
+}
+
 // config.inter_mc: the bad-ref counters cleared and the leaves of the MV grids (DAALA_B200_KF_LISTS), then OBMC into the
 // prediction planes (DAALA_B200_KF_FORWARD).
 static int enqueue_mc(daala_b200_kf* kf, int phases, cudaStream_t s) {
@@ -2525,12 +2588,6 @@ static int enqueue_mc(daala_b200_kf* kf, int phases, cudaStream_t s) {
   }
   return phases & DAALA_B200_KF_FORWARD ? daala_b200_launch_mc_obmc(&kf->mc, wide, s) : 0;
 }
-
-#define STEP_TRY(x)           \
-  do {                        \
-    const int rc_ = (int)(x); \
-    if (rc_) return rc_;      \
-  } while (0)
 
 // Everything between "inputs are in HBM" and "results are in HBM" for every lossy engine, each piece under its phase
 // bit.  The engine has keyframes (`key`: !inter, or frame_types) and / or P / B frames (`pb`: inter).  The whole step of
@@ -2554,7 +2611,7 @@ static int enqueue_mc(daala_b200_kf* kf, int phases, cudaStream_t s) {
 // leave idle.  The branches write disjoint buffers; only the order of independent work differs between the two forms.
 static int enqueue_step(daala_b200_kf* kf, int phases) {
   const daala_b200_kf_config& cfg = kf->cfg;
-  const bool key = !cfg.inter || cfg.frame_types, pb = cfg.inter != 0, mixed = cfg.frame_types != 0;
+  const bool key = kf->key, pb = kf->pb, mixed = kf->mixed;
   const bool hdc = cfg.haar_dc_quant != 0, core = (phases & DAALA_B200_KF_SEARCH_ONLY) != 0;
   cudaStream_t s = kf->stream, c = phases == DAALA_B200_KF_ALL && kf->side ? kf->side : s;
   const Lists& L = kf->lists;
@@ -2608,9 +2665,7 @@ static int enqueue_step(daala_b200_kf* kf, int phases) {
       if (mixed) k_begin_pvq<<<1, 256, 0, s>>>(K.cnt, K.ring, persist * kPersistThreads / 32);
       else k_begin_pvq<<<1, 32, 0, s>>>(K.cnt);
     }
-    if (!core && mixed) k_gather<kGatherLuma, false, true><<<wide, 256, 0, s>>>(kf->luma);
-    else if (!core && pb) k_gather<kGatherInter><<<wide, 256, 0, s>>>(kf->luma);
-    else if (!core) k_gather<kGatherLuma><<<wide, 256, 0, s>>>(kf->luma);
+    if (!core) enqueue_gather(kf->form, kf->luma, false, wide, s);
     if (pb) STEP_TRY(join(kEvLumaGather, s, c));
     if (key) k_pvq_persist<<<persist, kPersistThreads, 0, s>>>(K);
     if (pb) {
@@ -2620,34 +2675,26 @@ static int enqueue_step(daala_b200_kf* kf, int phases) {
   }
   STEP_TRY(join(kEvLumaBands, s, c));
   if (phases & DAALA_B200_KF_PVQ_CHROMA) {
-    if (!core && mixed) k_gather<kGatherChroma, true, true><<<wide, 256, 0, c>>>(kf->chroma);
-    else if (!core && pb) k_gather<kGatherInter><<<wide, 256, 0, c>>>(kf->chroma);
-    else if (!core && hdc) k_gather<kGatherChroma, true><<<wide, 256, 0, c>>>(kf->chroma);
-    else if (!core) k_gather<kGatherChroma><<<wide, 256, 0, c>>>(kf->chroma);
+    if (!core) enqueue_gather(kf->form, kf->chroma, true, wide, c);
     enqueue_split(kf, kf->chroma, c);
-    if (!core && mixed) k_finish_scatter<false, true, true><<<wide, 256, 0, c>>>(kf->chroma);
-    else if (!core && pb) k_finish_scatter<true><<<wide, 256, 0, c>>>(kf->chroma);
-    else if (!core && hdc) k_finish_scatter<false, true><<<wide, 256, 0, c>>>(kf->chroma);
-    else if (!core) k_finish_scatter<false><<<wide, 256, 0, c>>>(kf->chroma);
+    if (!core) enqueue_finish_scatter(kf->form, kf->chroma, wide, c);
   }
   if (!core && (phases & DAALA_B200_KF_PVQ_LUMA)) {
     if (hdc) STEP_TRY(wait(kEvHaarDc, s));
     if (pb) STEP_TRY(wait(kEvInterLuma, s));
     // forked: 16 waves of short CTAs instead of one resident wave: priority only orders CTAs that are still waiting, so
     // a grid that fits the GPU at once would hold every SM until it is done and stall the chroma gather behind it
-    const int grid = c != s ? kf->sms * 128 : wide;
-    if (mixed) k_finish_scatter<false, true, true><<<grid, 256, 0, s>>>(kf->luma);
-    else if (pb) k_finish_scatter<true><<<grid, 256, 0, s>>>(kf->luma);
-    else if (hdc) k_finish_scatter<false, true><<<grid, 256, 0, s>>>(kf->luma);
-    else k_finish_scatter<false><<<grid, 256, 0, s>>>(kf->luma);
+    enqueue_finish_scatter(kf->form, kf->luma, c != s ? kf->sms * 128 : wide, s);
   }
   if (!core && (phases & DAALA_B200_KF_PVQ_CHROMA) && (cfg.late_skip || cfg.symbol_stream)) {
     // after the luma scatter, and so (hdc) after kEvHaarDc too: the stream's DC records need the DC chain's grids
     STEP_TRY(join(kEvLumaScatter, s, c));
     if (cfg.late_skip) STEP_TRY(daala_b200_late_skip_enqueue(&kf->lsb, kf->sms * 3, c));
-    if (cfg.symbol_stream == 3) enqueue_sym<kSymMixed>(kf->sym, wide, c);
-    else if (cfg.symbol_stream && pb) enqueue_sym<kSymInter>(kf->sym, wide, c);
-    else if (cfg.symbol_stream) enqueue_sym<kSymKey>(kf->sym, wide, c);
+    if (cfg.symbol_stream) switch (kf->form) {
+      case kFormMixed: enqueue_sym<kSymMixed>(kf->sym, wide, c); break;
+      case kFormInter: enqueue_sym<kSymInter>(kf->sym, wide, c); break;
+      case kFormKeyHdc: case kFormKey: enqueue_sym<kSymKey>(kf->sym, wide, c); break;
+    }
   }
 
   if (phases & DAALA_B200_KF_INVERSE) {
@@ -2660,7 +2707,6 @@ static int enqueue_step(daala_b200_kf* kf, int phases) {
   }
   return (int)cudaGetLastError();
 }
-#undef STEP_TRY
 
 // config.lossless: the whole step, one phase.  [inter_mc: leaf enumeration and OBMC, unchanged], the lossless kernels.
 static int kf_enqueue_step_lossless(daala_b200_kf* kf, int phases) {
@@ -2696,9 +2742,11 @@ extern "C" {
 // why the last daala_b200_kf_create of this thread returned NULL (daala_b200_kf_error(NULL))
 static thread_local char g_create_err[256] = "null engine";
 
-daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
-  snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: invalid configuration");
-  if (cfg && cfg->frame_types) {
+// Why daala_b200_kf_create refuses cfg, or nullptr.  The first rule a config breaks names it.
+static const char* config_refusal(const daala_b200_kf_config* cfg) {
+  static const char kInvalid[] = "invalid configuration";
+  if (!cfg) return kInvalid;
+  if (cfg->frame_types) {
     // the mixed step is the keyframe path of keyframe_quant + haar_dc_quant beside the P-frame path of frame_quant, with
     // keyframe deringing in the finishing pass; the stages below have no mixed form
     const char* why = cfg->frame_types != 1 ? "frame_types is 0 or 1"
@@ -2712,110 +2760,89 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
                       : cfg->lossless ? "frame_types is not defined with lossless"
                       : cfg->dering ? "frame_types is not defined with dering (keyframes are deringed in the finishing pass)"
                       : cfg->sb_rows > 0 ? "frame_types is not defined with a row shard (sb_rows > 0)" : nullptr;
-    if (why) {
-      snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: %s", why);
-      return nullptr;
-    }
+    if (why) return why;
   }
-  if (cfg && cfg->inter_mc && (cfg->inter_mc != 1 || cfg->inter != 1)) {
-    snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: inter_mc is 0 or 1, and 1 requires inter = 1");
-    return nullptr;
+  if (cfg->inter_mc && (cfg->inter_mc != 1 || cfg->inter != 1)) return "inter_mc is 0 or 1, and 1 requires inter = 1";
+  if (cfg->mc_next && (cfg->mc_next != 1 || cfg->inter_mc != 1)) return "mc_next is 0 or 1, and 1 requires inter_mc = 1";
+  if (cfg->inter_finish && (cfg->inter_finish < 0 || cfg->inter_finish > 2 || cfg->inter != 1))
+    return "inter_finish is 0, 1 or 2, and 1 and 2 require inter = 1";
+  if (cfg->symbol_stream < 0 || cfg->symbol_stream > 3 || (cfg->symbol_stream == 2 && cfg->inter != 1) ||
+      (cfg->symbol_stream == 3 && cfg->frame_types != 1))
+    return "symbol_stream is 0, 1, 2 or 3; 2 requires inter = 1 (a keyframe's DC goes through the Haar pyramid and has "
+           "no scalar index) and 3 (the mixed stream) frame_types = 1";
+  if (cfg->late_skip && (cfg->late_skip != 1 || cfg->inter != 1))
+    return "late_skip is 0 or 1, and 1 requires inter = 1 (keyframes have no late skip)";
+  if (cfg->frame_quant && (cfg->frame_quant != 1 || cfg->inter != 1))
+    return "frame_quant is 0 or 1, and 1 requires inter = 1 (keyframes: keyframe_quant = 1)";
+  // "<mode> is not defined with <with>": the first setting the mode has no form for
+  static thread_local char msg[200];   // the longest message fits, with its prefix, in an error string
+  auto undefined = [](const char* mode, const char* with) {
+    if (with) snprintf(msg, sizeof(msg), "%s is not defined with %s", mode, with);
+    return with ? msg : nullptr;
+  };
+  const char* why = nullptr;
+  // the kernels that read the quantizer in these modes have no per-frame form
+  if (cfg->keyframe_quant)
+    why = undefined("keyframe_quant", cfg->keyframe_quant != 1 ? "a value other than 0 or 1"
+                                      : cfg->inter ? "inter (P and B frames take their records with frame_quant = 1)"
+                                      : cfg->lossless ? "lossless (every frame is at quantizer 0)"
+                                      : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr);
+  // the lossless path has no PVQ, no deringing and no coder-side state: none of these stages exists for it
+  if (!why && cfg->lossless)
+    why = undefined("lossless", cfg->lossless != 1 ? "a value other than 0 or 1"
+                                : cfg->dering ? "dering (lossless frames skip deringing)"
+                                : cfg->symbol_stream ? "symbol_stream (the stream is the PVQ symbols)"
+                                : cfg->late_skip ? "late_skip"
+                                : cfg->inter_finish ? "inter_finish"
+                                : cfg->frame_quant ? "frame_quant (every frame is at quantizer 0)"
+                                : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr);
+  // the chain quantises the Haar DC pyramid of lossy keyframes; the superblock predictor reads the superblocks above,
+  // across any row shard
+  if (!why && cfg->haar_dc_quant)
+    why = undefined("haar_dc_quant", cfg->haar_dc_quant != 1 ? "a value other than 0 or 1"
+                                     : cfg->inter && !cfg->frame_types ? "inter (P and B frames code a scalar DC per block)"
+                                     : cfg->lossless ? "lossless (its keyframe DCs are coded exactly)"
+                                     : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr);
+  if (why) return why;
+  // the records made from the config follow the records' rule (quantizer 0 is the lossless engine's)
+  if (!cfg->lossless && (cfg->q0 < 1 || cfg->q0 > DAALA_B200_KF_MAX_Q0)) {
+    snprintf(msg, sizeof(msg), "q0 is outside [1, %d] (lossless = 1 codes quantizer 0)", DAALA_B200_KF_MAX_Q0);
+    return msg;
   }
-  if (cfg && cfg->mc_next && (cfg->mc_next != 1 || cfg->inter_mc != 1)) {
-    snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: mc_next is 0 or 1, and 1 requires inter_mc = 1");
-    return nullptr;
-  }
-  if (cfg && cfg->inter_finish && (cfg->inter_finish < 0 || cfg->inter_finish > 2 || cfg->inter != 1)) {
-    snprintf(g_create_err, sizeof(g_create_err),
-             "daala_b200_kf_create: inter_finish is 0, 1 or 2, and 1 and 2 require inter = 1");
-    return nullptr;
-  }
-  if (cfg && (cfg->symbol_stream < 0 || cfg->symbol_stream > 3 || (cfg->symbol_stream == 2 && cfg->inter != 1) ||
-              (cfg->symbol_stream == 3 && cfg->frame_types != 1))) {
-    snprintf(g_create_err, sizeof(g_create_err),
-             "daala_b200_kf_create: symbol_stream is 0, 1, 2 or 3; 2 requires inter = 1 (a keyframe's DC goes through "
-             "the Haar pyramid and has no scalar index) and 3 (the mixed stream) frame_types = 1");
-    return nullptr;
-  }
-  if (cfg && cfg->late_skip && (cfg->late_skip != 1 || cfg->inter != 1)) {
-    snprintf(g_create_err, sizeof(g_create_err),
-             "daala_b200_kf_create: late_skip is 0 or 1, and 1 requires inter = 1 (keyframes have no late skip)");
-    return nullptr;
-  }
-  if (cfg && cfg->frame_quant && (cfg->frame_quant != 1 || cfg->inter != 1)) {
-    snprintf(g_create_err, sizeof(g_create_err),
-             "daala_b200_kf_create: frame_quant is 0 or 1, and 1 requires inter = 1 (keyframes: keyframe_quant = 1)");
-    return nullptr;
-  }
-  if (cfg && cfg->keyframe_quant) {
-    // the kernels that read the quantizer in these modes have no per-frame form
-    const char* with = cfg->keyframe_quant != 1 ? "a value other than 0 or 1"
-                       : cfg->inter ? "inter (P and B frames take their records with frame_quant = 1)"
-                       : cfg->lossless ? "lossless (every frame is at quantizer 0)"
-                       : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
-    if (with) {
-      snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: keyframe_quant is not defined with %s", with);
-      return nullptr;
-    }
-  }
-  if (cfg && cfg->lossless) {
-    // the lossless path has no PVQ, no deringing and no coder-side state: none of these stages exists for it
-    const char* with = cfg->lossless != 1 ? "a value other than 0 or 1"
-                       : cfg->dering ? "dering (lossless frames skip deringing)"
-                       : cfg->symbol_stream ? "symbol_stream (the stream is the PVQ symbols)"
-                       : cfg->late_skip ? "late_skip"
-                       : cfg->inter_finish ? "inter_finish"
-                       : cfg->frame_quant ? "frame_quant (every frame is at quantizer 0)"
-                       : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
-    if (with) {
-      snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: lossless is not defined with %s", with);
-      return nullptr;
-    }
-  }
-  if (cfg && cfg->haar_dc_quant) {
-    // the chain quantises the Haar DC pyramid of lossy keyframes; the superblock predictor reads the superblocks above,
-    // across any row shard
-    const char* with = cfg->haar_dc_quant != 1 ? "a value other than 0 or 1"
-                       : cfg->inter && !cfg->frame_types ? "inter (P and B frames code a scalar DC per block)"
-                       : cfg->lossless ? "lossless (its keyframe DCs are coded exactly)"
-                       : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
-    if (with) {
-      snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: haar_dc_quant is not defined with %s", with);
-      return nullptr;
-    }
-  }
-  if (cfg && !cfg->lossless && (cfg->q0 < 1 || cfg->q0 > DAALA_B200_KF_MAX_Q0)) {
-    // the records made from the config follow the records' rule (quantizer 0 is the lossless engine's)
-    snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: q0 is outside [1, %d] (lossless = 1 codes quantizer 0)",
-             DAALA_B200_KF_MAX_Q0);
-    return nullptr;
-  }
-  if (cfg && cfg->mc_refs < 0) {
-    snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: mc_refs < 0");
-    return nullptr;
-  }
-  if (cfg && cfg->inter) {
-    // P-frame residual mode is defined for whole frames through the phase kernels, without the stages whose
-    // inter form this engine does not have
-    const char* with = cfg->inter != 1 ? "a value other than 0 or 1"
-                       : cfg->dering ? "dering (the all-zero skip map of the deringing stage is a keyframe property)"
-                       : cfg->symbol_stream == 1 ? "symbol_stream = 1 (its block record has no DC field; "
-                                                   "symbol_stream = 2 is the P-frame stream)"
-                       : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr;
-    if (with) {
-      snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: inter is not defined with %s", with);
-      return nullptr;
-    }
-  }
-  if (!cfg || cfg->pic_w <= 0 || cfg->pic_h <= 0 || cfg->nframes <= 0 || cfg->nframes > 255 || !cfg->qm ||
-      !cfg->qm_inv || cfg->qm_stride <= 0)
-    return nullptr;
+  if (cfg->mc_refs < 0) return "mc_refs < 0";
+  // P-frame residual mode is defined for whole frames through the phase kernels, without the stages whose inter form
+  // this engine does not have
+  if (cfg->inter)
+    why = undefined("inter", cfg->inter != 1 ? "a value other than 0 or 1"
+                             : cfg->dering ? "dering (the all-zero skip map of the deringing stage is a keyframe property)"
+                             : cfg->symbol_stream == 1 ? "symbol_stream = 1 (its block record has no DC field; "
+                                                         "symbol_stream = 2 is the P-frame stream)"
+                             : cfg->sb_rows > 0 ? "a row shard (sb_rows > 0)" : nullptr);
+  if (why) return why;
+  if (cfg->pic_w <= 0 || cfg->pic_h <= 0 || cfg->nframes <= 0 || cfg->nframes > 255 || !cfg->qm || !cfg->qm_inv ||
+      cfg->qm_stride <= 0)
+    return kInvalid;
+  // coefficient offsets are 32-bit: the whole batch must stay below 2^31 coded coefficients
+  if ((long long)((cfg->pic_w + 63) / 64 * 64) * ((cfg->pic_h + 63) / 64 * 64) * cfg->nframes >= (1ll << 31))
+    return kInvalid;
+  return nullptr;
+}
+
+daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
+  const char* why = config_refusal(cfg);
+  // a device or stream failure below keeps the default message
+  snprintf(g_create_err, sizeof(g_create_err), "daala_b200_kf_create: %s", why ? why : "invalid configuration");
+  if (why) return nullptr;
   daala_b200_kf* kf = new (std::nothrow) daala_b200_kf();   // value-initialised: every field zero
   if (!kf) return nullptr;
   kf->cfg = *cfg;
   kf->nhsb = (cfg->pic_w + 63) / 64;
   kf->nvsb = (cfg->pic_h + 63) / 64;
   kf->F = cfg->nframes;
+  kf->key = !cfg->inter || cfg->frame_types;
+  kf->pb = cfg->inter != 0;
+  kf->mixed = cfg->frame_types != 0;
+  kf->form = kf->mixed ? kFormMixed : kf->pb ? kFormInter : cfg->haar_dc_quant ? kFormKeyHdc : kFormKey;
   if (kf->cfg.inter_mc && kf->cfg.mc_refs == 0) kf->cfg.mc_refs = (kf->cfg.mc_next ? 3 : 2) * kf->F;
   if (!kf->cfg.inter_mc) kf->cfg.mc_refs = 0;
   kf->slot_filled.assign((size_t)kf->cfg.mc_refs, 0);
@@ -2826,11 +2853,6 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
   for (int p = 0; p < 3; p++) {
     kf->plane_w[p] = (kf->nhsb * 64) >> (p ? 1 : 0);
     kf->plane_h[p] = (kf->nvsb * 64) >> (p ? 1 : 0);
-  }
-  // coefficient offsets are 32-bit (ADVICE r1): the whole batch must stay below 2^31 coded coefficients
-  if ((long long)kf->plane_w[0] * kf->plane_h[0] * kf->F >= (1ll << 31)) {
-    delete kf;
-    return nullptr;
   }
   int dev = 0;
   cudaDeviceProp prop;
@@ -2848,7 +2870,7 @@ daala_b200_kf* daala_b200_kf_create(const daala_b200_kf_config* cfg) {
     }
     kf->own_stream = true;
   }
-  if ((!cfg->inter && !cfg->lossless) || cfg->frame_types) {
+  if (kf->key && !cfg->lossless) {
     // the side branch carries the longer chain (the chroma stage) at the highest priority: the luma branch's CTAs
     // then take the SMs the chroma kernels leave idle instead of delaying them
     int least = 0, greatest = 0;
@@ -2905,7 +2927,7 @@ int daala_b200_kf_launches_per_step(const daala_b200_kf* kf) {
   const daala_b200_kf_config& cfg = kf->cfg;
   // lossless: [leaves + OBMC], the forward kernel, [keyframes: the DC + reconstruction kernel]
   if (cfg.lossless) return (cfg.inter_mc ? 2 : 0) + (cfg.inter ? 1 : 2);
-  const bool key = !cfg.inter || cfg.frame_types, pb = cfg.inter != 0;
+  const bool key = kf->key, pb = kf->pb;
   auto split = [](const Stage& S) { return 3 * (S.sp_chunks[0] + S.sp_chunks[1] + S.sp_chunks[2]); };
   int n = (cfg.inter_mc ? 2 : 0) + 1 + (pb ? 1 : 0);               // [leaves, OBMC], source transform, [prediction's]
   n += 3 + (key ? 1 : 0) + (pb ? 1 : 0) + 1;                          // work lists: scan, [deps], [luma items], chroma items
@@ -3005,25 +3027,29 @@ int daala_b200_kf_run_device(daala_b200_kf* kf, int phases, int use_graph) {
 // resident in HBM); returns the total in milliseconds.
 int daala_b200_kf_time_device(daala_b200_kf* kf, int phases, int use_graph, int reps, float* ms) {
   if (!kf || !ms || reps <= 0) return (int)cudaErrorInvalidValue;
-  cudaEvent_t e0, e1;
-  KF_CHECK(cudaEventCreate(&e0));
-  KF_CHECK(cudaEventCreate(&e1));
-  if (use_graph && phases == DAALA_B200_KF_ALL && !kf->captured) {
-    int rc = daala_b200_kf_run_device(kf, phases, 1);
-    if (rc) return rc;
-  }
-  KF_CHECK(cudaStreamSynchronize(kf->stream));
-  KF_CHECK(cudaEventRecord(e0, kf->stream));
-  for (int i = 0; i < reps; i++) {
-    int rc = daala_b200_kf_run_device(kf, phases, use_graph);
-    if (rc) return rc;
-  }
-  KF_CHECK(cudaEventRecord(e1, kf->stream));
-  KF_CHECK(cudaEventSynchronize(e1));
-  KF_CHECK(cudaEventElapsedTime(ms, e0, e1));
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  return 0;
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  auto timed = [&]() -> int {
+    KF_CHECK(cudaEventCreate(&e0));
+    KF_CHECK(cudaEventCreate(&e1));
+    if (use_graph && phases == DAALA_B200_KF_ALL && !kf->captured) {
+      int rc = daala_b200_kf_run_device(kf, phases, 1);
+      if (rc) return rc;
+    }
+    KF_CHECK(cudaStreamSynchronize(kf->stream));
+    KF_CHECK(cudaEventRecord(e0, kf->stream));
+    for (int i = 0; i < reps; i++) {
+      int rc = daala_b200_kf_run_device(kf, phases, use_graph);
+      if (rc) return rc;
+    }
+    KF_CHECK(cudaEventRecord(e1, kf->stream));
+    KF_CHECK(cudaEventSynchronize(e1));
+    KF_CHECK(cudaEventElapsedTime(ms, e0, e1));
+    return 0;
+  };
+  const int rc = timed();
+  if (e0) cudaEventDestroy(e0);
+  if (e1) cudaEventDestroy(e1);
+  return rc;
 }
 
 // Totals that follow from the block-size maps (what the host needs to size its result buffers):
@@ -3068,19 +3094,30 @@ int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals* t, int nframes, daal
   return 0;
 }
 
-// A requested stream buffer: large enough, and pinned host memory the device can write (its device address).
-static int sym_target(const void* p, long long cap, long long need, uint8_t** dev) {
-  *dev = nullptr;
-  if (!p) return 0;
-  if (cap < need) return (int)cudaErrorInvalidValue;
+// One array of the symbol stream a submit may request (segment i of SymCopy): the caller's buffer, its capacity and
+// what the batch needs at most (elements), bytes per element, the engine's array and its capacity (elements, 0: the
+// engine has none), the name and bound a refusal gives, and the buffer's device address once accepted.
+struct SymSeg {
+  const char *name, *bound;
+  const void* host;
+  long long cap, need, unit;
+  const uint8_t* src;
+  long long src_cap;
+  uint8_t* dst;
+};
+
+// A requested stream buffer: large enough, and pinned host memory the device can write (its device address in dst).
+static bool sym_target(SymSeg& g) {
+  if (!g.host) return true;
+  if (g.cap < g.need) return false;
   cudaPointerAttributes a;
-  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+  if (cudaPointerGetAttributes(&a, g.host) != cudaSuccess) {
     cudaGetLastError();
-    return (int)cudaErrorInvalidValue;
+    return false;
   }
-  if (a.type != cudaMemoryTypeHost || !a.devicePointer) return (int)cudaErrorInvalidValue;
-  *dev = (uint8_t*)a.devicePointer;
-  return 0;
+  if (a.type != cudaMemoryTypeHost || !a.devicePointer) return false;
+  g.dst = (uint8_t*)a.devicePointer;
+  return true;
 }
 
 int daala_b200_kf_load_frame_quant(daala_b200_kf* kf, const daala_b200_kf_frame_quant* rec) {
@@ -3098,73 +3135,54 @@ int daala_b200_kf_load_frame_quant(daala_b200_kf* kf, const daala_b200_kf_frame_
   return 0;
 }
 
-int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
-  if (!kf || !io) return (int)cudaErrorInvalidValue;
-  cudaStream_t s = kf->stream;
+// Why daala_b200_kf_submit refuses io, or nullptr.  Every check runs before anything is copied or launched.  When io
+// is accepted: *tot holds the batch's totals, *fq_dc_limit the finishing pass's DC limit of its records (frame_quant /
+// keyframe_quant engines, whose host tables then hold the step's) and seg[] the stream arrays it requests.
+static const char* submit_refusal(daala_b200_kf* kf, const daala_b200_kf_io* io, daala_b200_kf_totals* tot,
+                                  int* fq_dc_limit, SymSeg* seg) {
+  static thread_local char msg[200];   // the longest message fits, with its prefix, in an error string
+  if (!io) return "io is required";
+  const daala_b200_kf_config& cfg = kf->cfg;
   const int F = kf->F;
-  const bool lossless = kf->cfg.lossless != 0;
-  if (!io->bsize && !lossless) return (int)cudaErrorInvalidValue;
-  // refuse a batch with more blocks than the work lists hold before anything is copied or launched: the
-  // step would otherwise run on truncated lists (a lossless step has no block lists)
-  daala_b200_kf_totals tot;
-  memset(&tot, 0, sizeof(tot));
-  if (lossless) {
-  } else if (io->totals) {
-    tot = *io->totals;
-  } else {
+  const bool lossless = cfg.lossless != 0;
+  if (!io->bsize && !lossless) return "bsize is required";
+  // a batch with more blocks than the work lists hold would run on truncated lists (a lossless step has none)
+  memset(tot, 0, sizeof(*tot));
+  if (!lossless && io->totals)
+    *tot = *io->totals;
+  else if (!lossless)
     daala_b200_kf_count_blocks(io->bsize, F, (long long)kf->nhsb * 8 * kf->nvsb * 8, kf->nhsb * 8, kf->nhsb, kf->nvsb,
-                               kf->cfg.sb_row0, kf->cfg.sb_rows, &tot);
-  }
-  if (tot.n_luma > kf->lists.max_luma || tot.n_chroma > kf->lists.max_chroma) return (int)cudaErrorInvalidValue;
+                               cfg.sb_row0, cfg.sb_rows, tot);
+  if (tot->n_luma > kf->lists.max_luma || tot->n_chroma > kf->lists.max_chroma)
+    return "the batch has more luma or chroma blocks than the engine holds (config.max_blocks_div)";
   const bool have_pred = io->pred_pixels[0] || io->pred_pixels[1] || io->pred_pixels[2];
   // symbol_stream = 2 or 3: the stream's DC records carry the DC indices, so the classic arrays are optional; a
   // lossless step has no scalar DC index
-  const bool need_dc = !lossless && kf->cfg.symbol_stream < 2 && (!io->luma_dc || !io->chroma_dc);
+  const bool need_dc = !lossless && cfg.symbol_stream < 2 && (!io->luma_dc || !io->chroma_dc);
   // the lossless outputs: only a lossless engine has them, and only one with the pool stores into it
   const bool want_ll = io->ll_coeffs[0] || io->ll_coeffs[1] || io->ll_coeffs[2] || io->ll_blocks;
-  const char* ll_why = (want_ll || io->ll_ref_slot_out) && !lossless
-                           ? "ll_coeffs / ll_blocks / ll_ref_slot_out need an engine with lossless = 1"
-                       : io->ll_ref_slot_out && !kf->cfg.inter_mc
-                           ? "ll_ref_slot_out needs an engine with inter_mc (the reference-picture pool)"
-                           : nullptr;
-  for (int f = 0; !ll_why && io->ll_ref_slot_out && f < F; f++) {
+  if ((want_ll || io->ll_ref_slot_out) && !lossless)
+    return "ll_coeffs / ll_blocks / ll_ref_slot_out need an engine with lossless = 1";
+  if (io->ll_ref_slot_out && !cfg.inter_mc)
+    return "ll_ref_slot_out needs an engine with inter_mc (the reference-picture pool)";
+  for (int f = 0; io->ll_ref_slot_out && f < F; f++) {
     const int32_t r = io->ll_ref_slot_out[f];
-    if (r < -1 || r >= kf->cfg.mc_refs) ll_why = "an ll_ref_slot_out entry is outside [-1, mc_refs)";
-    for (int g = 0; !ll_why && r >= 0 && g < f; g++)
-      if (io->ll_ref_slot_out[g] == r) ll_why = "two frames name the same ll_ref_slot_out slot";
-  }
-  if (ll_why) {
-    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", ll_why);
-    return (int)cudaErrorInvalidValue;
+    if (r < -1 || r >= cfg.mc_refs) return "an ll_ref_slot_out entry is outside [-1, mc_refs)";
+    for (int g = 0; r >= 0 && g < f; g++)
+      if (io->ll_ref_slot_out[g] == r) return "two frames name the same ll_ref_slot_out slot";
   }
   // frame_types: a type per frame, 1 (keyframe) or 0 (P or B frame); refused by the other engines
-  const char* ft_why = !kf->cfg.frame_types ? (io->frame_type ? "frame_type needs an engine with frame_types = 1" : nullptr)
-                       : !io->frame_type ? "frame_types: frame_type ([nframes], 1 = keyframe, 0 = P or B frame) is required"
-                                         : nullptr;
-  for (int f = 0; !ft_why && kf->cfg.frame_types && f < F; f++)
-    if (io->frame_type[f] > 1) ft_why = "frame_types: a frame_type entry is neither 0 nor 1";
-  if (ft_why) {
-    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", ft_why);
-    return (int)cudaErrorInvalidValue;
-  }
-  if ((io->dc_index[0] || io->dc_index[1] || io->dc_index[2]) && !kf->cfg.haar_dc_quant) {
-    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: dc_index needs an engine with haar_dc_quant = 1");
-    return (int)cudaErrorInvalidValue;
-  }
-  if (kf->cfg.inter && !kf->cfg.inter_mc &&
-      (!io->pred_pixels[0] || !io->pred_pixels[1] || !io->pred_pixels[2] || need_dc)) {
-    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: an inter engine needs pred_pixels[0..2], luma_dc and chroma_dc");
-    return (int)cudaErrorInvalidValue;
-  }
-  if ((io->ref_slot_next || io->mv1_grid) && !kf->cfg.mc_next) {
-    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: ref_slot_next and mv1_grid need an engine with mc_next");
-    return (int)cudaErrorInvalidValue;
-  }
-  if (io->ref_resident && !kf->cfg.inter_mc) {
-    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: ref_resident needs an engine with inter_mc");
-    return (int)cudaErrorInvalidValue;
-  }
-  if (kf->cfg.inter_mc) {
+  if (!kf->mixed && io->frame_type) return "frame_type needs an engine with frame_types = 1";
+  if (kf->mixed && !io->frame_type) return "frame_types: frame_type ([nframes], 1 = keyframe, 0 = P or B frame) is required";
+  for (int f = 0; kf->mixed && f < F; f++)
+    if (io->frame_type[f] > 1) return "frame_types: a frame_type entry is neither 0 nor 1";
+  if ((io->dc_index[0] || io->dc_index[1] || io->dc_index[2]) && !cfg.haar_dc_quant)
+    return "dc_index needs an engine with haar_dc_quant = 1";
+  if (cfg.inter && !cfg.inter_mc && (!io->pred_pixels[0] || !io->pred_pixels[1] || !io->pred_pixels[2] || need_dc))
+    return "an inter engine needs pred_pixels[0..2], luma_dc and chroma_dc";
+  if ((io->ref_slot_next || io->mv1_grid) && !cfg.mc_next) return "ref_slot_next and mv1_grid need an engine with mc_next";
+  if (io->ref_resident && !cfg.inter_mc) return "ref_resident needs an engine with inter_mc";
+  if (cfg.inter_mc) {
     const bool resident = io->ref_resident != 0;
     const bool any_ref = io->ref_pixels[0] || io->ref_pixels[1] || io->ref_pixels[2];
     const char* why = need_dc ? "luma_dc and chroma_dc are required"
@@ -3175,124 +3193,92 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
                       : !resident && (!io->ref_pixels[0] || !io->ref_pixels[1] || !io->ref_pixels[2])
                           ? "ref_pixels[0..2] are required"
                       : !io->ref_slot ? "ref_slot is required"
-                      : kf->cfg.mc_next && !io->ref_slot_next ? "mc_next: ref_slot_next is required"
-                      : kf->cfg.mc_next && !io->mv1_grid ? "mc_next: mv1_grid is required"
+                      : cfg.mc_next && !io->ref_slot_next ? "mc_next: ref_slot_next is required"
+                      : cfg.mc_next && !io->mv1_grid ? "mc_next: mv1_grid is required"
                       : have_pred ? "pred_pixels is refused: the engine makes the prediction"
-                      : !resident && (io->nrefs < 1 || io->nrefs > kf->cfg.mc_refs) ? "nrefs is outside [1, mc_refs]"
-                                                                                    : nullptr;
+                      : !resident && (io->nrefs < 1 || io->nrefs > cfg.mc_refs) ? "nrefs is outside [1, mc_refs]"
+                                                                                : nullptr;
     // the GOLD / PREV slots, then (mc_next) the NEXT slots
-    const int nslot = (kf->cfg.mc_next ? 3 : 2) * F;
+    const int nslot = (cfg.mc_next ? 3 : 2) * F;
     bool in_next = false;
     for (int i = 0; !why && i < nslot; i++) {
       const int32_t r = i < 2 * F ? io->ref_slot[i] : io->ref_slot_next[i - 2 * F];
       in_next = i >= 2 * F;
-      if (kf->cfg.frame_types && io->frame_type[i < 2 * F ? i / 2 : i - 2 * F]) continue;   // a keyframe reads no picture
+      if (kf->mixed && io->frame_type[i < 2 * F ? i / 2 : i - 2 * F]) continue;   // a keyframe reads no picture
       if (!resident && (r < 0 || r >= io->nrefs)) why = "a ref_slot entry is outside [0, nrefs)";
-      else if (resident && (r < 0 || r >= kf->cfg.mc_refs)) why = "ref_resident: a ref_slot entry is outside [0, mc_refs)";
+      else if (resident && (r < 0 || r >= cfg.mc_refs)) why = "ref_resident: a ref_slot entry is outside [0, mc_refs)";
       else if (resident && !kf->slot_filled[r])
         why = "ref_resident: a ref_slot entry names a pool slot that holds no picture (pool_load, a host-upload "
               "submit or a finish with ref_slot_out writes one)";
     }
     if (why) {
-      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: inter_mc: %s%s", why, in_next ? " (ref_slot_next)" : "");
-      return (int)cudaErrorInvalidValue;
+      snprintf(msg, sizeof(msg), "inter_mc: %s%s", why, in_next ? " (ref_slot_next)" : "");
+      return msg;
     }
   }
   // late-skip records: only an engine with late_skip has them, and only a symbol_stream = 2 engine in stream order
-  const char* ls_why = (io->luma_late_skip || io->chroma_late_skip || io->sym_late_skip) && !kf->cfg.late_skip
-                           ? "luma_late_skip / chroma_late_skip / sym_late_skip need an engine with late_skip = 1"
-                       : io->sym_late_skip && kf->cfg.symbol_stream != 2
-                           ? "sym_late_skip needs an engine with symbol_stream = 2"
-                           : nullptr;
-  if (ls_why) {
-    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", ls_why);
-    return (int)cudaErrorInvalidValue;
-  }
+  if ((io->luma_late_skip || io->chroma_late_skip || io->sym_late_skip) && !cfg.late_skip)
+    return "luma_late_skip / chroma_late_skip / sym_late_skip need an engine with late_skip = 1";
+  if (io->sym_late_skip && cfg.symbol_stream != 2) return "sym_late_skip needs an engine with symbol_stream = 2";
   // per-frame quantizers: every record in range; then each frame's deringing thresholds and band quantisers and the
   // finishing pass's DC limit of this step
-  int fq_dc_limit = 0;
-  const bool fq_mode = kf->cfg.frame_quant || kf->cfg.keyframe_quant;
-  if (io->frame_quant || fq_mode) {
-    const char* why = !fq_mode ? "frame_quant needs an engine with frame_quant = 1 or keyframe_quant = 1"
-                               : fq_derive_host(kf, io->frame_quant, true, &fq_dc_limit);
-    if (why) {
-      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", why);
-      return (int)cudaErrorInvalidValue;
-    }
-  }
+  const bool fq_mode = cfg.frame_quant || cfg.keyframe_quant;
+  if (io->frame_quant && !fq_mode) return "frame_quant needs an engine with frame_quant = 1 or keyframe_quant = 1";
+  if (fq_mode)
+    if (const char* why = fq_derive_host(kf, io->frame_quant, true, fq_dc_limit)) return why;
   // symbol stream: the engine must produce it, and every requested buffer must hold the worst case and be pinned
-  SymCopy sc;
-  memset(&sc, 0, sizeof(sc));
-  const bool want_sym = io->sym_index || io->sym_blocks || io->sym_bands || io->sym_pulses || io->sym_dc ||
-                        io->sym_late_skip || io->sym_hdc;
+  daala_b200_kf_sym_bounds bd;
+  daala_b200_kf_symbol_bounds(tot, F, &bd);
+  const Sym& Y = kf->sym;
+  const long long blk = Y.cap_blocks;
+  seg[0] = {"sym_index", "index records", io->sym_index, io->sym_index_cap, bd.index,
+            sizeof(daala_b200_kf_sym_frame), (const uint8_t*)Y.index, F, nullptr};
+  seg[1] = {"sym_blocks", "blocks records", io->sym_blocks, io->sym_blocks_cap, bd.blocks,
+            sizeof(daala_b200_kf_sym_block), (const uint8_t*)Y.blocks, blk, nullptr};
+  seg[2] = {"sym_bands", "bands records", io->sym_bands, io->sym_bands_cap, bd.bands, 4 * sizeof(int16_t),
+            (const uint8_t*)Y.bands, Y.cap_bands, nullptr};
+  seg[3] = {"sym_pulses", "pulse_bytes bytes", io->sym_pulses, io->sym_pulses_cap, bd.pulse_bytes, 1, Y.pulses,
+            Y.cap_bytes, nullptr};
+  seg[4] = {"sym_dc", "blocks records", io->sym_dc, io->sym_dc_cap, bd.blocks, sizeof(daala_b200_kf_sym_dc),
+            (const uint8_t*)Y.dc, Y.dc ? blk : 0, nullptr};
+  seg[5] = {"sym_late_skip", "blocks records", io->sym_late_skip, io->sym_late_skip_cap, bd.blocks,
+            sizeof(daala_b200_kf_late_skip), (const uint8_t*)Y.late_skip, Y.late_skip ? blk : 0, nullptr};
+  seg[6] = {"sym_hdc", "blocks records", io->sym_hdc, io->sym_hdc_cap, bd.blocks, sizeof(daala_b200_kf_sym_hdc),
+            (const uint8_t*)Y.hdc, Y.hdc ? blk : 0, nullptr};
+  bool want_sym = false;
+  for (int i = 0; i < kSymSegs; i++) want_sym = want_sym || seg[i].host;
   if (want_sym) {
-    if (io->sym_hdc && !((kf->cfg.symbol_stream == 1 && kf->cfg.haar_dc_quant) || kf->cfg.symbol_stream == 3)) {
-      snprintf(kf->err, sizeof(kf->err),
-               "daala_b200_kf_submit: sym_hdc needs an engine with symbol_stream = 1 and haar_dc_quant = 1, or "
-               "symbol_stream = 3");
-      return (int)cudaErrorInvalidValue;
-    }
-    if (!kf->cfg.symbol_stream) return (int)cudaErrorInvalidValue;
-    if (io->sym_dc && kf->cfg.symbol_stream < 2) {
-      snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: sym_dc needs an engine with symbol_stream = 2 or 3");
-      return (int)cudaErrorInvalidValue;
-    }
-    daala_b200_kf_sym_bounds bd;
-    daala_b200_kf_symbol_bounds(&tot, F, &bd);
-    int e = sym_target(io->sym_index, io->sym_index_cap, bd.index, &sc.dst[0]);
-    if (!e) e = sym_target(io->sym_blocks, io->sym_blocks_cap, bd.blocks, &sc.dst[1]);
-    if (!e) e = sym_target(io->sym_bands, io->sym_bands_cap, bd.bands, &sc.dst[2]);
-    if (!e) e = sym_target(io->sym_pulses, io->sym_pulses_cap, bd.pulse_bytes, &sc.dst[3]);
-    if (e) return e;
-    if (sym_target(io->sym_dc, io->sym_dc_cap, bd.blocks, &sc.dst[4])) {
-      snprintf(kf->err, sizeof(kf->err),
-               "daala_b200_kf_submit: sym_dc must be pinned host memory of at least "
-               "daala_b200_kf_symbol_bounds(...).blocks records");
-      return (int)cudaErrorInvalidValue;
-    }
-    if (sym_target(io->sym_late_skip, io->sym_late_skip_cap, bd.blocks, &sc.dst[5])) {
-      snprintf(kf->err, sizeof(kf->err),
-               "daala_b200_kf_submit: sym_late_skip must be pinned host memory of at least "
-               "daala_b200_kf_symbol_bounds(...).blocks records");
-      return (int)cudaErrorInvalidValue;
-    }
-    if (sym_target(io->sym_hdc, io->sym_hdc_cap, bd.blocks, &sc.dst[6])) {
-      snprintf(kf->err, sizeof(kf->err),
-               "daala_b200_kf_submit: sym_hdc must be pinned host memory of at least "
-               "daala_b200_kf_symbol_bounds(...).blocks records");
-      return (int)cudaErrorInvalidValue;
-    }
-    const Sym& Y = kf->sym;
-    sc.src[0] = (const uint8_t*)Y.index;
-    sc.src[1] = (const uint8_t*)Y.blocks;
-    sc.src[2] = (const uint8_t*)Y.bands;
-    sc.src[3] = Y.pulses;
-    sc.src[4] = (const uint8_t*)Y.dc;
-    sc.src[5] = (const uint8_t*)Y.late_skip;
-    sc.src[6] = (const uint8_t*)Y.hdc;
-    sc.unit[1] = sizeof(daala_b200_kf_sym_block);
-    sc.unit[2] = 4 * sizeof(int16_t);
-    sc.unit[3] = 1;
-    sc.unit[4] = sizeof(daala_b200_kf_sym_dc);
-    sc.unit[5] = sizeof(daala_b200_kf_late_skip);
-    sc.unit[6] = sizeof(daala_b200_kf_sym_hdc);
-    sc.index_bytes = (long long)F * sizeof(daala_b200_kf_sym_frame);
-    sc.tot = Y.tot;
-    const long long host[kSymSegs] = {io->sym_index_cap * (long long)sizeof(daala_b200_kf_sym_frame),
-                                      io->sym_blocks_cap * (long long)sizeof(daala_b200_kf_sym_block),
-                                      io->sym_bands_cap * 8, io->sym_pulses_cap,
-                                      io->sym_dc_cap * (long long)sizeof(daala_b200_kf_sym_dc),
-                                      io->sym_late_skip_cap * (long long)sizeof(daala_b200_kf_late_skip),
-                                      io->sym_hdc_cap * (long long)sizeof(daala_b200_kf_sym_hdc)};
-    const long long dev[kSymSegs] = {sc.index_bytes, (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_block),
-                                     Y.cap_bands * 8, Y.cap_bytes,
-                                     Y.dc ? (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_dc) : 0,
-                                     Y.late_skip ? (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_late_skip) : 0,
-                                     Y.hdc ? (long long)Y.cap_blocks * (long long)sizeof(daala_b200_kf_sym_hdc) : 0};
-    for (int i = 0; i < kSymSegs; i++) sc.cap[i] = host[i] < dev[i] ? host[i] : dev[i];
+    if (io->sym_hdc && !((cfg.symbol_stream == 1 && cfg.haar_dc_quant) || cfg.symbol_stream == 3))
+      return "sym_hdc needs an engine with symbol_stream = 1 and haar_dc_quant = 1, or symbol_stream = 3";
+    if (!cfg.symbol_stream) return "sym_index / sym_blocks / sym_bands / sym_pulses need an engine with symbol_stream";
+    if (io->sym_dc && cfg.symbol_stream < 2) return "sym_dc needs an engine with symbol_stream = 2 or 3";
+    for (int i = 0; i < kSymSegs; i++)
+      if (!sym_target(seg[i])) {
+        snprintf(msg, sizeof(msg), "%s must be pinned host memory of at least daala_b200_kf_symbol_bounds(...).%s",
+                 seg[i].name, seg[i].bound);
+        return msg;
+      }
   }
+  for (int p = 0; p < 3; p++)
+    if (!io->pixels[p]) return "pixels[0..2] are required";
+  if (cfg.dering == 1 && !io->dering_level) return "dering_level is required on an engine with dering = 1";
+  return nullptr;
+}
+
+int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
+  if (!kf) return (int)cudaErrorInvalidValue;
+  daala_b200_kf_totals tot;
+  int fq_dc_limit = 0;
+  SymSeg seg[kSymSegs];
+  if (const char* why = submit_refusal(kf, io, &tot, &fq_dc_limit, seg)) {
+    snprintf(kf->err, sizeof(kf->err), "daala_b200_kf_submit: %s", why);
+    return (int)cudaErrorInvalidValue;
+  }
+  cudaStream_t s = kf->stream;
+  const int F = kf->F;
+  const bool lossless = kf->cfg.lossless != 0;
+  const bool fq_mode = kf->cfg.frame_quant || kf->cfg.keyframe_quant;
   for (int p = 0; p < 3; p++) {
-    if (!io->pixels[p]) return (int)cudaErrorInvalidValue;
     KF_CHECK(cudaMemcpyAsync(kf->pixels[p], io->pixels[p], (size_t)kf->plane_w[p] * kf->plane_h[p] * F,
                              cudaMemcpyHostToDevice, s));
     if (kf->cfg.inter_mc) {
@@ -3317,16 +3303,14 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
     }
   }
   if (fq_mode) KF_CHECK(fq_copy(kf, io->frame_quant, s));
-  if (kf->cfg.frame_types) KF_CHECK(cudaMemcpyAsync(kf->ftype, io->frame_type, (size_t)F, cudaMemcpyHostToDevice, s));
+  if (kf->mixed) KF_CHECK(cudaMemcpyAsync(kf->ftype, io->frame_type, (size_t)F, cudaMemcpyHostToDevice, s));
   const size_t map_bytes = (size_t)kf->nhsb * 8 * kf->nvsb * 8 * F;
   if (!lossless) KF_CHECK(cudaMemcpyAsync(kf->bsize, io->bsize, map_bytes, cudaMemcpyHostToDevice, s));
   // the graph's lossless kernels read the slot table: NULL stores nothing (every entry -1)
   if (io->ll_ref_slot_out) KF_CHECK(cudaMemcpyAsync(kf->ll_slot_out, io->ll_ref_slot_out, 4 * (size_t)F, cudaMemcpyHostToDevice, s));
   else if (kf->ll_slot_out) KF_CHECK(cudaMemsetAsync(kf->ll_slot_out, 0xFF, 4 * (size_t)F, s));
-  if (kf->cfg.dering == 1) {
-    if (!io->dering_level) return (int)cudaErrorInvalidValue;
+  if (kf->cfg.dering == 1)
     KF_CHECK(cudaMemcpyAsync(kf->dering.level, io->dering_level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyHostToDevice, s));
-  }
   const int rc = daala_b200_kf_run_device(kf, DAALA_B200_KF_ALL, 1);
   if (rc) return rc;
   kf->have_step = true;
@@ -3385,6 +3369,18 @@ int daala_b200_kf_submit(daala_b200_kf* kf, const daala_b200_kf_io* io) {
                                sizeof(int32_t) * (kf->plane_w[p] >> 2) * (kf->plane_h[p] >> 2) * F, cudaMemcpyDeviceToHost, s));
   if (io->dering_level_out && kf->cfg.dering)
     KF_CHECK(cudaMemcpyAsync(io->dering_level_out, kf->dering.level, (size_t)kf->nhsb * kf->nvsb * F, cudaMemcpyDeviceToHost, s));
+  SymCopy sc;
+  memset(&sc, 0, sizeof(sc));
+  bool want_sym = false;
+  for (int i = 0; i < kSymSegs; i++) {
+    sc.src[i] = seg[i].src;
+    sc.dst[i] = seg[i].dst;
+    sc.unit[i] = seg[i].unit;
+    sc.cap[i] = std::min(seg[i].cap, seg[i].src_cap) * seg[i].unit;
+    want_sym = want_sym || seg[i].dst;
+  }
+  sc.index_bytes = (long long)F * sizeof(daala_b200_kf_sym_frame);
+  sc.tot = kf->sym.tot;
   if (want_sym) {
     k_sym_copy<<<kf->sms * 4, 256, 0, s>>>(sc);
     KF_CHECK(cudaGetLastError());

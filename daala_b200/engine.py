@@ -494,20 +494,7 @@ class KeyframeEngine:
                 out["luma_late_skip"] = self._arr("lls", (nl,), sym.LATE_SKIP_DTYPE)
                 out["chroma_late_skip"] = self._arr("cls", (nc,), sym.LATE_SKIP_DTYPE)
                 io.luma_late_skip, io.chroma_late_skip = out["luma_late_skip"].ctypes.data, out["chroma_late_skip"].ctypes.data
-        if self.inter_mc:
-            io.ref_resident = int(self.resident)
-            for p in range(3):
-                if not self.resident:
-                    io.ref_pixels[p] = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8).ctypes.data
-                if pred:
-                    out["pred%d" % p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
-                    io.pred_pixels_out[p] = out["pred%d" % p].ctypes.data
-            io.nrefs = self.nrefs
-            io.ref_slot = self._arr("slot", (self.F, 2), np.int32).ctypes.data
-            io.mv_grid = self._arr("grid", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1), mvgrid.MV_PT_DTYPE).ctypes.data
-            if self.mc_next:
-                io.ref_slot_next = self._arr("slot_next", (self.F,), np.int32).ctypes.data
-                io.mv1_grid = self._arr("grid1", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1, 2), np.int32).ctypes.data
+        mc_h2d = self._prepare_io_mc(io, out, pred)
         if self.inter:
             if not self.inter_mc:
                 for p in range(3):
@@ -560,12 +547,8 @@ class KeyframeEngine:
                 io.sym_hdc, io.sym_hdc_cap = out["sym_hdc"].ctypes.data, int(b.blocks)
         self._io, self._out = io, out
         px = sum(int(np.prod(g.plane_shape(p))) for p in range(3))
-        self.h2d_bytes = px * self.F * (2 if self.inter and not self.inter_mc else 1) + int(np.prod(g.bsize_shape)) * self.F
-        if self.inter_mc:
-            self.h2d_bytes += (px * self.nrefs + 8 * self.F
-                               + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * mvgrid.MV_PT_DTYPE.itemsize)
-            if self.mc_next:   # the NEXT slot of each frame and the mv1 of each vertex
-                self.h2d_bytes += 4 * self.F + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * 8
+        self.h2d_bytes = (px * self.F * (2 if self.inter and not self.inter_mc else 1) + int(np.prod(g.bsize_shape)) * self.F
+                          + mc_h2d)
         if self._fq is not None:   # the records, each frame's deringing thresholds (int32 [2][6]) and band quantisers ([3][32])
             self.h2d_bytes += self.F * (FRAME_QUANT_DTYPE.itemsize + 48 + 384)
         if self._ftype is not None:
@@ -580,6 +563,32 @@ class KeyframeEngine:
             return
         self._ll_slot = self._arr("llslot", (self.F,), np.int32)
         self._ll_slot[...] = slots
+
+    def _prepare_io_mc(self, io, out, pred):
+        """The inter_mc inputs of `io` staged by stage_mc (the reference pictures unless resident, the slot map, the MV
+        grids) and, with pred, the prediction planes as outputs pred0..2; returns the bytes of those inputs (0 on an
+        engine without inter_mc)."""
+        if not self.inter_mc:
+            return 0
+        g = self.geom
+        io.ref_resident = int(self.resident)
+        for p in range(3):
+            if not self.resident:
+                io.ref_pixels[p] = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8).ctypes.data
+            if pred:
+                out["pred%d" % p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
+                io.pred_pixels_out[p] = out["pred%d" % p].ctypes.data
+        io.nrefs = self.nrefs
+        nvert = self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1)
+        io.ref_slot = self._arr("slot", (self.F, 2), np.int32).ctypes.data
+        io.mv_grid = self._arr("grid", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1), mvgrid.MV_PT_DTYPE).ctypes.data
+        px = sum(int(np.prod(g.plane_shape(p))) for p in range(3))
+        h2d = px * self.nrefs + 8 * self.F + nvert * mvgrid.MV_PT_DTYPE.itemsize
+        if self.mc_next:   # the NEXT slot of each frame and the mv1 of each vertex
+            io.ref_slot_next = self._arr("slot_next", (self.F,), np.int32).ctypes.data
+            io.mv1_grid = self._arr("grid1", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1, 2), np.int32).ctypes.data
+            h2d += 4 * self.F + nvert * 8
+        return h2d
 
     def _prepare_io_lossless(self, recon, pred):
         """prepare_io of a lossless engine: the inputs, [the prediction inputs], and as outputs the reconstruction
@@ -599,20 +608,7 @@ class KeyframeEngine:
                 io.pred_pixels[p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8).ctypes.data
         out["ll_blocks"] = self._arr("llb", (self.F, g.nvsb, g.nhsb, 3, 4), np.int32)
         io.ll_blocks = out["ll_blocks"].ctypes.data
-        if self.inter_mc:
-            io.ref_resident = int(self.resident)
-            for p in range(3):
-                if not self.resident:
-                    io.ref_pixels[p] = self._arr("ref%d" % p, (self.nrefs,) + g.plane_shape(p), np.uint8).ctypes.data
-                if pred:
-                    out["pred%d" % p] = self._arr("pred%d" % p, (self.F,) + g.plane_shape(p), np.uint8)
-                    io.pred_pixels_out[p] = out["pred%d" % p].ctypes.data
-            io.nrefs = self.nrefs
-            io.ref_slot = self._arr("slot", (self.F, 2), np.int32).ctypes.data
-            io.mv_grid = self._arr("grid", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1), mvgrid.MV_PT_DTYPE).ctypes.data
-            if self.mc_next:
-                io.ref_slot_next = self._arr("slot_next", (self.F,), np.int32).ctypes.data
-                io.mv1_grid = self._arr("grid1", (self.F, g.nvsb * 8 + 1, g.nhsb * 8 + 1, 2), np.int32).ctypes.data
+        mc_h2d = self._prepare_io_mc(io, out, pred)
         if self._ll_slot is not None:
             io.ll_ref_slot_out = self._ll_slot.ctypes.data
         out["counts"] = self._arr("cnt", (32,), np.int32)
@@ -620,12 +616,7 @@ class KeyframeEngine:
         self.d2h_bytes = sum(v.nbytes for v in out.values())
         self._io, self._out = io, out
         px = sum(int(np.prod(g.plane_shape(p))) for p in range(3))
-        self.h2d_bytes = px * self.F * (2 if self.inter and not self.inter_mc else 1)
-        if self.inter_mc:
-            self.h2d_bytes += (px * self.nrefs + 8 * self.F
-                               + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * mvgrid.MV_PT_DTYPE.itemsize)
-            if self.mc_next:
-                self.h2d_bytes += 4 * self.F + self.F * (g.nvsb * 8 + 1) * (g.nhsb * 8 + 1) * 8
+        self.h2d_bytes = px * self.F * (2 if self.inter and not self.inter_mc else 1) + mc_h2d
         if self._ll_slot is not None:
             self.h2d_bytes += 4 * self.F
         return out

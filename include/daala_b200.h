@@ -960,15 +960,16 @@ int daala_b200_kf_count_blocks(const uint8_t *bsize, int nframes, long long fram
    per coefficient. */
 int daala_b200_kf_symbol_bounds(const daala_b200_kf_totals *t, int nframes, daala_b200_kf_sym_bounds *out);
 /* With config.inter, DAALA_B200_KF_PVQ_LUMA selects the luma phase kernels.
-   H2D of the inputs, the whole step, D2H of the requested outputs: enqueued, not waited for.  A batch with more
-   luma or chroma blocks than the engine's capacity (see max_blocks_div) returns cudaErrorInvalidValue before
-   anything is copied or launched; so does a request for symbol stream outputs from an engine created without
-   symbol_stream (sym_dc: without symbol_stream 2 or 3), a stream capacity below daala_b200_kf_symbol_bounds, a stream
-   buffer that is not pinned host memory, or (config.inter) a NULL pred_pixels plane, luma_dc or chroma_dc (the last
-   two are optional with symbol_stream 2 or 3), a late-skip output on an engine without late_skip, sym_late_skip
-   without symbol_stream = 2, sym_dc below daala_b200_kf_symbol_bounds(...).blocks records or not pinned, and sym_hdc
-   on an engine without both symbol_stream = 1 and haar_dc_quant = 1 or symbol_stream = 3, below
-   daala_b200_kf_symbol_bounds(...).blocks records or not pinned (each with a message in daala_b200_kf_error).  With config.inter_mc it refuses, the same
+   H2D of the inputs, the whole step, D2H of the requested outputs: enqueued, not waited for.  Every refusal returns
+   cudaErrorInvalidValue with a message in daala_b200_kf_error, before anything is copied or launched: the device
+   buffers, the reference-picture pool and what run_device replays are those of the last accepted step.  Submit
+   refuses a NULL pixels plane, a NULL bsize (lossy engines), a NULL dering_level on a dering = 1 engine, a batch with
+   more luma or chroma blocks than the engine's capacity (see max_blocks_div), a request for symbol stream outputs
+   from an engine created without symbol_stream (sym_dc: without symbol_stream 2 or 3), a stream capacity below
+   daala_b200_kf_symbol_bounds, a stream buffer that is not pinned host memory, or (config.inter) a NULL pred_pixels
+   plane, luma_dc or chroma_dc (the last two are optional with symbol_stream 2 or 3), a late-skip output on an engine
+   without late_skip, sym_late_skip without symbol_stream = 2, and sym_hdc on an engine without both
+   symbol_stream = 1 and haar_dc_quant = 1 or symbol_stream = 3.  With config.inter_mc it refuses, the same
    way, a NULL mv_grid, ref_pixels plane or ref_slot, pred_pixels given, nrefs outside [1, mc_refs] and a slot outside
    [0, nrefs); with ref_resident = 1 it refuses instead ref_pixels given, nrefs other than 0, a slot outside
    [0, mc_refs) and a slot that holds no picture.  With config.mc_next the same checks cover ref_slot_next, and a NULL
